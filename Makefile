@@ -1,11 +1,13 @@
-# stencil_b200 build: hand-written sm_100a CUDA, no cmake needed.
-#   make            -> stencil_b200/libstencil_b200.so (C ABI + kernels) and lib/libstencil.a (C++ API, -rdc)
-#   make drivers    -> bin/ : the REFERENCE's own drivers and Catch2 suites compiled, unchanged, from
-#                      $(REF)/bin and $(REF)/test against OUR headers and library (needs $(REF))
+# stencil_b200 build: hand-written sm_90a (H100) CUDA, no cmake needed.
+#   make            -> stencil_b200/libstencil_b200.so (C ABI + kernels), lib/libstencil.a (C++ API, -rdc) and bin/ :
+#                      sb_mpirun, our jacobi3d_b200 driver and the multi-rank C++ exchange test
+#   make drivers REF=<cwpearson/stencil checkout>
+#                   -> bin/ : the REFERENCE's own drivers and Catch2 suites compiled, unchanged, from
+#                      $(REF)/bin and $(REF)/test against OUR headers and library
 #   make oracle     -> oracle/_build/liboracle.so (test infrastructure)
 NVCC      ?= /usr/local/cuda/bin/nvcc
-REF       ?= /root/reference
-ARCH      := -gencode arch=compute_100a,code=sm_100a
+REF       ?=
+ARCH      := -gencode arch=compute_90a,code=sm_90a
 NVCCFLAGS := -O3 -std=c++17 $(ARCH) -lineinfo -Xcompiler -fPIC -Xcompiler -Wall -Xcompiler -Wno-comment --expt-relaxed-constexpr
 INC       := -Iinclude -Istencil_b200/csrc
 
@@ -31,7 +33,7 @@ LIBA      := lib/libstencil.a
 # inside libstencil.a would shadow or clash with the real one)
 LIBMPI    := lib/libmpi_shim.a
 
-all: $(SO) $(LIBA) $(LIBMPI) bin/sb_mpirun
+all: $(SO) $(LIBA) $(LIBMPI) bin/sb_mpirun bin/jacobi3d_b200 bin/test_exchange_multigpu
 
 build/mpi_shim.o: src/mpi_shim.cpp include/mpi_shim/mpi.h
 	@mkdir -p build
@@ -66,6 +68,8 @@ $(LIBA): $(APIOBJ) $(CAPIOBJ)
 # ---- the reference's unchanged drivers / tests against our library
 DRVFLAGS  := -O3 -std=c++14 $(ARCH) -lineinfo -rdc=true --expt-extended-lambda -Xcompiler -w -w -x cu $(APIDEFS) \
              -DCATCH_CONFIG_NO_POSIX_SIGNALS $(APIINC) -I$(REF)/thirdparty -I$(REF)/bin
+# our own C++ programs: the same flags without the reference's include directories
+OWNDRVFLAGS := -O3 -std=c++14 $(ARCH) -lineinfo -rdc=true --expt-extended-lambda -Xcompiler -w -w -x cu $(APIDEFS) $(APIINC)
 DRVLINK    = $(ARCH) -rdc=true -L/usr/local/cuda/lib64/stubs -lnvidia-ml -ldl -lcudart -lrt
 DRIVERS   := jacobi3d jacobi3d_strong bench_exchange bench_pack exchange_weak exchange_strong
 TESTCUDA  := test_cuda_main test_cuda_align test_cuda_local_domain test_cuda_pack test_cuda_packer test_cuda_rcstream \
@@ -99,8 +103,8 @@ bin/test_cpu: $(patsubst %,build/drv/t_%.o,$(TESTCPU)) $(LIBA)
 # our own driver: the reference's jacobi3d loop over stencil::FusedJacobi3d (no reference sources involved)
 build/drv/jacobi3d_b200.o: drivers/jacobi3d_b200.cu $(wildcard include/stencil/*)
 	@mkdir -p $(dir $@)
-	$(NVCC) $(filter-out -I$(REF)/thirdparty -I$(REF)/bin,$(DRVFLAGS)) -c $< -o $@
-bin/jacobi3d_b200: build/drv/jacobi3d_b200.o $(LIBA)
+	$(NVCC) $(OWNDRVFLAGS) -c $< -o $@
+bin/jacobi3d_b200: build/drv/jacobi3d_b200.o $(LIBA) $(LIBMPI)
 	@mkdir -p bin
 	$(NVCC) $(DRVLINK) -o $@ $< $(LIBA) $(LIBMPI)
 
@@ -117,7 +121,10 @@ build/drv/exchange_uniform.o: oracle/ref/ref_exchange_uniform.cu $(wildcard incl
 # our own multi-GPU check of the C++ API
 build/drv/test_exchange_multigpu.o: tests/cpp/test_exchange_multigpu.cu $(wildcard include/stencil/*)
 	@mkdir -p $(dir $@)
-	$(NVCC) $(DRVFLAGS) -c $< -o $@
+	$(NVCC) $(OWNDRVFLAGS) -c $< -o $@
+bin/test_exchange_multigpu: build/drv/test_exchange_multigpu.o $(LIBA) $(LIBMPI)
+	@mkdir -p bin
+	$(NVCC) $(DRVLINK) -o $@ $< $(LIBA) $(LIBMPI)
 
 # the reference's astaroth driver (its own MHD kernels; halos through our library), unchanged
 ASTRO     := astaroth kernels astaroth_utils
@@ -140,7 +147,10 @@ bin/astaroth_b200: build/drv/astro_astaroth.o build/drv/astro_astaroth_utils.o b
 	@mkdir -p bin
 	$(NVCC) $(DRVLINK) -o $@ build/drv/astro_astaroth.o build/drv/astro_astaroth_utils.o build/drv/astro_b200_kernels.o build/drv/astro_statistics.o $(LIBA) $(LIBMPI)
 
-drivers: bin/sb_mpirun bin/jacobi3d_b200 $(patsubst %,bin/%,$(DRIVERS)) bin/test_cuda bin/test_cpu bin/exchange_uniform bin/astaroth bin/astaroth_b200 bin/test_exchange_multigpu
+drivers: check-ref bin/sb_mpirun bin/jacobi3d_b200 $(patsubst %,bin/%,$(DRIVERS)) bin/test_cuda bin/test_cpu bin/exchange_uniform bin/astaroth bin/astaroth_b200 bin/test_exchange_multigpu
+
+check-ref:
+	@test -n "$(REF)" -a -d "$(REF)/bin" || { echo "make drivers needs REF=<path of a cwpearson/stencil checkout>"; exit 1; }
 
 oracle:
 	$(MAKE) -C oracle
@@ -148,5 +158,5 @@ oracle:
 clean:
 	rm -rf build $(SO) lib bin
 
-.PHONY: all drivers oracle clean
+.PHONY: all drivers check-ref oracle clean
 .SECONDARY:

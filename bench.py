@@ -46,7 +46,13 @@ def parse():
                    help="fused: one kernel per iteration = jacobi update + halo push into the neighbours' ghost cells (Jacobi3D.step_fused); "
                    "queued: interior || exchange -> exterior with CUDA-event dependencies (step_async); host-sync: the reference's loop (step)")
     p.add_argument("--host-sync", action="store_true", help="block the host after the exchange and after the exterior kernels like bin/jacobi3d.cu:337-365 (default: iterations queue back to back, dependencies as CUDA events)")
-    return p.parse_args()
+    p.add_argument("--dump-outputs", metavar="DIR", default=None,
+                   help="after the timed steps, write the field every local subdomain holds after the last timed step to DIR/<name>.npy "
+                   "(a fixed, seeded sample of cells when the fields exceed 48 MB in all)")
+    args = p.parse_args()
+    if args.steps < 1:
+        p.error("--steps must be at least 1")
+    return args
 
 
 def measured_peaks():
@@ -54,32 +60,28 @@ def measured_peaks():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return json.load(f)["hbm_gbs"], "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not measured"
 
 
-def ncu_traffic(fused, n, dtype):
-    """DRAM bytes per launch of the dominant kernel from the committed ncu summary (profiles/), with the file's hash so that
-    a stale citation is detectable."""
-    import hashlib
-
-    if n != 512 or dtype != "f64":
-        return {"traffic": None, "traffic_source": None}
-    name = "jacobi_fused_r2.summary.txt" if fused else "jacobi_march_r1.summary.txt"
-    path = os.path.join(ROOT, "profiles", name)
-    try:
-        text = open(path).read()
-        for ln in text.splitlines():
-            if ln.startswith("traffic = dram read + write (bytes)"):
-                return {"traffic": int(float(ln.split()[-1])), "traffic_source": {"file": "profiles/" + name, "sha256": hashlib.sha256(text.encode()).hexdigest()[:16]}}
-    except OSError:
-        pass
-    return {"traffic": None, "traffic_source": None}
+def dump_outputs(out_dir, dd, dtype, n_subdomains):
+    """The field of every local subdomain (compute region, [z, y, x]) as <out_dir>/field_x<ox>_y<oy>_z<oz>.npy.  Above 48 MB
+    in all, each file holds the same seeded sample of cells (flat indices drawn with replacement, sorted) of its field."""
+    os.makedirs(out_dir, exist_ok=True)
+    es = np.dtype(dtype).itemsize
+    per_file = (48 << 20) // (es * n_subdomains)
+    for d in dd.domains():
+        a = d.interior_to_host(0).reshape(-1)
+        if a.size > per_file:
+            idx = np.sort(np.random.default_rng(20240921).integers(0, a.size, size=per_file))
+            a = a[idx]
+        o = d.origin()
+        np.save(os.path.join(out_dir, f"field_x{o[0]}_y{o[1]}_z{o[2]}.npy"), np.ascontiguousarray(a, dtype=dtype))
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons / power limit DURING the timed region."""
 
-    Q = "index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
+    Q = "index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,power.limit"
 
     def __init__(self, device: int):
         self.device, self.proc, self.lines = device, None, []
@@ -110,15 +112,16 @@ class ClockSampler:
             self.proc.wait(timeout=2)
         except Exception:
             self.proc.kill()
-        sm, mx, reasons, power = [], [], set(), []
+        sm, mx, reasons, power, limit = [], [], set(), [], []
         for ln in self.lines:
             f = [x.strip() for x in ln.split(",")]
-            if len(f) < 9:
+            if len(f) < 10:
                 continue
             try:
                 sm.append(float(f[1]))
                 mx.append(float(f[2]))
                 power.append(float(f[3]))
+                limit.append(float(f[9]))
             except ValueError:
                 continue
             for name, v in zip(("hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"), f[5:9]):
@@ -128,6 +131,7 @@ class ClockSampler:
             "sm_mhz": float(np.median(sm)) if sm else None,
             "sm_max_mhz": max(mx) if mx else None,
             "power_w_max": max(power) if power else None,
+            "power_limit_w": max(limit) if limit else None,
             "samples": len(sm),
             "reasons": sorted(reasons),
         }
@@ -257,7 +261,7 @@ def halo_exchange_metric(rank, world, gpus, ngpu, iters=30):
         "cross_gpu_bytes": int(peer),
         # payload every GPU sends (= receives) over NVLink per exchange / exchange time
         "nvlink_gbs_per_dir": (peer / ngpu) / (us * 1e-6) / 1e9 if peer > 0 else 0.0,
-        "nvlink_peak_gbs_per_dir": 900.0,
+        "nvlink_peak_gbs_per_dir": 450.0,  # H100 SXM data sheet: NVLink 4, 900 GB/s both directions together
         "transport": "fused direct write into the neighbours' ghost cells (peer access / CUDA IPC), thin rows staged; ready/done flags on the device",
     }
     barrier()
@@ -279,7 +283,11 @@ def halo_exchange_metric(rank, world, gpus, ngpu, iters=30):
         out["reference_us"] = ref("oracle/_ref/ref_exchange_uniform", "default")
         out["reference_cudampi_us"] = ref("oracle/_ref/ref_exchange_uniform", "cudampi")
         out["ours_cpp_one_process_us"] = ref("bin/exchange_uniform", "default")
-        out["reference_note"] = "reference library unmodified, 1 process x %d GPU(s) (no MPI here); cudampi = Method::CudaMpi over the single-process shim" % ngpu
+        out["reference_note"] = "reference library unmodified, 1 process x %d GPU(s) (no MPI); cudampi = Method::CudaMpi over the single-process shim" % ngpu
+        missing = [exe for exe in ("oracle/_ref/ref_exchange_uniform", "bin/exchange_uniform") if not os.path.exists(os.path.join(ROOT, exe))]
+        if missing:
+            # the reference is compiled only from a checkout of it: build() with STENCIL_REFERENCE=<checkout>
+            out["reference_note"] += "; not built, so the matching fields are null: %s (run build() with STENCIL_REFERENCE=<cwpearson/stencil checkout>)" % ", ".join(missing)
     barrier()
     return out
 
@@ -409,6 +417,8 @@ def run_ours(args, rank, world):
     t_wall = time.perf_counter() - t_wall0
     launches = L.sb_launch_count() - launches0
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, dd, dtype, ngpu)
     ms_total = ev_a.elapsed_time(ev_b)
     kern_ms = float(np.mean([a.elapsed_time(b) for a, b in zip(k0, k1)]))
     t = torch.tensor([ms_total, t_wall * 1e3], dtype=torch.float64, device="cuda")
@@ -437,9 +447,6 @@ def run_ours(args, rank, world):
         "peak_source": peak_src,
         "algorithmic_bytes_per_launch": alg_bytes,
         "kernel_ms": kern_ms,
-        # dram__bytes_read.sum + dram__bytes_write.sum of one launch of this kernel, read from the committed `ncu --set full`
-        # summary named in traffic_source (not re-measured by this run; null when no capture of this configuration exists)
-        **ncu_traffic(fused, n, args.dtype),
         "step_frac_of_roofline": (2 * es * cells / ngpu) / (ms_step * 1e-3) / 1e9 / peak,
     }
 
@@ -516,6 +523,7 @@ def run_ours(args, rank, world):
             "vs_baseline": None,
             "dtype": args.dtype,
             "data": "synthetic",
+            "gpu": torch.cuda.get_device_name(local),
             "per_gpu": value / ngpu,
             "wall_ms_per_step": wall_ms / args.steps,
             "config": {
@@ -528,7 +536,7 @@ def run_ours(args, rank, world):
                     "queued": "interior || exchange -> exterior, dependencies as CUDA events + ready/done flags (Jacobi3D.step_async)",
                     "host-sync": "host-side after exchange and exterior (Jacobi3D.step, the reference's loop)",
                 }[schedule],
-                "l2": "inputs larger than L2 (2 x %.2f GiB per GPU vs 126 MB)" % (2 * es * (n + 2) ** 3 / 2**31),
+                "l2": "inputs larger than L2 (2 x %.2f GiB per GPU vs %.0f MiB)" % (es * (n + 2) ** 3 / 2**30, torch.cuda.get_device_properties(local).L2_cache_size / 2**20),
                 "init": "0.5 everywhere, hot/cold spheres (bin/jacobi3d.cu:18-63)",
             },
             "roofline": roofline,

@@ -1,5 +1,5 @@
 // jacobi3d_b200: the reference's jacobi3d driver (bin/jacobi3d.cu) with its loop body replaced by
-// stencil::FusedJacobi3d::step() -- the hand-written sm_100a kernel with the halo push fused in -- so that C++ users
+// stencil::FusedJacobi3d::step() -- the hand-written sm_90a kernel with the halo push fused in -- so that C++ users
 // of the DistributedDomain API reach the roofline kernel.  Same weak-scaling size rule, same CSV line.
 //
 //   jacobi3d_b200 <x> <y> <z> [-n iters] [--f64] [--trivial] [--reference-schedule] [--dump file]

@@ -1,6 +1,6 @@
 /* mpi.h -- single-process MPI shim shipped with stencil_b200.
  *
- * Neither the build container nor the B200 boxes have an MPI installation, yet every public
+ * A machine need not have an MPI installation, yet every public
  * header of cwpearson/stencil includes <mpi.h> (reference include/stencil/stencil.hpp:10) and
  * every driver calls MPI_Init / MPI_Wtime / MPI_Allreduce directly (bin/jacobi3d.cu:139,298,371).
  * This header declares exactly the MPI surface the reference library, drivers and tests use

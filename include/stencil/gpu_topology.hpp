@@ -1,5 +1,5 @@
 #pragma once
-// What the placement code needs to know about the GPUs of a node.  On an NVSwitch node (B200 HGX) every pair of
+// What the placement code needs to know about the GPUs of a node.  On an NVSwitch node (H100 HGX) every pair of
 // GPUs is equally close, so bandwidth() only distinguishes same-device / peer / no-peer (src/gpu_topology.cpp).
 
 namespace gpu_topo {

@@ -1,5 +1,5 @@
 #pragma once
-// stencil::FusedJacobi3d -- the B200 fast path for the loop of the reference's jacobi3d driver
+// stencil::FusedJacobi3d -- the H100 fast path for the loop of the reference's jacobi3d driver
 // (bin/jacobi3d.cu:296-368), for C++ users of the DistributedDomain API.  NOT part of the reference's API: an
 // unchanged bin/jacobi3d.cu keeps launching its own stencil_kernel (7 global loads per cell); a driver that wants
 // the roofline kernel replaces its loop body by step():

@@ -3,7 +3,7 @@
 //   Trivial          RankPartition, subdomains dealt to ranks/GPUs in linear order
 //   NodeAware        NodePartition + a QAP per node matching halo traffic to GPU-GPU bandwidth
 //   IntraNodeRandom  NodePartition, random GPU assignment inside each node (placement_intranoderandom.hpp)
-// On a B200 NVSwitch node gpu_topo::bandwidth() is uniform for all distinct pairs, so the QAP cost is
+// On an H100 NVSwitch node gpu_topo::bandwidth() is uniform for all distinct pairs, so the QAP cost is
 // permutation invariant and NodeAware degenerates to the identity assignment (still solved, so the
 // code path and its tests stay alive for non-uniform hosts).
 

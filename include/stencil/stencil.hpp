@@ -1,7 +1,7 @@
 #pragma once
 // DistributedDomain: a periodic 3-D grid cut into one subdomain per GPU, with a halo exchange between
 // the 26 neighbours of every subdomain.  Public API of the reference's include/stencil/stencil.hpp;
-// the implementation (src/stencil.cu) is B200-native: realize() plans, for every local subdomain,
+// the implementation (src/stencil.cu) is H100-native: realize() plans, for every local subdomain,
 // ONE fused kernel that reads the outgoing halo regions of all quantities and stores them directly
 // into the ghost cells of the destination subdomains -- on the same GPU, or on a peer GPU through
 // NVLink/NVSwitch peer mappings -- with no send or receive buffers.

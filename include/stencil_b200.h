@@ -1,4 +1,4 @@
-/* stencil_b200.h -- C ABI of the B200-native halo-exchange / jacobi hot path.
+/* stencil_b200.h -- C ABI of the H100-native halo-exchange / jacobi hot path.
  *
  * This is the drop-in boundary below the C++ API (include/stencil/*.hpp): plain pointers and
  * sizes, no C++ or torch types.  Each entry point names the interface of cwpearson/stencil it
@@ -193,9 +193,9 @@ int sb_jacobi3d_fused(sb_pitched dst, sb_pitched src, int dtype_size, const int6
  * wait_rows[f][0] (this GPU's own mailbox for face f, written by the neighbour across f; ld.acquire.sys) until
  * (int32)(word - wait_value) >= 0.  Protocol: the launch of iteration e carries wait_value = signal_value = e -- a
  * neighbour that has STARTED iteration e has (a) filled the ghost cells iteration e reads here and (b) stopped reading
- * the ghost cells iteration e overwrites there.  Tiles that touch no face never wait.  (Round-2 measurements, 8 ranks:
- * one release per boundary tile cost 19 us per iteration -- the releasing warp lingers for an NVLink round trip and
- * keeps its CTA slot -- against a skew of a few microseconds between the ranks' kernel starts.)
+ * the ghost cells iteration e overwrites there.  Tiles that touch no face never wait.  (One release per boundary tile
+ * was slower on 8 ranks -- the releasing warp lingers for an NVLink round trip and keeps its CTA slot -- than the skew
+ * between the ranks' kernel starts that one release per kernel costs.)
  * Faces: -x,+x,-y,+y,-z,+z.  NULL rows: no wait / no signal on that face (neighbour in the same process: order the
  * launches with stream events).  sync == NULL: no handshake at all.  The rows keep SB_FUSED_MAX_GROUPS words (the
  * per-tile protocol's size); only word 0 is used. */

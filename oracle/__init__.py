@@ -18,6 +18,6 @@ and against vectors dumped from the reference's own host code compiled here
 (``oracle/ref/``, ``tests/golden/ref_geometry.json``).  Jacobi numerics have no
 golden in the reference (SURVEY.md 8c: "parity unpinned" for jacobi values);
 there the two independent restatements (numpy, C) are cross-checked bit-exactly
-and the reference's own ``stencil_kernel`` is run beside ours on the GPU box
+and the reference's own ``stencil_kernel`` is run beside ours on the GPU
 (``oracle/_ref``).
 """

@@ -12,7 +12,7 @@
  * (astaroth/kernels.cu:15, 27-29) over allocations that include the radius-3 ghost cells.
  *
  * Parity status: the reference holds NO test for these numerics (astaroth/astaroth.cu:538 "TODO"); the pin is
- * tests/golden/astaroth_solve_ref.npz, produced on a B200 by the reference's own solve<> kernels
+ * tests/golden/astaroth_solve_ref.npz, produced on a GPU by the reference's own solve<> kernels
  * (oracle/ref/ref_astaroth_solve.cu + oracle/ref/make_astaroth_golden.py).  Floating point: compiled with
  * -ffp-contract=off while nvcc contracts a*b+c into FMAs, so agreement is to rounding, not bit-exact.
  */

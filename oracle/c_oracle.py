@@ -49,7 +49,7 @@ def astaroth_conf_params(dt: float = 1e-8) -> AcParams:
 
 
 def build(force: bool = False) -> str:
-    """Compile the C oracle with gcc (present in this image and on the GPU box)."""
+    """Compile the C oracle with gcc."""
     srcs = [os.path.join(_HERE, f) for f in ("stencil_oracle.c", "astaroth_oracle.c")]
     stale = (not os.path.exists(_SO)) or os.path.getmtime(_SO) < max(os.path.getmtime(s) for s in srcs)
     if force or stale:

@@ -1,7 +1,7 @@
 """Integer geometry, partition and message planning of cwpearson/stencil -- CPU oracle.
 
 TEST INFRASTRUCTURE (see oracle/__init__.py).  Pure Python ints; every function
-cites the reference file:line (relative to /root/reference) that it restates.
+cites the reference file:line (relative to the reference checkout) that it restates.
 Coordinates are (x, y, z) tuples everywhere, x fastest in memory.
 """
 from __future__ import annotations

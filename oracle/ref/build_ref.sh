@@ -1,19 +1,19 @@
 #!/bin/bash
-# Builds the UNMODIFIED reference (cwpearson/stencil) from the sources where they lie under
-# /root/reference into oracle/_ref/ (git-ignored, travels to the GPU box with the gpurun snapshot):
-#   libref_stencil.a      the reference library (all 16 sources), sm_100a, Release, CUDA graphs on
+# Builds the UNMODIFIED reference (cwpearson/stencil) from the sources where they lie, in the checkout named by
+# $STENCIL_REFERENCE, into oracle/_ref/ (git-ignored; __graft_entry__.build() runs this when STENCIL_REFERENCE is set):
+#   libref_stencil.a      the reference library (all 16 sources), sm_90a, Release, CUDA graphs on
 #   ref_jacobi3d          bin/jacobi3d.cu           (reference stencil_kernel + transports)
 #   ref_bench_exchange    bin/bench_exchange.cu
 #   ref_bench_pack        bin/bench_pack.cu
 #   ref_test_cuda         the reference's own Catch2 GPU suite (test/test_cuda_*.cu + test_exchange.cu)
 #   ref_test_cpu          the reference's own Catch2 host suite
-# MPI does not exist in this image: the reference is linked against our single-process shim
-# (include/mpi_shim/mpi.h, src/mpi_shim.cpp).  Nothing is copied out of /root/reference.
+# No MPI installation is assumed: the reference is linked against our single-process shim
+# (include/mpi_shim/mpi.h, src/mpi_shim.cpp).  Nothing is copied out of the reference checkout.
 # TEST / BASELINE INFRASTRUCTURE ONLY -- the product never links these files.
 set -euo pipefail
 HERE="$(cd "$(dirname "$0")" && pwd)"
 REPO="$(cd "$HERE/../.." && pwd)"
-REF="${STENCIL_REFERENCE:-/root/reference}"
+REF="${STENCIL_REFERENCE:?set STENCIL_REFERENCE to a cwpearson/stencil checkout}"
 OUT="$REPO/oracle/_ref"
 OBJ="$OUT/obj"
 mkdir -p "$OUT" "$OBJ"
@@ -24,8 +24,8 @@ if [ -f "$STAMP" ] && [ "$STAMP" -nt "$HERE/build_ref.sh" ] && [ "$STAMP" -nt "$
 fi
 DEFS="-DSTENCIL_USE_MPI=1 -DSTENCIL_USE_CUDA=1 -DSTENCIL_USE_CUDA_AWARE_MPI=1 -DSTENCIL_USE_CUDA_GRAPH=1 -DSTENCIL_SETUP_STATS=1 -DSTENCIL_OUTPUT_LEVEL=2 -DNDEBUG -DCATCH_CONFIG_NO_POSIX_SIGNALS"
 INC="-I$REF/include -I$REF/thirdparty -I$REF/bin -I$REPO/include/mpi_shim -I/usr/local/cuda/include/nvtx3"
-FLAGS="-std=c++14 -O3 -gencode arch=compute_100a,code=sm_100a -lineinfo -rdc=true --expt-extended-lambda -Xcompiler -w -w -x cu $DEFS $INC"
-LINK="-gencode arch=compute_100a,code=sm_100a -rdc=true -L/usr/local/cuda/lib64/stubs -lnvidia-ml -ldl -lcudart"
+FLAGS="-std=c++14 -O3 -gencode arch=compute_90a,code=sm_90a -lineinfo -rdc=true --expt-extended-lambda -Xcompiler -w -w -x cu $DEFS $INC"
+LINK="-gencode arch=compute_90a,code=sm_90a -rdc=true -L/usr/local/cuda/lib64/stubs -lnvidia-ml -ldl -lcudart"
 
 compile() { # src obj
   if [ ! -f "$2" ] || [ "$1" -nt "$2" ]; then $NVCC $FLAGS -c "$1" -o "$2"; fi

@@ -1,10 +1,10 @@
 #!/usr/bin/env python
 """Golden vectors for the astaroth solve<step> substeps, produced by the REFERENCE's own kernels.
 
-Run on a GPU box (the reference kernels need a device):
-    bash oracle/ref/build_ref.sh                       # in the build container: oracle/_ref/ref_astaroth_solve
-    gpurun -- python oracle/ref/make_astaroth_golden.py   # writes gpurun_out/astaroth_solve_ref.npz
-then copy gpurun_out/astaroth_solve_ref.npz to tests/golden/.  Inputs: 16 arrays (in[8], out[8]) of (n+6)^3 doubles,
+Run on a GPU (the reference kernels need a device):
+    STENCIL_REFERENCE=<checkout> bash oracle/ref/build_ref.sh   # oracle/_ref/ref_astaroth_solve (no GPU needed)
+    python oracle/ref/make_astaroth_golden.py OUT_DIR           # writes OUT_DIR/astaroth_solve_ref.npz
+then copy OUT_DIR/astaroth_solve_ref.npz to tests/golden/.  Inputs: 16 arrays (in[8], out[8]) of (n+6)^3 doubles,
 seeded uniform(-1, 1) plus a smooth component; outputs: the compute region of all 8 `out` fields after substeps 0, 1, 2
 (no swap in between, like astaroth/astaroth.cu:551-640).  dt = 1e-3 (the driver's 1e-8 would hide the rate of change
 under the rounding of the state)."""
@@ -30,7 +30,7 @@ def make_inputs(n: int, seed: int) -> np.ndarray:
 
 def main():
     n, dt, seed = 8, 1e-3, 20240921
-    out_dir = os.path.join(ROOT, "gpurun_out")
+    out_dir = os.path.abspath(sys.argv[1] if len(sys.argv) > 1 else ".")
     os.makedirs(out_dir, exist_ok=True)
     a = make_inputs(n, seed)
     fin, fout = os.path.join(out_dir, "ac_in.bin"), os.path.join(out_dir, "ac_out.bin")
@@ -41,11 +41,11 @@ def main():
     np.savez_compressed(
         os.path.join(out_dir, "astaroth_solve_ref.npz"),
         n=n, dt=dt, seed=seed, inputs=a, outputs=res[:, :, 3:-3, 3:-3, 3:-3].copy(),
-        source="reference astaroth/kernels.cu solve<0,1,2> on B200 (sm_100a, --use_fast_math as in astaroth/CMakeLists.txt:55)",
+        source="reference astaroth/kernels.cu solve<0,1,2> on one GPU (--use_fast_math as in astaroth/CMakeLists.txt:55)",
     )  # fmt: skip
     os.remove(fin)
     os.remove(fout)
-    print("wrote gpurun_out/astaroth_solve_ref.npz", res.shape, float(np.abs(res).max()))
+    print("wrote", os.path.join(out_dir, "astaroth_solve_ref.npz"), res.shape, float(np.abs(res).max()))
 
 
 if __name__ == "__main__":

@@ -1,5 +1,5 @@
 // Golden-vector generator for the astaroth solve<step> kernels: runs the UNMODIFIED reference kernels
-// (/root/reference/astaroth/kernels.cu -> integrate_substep, acDeviceLoad*) on a small periodic-free box and dumps
+// (<reference>/astaroth/kernels.cu -> integrate_substep, acDeviceLoad*) on a small periodic-free box and dumps
 // the `out` fields after each of the three substeps.  Test / baseline infrastructure only (built by
 // oracle/ref/build_ref.sh into oracle/_ref/, never linked by the product).
 //

@@ -1,6 +1,6 @@
 // Golden-vector generator: links the REFERENCE's own host code (compiled where it lies under
-// /root/reference, never copied) and dumps its answers for the geometry / partition / ordering
-// functions of the halo-exchange path as JSON.  Runs in the build container (no GPU needed: only
+// the reference checkout, never copied) and dumps its answers for the geometry / partition / ordering
+// functions of the halo-exchange path as JSON.  Runs without a GPU (only
 // host functions are called).  Output is committed as tests/golden/ref_geometry.json by
 // oracle/ref/make_golden.sh.  TEST INFRASTRUCTURE.
 #include <cstdio>

@@ -1,5 +1,5 @@
 // Golden-vector generator for the jacobi numerics: drives the UNMODIFIED kernels of the reference driver
-// (/root/reference/bin/jacobi3d.cu:18-85 -- init_kernel, dist, stencil_kernel -- pulled in by #include with its main()
+// (<reference>/bin/jacobi3d.cu:18-85 -- init_kernel, dist, stencil_kernel -- pulled in by #include with its main()
 // renamed) through the reference library's own DistributedDomain on one GPU, and dumps the compute region after
 // selected iterations.  The reference has no test and no golden output for these numerics (SURVEY.md section 8c);
 // this is the pin.  Test / baseline infrastructure only (built by oracle/ref/build_ref.sh into oracle/_ref/, in two
@@ -12,7 +12,7 @@
 //          exchange -> stencil_kernel over the whole compute region -> swap (the --no-overlap order of
 //          bin/jacobi3d.cu:344-353; the overlapped order computes the same values).
 #define main reference_jacobi3d_main
-#include "jacobi3d.cu" // resolved through -I/root/reference/bin
+#include "jacobi3d.cu" // resolved through -I<reference>/bin
 #undef main
 
 #include <cstdio>

@@ -4,7 +4,7 @@
  * bench.py as the timed CPU baseline ("port").  The product (stencil_b200/, src/, include/)
  * never links or loads this file.
  *
- * All citations are relative to /root/reference.  Layout: x fastest, unpitched rows
+ * All citations are relative to the reference checkout.  Layout: x fastest, unpitched rows
  * (src/local_domain.cu:187-203), element (x,y,z) of an allocation with raw size (nx,ny,nz)
  * lives at byte offset ((z*ny + y)*nx + x)*elem_size.
  *

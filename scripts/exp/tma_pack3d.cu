@@ -4,8 +4,8 @@
 // 3-stage ring of 32 KiB stages, against the library's LSU path (sb_pack) on the same messages:
 //   y / z faces of a 512^3 FP32 / FP64 subdomain with radius 2 and 3, and one field-face of the astaroth exchange
 //   (256^3, radius 3, FP64).
-// Build (host has no GPU; run on the box):
-//   nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -Iinclude scripts/exp/tma_pack3d.cu -o scripts/exp/tma_pack3d \
+// Build (nvcc needs no GPU; run it on an H100):
+//   nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -Iinclude scripts/exp/tma_pack3d.cu -o scripts/exp/tma_pack3d \
 //        -Lstencil_b200 -lstencil_b200 -Xlinker -rpath -Xlinker '$ORIGIN/../../stencil_b200'
 // Prints one line per message: payload, LSU us, TMA us, GB/s (read + write) each, and whether the packed bytes agree.
 #include <cuda.h>
@@ -138,7 +138,7 @@ int main() {
   const Case cases[] = {{"512^3 f32 r=2 y-face", 512, 2, 4, 1}, {"512^3 f32 r=2 z-face", 512, 2, 4, 2}, {"512^3 f32 r=3 y-face", 512, 3, 4, 1},
                         {"512^3 f32 r=3 z-face", 512, 3, 4, 2}, {"512^3 f64 r=2 y-face", 512, 2, 8, 1}, {"512^3 f64 r=2 z-face", 512, 2, 8, 2},
                         {"256^3 f64 r=3 y-face (astaroth field)", 256, 3, 8, 1}, {"256^3 f64 r=3 z-face (astaroth field)", 256, 3, 8, 2}};
-  int sms = 148;
+  int sms = 132;
   CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0));
   CK(cudaFuncSetAttribute(tma_pack_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kStages * kStageBytes));
   for (const Case &c : cases) {

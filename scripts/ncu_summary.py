@@ -1,5 +1,5 @@
-"""Summarise an .ncu-rep (read here, no GPU needed) into a small text file for profiles/.
-usage: python scripts/ncu_summary.py gpurun_out/prof.ncu-rep profiles/name.summary.txt"""
+"""Summarise an .ncu-rep (no GPU needed to read it) into a small text file.
+usage: python scripts/ncu_summary.py prof.ncu-rep name.summary.txt"""
 import csv
 import io
 import subprocess

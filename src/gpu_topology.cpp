@@ -9,10 +9,10 @@
 #include "stencil/cuda_runtime.hpp"
 #include "stencil/logging.hpp"
 
-// Retargeted at NVLink 5 / NVSwitch nodes (HGX B200): every GPU reaches every peer at the same
+// Retargeted at NVLink / NVSwitch nodes (HGX H100): every GPU reaches every peer at the same
 // bandwidth through the switch, so the matrix has three levels only:
-//   same device (HBM3e)            8000
-//   peer-mappable pair (NVSwitch)   900   (per direction)
+//   same device (HBM3)             3350
+//   peer-mappable pair (NVSwitch)   450   (NVLink 4, per direction)
 //   no peer access (host bounce)     50
 // Only the ratios matter to the placement QAP.  The reference walks NVML NVLink link lists and PCIe
 // ancestors (src/gpu_topology.cpp:17-95) to rank V100 hybrid-cube-mesh pairs; on a switched fabric
@@ -59,13 +59,13 @@ bool peer(const int src, const int dst) {
 }
 
 double bandwidth(int src, int dst) {
-  if (src == dst) return 8000.0;
+  if (src == dst) return 3350.0;
   int can = 0;
   if (cudaSuccess != cudaDeviceCanAccessPeer(&can, src, dst)) {
     cudaGetLastError();
     can = 0;
   }
-  return can ? 900.0 : 50.0;
+  return can ? 450.0 : 50.0;
 }
 
 } // namespace gpu_topo

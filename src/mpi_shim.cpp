@@ -1,6 +1,6 @@
 // Node-local implementation of the MPI surface declared in include/mpi_shim/mpi.h (lib/libmpi_shim.a).
 //
-// Neither the build container nor the B200 boxes have an MPI.  This file provides the subset the reference library,
+// A machine need not have an MPI.  This file provides the subset the reference library,
 // its drivers and its tests use (SURVEY.md section 2c), for the ranks of ONE node:
 //   * started directly            -> a world of one rank (the reference's 1 rank x N GPUs deployment);
 //   * started by bin/sb_mpirun -n N -> N processes that share one POSIX shared-memory segment: a sense-reversing

@@ -1,6 +1,6 @@
-"""stencil_b200 -- B200-native halo exchange + jacobi hot path behind the cwpearson/stencil API.
+"""stencil_b200 -- H100-native halo exchange + jacobi hot path behind the cwpearson/stencil API.
 
-The compute lives in hand-written sm_100a CUDA (stencil_b200/csrc) behind a C ABI
+The compute lives in hand-written sm_90a CUDA (stencil_b200/csrc) behind a C ABI
 (include/stencil_b200.h); this package is the Python host mirror of the reference's domain API.
 """
 from ._lib import LIB_PATH, StencilError, lib  # noqa: F401

@@ -43,9 +43,9 @@ class Astaroth:
 
     def __init__(self, dd: DistributedDomain, handles: Sequence[DataHandle], params: Optional[AstarothParams] = None,
                  overlap: Optional[bool] = None, variant: int = AUTO):  # fmt: skip
-        """overlap=None picks the faster schedule measured on B200 (profiles/README.md section 5): the tile kernel fills
+        """overlap=None picks the faster schedule: the tile kernel fills
         every SM's shared memory, so a concurrent exchange only waits for it -- exchange first, then one launch over the
-        whole region (FP64 7.07 vs 7.34 ms, FP32 3.64 vs 3.85 ms per iteration at 256^3); overlap=True is the
+        whole region (measured faster than the split on the B200 it was tuned on; not re-timed on the H100); overlap=True is the
         interior || exchange -> exterior split of the reference driver."""
         import torch
 

@@ -1,4 +1,4 @@
-// Astaroth `solve<step>` for sm_100a.  See astaroth.cuh for the reference anchors.
+// Astaroth `solve<step>` for sm_90a (H100).  See astaroth.cuh for the reference anchors.
 //
 // What the reference does (astaroth/user_kernels.h:437-469 with block (32,1,4), astaroth/kernels.cu:67): every thread
 // rebuilds value + gradient + full hessian of all 8 fields from global memory -- 8 x 55 neighbour loads per cell, 254
@@ -16,7 +16,7 @@
 //  * cell kernel for thin boxes (the 3-cell exterior slabs): one thread per cell, neighbours through the read-only path.
 // Roofline: 8 reads + 8 reads of `out` + 8 writes per cell = 24 x sizeof(T) bytes (16 x for step 0, which ignores the
 // previous state); with ~300 shared-memory loads and ~900 FP instructions per cell the FP64 kernel is shared-memory /
-// DFMA-issue bound before it is HBM bound -- numbers in profiles/README.md.
+// DFMA-issue bound before it is HBM bound.
 #include "astaroth.cuh"
 
 #include <cuda.h>
@@ -363,7 +363,7 @@ int env_int(const char *name, int dflt);
 // Two threads per cell.  The tile kernel above keeps value + gradient + hessian of all 8 fields live until the physics
 // runs (238 registers -> 7 warps per SM), and all of its warps alternate between a shared-memory phase (296 LDS) and an
 // FP64 phase (~900 instructions) in lock step behind the per-plane barrier: ncu shows the two pipes at 53 % and 31 %,
-// never overlapping (profiles/astaroth_tile_f64_r1_v1.summary.txt).  Here
+// never overlapping.  Here
 //   team U (threads [0, NC))      derives lnrho, entropy, uux, uuy, uuz and folds every field into a handful of running
 //                                 sums the moment it is derived (advection, div u, lap u, grad div u, the six entries of
 //                                 the rate-of-strain tensor, ...), then integrates continuity, momentum and entropy;
@@ -863,7 +863,7 @@ template <int STEP, typename T, int TX, int TY> int launch_team(AcArgs<T> &A, cu
   static unsigned long long configured = 0;
   static const bool paced = env_int("SB_AC_PACE", 1) != 0;
   auto kern = paced ? ac_team_kernel<STEP, T, TX, TY, NSLOT, true> : ac_team_kernel<STEP, T, TX, TY, NSLOT, false>;
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   if (!(configured >> (dev & 63) & 1)) {
     if (cudaFuncSetAttribute(ac_team_kernel<STEP, T, TX, TY, NSLOT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)) != cudaSuccess) return -1;
@@ -897,7 +897,7 @@ template <int STEP, typename T, int TX, int TY, int NSLOT> int launch_tile(AcArg
   constexpr size_t smem = size_t(kAcFields) * NSLOT * (TX + 6) * (TY + 6) * sizeof(T);
   static unsigned long long configured = 0; // bit per device: the opt-in is per function and per context
   auto kern = ac_tile_kernel<STEP, T, TX, TY, NSLOT>;
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   if (!(configured >> (dev & 63) & 1)) {
     if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)) != cudaSuccess) return -1;
@@ -986,7 +986,7 @@ template <int STEP, int TX, int TY, int NTEAM> int launch_team_tma(AcArgs<double
   static const bool paced = env_int("SB_AC_PACE", 1) != 0;
   auto kern = paced ? ac_team_tma_kernel<STEP, TX, TY, NTEAM, true> : ac_team_tma_kernel<STEP, TX, TY, NTEAM, false>;
   static unsigned long long configured = 0;
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   if (!(configured >> (dev & 63) & 1)) {
     if (cudaFuncSetAttribute(ac_team_tma_kernel<STEP, TX, TY, NTEAM, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)) != cudaSuccess) return 0;
@@ -1025,15 +1025,14 @@ template <int STEP, typename T> int launch_cell(AcArgs<T> &A, cudaStream_t strea
 
 template <int STEP, typename T> int launch_step(AcArgs<T> &A, long long mz, int variant, cudaStream_t stream) {
   const int ex = A.hi[0] - A.lo[0], ey = A.hi[1] - A.lo[1], ez = A.hi[2] - A.lo[2];
-  // thick boxes: FP64 -> the TMA-fed two-team kernel (1.80 ms per 256^3 substep against 2.27 for the tile kernel and 2.21 for
-  // the reference's solve<>), FP32 -> the tile kernel (1.12 vs 1.19 ms); thin boxes (exterior slabs) -> one thread per cell
+  // thick boxes: FP64 -> the TMA-fed two-team kernel, FP32 -> the tile kernel (the faster of the variants where they were
+  // tuned, on a B200; not re-timed on the H100); thin boxes (exterior slabs) -> one thread per cell
   if (variant == AC_AUTO) variant = (ex >= 8 && ey >= 8 && ez >= 8) ? (sizeof(T) == 8 ? AC_TEAM : AC_TILE) : AC_CELL;
   if (variant == AC_CELL) return launch_cell<STEP>(A, stream);
   if (variant == AC_TEAM || variant == AC_TEAM_TMA || variant == AC_TEAM3_TMA) {
     if constexpr (sizeof(T) == 8) {
       if (variant != AC_TEAM || env_int("SB_AC_TMA", 1) != 0) {
-        // two teams by default: measured on B200, 256^3 FP64 substep 1: 1.80 ms with two teams, 1.98 ms with three
-        // (profiles/README.md section 5); SB_AC_TEAMS=3 or variant 5 = three teams
+        // two teams by default; SB_AC_TEAMS=3 or variant 5 = three teams
         const bool three = variant == AC_TEAM3_TMA || (variant == AC_TEAM && env_int("SB_AC_TEAMS", 2) == 3);
         const int n = three ? launch_team_tma<STEP, 16, 10, 3>(A, mz, stream) : launch_team_tma<STEP, 16, 12, 2>(A, mz, stream);
         if (n > 0) return n;
@@ -1050,7 +1049,7 @@ template <int STEP, typename T> int launch_step(AcArgs<T> &A, long long mz, int 
     if (shape == 1) return launch_tile<STEP, T, 16, 16, 7>(A, stream);
     return launch_tile<STEP, T, 16, 14, 8>(A, stream);
   } else {
-    // measured on B200, 256^3 (profiles/README.md section 5): 32x8 tiles (256 threads) 1.12 ms, 32x16 (512 threads) 1.23 ms
+    // 32x8 tiles (256 threads) by default, SB_AC_SHAPE=1 for 32x16 (512 threads)
     if (shape == 1) return launch_tile<STEP, T, 32, 16, 8>(A, stream);
     return launch_tile<STEP, T, 32, 8, 8>(A, stream);
   }

@@ -1,4 +1,4 @@
-// Astaroth MHD substep (`solve<step>`: 8 fields, 6th-order central differences, Williamson RK3) -- B200 rewrite of
+// Astaroth MHD substep (`solve<step>`: 8 fields, 6th-order central differences, Williamson RK3) -- H100 rewrite of
 // the reference's generated kernel (astaroth/user_kernels.h:36-183, 376-469; astaroth/integration.cuh:14-52;
 // astaroth/kernels.cu:62-87).  SURVEY.md section 8 row a18.
 #pragma once

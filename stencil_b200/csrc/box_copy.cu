@@ -1,4 +1,4 @@
-// Box-copy kernels (see box_copy.cuh for the design).  sm_100a only.
+// Box-copy kernels (see box_copy.cuh for the design).  sm_90a only.
 #include "box_copy.cuh"
 
 namespace sb {
@@ -6,9 +6,9 @@ namespace sb {
 namespace {
 
 // Halo source cells are read exactly once and never written by the same launch (sources are compute
-// cells, destinations ghost cells or dense buffers).  Measured on B200 (scripts/time_pack.py, 512^3):
-// wide rows are fastest through the read-only path (ld.global.nc: 4.2 us vs 6.2 us per 3 MB face),
-// thin strided rows with plain loads (8.4 us vs 12.5 us with evict-first .cs loads).
+// cells, destinations ghost cells or dense buffers).  Wide rows go through the read-only path
+// (ld.global.nc), thin strided rows through plain loads rather than evict-first .cs loads
+// (scripts/time_pack.py times both).
 template <typename V> __device__ __forceinline__ V ld_wide(const V *p) { return __ldg(p); }
 template <> __device__ __forceinline__ unsigned char ld_wide(const unsigned char *p) { return *p; }
 template <> __device__ __forceinline__ unsigned short ld_wide(const unsigned short *p) { return *p; }
@@ -344,7 +344,7 @@ __global__ void __launch_bounds__(kCopyThreads, 3) box_copy_single_kernel(const 
   for (unsigned long long row0 = (unsigned long long)blockIdx.x * rows_per_tile; row0 < total;
        row0 += (unsigned long long)gridDim.x * rows_per_tile) {
     // NOTE: written as end = min(row0 + rpt, total); nrows = end - row0.  The natural
-    // min(total - row0, rpt) is miscompiled by ptxas 12.9 for sm_100a: the subtract and the minimum
+    // min(total - row0, rpt) is miscompiled by ptxas 12.9 for sm_100a (Blackwell): the subtract and the minimum
     // are fused into VIADDMNMX.U32 with the negation dropped (it computes min(row0 + total, rpt)),
     // which turned every partial last tile into a full one (caught by tests/test_gpu_copy.py cases 7, 11).
     const unsigned long long stop = row0 + rows_per_tile;
@@ -384,7 +384,10 @@ void launch_box_copy_single(const Seg &seg, cudaStream_t stream) {
   const unsigned rows_per_tile = rows_per_tile_for(seg.row_bytes);
   unsigned ntiles = (total + rows_per_tile - 1) / rows_per_tile;
   if (ntiles == 0) return;
-  const unsigned cap = 148u * 8u;
+  int dev = 0, sms = 0;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  const unsigned cap = unsigned(sms > 0 ? sms : 1) * 8u;
   box_copy_single_kernel<<<ntiles < cap ? ntiles : cap, kCopyThreads, 0, stream>>>(seg, rows_per_tile);
 }
 

@@ -10,7 +10,7 @@
 // destination may be a dense buffer (pack), a local allocation (translate/unpack) or a peer GPU's
 // ghost cells mapped over NVLink (fused exchange: no send or receive buffer ever touches HBM).
 //
-// Work decomposition (sm_100a, 148 SMs): each segment is cut into tiles of consecutive rows sized
+// Work decomposition (sm_90a, 132 SMs on an H100): each segment is cut into tiles of consecutive rows sized
 // to ~16 KiB of payload; a persistent grid (a multiple of the SM count) walks the tile table.
 // Inside a tile a power-of-two group of lanes owns one row, so a 4 KiB z-face row is moved by a
 // full warp with 16-byte accesses (512 B per warp instruction) while an 8-byte x-face "row" is
@@ -36,15 +36,15 @@ struct Seg {
   unsigned long long ny_magic;
 };
 
-// Opt-in (SB_TMA=1) TMA tile kinds for wide segments.  Measured constraints on sm_100a (scripts/exp/tma_probe3.cu):
+// Opt-in (SB_TMA=1) TMA tile kinds for wide segments.  Constraints (probed with scripts/exp/tma_probe3.cu):
 // a box's global START address must be 16-byte aligned (element-granular coordinates do NOT absorb an 8-byte row
 // phase: UTMALDG/UTMASTG raise "illegal instruction"), and its shared-memory address must be 128-byte aligned.
 //   kind 1  both sides TMA-legal (16-byte aligned base, strides and box start, e.g. r=2 FP64): cp.async.bulk.tensor
 //           global -> shared (mbarrier complete_tx) then shared -> global (bulk_group), ONE elected thread per CTA,
 //           4-stage shared-memory ring, a row cut into chunks of `bx` elements (box = bx x 1 x 1).
 //   kind 2  source rows start off a 16-byte boundary (r=1 FP64): aligned-down TMA load, vector stores by all threads.
-// Measured result (profiles/README.md section 4): for halo-sized messages (2-4 MB, <1 tile per SM) both kinds are
-// 2-4x SLOWER than the LSU path below, which is why they are off by default.
+// Result on the B200 they were written on (not re-timed on the H100): for halo-sized messages (2-4 MB, <1 tile per
+// SM) both kinds were slower than the LSU path below, which is why they are off by default.
 constexpr int kMaxTmaMaps = 16;
 
 // The CUtensorMap descriptors travel as a __grid_constant__ kernel parameter (the documented-safe home

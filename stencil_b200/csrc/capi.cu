@@ -248,7 +248,7 @@ int tma_map_index(TmaBuild &tb, const sb_pitched &a, int64_t es, unsigned bx) {
 
 // returns true if the copy was taken over by the TMA path
 bool try_tma_segment(const sb_box_copy &c, TmaBuild &tb, int plan_device) {
-  const int enabled = env_int("SB_TMA", 0); // opt-in: measured slower than the LSU path (profiles/README.md section 4)
+  const int enabled = env_int("SB_TMA", 0); // opt-in: slower than the LSU path for halo-sized messages
   static const int peer_ok = env_int("SB_TMA_PEER", 1); // TMA stores into peer-mapped (NVLink) memory
   if (!enabled || !encode_tiled_fn()) return false;
   if (!peer_ok) {
@@ -267,7 +267,7 @@ bool try_tma_segment(const sb_box_copy &c, TmaBuild &tb, int plan_device) {
     if ((uintptr_t(a->ptr) & 15) || (a->pitch & 15) || ((a->pitch * a->ysize) & 15) || (a->pitch % es)) return false;
     if (a->pitch * a->ysize >= (int64_t(1) << 40)) return false;
   }
-  // MEASURED on B200 (scripts/exp/tma_probe3.cu): the global address a box starts at must itself be 16-byte
+  // Probed with scripts/exp/tma_probe3.cu: the global address a box starts at must itself be 16-byte
   // aligned -- a UINT64 box at x = 1 (or an INT32 box at x = 1..3) raises "illegal instruction" at the
   // UTMALDG, x = 2 (x = 4) is fine.  Rows of an FP64 r=1 halo start 8 bytes into the row, so they are NOT
   // directly TMA-addressable; such segments take the LSU path (or the aligned-down TMA-load kind).
@@ -632,7 +632,7 @@ int sb_copy_plan_create(sb_copy_plan **out, int device, const sb_box_copy *copie
     SB_CUDA(cudaMalloc(&p->tiles_dev, tiles.size() * sizeof(sb::Tile)));
     SB_CUDA(cudaMemcpy(p->segs_dev, segs.data(), segs.size() * sizeof(sb::Seg), cudaMemcpyHostToDevice));
     SB_CUDA(cudaMemcpy(p->tiles_dev, tiles.data(), tiles.size() * sizeof(sb::Tile), cudaMemcpyHostToDevice));
-    int sms = 148;
+    int sms = 132;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
     const int per_sm = env_int("SB_COPY_CTAS_PER_SM", 8);
     const long long cap = (long long)sms * per_sm;

@@ -1,4 +1,4 @@
-// 7-point jacobi kernels for sm_100a (see jacobi.cuh).
+// 7-point jacobi kernels for sm_90a (see jacobi.cuh).
 //
 // jacobi_march_kernel: register-blocked z-march.  A warp owns a strip of 32*VX cells in x and RY
 // rows in y; each lane keeps the z-1 / z / z+1 values of its VX*RY columns in registers, so every
@@ -6,7 +6,7 @@
 // with 16-byte vector loads.  x-neighbours come from the adjacent lane by warp shuffle (lanes 0
 // and 31 fetch one scalar), y-neighbours inside the RY rows from registers and across warps from
 // L1 (the neighbouring warp loaded that row one step earlier).  Eight warps are stacked in y, the
-// z axis is cut into chunks so that the grid has several waves on 148 SMs, and an optional
+// z axis is cut into chunks so that the grid has several waves on the GPU's SMs, and an optional
 // prefetch.global.L2 runs a few planes ahead of the march to deepen the memory pipeline without
 // spending registers.  Algorithmic traffic: one read + one write per cell (2*sizeof(T) B/cell).
 //
@@ -237,7 +237,7 @@ __device__ __forceinline__ void march_body(const JacobiParams &p, const int bx, 
   int z = z0;
   // XPUSH: the x neighbour of the first / last compute cell may come from a dense received array [y][z] (z fastest), which
   // is not part of the rows the march prefetches: a load per step put an L2 miss on every fourth step's critical path
-  // (measured: 15 us per iteration with a quarter of the tiles on x faces).  The chunk's 256-byte line of this row is
+  // (a quarter of the tiles sit on x faces).  The chunk's 256-byte line of this row is
   // pulled into L1 here, one plane per lane; the edge lane's loads then hit.
   if (XP) {
     const int gside = (x0w == p.lo[0] && p.xghost_ptr[0]) ? 0 : ((x0w + 32 * VX == p.hi[0] && p.xghost_ptr[1]) ? 1 : -1);
@@ -535,7 +535,7 @@ __device__ __forceinline__ void march_column(const JacobiParams &p, const int xc
 //    face (own memory, ld.acquire.sys by one thread): "the neighbour has started iteration e" says both "the ghost cells
 //    I read are filled" and "the neighbour is done reading the ghost cells I am about to overwrite".  Inner tiles never
 //    wait.  Tried first: one flag per boundary tile, released by the tile after its pushes -- the releasing warp waits for
-//    an NVLink round trip and keeps its CTA's registers (4 x 256 x 64 = the whole file), 19 us per iteration on 8 ranks;
+//    an NVLink round trip and keeps its CTA's registers (4 x 256 x 64 = the whole file), so it was slower on 8 ranks;
 //    what the per-kernel flag costs instead is the skew between the ranks' kernel starts, a few microseconds in the
 //    first wave.  Every acquire also invalidates the SM's whole L1 (CCTL.IVALL): exactly one per face and tile.
 constexpr int kMaxGroups = SB_FUSED_MAX_GROUPS;
@@ -614,9 +614,8 @@ __device__ __forceinline__ void fused_body(const JacobiParams &p, const FusedSyn
   if (waits && threadIdx.x == 0) {
     const uint32_t want = s.wait_value;
     // ld.acquire.sys = LDG.STRONG.SYS + CCTL.IVALL (the SM's L1 is dropped, so that ghost cells fetched before the
-    // neighbour wrote them cannot be served from it).  Measured alternatives: relaxed loads + one fence.acq_rel.sys cost
-    // 32 us per iteration at N = 2 (MEMBAR.ALL.SYS at the start of every boundary CTA), three acquiring threads nothing more
-    // than one.
+    // neighbour wrote them cannot be served from it).  Alternatives tried: relaxed loads + one fence.acq_rel.sys were slower
+    // (MEMBAR.ALL.SYS at the start of every boundary CTA); three acquiring threads gained nothing over one.
     auto poll = [&](const uint32_t *slot) {
       uint32_t v;
       while (true) {
@@ -1000,6 +999,14 @@ int env_int(const char *name, int dflt) {
   return (s && *s) ? atoi(s) : dflt;
 }
 
+// SMs of the current device: the grid-stride kernels below cap their grids at a few CTAs per SM
+long long sm_count() {
+  int dev = 0, sms = 0;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  return sms > 0 ? sms : 1;
+}
+
 } // namespace
 
 int launch_jacobi_regions(const JacobiParams &p, const JacobiRegions &r, int dtype_size, cudaStream_t stream) {
@@ -1007,7 +1014,7 @@ int launch_jacobi_regions(const JacobiParams &p, const JacobiRegions &r, int dty
   if (r.n <= 0 || total <= 0) return 0;
   long long blocks = (total + 255) / 256;
   static const int per_sm = env_int("SB_JACOBI_EXT_CTAS_PER_SM", 32);
-  if (blocks > 148ll * per_sm) blocks = 148ll * per_sm;
+  if (blocks > sm_count() * per_sm) blocks = sm_count() * per_sm;
   if (dtype_size == 4)
     jacobi_regions_kernel<float><<<(unsigned)blocks, 256, 0, stream>>>(p, r);
   else
@@ -1031,7 +1038,7 @@ int launch_jacobi(const JacobiParams &p_in, int dtype_size, cudaStream_t stream)
   if (ex < thin) {
     const long long total = (long long)ex * ey * ez;
     long long blocks = (total + 255) / 256;
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > sm_count() * 16) blocks = sm_count() * 16;
     if (dtype_size == 4)
       jacobi_cell_kernel<float><<<(unsigned)blocks, 256, 0, stream>>>(p);
     else
@@ -1039,7 +1046,7 @@ int launch_jacobi(const JacobiParams &p_in, int dtype_size, cudaStream_t stream)
     return 1;
   }
 
-  // z chunk: enough CTAs for >= ~6 waves of 148 SMs x 4 resident CTAs, but chunks no shorter than 16 planes
+  // z chunk: enough CTAs for several waves of 4 resident CTAs per SM, but chunks no shorter than 16 planes
   if (zchunk_env > 0) {
     p.zchunk = zchunk_env;
   } else if (p.zchunk <= 0) {
@@ -1093,10 +1100,10 @@ int launch_jacobi_fused(const JacobiParams &p_in, const FusedSync &sync_in, int 
   const int ex = p.hi[0] - p.lo[0], ey = p.hi[1] - p.lo[1], ez = p.hi[2] - p.lo[2];
   if (ex <= 0 || ey <= 0 || ez <= 0) return 0;
   const int zchunk_env = env_int("SB_JACOBI_ZCHUNK", 0);
-  const int pf = env_int("SB_JACOBI_PREFETCH", 2);
+  // H100 80GB HBM3 (400 W), 512^3 FP64, one GPU: 16-plane chunks with a 1-plane L2 prefetch take 0.80 ms per iteration,
+  // 32 planes with a 2-plane prefetch 0.88 ms (alternating runs, DESIGN.md section 2.2)
+  const int pf = env_int("SB_JACOBI_PREFETCH", 1);
   const int allow_shift = env_int("SB_JACOBI_SHIFT", 1);
-  p.zchunk = (zchunk_env > 0 && zchunk_env <= 32) ? zchunk_env : 32; // the x faces are staged 32 planes at a time
-  if (p.zchunk > ez) p.zchunk = ez;
   p.prefetch = pf;
   FusedSync sync = sync_in;
   const int dbg = env_int("SB_DEBUG_FUSED", 0); // timing diagnostics only (results may be wrong): 1 no waits, 2 no signals
@@ -1107,6 +1114,16 @@ int launch_jacobi_fused(const JacobiParams &p_in, const FusedSync &sync_in, int 
   sync.debug = dbg;
   bool shift = false;
   const int vx = pick_vectors(p, dtype_size, allow_shift != 0, &shift);
+  // z chunk (the x faces are staged at most 32 planes at a time): 16 planes by default, 32 where 16-plane chunks would give
+  // a face more tiles than launch_fused's group limit (subdomains taller than ~720 cells in z)
+  if (zchunk_env > 0 && zchunk_env <= 32) {
+    p.zchunk = zchunk_env;
+  } else {
+    const long long tiles_x = (p.hi[0] - p.x0a + (shift ? vx / 2 : 0) + 32 * vx - 1) / (32 * vx), tiles_y = (ey + 7) / 8;
+    const long long across = tiles_x > tiles_y ? tiles_x : tiles_y;
+    p.zchunk = ((ez + 15) / 16) * across <= kMaxGroups ? 16 : 32;
+  }
+  if (p.zchunk > ez) p.zchunk = ez;
   // x wrap (periodic self-neighbour read in place) works through the edge lanes' scalar load, so the first compute cell
   // must open lane 0 of the first strip and the last one must close lane 31 of the last strip; otherwise the ghost
   // column is read by a vector load or a shuffle and the x faces are pushed into the ghost cells like any other face
@@ -1132,7 +1149,7 @@ int launch_fill(char *dst, long long pitch, long long slice, const int lo[3], co
   const int ex = hi[0] - lo[0], ey = hi[1] - lo[1], ez = hi[2] - lo[2];
   if (ex <= 0 || ey <= 0 || ez <= 0) return 0;
   long long blocks = ((long long)ex * ey * ez + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > sm_count() * 16) blocks = sm_count() * 16;
   if (dtype_size == 4)
     fill_kernel<float><<<(unsigned)blocks, 256, 0, stream>>>(dst, pitch, slice, lo[0], lo[1], lo[2], ex, ey, ez, (float)value);
   else
@@ -1146,7 +1163,7 @@ int launch_sqdiff(const char *a, const char *b, long long pitch, long long slice
   const int ex = hi[0] - lo[0], ey = hi[1] - lo[1], ez = hi[2] - lo[2];
   if (ex <= 0 || ey <= 0 || ez <= 0) return 0;
   long long blocks = ((long long)ex * ey * ez + 255) / 256;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > sm_count() * 8) blocks = sm_count() * 8;
   if (dtype_size == 4)
     sqdiff_kernel<float><<<(unsigned)blocks, 256, 0, stream>>>(a, b, pitch, slice, lo[0], lo[1], lo[2], ex, ey, ez, out_dev);
   else

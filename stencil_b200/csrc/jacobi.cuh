@@ -1,4 +1,4 @@
-// 7-point jacobi step with hot/cold Dirichlet spheres -- B200 rewrite of the reference's user
+// 7-point jacobi step with hot/cold Dirichlet spheres -- H100 rewrite of the reference's user
 // kernel (bin/jacobi3d.cu:40-85).  Bandwidth-bound pointwise stencil: no tensor cores.
 #pragma once
 
@@ -45,7 +45,8 @@ struct JacobiParams {
 };
 
 // Mailbox rows of the fused kernel (see jacobi_fused_kernel): one word per boundary tile of a face -- (z chunks x tile rows)
-// for x faces, (z chunks x strips) for y faces, (tile rows x strips) for z faces; 16 x 64 = 1024 at 512^3 FP64
+// for x faces, (z chunks x strips) for y faces, (tile rows x strips) for z faces; 32 x 64 = 2048 at 512^3 FP64 with the
+// default 16-plane chunks (launch_jacobi_fused falls back to 32-plane chunks where 16 would exceed the limit)
 #ifndef SB_FUSED_MAX_GROUPS
 #define SB_FUSED_MAX_GROUPS 4096
 #endif

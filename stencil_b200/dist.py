@@ -253,7 +253,7 @@ STAGE_MAX_ROW_BYTES = 64
 def staging_layout(dd, src_idx, dst_idx):
     """Messages from subdomain src_idx to subdomain dst_idx (on a DIFFERENT GPU) whose rows are shorter than
     STAGE_MAX_ROW_BYTES (x-faces, x-edges, corners): storing such rows straight into the peer's ghost cells costs one
-    tiny NVLink transaction per row (measured on 2x B200: 1.6 M 8-byte remote stores = 194 us and a 70 % slower
+    tiny NVLink transaction per row (1.6 M 8-byte remote stores per exchange on two GPUs, and a much slower
     interior kernel), so the sender packs them into ONE dense receive buffer in the peer's memory (contiguous 128-byte
     NVLink packets) and the receiver scatters them locally.  Pure geometry: both sides compute the same layout.
     Returns (total_bytes, [dict(dir, q, offset, ext, src_pos, dst_pos, es)])."""

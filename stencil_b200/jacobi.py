@@ -266,7 +266,7 @@ class Jacobi3D:
             return _dist.all_gather_object(obj) if multi_rank else [obj]
 
         # An x face is one cell per row: 8 bytes every 4112.  Stored cell by cell into another GPU it is one tiny NVLink
-        # transaction per row (78 us per iteration through CUDA-IPC mappings, profiles/README.md section 6.1), so towards
+        # transaction per row (tens of microseconds per iteration through CUDA-IPC mappings), so towards
         # any OTHER subdomain the column travels as a dense [y][z] array (z fastest, like the march): the shipping CTA
         # writes 256-byte lines into the neighbour's receive array (double buffered by swap parity) and the neighbour's
         # edge lanes read their x ghosts from it.  Needs whole warp strips along x and a 16-byte aligned first compute

@@ -1,5 +1,5 @@
 """GPU parity of the astaroth solve<step> kernels (stencil_b200/csrc/astaroth.cu) against the CPU oracle
-(oracle/astaroth_oracle.c), against golden vectors produced by the REFERENCE's own kernels on a B200
+(oracle/astaroth_oracle.c), against golden vectors produced by the REFERENCE's own kernels
 (tests/golden/astaroth_solve_ref.npz), and through DistributedDomain (interior || exchange -> exterior, 3 substeps,
 swap) against the oracle's single-address-space exchange.  Floating point: tolerances in astaroth_util.tolerance."""
 import os
@@ -100,7 +100,7 @@ def test_tile_shapes_and_zchunks(variant, shape, monkeypatch):
 @pytest.mark.skipif(not os.path.exists(GOLDEN), reason="golden vectors not generated yet (oracle/ref/make_astaroth_golden.py)")
 @pytest.mark.parametrize("variant", [ac.CELL, ac.TILE, ac.TEAM, ac.TEAM_TMA, ac.TEAM3_TMA])
 def test_matches_reference_kernel_golden(variant):
-    """The reference's own solve<0,1,2> (astaroth/kernels.cu, compiled unmodified for sm_100a) produced these."""
+    """The reference's own solve<0,1,2> (astaroth/kernels.cu, compiled unmodified) produced these."""
     z = np.load(GOLDEN)
     n, dt = int(z["n"]), float(z["dt"])
     inputs, outputs = z["inputs"], z["outputs"]

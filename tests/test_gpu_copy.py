@@ -202,9 +202,9 @@ def test_full_size_face_roundtrip_512():
 def test_tma_path_is_taken_and_exact(dtype, n, r, monkeypatch):
     """Wide rows with 16-byte aligned bases/strides are moved by the TMA tile kind (cp.async.bulk.tensor load +
     store through a shared-memory ring).  Halo regions of every wide class (y face, z face, yz edge) + pack +
-    unpack, byte-compared with the oracle; the plan must report TMA segments.  The path is opt-in (SB_TMA=1): measured on B200 it is slower than the LSU path for halo-sized
-    messages (profiles/README.md), but it stays parity-tested."""
-    monkeypatch.setenv("SB_TMA", "1")  # opt-in path: slower than the LSU path on B200 for halo-sized messages
+    unpack, byte-compared with the oracle; the plan must report TMA segments.  The path is opt-in (SB_TMA=1): it is slower than the LSU path for halo-sized
+    messages, but it stays parity-tested."""
+    monkeypatch.setenv("SB_TMA", "1")  # opt-in path: slower than the LSU path for halo-sized messages
     ro = g.Radius.constant(r)
     sz = (n, n, n)
     raw = g.raw_size(sz, ro)

@@ -247,12 +247,14 @@ def test_fused_kernel_tile_walks(monkeypatch, rotate, dtype):
     """jacobi_fused_kernel walks its tiles from a rotated origin on every axis (SB_FUSED_ROTATE, default on) so that the
     walk does not end with tiles that push; inner tiles take the plain loop, boundary tiles the variant their faces need.
     Either walk, on shapes with 1..N tiles per axis (also fewer than the two boundary tiles, partial tiles, one-plane
-    chunks), must reproduce Jacobi3D.step bit for bit."""
+    chunks, and subdomains 768 cells tall in y and z, whose 16-plane chunks would exceed the face-group limit), must
+    reproduce Jacobi3D.step bit for bit."""
     from stencil_b200.jacobi import Jacobi3D, jacobi_radius
 
     monkeypatch.setenv("SB_FUSED_ROTATE", str(rotate))
     for size, ndom in [((40, 24, 70), 1), ((200, 20, 40), 1), ((256, 40, 100), 1), ((384, 30, 66), 2), ((130, 17, 33), 1), ((64, 40, 65), 2), ((128, 7, 1), 1),
-                       ((128, 300, 40), 2), ((129, 40, 300), 2), ((256, 600, 9), 2)]:  # FP32: tail-column tiles that push y / z faces
+                       ((128, 300, 40), 2), ((129, 40, 300), 2), ((256, 600, 9), 2),  # FP32: tail-column tiles that push y / z faces
+                       ((64, 768, 768), 1), ((64, 768, 1536), 2)]:
         fields = []
         for mode in ("sync", "fused"):
             dd = sb.DistributedDomain(*size)
@@ -278,7 +280,7 @@ def test_fused_kernel_tile_walks(monkeypatch, rotate, dtype):
 @pytest.mark.parametrize("schedule", ["host-sync", "queued", "fused"])
 def test_jacobi_vs_reference_kernel_golden(schedule):
     """The CUDA kernels (all three schedules, FP32 = the reference's dtype) against the reference's own stencil_kernel run
-    on a B200 (tests/golden/jacobi_ref.npz): bit for bit against its IEEE build, one ulp per iteration against its
+    on a GPU (tests/golden/jacobi_ref.npz): bit for bit against its IEEE build, one ulp per iteration against its
     --use_fast_math build (approximate divide, bin/CMakeLists.txt:56)."""
     import os
 
