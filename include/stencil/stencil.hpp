@@ -22,6 +22,7 @@
 
 #include "stencil/cuda_runtime.hpp"
 
+#include "stencil/boundary_condition.hpp"
 #include "stencil/dim3.hpp"
 #include "stencil/direction_map.hpp"
 #include "stencil/gpu_topology.hpp"
@@ -40,6 +41,7 @@
 #include "stencil/tx.hpp"
 
 struct sb_copy_plan;
+struct sb_bc_plan;
 
 class DistributedDomain {
 private:
@@ -63,7 +65,16 @@ private:
 
   Method flags_;
   PlacementStrategy strategy_;
-  Topology::Boundary boundary_; // PERIODIC (the reference's only kind) or FIXED
+  Topology::Boundary boundary_[3]; // per axis: PERIODIC (the reference's only kind) or FIXED
+
+  // boundary conditions on the wall faces: (quantity, face 0..5 = -x,+x,-y,+y,-z,+z) -> BC, and each quantity's sb_dtype
+  std::map<std::pair<size_t, int>, stencil::BC> bcs_;
+  std::vector<int> dataDtype_;
+  // after the exchange: bcPlans_[parity][local domain] (nullptr where the subdomain has no BC to apply), launched on the
+  // subdomain's exchange stream after its phase 2 and after the phase 1 of bcSenders_[domain] (local subdomains)
+  std::vector<sb_bc_plan *> bcPlans_[2];
+  std::vector<std::vector<size_t>> bcSenders_;
+  void plan_boundaries(std::ofstream &planFile);
 
   // the fused exchange: plans_[parity][local domain]; parity = number of swap() calls mod 2.
   // Phase 1 (plans_): each subdomain stores its outgoing halos into the neighbours' ghost cells -- except
@@ -145,15 +156,40 @@ public:
   template <typename T> DataHandle<T> add_data(const std::string &name = "") {
     dataElemSize_.push_back(sizeof(T));
     dataName_.push_back(name);
+    dataDtype_.push_back(stencil::bc_dtype<T>());
     return DataHandle<T>(dataElemSize_.size() - 1, name);
   }
 
   // choose transports (before realize):  d.set_methods(Method::CudaMpi | Method::CudaKernel);
   void set_methods(Method flags) noexcept;
   void set_placement(PlacementStrategy strategy) noexcept { strategy_ = strategy; }
-  // how the grid closes at its faces (before realize).  PERIODIC is the reference's behaviour; FIXED plans no messages
-  // across the faces of the whole grid (the ghost cells there keep what the application put into them)
-  void set_boundary(Topology::Boundary boundary) noexcept { boundary_ = boundary; }
+  // how the grid closes at its faces (before realize), for all axes or per axis.  PERIODIC is the reference's behaviour;
+  // FIXED plans no messages across the faces of the whole grid along that axis (the ghost cells there keep what the
+  // application put into them, unless set_boundary_condition gives them a BC)
+  void set_boundary(Topology::Boundary boundary) noexcept { boundary_[0] = boundary_[1] = boundary_[2] = boundary; }
+  void set_boundary(Topology::Boundary x, Topology::Boundary y, Topology::Boundary z) noexcept {
+    boundary_[0] = x;
+    boundary_[1] = y;
+    boundary_[2] = z;
+  }
+  // the BC of quantity h on the wall face `face` ((+-1,0,0), (0,+-1,0) or (0,0,+-1)) of the whole grid (before realize):
+  // exchange() fills the ghost cells behind it.  realize() rejects a BC on a periodic axis, VALUE / ODD on a quantity
+  // that is not float or double, and EVEN / ODD with a ghost width larger than a subdomain.
+  template <typename T> void set_boundary_condition(const DataHandle<T> &h, const Dim3 &face, const stencil::BC &bc) {
+    int f = -1;
+    for (int a = 0; a < 3; ++a) {
+      const int64_t c = a == 0 ? face.x : a == 1 ? face.y : face.z;
+      if (c != 0) f = (f == -1 && (c == 1 || c == -1)) ? 2 * a + (c > 0) : -2;
+    }
+    if (f < 0) LOG_FATAL("set_boundary_condition: " << face << " is not a face direction");
+    if (dataDtype_.size() <= h.id() || dataDtype_[h.id()] != stencil::bc_dtype<T>()) LOG_FATAL("set_boundary_condition: unknown data handle");
+    bcs_[std::make_pair(h.id(), f)] = bc;
+  }
+  bool has_boundary_conditions() const noexcept {
+    for (const auto &kv : bcs_)
+      if (kv.second.kind != stencil::BC::Kind::NONE) return true;
+    return false;
+  }
   bool any_methods(Method methods) const noexcept { return methods && flags_; }
   // CUDA devices for this rank (before realize); repeats are allowed (several subdomains per GPU)
   void set_gpus(const std::vector<int> &cudaIds) { gpus_ = cudaIds; }

@@ -121,6 +121,68 @@ int sb_signal(uint32_t *const *remote_slots, int n, uint32_t value, int device, 
 int sb_wait(const uint32_t *local_slots, int n, uint32_t value, int device, void *stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Physical boundary conditions (BCs) on non-periodic grids (not in the reference, whose grids are periodic).
+ * A wall face of a subdomain is a face across which the grid does not continue (an axis that does not wrap).  The
+ * ghost cells behind it are filled after the halo exchange by ONE launch per subdomain.  Faces are numbered
+ * 0..5 = -x, +x, -y, +y, -z, +z.  Each (quantity, face) has a kind and a value c:
+ *   SB_BC_NONE   ghost cells untouched
+ *   SB_BC_VALUE  ghost = c                                  (float / double quantities)
+ *   SB_BC_EVEN   ghost = its mirror image about the face    (any element type: a plain copy)
+ *   SB_BC_ODD    ghost = 2c - its mirror image              (float / double; c is the value AT the face, ODD(0) = antisymmetric)
+ * Mirror along axis a in allocation coordinates, with ghost widths g- / g+ and compute cells [g-, g- + n): a low ghost
+ * cell i reads 2 g- - 1 - i, a high ghost cell i reads 2 (g- + n) - 1 - i.  EVEN and ODD need g <= n on their side.
+ * Regions: for each of the 26 directions d with radius27(d) > 0, the ghost box halo_pos(d, size, r, 1) of extent
+ * halo_extent(d, size, r).  A region is written when a non-zero component of d points across a face whose kind is not
+ * NONE; those are its wall axes A.  For a cell p of it: v = the allocation at p mirrored on every axis of A, then for each
+ * a in A, in order x, y, z: VALUE v = c, EVEN v unchanged, ODD v = 2c - v, all in the quantity's type.  This equals the x
+ * walls, then the y walls, then the z walls applied as separate passes, but every source cell is one no BC writes, so
+ * the launch needs no ordering inside.  On non-wall axes the source is a ghost cell the exchange filled: launch after
+ * every write of the exchange into this subdomain has completed.
+ * ------------------------------------------------------------------------------------------- */
+typedef enum sb_bc_kind { SB_BC_NONE = 0, SB_BC_VALUE = 1, SB_BC_EVEN = 2, SB_BC_ODD = 3 } sb_bc_kind;
+typedef enum sb_dtype { SB_DTYPE_RAW = 0, SB_DTYPE_F32 = 1, SB_DTYPE_F64 = 2 } sb_dtype;
+
+/* One BC region of a subdomain.  pos / extent: the ghost box in allocation coordinates.  mirror[a]: on a wall axis the
+ * source coordinate is mirror[a] - p[a]; on the other axes mirror[a] = -1 and the source coordinate is p[a].
+ * faces: bit f set when face f (numbered as above) is applied to this region; they are applied in order x, y, z. */
+typedef struct sb_bc_region {
+  int64_t dir[3];
+  int64_t pos[3];
+  int64_t extent[3];
+  int64_t mirror[3];
+  int32_t faces;
+  int32_t reserved;
+} sb_bc_region;
+
+/* Host only.  The BC regions of a subdomain of compute size `size` whose faces carry `kinds` (sb_bc_kind, per face;
+ * NONE on every face that is not a wall of this subdomain), in direction order z, y, x ascending (dir -1 first).
+ * Writes at most cap regions to out (out may be NULL with cap 0) and returns their total number (<= 26), or
+ * SB_ERR_INVALID when a kind is unknown or an EVEN / ODD face has a ghost width larger than the subdomain on its axis. */
+int sb_bc_regions(const int64_t size[3], const int64_t radius27[27], const int32_t kinds[6], sb_bc_region *out, int cap);
+
+/* One quantity of a BC plan: its allocation (the CURRENT buffer the plan will read and write), element type, and
+ * per-face kind and value.  dtype RAW takes elem_size 1, 2, 4, 8 or 16 and allows NONE and EVEN only; F32 needs
+ * elem_size 4, F64 elem_size 8.  value[f] is converted to the quantity's type. */
+typedef struct sb_bc_quantity {
+  sb_pitched data;
+  int64_t elem_size;
+  double value[6];
+  int32_t dtype;
+  int32_t kind[6];
+} sb_bc_quantity;
+
+/* A persistent plan: every BC region of every quantity of one subdomain, filled by ONE launch on `device`.  The tile
+ * table is uploaded here; size / radius27 describe the subdomain (every quantity has the same geometry).  Errors
+ * (SB_ERR_INVALID with a message): a kind outside sb_bc_kind, VALUE or ODD on a RAW quantity, a mismatched elem_size,
+ * EVEN or ODD with a ghost width larger than the subdomain.  A plan with nothing to write launches nothing. */
+typedef struct sb_bc_plan sb_bc_plan;
+int sb_bc_plan_create(sb_bc_plan **out, int device, const sb_bc_quantity *quantities, int64_t n, const int64_t size[3],
+                      const int64_t radius27[27]);
+int sb_bc_plan_launch(sb_bc_plan *plan, void *stream);
+int64_t sb_bc_plan_bytes(const sb_bc_plan *plan); /* ghost-cell bytes written per launch */
+int sb_bc_plan_destroy(sb_bc_plan *plan);
+
+/* ---------------------------------------------------------------------------------------------
  * 7-point jacobi step (the reference's user kernel, bin/jacobi3d.cu:40-85) over a region.
  * dtype_size 4 = float, 8 = double.  acc_origin = global coordinate of allocation element (0,0,0)
  * (Accessor origin, include/stencil/local_domain.cuh:153-173).  [lo,hi) = region to update,

@@ -34,6 +34,7 @@ FusedJacobi3d::FusedJacobi3d(DistributedDomain &dd, size_t quantity, size_t elem
     if (1 != r.dir(f)) fused_ = false;
   for (const LocalDomain &d : doms) // the fused kernel wants >= 16 cells along x and neighbours of its own extent
     if (d.size().x < 16 || !(d.size() == doms[0].size())) fused_ = false;
+  if (dd_.has_boundary_conditions()) fused_ = false; // the wall ghost cells are filled by exchange(), which the fused kernel replaces
 
   Placement *pl = dd_.get_placement();
   const Topology &topo = dd_.get_topology();

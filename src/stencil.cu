@@ -29,7 +29,7 @@ void set3(int64_t out[3], const Dim3 &d) {
 
 DistributedDomain::DistributedDomain(size_t x, size_t y, size_t z)
     : size_(x, y, z), placement_(nullptr), radius_(Radius::constant(0)), flags_(Method::Default),
-      strategy_(PlacementStrategy::NodeAware), boundary_(Topology::Boundary::PERIODIC), parity_(0), mailbox_(nullptr), epoch_(0), numBytesCudaMpi_(0), numBytesColoDirectAccess_(0),
+      strategy_(PlacementStrategy::NodeAware), boundary_{Topology::Boundary::PERIODIC, Topology::Boundary::PERIODIC, Topology::Boundary::PERIODIC}, parity_(0), mailbox_(nullptr), epoch_(0), numBytesCudaMpi_(0), numBytesColoDirectAccess_(0),
       numBytesColoPackMemcpyUnpack_(0), numBytesCudaMemcpyPeer_(0), numBytesCudaKernel_(0) {
 #ifdef STENCIL_SETUP_STATS
   timeMpiTopo_ = timeNodeGpus_ = timePeerEn_ = timePlacement_ = timePlan_ = timeRealize_ = timeCreate_ = 0;
@@ -81,6 +81,12 @@ void DistributedDomain::destroy_plans() {
       (*sides)[parity].clear();
     }
   }
+  for (int parity = 0; parity < 2; ++parity) {
+    for (sb_bc_plan *p : bcPlans_[parity])
+      if (p) sb_bc_plan_destroy(p);
+    bcPlans_[parity].clear();
+  }
+  bcSenders_.clear();
   for (size_t i = 0; i < stagingBufs_.size(); ++i) {
     cudaSetDevice(stagingDevs_[i]);
     cudaFree(stagingBufs_[i]);
@@ -129,11 +135,21 @@ void DistributedDomain::do_placement() {
     break;
   }
   nvtxRangePop();
-  topology_ = Topology(placement_->dim(), boundary_);
+  topology_ = Topology(placement_->dim(), boundary_[0], boundary_[1], boundary_[2]);
 }
 
 void DistributedDomain::realize() {
   do_placement();
+  for (const auto &kv : bcs_) { // the BC errors that need no subdomain geometry (sb_bc_plan_create checks the rest)
+    const stencil::BC &bc = kv.second;
+    const size_t q = kv.first.first;
+    const int f = kv.first.second;
+    if (bc.kind == stencil::BC::Kind::NONE) continue;
+    if (boundary_[f / 2] == Topology::Boundary::PERIODIC)
+      LOG_FATAL("quantity " << q << ": a boundary condition on face " << f << " (-x,+x,-y,+y,-z,+z) of a periodic axis; set_boundary FIXED first");
+    if ((bc.kind == stencil::BC::Kind::VALUE || bc.kind == stencil::BC::Kind::ODD) && 0 == dataDtype_[q])
+      LOG_FATAL("quantity " << q << ": VALUE and ODD boundary conditions need a float or double quantity (EVEN copies any type)");
+  }
 
   // LocalDomain copies share raw device pointers: fill the vector while they are still null,
   // then allocate in place.
@@ -533,6 +549,7 @@ void DistributedDomain::plan_exchange() {
       unpackPlans_[parity].push_back(up);
     }
   }
+  plan_boundaries(planFile);
   planFile.close();
   parity_ = 0;
 
@@ -558,6 +575,62 @@ void DistributedDomain::plan_exchange() {
   // every rank learns the global volume
   for (uint64_t *b : {&numBytesCudaMpi_, &numBytesColoDirectAccess_, &numBytesColoPackMemcpyUnpack_, &numBytesCudaMemcpyPeer_, &numBytesCudaKernel_})
     MPI_Allreduce(MPI_IN_PLACE, b, 1, MPI_UINT64_T, MPI_SUM, MPI_COMM_WORLD);
+}
+
+// Boundary conditions: per local subdomain and swap parity, one sb_bc_plan over the BCs of its wall faces (faces with no
+// neighbour), and the local subdomains whose phase 1 writes into it.
+void DistributedDomain::plan_boundaries(std::ofstream &planFile) {
+  bcSenders_.assign(domains_.size(), {});
+  if (!has_boundary_conditions()) return;
+  static const char *const kKind[4] = {"NONE", "VALUE", "EVEN", "ODD"};
+  static const char *const kFace[6] = {"-x", "+x", "-y", "+y", "-z", "+z"};
+  const Dim3 faceDir[6] = {Dim3(-1, 0, 0), Dim3(1, 0, 0), Dim3(0, -1, 0), Dim3(0, 1, 0), Dim3(0, 0, -1), Dim3(0, 0, 1)};
+  int64_t r27[27];
+  for (int z = -1, i = 0; z <= 1; ++z)
+    for (int y = -1; y <= 1; ++y)
+      for (int x = -1; x <= 1; ++x) r27[i++] = int64_t(radius_.dir(x, y, z));
+  planFile << "\n== boundary conditions ==\n";
+  for (int parity = 0; parity < 2; ++parity) {
+    for (size_t di = 0; di < domains_.size(); ++di) {
+      const LocalDomain &d = domains_[di];
+      std::vector<sb_bc_quantity> qs(dataElemSize_.size());
+      for (size_t q = 0; q < qs.size(); ++q) {
+        sb_bc_quantity &Q = qs[q];
+        Q = sb_bc_quantity{};
+        Q.data = as_sb(0 == parity ? d.curr_data(q) : d.next_data(q));
+        Q.elem_size = int64_t(dataElemSize_[q]);
+        Q.dtype = dataDtype_[q];
+        for (int f = 0; f < 6; ++f) {
+          const auto it = bcs_.find(std::make_pair(q, f));
+          if (it == bcs_.end() || topology_.get_neighbor(domainIdx_[di], faceDir[f]).exists) continue;
+          Q.kind[f] = int32_t(it->second.kind);
+          Q.value[f] = it->second.value;
+          if (0 == parity && it->second.kind != stencil::BC::Kind::NONE)
+            planFile << domainIdx_[di] << " q" << q << " " << kFace[f] << " " << kKind[int(it->second.kind)] << "(" << it->second.value << ")\n";
+        }
+      }
+      int64_t sz[3];
+      set3(sz, d.size());
+      sb_bc_plan *plan = nullptr;
+      if (SB_OK != sb_bc_plan_create(&plan, d.gpu(), qs.data(), int64_t(qs.size()), sz, r27)) LOG_FATAL("boundary conditions: " << sb_last_error());
+      if (0 == parity) planFile << domainIdx_[di] << " BC plan: " << sb_bc_plan_bytes(plan) << "B per exchange\n";
+      if (0 == sb_bc_plan_bytes(plan)) {
+        sb_bc_plan_destroy(plan);
+        plan = nullptr;
+      }
+      bcPlans_[parity].push_back(plan);
+    }
+  }
+  for (size_t di = 0; di < domains_.size(); ++di) {
+    std::set<size_t> senders;
+    for (int z = -1; z <= 1; ++z)
+      for (int y = -1; y <= 1; ++y)
+        for (int x = -1; x <= 1; ++x) {
+          const Topology::OptionalNeighbor nb = topology_.get_neighbor(domainIdx_[di], Dim3(x, y, z));
+          if ((x || y || z) && nb.exists && placement_->get_rank(nb.index) == rank_) senders.insert(size_t(placement_->get_subdomain_id(nb.index)));
+        }
+    bcSenders_[di].assign(senders.begin(), senders.end());
+  }
 }
 
 void DistributedDomain::swap() {
@@ -605,13 +678,14 @@ void DistributedDomain::exchange_async() {
     anyStaged = anyStaged || (scatter[di] != nullptr);
   }
   if (ranks) flags_finish(); // every remote sender's phase 1 has landed (and stream order covers the local ones below)
-  if (anyStaged) {
-    if (!ranks) {
-      for (size_t di = 0; di < plans.size(); ++di) {
-        CUDA_RUNTIME(cudaSetDevice(domains_[di].gpu()));
-        CUDA_RUNTIME(cudaEventRecord(phase1Done_[di], streams_[di]));
-      }
+  const std::vector<sb_bc_plan *> &bc = bcPlans_[parity_];
+  if (!ranks && (anyStaged || !bc.empty())) {
+    for (size_t di = 0; di < plans.size(); ++di) {
+      CUDA_RUNTIME(cudaSetDevice(domains_[di].gpu()));
+      CUDA_RUNTIME(cudaEventRecord(phase1Done_[di], streams_[di]));
     }
+  }
+  if (anyStaged) {
     for (size_t di = 0; di < plans.size(); ++di) {
       if (!scatter[di]) continue;
       CUDA_RUNTIME(cudaSetDevice(domains_[di].gpu()));
@@ -621,6 +695,16 @@ void DistributedDomain::exchange_async() {
         LOG_FATAL("exchange scatter: " << sb_last_error());
       }
     }
+  }
+  // boundary conditions: after this subdomain's phase 2 (stream order), the phase 1 of its local senders (events) and,
+  // with ranks, every remote sender's phase 1 (flags_finish made every stream wait for it)
+  for (size_t di = 0; di < bc.size(); ++di) {
+    if (!bc[di]) continue;
+    CUDA_RUNTIME(cudaSetDevice(domains_[di].gpu()));
+    if (!ranks)
+      for (size_t sj : bcSenders_[di])
+        if (sj != di) CUDA_RUNTIME(cudaStreamWaitEvent(streams_[di], phase1Done_[sj], 0));
+    if (SB_OK != sb_bc_plan_launch(bc[di], streams_[di])) LOG_FATAL("exchange boundary conditions: " << sb_last_error());
   }
   nvtxRangePop();
 }

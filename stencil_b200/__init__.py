@@ -6,7 +6,14 @@ The compute lives in hand-written sm_90a CUDA (stencil_b200/csrc) behind a C ABI
 from ._lib import LIB_PATH, StencilError, lib  # noqa: F401
 from .domain import (  # noqa: F401
     ALL_DIRS,
+    BC,
+    BCKind,
+    BCPlan,
+    Boundary,
     CopyPlan,
+    FACES,
+    Topology,
+    bc_regions,
     DataHandle,
     DistributedDomain,
     LocalDomain,

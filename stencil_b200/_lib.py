@@ -50,6 +50,33 @@ class HaloPush(C.Structure):
     _fields_ = [("nbr", Pitched * 6), ("nbr_zsize", C.c_int64 * 6), ("x_dense", C.c_int64 * 2), ("x_recv", C.c_void_p * 2)]
 
 
+class BcRegion(C.Structure):
+    """sb_bc_region: one ghost box a boundary condition writes, with its source map."""
+
+    _fields_ = [
+        ("dir", C.c_int64 * 3),
+        ("pos", C.c_int64 * 3),
+        ("extent", C.c_int64 * 3),
+        ("mirror", C.c_int64 * 3),
+        ("faces", C.c_int32),
+        ("reserved", C.c_int32),
+    ]
+
+
+class BcQuantity(C.Structure):
+    """sb_bc_quantity: one quantity of a boundary-condition plan."""
+
+    _fields_ = [
+        ("data", Pitched),
+        ("elem_size", C.c_int64),
+        ("value", C.c_double * 6),
+        ("dtype", C.c_int32),
+        ("kind", C.c_int32 * 6),
+    ]
+
+
+I6 = C.c_int32 * 6
+
 FUSED_MAX_GROUPS = 4096  # SB_FUSED_MAX_GROUPS
 
 
@@ -83,6 +110,11 @@ _SIGS = {
     "sb_copy_plan_num_tiles": (C.c_int64, [C.c_void_p]),
     "sb_copy_plan_num_tma_segments": (C.c_int64, [C.c_void_p]),
     "sb_copy_plan_destroy": (C.c_int, [C.c_void_p]),
+    "sb_bc_regions": (C.c_int, [I3, I27, I6, C.POINTER(BcRegion), C.c_int]),
+    "sb_bc_plan_create": (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.POINTER(BcQuantity), C.c_int64, I3, I27]),
+    "sb_bc_plan_launch": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "sb_bc_plan_bytes": (C.c_int64, [C.c_void_p]),
+    "sb_bc_plan_destroy": (C.c_int, [C.c_void_p]),
     "sb_signal": (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.c_uint32, C.c_int, C.c_void_p]),
     "sb_wait": (C.c_int, [C.c_void_p, C.c_int, C.c_uint32, C.c_int, C.c_void_p]),
     "sb_jacobi3d": (C.c_int, [Pitched, Pitched, C.c_int, I3, I3, I3, I3, I3, C.c_void_p]),

@@ -14,6 +14,7 @@
 #include <cuda_runtime.h>
 
 #include "box_copy.cuh"
+#include "boundary.cuh"
 #include "astaroth.cuh"
 #include "jacobi.cuh"
 
@@ -455,7 +456,60 @@ __global__ void wait_kernel(const uint32_t *slots, int n, uint32_t value) {
   __threadfence_system();
 }
 
+// ------------------------------------------------------------------------------------------- boundary conditions
+const char *const kFaceName[6] = {"-x", "+x", "-y", "+y", "-z", "+z"};
+
+// The BC regions of one subdomain (the geometry behind sb_bc_regions and sb_bc_plan_create).
+int bc_regions(const int64_t size[3], const int64_t r27[27], const int32_t kinds[6], std::vector<sb_bc_region> &out) {
+  if (!size || !r27 || !kinds) return fail(SB_ERR_INVALID, "null argument");
+  for (int f = 0; f < 6; ++f) {
+    if (kinds[f] < SB_BC_NONE || kinds[f] > SB_BC_ODD) return fail(SB_ERR_INVALID, "face %s: unknown BC kind %d", kFaceName[f], int(kinds[f]));
+    const int a = f / 2, s = (f % 2) ? 1 : -1;
+    const int64_t g = r27[(a == 2 ? s + 1 : 1) * 9 + (a == 1 ? s + 1 : 1) * 3 + (a == 0 ? s + 1 : 1)];
+    if ((kinds[f] == SB_BC_EVEN || kinds[f] == SB_BC_ODD) && g > size[a])
+      return fail(SB_ERR_INVALID, "face %s: EVEN and ODD mirror the compute cells, the ghost width %lld exceeds the subdomain's %lld cells",
+                  kFaceName[f], (long long)g, (long long)size[a]);
+  }
+  const Radius r = radius_of(r27);
+  const Dim3 sz = d3(size);
+  for (int z = -1; z <= 1; ++z)
+    for (int y = -1; y <= 1; ++y)
+      for (int x = -1; x <= 1; ++x) {
+        const int d[3] = {x, y, z};
+        if ((0 == x && 0 == y && 0 == z) || 0 == r27[(z + 1) * 9 + (y + 1) * 3 + (x + 1)]) continue;
+        int32_t faces = 0;
+        for (int a = 0; a < 3; ++a)
+          if (d[a] && kinds[2 * a + (d[a] > 0)] != SB_BC_NONE) faces |= 1 << (2 * a + (d[a] > 0));
+        if (!faces) continue;
+        const Dim3 dir(x, y, z);
+        const Dim3 pos = stencil::geom::halo_pos(dir, sz, r, true), ext = stencil::geom::halo_extent(dir, sz, r);
+        if (0 == ext.flatten()) continue;
+        sb_bc_region reg{};
+        put(dir, reg.dir);
+        put(pos, reg.pos);
+        put(ext, reg.extent);
+        for (int a = 0; a < 3; ++a) {
+          reg.mirror[a] = -1;
+          if (!(faces & (3 << (2 * a)))) continue;
+          const int64_t gm = a == 0 ? r.x(-1) : a == 1 ? r.y(-1) : r.z(-1);
+          reg.mirror[a] = d[a] < 0 ? 2 * gm - 1 : 2 * (gm + size[a]) - 1;
+        }
+        reg.faces = faces;
+        out.push_back(reg);
+      }
+  return SB_OK;
+}
+
 } // namespace
+
+struct sb_bc_plan {
+  int device = 0;
+  sb::BcSeg *segs_dev = nullptr;
+  sb::BcTile *tiles_dev = nullptr;
+  unsigned ntiles = 0;
+  int grid = 0;
+  int64_t bytes = 0;
+};
 
 struct sb_copy_plan {
   int device = 0;
@@ -663,6 +717,136 @@ int sb_copy_plan_destroy(sb_copy_plan *p) {
   if (p->segs_dev) cudaFree(p->segs_dev);
   if (p->tsegs_dev) cudaFree(p->tsegs_dev);
   delete p->maps_host;
+  if (p->tiles_dev) cudaFree(p->tiles_dev);
+  delete p;
+  return SB_OK;
+}
+
+// ----------------------------------------------------------------------------------------- boundary conditions
+int sb_bc_regions(const int64_t size[3], const int64_t radius27[27], const int32_t kinds[6], sb_bc_region *out, int cap) {
+  if (cap < 0 || (cap > 0 && !out)) return fail(SB_ERR_INVALID, "bad output buffer");
+  std::vector<sb_bc_region> regs;
+  const int rc = bc_regions(size, radius27, kinds, regs);
+  if (rc != SB_OK) return rc;
+  for (size_t i = 0; i < regs.size() && int(i) < cap; ++i) out[i] = regs[i];
+  return int(regs.size());
+}
+
+int sb_bc_plan_create(sb_bc_plan **out, int device, const sb_bc_quantity *quantities, int64_t n, const int64_t size[3],
+                      const int64_t radius27[27]) {
+  if (!out || n < 0 || (n > 0 && !quantities) || !size || !radius27) return fail(SB_ERR_INVALID, "bad arguments to sb_bc_plan_create");
+  for (int a = 0; a < 3; ++a)
+    if (size[a] < 1 || size[a] >= (1ll << 30)) return fail(SB_ERR_INVALID, "subdomain size must be in [1, 2^30) on every axis");
+  std::vector<sb::BcSeg> segs;
+  std::vector<sb::BcTile> tiles;
+  int64_t bytes = 0;
+  for (int64_t q = 0; q < n; ++q) {
+    const sb_bc_quantity &Q = quantities[q];
+    const int64_t es = Q.elem_size;
+    if (Q.dtype == SB_DTYPE_RAW) {
+      if (es <= 0 || (es & (es - 1)) || es > 16) return fail(SB_ERR_INVALID, "quantity %lld: elem_size %lld must be 1, 2, 4, 8 or 16", (long long)q, (long long)es);
+    } else if (Q.dtype == SB_DTYPE_F32 || Q.dtype == SB_DTYPE_F64) {
+      if (es != (Q.dtype == SB_DTYPE_F32 ? 4 : 8)) return fail(SB_ERR_INVALID, "quantity %lld: elem_size %lld does not match its dtype", (long long)q, (long long)es);
+    } else {
+      return fail(SB_ERR_INVALID, "quantity %lld: unknown dtype %d", (long long)q, int(Q.dtype));
+    }
+    for (int f = 0; f < 6; ++f)
+      if (Q.dtype == SB_DTYPE_RAW && (Q.kind[f] == SB_BC_VALUE || Q.kind[f] == SB_BC_ODD))
+        return fail(SB_ERR_INVALID, "quantity %lld, face %s: VALUE and ODD need a floating-point quantity (EVEN copies any type)", (long long)q, kFaceName[f]);
+    std::vector<sb_bc_region> regs;
+    int rc = bc_regions(size, radius27, Q.kind, regs);
+    if (rc != SB_OK) return rc;
+    if (regs.empty()) continue;
+    if (!Q.data.ptr || Q.data.pitch <= 0 || Q.data.ysize <= 0) return fail(SB_ERR_INVALID, "quantity %lld: bad pitched pointer", (long long)q);
+    if ((uintptr_t(Q.data.ptr) % uintptr_t(es)) || (Q.data.pitch % es))
+      return fail(SB_ERR_INVALID, "quantity %lld: pointer and pitch must be multiples of the %lld-byte element", (long long)q, (long long)es);
+    // a value in the quantity's type, carried as an (exact) double
+    auto in_type = [&](double c) { return Q.dtype == SB_DTYPE_F32 ? double(float(c)) : c; };
+    auto twice = [&](double c) { return Q.dtype == SB_DTYPE_F32 ? double(2.0f * float(c)) : 2.0 * c; };
+    for (const sb_bc_region &reg : regs) {
+      sb::BcSeg g{};
+      g.base = static_cast<char *>(Q.data.ptr);
+      g.pitch = Q.data.pitch;
+      g.slice = Q.data.pitch * Q.data.ysize;
+      for (int a = 0; a < 3; ++a) {
+        g.pos[a] = int(reg.pos[a]);
+        g.ext[a] = int(reg.extent[a]);
+        g.mirror[a] = int(reg.mirror[a]);
+      }
+      g.read = 1;
+      for (int a = 0; a < 3; ++a) { // wall faces in order x, y, z: a VALUE face restarts the chain, ODD appends a step
+        if (reg.mirror[a] < 0) continue;
+        const int f = 2 * a + (reg.dir[a] > 0);
+        if (Q.kind[f] == SB_BC_VALUE) {
+          g.read = 0;
+          g.nops = 0;
+          g.value0 = in_type(Q.value[f]);
+        } else if (Q.kind[f] == SB_BC_ODD) {
+          g.twoc[g.nops++] = twice(Q.value[f]);
+        }
+      }
+      g.es = unsigned(es);
+      g.dtype = unsigned(Q.dtype);
+      const long long row_bytes = reg.extent[0] * es;
+      const unsigned rows = unsigned(reg.extent[1] * reg.extent[2]);
+      unsigned rows_per_tile = unsigned(sb::kBcThreads);
+      if (reg.mirror[0] < 0) { // row segment: widest access that divides every row start and the row length
+        const unsigned long long align =
+            (unsigned long long)(uintptr_t)(g.base + reg.pos[0] * es) | (unsigned long long)g.pitch | (unsigned long long)g.slice | (unsigned long long)row_bytes;
+        unsigned vec = 16;
+        while (vec > 1 && (align & (vec - 1))) vec >>= 1;
+        g.vec = vec;
+        g.lg_group = std::min(5u, ceil_log2(unsigned(row_bytes / vec)));
+        // ~16 KiB of payload, and at least one pass of the whole block (kBcThreads >> lg_group rows)
+        rows_per_tile = unsigned(std::max<long long>(sb::kBcThreads >> g.lg_group, sb::kTileBytes / row_bytes));
+      }
+      const unsigned si = unsigned(segs.size());
+      segs.push_back(g);
+      for (unsigned r0 = 0; r0 < rows; r0 += rows_per_tile) tiles.push_back(sb::BcTile{si, r0, std::min(rows_per_tile, rows - r0)});
+      bytes += row_bytes * reg.extent[1] * reg.extent[2];
+    }
+  }
+  DeviceGuard guard(device);
+  if (!guard.ok) return fail(SB_ERR_NOGPU, "cannot select CUDA device %d", device);
+  sb_bc_plan *p = new sb_bc_plan();
+  p->device = device;
+  p->bytes = bytes;
+  p->ntiles = unsigned(tiles.size());
+  if (p->ntiles) {
+    cudaError_t e = cudaMalloc(&p->segs_dev, segs.size() * sizeof(sb::BcSeg));
+    if (e == cudaSuccess) e = cudaMalloc(&p->tiles_dev, tiles.size() * sizeof(sb::BcTile));
+    if (e == cudaSuccess) e = cudaMemcpy(p->segs_dev, segs.data(), segs.size() * sizeof(sb::BcSeg), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(p->tiles_dev, tiles.data(), tiles.size() * sizeof(sb::BcTile), cudaMemcpyHostToDevice);
+    if (e != cudaSuccess) {
+      sb_bc_plan_destroy(p);
+      return fail(SB_ERR_CUDA, "BC plan upload: %s", cudaGetErrorString(e));
+    }
+    int sms = 132;
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
+    const long long cap = (long long)sms * 8;
+    p->grid = int(p->ntiles < cap ? p->ntiles : cap);
+  }
+  *out = p;
+  return SB_OK;
+}
+
+int sb_bc_plan_launch(sb_bc_plan *p, void *stream) {
+  if (!p) return fail(SB_ERR_INVALID, "null plan");
+  if (0 == p->ntiles) return SB_OK;
+  DeviceGuard guard(p->device);
+  if (!guard.ok) return fail(SB_ERR_NOGPU, "cannot select CUDA device %d", p->device);
+  sb::launch_bc_fill(p->segs_dev, p->tiles_dev, p->ntiles, p->grid, static_cast<cudaStream_t>(stream));
+  ++g_launches;
+  SB_CUDA(cudaGetLastError());
+  return SB_OK;
+}
+
+int64_t sb_bc_plan_bytes(const sb_bc_plan *p) { return p ? p->bytes : 0; }
+
+int sb_bc_plan_destroy(sb_bc_plan *p) {
+  if (!p) return SB_OK;
+  DeviceGuard guard(p->device);
+  if (p->segs_dev) cudaFree(p->segs_dev);
   if (p->tiles_dev) cudaFree(p->tiles_dev);
   delete p;
   return SB_OK;

@@ -135,7 +135,11 @@ __device__ __forceinline__ void march_body(const JacobiParams &p, const int bx, 
   const char *pc[RY]; // centre rows, plane z+1
   const char *ph[RY]; // edge scalar of each row, plane z
   char *pw[RY];       // output rows, plane z
-  const bool edge_lane = (lane == 0) || (lane == 31);
+  // A region that ends inside a strip: when the vector after the last compute cell would hang over the end of the row
+  // (ghost width 1, the ghost cell is its first element), the next lane loads a stand-in vector instead (xin above), so the
+  // lane holding the last cell loads the ghost cell as its edge scalar, like lane 31 at the end of a strip.
+  const bool tail_lane = !SHIFT && lane != 31 && x + VX == p.hi[0] && x + 2 * VX > p.raw[0];
+  const bool edge_lane = (lane == 0) || (lane == 31) || tail_lane;
   long long phstep = S; // per-plane advance of ph (XPUSH: a dense x-ghost array is z fastest)
   int hxv = lane == 0 ? x - 1 : x + VX;
   bool far = false; // this lane's edge scalar / patched element comes from the other end of the row
@@ -298,7 +302,7 @@ __device__ __forceinline__ void march_body(const JacobiParams &p, const int bx, 
       T left = __shfl_up_sync(0xffffffffu, cc[j].v[VX - 1], 1);
       T right = __shfl_down_sync(0xffffffffu, cc[j].v[0], 1);
       if (lane == 0) left = h;
-      if (lane == 31) right = h;
+      if (lane == 31 || tail_lane) right = h;
       V out;
 #pragma unroll
       for (int i = 0; i < VX; ++i) {
@@ -1057,7 +1061,14 @@ int launch_jacobi(const JacobiParams &p_in, int dtype_size, cudaStream_t stream)
 
   static const int allow_shift = env_int("SB_JACOBI_SHIFT", 1);
   bool shift = false;
-  const int vx = pick_vectors(p, dtype_size, allow_shift != 0, &shift);
+  int vx = pick_vectors(p, dtype_size, allow_shift != 0, &shift);
+  // Unshifted rows: a vector that holds compute cells but hangs over the end of its row is replaced by a stand-in load
+  // (march_body, xin), which would feed wrong values to those cells.  Such a region (e.g. 30 floats with one ghost cell
+  // behind a 12-byte lead) takes the scalar path.  A vector that holds only the ghost cell is handled in march_body.
+  if (!shift && vx > 1 && p.x0a + ((p.hi[0] - 1 - p.x0a) / vx) * vx + vx > p.raw[0]) {
+    vx = 1;
+    p.x0a = p.lo[0];
+  }
   if (dtype_size == 8) {
     if (vx == 2) return shift ? launch_march<double, 2, true>(p, ry, mb, stream) : launch_march<double, 2, false>(p, ry, mb, stream);
     return launch_march<double, 1, false>(p, ry, mb, stream);

@@ -115,13 +115,15 @@ class RemoteDomains:
                     "curr": [open_(h) + off for h, off in dom["curr"]],
                     "next": [open_(h) + off for h, off in dom["next"]],
                 }
-        # neighbour ranks: owners of any subdomain adjacent to one of mine (periodic, symmetric)
-        from .domain import ALL_DIRS, get_neighbor
+        # neighbour ranks: owners of any subdomain adjacent to one of mine (symmetric; none across a wall)
+        from .domain import ALL_DIRS
 
         nbrs = set()
         for idx in dd.domain_idx_:
             for d in ALL_DIRS:
-                nbrs.add(dd._owner[get_neighbor(idx, d, dd.partition_.dim)][0])
+                nb = dd.topology_.get_neighbor(idx, d)
+                if nb is not None:
+                    nbrs.add(dd._owner[nb][0])
         nbrs.discard(w.rank)
         self.nbrs = sorted(nbrs)
         k = len(self.nbrs)
@@ -222,7 +224,7 @@ def share_domains(dd, w: World) -> RemoteDomains:
 # --------------------------------------------------------------------------------------------- NCCL fallback
 def messages_from(dd, src_rank: int) -> List[dict]:
     """The send plan of ANY rank (pure geometry: every rank can compute every other rank's plan)."""
-    from .domain import ALL_DIRS, get_neighbor, halo_extent, halo_pos
+    from .domain import ALL_DIRS, halo_extent, halo_pos
 
     part, radius = dd.partition_, dd.radius_
     out = []
@@ -235,7 +237,9 @@ def messages_from(dd, src_rank: int) -> List[dict]:
             nd = (-d[0], -d[1], -d[2])
             if radius.dir(nd) == 0:
                 continue
-            dst_idx = get_neighbor(idx, d, part.dim)
+            dst_idx = dd.topology_.get_neighbor(idx, d)
+            if dst_idx is None:
+                continue  # a wall: nothing crosses it
             dst_sz = part.subdomain_size(dst_idx)
             ext = halo_extent(nd, dst_sz, radius)
             if ext[0] * ext[1] * ext[2] == 0:

@@ -194,6 +194,137 @@ def get_neighbor(idx: Vec, d: Vec, dim: Vec) -> Vec:
     return tuple((idx[a] + d[a]) % dim[a] for a in range(3))
 
 
+# ------------------------------------------------------------------------------------------ topology and boundaries
+class Boundary(enum.Enum):
+    """How the grid closes along one axis (include/stencil/topology.hpp): PERIODIC wraps around, FIXED ends at a wall."""
+
+    PERIODIC = 1
+    FIXED = 2
+
+
+class Topology:
+    """The grid of subdomains with one Boundary per axis (include/stencil/topology.hpp)."""
+
+    def __init__(self, dim: Vec, boundaries: Sequence[Boundary] = (Boundary.PERIODIC,) * 3):
+        self.dim = tuple(int(v) for v in dim)
+        self.boundaries = tuple(boundaries)
+
+    def get_neighbor(self, idx: Vec, d: Vec) -> Optional[Vec]:
+        """The subdomain one step in direction d from idx; None when the step leaves the grid along a FIXED axis."""
+        out = []
+        for a in range(3):
+            v = idx[a] + d[a]
+            if self.boundaries[a] == Boundary.PERIODIC:
+                v %= self.dim[a]
+            elif not 0 <= v < self.dim[a]:
+                return None
+            out.append(v)
+        return tuple(out)
+
+    def is_wall(self, idx: Vec, face: int) -> bool:
+        """Is face `face` (0..5 = -x, +x, -y, +y, -z, +z) of subdomain idx a wall face (its step has no neighbour)?"""
+        d = [0, 0, 0]
+        d[face // 2] = 1 if face % 2 else -1
+        return self.get_neighbor(idx, tuple(d)) is None
+
+
+class BCKind(enum.IntEnum):
+    """sb_bc_kind"""
+
+    NONE = 0
+    VALUE = 1
+    EVEN = 2
+    ODD = 3
+
+
+FACES: List[Vec] = [(-1, 0, 0), (1, 0, 0), (0, -1, 0), (0, 1, 0), (0, 0, -1), (0, 0, 1)]  # face numbering 0..5
+
+
+def face_index(face: Vec) -> int:
+    face = tuple(int(v) for v in face)
+    if face not in FACES:
+        raise _lib.StencilError(f"{face} is not a face direction (one component +-1, the others 0)")
+    return FACES.index(face)
+
+
+class BC:
+    """A boundary condition of one quantity on one wall face (include/stencil/boundary_condition.hpp):
+    BC.NONE() (ghost cells untouched), BC.VALUE(c) (ghost = c), BC.EVEN() (mirror image), BC.ODD(c=0) (2c - mirror
+    image; c is the value at the face).  The mirror and the order in which walls compose are those of sb_bc_regions."""
+
+    def __init__(self, kind: BCKind = BCKind.NONE, value: float = 0.0):
+        self.kind = BCKind(kind)
+        self.value = float(value)
+
+    @staticmethod
+    def NONE() -> "BC":
+        return BC(BCKind.NONE)
+
+    @staticmethod
+    def VALUE(c: float) -> "BC":
+        return BC(BCKind.VALUE, c)
+
+    @staticmethod
+    def EVEN() -> "BC":
+        return BC(BCKind.EVEN)
+
+    @staticmethod
+    def ODD(c: float = 0.0) -> "BC":
+        return BC(BCKind.ODD, c)
+
+    def __eq__(self, o) -> bool:
+        return isinstance(o, BC) and (self.kind, self.value) == (o.kind, o.value)
+
+    def __repr__(self) -> str:
+        return f"BC({self.kind.name}, {self.value})"
+
+
+def bc_dtype(dtype) -> int:
+    """sb_dtype of a numpy dtype: float32 / float64 carry arithmetic, anything else is copied as raw bytes."""
+    dt = np.dtype(dtype)
+    if dt == np.float32:
+        return 1
+    if dt == np.float64:
+        return 2
+    return 0
+
+
+def bc_regions(size: Vec, radius: Radius, kinds: Sequence[int]) -> List[dict]:
+    """sb_bc_regions: the ghost boxes a subdomain's boundary conditions write (pure geometry, host only).
+    dict(dir, pos, ext, mirror, faces): source coordinate = mirror[a] - p[a] on wall axes (mirror[a] >= 0), else p[a]."""
+    buf = (_lib.BcRegion * 26)()
+    n = check(lib().sb_bc_regions(i3(size), radius.c27(), _lib.I6(*[int(k) for k in kinds]), buf, 26))
+    return [
+        dict(dir=t3(r.dir), pos=t3(r.pos), ext=t3(r.extent), mirror=t3(r.mirror), faces=int(r.faces)) for r in buf[:n]
+    ]
+
+
+class BCPlan:
+    """sb_bc_plan: every boundary-condition region of every quantity of one subdomain, one launch."""
+
+    def __init__(self, device: int, quantities: Sequence[_lib.BcQuantity], size: Vec, radius: Radius):
+        arr = (_lib.BcQuantity * max(1, len(quantities)))(*quantities)
+        h = C.c_void_p()
+        check(lib().sb_bc_plan_create(C.byref(h), device, arr, len(quantities), i3(size), radius.c27()))
+        self._h = h
+        self.device = device
+        self.bytes = int(lib().sb_bc_plan_bytes(h))
+
+    def launch(self, stream=None) -> None:
+        check(lib().sb_bc_plan_launch(self._h, stream_ptr(stream)))
+
+    def destroy(self) -> None:
+        if self._h:
+            lib().sb_bc_plan_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.destroy()
+        except Exception:
+            pass
+
+
 # ------------------------------------------------------------------------------------------ LocalDomain
 class LocalDomain:
     """One subdomain on one GPU: curr/next allocation per quantity (local_domain.cuh:34-276,
@@ -401,10 +532,60 @@ class DistributedDomain:
         self._nccl = None  # NCCL fallback (dist.NcclExchange)
         self._use_nccl = False
         self._epoch = 0
+        self.boundary_: Tuple[Boundary, Boundary, Boundary] = (Boundary.PERIODIC,) * 3
+        self.bcs_: Dict[Tuple[int, int], BC] = {}  # (quantity, face 0..5) -> BC
+        self.topology_: Optional[Topology] = None
+        self._bc_plans: List[List[Optional[BCPlan]]] = []  # [parity][local domain]
 
     # -- configuration (call before realize)
     def set_radius(self, r) -> None:
         self.radius_ = r if isinstance(r, Radius) else Radius.constant(int(r))
+
+    def set_boundary(self, x: Boundary, y: Optional[Boundary] = None, z: Optional[Boundary] = None) -> None:
+        """How the grid closes: one Boundary for all three axes, or one per axis (x, y, z).  On a FIXED axis no message
+        crosses the grid's outer faces; their ghost cells are filled by the boundary conditions set for them."""
+        if (y is None) != (z is None):
+            raise _lib.StencilError("set_boundary takes one Boundary (all axes) or three (x, y, z)")
+        b = (x, x, x) if y is None else (x, y, z)
+        for v in b:
+            if not isinstance(v, Boundary):
+                raise _lib.StencilError(f"{v!r} is not a Boundary")
+        self.boundary_ = tuple(b)
+
+    def set_boundary_condition(self, h: DataHandle, face: Vec, bc: BC) -> None:
+        """The boundary condition of quantity h on the wall face `face` ((+-1,0,0), (0,+-1,0) or (0,0,+-1)) of the whole
+        grid; call before realize().  exchange() fills the ghost cells behind that face."""
+        if not isinstance(bc, BC):
+            raise _lib.StencilError(f"{bc!r} is not a BC")
+        self.bcs_[(h.id, face_index(face))] = bc
+
+    def get_topology(self) -> Optional[Topology]:
+        return self.topology_
+
+    def has_boundary_conditions(self) -> bool:
+        return any(bc.kind != BCKind.NONE for bc in self.bcs_.values())
+
+    def wall_kinds(self, idx: Vec, q: int) -> Tuple[List[int], List[float]]:
+        """Per face of subdomain idx: (sb_bc_kind, value) of quantity q, NONE on faces that are not walls of idx."""
+        kinds, values = [0] * 6, [0.0] * 6
+        for (qq, f), bc in self.bcs_.items():
+            if qq == q and self.topology_.is_wall(idx, f):
+                kinds[f], values[f] = int(bc.kind), bc.value
+        return kinds, values
+
+    def _check_boundaries(self) -> None:
+        """The errors realize() reports before it allocates anything (host only)."""
+        for (q, f), bc in sorted(self.bcs_.items()):
+            if bc.kind == BCKind.NONE:
+                continue
+            if self.boundary_[f // 2] == Boundary.PERIODIC:
+                raise _lib.StencilError(f"quantity {q}: a boundary condition on face {FACES[f]} of a periodic axis (set_boundary FIXED first)")
+            if bc.kind in (BCKind.VALUE, BCKind.ODD) and bc_dtype(self.dtypes_[q]) == 0:
+                raise _lib.StencilError(f"quantity {q} ({self.dtypes_[q]}): {bc.kind.name} needs float32 or float64 (EVEN copies any type)")
+        if self.has_boundary_conditions():
+            for idx in self.partition_.indices():
+                for q in range(len(self.dtypes_)):
+                    bc_regions(self.partition_.subdomain_size(idx), self.radius_, self.wall_kinds(idx, q)[0])  # raises on g > n
 
     def add_data(self, dtype, name: str = "") -> DataHandle:
         self.dtypes_.append(np.dtype(dtype))
@@ -479,6 +660,7 @@ class DistributedDomain:
         trivial = self.strategy_ == PlacementStrategy.Trivial
         # one node: NodePartition(size, radius, 1 node, n_sub gpus)  (partition.hpp:157-211)
         self.partition_ = Partition(self.size_, self.radius_, 1, n_sub, trivial=trivial)
+        self.topology_ = Topology(self.partition_.dim, self.boundary_)
         self._world = world
         self._assign_owners()
 
@@ -486,6 +668,7 @@ class DistributedDomain:
         from . import dist as _dist
 
         self.do_placement()
+        self._check_boundaries()
         world = self._world
         part = self.partition_
         all_idx = part.indices()
@@ -567,7 +750,7 @@ class DistributedDomain:
         if os.environ.get("SB_NO_STAGING", "0") == "1":
             return
         for di, dst_idx in enumerate(self.domain_idx_):
-            srcs = {get_neighbor(dst_idx, d, self.partition_.dim) for d in ALL_DIRS}
+            srcs = {self.topology_.get_neighbor(dst_idx, d) for d in ALL_DIRS} - {None}
             for src_idx in sorted(srcs):
                 if self._gpu_key(src_idx) == self._gpu_key(dst_idx):
                     continue
@@ -600,7 +783,9 @@ class DistributedDomain:
             for dirv in ALL_DIRS:
                 if self.radius_.dir(_neg(dirv)) == 0:
                     continue  # src/stencil.cu:344
-                dst_idx = get_neighbor(idx, dirv, part.dim)
+                dst_idx = self.topology_.get_neighbor(idx, dirv)
+                if dst_idx is None:
+                    continue  # a wall: nothing crosses it
                 dst_sz = part.subdomain_size(dst_idx)
                 ext = halo_extent(_neg(dirv), dst_sz, self.radius_)  # stencil.cu:361-363
                 if ext[0] * ext[1] * ext[2] == 0:
@@ -695,6 +880,29 @@ class DistributedDomain:
                 if d_idx == tuple(dst_idx) and self._owner[src_idx][0] == self._world.rank:
                     snd.add(self._owner[src_idx][1])
             self._stage_senders.append(sorted(snd))
+        self._build_bc_plans()
+
+    def _build_bc_plans(self) -> None:
+        """One boundary-condition plan per local subdomain and swap parity (None where the subdomain has no wall face
+        with a BC), and the local subdomains whose phase 1 writes into each one (the BC launch waits for them)."""
+        self._bc_plans, self._bc_senders = [], []
+        if not self.has_boundary_conditions():
+            return
+        for parity in (0, 1):
+            plans = []
+            for di, d in enumerate(self.domains_):
+                idx = self.domain_idx_[di]
+                qs = []
+                for q in range(d.num_data()):
+                    kinds, values = self.wall_kinds(idx, q)
+                    p, _ = self._pitched_of(idx, q, parity)
+                    qs.append(_lib.BcQuantity(p, d.elem_size(q), (C.c_double * 6)(*values), bc_dtype(self.dtypes_[q]), _lib.I6(*kinds)))
+                plan = BCPlan(d.gpu(), qs, d.size(), self.radius_)
+                plans.append(plan if plan.bytes else None)
+            self._bc_plans.append(plans)
+        for idx in self.domain_idx_:
+            srcs = {self.topology_.get_neighbor(idx, dv) for dv in ALL_DIRS} - {None}
+            self._bc_senders.append(sorted({self._owner[s][1] for s in srcs if self._owner[s][0] == self._world.rank}))
 
     # -- the hot path
     def exchange_async(self) -> None:
@@ -702,11 +910,17 @@ class DistributedDomain:
         import torch
 
         plans, unplans = self._plans[self._parity], self._unpack_plans[self._parity]
+        bcs = self._bc_plans[self._parity] if self._bc_plans else None
         if self._remote is not None:
             self._epoch += 1
             self._remote.begin(self._epoch, self._streams)
+        phase1 = []
         for plan, s in zip(plans, self._streams):
             plan.launch(s)
+            if bcs is not None:  # the BC launch of every receiver waits for its local senders' phase 1
+                ev = torch.cuda.Event()
+                ev.record(s)
+                phase1.append(ev)
         if self._remote is not None:
             self._remote.finish(self._epoch, self._streams)  # every remote sender's phase 1 has landed
             if len(self._streams) > 1:
@@ -732,6 +946,23 @@ class DistributedDomain:
                     if sj != di:
                         self._streams[di].wait_event(events[sj])
                 u.launch(self._streams[di])
+        # boundary conditions: after this subdomain's phase 2 (stream order), its local senders' phase 1 (events), the
+        # remote senders' phase 1 (RemoteDomains.finish above) and the NCCL unpack (stream 0)
+        if bcs is not None:
+            nccl_done = None
+            if self._nccl is not None and len(self._streams) > 1:
+                nccl_done = torch.cuda.Event()
+                nccl_done.record(self._streams[0])
+            for di, b in enumerate(bcs):
+                if b is None:
+                    continue
+                s = self._streams[di]
+                for sj in self._bc_senders[di]:
+                    if sj != di:
+                        s.wait_event(phase1[sj])
+                if nccl_done is not None and di != 0:
+                    s.wait_event(nccl_done)
+                b.launch(s)
 
     def exchange(self) -> None:
         """DistributedDomain::exchange (src/stencil.cu:1002-1186): returns when every ghost cell of
@@ -752,11 +983,11 @@ class DistributedDomain:
         self._parity ^= 1
 
     def close(self) -> None:
-        for plans in self._plans + getattr(self, "_unpack_plans", []):
+        for plans in self._plans + getattr(self, "_unpack_plans", []) + self._bc_plans:
             for p in plans:
                 if p is not None:
                     p.destroy()
-        self._plans, self._unpack_plans = [], []
+        self._plans, self._unpack_plans, self._bc_plans = [], [], []
 
         if self._remote is not None:
             self._remote.close()

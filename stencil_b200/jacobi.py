@@ -13,8 +13,8 @@ from typing import Tuple
 
 import numpy as np
 
-from ._lib import HaloPush, Pitched, check, i3, lib, stream_ptr
-from .domain import DataHandle, DistributedDomain, Radius
+from ._lib import HaloPush, Pitched, StencilError, check, i3, lib, stream_ptr
+from .domain import Boundary, DataHandle, DistributedDomain, Radius
 
 
 def jacobi_radius() -> Radius:
@@ -82,6 +82,8 @@ class Jacobi3D:
     def __init__(self, dd: DistributedDomain, h: DataHandle, overlap: bool = True):
         import torch
 
+        if any(b != Boundary.PERIODIC for b in dd.boundary_):
+            raise StencilError("Jacobi3D runs on periodic grids only: this domain has a non-periodic axis")
         self.dd, self.h, self.overlap = dd, h, overlap
         self.creg = dd.get_compute_region()
         self.streams = [torch.cuda.Stream(device=d.gpu()) for d in dd.domains()]

@@ -1,0 +1,35 @@
+"""Boundary conditions across processes: the Python layer under torchrun (tests/mp_boundary_check.py) and the C++ API
+under bin/sb_mpirun (tests/cpp/test_boundary_multigpu.cu, which also checks FusedJacobi3d on a walled domain).  With
+fewer GPUs than ranks the ranks share GPUs, so both run on a one-GPU machine."""
+import os
+import subprocess
+import sys
+
+import pytest
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+BIN = os.path.join(ROOT, "bin")
+pytestmark = pytest.mark.gpu
+
+
+def mpirun_env():
+    return {k: v for k, v in os.environ.items() if k not in ("WORLD_SIZE", "RANK", "LOCAL_RANK")}
+
+
+@pytest.mark.parametrize("ranks", [1, 2, 4])
+def test_cpp_boundary_conditions(tmp_path, ranks):
+    exe = os.path.join(BIN, "test_boundary_multigpu")
+    if not os.path.exists(exe):
+        pytest.fail("bin/test_boundary_multigpu not built -- run `make`")
+    cmd = [exe] if ranks == 1 else [os.path.join(BIN, "sb_mpirun"), "-n", str(ranks), exe]
+    out = subprocess.run(cmd, cwd=tmp_path, env=mpirun_env(), capture_output=True, text=True, timeout=900)
+    assert out.returncode == 0 and "ALL OK" in out.stdout, out.stdout[-3000:] + out.stderr[-3000:]
+    assert f"on {ranks} rank(s)" in out.stdout
+
+
+@pytest.mark.parametrize("ranks", [2, 4])
+def test_python_boundary_conditions_one_process_per_rank(ranks):
+    cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", f"--nproc-per-node={ranks}", "--master-addr", "127.0.0.1",
+           "--master-port", str(29540 + ranks), os.path.join(ROOT, "tests", "mp_boundary_check.py")]
+    out = subprocess.run(cmd, env=mpirun_env(), capture_output=True, text=True, timeout=900)
+    assert out.returncode == 0 and "mp_boundary_check OK" in out.stdout, out.stdout[-2000:] + out.stderr[-4000:]
