@@ -1,6 +1,6 @@
 # stencil_b200 build: hand-written sm_90a (H100) CUDA, no cmake needed.
 #   make            -> stencil_b200/libstencil_b200.so (C ABI + kernels), lib/libstencil.a (C++ API, -rdc) and bin/ :
-#                      sb_mpirun, our jacobi3d_b200 driver and the multi-rank C++ exchange and boundary tests
+#                      sb_mpirun, our jacobi3d_b200 driver and the multi-rank C++ exchange, boundary and reduction tests
 #   make drivers REF=<cwpearson/stencil checkout>
 #                   -> bin/ : the REFERENCE's own drivers and Catch2 suites compiled, unchanged, from
 #                      $(REF)/bin and $(REF)/test against OUR headers and library
@@ -12,7 +12,7 @@ NVCCFLAGS := -O3 -std=c++17 $(ARCH) -lineinfo -Xcompiler -fPIC -Xcompiler -Wall 
 INC       := -Iinclude -Istencil_b200/csrc
 
 # ---- core: kernels + C ABI (shared library, loaded by python and linked by the C++ API)
-CSRC      := stencil_b200/csrc/box_copy.cu stencil_b200/csrc/boundary.cu stencil_b200/csrc/jacobi.cu stencil_b200/csrc/astaroth.cu stencil_b200/csrc/capi.cu
+CSRC      := stencil_b200/csrc/box_copy.cu stencil_b200/csrc/boundary.cu stencil_b200/csrc/reduce.cu stencil_b200/csrc/jacobi.cu stencil_b200/csrc/astaroth.cu stencil_b200/csrc/capi.cu
 COBJ      := $(patsubst stencil_b200/csrc/%.cu,build/csrc/%.o,$(CSRC))
 SO        := stencil_b200/libstencil_b200.so
 
@@ -33,7 +33,8 @@ LIBA      := lib/libstencil.a
 # inside libstencil.a would shadow or clash with the real one)
 LIBMPI    := lib/libmpi_shim.a
 
-all: $(SO) $(LIBA) $(LIBMPI) bin/sb_mpirun bin/jacobi3d_b200 bin/test_exchange_multigpu bin/test_boundary_multigpu
+all: $(SO) $(LIBA) $(LIBMPI) bin/sb_mpirun bin/jacobi3d_b200 bin/test_exchange_multigpu bin/test_boundary_multigpu \
+          bin/test_reduce_multigpu
 
 build/mpi_shim.o: src/mpi_shim.cpp include/mpi_shim/mpi.h
 	@mkdir -p build
@@ -129,6 +130,12 @@ build/drv/test_boundary_multigpu.o: tests/cpp/test_boundary_multigpu.cu $(wildca
 	@mkdir -p $(dir $@)
 	$(NVCC) $(OWNDRVFLAGS) -c $< -o $@
 bin/test_boundary_multigpu: build/drv/test_boundary_multigpu.o $(LIBA) $(LIBMPI)
+	@mkdir -p bin
+	$(NVCC) $(DRVLINK) -o $@ $< $(LIBA) $(LIBMPI)
+build/drv/test_reduce_multigpu.o: tests/cpp/test_reduce_multigpu.cu $(wildcard include/stencil/*) include/stencil_b200.h
+	@mkdir -p $(dir $@)
+	$(NVCC) $(OWNDRVFLAGS) -c $< -o $@
+bin/test_reduce_multigpu: build/drv/test_reduce_multigpu.o $(LIBA) $(LIBMPI)
 	@mkdir -p bin
 	$(NVCC) $(DRVLINK) -o $@ $< $(LIBA) $(LIBMPI)
 

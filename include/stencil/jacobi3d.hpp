@@ -34,6 +34,9 @@ public:
   void init(double value = 0.5); // compute region of curr := value
   void step();                   // one iteration, swap included
   void synchronize();            // wait for everything step() queued
+  // ||curr - next||_2 over the whole grid and every rank (after step(): the 2-norm of the last update); collective,
+  // ordered after the iterations step() queued
+  double residual();
   bool fused() const noexcept { return fused_; }
 
 private:

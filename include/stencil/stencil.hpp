@@ -37,11 +37,13 @@
 #include "stencil/placement_intranoderandom.hpp"
 #include "stencil/radius.hpp"
 #include "stencil/rcstream.hpp"
+#include "stencil/reduce.hpp"
 #include "stencil/topology.hpp"
 #include "stencil/tx.hpp"
 
 struct sb_copy_plan;
 struct sb_bc_plan;
+struct sb_reduce_plan;
 
 class DistributedDomain {
 private:
@@ -112,6 +114,14 @@ private:
   void close_ranks();
   void flags_begin();
   void flags_finish();
+
+  // reductions: per (item list, swap parity), one plan and one device result buffer per local domain
+  struct ReduceCache {
+    std::vector<sb_reduce_plan *> plans;
+    std::vector<sb_reduce_result *> out;
+  };
+  std::map<std::vector<int64_t>, ReduceCache> reducePlans_;
+  void destroy_reduce_plans();
 
   std::string outputPrefix_;
 
@@ -222,6 +232,21 @@ public:
   void exchange_async();
   void exchange_wait();
   cudaStream_t exchange_stream(size_t domain) const { return streams_[domain]; }
+
+  // Reductions over the whole compute region (DESIGN.md section 2.6), the same bits on every rank.  Each call waits for
+  // all work queued on the local devices, launches one plan per local subdomain on its exchange stream, gathers every
+  // rank's per-subdomain results with MPI_Allgather and merges them with sb_reduce_combine in global subdomain-index order
+  // (x fastest).  Collective: every rank must call it with the same items.  The plans (tile tables, scratch, result
+  // buffer) are built once per item list and swap parity and kept until the domain is destroyed, so a program should
+  // reduce a fixed set of item lists rather than build new ones every iteration.
+  template <typename T> stencil::Reduction reduce(const DataHandle<T> &h, stencil::Which which = stencil::Which::curr) {
+    return reduce_many(std::vector<stencil::ReduceItem>(1, stencil::ReduceItem::scalar(h, which)))[0];
+  }
+  template <typename T> stencil::Reduction reduce_diff(const DataHandle<T> &h) { return reduce_many(std::vector<stencil::ReduceItem>(1, stencil::ReduceItem::diff(h)))[0]; }
+  template <typename T> stencil::Reduction reduce_norm(const DataHandle<T> &x, const DataHandle<T> &y, const DataHandle<T> &z) {
+    return reduce_many(std::vector<stencil::ReduceItem>(1, stencil::ReduceItem::norm(x, y, z)))[0];
+  }
+  std::vector<stencil::Reduction> reduce_many(const std::vector<stencil::ReduceItem> &items);
 
   // one CSV file per subdomain: Z,Y,X,<quantities...>
   void write_paraview(const std::string &prefix, bool zeroNaNs = false);

@@ -183,6 +183,54 @@ int64_t sb_bc_plan_bytes(const sb_bc_plan *plan); /* ghost-cell bytes written pe
 int sb_bc_plan_destroy(sb_bc_plan *plan);
 
 /* ---------------------------------------------------------------------------------------------
+ * Deterministic reductions over a box of compute cells (the reference's astaroth reductions, astaroth/reductions.cuh,
+ * RTYPE_MIN / MAX / SUM / RMS of astaroth/user_defines.h:161-169; its jacobi driver has none).
+ * An item is a source evaluated at every cell of the box [lo, hi) (global coordinates; acc_origin = global coordinate
+ * of allocation element (0,0,0), as for sb_jacobi3d).  Ghost cells are never read.  Per cell, in FP64 with separately
+ * rounded operations (no FMA):
+ *   SB_REDUCE_SCALAR  v = a                                   q = v*v
+ *   SB_REDUCE_DIFF    v = a - b                               q = v*v
+ *   SB_REDUCE_NORM3   s = ((a*a + b*b) + c*c), v = sqrt(s)    q = s
+ * with a, b, c = src[0..2] widened to double.  Result: min and max of v (a NaN v makes both NaN), sum = sum of v,
+ * sumsq = sum of q, count = cells.  An empty box gives min = +inf, max = -inf, sum = sumsq = 0, count = 0.
+ * Determinism: the order of every sum is a function of the box and the allocation layout only (not of the SM count or
+ * of which CTA took which tile), so a plan gives the same bits on every launch, in a CUDA graph, and on every rank.
+ * ------------------------------------------------------------------------------------------- */
+typedef enum sb_reduce_kind { SB_REDUCE_SCALAR = 0, SB_REDUCE_DIFF = 1, SB_REDUCE_NORM3 = 2 } sb_reduce_kind;
+
+/* One item.  dtype: SB_DTYPE_F32 or SB_DTYPE_F64, shared by its sources, which also share pitch and ysize.  SCALAR reads
+ * src[0], DIFF src[0] - src[1], NORM3 src[0..2]; unused sources are ignored. */
+typedef struct sb_reduce_item {
+  int32_t kind, dtype;
+  sb_pitched src[3];
+  int64_t acc_origin[3], lo[3], hi[3];
+} sb_reduce_item;
+
+typedef struct sb_reduce_result {
+  double min, max, sum, sumsq;
+  int64_t count;
+} sb_reduce_result;
+
+/* A persistent plan: n >= 1 items, reduced by one launch sequence on `device` (a tile kernel and a small per-item
+ * combine).  Errors (SB_ERR_INVALID with a message, before anything is allocated): n < 1, an unknown kind or dtype,
+ * sources of one item with different pitches or row counts, a pointer or pitch that is not a multiple of the element
+ * size, lo > hi on an axis, a box outside the allocation.
+ * sb_reduce_plan_launch writes one sb_reduce_result per item, in item order, to out_dev (device memory, n results)
+ * in the order of `stream`.  It allocates nothing and never synchronises the host, so it may be captured in a CUDA
+ * graph.  The plan owns the scratch memory the launch uses: at most ONE launch of a plan may be in flight at a time
+ * (order launches of the same plan on one stream, or wait for the previous one). */
+typedef struct sb_reduce_plan sb_reduce_plan;
+int sb_reduce_plan_create(sb_reduce_plan **out, int device, const sb_reduce_item *items, int64_t n);
+int sb_reduce_plan_launch(sb_reduce_plan *plan, sb_reduce_result *out_dev, void *stream);
+int64_t sb_reduce_plan_bytes(const sb_reduce_plan *plan); /* source bytes read per launch */
+int sb_reduce_plan_destroy(sb_reduce_plan *plan);
+/* Host only.  The one place that defines how results merge: parts[0..n) (n >= 1) combined by the pairwise tree
+ * "parts[i] = merge(parts[i], parts[i + s]) for every i % 2s == 0, i + s < n" for s = 1, 2, 4, ..., result parts[0];
+ * merge takes the NaN-propagating min and max and adds sum, sumsq and count.  Callers pass per-subdomain results in
+ * global subdomain-index order (partition index (i, j, k), x fastest). */
+int sb_reduce_combine(const sb_reduce_result *parts, int64_t n, sb_reduce_result *out);
+
+/* ---------------------------------------------------------------------------------------------
  * 7-point jacobi step (the reference's user kernel, bin/jacobi3d.cu:40-85) over a region.
  * dtype_size 4 = float, 8 = double.  acc_origin = global coordinate of allocation element (0,0,0)
  * (Accessor origin, include/stencil/local_domain.cuh:153-173).  [lo,hi) = region to update,

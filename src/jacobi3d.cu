@@ -112,6 +112,8 @@ void FusedJacobi3d::init(double value) {
   ghostsCurrent_ = false;
 }
 
+double FusedJacobi3d::residual() { return dd_.reduce_many(std::vector<ReduceItem>(1, ReduceItem{SB_REDUCE_DIFF, {q_, q_, q_}, Which::curr}))[0].l2(); }
+
 void FusedJacobi3d::synchronize() {
   for (size_t di = 0; di < streams_.size(); ++di) {
     CUDA_RUNTIME(cudaSetDevice(streams_[di].device()));

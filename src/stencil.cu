@@ -74,6 +74,7 @@ DistributedDomain::~DistributedDomain() {
 }
 
 void DistributedDomain::destroy_plans() {
+  destroy_reduce_plans();
   for (auto *sides : {&plans_, &unpackPlans_}) {
     for (int parity = 0; parity < 2; ++parity) {
       for (sb_copy_plan *p : (*sides)[parity])
@@ -645,6 +646,124 @@ void DistributedDomain::swap() {
   MPI_Reduce(&elapsed, &maxElapsed, 1, MPI_DOUBLE, MPI_MAX, 0, MPI_COMM_WORLD);
   if (0 == rank_) timeSwap_ += maxElapsed;
 #endif
+}
+
+void DistributedDomain::destroy_reduce_plans() {
+  for (auto &kv : reducePlans_) {
+    for (size_t di = 0; di < kv.second.plans.size(); ++di) {
+      sb_reduce_plan_destroy(kv.second.plans[di]);
+      cudaSetDevice(domains_[di].gpu());
+      cudaFree(kv.second.out[di]);
+    }
+  }
+  reducePlans_.clear();
+}
+
+std::vector<stencil::Reduction> DistributedDomain::reduce_many(const std::vector<stencil::ReduceItem> &items) {
+  using stencil::Which;
+  const size_t n = items.size();
+  if (0 == n) return {};
+  std::vector<int64_t> key;
+  for (const stencil::ReduceItem &it : items) {
+    const int ns = it.kind == SB_REDUCE_SCALAR ? 1 : it.kind == SB_REDUCE_DIFF ? 1 : 3;
+    if (it.kind < SB_REDUCE_SCALAR || it.kind > SB_REDUCE_NORM3) LOG_FATAL("reduce: unknown kind " << int(it.kind));
+    for (int s = 0; s < ns; ++s) {
+      if (it.q[s] >= dataDtype_.size()) LOG_FATAL("reduce: unknown data handle " << it.q[s]);
+      if (dataDtype_[it.q[s]] != SB_DTYPE_F32 && dataDtype_[it.q[s]] != SB_DTYPE_F64) LOG_FATAL("reduce: quantity " << it.q[s] << " is not float or double");
+      if (dataDtype_[it.q[s]] != dataDtype_[it.q[0]]) LOG_FATAL("reduce: the sources of a norm must share one type");
+    }
+    key.insert(key.end(), {int64_t(it.kind), int64_t(it.q[0]), int64_t(ns == 3 ? it.q[1] : it.q[0]), int64_t(ns == 3 ? it.q[2] : it.q[0]),
+                           int64_t(it.kind == SB_REDUCE_SCALAR && it.which == Which::next)});
+  }
+  key.push_back(parity_);
+  auto found = reducePlans_.find(key);
+  if (found == reducePlans_.end()) {
+    ReduceCache c;
+    for (LocalDomain &d : domains_) {
+      const Rect3 cr = d.get_compute_region();
+      const Dim3 ao = d.origin() - Dim3(radius_.x(-1), radius_.y(-1), radius_.z(-1));
+      std::vector<sb_reduce_item> its(n);
+      for (size_t i = 0; i < n; ++i) {
+        const stencil::ReduceItem &it = items[i];
+        sb_reduce_item &r = its[i];
+        r.kind = it.kind;
+        r.dtype = dataDtype_[it.q[0]];
+        for (int s = 0; s < 3; ++s) {
+          cudaPitchedPtr p = d.curr_data(it.kind == SB_REDUCE_NORM3 ? it.q[s] : it.q[0]);
+          if ((it.kind == SB_REDUCE_SCALAR && it.which == Which::next) || (it.kind == SB_REDUCE_DIFF && s == 1)) p = d.next_data(it.q[0]);
+          r.src[s] = sb_pitched{p.ptr, int64_t(p.pitch), int64_t(p.ysize)};
+        }
+        const int64_t acc[3] = {ao.x, ao.y, ao.z}, lo[3] = {cr.lo.x, cr.lo.y, cr.lo.z}, hi[3] = {cr.hi.x, cr.hi.y, cr.hi.z};
+        for (int a = 0; a < 3; ++a) {
+          r.acc_origin[a] = acc[a];
+          r.lo[a] = lo[a];
+          r.hi[a] = hi[a];
+        }
+      }
+      sb_reduce_plan *plan = nullptr;
+      if (SB_OK != sb_reduce_plan_create(&plan, d.gpu(), its.data(), int64_t(n))) LOG_FATAL("reduce: " << sb_last_error());
+      sb_reduce_result *out = nullptr;
+      d.set_device();
+      CUDA_RUNTIME(cudaMalloc(&out, n * sizeof(sb_reduce_result)));
+      c.plans.push_back(plan);
+      c.out.push_back(out);
+    }
+    found = reducePlans_.emplace(key, std::move(c)).first;
+  }
+  const ReduceCache &c = found->second;
+  // 1. all work already queued on the local devices
+  for (const int dev : std::set<int>(gpus_.begin(), gpus_.end())) {
+    CUDA_RUNTIME(cudaSetDevice(dev));
+    CUDA_RUNTIME(cudaDeviceSynchronize());
+  }
+  // 2. one launch sequence per local subdomain on its exchange stream; records: global index, then n results
+  const Dim3 dim = placement_->dim();
+  const size_t rec = sizeof(int64_t) + n * sizeof(sb_reduce_result);
+  std::vector<unsigned char> mine(domains_.size() * rec);
+  for (size_t di = 0; di < domains_.size(); ++di) {
+    domains_[di].set_device();
+    if (SB_OK != sb_reduce_plan_launch(c.plans[di], c.out[di], streams_[di])) LOG_FATAL("reduce: " << sb_last_error());
+    const Dim3 &idx = domainIdx_[di];
+    const int64_t lin = idx.x + dim.x * (idx.y + dim.y * idx.z);
+    std::memcpy(&mine[di * rec], &lin, sizeof(lin));
+    CUDA_RUNTIME(cudaMemcpyAsync(&mine[di * rec + sizeof(int64_t)], c.out[di], n * sizeof(sb_reduce_result), cudaMemcpyDeviceToHost, streams_[di]));
+  }
+  for (size_t di = 0; di < domains_.size(); ++di) {
+    domains_[di].set_device();
+    CUDA_RUNTIME(cudaStreamSynchronize(streams_[di]));
+  }
+  // 3. every rank's records
+  std::vector<unsigned char> all = mine;
+  if (worldSize_ > 1) {
+    const int count = int(mine.size());
+    std::vector<int> counts(static_cast<size_t>(worldSize_)), displs(static_cast<size_t>(worldSize_));
+    MPI_Allgather(&count, 1, MPI_INT, counts.data(), 1, MPI_INT, MPI_COMM_WORLD);
+    int total = 0;
+    for (int r = 0; r < worldSize_; ++r) {
+      displs[size_t(r)] = total;
+      total += counts[size_t(r)];
+    }
+    all.assign(size_t(total), 0);
+    MPI_Allgatherv(mine.data(), count, MPI_BYTE, all.data(), counts.data(), displs.data(), MPI_BYTE, MPI_COMM_WORLD);
+  }
+  // 4. merge in global subdomain-index order, the same on every rank
+  const size_t nrec = all.size() / rec;
+  std::vector<std::pair<int64_t, size_t>> order(nrec);
+  for (size_t k = 0; k < nrec; ++k) {
+    std::memcpy(&order[k].first, &all[k * rec], sizeof(int64_t));
+    order[k].second = k;
+  }
+  std::sort(order.begin(), order.end());
+  std::vector<stencil::Reduction> result(n);
+  std::vector<sb_reduce_result> parts(nrec);
+  for (size_t i = 0; i < n; ++i) {
+    for (size_t k = 0; k < nrec; ++k)
+      std::memcpy(&parts[k], &all[order[k].second * rec + sizeof(int64_t) + i * sizeof(sb_reduce_result)], sizeof(sb_reduce_result));
+    sb_reduce_result r;
+    if (SB_OK != sb_reduce_combine(parts.data(), int64_t(nrec), &r)) LOG_FATAL("reduce: " << sb_last_error());
+    result[i] = stencil::Reduction{r.min, r.max, r.sum, r.sumsq, r.count};
+  }
+  return result;
 }
 
 std::vector<Rect3> DistributedDomain::get_interior() const {

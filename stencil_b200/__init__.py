@@ -21,6 +21,8 @@ from .domain import (  # noqa: F401
     Partition,
     PlacementStrategy,
     Radius,
+    Reduction,
+    ReducePlan,
     box_copy,
     fill,
     get_neighbor,
@@ -29,6 +31,7 @@ from .domain import (  # noqa: F401
     jacobi3d,
     prime_factors,
     raw_size,
+    reduce_combine,
 )
 
 __all__ = [n for n in dir() if not n.startswith("_")]

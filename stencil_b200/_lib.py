@@ -75,6 +75,27 @@ class BcQuantity(C.Structure):
     ]
 
 
+class ReduceItem(C.Structure):
+    """sb_reduce_item: one reduction over a box [lo, hi) of compute cells (global coordinates)."""
+
+    _fields_ = [
+        ("kind", C.c_int32),
+        ("dtype", C.c_int32),
+        ("src", Pitched * 3),
+        ("acc_origin", C.c_int64 * 3),
+        ("lo", C.c_int64 * 3),
+        ("hi", C.c_int64 * 3),
+    ]
+
+
+class ReduceResult(C.Structure):
+    """sb_reduce_result"""
+
+    _fields_ = [("min", C.c_double), ("max", C.c_double), ("sum", C.c_double), ("sumsq", C.c_double), ("count", C.c_int64)]
+
+
+REDUCE_SCALAR, REDUCE_DIFF, REDUCE_NORM3 = 0, 1, 2  # sb_reduce_kind
+
 I6 = C.c_int32 * 6
 
 FUSED_MAX_GROUPS = 4096  # SB_FUSED_MAX_GROUPS
@@ -115,6 +136,11 @@ _SIGS = {
     "sb_bc_plan_launch": (C.c_int, [C.c_void_p, C.c_void_p]),
     "sb_bc_plan_bytes": (C.c_int64, [C.c_void_p]),
     "sb_bc_plan_destroy": (C.c_int, [C.c_void_p]),
+    "sb_reduce_plan_create": (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.POINTER(ReduceItem), C.c_int64]),
+    "sb_reduce_plan_launch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
+    "sb_reduce_plan_bytes": (C.c_int64, [C.c_void_p]),
+    "sb_reduce_plan_destroy": (C.c_int, [C.c_void_p]),
+    "sb_reduce_combine": (C.c_int, [C.POINTER(ReduceResult), C.c_int64, C.POINTER(ReduceResult)]),
     "sb_signal": (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.c_uint32, C.c_int, C.c_void_p]),
     "sb_wait": (C.c_int, [C.c_void_p, C.c_int, C.c_uint32, C.c_int, C.c_void_p]),
     "sb_jacobi3d": (C.c_int, [Pitched, Pitched, C.c_int, I3, I3, I3, I3, I3, C.c_void_p]),

@@ -9,12 +9,12 @@ reference (AcReal = double) and FP32 as well here.  The kernel is `sb_astaroth_s
 from __future__ import annotations
 
 import ctypes as C
-from typing import Optional, Sequence
+from typing import Dict, Optional, Sequence
 
 import numpy as np
 
 from ._lib import AstarothParams, check, i3, lib, stream_ptr
-from .domain import DataHandle, DistributedDomain
+from .domain import DataHandle, DistributedDomain, Reduction
 
 FIELDS = ("lnrho", "uux", "uuy", "uuz", "ax", "ay", "az", "entropy")
 NGHOST = 3  # STENCIL_ORDER / 2, astaroth/astaroth.h:8-9
@@ -101,6 +101,15 @@ class Astaroth:
             packs = a[which] if which == 1 else [a[which]]
             for p in packs:
                 check(self._fn(step, p[0], p[1], p[2], p[3], p[4], p[5], p[6], p[7], p[8]))
+
+    def diagnostics(self) -> Dict[str, Reduction]:
+        """The reference's RTYPE_MIN / MAX / RMS diagnostics (astaroth/user_defines.h:161-169) of the current fields, as
+        Reductions: one per field of FIELDS (min, max, rms) and "uu", "aa" for the norms |(uux, uuy, uuz)| and
+        |(ax, ay, az)| (max, rms).  Ten items in one plan: one launch sequence per subdomain."""
+        h = self.handles
+        items = [("scalar", x) for x in h] + [("norm", h[1], h[2], h[3]), ("norm", h[4], h[5], h[6])]
+        res = self.dd.reduce_many(items)
+        return dict(zip(FIELDS + ("uu", "aa"), res))
 
     def synchronize(self) -> None:
         for s in self.streams + self.ext_streams:

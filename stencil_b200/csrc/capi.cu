@@ -15,6 +15,7 @@
 
 #include "box_copy.cuh"
 #include "boundary.cuh"
+#include "reduce.cuh"
 #include "astaroth.cuh"
 #include "jacobi.cuh"
 
@@ -508,6 +509,17 @@ struct sb_bc_plan {
   sb::BcTile *tiles_dev = nullptr;
   unsigned ntiles = 0;
   int grid = 0;
+  int64_t bytes = 0;
+};
+
+struct sb_reduce_plan {
+  int device = 0;
+  sb::RedItem *items_dev = nullptr;
+  sb::RedTile *tiles_dev = nullptr;
+  sb::RedPartial *scratch = nullptr; // one partial per tile, rewritten by every launch
+  unsigned nitems = 0, ntiles = 0;
+  unsigned class_tiles[sb::kRedClasses][2] = {}; // tiles [begin, end) of each class
+  int grids[sb::kRedClasses] = {};
   int64_t bytes = 0;
 };
 
@@ -1103,6 +1115,135 @@ int sb_sqdiff(sb_pitched a, sb_pitched b, int dtype_size, const int64_t acc_orig
   g_launches += uint64_t(sb::launch_sqdiff(static_cast<const char *>(a.ptr), static_cast<const char *>(b.ptr), a.pitch,
                                            a.pitch * a.ysize, alo, ahi, dtype_size, out_dev, static_cast<cudaStream_t>(stream)));
   SB_CUDA(cudaGetLastError());
+  return SB_OK;
+}
+
+// ----------------------------------------------------------------------------------------- reductions
+int sb_reduce_plan_create(sb_reduce_plan **out, int device, const sb_reduce_item *items, int64_t n) {
+  if (!out || !items || n < 1) return fail(SB_ERR_INVALID, "sb_reduce_plan_create needs an output handle and n >= 1 items");
+  if (n > (1 << 20)) return fail(SB_ERR_INVALID, "at most 2^20 items per plan");
+  std::vector<sb::RedItem> its;
+  std::vector<sb::RedTile> tiles;
+  int64_t bytes = 0;
+  for (int64_t i = 0; i < n; ++i) {
+    const sb_reduce_item &I = items[i];
+    const long long li = (long long)i;
+    if (I.kind < SB_REDUCE_SCALAR || I.kind > SB_REDUCE_NORM3) return fail(SB_ERR_INVALID, "item %lld: unknown kind %d", li, int(I.kind));
+    if (I.dtype != SB_DTYPE_F32 && I.dtype != SB_DTYPE_F64)
+      return fail(SB_ERR_INVALID, "item %lld: dtype %d must be SB_DTYPE_F32 or SB_DTYPE_F64", li, int(I.dtype));
+    const int es = I.dtype == SB_DTYPE_F32 ? 4 : 8;
+    const int ns = I.kind == SB_REDUCE_SCALAR ? 1 : I.kind == SB_REDUCE_DIFF ? 2 : 3;
+    for (int a = 0; a < 3; ++a)
+      if (I.lo[a] > I.hi[a]) return fail(SB_ERR_INVALID, "item %lld: lo > hi on axis %d", li, a);
+    int alo[3] = {0, 0, 0}, ahi[3] = {0, 0, 0};
+    for (int s = 0; s < ns; ++s) {
+      const sb_pitched &P = I.src[s];
+      const int rc = to_alloc_box(P, es, I.acc_origin, I.lo, I.hi, alo, ahi);
+      if (rc != SB_OK) return fail(SB_ERR_INVALID, "item %lld, source %d: %s", li, s, g_err.c_str());
+      if (P.pitch != I.src[0].pitch || P.ysize != I.src[0].ysize)
+        return fail(SB_ERR_INVALID, "item %lld: its sources have different pitches or row counts", li);
+      if ((uintptr_t(P.ptr) % uintptr_t(es)) || (P.pitch % es))
+        return fail(SB_ERR_INVALID, "item %lld, source %d: pointer and pitch must be multiples of the %d-byte element", li, s, es);
+    }
+    const sb_pitched &P0 = I.src[0];
+    if ((long long)ahi[0] * es > P0.pitch || ahi[1] > P0.ysize) return fail(SB_ERR_INVALID, "item %lld: box outside the allocation", li);
+    sb::RedItem r{};
+    r.pitch = P0.pitch;
+    r.slice = P0.pitch * P0.ysize;
+    for (int a = 0; a < 3; ++a) r.ext[a] = ahi[a] - alo[a];
+    const long long off = (long long)alo[2] * r.slice + (long long)alo[1] * r.pitch + (long long)alo[0] * es;
+    bool wide = true;
+    for (int s = 0; s < 3; ++s) {
+      r.src[s] = static_cast<const char *>(I.src[s < ns ? s : 0].ptr) + off;
+      wide = wide && ((uintptr_t(r.src[s]) - uintptr_t(r.src[0])) % 16 == 0);
+    }
+    r.kind = I.kind;
+    r.dtype = I.dtype;
+    r.vec = wide ? 16 : es;
+    // lanes per row and tile rows: functions of the box and the access width only
+    const long long nx = r.ext[0], rows = (long long)r.ext[1] * r.ext[2];
+    r.lg_group = int(std::min(5u, ceil_log2(unsigned(std::max(1ll, (nx * es + 15) / 16)))));
+    r.count = nx * rows;
+    if (rows >= (1ll << 31)) return fail(SB_ERR_INVALID, "item %lld: more than 2^31 rows", li);
+    its.push_back(r);
+    bytes += r.count * es * ns;
+  }
+  // the tile table, class by class; inside a class item by item
+  unsigned class_tiles[sb::kRedClasses][2];
+  for (int c = 0; c < sb::kRedClasses; ++c) {
+    class_tiles[c][0] = unsigned(tiles.size());
+    for (size_t i = 0; i < its.size(); ++i) {
+      sb::RedItem &r = its[i];
+      if (sb::reduce_class(r) != c) continue;
+      r.tile0 = unsigned(tiles.size());
+      if (r.count > 0) {
+        const long long nx = r.ext[0], rows = (long long)r.ext[1] * r.ext[2];
+        const long long N = r.vec / (r.dtype == SB_DTYPE_F32 ? 4 : 8), G = 1ll << r.lg_group;
+        // longest chain of one lane over one row: its body vectors, one head and one tail cell
+        const long long per_row = N * (((nx / N) + G - 1) / G) + 2 * ((std::min(nx, N - 1) + G - 1) / G);
+        const long long rows_per_tile = std::max(1ll, sb::kRedChain / std::max(1ll, per_row)) * (sb::kRedThreads >> r.lg_group);
+        for (long long r0 = 0; r0 < rows; r0 += rows_per_tile)
+          tiles.push_back(sb::RedTile{unsigned(i), unsigned(r0), unsigned(std::min(rows_per_tile, rows - r0))});
+        if (tiles.size() >= (1ull << 31)) return fail(SB_ERR_INVALID, "too many tiles");
+      }
+      r.ntiles = unsigned(tiles.size()) - r.tile0;
+    }
+    class_tiles[c][1] = unsigned(tiles.size());
+  }
+  DeviceGuard guard(device);
+  if (!guard.ok) return fail(SB_ERR_NOGPU, "cannot select CUDA device %d", device);
+  sb_reduce_plan *p = new sb_reduce_plan();
+  p->device = device;
+  p->bytes = bytes;
+  p->nitems = unsigned(its.size());
+  p->ntiles = unsigned(tiles.size());
+  cudaError_t e = cudaMalloc(&p->items_dev, its.size() * sizeof(sb::RedItem));
+  if (e == cudaSuccess) e = cudaMalloc(&p->tiles_dev, std::max<size_t>(1, tiles.size()) * sizeof(sb::RedTile));
+  if (e == cudaSuccess) e = cudaMalloc(&p->scratch, std::max<size_t>(1, tiles.size()) * sizeof(sb::RedPartial));
+  if (e == cudaSuccess) e = cudaMemcpy(p->items_dev, its.data(), its.size() * sizeof(sb::RedItem), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess && !tiles.empty()) e = cudaMemcpy(p->tiles_dev, tiles.data(), tiles.size() * sizeof(sb::RedTile), cudaMemcpyHostToDevice);
+  if (e != cudaSuccess) {
+    sb_reduce_plan_destroy(p);
+    return fail(SB_ERR_CUDA, "reduction plan upload: %s", cudaGetErrorString(e));
+  }
+  for (int c = 0; c < sb::kRedClasses; ++c) {
+    p->class_tiles[c][0] = class_tiles[c][0];
+    p->class_tiles[c][1] = class_tiles[c][1];
+    p->grids[c] = sb::reduce_grid(device, c, class_tiles[c][1] - class_tiles[c][0]);
+  }
+  *out = p;
+  return SB_OK;
+}
+
+int sb_reduce_plan_launch(sb_reduce_plan *p, sb_reduce_result *out_dev, void *stream) {
+  if (!p) return fail(SB_ERR_INVALID, "null plan");
+  if (!out_dev) return fail(SB_ERR_INVALID, "null output buffer");
+  DeviceGuard guard(p->device);
+  if (!guard.ok) return fail(SB_ERR_NOGPU, "cannot select CUDA device %d", p->device);
+  g_launches += uint64_t(sb::launch_reduce(p->items_dev, p->nitems, p->tiles_dev, p->class_tiles, p->grids, p->scratch, out_dev,
+                                           static_cast<cudaStream_t>(stream)));
+  SB_CUDA(cudaGetLastError());
+  return SB_OK;
+}
+
+int64_t sb_reduce_plan_bytes(const sb_reduce_plan *p) { return p ? p->bytes : 0; }
+
+int sb_reduce_plan_destroy(sb_reduce_plan *p) {
+  if (!p) return SB_OK;
+  DeviceGuard guard(p->device);
+  if (p->items_dev) cudaFree(p->items_dev);
+  if (p->tiles_dev) cudaFree(p->tiles_dev);
+  if (p->scratch) cudaFree(p->scratch);
+  delete p;
+  return SB_OK;
+}
+
+int sb_reduce_combine(const sb_reduce_result *parts, int64_t n, sb_reduce_result *out) {
+  if (!parts || !out || n < 1) return fail(SB_ERR_INVALID, "sb_reduce_combine needs n >= 1 results and an output");
+  std::vector<sb_reduce_result> a(parts, parts + n);
+  for (int64_t s = 1; s < n; s *= 2)
+    for (int64_t i = 0; i + s < n; i += 2 * s) a[size_t(i)] = sb::red_merge(a[size_t(i)], a[size_t(i + s)]);
+  *out = a[0];
   return SB_OK;
 }
 

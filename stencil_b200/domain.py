@@ -24,7 +24,9 @@ this module only sequences calls.  No CPU fallback exists.
 from __future__ import annotations
 
 import ctypes as C
+import dataclasses
 import enum
+import math
 import os
 from typing import Dict, List, Optional, Sequence, Tuple
 
@@ -325,6 +327,88 @@ class BCPlan:
             pass
 
 
+# ------------------------------------------------------------------------------------------ reductions
+@dataclasses.dataclass(frozen=True)
+class Reduction:
+    """sb_reduce_result: min and max of the per-cell value v, sum of v, sum of its squared term q, number of cells."""
+
+    min: float
+    max: float
+    sum: float
+    sumsq: float
+    count: int
+
+    def mean(self) -> float:
+        return self.sum / self.count if self.count else math.nan
+
+    def rms(self) -> float:
+        """sqrt(sumsq / count): the RMS of a scalar, or of |u| for a NORM3 item."""
+        return math.sqrt(self.sumsq / self.count) if self.count else math.nan
+
+    def l2(self) -> float:
+        """sqrt(sumsq): the 2-norm (of a - b for a DIFF item)."""
+        return math.sqrt(self.sumsq)
+
+    @staticmethod
+    def of(r: _lib.ReduceResult) -> "Reduction":
+        return Reduction(r.min, r.max, r.sum, r.sumsq, int(r.count))
+
+    def to_c(self) -> _lib.ReduceResult:
+        return _lib.ReduceResult(self.min, self.max, self.sum, self.sumsq, self.count)
+
+
+def reduce_combine(parts: Sequence[Reduction]) -> Reduction:
+    """sb_reduce_combine: per-subdomain results merged by the library's fixed pairwise tree, in the order given."""
+    arr = (_lib.ReduceResult * max(1, len(parts)))(*[p.to_c() for p in parts])
+    out = _lib.ReduceResult()
+    check(lib().sb_reduce_combine(arr, len(parts), C.byref(out)))
+    return Reduction.of(out)
+
+
+class ReducePlan:
+    """sb_reduce_plan: several reductions of one subdomain, one launch sequence, results into a device buffer the plan
+    owns.  One launch in flight at a time."""
+
+    def __init__(self, device: int, items: Sequence[_lib.ReduceItem]):
+        arr = (_lib.ReduceItem * len(items))(*items)
+        h = C.c_void_p()
+        check(lib().sb_reduce_plan_create(C.byref(h), device, arr, len(items)))
+        self._h = h
+        self.device = device
+        self.n = len(items)
+        self.bytes = int(lib().sb_reduce_plan_bytes(h))
+        out = C.c_void_p()
+        nbytes = self.n * C.sizeof(_lib.ReduceResult)
+        if lib().sb_malloc(C.byref(out), nbytes, device) != 0:
+            self.destroy()
+            raise _lib.StencilError(f"reduction output buffer: {lib().sb_last_error().decode()}")
+        self.out_dev = out.value
+
+    def launch(self, stream=None) -> None:
+        check(lib().sb_reduce_plan_launch(self._h, C.c_void_p(self.out_dev), stream_ptr(stream)))
+
+    def results(self, stream=None) -> List[Reduction]:
+        """Copy the last launch's results (ordered after it on `stream`) to the host."""
+        host = (_lib.ReduceResult * self.n)()
+        check(lib().sb_memcpy(C.addressof(host), C.c_void_p(self.out_dev), C.sizeof(host), self.device, stream_ptr(stream)))
+        check(lib().sb_stream_sync(self.device, stream_ptr(stream)))
+        return [Reduction.of(r) for r in host]
+
+    def destroy(self) -> None:
+        if getattr(self, "out_dev", None):
+            lib().sb_free(C.c_void_p(self.out_dev), self.device)
+            self.out_dev = None
+        if self._h:
+            lib().sb_reduce_plan_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.destroy()
+        except Exception:
+            pass
+
+
 # ------------------------------------------------------------------------------------------ LocalDomain
 class LocalDomain:
     """One subdomain on one GPU: curr/next allocation per quantity (local_domain.cuh:34-276,
@@ -536,6 +620,7 @@ class DistributedDomain:
         self.bcs_: Dict[Tuple[int, int], BC] = {}  # (quantity, face 0..5) -> BC
         self.topology_: Optional[Topology] = None
         self._bc_plans: List[List[Optional[BCPlan]]] = []  # [parity][local domain]
+        self._reduce_plans: Dict[tuple, List[ReducePlan]] = {}  # (item keys, parity) -> one plan per local domain
 
     # -- configuration (call before realize)
     def set_radius(self, r) -> None:
@@ -982,7 +1067,93 @@ class DistributedDomain:
             d.swap()
         self._parity ^= 1
 
+    # -- reductions
+    _REDUCE_KINDS = {"scalar": (_lib.REDUCE_SCALAR, 1), "diff": (_lib.REDUCE_DIFF, 1), "norm": (_lib.REDUCE_NORM3, 3)}
+
+    def reduce(self, h: DataHandle, which: str = "curr") -> Reduction:
+        """min, max, sum and sum of squares of quantity h (its curr or next buffer) over the whole compute region."""
+        return self.reduce_many([("scalar", h, which)])[0]
+
+    def reduce_diff(self, h: DataHandle) -> Reduction:
+        """The same statistics of curr - next of quantity h; .l2() is the 2-norm of the last update after a swap."""
+        return self.reduce_many([("diff", h)])[0]
+
+    def reduce_norm(self, hx: DataHandle, hy: DataHandle, hz: DataHandle) -> Reduction:
+        """Statistics of |u| = sqrt(hx^2 + hy^2 + hz^2) (curr buffers); .rms() is sqrt(sum |u|^2 / N)."""
+        return self.reduce_many([("norm", hx, hy, hz)])[0]
+
+    def reduce_plans(self, items: Sequence[tuple]) -> List[ReducePlan]:
+        """The plans reduce_many(items) launches, one per local subdomain, for the current swap parity.  They are built
+        on first use and kept, per item list and parity, until close(): a program should reduce a fixed set of item
+        lists rather than build a new list every iteration, or each new list holds device memory until close()."""
+        keys = [self._reduce_key(it) for it in items]
+        if not keys:
+            raise _lib.StencilError("reduce_plans: no items")
+        ck = (tuple(keys), self._parity)
+        plans = self._reduce_plans.get(ck)
+        if plans is None:
+            plans = [ReducePlan(d.gpu(), [self._reduce_item(di, k) for k in keys]) for di, d in enumerate(self.domains_)]
+            self._reduce_plans[ck] = plans
+        return plans
+
+    def reduce_many(self, items: Sequence[tuple]) -> List[Reduction]:
+        """Several reductions, one launch sequence per local subdomain.  Items: ("scalar", h[, "curr" | "next"]),
+        ("diff", h) (curr - next), ("norm", hx, hy, hz).  Waits for all work queued on the local devices, reduces on
+        the exchange streams, gathers every rank's per-subdomain results and merges them with sb_reduce_combine in
+        global subdomain-index order (x fastest), so every rank returns the same bits.  Collective under torchrun.  The
+        plans are cached as reduce_plans() describes."""
+        from . import dist as _dist
+
+        if not items:
+            return []
+        n = len(items)
+        plans = self.reduce_plans(items)
+        for dev in sorted({d.gpu() for d in self.domains_}):
+            check(lib().sb_device_sync(dev))
+        for plan, s in zip(plans, self._streams):
+            plan.launch(s)
+        dim = self.partition_.dim
+        mine = [(idx, [(r.min, r.max, r.sum, r.sumsq, r.count) for r in plan.results(s)])
+                for idx, plan, s in zip(self.domain_idx_, plans, self._streams)]  # fmt: skip
+        everyone = _dist.all_gather_object(mine) if self._world.size > 1 else [mine]
+        parts = sorted((p for rank_parts in everyone for p in rank_parts), key=lambda p: p[0][0] + dim[0] * (p[0][1] + dim[1] * p[0][2]))
+        return [reduce_combine([Reduction(*p[1][i]) for p in parts]) for i in range(n)]
+
+    def _reduce_key(self, it: tuple) -> tuple:
+        if not it or it[0] not in self._REDUCE_KINDS:
+            raise _lib.StencilError(f"reduction item {it!r}: the first element must be 'scalar', 'diff' or 'norm'")
+        kind, nsrc = self._REDUCE_KINDS[it[0]]
+        hs = it[1 : 1 + nsrc]
+        rest = it[1 + nsrc :]
+        if len(hs) != nsrc or not all(isinstance(h, DataHandle) for h in hs):
+            raise _lib.StencilError(f"reduction item {it!r}: '{it[0]}' takes {nsrc} DataHandle(s)")
+        which = "curr"
+        if kind == _lib.REDUCE_SCALAR and rest:
+            which = rest[0]
+            rest = rest[1:]
+        if rest or which not in ("curr", "next"):
+            raise _lib.StencilError(f"reduction item {it!r}: unexpected {rest or which!r}")
+        dts = {self.dtypes_[h.id] for h in hs}
+        if len(dts) != 1 or bc_dtype(dts.pop()) == 0:
+            raise _lib.StencilError(f"reduction item {it!r}: the sources must all be float32 or all float64")
+        return (kind, tuple(h.id for h in hs), which)
+
+    def _reduce_item(self, di: int, key: tuple) -> _lib.ReduceItem:
+        kind, qs, which = key
+        d, idx = self.domains_[di], self.domain_idx_[di]
+        parity = self._parity if which == "curr" else self._parity ^ 1
+        srcs = [self._pitched_of(idx, q, parity)[0] for q in qs]
+        srcs += [srcs[0]] * (3 - len(srcs))
+        if kind == _lib.REDUCE_DIFF:
+            srcs[1] = self._pitched_of(idx, qs[0], self._parity ^ 1)[0]
+        lo, hi = d.get_compute_region()
+        return _lib.ReduceItem(kind, bc_dtype(self.dtypes_[qs[0]]), (Pitched * 3)(*srcs), i3(d.accessor_origin()), i3(lo), i3(hi))
+
     def close(self) -> None:
+        for plans in self._reduce_plans.values():
+            for p in plans:
+                p.destroy()
+        self._reduce_plans = {}
         for plans in self._plans + getattr(self, "_unpack_plans", []) + self._bc_plans:
             for p in plans:
                 if p is not None:

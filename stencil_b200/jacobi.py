@@ -556,6 +556,11 @@ class Jacobi3D:
         if hasattr(self, "_fused_calls"):
             del self._fused_calls  # a later step_fused() builds everything again
 
+    def residual(self) -> float:
+        """||curr - next||_2 over the whole grid and every rank: after a step, the 2-norm of the last update.  Orders
+        after the iterations step_async / step_fused have queued (the reduction waits for the devices)."""
+        return self.dd.reduce_diff(self.h).l2()
+
     def synchronize(self) -> None:
         """Wait for the compute streams (bin/jacobi3d.cu:363-365)."""
         for s in self.streams:
