@@ -256,3 +256,5 @@ enum { LNRHO = 0, UUX, UUY, UUZ, AX, AY, AZ, ENTROPY, NFIELDS };
 
 AC_TEMPLATE(double, f64, exp)
 AC_TEMPLATE(float, f32, expf)
+/* extended precision (x87: 64-bit significand): the reference the rounding of the f32 / f64 paths is measured against */
+AC_TEMPLATE(long double, f80, expl)

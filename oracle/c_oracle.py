@@ -48,6 +48,23 @@ def astaroth_conf_params(dt: float = 1e-8) -> AcParams:
     return AcParams(1.0 / ds, 1.0 / ds, 1.0 / ds, dt, 1.0, 0.5, 1.0, 1.3, 1.2, 1.4, 5e-3, 0.01, 5e-3)
 
 
+# Anisotropic spacing and physical constants that are pairwise distinct, none 0 or 1 and none a simple multiple of another:
+# unlike the conf set (equal spacings, nu == eta, cs2 == cp == 1), swapping two of them or dropping a 1 / cp changes the
+# result.  Same values as stencil_b200.astaroth.distinct_params.
+DISTINCT_DS = (0.049, 0.061, 0.037)
+DISTINCT = dict(cs2_sound=0.83, gamma=0.61, cp_sound=1.37, lnrho0=0.42, lnT0=-0.73, mu0=1.91, nu_visc=0.0172, zeta=0.0291, eta=0.0113)
+
+
+def distinct_params(dt: float = 1e-3) -> AcParams:
+    dx, dy, dz = DISTINCT_DS
+    return AcParams(1.0 / dx, 1.0 / dy, 1.0 / dz, dt, **DISTINCT)
+
+
+# The extended-precision reference (so_astaroth_substep_f80) needs a long double with at least the x87 64-bit significand;
+# where long double is plain double it would measure nothing.
+HAS_F80 = np.finfo(np.longdouble).nmant >= 63
+
+
 def build(force: bool = False) -> str:
     """Compile the C oracle with gcc."""
     srcs = [os.path.join(_HERE, f) for f in ("stencil_oracle.c", "astaroth_oracle.c")]
@@ -87,6 +104,7 @@ def lib() -> C.CDLL:
                 C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_int64, C.c_int64,
                 C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(AcParams),
             ]  # fmt: skip
+        L.so_astaroth_substep_f80.argtypes = L.so_astaroth_substep_f64.argtypes
         _lib = L
     return _lib
 
@@ -97,7 +115,7 @@ def _raw(a: np.ndarray) -> Vec:
 
 
 def _suffix(a: np.ndarray) -> str:
-    return {np.dtype(np.float32): "f32", np.dtype(np.float64): "f64"}[a.dtype]
+    return {np.dtype(np.float32): "f32", np.dtype(np.float64): "f64", np.dtype(np.longdouble): "f80"}[a.dtype]
 
 
 def num_threads() -> int:
@@ -154,8 +172,11 @@ def sqdiff(a: np.ndarray, b: np.ndarray, pos, ext) -> float:
 
 def astaroth_substep(step: int, fin, fout, lo, hi, params: "AcParams") -> None:
     """solve<step> on the memory-offset box [lo, hi) (astaroth/kernels.cu:62-87).  fin / fout: 8 arrays
-    (lnrho, uux, uuy, uuz, ax, ay, az, entropy) of identical (mz, my, mx) shape and dtype; fout is updated in place."""
+    (lnrho, uux, uuy, uuz, ax, ay, az, entropy) of identical (mz, my, mx) shape and dtype (float32, float64, or
+    np.longdouble where HAS_F80); fout is updated in place."""
     a0 = fin[0]
+    if a0.dtype == np.longdouble and not HAS_F80:
+        raise ValueError("np.longdouble is not the x87 80-bit type here: no extended-precision astaroth oracle")
     assert len(fin) == 8 and len(fout) == 8
     for a in list(fin) + list(fout):
         assert a.shape == a0.shape and a.dtype == a0.dtype and a.flags.c_contiguous

@@ -3,12 +3,16 @@
 // the `out` fields after each of the three substeps.  Test / baseline infrastructure only (built by
 // oracle/ref/build_ref.sh into oracle/_ref/, never linked by the product).
 //
-//   ref_astaroth_solve <n> <dt> <in.bin> <out.bin>
+//   ref_astaroth_solve <n> <dt> <in.bin> <out.bin> [nx ny nz dsx dsy dsz cs2_sound gamma cp_sound lnrho0 lnT0 mu0 nu_visc zeta eta]
 //
-// in.bin  : 16 arrays of (n+6)^3 doubles: in[0..8) then out[0..8), x fastest (the layout LocalDomain gives the driver,
-//           astaroth/astaroth.cu:462-473)
-// out.bin : 3 x 8 arrays of (n+6)^3 doubles: all `out` fields after substep 0, 1, 2 (no swap in between, as in the
-//           reference driver's loop, astaroth/astaroth.cu:551-640)
+// in.bin  : 16 arrays of (nx+6)(ny+6)(nz+6) doubles: in[0..8) then out[0..8), x fastest (the layout LocalDomain gives the
+//           driver, astaroth/astaroth.cu:462-473); nx = ny = nz = n unless the overrides are given
+// out.bin : 3 x 8 such arrays: all `out` fields after substep 0, 1, 2 (no swap in between, as in the reference driver's
+//           loop, astaroth/astaroth.cu:551-640)
+// The 15 optional overrides replace the grid size, the spacings and the nine physical constants of astaroth.conf before
+// the mesh info is loaded into the device constants.  AC_inv_ds* is set here as 1 / AC_ds*: acHostUpdateBuiltinParams
+// derives it only `#ifdef AC_dsx`, and AC_dsx is an enumerator, not a macro, so solve<> would otherwise keep reading the
+// default 1 / 0.04908738521 (user_kernels.h:33) whatever the spacing.
 #include <cstdio>
 #include <cstdlib>
 #include <vector>
@@ -34,13 +38,30 @@ int main(int argc, char **argv) {
   }
   const int n = atoi(argv[1]);
   const double dt = atof(argv[2]);
-  const size_t m = size_t(n) + STENCIL_ORDER;
-  const size_t cells = m * m * m;
+  int nn[3] = {n, n, n};
+  const bool over = argc >= 5 + 15;
+  if (argc > 5 && !over) {
+    fprintf(stderr, "overrides: nx ny nz dsx dsy dsz cs2_sound gamma cp_sound lnrho0 lnT0 mu0 nu_visc zeta eta (all 15)\n");
+    return 2;
+  }
+  if (over)
+    for (int k = 0; k < 3; ++k) nn[k] = atoi(argv[5 + k]);
+  const size_t cells = size_t(nn[0] + STENCIL_ORDER) * size_t(nn[1] + STENCIL_ORDER) * size_t(nn[2] + STENCIL_ORDER);
 
   AcMeshInfo info{};
   acLoadConfig(AC_DEFAULT_CONFIG, &info);
-  info.int_params[AC_nx] = info.int_params[AC_ny] = info.int_params[AC_nz] = n;
+  info.int_params[AC_nx] = nn[0], info.int_params[AC_ny] = nn[1], info.int_params[AC_nz] = nn[2];
+  if (over) {
+    const AcRealParam real[12] = {AC_dsx, AC_dsy, AC_dsz, AC_cs2_sound, AC_gamma, AC_cp_sound,
+                                  AC_lnrho0, AC_lnT0, AC_mu0, AC_nu_visc, AC_zeta, AC_eta};
+    for (int k = 0; k < 12; ++k) info.real_params[real[k]] = AcReal(atof(argv[8 + k]));
+  }
   acHostUpdateBuiltinParams(&info);
+  if (over) {
+    info.real_params[AC_inv_dsx] = AcReal(1.) / info.real_params[AC_dsx];
+    info.real_params[AC_inv_dsy] = AcReal(1.) / info.real_params[AC_dsy];
+    info.real_params[AC_inv_dsz] = AcReal(1.) / info.real_params[AC_dsz];
+  }
   info.int3_params[AC_multigpu_offset] = {0, 0, 0};
   CK(cudaSetDevice(0));
   acDeviceLoadDefaultUniforms(0);
@@ -72,7 +93,7 @@ int main(int argc, char **argv) {
   cudaStream_t s;
   CK(cudaStreamCreate(&s));
   acDeviceLoadScalarUniform(0, s, AC_dt, dt);
-  Rect3 cr(Dim3(3, 3, 3), Dim3(3 + n, 3 + n, 3 + n));
+  Rect3 cr(Dim3(3, 3, 3), Dim3(3 + nn[0], 3 + nn[1], 3 + nn[2]));
   if (timing_only) {
     cudaEvent_t e0, e1;
     CK(cudaEventCreate(&e0));
@@ -103,6 +124,6 @@ int main(int argc, char **argv) {
   }
   fclose(g);
   // timing of the reference kernel on the conf's own size is printed by ref_astaroth; here only a marker
-  printf("ref_astaroth_solve n=%d dt=%g ok\n", n, dt);
+  printf("ref_astaroth_solve n=%d,%d,%d dt=%g ok\n", nn[0], nn[1], nn[2], dt);
   return 0;
 }

@@ -30,6 +30,15 @@ def conf_params(dt: float = 1e-8) -> AstarothParams:
     return AstarothParams(1.0 / ds, 1.0 / ds, 1.0 / ds, dt, 1.0, 0.5, 1.0, 1.3, 1.2, 1.4, 5e-3, 0.01, 5e-3)
 
 
+def distinct_params(dt: float = 1e-3) -> AstarothParams:
+    """A set in which no parameter can stand in for another: spacings dsx, dsy, dsz = 0.049, 0.061, 0.037, and physical
+    constants that are pairwise distinct, none 0 or 1 and none a simple multiple of another.  In the conf set
+    inv_dsx == inv_dsy == inv_dsz, nu_visc == eta and cs2_sound == cp_sound == 1, so a swapped pair or a missing 1 / cp
+    would not change the result there; here it does."""
+    dx, dy, dz = 0.049, 0.061, 0.037
+    return AstarothParams(1.0 / dx, 1.0 / dy, 1.0 / dz, dt, 0.83, 0.61, 1.37, 0.42, -0.73, 1.91, 0.0172, 0.0291, 0.0113)
+
+
 def substep(step: int, fin: Sequence[int], fout: Sequence[int], dtype_size: int, raw, lo, hi, params: AstarothParams, variant: int = AUTO,
             stream=None) -> None:  # fmt: skip
     """integrate_substep (astaroth/kernels.cu:62-87) on raw device pointers; [lo, hi) in memory-offset coordinates."""

@@ -9,13 +9,16 @@ from stencil_b200._lib import Pitched, check, lib
 class DevArray:
     """A 3-D [z,y,x] array in device memory (unpitched, like the reference's allocations)."""
 
-    def __init__(self, host: np.ndarray, device: int = 0, extra: int = 0):
+    def __init__(self, host: np.ndarray, device: int = 0, extra: int = 0, lead: int = 0):
+        """lead: bytes between the start of the sb_malloc block (256-byte aligned) and element 0, as LocalDomain leaves
+        in front of an allocation so that its first compute cell is 16-byte aligned."""
         host = np.ascontiguousarray(host)
         self.shape, self.dtype, self.device = host.shape, host.dtype, device
         self.nbytes = host.nbytes
         p = C.c_void_p()
-        check(lib().sb_malloc(C.byref(p), max(self.nbytes + extra, 16), device))
-        self.ptr = int(p.value)
+        check(lib().sb_malloc(C.byref(p), max(lead + self.nbytes + extra, 16), device))
+        self.base = int(p.value)
+        self.ptr = self.base + lead
         check(lib().sb_memcpy(C.c_void_p(self.ptr), host.ctypes.data, self.nbytes, device, None))
         check(lib().sb_stream_sync(device, None))
 
@@ -32,7 +35,7 @@ class DevArray:
 
     def free(self):
         if self.ptr:
-            lib().sb_free(C.c_void_p(self.ptr), self.device)
+            lib().sb_free(C.c_void_p(self.base), self.device)
             self.ptr = 0
 
     def __del__(self):

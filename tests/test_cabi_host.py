@@ -179,6 +179,29 @@ def test_ctypes_structs_match_the_header(tmp_path):
     assert sizes == [C.sizeof(Pitched), C.sizeof(BoxCopy), C.sizeof(HaloPush), C.sizeof(AstarothParams), C.sizeof(StepSync)]
 
 
+def test_astaroth_params_field_order_matches_the_header(tmp_path):
+    """sb_astaroth_params is thirteen doubles: two swapped fields keep the size, so compare each field's offset in the
+    header with the product's ctypes mirror (stencil_b200._lib.AstarothParams) and the oracle's (oracle.c_oracle.AcParams)."""
+    import subprocess
+
+    from oracle.c_oracle import AcParams
+    from stencil_b200._lib import AstarothParams
+
+    names = [n for n, _ in AstarothParams._fields_]
+    assert len(names) == 13
+    src = tmp_path / "probe.c"
+    body = "".join(f'  printf("{n} %zu\\n", offsetof(sb_astaroth_params, {n}));\n' for n in names)
+    src.write_text('#include <stddef.h>\n#include <stdio.h>\n#include "stencil_b200.h"\nint main(void) {\n' + body + "  return 0;\n}\n")
+    exe = tmp_path / "probe"
+    subprocess.check_call(["gcc", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)])
+    header = {n: int(v) for n, v in (line.split() for line in subprocess.check_output([str(exe)], text=True).splitlines())}
+    assert len(header) == 13
+    for struct in (AstarothParams, AcParams):
+        assert {n: getattr(struct, n).offset for n, _ in struct._fields_} == header, struct
+    # and the header has no field the mirrors lack: the offsets cover the whole struct
+    assert sorted(header.values()) == [8 * k for k in range(13)]
+
+
 def test_allocation_lead_rule(monkeypatch):
     """LocalDomain.lead_bytes (DESIGN.md section 1): when all rows share one 16-byte phase the allocation starts so that
     the first COMPUTE cell is 16-byte aligned; rows with alternating phase (FP32, 514 cells) keep the reference placement."""
