@@ -23,7 +23,7 @@ APIINC    := -Iinclude -Iinclude/mpi_shim -I/usr/local/cuda/include/nvtx3
 APIFLAGS  := -O3 -std=c++17 $(ARCH) -lineinfo -rdc=true --expt-extended-lambda -Xcompiler -fPIC -Xcompiler -Wall \
              -Xcompiler -Wno-comment -x cu $(APIDEFS) $(APIINC)
 APISRC    := src/compat_kernels.cu src/local_domain.cu src/packer.cu src/translator.cu src/stencil.cu src/jacobi3d.cu \
-             src/numeric.cpp src/timer.cpp src/rcstream.cpp src/topology.cpp src/gpu_topology.cpp \
+             src/numeric.cpp src/timer.cpp src/rcstream.cpp src/gpu_topology.cpp \
              src/placement_intranoderandom.cpp
 APIOBJ    := $(patsubst src/%,build/api/%.o,$(APISRC))
 # the core objects are compiled a second time with -rdc for the static library

@@ -7,9 +7,10 @@
 // them, unless a boundary condition is set for them (DistributedDomain::set_boundary_condition).
 
 #include <cassert>
+#include <cstdio>
+#include <cstdlib>
 
 #include "stencil/dim3.hpp"
-#include "stencil/logging.hpp"
 
 class Topology {
 public:
@@ -25,7 +26,28 @@ public:
   Topology(const Dim3 &extent, const Boundary &boundary) : grid_(extent), kind_{boundary, boundary, boundary} {}
   Topology(const Dim3 &extent, Boundary x, Boundary y, Boundary z) : grid_(extent), kind_{x, y, z} {}
 
-  OptionalNeighbor get_neighbor(const Dim3 &index, const Dim3 &dir) const noexcept;
+  OptionalNeighbor get_neighbor(const Dim3 &index, const Dim3 &dir) const noexcept {
+    assert(index.all_ge(0) && "subdomain indices are non-negative");
+    assert(dir.all_gt(-2) && dir.all_lt(2) && "a direction has components in {-1, 0, +1}");
+    OptionalNeighbor answer;
+    Dim3 to = index + dir;
+    answer.exists = true;
+    for (int a = 0; a < 3; ++a) {
+      switch (kind_[a]) {
+      case Boundary::PERIODIC: // a periodic axis wraps: stepping off one face re-enters through the opposite one
+        to[a] = ((to[a] % grid_[a]) + grid_[a]) % grid_[a];
+        break;
+      case Boundary::FIXED: // the grid ends at its faces along this axis: a step that leaves it has no neighbour
+        if (to[a] < 0 || to[a] >= grid_[a]) answer.exists = false;
+        break;
+      default:
+        std::fprintf(stderr, "Topology::get_neighbor: the topology has no boundary kind (default-constructed?)\n");
+        std::exit(1);
+      }
+    }
+    answer.index = answer.exists ? to : index;
+    return answer;
+  }
 
   const Dim3 &extent() const noexcept { return grid_; }
   Boundary boundary(int axis) const noexcept { return kind_[axis]; }

@@ -160,6 +160,43 @@ typedef struct sb_bc_region {
  * SB_ERR_INVALID when a kind is unknown or an EVEN / ODD face has a ghost width larger than the subdomain on its axis. */
 int sb_bc_regions(const int64_t size[3], const int64_t radius27[27], const int32_t kinds[6], sb_bc_region *out, int cap);
 
+/* ---------------------------------------------------------------------------------------------
+ * The exchange plan (include/stencil/exchange_plan.hpp), host only.  A grid of dim subdomains cut as (base, rem) --
+ * the pair sb_node_partition / sb_rank_partition return -- closed per axis by boundary[a] = 1 (PERIODIC: wraps) or
+ * 2 (FIXED: a wall), the values of Topology::Boundary.  Errors (SB_ERR_INVALID with a message): dim < 1 on an axis, an
+ * index outside the grid, another boundary value, an elem_size <= 0, an output capacity below the count.
+ * ------------------------------------------------------------------------------------------- */
+/* One message: the outermost compute cells of the source on side dir, at src_pos, go to the ghost cells of subdomain
+ * dst_idx on side -dir, at dst_pos; extent elements. */
+typedef struct sb_message {
+  int64_t dir[3];
+  int64_t dst_idx[3];
+  int64_t src_pos[3];
+  int64_t dst_pos[3];
+  int64_t extent[3];
+} sb_message;
+/* Every message subdomain src_idx sends, in direction order z, y, x ascending: a direction is skipped when
+ * radius27(-dir) == 0, when the step crosses a wall, or when the box is empty.  Returns the count (<= 26). */
+int sb_exchange_messages(const int64_t dim[3], const int64_t base[3], const int64_t rem[3], const int32_t boundary[3],
+                         const int64_t radius27[27], const int64_t src_idx[3], sb_message *out, int cap);
+
+/* Rows shorter than SB_STAGE_MAX_ROW_BYTES bound for another GPU travel through one dense staging buffer per
+ * (src, dst) pair in the receiver's memory.  Entry: quantity q of message msg (an index into src_idx's
+ * sb_exchange_messages list) sits at byte offset of that buffer. */
+#define SB_STAGE_MAX_ROW_BYTES 64
+typedef struct sb_staged {
+  int64_t msg;
+  int64_t q;
+  int64_t offset;
+} sb_staged;
+/* The layout of the (src_idx -> dst_idx) staging buffer for quantities of elem_sizes[0..nq): src_idx's messages to
+ * dst_idx in order, each one's quantities in order; a pair is staged when extent[0] * elem_size < SB_STAGE_MAX_ROW_BYTES.
+ * Each entry starts at a 16-byte boundary; *total = the end of the last one (0: nothing staged).  Returns the count.
+ * Whether staging applies at all (the two subdomains live on different GPUs) is the caller's decision. */
+int sb_staging_layout(const int64_t dim[3], const int64_t base[3], const int64_t rem[3], const int32_t boundary[3],
+                      const int64_t radius27[27], const int64_t src_idx[3], const int64_t dst_idx[3],
+                      const int64_t *elem_sizes, int nq, sb_staged *out, int cap, int64_t *total);
+
 /* One quantity of a BC plan: its allocation (the CURRENT buffer the plan will read and write), element type, and
  * per-face kind and value.  dtype RAW takes elem_size 1, 2, 4, 8 or 16 and allows NONE and EVEN only; F32 needs
  * elem_size 4, F64 elem_size 8.  value[f] is converted to the quantity's type. */

@@ -7,6 +7,7 @@
 // into the ghost cells of the destination subdomain -- same GPU, or a peer GPU through the
 // NVLink/NVSwitch peer mapping.  exchange() = N launches + N stream syncs, nothing else.
 #include "stencil/stencil.hpp"
+#include "stencil/exchange_plan.hpp"
 
 #include "stencil_b200.h"
 
@@ -361,84 +362,58 @@ void DistributedDomain::plan_exchange() {
     planFile << di << ":cuda" << domains_[di].gpu() << ":" << domainIdx_[di] << " sz=" << domains_[di].size() << "\n";
   planFile << "\n== fused direct-write messages ==\n";
 
-  // ---- geometry of every message that starts or ends at a local subdomain ------------------------------
-  struct Msg {
-    Dim3 srcIdx, dstIdx, dir, srcPos, dstPos, ext;
-  };
   auto gpu_key = [&](const Dim3 &idx) { return std::make_pair(placement_->get_rank(idx), placement_->get_cuda(idx)); };
   auto local_id = [&](const Dim3 &idx) { return placement_->get_rank(idx) == rank_ ? placement_->get_subdomain_id(idx) : -1; };
-  // all messages src -> dst in one canonical order (direction z, y, x ascending): both ends derive the same list
-  auto messages_from = [&](const Dim3 &srcIdx) {
-    std::vector<Msg> out;
-    const Dim3 srcSz = placement_->subdomain_size(srcIdx);
-    for (int z = -1; z <= 1; ++z)
-      for (int y = -1; y <= 1; ++y)
-        for (int x = -1; x <= 1; ++x) {
-          const Dim3 dir(x, y, z);
-          if (Dim3(0, 0, 0) == dir) continue;
-          // the neighbour on side dir needs our cells only if ITS stencil reaches back (-dir)
-          if (0 == radius_.dir(dir * -1)) continue;
-          const Topology::OptionalNeighbor nbr = topology_.get_neighbor(srcIdx, dir);
-          if (!nbr.exists) continue;
-          const Dim3 dstSz = placement_->subdomain_size(nbr.index);
-          const Dim3 ext = LocalDomain::halo_extent(dir * -1, dstSz, radius_);
-          if (0 == ext.flatten()) continue;
-          out.push_back(Msg{srcIdx, nbr.index, dir, LocalDomain::halo_pos(dir, srcSz, radius_, false),
-                            LocalDomain::halo_pos(dir * -1, dstSz, radius_, true), ext});
-        }
-    return out;
-  };
-  // thin rows (x-faces, x-edges, corners) bound for ANOTHER GPU are packed into one dense staging buffer in the receiver's
-  // memory and scattered there: layout of the (src -> dst) buffer, identical on both sides
-  constexpr int64_t kStageMaxRowBytes = 64;
-  struct Staged {
-    Msg m;
-    int64_t q, offset;
-  };
-  auto staging_layout = [&](const Dim3 &srcIdx, const Dim3 &dstIdx, int64_t *total) {
-    std::vector<Staged> out;
-    int64_t off = 0;
-    if (!(gpu_key(srcIdx) == gpu_key(dstIdx))) {
-      for (const Msg &m : messages_from(srcIdx)) {
-        if (!(m.dstIdx == dstIdx)) continue;
-        for (size_t q = 0; q < dataElemSize_.size(); ++q) {
-          const int64_t es = int64_t(dataElemSize_[q]);
-          if (m.ext.x * es >= kStageMaxRowBytes) continue;
-          off = (off + 15) & ~int64_t(15);
-          out.push_back(Staged{m, int64_t(q), off});
-          off += es * int64_t(m.ext.flatten());
-        }
-      }
-    }
-    *total = off;
-    return out;
-  };
-
-  // ---- staging buffers I receive into (allocated here, published to the senders) ----------------------------
-  std::map<std::pair<Dim3, Dim3>, char *> myStage;                  // (src idx, dst idx) -> buffer on dst's GPU
-  std::map<std::pair<Dim3, Dim3>, std::vector<Staged>> myStageEntries;
-  stageSenders_.assign(domains_.size(), {});
-  for (size_t dj = 0; dj < domains_.size(); ++dj) {
-    std::set<Dim3> sources;
+  auto neighbors = [&](const Dim3 &idx) {
+    std::set<Dim3> out;
     for (int z = -1; z <= 1; ++z)
       for (int y = -1; y <= 1; ++y)
         for (int x = -1; x <= 1; ++x) {
           if (0 == x && 0 == y && 0 == z) continue;
-          const Topology::OptionalNeighbor nb = topology_.get_neighbor(domainIdx_[dj], Dim3(x, y, z));
-          if (nb.exists) sources.insert(nb.index);
+          const Topology::OptionalNeighbor nb = topology_.get_neighbor(idx, Dim3(x, y, z));
+          if (nb.exists) out.insert(nb.index);
         }
-    for (const Dim3 &srcIdx : sources) {
-      int64_t total = 0;
-      std::vector<Staged> entries = staging_layout(srcIdx, domainIdx_[dj], &total);
-      if (0 == total) continue;
+    return out;
+  };
+
+  // ---- the plan (include/stencil/exchange_plan.hpp), computed once: the messages of every subdomain that sends to or
+  // receives from a local one, and the staging layout of every such (src, dst) pair on different GPUs
+  std::map<Dim3, std::vector<stencil::Message>> sends;
+  for (const Dim3 &idx : domainIdx_) {
+    sends[idx];
+    for (const Dim3 &nb : neighbors(idx)) sends[nb];
+  }
+  for (auto &kv : sends)
+    kv.second = stencil::messages_from(kv.first, topology_, radius_, [&](const Dim3 &idx) { return placement_->subdomain_size(idx); });
+  const std::vector<int64_t> elemSizes(dataElemSize_.begin(), dataElemSize_.end());
+  struct Layout {
+    std::vector<stencil::Staged> entries;
+    int64_t total = 0;
+  };
+  std::map<std::pair<Dim3, Dim3>, Layout> layouts; // only pairs with something staged
+  for (const auto &kv : sends)
+    for (const stencil::Message &m : kv.second) {
+      const auto key = std::make_pair(m.srcIdx, m.dstIdx);
+      if ((local_id(m.srcIdx) < 0 && local_id(m.dstIdx) < 0) || gpu_key(m.srcIdx) == gpu_key(m.dstIdx) || layouts.count(key)) continue;
+      Layout l;
+      l.entries = stencil::staging_layout(kv.second, m.dstIdx, elemSizes, &l.total);
+      if (l.total > 0) layouts[key] = l;
+    }
+
+  // ---- staging buffers I receive into (allocated here, published to the senders) ----------------------------
+  std::map<std::pair<Dim3, Dim3>, char *> myStage; // (src idx, dst idx) -> buffer on dst's GPU
+  stageSenders_.assign(domains_.size(), {});
+  for (size_t dj = 0; dj < domains_.size(); ++dj) {
+    for (const Dim3 &srcIdx : neighbors(domainIdx_[dj])) {
+      const auto key = std::make_pair(srcIdx, domainIdx_[dj]);
+      const auto it = layouts.find(key);
+      if (it == layouts.end()) continue;
       void *buf = nullptr;
       CUDA_RUNTIME(cudaSetDevice(domains_[dj].gpu()));
-      CUDA_RUNTIME(cudaMalloc(&buf, size_t(total)));
+      CUDA_RUNTIME(cudaMalloc(&buf, size_t(it->second.total)));
       stagingBufs_.push_back(buf);
       stagingDevs_.push_back(domains_[dj].gpu());
-      const auto key = std::make_pair(srcIdx, domainIdx_[dj]);
       myStage[key] = static_cast<char *>(buf);
-      myStageEntries[key] = entries;
       if (local_id(srcIdx) >= 0) stageSenders_[dj].push_back(size_t(local_id(srcIdx)));
     }
   }
@@ -464,11 +439,19 @@ void DistributedDomain::plan_exchange() {
   };
 
   // ---- the two plans per subdomain and swap parity -----------------------------------------------------
+  const size_t nq = dataElemSize_.size();
   for (int parity = 0; parity < 2; ++parity) {
     for (size_t di = 0; di < domains_.size(); ++di) {
       const LocalDomain &src = domains_[di];
+      const std::vector<stencil::Message> &msgs = sends.at(domainIdx_[di]);
+      // staging offset of quantity q of message i at [i * nq + q], -1 where it goes straight into the ghost cells
+      std::vector<int64_t> stagedAt(msgs.size() * nq, -1);
+      for (const auto &kv : layouts)
+        if (kv.first.first == domainIdx_[di])
+          for (const stencil::Staged &st : kv.second.entries) stagedAt[st.msg * nq + size_t(st.q)] = st.offset;
       std::vector<sb_box_copy> copies;
-      for (const Msg &m : messages_from(domainIdx_[di])) {
+      for (size_t i = 0; i < msgs.size(); ++i) {
+        const stencil::Message &m = msgs[i];
         const bool sameGpu = gpu_key(m.srcIdx) == gpu_key(m.dstIdx);
         const bool remote = placement_->get_rank(m.dstIdx) != rank_;
         if (!remote && !gpu_topo::peer(src.gpu(), placement_->get_cuda(m.dstIdx)))
@@ -476,28 +459,21 @@ void DistributedDomain::plan_exchange() {
         // where this pair's thin rows go, if anywhere
         const auto key = std::make_pair(m.srcIdx, m.dstIdx);
         char *stageBase = nullptr;
-        std::vector<Staged> entries;
-        if (!sameGpu) {
-          int64_t total = 0;
-          entries = staging_layout(m.srcIdx, m.dstIdx, &total);
-          if (total > 0) {
-            stageBase = remote ? remoteStage_[key] : myStage[key];
-            if (!stageBase) LOG_FATAL("no staging buffer for " << m.srcIdx << " -> " << m.dstIdx);
-          }
+        if (layouts.count(key)) {
+          stageBase = remote ? remoteStage_[key] : myStage[key];
+          if (!stageBase) LOG_FATAL("no staging buffer for " << m.srcIdx << " -> " << m.dstIdx);
         }
         uint64_t msgBytes = 0;
-        for (size_t q = 0; q < dataElemSize_.size(); ++q) {
+        for (size_t q = 0; q < nq; ++q) {
           sb_box_copy c{};
           c.elem_size = int64_t(dataElemSize_[q]);
           msgBytes += uint64_t(c.elem_size) * m.ext.flatten();
           c.src = pitched_of(m.srcIdx, q, parity);
           set3(c.src_pos, m.srcPos);
           set3(c.extent, m.ext);
-          const Staged *st = nullptr;
-          for (const Staged &cand : entries)
-            if (cand.m.dir == m.dir && cand.q == int64_t(q)) st = &cand;
-          if (st) { // dense staging buffer in the receiver's memory
-            c.dst = sb_pitched{stageBase + st->offset, m.ext.x * c.elem_size, m.ext.y};
+          const int64_t offset = stagedAt[i * nq + q];
+          if (offset >= 0) { // dense staging buffer in the receiver's memory
+            c.dst = sb_pitched{stageBase + offset, m.ext.x * c.elem_size, m.ext.y};
           } else {
             c.dst = pitched_of(m.dstIdx, q, parity);
             set3(c.dst_pos, m.dstPos);
@@ -531,15 +507,16 @@ void DistributedDomain::plan_exchange() {
 
       // phase 2 of this subdomain as a receiver
       std::vector<sb_box_copy> scatter;
-      for (const auto &kv : myStageEntries) {
+      for (const auto &kv : layouts) {
         if (!(kv.first.second == domainIdx_[di])) continue;
-        for (const Staged &st : kv.second) {
+        for (const stencil::Staged &st : kv.second.entries) {
+          const stencil::Message &m = sends.at(kv.first.first)[st.msg];
           sb_box_copy c{};
           c.elem_size = int64_t(dataElemSize_[size_t(st.q)]);
-          c.src = sb_pitched{myStage[kv.first] + st.offset, st.m.ext.x * c.elem_size, st.m.ext.y};
+          c.src = sb_pitched{myStage[kv.first] + st.offset, m.ext.x * c.elem_size, m.ext.y};
           c.dst = pitched_of(domainIdx_[di], size_t(st.q), parity);
-          set3(c.dst_pos, st.m.dstPos);
-          set3(c.extent, st.m.ext);
+          set3(c.dst_pos, m.dstPos);
+          set3(c.extent, m.ext);
           scatter.push_back(c);
         }
       }
@@ -558,7 +535,7 @@ void DistributedDomain::plan_exchange() {
   {
     std::vector<double> mat(size_t(worldSize_) * size_t(worldSize_), 0.0);
     for (size_t di = 0; di < domains_.size(); ++di)
-      for (const Msg &m : messages_from(domainIdx_[di])) {
+      for (const stencil::Message &m : sends.at(domainIdx_[di])) {
         double bytes = 0;
         for (size_t q = 0; q < dataElemSize_.size(); ++q) bytes += double(dataElemSize_[q]) * double(m.ext.flatten());
         mat[size_t(rank_) * size_t(worldSize_) + size_t(placement_->get_rank(m.dstIdx))] += bytes;

@@ -63,6 +63,24 @@ class BcRegion(C.Structure):
     ]
 
 
+class Message(C.Structure):
+    """sb_message: one halo message of the exchange plan."""
+
+    _fields_ = [
+        ("dir", C.c_int64 * 3),
+        ("dst_idx", C.c_int64 * 3),
+        ("src_pos", C.c_int64 * 3),
+        ("dst_pos", C.c_int64 * 3),
+        ("extent", C.c_int64 * 3),
+    ]
+
+
+class Staged(C.Structure):
+    """sb_staged: quantity q of message msg at byte offset of a staging buffer."""
+
+    _fields_ = [("msg", C.c_int64), ("q", C.c_int64), ("offset", C.c_int64)]
+
+
 class BcQuantity(C.Structure):
     """sb_bc_quantity: one quantity of a boundary-condition plan."""
 
@@ -132,6 +150,8 @@ _SIGS = {
     "sb_copy_plan_num_tma_segments": (C.c_int64, [C.c_void_p]),
     "sb_copy_plan_destroy": (C.c_int, [C.c_void_p]),
     "sb_bc_regions": (C.c_int, [I3, I27, I6, C.POINTER(BcRegion), C.c_int]),
+    "sb_exchange_messages": (C.c_int, [I3, I3, I3, C.c_int32 * 3, I27, I3, C.POINTER(Message), C.c_int]),
+    "sb_staging_layout": (C.c_int, [I3, I3, I3, C.c_int32 * 3, I27, I3, I3, C.POINTER(C.c_int64), C.c_int, C.POINTER(Staged), C.c_int, C.POINTER(C.c_int64)]),
     "sb_bc_plan_create": (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.POINTER(BcQuantity), C.c_int64, I3, I27]),
     "sb_bc_plan_launch": (C.c_int, [C.c_void_p, C.c_void_p]),
     "sb_bc_plan_bytes": (C.c_int64, [C.c_void_p]),

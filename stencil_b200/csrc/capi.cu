@@ -19,6 +19,7 @@
 #include "astaroth.cuh"
 #include "jacobi.cuh"
 
+#include "stencil/exchange_plan.hpp"
 #include "stencil/geometry.hpp"
 #include "stencil/partition_core.hpp"
 
@@ -501,6 +502,31 @@ int bc_regions(const int64_t size[3], const int64_t r27[27], const int32_t kinds
   return SB_OK;
 }
 
+// ------------------------------------------------------------------------------------------- exchange plan
+bool in_grid(const int64_t idx[3], const int64_t dim[3]) {
+  for (int a = 0; a < 3; ++a)
+    if (idx[a] < 0 || idx[a] >= dim[a]) return false;
+  return true;
+}
+
+// The messages of src_idx (the arithmetic behind sb_exchange_messages and sb_staging_layout), after checking the grid.
+int exchange_messages(const int64_t dim[3], const int64_t base[3], const int64_t rem[3], const int32_t boundary[3],
+                      const int64_t r27[27], const int64_t src_idx[3], std::vector<stencil::Message> &out) {
+  if (!dim || !base || !rem || !boundary || !r27 || !src_idx) return fail(SB_ERR_INVALID, "null argument");
+  Topology::Boundary kind[3];
+  for (int a = 0; a < 3; ++a) {
+    if (dim[a] < 1) return fail(SB_ERR_INVALID, "the grid needs at least one subdomain per axis (dim[%d] = %lld)", a, (long long)dim[a]);
+    if (boundary[a] != int32_t(Topology::Boundary::PERIODIC) && boundary[a] != int32_t(Topology::Boundary::FIXED))
+      return fail(SB_ERR_INVALID, "boundary[%d] = %d: must be 1 (PERIODIC) or 2 (FIXED)", a, int(boundary[a]));
+    kind[a] = Topology::Boundary(boundary[a]);
+  }
+  if (!in_grid(src_idx, dim)) return fail(SB_ERR_INVALID, "source subdomain index outside the grid");
+  const stencil::detail::CutGrid grid{d3(base), d3(rem)};
+  out = stencil::messages_from(d3(src_idx), Topology(d3(dim), kind[0], kind[1], kind[2]), radius_of(r27),
+                               [&](const Dim3 &idx) { return grid.size_of(idx); });
+  return SB_OK;
+}
+
 } // namespace
 
 struct sb_bc_plan {
@@ -742,6 +768,43 @@ int sb_bc_regions(const int64_t size[3], const int64_t radius27[27], const int32
   if (rc != SB_OK) return rc;
   for (size_t i = 0; i < regs.size() && int(i) < cap; ++i) out[i] = regs[i];
   return int(regs.size());
+}
+
+// ----------------------------------------------------------------------------------------- exchange plan
+int sb_exchange_messages(const int64_t dim[3], const int64_t base[3], const int64_t rem[3], const int32_t boundary[3],
+                         const int64_t radius27[27], const int64_t src_idx[3], sb_message *out, int cap) {
+  std::vector<stencil::Message> msgs;
+  const int rc = exchange_messages(dim, base, rem, boundary, radius27, src_idx, msgs);
+  if (rc != SB_OK) return rc;
+  if (cap < int(msgs.size()) || (!msgs.empty() && !out))
+    return fail(SB_ERR_INVALID, "output capacity %d too small for %zu messages", cap, msgs.size());
+  for (size_t i = 0; i < msgs.size(); ++i) {
+    put(msgs[i].dir, out[i].dir);
+    put(msgs[i].dstIdx, out[i].dst_idx);
+    put(msgs[i].srcPos, out[i].src_pos);
+    put(msgs[i].dstPos, out[i].dst_pos);
+    put(msgs[i].ext, out[i].extent);
+  }
+  return int(msgs.size());
+}
+
+int sb_staging_layout(const int64_t dim[3], const int64_t base[3], const int64_t rem[3], const int32_t boundary[3],
+                      const int64_t radius27[27], const int64_t src_idx[3], const int64_t dst_idx[3],
+                      const int64_t *elem_sizes, int nq, sb_staged *out, int cap, int64_t *total) {
+  static_assert(SB_STAGE_MAX_ROW_BYTES == stencil::kStageMaxRowBytes, "one staging threshold");
+  if (!dst_idx || !total || nq < 0 || (nq > 0 && !elem_sizes)) return fail(SB_ERR_INVALID, "bad arguments to sb_staging_layout");
+  std::vector<stencil::Message> msgs;
+  const int rc = exchange_messages(dim, base, rem, boundary, radius27, src_idx, msgs);
+  if (rc != SB_OK) return rc;
+  if (!in_grid(dst_idx, dim)) return fail(SB_ERR_INVALID, "destination subdomain index outside the grid");
+  for (int q = 0; q < nq; ++q)
+    if (elem_sizes[q] <= 0) return fail(SB_ERR_INVALID, "quantity %d: elem_size %lld must be > 0", q, (long long)elem_sizes[q]);
+  const std::vector<stencil::Staged> staged =
+      stencil::staging_layout(msgs, d3(dst_idx), std::vector<int64_t>(elem_sizes, elem_sizes + nq), total);
+  if (cap < int(staged.size()) || (!staged.empty() && !out))
+    return fail(SB_ERR_INVALID, "output capacity %d too small for %zu staged entries", cap, staged.size());
+  for (size_t i = 0; i < staged.size(); ++i) out[i] = sb_staged{int64_t(staged[i].msg), staged[i].q, staged[i].offset};
+  return int(staged.size());
 }
 
 int sb_bc_plan_create(sb_bc_plan **out, int device, const sb_bc_quantity *quantities, int64_t n, const int64_t size[3],

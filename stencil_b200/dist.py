@@ -21,7 +21,7 @@ import os
 from dataclasses import dataclass
 from typing import Dict, List, Tuple
 
-from ._lib import Pitched, check, lib, stream_ptr
+from ._lib import Pitched, Staged, check, i3, lib, stream_ptr
 
 Vec = Tuple[int, int, int]
 
@@ -221,62 +221,35 @@ def share_domains(dd, w: World) -> RemoteDomains:
     return RemoteDomains(dd, w)
 
 
-# --------------------------------------------------------------------------------------------- NCCL fallback
 def messages_from(dd, src_rank: int) -> List[dict]:
-    """The send plan of ANY rank (pure geometry: every rank can compute every other rank's plan)."""
-    from .domain import ALL_DIRS, halo_extent, halo_pos
-
-    part, radius = dd.partition_, dd.radius_
-    out = []
-    for idx in part.indices():
-        rank, slot = dd._owner[idx]
-        if rank != src_rank:
-            continue
-        sz = part.subdomain_size(idx)
-        for d in ALL_DIRS:
-            nd = (-d[0], -d[1], -d[2])
-            if radius.dir(nd) == 0:
-                continue
-            dst_idx = dd.topology_.get_neighbor(idx, d)
-            if dst_idx is None:
-                continue  # a wall: nothing crosses it
-            dst_sz = part.subdomain_size(dst_idx)
-            ext = halo_extent(nd, dst_sz, radius)
-            if ext[0] * ext[1] * ext[2] == 0:
-                continue
-            out.append(
-                dict(src_idx=idx, src_slot=slot, dst_idx=dst_idx, dst_rank=dd._owner[dst_idx][0], dst_slot=dd._owner[dst_idx][1], dir=d,
-                     src_pos=halo_pos(d, sz, radius, False), dst_pos=halo_pos(nd, dst_sz, radius, True), ext=ext)
-            )
-    return out
-
-
-STAGE_MAX_ROW_BYTES = 64
+    """The send plan of ANY rank: DistributedDomain.plan_messages(src_rank) (every rank can compute every other rank's
+    plan)."""
+    return dd.plan_messages(src_rank)
 
 
 def staging_layout(dd, src_idx, dst_idx):
     """Messages from subdomain src_idx to subdomain dst_idx (on a DIFFERENT GPU) whose rows are shorter than
-    STAGE_MAX_ROW_BYTES (x-faces, x-edges, corners): storing such rows straight into the peer's ghost cells costs one
+    SB_STAGE_MAX_ROW_BYTES (x-faces, x-edges, corners): storing such rows straight into the peer's ghost cells costs one
     tiny NVLink transaction per row (1.6 M 8-byte remote stores per exchange on two GPUs, and a much slower
     interior kernel), so the sender packs them into ONE dense receive buffer in the peer's memory (contiguous 128-byte
-    NVLink packets) and the receiver scatters them locally.  Pure geometry: both sides compute the same layout.
-    Returns (total_bytes, [dict(dir, q, offset, ext, src_pos, dst_pos, es)])."""
-    es = [int(e) for e in dd._elem_sizes()]
-    entries, off = [], 0
-    src_rank = dd._owner[tuple(src_idx)][0]
-    for m in messages_from(dd, src_rank):
-        if tuple(m["src_idx"]) != tuple(src_idx) or tuple(m["dst_idx"]) != tuple(dst_idx):
-            continue
-        n = m["ext"][0] * m["ext"][1] * m["ext"][2]
-        for q, e in enumerate(es):
-            if m["ext"][0] * e >= STAGE_MAX_ROW_BYTES:
-                continue
-            off = (off + 15) & ~15
-            entries.append(dict(dir=m["dir"], q=q, offset=off, ext=m["ext"], src_pos=m["src_pos"], dst_pos=m["dst_pos"], es=e))
-            off += n * e
-    return off, entries
+    NVLink packets) and the receiver scatters them locally.  Pure geometry (sb_staging_layout): both sides compute the
+    same layout.  Returns (total_bytes, [dict(dir, q, offset, ext, src_pos, dst_pos, es)])."""
+    from .domain import exchange_messages, grid_args
+
+    es = dd._elem_sizes()
+    msgs = exchange_messages(dd.partition_, dd.topology_, dd.radius_, src_idx)
+    cap = len(msgs) * len(es)
+    out, total = (Staged * max(cap, 1))(), C.c_int64(0)
+    n = check(lib().sb_staging_layout(*grid_args(dd.partition_, dd.topology_, dd.radius_), i3(src_idx), i3(dst_idx),
+                                      (C.c_int64 * len(es))(*es), len(es), out, cap, C.byref(total)))
+    entries = []
+    for st in out[:n]:
+        m = msgs[st.msg]
+        entries.append(dict(dir=m["dir"], q=st.q, offset=st.offset, ext=m["ext"], src_pos=m["src_pos"], dst_pos=m["dst_pos"], es=es[st.q]))
+    return total.value, entries
 
 
+# --------------------------------------------------------------------------------------------- NCCL fallback
 def wire_order(msgs: List[dict]) -> List[dict]:
     """Sender and receiver agree on one order per (src rank -> dst rank) buffer: larger messages first, ties by
     (src subdomain, direction) -- Message::by_size of the reference (tx_common.hpp:25-36) extended to several
@@ -310,12 +283,12 @@ class NcclExchange:
                     off += n * e
             return off, entries
 
-        mine = messages_from(dd, w.rank)
+        mine = dd.plan_messages(w.rank)
         self.peers = sorted({m["dst_rank"] for m in mine} - {w.rank})
         self.send_buf, self.recv_buf, self.pack, self.unpack = {}, {}, {}, {}
         for b in self.peers:
             out_total, out_entries = layout([m for m in mine if m["dst_rank"] == b])
-            in_total, in_entries = layout([m for m in messages_from(dd, b) if m["dst_rank"] == w.rank])
+            in_total, in_entries = layout([m for m in dd.plan_messages(b) if m["dst_rank"] == w.rank])
             self.send_buf[b] = torch.empty(max(out_total, 1), dtype=torch.uint8, device=f"cuda:{self.dev}")
             self.recv_buf[b] = torch.empty(max(in_total, 1), dtype=torch.uint8, device=f"cuda:{self.dev}")
             self.pack[b], self.unpack[b] = [], []

@@ -18,8 +18,8 @@ Two deployment modes, one code path:
     through the IPC mappings over NVLink, ordered by device-side ready/done flags (no host barrier
     in the exchange).
 
-All arithmetic on coordinates is delegated to the C ABI (sb_halo_pos, sb_node_partition, ...);
-this module only sequences calls.  No CPU fallback exists.
+All arithmetic on coordinates is delegated to the C ABI (sb_halo_pos, sb_node_partition,
+sb_exchange_messages, sb_staging_layout, ...); this module only sequences calls.  No CPU fallback exists.
 """
 from __future__ import annotations
 
@@ -40,10 +40,6 @@ Vec = Tuple[int, int, int]
 ALL_DIRS: List[Vec] = [
     (x, y, z) for z in (-1, 0, 1) for y in (-1, 0, 1) for x in (-1, 0, 1) if (x, y, z) != (0, 0, 0)
 ]
-
-
-def _neg(d: Vec) -> Vec:
-    return (-d[0], -d[1], -d[2])
 
 
 class Method(enum.IntFlag):
@@ -228,6 +224,22 @@ class Topology:
         d = [0, 0, 0]
         d[face // 2] = 1 if face % 2 else -1
         return self.get_neighbor(idx, tuple(d)) is None
+
+
+def grid_args(part: Partition, topology: Topology, radius: Radius) -> tuple:
+    """The (dim, base, rem, boundary, radius27) arguments of sb_exchange_messages and sb_staging_layout."""
+    return i3(part.dim), part._base, part._rem, (C.c_int32 * 3)(*[b.value for b in topology.boundaries]), radius.c27()
+
+
+def exchange_messages(part: Partition, topology: Topology, radius: Radius, src_idx: Vec) -> List[dict]:
+    """sb_exchange_messages: every message subdomain src_idx sends, in direction order z, y, x ascending.
+    dict(src_idx, dst_idx, dir, src_pos, dst_pos, ext)."""
+    out = (_lib.Message * 26)()
+    n = check(lib().sb_exchange_messages(*grid_args(part, topology, radius), i3(src_idx), out, 26))
+    return [
+        dict(src_idx=tuple(src_idx), dst_idx=t3(m.dst_idx), dir=t3(m.dir), src_pos=t3(m.src_pos), dst_pos=t3(m.dst_pos), ext=t3(m.extent))
+        for m in out[:n]
+    ]
 
 
 class BCKind(enum.IntEnum):
@@ -824,28 +836,31 @@ class DistributedDomain:
         """NCCL mode: messages from other ranks arrive packed through NCCL, not through staging buffers."""
         for key in [k for k in self._recv_local if self._owner[k[0]][0] != self._world.rank]:
             lib().sb_free(C.c_void_p(self._recv_local.pop(key)), self.domains_[0].gpu())
-            self._recv_entries.pop(key)
+
+    def _layout(self, src_idx: Vec, dst_idx: Vec) -> Tuple[int, List[dict]]:
+        """dist.staging_layout of the (src -> dst) pair, computed once per realize()."""
+        from . import dist as _dist
+
+        key = (tuple(src_idx), tuple(dst_idx))
+        if key not in self._layouts:
+            self._layouts[key] = _dist.staging_layout(self, *key)
+        return self._layouts[key]
 
     def _alloc_staging(self) -> None:
         """Receive buffers (on MY GPUs) for the thin messages other GPUs send to my subdomains (dist.staging_layout)."""
-        from . import dist as _dist
-
         self._recv_local: Dict[tuple, int] = {}
-        self._recv_entries: Dict[tuple, list] = {}
-        if os.environ.get("SB_NO_STAGING", "0") == "1":
-            return
+        self._layouts: Dict[tuple, Tuple[int, List[dict]]] = {}
         for di, dst_idx in enumerate(self.domain_idx_):
             srcs = {self.topology_.get_neighbor(dst_idx, d) for d in ALL_DIRS} - {None}
             for src_idx in sorted(srcs):
                 if self._gpu_key(src_idx) == self._gpu_key(dst_idx):
                     continue
-                total, entries = _dist.staging_layout(self, src_idx, dst_idx)
+                total, _ = self._layout(src_idx, dst_idx)
                 if total == 0:
                     continue
                 p = C.c_void_p()
                 check(lib().sb_malloc(C.byref(p), total, self.domains_[di].gpu()))
                 self._recv_local[(tuple(src_idx), tuple(dst_idx))] = int(p.value)
-                self._recv_entries[(tuple(src_idx), tuple(dst_idx))] = entries
 
     def _staging_target(self, src_idx: Vec, dst_idx: Vec):
         """Address of the staging buffer for (src -> dst), wherever dst lives; None if this pair is not staged."""
@@ -856,38 +871,19 @@ class DistributedDomain:
             return self._remote.recv[key]
         return None
 
-    def plan_messages(self) -> List[dict]:
-        """The send plan of this rank (pure geometry, no GPU): one entry per (local subdomain, direction)
-        with a non-zero receiving radius -- src/stencil.cu:327-412.  dict(src_slot, src_idx, dst_idx,
-        dst_rank, dst_slot, dir, src_pos, dst_pos, ext)."""
-        part = self.partition_
-        my = [idx for idx in part.indices() if self._owner[idx][0] == self._world.rank]
+    def plan_messages(self, rank: Optional[int] = None) -> List[dict]:
+        """The send plan of `rank` (default: this rank).  Pure geometry, no GPU: every rank can compute every other
+        rank's plan.  exchange_messages of each subdomain the rank owns, in partition order, with the owners added:
+        dict(src_slot, src_idx, dst_idx, dst_rank, dst_slot, dir, src_pos, dst_pos, ext)."""
+        rank = self._world.rank if rank is None else rank
         out = []
-        for slot, idx in enumerate(my):
-            sz = part.subdomain_size(idx)
-            for dirv in ALL_DIRS:
-                if self.radius_.dir(_neg(dirv)) == 0:
-                    continue  # src/stencil.cu:344
-                dst_idx = self.topology_.get_neighbor(idx, dirv)
-                if dst_idx is None:
-                    continue  # a wall: nothing crosses it
-                dst_sz = part.subdomain_size(dst_idx)
-                ext = halo_extent(_neg(dirv), dst_sz, self.radius_)  # stencil.cu:361-363
-                if ext[0] * ext[1] * ext[2] == 0:
-                    continue
-                out.append(
-                    dict(
-                        src_slot=slot,
-                        src_idx=idx,
-                        dst_idx=dst_idx,
-                        dst_rank=self._owner[dst_idx][0],
-                        dst_slot=self._owner[dst_idx][1],
-                        dir=dirv,
-                        src_pos=halo_pos(dirv, sz, self.radius_, False),
-                        dst_pos=halo_pos(_neg(dirv), dst_sz, self.radius_, True),
-                        ext=ext,
-                    )
-                )
+        for idx in self.partition_.indices():
+            owner, slot = self._owner[idx]
+            if owner != rank:
+                continue
+            for m in exchange_messages(self.partition_, self.topology_, self.radius_, idx):
+                dst_rank, dst_slot = self._owner[m["dst_idx"]]
+                out.append(dict(m, src_slot=slot, dst_rank=dst_rank, dst_slot=dst_slot))
         return out
 
     def _assign_owners(self) -> None:
@@ -902,8 +898,6 @@ class DistributedDomain:
         neighbour's ghost cells (same GPU, or wide rows over NVLink) or, for thin rows bound for another GPU, into
         the neighbour's dense staging buffer.  Phase 2 (one launch per local subdomain that has staged senders):
         scatter the staging buffers into the ghost cells."""
-        from . import dist as _dist
-
         for d in self.domains_:
             d._curr0, d._next0 = list(d.curr_), list(d.next_)
         self._plans, self._unpack_plans = [], []
@@ -925,8 +919,7 @@ class DistributedDomain:
                     stage_base = None if self._gpu_key(m["src_idx"]) == self._gpu_key(m["dst_idx"]) else self._staging_target(m["src_idx"], m["dst_idx"])
                     staged = {}
                     if stage_base is not None:
-                        _, entries = _dist.staging_layout(self, m["src_idx"], m["dst_idx"])
-                        staged = {e["q"]: e for e in entries if e["dir"] == m["dir"]}
+                        staged = {e["q"]: e for e in self._layout(m["src_idx"], m["dst_idx"])[1] if e["dir"] == m["dir"]}
                     for q in range(d.num_data()):
                         es = d.elem_size(q)
                         src_p, _ = self._pitched_of(m["src_idx"], q, parity)
@@ -950,7 +943,7 @@ class DistributedDomain:
                 for (src_idx, dst_idx), base in self._recv_local.items():
                     if dst_idx != tuple(self.domain_idx_[di]):
                         continue
-                    for e in self._recv_entries[(src_idx, dst_idx)]:
+                    for e in self._layout(src_idx, dst_idx)[1]:
                         dst_p, _ = self._pitched_of(dst_idx, e["q"], parity)
                         dense = Pitched(base + e["offset"], e["ext"][0] * e["es"], e["ext"][1])
                         ucopies.append(box_copy(dst_p, e["dst_pos"], dense, (0, 0, 0), e["ext"], e["es"]))

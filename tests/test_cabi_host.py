@@ -202,6 +202,34 @@ def test_astaroth_params_field_order_matches_the_header(tmp_path):
     assert sorted(header.values()) == [8 * k for k in range(13)]
 
 
+def test_exchange_plan_structs_match_the_header(tmp_path):
+    """sb_message and sb_staged hold only int64 fields, so a swapped pair keeps the size: compare each field's offset
+    and each struct's size in the header with the ctypes mirrors, and check that the exchange-plan entry points exist."""
+    import subprocess
+
+    from stencil_b200._lib import Message, Staged
+
+    structs = {"sb_message": Message, "sb_staged": Staged}
+    body = ""
+    for cname, struct in structs.items():
+        body += f'  printf("{cname} sizeof %zu\\n", sizeof({cname}));\n'
+        body += "".join(f'  printf("{cname} {n} %zu\\n", offsetof({cname}, {n}));\n' for n, _ in struct._fields_)
+    src = tmp_path / "probe.c"
+    src.write_text('#include <stddef.h>\n#include <stdio.h>\n#include "stencil_b200.h"\nint main(void) {\n' + body + "  return 0;\n}\n")
+    exe = tmp_path / "probe"
+    subprocess.check_call(["gcc", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)])
+    header = {}
+    for line in subprocess.check_output([str(exe)], text=True).splitlines():
+        cname, field, value = line.split()
+        header[(cname, field)] = int(value)
+    for cname, struct in structs.items():
+        assert header[(cname, "sizeof")] == C.sizeof(struct), cname
+        for n, _ in struct._fields_:
+            assert header[(cname, n)] == getattr(struct, n).offset, (cname, n)
+    L = C.CDLL(sb.LIB_PATH)
+    assert hasattr(L, "sb_exchange_messages") and hasattr(L, "sb_staging_layout")
+
+
 def test_allocation_lead_rule(monkeypatch):
     """LocalDomain.lead_bytes (DESIGN.md section 1): when all rows share one 16-byte phase the allocation starts so that
     the first COMPUTE cell is 16-byte aligned; rows with alternating phase (FP32, 514 cells) keep the reference placement."""
