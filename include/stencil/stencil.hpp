@@ -26,6 +26,7 @@
 #include "stencil/dim3.hpp"
 #include "stencil/direction_map.hpp"
 #include "stencil/gpu_topology.hpp"
+#include "stencil/linear_stencil.hpp"
 #include "stencil/local_domain.cuh"
 #include "stencil/logging.hpp"
 #include "stencil/machine.hpp"
@@ -44,6 +45,7 @@
 struct sb_copy_plan;
 struct sb_bc_plan;
 struct sb_reduce_plan;
+struct sb_stencil_plan;
 
 class DistributedDomain {
 private:
@@ -122,6 +124,14 @@ private:
   };
   std::map<std::vector<int64_t>, ReduceCache> reducePlans_;
   void destroy_reduce_plans();
+
+  // linear stencil operators: per (op, buffers, exchange, swap parity), per local domain the interior and exterior plans
+  // (exchange = true) or the whole-region plan; two streams per local domain (interior, exterior)
+  std::map<std::vector<int64_t>, std::vector<std::vector<sb_stencil_plan *>>> stencilPlans_;
+  std::vector<cudaStream_t> applyStreams_;
+  void destroy_stencil_plans();
+  void apply_op(const stencil::LinearStencil &op, int dtype, size_t dq, stencil::Which dw, size_t sq, int64_t aq, stencil::Which aw,
+                bool exchange);
 
   std::string outputPrefix_;
 
@@ -247,6 +257,23 @@ public:
     return reduce_many(std::vector<stencil::ReduceItem>(1, stencil::ReduceItem::norm(x, y, z)))[0];
   }
   std::vector<stencil::Reduction> reduce_many(const std::vector<stencil::ReduceItem> &items);
+
+  // dst = op(src, aux) over the whole compute region of every local subdomain (DESIGN.md section 2.7).  src is the curr
+  // buffer (the one exchange() fills); dst is curr or next of any quantity of the same type, never src itself; aux is curr
+  // or next and may be dst.  Fails loudly unless realize() has run and sb_stencil_check accepts the op for this domain's
+  // radius.  exchange = true: the interior runs on its own stream while exchange() fills the ghost cells, then one launch
+  // per subdomain covers its exterior slabs; exchange = false: one launch over the whole region, the caller guarantees the
+  // ghost cells are current.  Returns when the update is complete.  The plans are kept, per (op, buffers, exchange, swap
+  // parity), until the domain is destroyed.
+  template <typename T>
+  void apply(const stencil::LinearStencil &op, const stencil::Buffer<T> &dst, const DataHandle<T> &src, bool exchange = true) {
+    apply_op(op, stencil::bc_dtype<T>(), dst.h.id(), dst.which, src.id(), -1, stencil::Which::curr, exchange);
+  }
+  template <typename T>
+  void apply(const stencil::LinearStencil &op, const stencil::Buffer<T> &dst, const DataHandle<T> &src, const stencil::Buffer<T> &aux,
+             bool exchange = true) {
+    apply_op(op, stencil::bc_dtype<T>(), dst.h.id(), dst.which, src.id(), int64_t(aux.h.id()), aux.which, exchange);
+  }
 
   // one CSV file per subdomain: Z,Y,X,<quantities...>
   void write_paraview(const std::string &prefix, bool zeroNaNs = false);

@@ -268,6 +268,54 @@ int sb_reduce_plan_destroy(sb_reduce_plan *plan);
 int sb_reduce_combine(const sb_reduce_result *parts, int64_t n, sb_reduce_result *out);
 
 /* ---------------------------------------------------------------------------------------------
+ * Constant-coefficient linear stencil operators (not in the reference; DESIGN.md section 2.7).
+ * An operator is a list of 1 <= n <= SB_STENCIL_MAX_TERMS terms (source s, offset o, weight w): s = 0 reads src at
+ * p + o, s = 1 reads aux at p (aux terms have offset 0: a previous time level, a right-hand side, a blend);
+ * |o_a| <= SB_STENCIL_MAX_REACH.  For every cell p of a box, in the quantity's type T with every multiply and add
+ * rounded to nearest separately (no FMA contraction), T(w) = w rounded to T:
+ *   acc = T(w_0) * S_0(p + o_0);  acc = acc + T(w_k) * S_k(p + o_k) for k = 1 .. n-1 in list order;  dst[p] = acc
+ * dst may be aux (each cell's aux value is read before that cell is written, by the same thread); dst must not be src.
+ * Reads stay inside the allocation; cells of dst outside the boxes are not written.  The result does not depend on the
+ * launch shape.
+ * ------------------------------------------------------------------------------------------- */
+#define SB_STENCIL_MAX_TERMS 64
+#define SB_STENCIL_MAX_REACH 4
+typedef struct sb_stencil_term {
+  int32_t source;    /* 0 = src, 1 = aux */
+  int32_t offset[3]; /* dx, dy, dz */
+  double weight;
+} sb_stencil_term;
+
+/* Host only.  Whether a subdomain with ghost widths radius27 can apply the op: every term with o != 0 needs
+ * radius27(sign(o)) > 0 (that ghost box is exchanged) and |o_a| <= the face radius on side sign(o_a) of every axis a with
+ * o_a != 0.  SB_ERR_INVALID, with a message naming the term, for a term that breaks either condition or a list outside
+ * the limits above (n, source, |o_a|, an aux term with an offset).  A wall face passes like any other face. */
+int sb_stencil_check(const sb_stencil_term *terms, int n, const int64_t radius27[27]);
+/* Host only.  The central-difference Laplacian of order 2, 4, 6 or 8 (radius 1 to 4) on a grid of spacing[3]: the centre
+ * term, then for k = 1..R the axes x, y, z, side - then side +.  In double with i_a = 1 / (h_a * h_a): an axis term is
+ * c_k * i_a, the centre (c_0 * i_x + c_0 * i_y) + c_0 * i_z, with c = (-2, 1), (-5/2, 4/3, -1/12),
+ * (-49/18, 3/2, -3/20, 1/90), (-205/72, 8/5, -1/5, 8/315, -1/560).  Writes at most cap terms (out may be NULL with cap 0)
+ * and returns their total number 1 + 6R, or SB_ERR_INVALID for another order or a spacing that is not finite and > 0. */
+int sb_stencil_laplacian(int order, const double spacing[3], sb_stencil_term *out, int cap);
+
+/* A persistent plan: the op over nbox boxes [lo, hi) (global coordinates, nbox*3 int64 each; acc_origin = global
+ * coordinate of allocation element (0,0,0), as for sb_jacobi3d) of three allocations of zsize planes that share pitch and
+ * ysize.  dtype SB_DTYPE_F32 or SB_DTYPE_F64; aux.ptr may be NULL when no term reads aux.  Boxes of at least 8 cells on
+ * every axis go to the z-marching tile kernel, one launch each; thinner boxes (exterior slabs) share one-thread-per-cell
+ * launches of up to 16 boxes.  Errors (SB_ERR_INVALID with a message, checked before anything is allocated): an unknown
+ * dtype, an invalid term list, an aux term without aux, dst == src, mismatched pitches or row counts, a pointer or pitch
+ * that is not a multiple of the element size, lo > hi, and a box whose reads leave the allocation.
+ * sb_stencil_plan_launch allocates nothing and never synchronises the host. */
+typedef struct sb_stencil_plan sb_stencil_plan;
+int sb_stencil_plan_create(sb_stencil_plan **out, int device, int dtype, const sb_stencil_term *terms, int n, sb_pitched dst,
+                           sb_pitched src, sb_pitched aux, const int64_t acc_origin[3], int64_t zsize, int nbox,
+                           const int64_t *lo, const int64_t *hi);
+int sb_stencil_plan_launch(sb_stencil_plan *plan, void *stream);
+/* algorithmic bytes per launch: per cell, one element read of src, one of aux if a term reads it, one written */
+int64_t sb_stencil_plan_bytes(const sb_stencil_plan *plan);
+int sb_stencil_plan_destroy(sb_stencil_plan *plan);
+
+/* ---------------------------------------------------------------------------------------------
  * 7-point jacobi step (the reference's user kernel, bin/jacobi3d.cu:40-85) over a region.
  * dtype_size 4 = float, 8 = double.  acc_origin = global coordinate of allocation element (0,0,0)
  * (Accessor origin, include/stencil/local_domain.cuh:153-173).  [lo,hi) = region to update,

@@ -76,6 +76,7 @@ DistributedDomain::~DistributedDomain() {
 
 void DistributedDomain::destroy_plans() {
   destroy_reduce_plans();
+  destroy_stencil_plans();
   for (auto *sides : {&plans_, &unpackPlans_}) {
     for (int parity = 0; parity < 2; ++parity) {
       for (sb_copy_plan *p : (*sides)[parity])
@@ -634,6 +635,96 @@ void DistributedDomain::destroy_reduce_plans() {
     }
   }
   reducePlans_.clear();
+}
+
+void DistributedDomain::destroy_stencil_plans() {
+  for (auto &kv : stencilPlans_)
+    for (auto &per_dom : kv.second)
+      for (sb_stencil_plan *p : per_dom) sb_stencil_plan_destroy(p);
+  stencilPlans_.clear();
+  for (size_t i = 0; i < applyStreams_.size(); ++i) {
+    cudaSetDevice(domains_[i / 2].gpu());
+    cudaStreamDestroy(applyStreams_[i]);
+  }
+  applyStreams_.clear();
+}
+
+void DistributedDomain::apply_op(const stencil::LinearStencil &op, int dtype, size_t dq, stencil::Which dw, size_t sq, int64_t aq,
+                                 stencil::Which aw, bool exchange) {
+  using stencil::Which;
+  if (domains_.empty() || plans_[0].size() != domains_.size()) LOG_FATAL("apply: call realize() first");
+  if (dtype != SB_DTYPE_F32 && dtype != SB_DTYPE_F64) LOG_FATAL("apply: a stencil operator computes in float or double");
+  for (const int64_t q : {int64_t(dq), int64_t(sq), aq})
+    if (q >= 0 && (size_t(q) >= dataDtype_.size() || dataDtype_[size_t(q)] != dtype)) LOG_FATAL("apply: unknown data handle " << q);
+  if (dq == sq && dw == Which::curr) LOG_FATAL("apply: dst must not be src");
+  if (op.has_aux() && aq < 0) LOG_FATAL("apply: the op has a term on aux, but no aux buffer was given");
+  int64_t r27[27];
+  for (int z = -1, i = 0; z <= 1; ++z)
+    for (int y = -1; y <= 1; ++y)
+      for (int x = -1; x <= 1; ++x) r27[i++] = int64_t(radius_.dir(x, y, z));
+  const std::vector<sb_stencil_term> &terms = op.terms();
+  if (SB_OK != sb_stencil_check(terms.data(), int(terms.size()), r27)) LOG_FATAL("apply: " << sb_last_error());
+  if (!op.has_aux()) aq = -1;
+  std::vector<int64_t> key = {dtype, int64_t(dq), int64_t(dw == Which::next), int64_t(sq), aq, int64_t(aw == Which::next), int64_t(exchange), parity_};
+  for (const sb_stencil_term &t : terms) {
+    int64_t wbits;
+    std::memcpy(&wbits, &t.weight, 8);
+    key.insert(key.end(), {t.source, t.offset[0], t.offset[1], t.offset[2], wbits});
+  }
+  auto found = stencilPlans_.find(key);
+  if (found == stencilPlans_.end()) {
+    const std::vector<Rect3> interiors = exchange ? get_interior() : std::vector<Rect3>();
+    const std::vector<std::vector<Rect3>> exteriors = exchange ? get_exterior() : std::vector<std::vector<Rect3>>();
+    std::vector<std::vector<sb_stencil_plan *>> per_dom;
+    for (size_t di = 0; di < domains_.size(); ++di) {
+      LocalDomain &d = domains_[di];
+      const sb_pitched dst = as_sb(dw == Which::curr ? d.curr_data(dq) : d.next_data(dq)), src = as_sb(d.curr_data(sq));
+      const sb_pitched aux = aq < 0 ? sb_pitched{nullptr, 0, 0} : as_sb(aw == Which::curr ? d.curr_data(size_t(aq)) : d.next_data(size_t(aq)));
+      int64_t acc[3];
+      set3(acc, d.origin() - Dim3(radius_.x(-1), radius_.y(-1), radius_.z(-1)));
+      auto make = [&](const std::vector<Rect3> &boxes) {
+        std::vector<int64_t> lo, hi;
+        for (const Rect3 &b : boxes) {
+          lo.insert(lo.end(), {b.lo.x, b.lo.y, b.lo.z});
+          hi.insert(hi.end(), {b.hi.x, b.hi.y, b.hi.z});
+        }
+        sb_stencil_plan *p = nullptr;
+        if (SB_OK != sb_stencil_plan_create(&p, d.gpu(), dtype, terms.data(), int(terms.size()), dst, src, aux, acc, d.raw_size().z,
+                                            int(boxes.size()), lo.data(), hi.data()))
+          LOG_FATAL("apply: " << sb_last_error());
+        return p;
+      };
+      if (exchange)
+        per_dom.push_back({make({interiors[di]}), make(exteriors[di])});
+      else
+        per_dom.push_back({make({d.get_compute_region()})});
+    }
+    found = stencilPlans_.emplace(key, std::move(per_dom)).first;
+  }
+  if (applyStreams_.empty()) {
+    // blocking streams: ordered after the work the caller queued on the legacy default stream
+    for (LocalDomain &d : domains_) {
+      d.set_device();
+      for (int k = 0; k < 2; ++k) {
+        cudaStream_t s;
+        CUDA_RUNTIME(cudaStreamCreate(&s));
+        applyStreams_.push_back(s);
+      }
+    }
+  }
+  const std::vector<std::vector<sb_stencil_plan *>> &plans = found->second;
+  for (size_t di = 0; di < domains_.size(); ++di)
+    if (SB_OK != sb_stencil_plan_launch(plans[di][0], applyStreams_[2 * di])) LOG_FATAL("apply: " << sb_last_error());
+  if (exchange) {
+    this->exchange(); // returns when every ghost cell of this rank is filled
+    for (size_t di = 0; di < domains_.size(); ++di)
+      if (SB_OK != sb_stencil_plan_launch(plans[di][1], applyStreams_[2 * di + 1])) LOG_FATAL("apply: " << sb_last_error());
+  }
+  for (size_t di = 0; di < domains_.size(); ++di) {
+    domains_[di].set_device();
+    CUDA_RUNTIME(cudaStreamSynchronize(applyStreams_[2 * di]));
+    CUDA_RUNTIME(cudaStreamSynchronize(applyStreams_[2 * di + 1]));
+  }
 }
 
 std::vector<stencil::Reduction> DistributedDomain::reduce_many(const std::vector<stencil::ReduceItem> &items) {

@@ -114,6 +114,15 @@ class ReduceResult(C.Structure):
 
 REDUCE_SCALAR, REDUCE_DIFF, REDUCE_NORM3 = 0, 1, 2  # sb_reduce_kind
 
+
+class StencilTerm(C.Structure):
+    """sb_stencil_term: one term of a linear stencil operator (source 0 = src, 1 = aux; offset; weight)."""
+
+    _fields_ = [("source", C.c_int32), ("offset", C.c_int32 * 3), ("weight", C.c_double)]
+
+
+STENCIL_MAX_TERMS, STENCIL_MAX_REACH = 64, 4  # SB_STENCIL_MAX_TERMS, SB_STENCIL_MAX_REACH
+
 I6 = C.c_int32 * 6
 
 FUSED_MAX_GROUPS = 4096  # SB_FUSED_MAX_GROUPS
@@ -161,6 +170,16 @@ _SIGS = {
     "sb_reduce_plan_bytes": (C.c_int64, [C.c_void_p]),
     "sb_reduce_plan_destroy": (C.c_int, [C.c_void_p]),
     "sb_reduce_combine": (C.c_int, [C.POINTER(ReduceResult), C.c_int64, C.POINTER(ReduceResult)]),
+    "sb_stencil_check": (C.c_int, [C.POINTER(StencilTerm), C.c_int, I27]),
+    "sb_stencil_laplacian": (C.c_int, [C.c_int, C.c_double * 3, C.POINTER(StencilTerm), C.c_int]),
+    "sb_stencil_plan_create": (
+        C.c_int,
+        [C.POINTER(C.c_void_p), C.c_int, C.c_int, C.POINTER(StencilTerm), C.c_int, Pitched, Pitched, Pitched, I3, C.c_int64, C.c_int,
+         C.POINTER(C.c_int64), C.POINTER(C.c_int64)],
+    ),
+    "sb_stencil_plan_launch": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "sb_stencil_plan_bytes": (C.c_int64, [C.c_void_p]),
+    "sb_stencil_plan_destroy": (C.c_int, [C.c_void_p]),
     "sb_signal": (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.c_uint32, C.c_int, C.c_void_p]),
     "sb_wait": (C.c_int, [C.c_void_p, C.c_int, C.c_uint32, C.c_int, C.c_void_p]),
     "sb_jacobi3d": (C.c_int, [Pitched, Pitched, C.c_int, I3, I3, I3, I3, I3, C.c_void_p]),

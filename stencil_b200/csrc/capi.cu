@@ -2,7 +2,10 @@
 // (include/stencil/*.hpp), copy plans over box_copy.cu, jacobi launches, device/peer/IPC plumbing.
 #include "stencil_b200.h"
 
+#include <algorithm>
+#include <array>
 #include <atomic>
+#include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
@@ -18,6 +21,7 @@
 #include "reduce.cuh"
 #include "astaroth.cuh"
 #include "jacobi.cuh"
+#include "stencil_op.cuh"
 
 #include "stencil/exchange_plan.hpp"
 #include "stencil/geometry.hpp"
@@ -546,6 +550,16 @@ struct sb_reduce_plan {
   unsigned nitems = 0, ntiles = 0;
   unsigned class_tiles[sb::kRedClasses][2] = {}; // tiles [begin, end) of each class
   int grids[sb::kRedClasses] = {};
+  int64_t bytes = 0;
+};
+
+struct sb_stencil_plan {
+  int device = 0;
+  int es = 8, R = 1;
+  std::vector<sb::OpTileParams> tiles; // one tile-kernel launch per thick box
+  std::vector<int> tile_grids;
+  std::vector<sb::OpCellParams> cells; // one cell-kernel launch per group of thin boxes
+  std::vector<int> cell_grids;
   int64_t bytes = 0;
 };
 
@@ -1307,6 +1321,239 @@ int sb_reduce_combine(const sb_reduce_result *parts, int64_t n, sb_reduce_result
   for (int64_t s = 1; s < n; s *= 2)
     for (int64_t i = 0; i + s < n; i += 2 * s) a[size_t(i)] = sb::red_merge(a[size_t(i)], a[size_t(i + s)]);
   *out = a[0];
+  return SB_OK;
+}
+
+// ----------------------------------------------------------------------------------------- linear stencil operators
+// The limits every term list obeys, whatever the domain: n, sources, |o_a| <= 4, aux terms without offset.
+static int stencil_terms_ok(const sb_stencil_term *terms, int n) {
+  if (!terms || n < 1 || n > SB_STENCIL_MAX_TERMS) return fail(SB_ERR_INVALID, "an op has 1 to %d terms, not %d", SB_STENCIL_MAX_TERMS, terms ? n : 0);
+  for (int t = 0; t < n; ++t) {
+    const sb_stencil_term &T = terms[t];
+    if (T.source != 0 && T.source != 1) return fail(SB_ERR_INVALID, "term %d: source %d must be 0 (src) or 1 (aux)", t, int(T.source));
+    for (int a = 0; a < 3; ++a)
+      if (T.offset[a] < -SB_STENCIL_MAX_REACH || T.offset[a] > SB_STENCIL_MAX_REACH)
+        return fail(SB_ERR_INVALID, "term %d: offset (%d, %d, %d) reaches beyond %d cells", t, int(T.offset[0]), int(T.offset[1]),
+                    int(T.offset[2]), SB_STENCIL_MAX_REACH);
+    if (T.source == 1 && (T.offset[0] || T.offset[1] || T.offset[2]))
+      return fail(SB_ERR_INVALID, "term %d: an aux term has offset (0, 0, 0), not (%d, %d, %d)", t, int(T.offset[0]), int(T.offset[1]),
+                  int(T.offset[2]));
+  }
+  return SB_OK;
+}
+
+int sb_stencil_check(const sb_stencil_term *terms, int n, const int64_t radius27[27]) {
+  if (!radius27) return fail(SB_ERR_INVALID, "sb_stencil_check needs radius27");
+  int rc = stencil_terms_ok(terms, n);
+  if (rc != SB_OK) return rc;
+  for (int t = 0; t < n; ++t) {
+    const int32_t *o = terms[t].offset;
+    if (!o[0] && !o[1] && !o[2]) continue;
+    int s[3];
+    for (int a = 0; a < 3; ++a) s[a] = (o[a] > 0) - (o[a] < 0);
+    if (radius27[(s[2] + 1) * 9 + (s[1] + 1) * 3 + (s[0] + 1)] <= 0)
+      return fail(SB_ERR_INVALID, "term %d: offset (%d, %d, %d) reads the ghost box in direction (%d, %d, %d), whose radius is 0", t,
+                  int(o[0]), int(o[1]), int(o[2]), s[0], s[1], s[2]);
+    for (int a = 0; a < 3; ++a) {
+      if (!o[a]) continue;
+      int d[3] = {0, 0, 0};
+      d[a] = s[a];
+      const int64_t face = radius27[(d[2] + 1) * 9 + (d[1] + 1) * 3 + (d[0] + 1)];
+      if (int64_t(o[a] < 0 ? -o[a] : o[a]) > face)
+        return fail(SB_ERR_INVALID, "term %d: offset (%d, %d, %d) reaches %d cells on side %c%c, whose face radius is %lld", t,
+                    int(o[0]), int(o[1]), int(o[2]), int(o[a] < 0 ? -o[a] : o[a]), s[a] < 0 ? '-' : '+', "xyz"[a], (long long)face);
+    }
+  }
+  return SB_OK;
+}
+
+int sb_stencil_laplacian(int order, const double spacing[3], sb_stencil_term *out, int cap) {
+  // c_0 .. c_R of the central second difference, as exact quotients rounded once to double
+  static const double c2[] = {-2.0, 1.0};
+  static const double c4[] = {-5.0 / 2.0, 4.0 / 3.0, -1.0 / 12.0};
+  static const double c6[] = {-49.0 / 18.0, 3.0 / 2.0, -3.0 / 20.0, 1.0 / 90.0};
+  static const double c8[] = {-205.0 / 72.0, 8.0 / 5.0, -1.0 / 5.0, 8.0 / 315.0, -1.0 / 560.0};
+  const double *c = order == 2 ? c2 : order == 4 ? c4 : order == 6 ? c6 : order == 8 ? c8 : nullptr;
+  if (!c) return fail(SB_ERR_INVALID, "Laplacian order %d: 2, 4, 6 or 8", order);
+  if (!spacing) return fail(SB_ERR_INVALID, "sb_stencil_laplacian needs spacing[3]");
+  for (int a = 0; a < 3; ++a)
+    if (!(spacing[a] > 0.0) || !std::isfinite(spacing[a])) return fail(SB_ERR_INVALID, "spacing[%d] = %g must be finite and > 0", a, spacing[a]);
+  if (cap < 0 || (cap > 0 && !out)) return fail(SB_ERR_INVALID, "sb_stencil_laplacian: bad output buffer");
+  const int R = order / 2, total = 1 + 6 * R;
+  double inv[3];
+  for (int a = 0; a < 3; ++a) {
+    const double h2 = spacing[a] * spacing[a];
+    inv[a] = 1.0 / h2;
+  }
+  std::vector<sb_stencil_term> terms;
+  const double cx = c[0] * inv[0], cy = c[0] * inv[1], cz = c[0] * inv[2];
+  const double cxy = cx + cy;
+  terms.push_back(sb_stencil_term{0, {0, 0, 0}, cxy + cz});
+  for (int k = 1; k <= R; ++k)
+    for (int a = 0; a < 3; ++a)
+      for (int side = -1; side <= 1; side += 2) {
+        sb_stencil_term t{0, {0, 0, 0}, c[k] * inv[a]};
+        t.offset[a] = side * k;
+        terms.push_back(t);
+      }
+  for (int i = 0; i < total && i < cap; ++i) out[i] = terms[size_t(i)];
+  return total;
+}
+
+int sb_stencil_plan_create(sb_stencil_plan **out, int device, int dtype, const sb_stencil_term *terms, int n, sb_pitched dst,
+                           sb_pitched src, sb_pitched aux, const int64_t acc_origin[3], int64_t zsize, int nbox, const int64_t *lo,
+                           const int64_t *hi) {
+  if (!out) return fail(SB_ERR_INVALID, "sb_stencil_plan_create needs an output handle");
+  if (dtype != SB_DTYPE_F32 && dtype != SB_DTYPE_F64) return fail(SB_ERR_INVALID, "dtype %d must be SB_DTYPE_F32 or SB_DTYPE_F64", dtype);
+  const int es = dtype == SB_DTYPE_F32 ? 4 : 8;
+  int rc = stencil_terms_ok(terms, n);
+  if (rc != SB_OK) return rc;
+  bool has_aux = false;
+  int rm[3] = {0, 0, 0}, rp[3] = {0, 0, 0}, R = 1;
+  for (int t = 0; t < n; ++t) {
+    has_aux = has_aux || terms[t].source == 1;
+    for (int a = 0; a < 3; ++a) {
+      const int o = terms[t].offset[a];
+      rm[a] = std::max(rm[a], -o);
+      rp[a] = std::max(rp[a], o);
+      R = std::max(R, std::abs(o));
+    }
+  }
+  if (has_aux && !aux.ptr) return fail(SB_ERR_INVALID, "the op has a term on aux, but aux is NULL");
+  if (!dst.ptr || !src.ptr) return fail(SB_ERR_INVALID, "dst and src must not be NULL");
+  if (dst.ptr == src.ptr) return fail(SB_ERR_INVALID, "dst must not be src (dst may be aux)");
+  const sb_pitched *bufs[3] = {&dst, &src, &aux};
+  const char *names[3] = {"dst", "src", "aux"};
+  for (int b = 0; b < (has_aux ? 3 : 2); ++b) {
+    const sb_pitched &P = *bufs[b];
+    if (P.pitch != src.pitch || P.ysize != src.ysize) return fail(SB_ERR_INVALID, "%s has another pitch or row count than src", names[b]);
+    if ((uintptr_t(P.ptr) % uintptr_t(es)) || P.pitch <= 0 || (P.pitch % es) || P.ysize <= 0)
+      return fail(SB_ERR_INVALID, "%s: pointer and pitch must be positive multiples of the %d-byte element", names[b], es);
+  }
+  if (!acc_origin || zsize < 1) return fail(SB_ERR_INVALID, "sb_stencil_plan_create needs acc_origin and zsize >= 1");
+  if (nbox < 0 || (nbox > 0 && (!lo || !hi))) return fail(SB_ERR_INVALID, "nbox %d: needs nbox >= 0 and lo / hi arrays", nbox);
+  const int64_t size[3] = {src.pitch / es, src.ysize, zsize};
+  std::vector<std::array<int, 6>> thick, thin; // allocation-relative lo, ext
+  int64_t cells = 0;
+  for (int b = 0; b < nbox; ++b) {
+    int64_t l[3], e[3];
+    bool empty = false;
+    for (int a = 0; a < 3; ++a) {
+      if (lo[3 * b + a] > hi[3 * b + a]) return fail(SB_ERR_INVALID, "box %d: lo > hi on axis %d", b, a);
+      l[a] = lo[3 * b + a] - acc_origin[a];
+      e[a] = hi[3 * b + a] - lo[3 * b + a];
+      empty = empty || e[a] == 0;
+    }
+    if (empty) continue;
+    for (int a = 0; a < 3; ++a)
+      if (l[a] - rm[a] < 0 || l[a] + e[a] + rp[a] > size[a])
+        return fail(SB_ERR_INVALID, "box %d: the op reads cells %lld .. %lld on axis %c, outside the allocation's 0 .. %lld", b,
+                    (long long)(l[a] - rm[a]), (long long)(l[a] + e[a] + rp[a] - 1), "xyz"[a], (long long)(size[a] - 1));
+    if (e[0] * e[1] * e[2] >= (1ll << 32)) return fail(SB_ERR_INVALID, "box %d: more than 2^32 cells", b);
+    const std::array<int, 6> bx = {int(l[0]), int(l[1]), int(l[2]), int(e[0]), int(e[1]), int(e[2])};
+    (e[0] >= 8 && e[1] >= 8 && e[2] >= 8 ? thick : thin).push_back(bx);
+    cells += e[0] * e[1] * e[2];
+  }
+
+  sb::OpCommon com{};
+  com.dst = static_cast<char *>(dst.ptr);
+  com.src = static_cast<const char *>(src.ptr);
+  com.aux = has_aux ? static_cast<const char *>(aux.ptr) : nullptr;
+  com.pitch = src.pitch;
+  com.slice = src.pitch * src.ysize;
+  com.n = n;
+  com.has_aux = has_aux ? 1 : 0;
+  for (int t = 0; t < n; ++t) {
+    com.source[t] = (signed char)terms[t].source;
+    com.w[t] = terms[t].weight;
+    com.wf[t] = float(terms[t].weight); // round to nearest
+  }
+
+  DeviceGuard guard(device);
+  if (!guard.ok) return fail(SB_ERR_NOGPU, "cannot select CUDA device %d", device);
+  int sms = 0;
+  SB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
+  sb_stencil_plan *p = new sb_stencil_plan();
+  p->device = device;
+  p->es = es;
+  p->R = R;
+  p->bytes = cells * es * (has_aux ? 3 : 2);
+  if (!thick.empty()) {
+    const int per_sm = sb::op_tile_prepare(R, es, device);
+    if (per_sm <= 0) {
+      delete p;
+      return fail(SB_ERR_CUDA, "the R = %d tile kernel cannot be configured: %s", R, cudaGetErrorString(cudaGetLastError()));
+    }
+    const int SW = sb::op_tile_sw(R), P = sb::op_tile_plane(R), NS = 2 * R + 1;
+    for (const auto &b : thick) {
+      sb::OpTileParams tp{};
+      tp.c = com;
+      tp.src_end = com.src + com.slice * zsize;
+      for (int a = 0; a < 3; ++a) {
+        tp.lo[a] = b[a];
+        tp.ext[a] = b[3 + a];
+        tp.rm[a] = rm[a];
+        tp.rp[a] = rp[a];
+      }
+      tp.tiles_x = (tp.ext[0] + sb::kOpTileX - 1) / sb::kOpTileX;
+      tp.tiles_y = (tp.ext[1] + sb::kOpTileY - 1) / sb::kOpTileY;
+      // z chunks: at least two waves of resident CTAs, chunks no shorter than 16 planes (each chunk reloads rm + rp planes)
+      const long long cols = (long long)tp.tiles_x * tp.tiles_y;
+      const long long want = (2ll * sms * per_sm + cols - 1) / cols;
+      int zc = int((tp.ext[2] + want - 1) / want);
+      zc = std::max(zc, std::min(16, tp.ext[2]));
+      tp.zchunk = zc;
+      const long long grid = cols * ((tp.ext[2] + zc - 1) / zc);
+      if (grid >= (1ll << 31)) {
+        delete p;
+        return fail(SB_ERR_INVALID, "box too large for the tile kernel");
+      }
+      for (int c = 0; c < NS; ++c)
+        for (int t = 0; t < n; ++t) {
+          const int32_t *o = terms[t].offset;
+          tp.toff[c][t] = ((c + o[2] + NS) % NS) * P + o[1] * SW + o[0];
+        }
+      p->tiles.push_back(tp);
+      p->tile_grids.push_back(int(grid));
+    }
+  }
+  for (size_t b0 = 0; b0 < thin.size(); b0 += sb::kOpMaxBoxes) {
+    sb::OpCellParams cp{};
+    cp.c = com;
+    for (int t = 0; t < n; ++t)
+      cp.goff[t] = (long long)terms[t].offset[2] * com.slice + (long long)terms[t].offset[1] * com.pitch + (long long)terms[t].offset[0] * es;
+    cp.first[0] = 0;
+    for (size_t b = b0; b < thin.size() && b < b0 + sb::kOpMaxBoxes; ++b) {
+      const int m = cp.n++;
+      for (int a = 0; a < 3; ++a) {
+        cp.lo[m][a] = thin[b][a];
+        cp.ext[m][a] = thin[b][3 + a];
+      }
+      cp.first[m + 1] = cp.first[m] + (long long)thin[b][3] * thin[b][4] * thin[b][5];
+    }
+    const long long total = cp.first[cp.n];
+    p->cells.push_back(cp);
+    p->cell_grids.push_back(int(std::min<long long>((total + 255) / 256, 32ll * sms)));
+  }
+  *out = p;
+  return SB_OK;
+}
+
+int sb_stencil_plan_launch(sb_stencil_plan *p, void *stream) {
+  if (!p) return fail(SB_ERR_INVALID, "null plan");
+  DeviceGuard guard(p->device);
+  if (!guard.ok) return fail(SB_ERR_NOGPU, "cannot select CUDA device %d", p->device);
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  for (size_t i = 0; i < p->tiles.size(); ++i) g_launches += uint64_t(sb::launch_op_tile(p->tiles[i], p->R, p->es, p->tile_grids[i], s));
+  for (size_t i = 0; i < p->cells.size(); ++i) g_launches += uint64_t(sb::launch_op_cells(p->cells[i], p->es, p->cell_grids[i], s));
+  SB_CUDA(cudaGetLastError());
+  return SB_OK;
+}
+
+int64_t sb_stencil_plan_bytes(const sb_stencil_plan *p) { return p ? p->bytes : 0; }
+
+int sb_stencil_plan_destroy(sb_stencil_plan *p) {
+  delete p;
   return SB_OK;
 }
 

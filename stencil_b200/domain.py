@@ -633,6 +633,8 @@ class DistributedDomain:
         self.topology_: Optional[Topology] = None
         self._bc_plans: List[List[Optional[BCPlan]]] = []  # [parity][local domain]
         self._reduce_plans: Dict[tuple, List[ReducePlan]] = {}  # (item keys, parity) -> one plan per local domain
+        self._stencil_plans: Dict[tuple, list] = {}  # (op, buffers, exchange, parity) -> per local domain: plans
+        self._apply_streams: list = []  # per local domain: (interior stream, exterior stream)
 
     # -- configuration (call before realize)
     def set_radius(self, r) -> None:
@@ -1142,7 +1144,89 @@ class DistributedDomain:
         lo, hi = d.get_compute_region()
         return _lib.ReduceItem(kind, bc_dtype(self.dtypes_[qs[0]]), (Pitched * 3)(*srcs), i3(d.accessor_origin()), i3(lo), i3(hi))
 
+    # -- linear stencil operators
+    def apply(self, op, dst, src, aux=None, exchange: bool = True) -> None:
+        """dst = op(src, aux) over the whole compute region of every local subdomain (DESIGN.md section 2.7).
+
+        Buffers are (DataHandle, "curr" | "next"); a bare handle means "next" for dst and "curr" for src and aux.  src is
+        always a curr buffer (the one exchange() fills); dst may be aux, never src; all share op's element type.
+        exchange=True: the interior runs on its own stream while exchange() fills the ghost cells, then the exterior slabs
+        of each subdomain run as one launch; exchange=False: one launch over the whole region, and the caller guarantees
+        the ghost cells are current.  Returns when the update is complete.  The plans are built on first use and kept,
+        per (op, buffers, exchange, swap parity), until close().  Under torchrun every rank calls it (exchange() is
+        collective)."""
+        import torch
+
+        from .stencil_op import StencilOp, StencilPlan
+
+        if not isinstance(op, StencilOp):
+            raise _lib.StencilError(f"{op!r} is not a StencilOp")
+        if self.partition_ is None or not self._plans:
+            raise _lib.StencilError("apply: call realize() first")
+
+        def buf(arg, default, role):
+            h, which = (arg, default) if isinstance(arg, DataHandle) else tuple(arg)
+            if not isinstance(h, DataHandle) or which not in ("curr", "next"):
+                raise _lib.StencilError(f"apply: {role} must be a DataHandle or (DataHandle, 'curr' | 'next'), not {arg!r}")
+            if self.dtypes_[h.id] != op.dtype:
+                raise _lib.StencilError(f"apply: {role} is {self.dtypes_[h.id]}, the op computes in {op.dtype}")
+            return h.id, which
+
+        d_q, d_w = buf(dst, "next", "dst")
+        s_q, s_w = buf(src, "curr", "src")
+        if s_w != "curr":
+            raise _lib.StencilError("apply: src must be a curr buffer (the one exchange() fills)")
+        if (d_q, d_w) == (s_q, s_w):
+            raise _lib.StencilError("apply: dst must not be src")
+        a = buf(aux, "curr", "aux") if aux is not None else None
+        if op.has_aux and a is None:
+            raise _lib.StencilError("apply: the op has a term on aux, but no aux buffer was given")
+        op.check(self.radius_)
+        key = (op.key(), (d_q, d_w), s_q, a if op.has_aux else None, bool(exchange), self._parity)
+        plans = self._stencil_plans.get(key)
+        if plans is None:
+            plans = []
+            interiors, exteriors = (self.get_interior(), self.get_exterior()) if exchange else (None, None)
+            for di, d in enumerate(self.domains_):
+                P = (d.pitched(d_q, d_w), d.pitched(s_q, "curr"), d.pitched(a[0], a[1]) if a is not None and op.has_aux else Pitched(None, 0, 0))
+                mk = lambda boxes: StencilPlan(d.gpu(), op, *P, d.accessor_origin(), d.raw_size()[2], boxes)  # noqa: E731
+                if exchange:
+                    plans.append((mk([interiors[di]]), mk(exteriors[di])))
+                else:
+                    plans.append((mk([d.get_compute_region()]),))
+            self._stencil_plans[key] = plans
+        if not self._apply_streams:
+            self._apply_streams = [(torch.cuda.Stream(device=d.gpu()), torch.cuda.Stream(device=d.gpu())) for d in self.domains_]
+        for d, (si, se) in zip(self.domains_, self._apply_streams):  # after the work queued on the caller's stream
+            si.wait_stream(torch.cuda.current_stream(d.gpu()))
+            se.wait_stream(torch.cuda.current_stream(d.gpu()))
+        multi = len({d.gpu() for d in self.domains_}) > 1
+        if exchange:
+            for d, p, (si, _) in zip(self.domains_, plans, self._apply_streams):
+                if multi:
+                    _set_current_device(d.gpu())
+                p[0].launch(si)
+            self.exchange()  # returns when every ghost cell of every local subdomain is filled
+            for d, p, (_, se) in zip(self.domains_, plans, self._apply_streams):
+                if multi:
+                    _set_current_device(d.gpu())
+                p[1].launch(se)
+        else:
+            for d, p, (si, _) in zip(self.domains_, plans, self._apply_streams):
+                if multi:
+                    _set_current_device(d.gpu())
+                p[0].launch(si)
+        for si, se in self._apply_streams:
+            si.synchronize()
+            se.synchronize()
+
     def close(self) -> None:
+        for plans in self._stencil_plans.values():
+            for per_dom in plans:
+                for p in per_dom:
+                    p.destroy()
+        self._stencil_plans = {}
+        self._apply_streams = []
         for plans in self._reduce_plans.values():
             for p in plans:
                 p.destroy()
