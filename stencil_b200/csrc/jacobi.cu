@@ -1111,8 +1111,8 @@ int launch_jacobi_fused(const JacobiParams &p_in, const FusedSync &sync_in, int 
   const int ex = p.hi[0] - p.lo[0], ey = p.hi[1] - p.lo[1], ez = p.hi[2] - p.lo[2];
   if (ex <= 0 || ey <= 0 || ez <= 0) return 0;
   const int zchunk_env = env_int("SB_JACOBI_ZCHUNK", 0);
-  // H100 80GB HBM3 (400 W), 512^3 FP64, one GPU: 16-plane chunks with a 1-plane L2 prefetch take 0.80 ms per iteration,
-  // 32 planes with a 2-plane prefetch 0.88 ms (alternating runs, DESIGN.md section 2.2)
+  // H100 80GB HBM3 (400 W), 512^3 FP64, one GPU, 1-plane L2 prefetch: 8-plane chunks take 0.78 ms per iteration, 16-plane
+  // chunks 0.80 ms, 32 planes with a 2-plane prefetch 0.88 ms; deeper prefetch is slower (DESIGN.md section 2.2)
   const int pf = env_int("SB_JACOBI_PREFETCH", 1);
   const int allow_shift = env_int("SB_JACOBI_SHIFT", 1);
   p.prefetch = pf;
@@ -1125,14 +1125,15 @@ int launch_jacobi_fused(const JacobiParams &p_in, const FusedSync &sync_in, int 
   sync.debug = dbg;
   bool shift = false;
   const int vx = pick_vectors(p, dtype_size, allow_shift != 0, &shift);
-  // z chunk (the x faces are staged at most 32 planes at a time): 16 planes by default, 32 where 16-plane chunks would give
-  // a face more tiles than launch_fused's group limit (subdomains taller than ~720 cells in z)
+  // z chunk (the x faces are staged at most 32 planes at a time): 8 planes by default, 16 or 32 where shorter chunks would
+  // give a face more tiles than launch_fused's group limit (8: subdomains up to 512 cells in z at 512 cells in y; 16: up to
+  // ~720 cells in y and z)
   if (zchunk_env > 0 && zchunk_env <= 32) {
     p.zchunk = zchunk_env;
   } else {
     const long long tiles_x = (p.hi[0] - p.x0a + (shift ? vx / 2 : 0) + 32 * vx - 1) / (32 * vx), tiles_y = (ey + 7) / 8;
     const long long across = tiles_x > tiles_y ? tiles_x : tiles_y;
-    p.zchunk = ((ez + 15) / 16) * across <= kMaxGroups ? 16 : 32;
+    p.zchunk = ((ez + 7) / 8) * across <= kMaxGroups ? 8 : (((ez + 15) / 16) * across <= kMaxGroups ? 16 : 32);
   }
   if (p.zchunk > ez) p.zchunk = ez;
   // x wrap (periodic self-neighbour read in place) works through the edge lanes' scalar load, so the first compute cell

@@ -45,8 +45,8 @@ struct JacobiParams {
 };
 
 // Mailbox rows of the fused kernel (see jacobi_fused_kernel): one word per boundary tile of a face -- (z chunks x tile rows)
-// for x faces, (z chunks x strips) for y faces, (tile rows x strips) for z faces; 32 x 64 = 2048 at 512^3 FP64 with the
-// default 16-plane chunks (launch_jacobi_fused falls back to 32-plane chunks where 16 would exceed the limit)
+// for x faces, (z chunks x strips) for y faces, (tile rows x strips) for z faces; 64 x 64 = 4096 at 512^3 FP64 with the
+// default 8-plane chunks (launch_jacobi_fused falls back to 16- and 32-plane chunks where shorter ones would exceed the limit)
 #ifndef SB_FUSED_MAX_GROUPS
 #define SB_FUSED_MAX_GROUPS 4096
 #endif
