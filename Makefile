@@ -34,7 +34,7 @@ LIBA      := lib/libstencil.a
 LIBMPI    := lib/libmpi_shim.a
 
 all: $(SO) $(LIBA) $(LIBMPI) bin/sb_mpirun bin/jacobi3d_b200 bin/test_exchange_multigpu bin/test_boundary_multigpu \
-          bin/test_reduce_multigpu bin/test_stencil_multigpu
+          bin/test_reduce_multigpu bin/test_stencil_multigpu bin/test_vstencil_multigpu
 
 build/mpi_shim.o: src/mpi_shim.cpp include/mpi_shim/mpi.h
 	@mkdir -p build
@@ -142,6 +142,12 @@ build/drv/test_stencil_multigpu.o: tests/cpp/test_stencil_multigpu.cu $(wildcard
 	@mkdir -p $(dir $@)
 	$(NVCC) $(OWNDRVFLAGS) -c $< -o $@
 bin/test_stencil_multigpu: build/drv/test_stencil_multigpu.o $(LIBA) $(LIBMPI)
+	@mkdir -p bin
+	$(NVCC) $(DRVLINK) -o $@ $< $(LIBA) $(LIBMPI)
+build/drv/test_vstencil_multigpu.o: tests/cpp/test_vstencil_multigpu.cu $(wildcard include/stencil/*) include/stencil_b200.h
+	@mkdir -p $(dir $@)
+	$(NVCC) $(OWNDRVFLAGS) -c $< -o $@
+bin/test_vstencil_multigpu: build/drv/test_vstencil_multigpu.o $(LIBA) $(LIBMPI)
 	@mkdir -p bin
 	$(NVCC) $(DRVLINK) -o $@ $< $(LIBA) $(LIBMPI)
 

@@ -1,11 +1,15 @@
 #pragma once
-// Constant-coefficient linear stencil operators on a DistributedDomain (DESIGN.md section 2.7; the rule, the reach check
-// and the Laplacian table are the C ABI's sb_stencil_* of include/stencil_b200.h).
+// Linear stencil operators on a DistributedDomain, constant and variable coefficients (DESIGN.md section 2.7; the rule,
+// the reach check and the Laplacian and div-grad tables are the C ABI's sb_stencil_* of include/stencil_b200.h).
 //
 //     stencil::LinearStencil lap = stencil::LinearStencil::laplacian(4, hx, hy, hz);
 //     stencil::LinearStencil heat = lap.scaled(dt).add(stencil::Source::src, 0, 0, 0, 1.0);   // u + dt lap(u)
 //     dd.apply(heat, stencil::next(h), h);                                                        // overlapped with exchange()
 //     dd.swap();
+//
+//     // u + dt div(kappa grad u), kappa on the x / y / z faces in three quantities (their curr buffers)
+//     stencil::LinearStencil kheat = stencil::LinearStencil::div_grad(hx, hy, hz).scaled(dt).add(stencil::Source::src, 0, 0, 0, 1.0);
+//     dd.apply(kheat, stencil::next(h), h, {kx, ky, kz});
 #include <cstdint>
 #include <vector>
 
@@ -18,23 +22,49 @@ namespace stencil {
 
 enum class Source { src = 0, aux = 1 };
 
-// An operator: terms (source, offset, weight) applied in list order.  Terms on aux have offset 0.
+// An operator: terms (source, offset, weight) applied in list order, each of which may also read a coefficient field k at
+// an offset of reach 1 (then it contributes (T(w) * C_k) * S).  Terms on aux have offset 0.
 class LinearStencil {
-  std::vector<sb_stencil_term> terms_;
+  std::vector<sb_stencil_term> terms_;   // every term without its coefficient
+  std::vector<sb_stencil_vterm> vterms_; // every term with its coefficient (coef = -1: none)
 
 public:
   LinearStencil() = default;
-  explicit LinearStencil(std::vector<sb_stencil_term> terms) : terms_(std::move(terms)) {}
+  explicit LinearStencil(std::vector<sb_stencil_term> terms) : terms_(std::move(terms)) {
+    for (const sb_stencil_term &t : terms_)
+      vterms_.push_back(sb_stencil_vterm{t.source, {t.offset[0], t.offset[1], t.offset[2]}, -1, {0, 0, 0}, t.weight});
+  }
+  explicit LinearStencil(const std::vector<sb_stencil_vterm> &vterms) {
+    for (const sb_stencil_vterm &t : vterms) add(Source(t.source), t.offset[0], t.offset[1], t.offset[2], t.weight, t.coef, t.coef_offset[0], t.coef_offset[1], t.coef_offset[2]);
+  }
 
   LinearStencil &add(Source s, int dx, int dy, int dz, double w) {
     terms_.push_back(sb_stencil_term{int32_t(s), {dx, dy, dz}, w});
+    vterms_.push_back(sb_stencil_vterm{int32_t(s), {dx, dy, dz}, -1, {0, 0, 0}, w});
+    return *this;
+  }
+  // a coefficient term: also reads coefficient field coef (-1: none) at (cx, cy, cz)
+  LinearStencil &add(Source s, int dx, int dy, int dz, double w, int coef, int cx, int cy, int cz) {
+    terms_.push_back(sb_stencil_term{int32_t(s), {dx, dy, dz}, w});
+    vterms_.push_back(sb_stencil_vterm{int32_t(s), {dx, dy, dz}, coef, {cx, cy, cz}, w});
     return *this;
   }
   // every weight multiplied by f (in double)
   LinearStencil scaled(double f) const {
     LinearStencil out(*this);
     for (sb_stencil_term &t : out.terms_) t.weight *= f;
+    for (sb_stencil_vterm &t : out.vterms_) t.weight *= f;
     return out;
+  }
+  // the conservative second-order div(kappa grad u) on a grid of spacing (hx, hy, hz): sb_stencil_div_grad.  Coefficient
+  // field a holds kappa on the faces normal to axis a (C_a(p) on the face between p - e_a and p).
+  static LinearStencil div_grad(double hx, double hy, double hz) {
+    const double h[3] = {hx, hy, hz};
+    const int n = sb_stencil_div_grad(h, nullptr, 0);
+    if (n < 0) LOG_FATAL("LinearStencil::div_grad: " << sb_last_error());
+    std::vector<sb_stencil_vterm> terms(static_cast<size_t>(n));
+    sb_stencil_div_grad(h, terms.data(), n);
+    return LinearStencil(terms);
   }
   // the central-difference Laplacian of order 2, 4, 6 or 8 on a grid of spacing (hx, hy, hz): sb_stencil_laplacian
   static LinearStencil laplacian(int order, double hx, double hy, double hz) {
@@ -47,10 +77,17 @@ public:
   }
 
   const std::vector<sb_stencil_term> &terms() const noexcept { return terms_; }
+  const std::vector<sb_stencil_vterm> &vterms() const noexcept { return vterms_; }
   bool has_aux() const noexcept {
     for (const sb_stencil_term &t : terms_)
       if (t.source == 1) return true;
     return false;
+  }
+  // the number of coefficient fields DistributedDomain::apply takes: the highest field a term names, plus one
+  int ncoef() const noexcept {
+    int n = 0;
+    for (const sb_stencil_vterm &t : vterms_) n = t.coef + 1 > n ? t.coef + 1 : n;
+    return n;
   }
 };
 

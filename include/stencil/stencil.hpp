@@ -131,7 +131,7 @@ private:
   std::vector<cudaStream_t> applyStreams_;
   void destroy_stencil_plans();
   void apply_op(const stencil::LinearStencil &op, int dtype, size_t dq, stencil::Which dw, size_t sq, int64_t aq, stencil::Which aw,
-                bool exchange);
+                const std::vector<size_t> &cq, bool exchange);
 
   std::string outputPrefix_;
 
@@ -267,12 +267,31 @@ public:
   // parity), until the domain is destroyed.
   template <typename T>
   void apply(const stencil::LinearStencil &op, const stencil::Buffer<T> &dst, const DataHandle<T> &src, bool exchange = true) {
-    apply_op(op, stencil::bc_dtype<T>(), dst.h.id(), dst.which, src.id(), -1, stencil::Which::curr, exchange);
+    apply_op(op, stencil::bc_dtype<T>(), dst.h.id(), dst.which, src.id(), -1, stencil::Which::curr, {}, exchange);
   }
   template <typename T>
   void apply(const stencil::LinearStencil &op, const stencil::Buffer<T> &dst, const DataHandle<T> &src, const stencil::Buffer<T> &aux,
              bool exchange = true) {
-    apply_op(op, stencil::bc_dtype<T>(), dst.h.id(), dst.which, src.id(), int64_t(aux.h.id()), aux.which, exchange);
+    apply_op(op, stencil::bc_dtype<T>(), dst.h.id(), dst.which, src.id(), int64_t(aux.h.id()), aux.which, {}, exchange);
+  }
+  // The same with coefficient fields: coefs[k] is field k of the op (op.ncoef() of them), read from its curr buffer, which
+  // exchange() fills like src's (with the quantity's own BC on a wall); a coefficient may alias src or aux, never dst.
+  // swap() turns every quantity's buffers, coefficients included: a static coefficient holds the same compute cells in
+  // curr and next.
+  template <typename T>
+  void apply(const stencil::LinearStencil &op, const stencil::Buffer<T> &dst, const DataHandle<T> &src, const std::vector<DataHandle<T>> &coefs,
+             bool exchange = true) {
+    apply_op(op, stencil::bc_dtype<T>(), dst.h.id(), dst.which, src.id(), -1, stencil::Which::curr, ids_of(coefs), exchange);
+  }
+  template <typename T>
+  void apply(const stencil::LinearStencil &op, const stencil::Buffer<T> &dst, const DataHandle<T> &src, const stencil::Buffer<T> &aux,
+             const std::vector<DataHandle<T>> &coefs, bool exchange = true) {
+    apply_op(op, stencil::bc_dtype<T>(), dst.h.id(), dst.which, src.id(), int64_t(aux.h.id()), aux.which, ids_of(coefs), exchange);
+  }
+  template <typename T> static std::vector<size_t> ids_of(const std::vector<DataHandle<T>> &hs) {
+    std::vector<size_t> ids;
+    for (const DataHandle<T> &h : hs) ids.push_back(h.id());
+    return ids;
   }
 
   // one CSV file per subdomain: Z,Y,X,<quantities...>

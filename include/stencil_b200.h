@@ -311,9 +311,49 @@ int sb_stencil_plan_create(sb_stencil_plan **out, int device, int dtype, const s
                            sb_pitched src, sb_pitched aux, const int64_t acc_origin[3], int64_t zsize, int nbox,
                            const int64_t *lo, const int64_t *hi);
 int sb_stencil_plan_launch(sb_stencil_plan *plan, void *stream);
-/* algorithmic bytes per launch: per cell, one element read of src, one of aux if a term reads it, one written */
+/* algorithmic bytes per launch: per cell, one element read of src, one of aux if a term reads it, one of each coefficient
+ * field the op references (sb_stencil_vplan_create), one written */
 int64_t sb_stencil_plan_bytes(const sb_stencil_plan *plan);
 int sb_stencil_plan_destroy(sb_stencil_plan *plan);
+
+/* ---------------------------------------------------------------------------------------------
+ * Variable-coefficient linear stencil operators: the rule above, where a term may also name a coefficient field k
+ * (0 <= k < SB_STENCIL_MAX_COEFS) read at p + c, |c_a| <= SB_STENCIL_COEF_REACH.  Per cell, in T, no FMA contraction:
+ *   coefficient term  m_t = (T(w_t) * C_k(p + c_t)) * S_t(p + o_t)      (two multiplies, each rounded)
+ *   plain term        m_t = T(w_t) * S_t(p + o_t)
+ *   acc = m_0;  acc = acc + m_t for t = 1 .. n-1 in list order;  dst[p] = acc
+ * With every C = 1 the result is the plain op's, bit for bit (T(w) * 1 is exact).  Coefficient fields are read only:
+ * they must not be dst, may alias src, aux or each other, and share pitch and row count with src.  Aux terms keep offset
+ * 0 and may carry a coefficient.
+ * ------------------------------------------------------------------------------------------- */
+#define SB_STENCIL_MAX_COEFS 4
+#define SB_STENCIL_COEF_REACH 1
+typedef struct sb_stencil_vterm {
+  int32_t source;         /* 0 = src, 1 = aux */
+  int32_t offset[3];      /* dx, dy, dz of the source read */
+  int32_t coef;           /* coefficient field, or -1 for a plain term */
+  int32_t coef_offset[3]; /* dx, dy, dz of the coefficient read; (0, 0, 0) on a plain term */
+  double weight;
+} sb_stencil_vterm;
+
+/* Host only.  sb_stencil_check for coefficient terms: the same limits plus coef in -1 .. SB_STENCIL_MAX_COEFS - 1 and
+ * |c_a| <= SB_STENCIL_COEF_REACH, and the same reach test applied to every src offset and every coefficient offset. */
+int sb_stencil_vcheck(const sb_stencil_vterm *terms, int n, const int64_t radius27[27]);
+/* Host only.  The conservative second-order div(kappa grad u) on a grid of spacing[3]: 12 terms.  Coefficient field a
+ * holds kappa on the faces normal to axis a, C_a(p) on the face between p - e_a and p.  In double, i_a = 1 / (h_a * h_a);
+ * for the axes x, y, z in order: (src +e_a, i_a, coef a at +e_a), (src 0, -i_a, coef a at +e_a), (src 0, -i_a, coef a
+ * at 0), (src -e_a, i_a, coef a at 0).  Writes at most cap terms (out may be NULL with cap 0) and returns 12, or
+ * SB_ERR_INVALID for a spacing that is not finite and > 0. */
+int sb_stencil_div_grad(const double spacing[3], sb_stencil_vterm *out, int cap);
+/* sb_stencil_plan_create with coefficient terms and ncoef (0 .. SB_STENCIL_MAX_COEFS) coefficient allocations coef[k],
+ * which share dst's zsize.  sb_stencil_plan_create is this call with every coef = -1 and no fields.  Errors beyond
+ * sb_stencil_plan_create's (SB_ERR_INVALID with a message, before anything is allocated): ncoef outside 0 .. 4, a term
+ * naming a field >= ncoef, a NULL coefficient pointer, a coefficient offset beyond reach 1, a coefficient buffer equal to
+ * dst, a coefficient with another pitch or row count or a misaligned pointer, a box whose coefficient reads leave the
+ * allocation. */
+int sb_stencil_vplan_create(sb_stencil_plan **out, int device, int dtype, const sb_stencil_vterm *terms, int n, sb_pitched dst,
+                            sb_pitched src, sb_pitched aux, const sb_pitched *coef, int ncoef, const int64_t acc_origin[3],
+                            int64_t zsize, int nbox, const int64_t *lo, const int64_t *hi);
 
 /* ---------------------------------------------------------------------------------------------
  * 7-point jacobi step (the reference's user kernel, bin/jacobi3d.cu:40-85) over a region.

@@ -650,7 +650,7 @@ void DistributedDomain::destroy_stencil_plans() {
 }
 
 void DistributedDomain::apply_op(const stencil::LinearStencil &op, int dtype, size_t dq, stencil::Which dw, size_t sq, int64_t aq,
-                                 stencil::Which aw, bool exchange) {
+                                 stencil::Which aw, const std::vector<size_t> &cq, bool exchange) {
   using stencil::Which;
   if (domains_.empty() || plans_[0].size() != domains_.size()) LOG_FATAL("apply: call realize() first");
   if (dtype != SB_DTYPE_F32 && dtype != SB_DTYPE_F64) LOG_FATAL("apply: a stencil operator computes in float or double");
@@ -658,18 +658,25 @@ void DistributedDomain::apply_op(const stencil::LinearStencil &op, int dtype, si
     if (q >= 0 && (size_t(q) >= dataDtype_.size() || dataDtype_[size_t(q)] != dtype)) LOG_FATAL("apply: unknown data handle " << q);
   if (dq == sq && dw == Which::curr) LOG_FATAL("apply: dst must not be src");
   if (op.has_aux() && aq < 0) LOG_FATAL("apply: the op has a term on aux, but no aux buffer was given");
+  if (int(cq.size()) != op.ncoef()) LOG_FATAL("apply: the op reads " << op.ncoef() << " coefficient fields, but " << cq.size() << " were given");
+  for (size_t k = 0; k < cq.size(); ++k) {
+    if (cq[k] >= dataDtype_.size() || dataDtype_[cq[k]] != dtype) LOG_FATAL("apply: coefficient " << k << " is not a quantity of the op's type");
+    if (cq[k] == dq && dw == Which::curr) LOG_FATAL("apply: coefficient " << k << " must not be dst");
+  }
   int64_t r27[27];
   for (int z = -1, i = 0; z <= 1; ++z)
     for (int y = -1; y <= 1; ++y)
       for (int x = -1; x <= 1; ++x) r27[i++] = int64_t(radius_.dir(x, y, z));
-  const std::vector<sb_stencil_term> &terms = op.terms();
-  if (SB_OK != sb_stencil_check(terms.data(), int(terms.size()), r27)) LOG_FATAL("apply: " << sb_last_error());
+  const std::vector<sb_stencil_vterm> &terms = op.vterms();
+  if (SB_OK != sb_stencil_vcheck(terms.data(), int(terms.size()), r27)) LOG_FATAL("apply: " << sb_last_error());
   if (!op.has_aux()) aq = -1;
-  std::vector<int64_t> key = {dtype, int64_t(dq), int64_t(dw == Which::next), int64_t(sq), aq, int64_t(aw == Which::next), int64_t(exchange), parity_};
-  for (const sb_stencil_term &t : terms) {
+  std::vector<int64_t> key = {dtype, int64_t(dq), int64_t(dw == Which::next), int64_t(sq), aq, int64_t(aw == Which::next), int64_t(exchange), parity_,
+                              int64_t(cq.size())};
+  for (const size_t q : cq) key.push_back(int64_t(q));
+  for (const sb_stencil_vterm &t : terms) {
     int64_t wbits;
     std::memcpy(&wbits, &t.weight, 8);
-    key.insert(key.end(), {t.source, t.offset[0], t.offset[1], t.offset[2], wbits});
+    key.insert(key.end(), {t.source, t.offset[0], t.offset[1], t.offset[2], t.coef, t.coef_offset[0], t.coef_offset[1], t.coef_offset[2], wbits});
   }
   auto found = stencilPlans_.find(key);
   if (found == stencilPlans_.end()) {
@@ -680,6 +687,8 @@ void DistributedDomain::apply_op(const stencil::LinearStencil &op, int dtype, si
       LocalDomain &d = domains_[di];
       const sb_pitched dst = as_sb(dw == Which::curr ? d.curr_data(dq) : d.next_data(dq)), src = as_sb(d.curr_data(sq));
       const sb_pitched aux = aq < 0 ? sb_pitched{nullptr, 0, 0} : as_sb(aw == Which::curr ? d.curr_data(size_t(aq)) : d.next_data(size_t(aq)));
+      std::vector<sb_pitched> coef;
+      for (const size_t q : cq) coef.push_back(as_sb(d.curr_data(q)));
       int64_t acc[3];
       set3(acc, d.origin() - Dim3(radius_.x(-1), radius_.y(-1), radius_.z(-1)));
       auto make = [&](const std::vector<Rect3> &boxes) {
@@ -689,8 +698,8 @@ void DistributedDomain::apply_op(const stencil::LinearStencil &op, int dtype, si
           hi.insert(hi.end(), {b.hi.x, b.hi.y, b.hi.z});
         }
         sb_stencil_plan *p = nullptr;
-        if (SB_OK != sb_stencil_plan_create(&p, d.gpu(), dtype, terms.data(), int(terms.size()), dst, src, aux, acc, d.raw_size().z,
-                                            int(boxes.size()), lo.data(), hi.data()))
+        if (SB_OK != sb_stencil_vplan_create(&p, d.gpu(), dtype, terms.data(), int(terms.size()), dst, src, aux, coef.data(), int(coef.size()),
+                                             acc, d.raw_size().z, int(boxes.size()), lo.data(), hi.data()))
           LOG_FATAL("apply: " << sb_last_error());
         return p;
       };

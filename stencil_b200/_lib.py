@@ -123,6 +123,15 @@ class StencilTerm(C.Structure):
 
 STENCIL_MAX_TERMS, STENCIL_MAX_REACH = 64, 4  # SB_STENCIL_MAX_TERMS, SB_STENCIL_MAX_REACH
 
+
+class StencilVTerm(C.Structure):
+    """sb_stencil_vterm: a term that may also read coefficient field `coef` (-1: none) at `coef_offset`."""
+
+    _fields_ = [("source", C.c_int32), ("offset", C.c_int32 * 3), ("coef", C.c_int32), ("coef_offset", C.c_int32 * 3), ("weight", C.c_double)]
+
+
+STENCIL_MAX_COEFS, STENCIL_COEF_REACH = 4, 1  # SB_STENCIL_MAX_COEFS, SB_STENCIL_COEF_REACH
+
 I6 = C.c_int32 * 6
 
 FUSED_MAX_GROUPS = 4096  # SB_FUSED_MAX_GROUPS
@@ -176,6 +185,13 @@ _SIGS = {
         C.c_int,
         [C.POINTER(C.c_void_p), C.c_int, C.c_int, C.POINTER(StencilTerm), C.c_int, Pitched, Pitched, Pitched, I3, C.c_int64, C.c_int,
          C.POINTER(C.c_int64), C.POINTER(C.c_int64)],
+    ),
+    "sb_stencil_vcheck": (C.c_int, [C.POINTER(StencilVTerm), C.c_int, I27]),
+    "sb_stencil_div_grad": (C.c_int, [C.c_double * 3, C.POINTER(StencilVTerm), C.c_int]),
+    "sb_stencil_vplan_create": (
+        C.c_int,
+        [C.POINTER(C.c_void_p), C.c_int, C.c_int, C.POINTER(StencilVTerm), C.c_int, Pitched, Pitched, Pitched, C.POINTER(Pitched), C.c_int,
+         I3, C.c_int64, C.c_int, C.POINTER(C.c_int64), C.POINTER(C.c_int64)],
     ),
     "sb_stencil_plan_launch": (C.c_int, [C.c_void_p, C.c_void_p]),
     "sb_stencil_plan_bytes": (C.c_int64, [C.c_void_p]),

@@ -556,9 +556,10 @@ struct sb_reduce_plan {
 struct sb_stencil_plan {
   int device = 0;
   int es = 8, R = 1;
-  std::vector<sb::OpTileParams> tiles; // one tile-kernel launch per thick box
+  bool has_coef = false;                // some term reads a coefficient field: the HAS_COEF kernels
+  std::vector<sb::OpVTileParams> tiles; // one tile-kernel launch per thick box
   std::vector<int> tile_grids;
-  std::vector<sb::OpCellParams> cells; // one cell-kernel launch per group of thin boxes
+  std::vector<sb::OpVCellParams> cells; // one cell-kernel launch per group of thin boxes
   std::vector<int> cell_grids;
   int64_t bytes = 0;
 };
@@ -1325,11 +1326,12 @@ int sb_reduce_combine(const sb_reduce_result *parts, int64_t n, sb_reduce_result
 }
 
 // ----------------------------------------------------------------------------------------- linear stencil operators
-// The limits every term list obeys, whatever the domain: n, sources, |o_a| <= 4, aux terms without offset.
-static int stencil_terms_ok(const sb_stencil_term *terms, int n) {
+// The limits every term list obeys, whatever the domain: n, sources, |o_a| <= 4, aux terms without offset, coefficient
+// fields 0 .. 3 (or -1) read within reach 1, plain terms without a coefficient offset.
+static int stencil_terms_ok(const sb_stencil_vterm *terms, int n) {
   if (!terms || n < 1 || n > SB_STENCIL_MAX_TERMS) return fail(SB_ERR_INVALID, "an op has 1 to %d terms, not %d", SB_STENCIL_MAX_TERMS, terms ? n : 0);
   for (int t = 0; t < n; ++t) {
-    const sb_stencil_term &T = terms[t];
+    const sb_stencil_vterm &T = terms[t];
     if (T.source != 0 && T.source != 1) return fail(SB_ERR_INVALID, "term %d: source %d must be 0 (src) or 1 (aux)", t, int(T.source));
     for (int a = 0; a < 3; ++a)
       if (T.offset[a] < -SB_STENCIL_MAX_REACH || T.offset[a] > SB_STENCIL_MAX_REACH)
@@ -1338,33 +1340,90 @@ static int stencil_terms_ok(const sb_stencil_term *terms, int n) {
     if (T.source == 1 && (T.offset[0] || T.offset[1] || T.offset[2]))
       return fail(SB_ERR_INVALID, "term %d: an aux term has offset (0, 0, 0), not (%d, %d, %d)", t, int(T.offset[0]), int(T.offset[1]),
                   int(T.offset[2]));
+    if (T.coef < -1 || T.coef >= SB_STENCIL_MAX_COEFS)
+      return fail(SB_ERR_INVALID, "term %d: coefficient field %d must be -1 (none) or 0 .. %d", t, int(T.coef), SB_STENCIL_MAX_COEFS - 1);
+    const int32_t *c = T.coef_offset;
+    if (T.coef == -1 && (c[0] || c[1] || c[2]))
+      return fail(SB_ERR_INVALID, "term %d: a term without a coefficient field has coefficient offset (0, 0, 0), not (%d, %d, %d)", t,
+                  int(c[0]), int(c[1]), int(c[2]));
+    for (int a = 0; a < 3; ++a)
+      if (c[a] < -SB_STENCIL_COEF_REACH || c[a] > SB_STENCIL_COEF_REACH)
+        return fail(SB_ERR_INVALID, "term %d: coefficient offset (%d, %d, %d) reaches beyond %d cell", t, int(c[0]), int(c[1]), int(c[2]),
+                    SB_STENCIL_COEF_REACH);
+  }
+  return SB_OK;
+}
+
+// Whether a subdomain with ghost widths radius27 holds the cell at offset o of term t (what: "offset" or "coefficient
+// offset"): the ghost box of sign(o) is exchanged and each non-zero component fits the face radius on its side.
+static int stencil_offset_in_reach(int t, const char *what, const int32_t o[3], const int64_t radius27[27]) {
+  if (!o[0] && !o[1] && !o[2]) return SB_OK;
+  int s[3];
+  for (int a = 0; a < 3; ++a) s[a] = (o[a] > 0) - (o[a] < 0);
+  if (radius27[(s[2] + 1) * 9 + (s[1] + 1) * 3 + (s[0] + 1)] <= 0)
+    return fail(SB_ERR_INVALID, "term %d: %s (%d, %d, %d) reads the ghost box in direction (%d, %d, %d), whose radius is 0", t, what,
+                int(o[0]), int(o[1]), int(o[2]), s[0], s[1], s[2]);
+  for (int a = 0; a < 3; ++a) {
+    if (!o[a]) continue;
+    int d[3] = {0, 0, 0};
+    d[a] = s[a];
+    const int64_t face = radius27[(d[2] + 1) * 9 + (d[1] + 1) * 3 + (d[0] + 1)];
+    if (int64_t(o[a] < 0 ? -o[a] : o[a]) > face)
+      return fail(SB_ERR_INVALID, "term %d: %s (%d, %d, %d) reaches %d cells on side %c%c, whose face radius is %lld", t, what,
+                  int(o[0]), int(o[1]), int(o[2]), int(o[a] < 0 ? -o[a] : o[a]), s[a] < 0 ? '-' : '+', "xyz"[a], (long long)face);
+  }
+  return SB_OK;
+}
+
+// A plain term list as coefficient terms without a field (at most SB_STENCIL_MAX_TERMS are converted: a longer list is
+// rejected by stencil_terms_ok on its count; the result holds at least one element so that its data() is not NULL).
+static std::vector<sb_stencil_vterm> stencil_vterms_of(const sb_stencil_term *terms, int n) {
+  std::vector<sb_stencil_vterm> v(size_t(std::max(1, std::min(n, SB_STENCIL_MAX_TERMS))), sb_stencil_vterm{0, {0, 0, 0}, -1, {0, 0, 0}, 0.0});
+  for (int t = 0; terms && t < std::min(n, SB_STENCIL_MAX_TERMS); ++t) {
+    sb_stencil_vterm &V = v[size_t(t)];
+    V.source = terms[t].source;
+    for (int a = 0; a < 3; ++a) V.offset[a] = terms[t].offset[a];
+    V.weight = terms[t].weight;
+  }
+  return v;
+}
+
+int sb_stencil_vcheck(const sb_stencil_vterm *terms, int n, const int64_t radius27[27]) {
+  if (!radius27) return fail(SB_ERR_INVALID, "sb_stencil_check needs radius27");
+  int rc = stencil_terms_ok(terms, n);
+  if (rc != SB_OK) return rc;
+  for (int t = 0; t < n; ++t) {
+    if ((rc = stencil_offset_in_reach(t, "offset", terms[t].offset, radius27)) != SB_OK) return rc;
+    if (terms[t].coef >= 0 && (rc = stencil_offset_in_reach(t, "coefficient offset", terms[t].coef_offset, radius27)) != SB_OK) return rc;
   }
   return SB_OK;
 }
 
 int sb_stencil_check(const sb_stencil_term *terms, int n, const int64_t radius27[27]) {
-  if (!radius27) return fail(SB_ERR_INVALID, "sb_stencil_check needs radius27");
-  int rc = stencil_terms_ok(terms, n);
-  if (rc != SB_OK) return rc;
-  for (int t = 0; t < n; ++t) {
-    const int32_t *o = terms[t].offset;
-    if (!o[0] && !o[1] && !o[2]) continue;
-    int s[3];
-    for (int a = 0; a < 3; ++a) s[a] = (o[a] > 0) - (o[a] < 0);
-    if (radius27[(s[2] + 1) * 9 + (s[1] + 1) * 3 + (s[0] + 1)] <= 0)
-      return fail(SB_ERR_INVALID, "term %d: offset (%d, %d, %d) reads the ghost box in direction (%d, %d, %d), whose radius is 0", t,
-                  int(o[0]), int(o[1]), int(o[2]), s[0], s[1], s[2]);
-    for (int a = 0; a < 3; ++a) {
-      if (!o[a]) continue;
-      int d[3] = {0, 0, 0};
-      d[a] = s[a];
-      const int64_t face = radius27[(d[2] + 1) * 9 + (d[1] + 1) * 3 + (d[0] + 1)];
-      if (int64_t(o[a] < 0 ? -o[a] : o[a]) > face)
-        return fail(SB_ERR_INVALID, "term %d: offset (%d, %d, %d) reaches %d cells on side %c%c, whose face radius is %lld", t,
-                    int(o[0]), int(o[1]), int(o[2]), int(o[a] < 0 ? -o[a] : o[a]), s[a] < 0 ? '-' : '+', "xyz"[a], (long long)face);
+  const std::vector<sb_stencil_vterm> v = stencil_vterms_of(terms, n);
+  return sb_stencil_vcheck(terms ? v.data() : nullptr, n, radius27);
+}
+
+int sb_stencil_div_grad(const double spacing[3], sb_stencil_vterm *out, int cap) {
+  if (!spacing) return fail(SB_ERR_INVALID, "sb_stencil_div_grad needs spacing[3]");
+  for (int a = 0; a < 3; ++a)
+    if (!(spacing[a] > 0.0) || !std::isfinite(spacing[a])) return fail(SB_ERR_INVALID, "spacing[%d] = %g must be finite and > 0", a, spacing[a]);
+  if (cap < 0 || (cap > 0 && !out)) return fail(SB_ERR_INVALID, "sb_stencil_div_grad: bad output buffer");
+  const int total = 12;
+  for (int a = 0, i = 0; a < 3; ++a) {
+    const double h2 = spacing[a] * spacing[a];
+    const double inv = 1.0 / h2;
+    // (src offset, weight, coefficient offset) along axis a, in units of e_a
+    const int rows[4][3] = {{1, 1, 1}, {0, -1, 1}, {0, -1, 0}, {-1, 1, 0}};
+    for (const auto &r : rows) {
+      sb_stencil_vterm t{0, {0, 0, 0}, a, {0, 0, 0}, r[1] * inv};
+      t.offset[a] = r[0];
+      t.coef_offset[a] = r[2];
+      if (i < cap) out[i] = t;
+      ++i;
     }
   }
-  return SB_OK;
+  return total;
 }
 
 int sb_stencil_laplacian(int order, const double spacing[3], sb_stencil_term *out, int cap) {
@@ -1404,12 +1463,26 @@ int sb_stencil_plan_create(sb_stencil_plan **out, int device, int dtype, const s
                            sb_pitched src, sb_pitched aux, const int64_t acc_origin[3], int64_t zsize, int nbox, const int64_t *lo,
                            const int64_t *hi) {
   if (!out) return fail(SB_ERR_INVALID, "sb_stencil_plan_create needs an output handle");
+  const std::vector<sb_stencil_vterm> v = stencil_vterms_of(terms, n);
+  return sb_stencil_vplan_create(out, device, dtype, terms ? v.data() : nullptr, n, dst, src, aux, nullptr, 0, acc_origin, zsize, nbox,
+                                 lo, hi);
+}
+
+int sb_stencil_vplan_create(sb_stencil_plan **out, int device, int dtype, const sb_stencil_vterm *terms, int n, sb_pitched dst,
+                            sb_pitched src, sb_pitched aux, const sb_pitched *coef, int ncoef, const int64_t acc_origin[3],
+                            int64_t zsize, int nbox, const int64_t *lo, const int64_t *hi) {
+  if (!out) return fail(SB_ERR_INVALID, "sb_stencil_plan_create needs an output handle");
   if (dtype != SB_DTYPE_F32 && dtype != SB_DTYPE_F64) return fail(SB_ERR_INVALID, "dtype %d must be SB_DTYPE_F32 or SB_DTYPE_F64", dtype);
   const int es = dtype == SB_DTYPE_F32 ? 4 : 8;
   int rc = stencil_terms_ok(terms, n);
   if (rc != SB_OK) return rc;
+  if (ncoef < 0 || ncoef > SB_STENCIL_MAX_COEFS) return fail(SB_ERR_INVALID, "ncoef %d: 0 to %d coefficient fields", ncoef, SB_STENCIL_MAX_COEFS);
+  if (ncoef > 0 && !coef) return fail(SB_ERR_INVALID, "ncoef %d, but the coefficient array is NULL", ncoef);
   bool has_aux = false;
   int rm[3] = {0, 0, 0}, rp[3] = {0, 0, 0}, R = 1;
+  // coefficient fields the op references, renumbered 0 .. nf - 1 in order of their index, with their reach per axis
+  int fmap[SB_STENCIL_MAX_COEFS] = {-1, -1, -1, -1}, fsrc[SB_STENCIL_MAX_COEFS] = {}, nf = 0;
+  int crm[SB_STENCIL_MAX_COEFS][3] = {}, crp[SB_STENCIL_MAX_COEFS][3] = {};
   for (int t = 0; t < n; ++t) {
     has_aux = has_aux || terms[t].source == 1;
     for (int a = 0; a < 3; ++a) {
@@ -1418,17 +1491,42 @@ int sb_stencil_plan_create(sb_stencil_plan **out, int device, int dtype, const s
       rp[a] = std::max(rp[a], o);
       R = std::max(R, std::abs(o));
     }
+    const int k = terms[t].coef;
+    if (k >= ncoef) return fail(SB_ERR_INVALID, "term %d names coefficient field %d, but ncoef is %d", t, k, ncoef);
+    if (k >= 0 && !coef[k].ptr) return fail(SB_ERR_INVALID, "coefficient field %d is NULL", k);
   }
+  for (int k = 0; k < ncoef; ++k)
+    for (int t = 0; t < n; ++t)
+      if (terms[t].coef == k) {
+        if (fmap[k] < 0) {
+          fmap[k] = nf;
+          fsrc[nf++] = k;
+        }
+        for (int a = 0; a < 3; ++a) {
+          crm[fmap[k]][a] = std::max(crm[fmap[k]][a], -terms[t].coef_offset[a]);
+          crp[fmap[k]][a] = std::max(crp[fmap[k]][a], terms[t].coef_offset[a]);
+        }
+      }
   if (has_aux && !aux.ptr) return fail(SB_ERR_INVALID, "the op has a term on aux, but aux is NULL");
   if (!dst.ptr || !src.ptr) return fail(SB_ERR_INVALID, "dst and src must not be NULL");
   if (dst.ptr == src.ptr) return fail(SB_ERR_INVALID, "dst must not be src (dst may be aux)");
-  const sb_pitched *bufs[3] = {&dst, &src, &aux};
-  const char *names[3] = {"dst", "src", "aux"};
-  for (int b = 0; b < (has_aux ? 3 : 2); ++b) {
+  for (int f = 0; f < nf; ++f)
+    if (coef[fsrc[f]].ptr == dst.ptr) return fail(SB_ERR_INVALID, "coefficient field %d is dst (coefficients are read only)", fsrc[f]);
+  std::vector<const sb_pitched *> bufs = {&dst, &src};
+  std::vector<std::string> names = {"dst", "src"};
+  if (has_aux) {
+    bufs.push_back(&aux);
+    names.push_back("aux");
+  }
+  for (int f = 0; f < nf; ++f) {
+    bufs.push_back(&coef[fsrc[f]]);
+    names.push_back("coefficient field " + std::to_string(fsrc[f]));
+  }
+  for (size_t b = 0; b < bufs.size(); ++b) {
     const sb_pitched &P = *bufs[b];
-    if (P.pitch != src.pitch || P.ysize != src.ysize) return fail(SB_ERR_INVALID, "%s has another pitch or row count than src", names[b]);
+    if (P.pitch != src.pitch || P.ysize != src.ysize) return fail(SB_ERR_INVALID, "%s has another pitch or row count than src", names[b].c_str());
     if ((uintptr_t(P.ptr) % uintptr_t(es)) || P.pitch <= 0 || (P.pitch % es) || P.ysize <= 0)
-      return fail(SB_ERR_INVALID, "%s: pointer and pitch must be positive multiples of the %d-byte element", names[b], es);
+      return fail(SB_ERR_INVALID, "%s: pointer and pitch must be positive multiples of the %d-byte element", names[b].c_str(), es);
   }
   if (!acc_origin || zsize < 1) return fail(SB_ERR_INVALID, "sb_stencil_plan_create needs acc_origin and zsize >= 1");
   if (nbox < 0 || (nbox > 0 && (!lo || !hi))) return fail(SB_ERR_INVALID, "nbox %d: needs nbox >= 0 and lo / hi arrays", nbox);
@@ -1449,6 +1547,11 @@ int sb_stencil_plan_create(sb_stencil_plan **out, int device, int dtype, const s
       if (l[a] - rm[a] < 0 || l[a] + e[a] + rp[a] > size[a])
         return fail(SB_ERR_INVALID, "box %d: the op reads cells %lld .. %lld on axis %c, outside the allocation's 0 .. %lld", b,
                     (long long)(l[a] - rm[a]), (long long)(l[a] + e[a] + rp[a] - 1), "xyz"[a], (long long)(size[a] - 1));
+    for (int f = 0; f < nf; ++f)
+      for (int a = 0; a < 3; ++a)
+        if (l[a] - crm[f][a] < 0 || l[a] + e[a] + crp[f][a] > size[a])
+          return fail(SB_ERR_INVALID, "box %d: coefficient field %d is read at cells %lld .. %lld on axis %c, outside the allocation's 0 .. %lld",
+                      b, fsrc[f], (long long)(l[a] - crm[f][a]), (long long)(l[a] + e[a] + crp[f][a] - 1), "xyz"[a], (long long)(size[a] - 1));
     if (e[0] * e[1] * e[2] >= (1ll << 32)) return fail(SB_ERR_INVALID, "box %d: more than 2^32 cells", b);
     const std::array<int, 6> bx = {int(l[0]), int(l[1]), int(l[2]), int(e[0]), int(e[1]), int(e[2])};
     (e[0] >= 8 && e[1] >= 8 && e[2] >= 8 ? thick : thin).push_back(bx);
@@ -1477,17 +1580,33 @@ int sb_stencil_plan_create(sb_stencil_plan **out, int device, int dtype, const s
   p->device = device;
   p->es = es;
   p->R = R;
-  p->bytes = cells * es * (has_aux ? 3 : 2);
+  p->has_coef = nf > 0;
+  p->bytes = cells * es * ((has_aux ? 3 : 2) + nf);
   if (!thick.empty()) {
-    const int per_sm = sb::op_tile_prepare(R, es, device);
+    const int per_sm = sb::op_tile_prepare(R, es, device, nf);
     if (per_sm <= 0) {
       delete p;
       return fail(SB_ERR_CUDA, "the R = %d tile kernel cannot be configured: %s", R, cudaGetErrorString(cudaGetLastError()));
     }
     const int SW = sb::op_tile_sw(R), P = sb::op_tile_plane(R), NS = 2 * R + 1;
+    const int CSW = sb::op_tile_sw(1), CP = sb::op_tile_plane(1), CS = sb::kOpCoefSlots;
     for (const auto &b : thick) {
-      sb::OpTileParams tp{};
+      sb::OpVTileParams tp{};
       tp.c = com;
+      tp.k.nf = nf;
+      for (int f = 0; f < nf; ++f) {
+        tp.k.coef[f] = static_cast<const char *>(coef[fsrc[f]].ptr);
+        for (int a = 0; a < 3; ++a) {
+          tp.k.crm[f][a] = crm[f][a];
+          tp.k.crp[f][a] = crp[f][a];
+        }
+      }
+      for (int t = 0; t < n; ++t) {
+        const int f = terms[t].coef < 0 ? -1 : fmap[terms[t].coef];
+        tp.k.cfield[t] = (signed char)f;
+        const int32_t *c = terms[t].coef_offset;
+        for (int s = 0; s < CS && f >= 0; ++s) tp.k.coff[s][t] = short((f * CS + (s + c[2] + CS) % CS) * CP + c[1] * CSW + c[0]);
+      }
       tp.src_end = com.src + com.slice * zsize;
       for (int a = 0; a < 3; ++a) {
         tp.lo[a] = b[a];
@@ -1518,10 +1637,16 @@ int sb_stencil_plan_create(sb_stencil_plan **out, int device, int dtype, const s
     }
   }
   for (size_t b0 = 0; b0 < thin.size(); b0 += sb::kOpMaxBoxes) {
-    sb::OpCellParams cp{};
+    sb::OpVCellParams cp{};
     cp.c = com;
     for (int t = 0; t < n; ++t)
       cp.goff[t] = (long long)terms[t].offset[2] * com.slice + (long long)terms[t].offset[1] * com.pitch + (long long)terms[t].offset[0] * es;
+    for (int f = 0; f < nf; ++f) cp.coef[f] = static_cast<const char *>(coef[fsrc[f]].ptr);
+    for (int t = 0; t < n; ++t) {
+      const int32_t *c = terms[t].coef_offset;
+      cp.cfield[t] = (signed char)(terms[t].coef < 0 ? -1 : fmap[terms[t].coef]);
+      cp.cgoff[t] = (long long)c[2] * com.slice + (long long)c[1] * com.pitch + (long long)c[0] * es;
+    }
     cp.first[0] = 0;
     for (size_t b = b0; b < thin.size() && b < b0 + sb::kOpMaxBoxes; ++b) {
       const int m = cp.n++;
@@ -1545,7 +1670,7 @@ int sb_stencil_plan_launch(sb_stencil_plan *p, void *stream) {
   if (!guard.ok) return fail(SB_ERR_NOGPU, "cannot select CUDA device %d", p->device);
   const cudaStream_t s = static_cast<cudaStream_t>(stream);
   for (size_t i = 0; i < p->tiles.size(); ++i) g_launches += uint64_t(sb::launch_op_tile(p->tiles[i], p->R, p->es, p->tile_grids[i], s));
-  for (size_t i = 0; i < p->cells.size(); ++i) g_launches += uint64_t(sb::launch_op_cells(p->cells[i], p->es, p->cell_grids[i], s));
+  for (size_t i = 0; i < p->cells.size(); ++i) g_launches += uint64_t(sb::launch_op_cells(p->cells[i], p->es, p->has_coef, p->cell_grids[i], s));
   SB_CUDA(cudaGetLastError());
   return SB_OK;
 }

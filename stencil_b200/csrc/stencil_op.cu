@@ -1,4 +1,4 @@
-// Constant-coefficient linear stencil operators for sm_90a (see stencil_op.cuh and include/stencil_b200.h).
+// Linear stencil operators for sm_90a, constant and variable coefficients (see stencil_op.cuh and include/stencil_b200.h).
 //
 // op_tile_kernel<T, R>: z-march over thick boxes.  A CTA owns a 64 x 8 tile of cells and a z chunk; the halo'd planes
 // z - R .. z + R of the tile sit in a shared-memory ring of 2R + 1 slots, so each input plane of the tile is read from
@@ -14,9 +14,16 @@
 // Numerics (both kernels): acc = T(w_0) * S_0; acc = acc + T(w_k) * S_k in list order, every multiply and add rounded
 // separately (__fmul_rn / __fadd_rn, __dmul_rn / __dadd_rn: no FMA contraction), so the result is a function of the
 // inputs only, whatever the launch shape.
+//
+// Coefficient fields (HAS_COEF, a compile-time switch, so the plain instantiations are the code they were): a term may
+// carry a field C read at p + c, |c_a| <= 1, and contributes (T(w) * C) * S.  The tile kernel keeps a ring of
+// kOpCoefSlots halo'd planes per referenced field behind the src ring, filled one plane ahead by cp.async (no register
+// staging), each field's window cut to its own reach; the term table carries each term's coefficient offset per slot.
+// The cell kernel reads coefficients through __ldg at per-term byte offsets.
 #include "stencil_op.cuh"
 
 #include <cstring>
+#include <type_traits>
 
 namespace sb {
 namespace {
@@ -33,8 +40,17 @@ template <> struct OpNum<double> {
   static __device__ __forceinline__ double w(const OpCommon &c, int t) { return c.w[t]; }
 };
 
-template <typename T, int R>
-__global__ void __launch_bounds__(kOpThreads, 2) op_tile_kernel(const __grid_constant__ OpTileParams p) {
+// one element global -> shared, asynchronously (cp.async, sm_80+); completion by cp_async_wait_all
+template <typename T> __device__ __forceinline__ void cp_async_elem(T *dst, const T *src) {
+  const unsigned s = unsigned(__cvta_generic_to_shared(dst));
+  asm volatile("cp.async.ca.shared.global [%0], [%1], %2;\n" ::"r"(s), "l"(src), "n"(int(sizeof(T))) : "memory");
+}
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;\n" ::: "memory"); }
+
+template <bool HAS_COEF> using OpTileParamsOf = typename std::conditional<HAS_COEF, OpVTileParams, OpTileParams>::type;
+
+template <typename T, int R, bool HAS_COEF>
+__global__ void __launch_bounds__(kOpThreads, 2) op_tile_kernel(const __grid_constant__ OpTileParamsOf<HAS_COEF> p) {
   extern __shared__ __align__(16) unsigned char op_smem[];
   T *ring = reinterpret_cast<T *>(op_smem);
   constexpr int SW = op_tile_sw(R), P = op_tile_plane(R), NS = 2 * R + 1;
@@ -104,6 +120,28 @@ __global__ void __launch_bounds__(kOpThreads, 2) op_tile_kernel(const __grid_con
   };
   auto slot_of = [&](int z) { return (z - z0 + R) % NS; };
 
+  // coefficient rings: field f's kOpCoefSlots planes of (kOpTileX + 2) x (kOpTileY + 2) after the src ring; plane z of
+  // its window (its own reach only) goes element by element through cp.async, so no registers hold it in flight
+  constexpr int CSW = op_tile_sw(1), CP = op_tile_plane(1);
+  T *const cring = ring + NS * P;
+  auto coef_plane = [&](int f, int z) {
+    if constexpr (HAS_COEF) {
+      const int cxa = x0 - p.k.crm[f][0], w = xe + p.k.crp[f][0] - cxa;
+      const int cya = y0 - p.k.crm[f][1], rows = ye + p.k.crp[f][1] - cya;
+      const char *plane = p.k.coef[f] + (long long)z * p.c.slice;
+      T *dst = cring + (f * kOpCoefSlots + ((z - z0 + 1) & (kOpCoefSlots - 1))) * CP + (1 - p.k.crm[f][1]) * CSW + (1 - p.k.crm[f][0]);
+      for (int j = wy; j < rows; j += kOpThreads / 32) { // warps own rows, lanes columns
+        const T *row = reinterpret_cast<const T *>(plane + (long long)(cya + j) * p.c.pitch) + cxa;
+        for (int i = lane; i < w; i += 32) cp_async_elem(dst + j * CSW + i, row + i);
+      }
+    }
+  };
+  if constexpr (HAS_COEF) {
+    if (z0 < z1)
+      for (int f = 0; f < p.k.nf; ++f)
+        for (int z = z0 - p.k.crm[f][2]; z <= z0 + p.k.crp[f][2]; ++z) coef_plane(f, z);
+  }
+
   for (int z = z0 - p.rm[2]; z < z0 + p.rp[2]; ++z) {
     fetch(z);
     store(slot_of(z));
@@ -113,10 +151,16 @@ __global__ void __launch_bounds__(kOpThreads, 2) op_tile_kernel(const __grid_con
   const int y = y0 + wy, xA = x0 + lane, xB = xA + 32;
   const bool okA = y < ye && xA < xe, okB = y < ye && xB < xe;
   const T *own = ring + (wy + R) * SW + lane + R;
+  const T *const cown = cring + (wy + 1) * CSW + lane + 1;
   for (int zc = z0; zc < z1; ++zc) {
     store(slot_of(zc + p.rp[2])); // the slot of plane zc + rp - (2R + 1), which no cell of plane zc reads
+    if constexpr (HAS_COEF) cp_async_wait_all(); // this thread's coefficient planes up to zc + crp have landed
     __syncthreads();
     if (zc + 1 < z1) fetch(zc + 1 + p.rp[2]);
+    if constexpr (HAS_COEF) {
+      if (zc + 1 < z1) // into the slot of plane zc - 2 (or older), which no cell of plane zc reads
+        for (int f = 0; f < p.k.nf; ++f) coef_plane(f, zc + 1 + p.k.crp[f][2]);
+    }
     const long long cell = (long long)zc * p.c.slice + (long long)y * p.c.pitch;
     T auxA = T(0), auxB = T(0);
     if (p.c.has_aux) { // read before the cell is written: dst may be aux
@@ -124,6 +168,8 @@ __global__ void __launch_bounds__(kOpThreads, 2) op_tile_kernel(const __grid_con
       if (okB) auxB = *reinterpret_cast<const T *>(p.c.aux + cell + xB * ES);
     }
     const int c = slot_of(zc);
+    const int cs = (zc - z0 + 1) & (kOpCoefSlots - 1);
+    (void)cs;
     T accA = T(0), accB = T(0);
     for (int t = 0; t < p.c.n; ++t) {
       T vA, vB;
@@ -136,7 +182,20 @@ __global__ void __launch_bounds__(kOpThreads, 2) op_tile_kernel(const __grid_con
         vB = auxB;
       }
       const T w = OpNum<T>::w(p.c, t);
-      const T mA = OpNum<T>::mul(w, vA), mB = OpNum<T>::mul(w, vB);
+      T mA, mB;
+      if constexpr (HAS_COEF) { // (T(w) * C) * S
+        T wA = w, wB = w;
+        if (p.k.cfield[t] >= 0) {
+          const int o = p.k.coff[cs][t];
+          wA = OpNum<T>::mul(w, cown[o]);
+          wB = OpNum<T>::mul(w, cown[o + 32]);
+        }
+        mA = OpNum<T>::mul(wA, vA);
+        mB = OpNum<T>::mul(wB, vB);
+      } else {
+        mA = OpNum<T>::mul(w, vA);
+        mB = OpNum<T>::mul(w, vB);
+      }
       accA = t == 0 ? mA : OpNum<T>::add(accA, mA);
       accB = t == 0 ? mB : OpNum<T>::add(accB, mB);
     }
@@ -146,7 +205,10 @@ __global__ void __launch_bounds__(kOpThreads, 2) op_tile_kernel(const __grid_con
   }
 }
 
-template <typename T> __global__ void __launch_bounds__(256) op_cell_kernel(const __grid_constant__ OpCellParams p) {
+template <bool HAS_COEF> using OpCellParamsOf = typename std::conditional<HAS_COEF, OpVCellParams, OpCellParams>::type;
+
+template <typename T, bool HAS_COEF>
+__global__ void __launch_bounds__(256) op_cell_kernel(const __grid_constant__ OpCellParamsOf<HAS_COEF> p) {
   const long long total = p.first[p.n];
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     int k = 0;
@@ -172,59 +234,76 @@ template <typename T> __global__ void __launch_bounds__(256) op_cell_kernel(cons
     T acc = T(0);
     for (int t = 0; t < p.c.n; ++t) {
       const T v = p.c.source[t] == 0 ? __ldg(reinterpret_cast<const T *>(s + p.goff[t])) : a;
-      const T m = OpNum<T>::mul(OpNum<T>::w(p.c, t), v);
+      T w = OpNum<T>::w(p.c, t);
+      if constexpr (HAS_COEF) {
+        const int f = p.cfield[t];
+        if (f >= 0) w = OpNum<T>::mul(w, __ldg(reinterpret_cast<const T *>(p.coef[f] + off + p.cgoff[t])));
+      }
+      const T m = OpNum<T>::mul(w, v);
       acc = t == 0 ? m : OpNum<T>::add(acc, m);
     }
     *reinterpret_cast<T *>(p.c.dst + off) = acc;
   }
 }
 
-template <typename T, int R> const void *tile_fn() { return reinterpret_cast<const void *>(&op_tile_kernel<T, R>); }
+template <typename T, int R> const void *tile_fn(bool coef) {
+  return coef ? reinterpret_cast<const void *>(&op_tile_kernel<T, R, true>) : reinterpret_cast<const void *>(&op_tile_kernel<T, R, false>);
+}
 
-const void *tile_kernel(int R, int es) {
+const void *tile_kernel(int R, int es, bool coef) {
   switch (R * 10 + es) {
-  case 14: return tile_fn<float, 1>();
-  case 24: return tile_fn<float, 2>();
-  case 34: return tile_fn<float, 3>();
-  case 44: return tile_fn<float, 4>();
-  case 18: return tile_fn<double, 1>();
-  case 28: return tile_fn<double, 2>();
-  case 38: return tile_fn<double, 3>();
-  case 48: return tile_fn<double, 4>();
+  case 14: return tile_fn<float, 1>(coef);
+  case 24: return tile_fn<float, 2>(coef);
+  case 34: return tile_fn<float, 3>(coef);
+  case 44: return tile_fn<float, 4>(coef);
+  case 18: return tile_fn<double, 1>(coef);
+  case 28: return tile_fn<double, 2>(coef);
+  case 38: return tile_fn<double, 3>(coef);
+  case 48: return tile_fn<double, 4>(coef);
   default: return nullptr;
   }
 }
 
 } // namespace
 
-size_t op_tile_smem(int R, int es) { return size_t(2 * R + 1) * size_t(op_tile_plane(R)) * size_t(es); }
+size_t op_tile_smem(int R, int es, int nf) {
+  return (size_t(2 * R + 1) * size_t(op_tile_plane(R)) + size_t(nf) * kOpCoefSlots * size_t(op_tile_plane(1))) * size_t(es);
+}
 
-int op_tile_prepare(int R, int es, int device) {
-  const void *fn = tile_kernel(R, es);
+int op_tile_prepare(int R, int es, int device, int nf) {
+  const void *fn = tile_kernel(R, es, nf > 0);
   if (!fn) return 0;
-  const int smem = int(op_tile_smem(R, es));
-  if (cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) return 0;
+  // the coefficient kernel's limit covers every field count, so plans with different counts can share it
+  const int limit = int(op_tile_smem(R, es, nf > 0 ? kOpMaxCoefs : 0));
+  if (cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, limit) != cudaSuccess) return 0;
   int ctas = 0;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctas, fn, kOpThreads, smem) != cudaSuccess) return 0;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctas, fn, kOpThreads, op_tile_smem(R, es, nf)) != cudaSuccess) return 0;
   (void)device;
   return ctas;
 }
 
-int launch_op_tile(const OpTileParams &p, int R, int es, int grid, cudaStream_t stream) {
+int launch_op_tile(const OpVTileParams &p, int R, int es, int grid, cudaStream_t stream) {
   if (grid <= 0) return 0;
-  const void *fn = tile_kernel(R, es);
+  const bool coef = p.k.nf > 0;
+  const void *fn = tile_kernel(R, es, coef);
   if (!fn) return 0;
-  void *args[] = {const_cast<OpTileParams *>(&p)};
-  cudaLaunchKernel(fn, dim3(unsigned(grid)), dim3(kOpThreads), args, op_tile_smem(R, es), stream);
+  // the plain kernel takes the OpTileParams part only
+  void *args[] = {coef ? const_cast<OpVTileParams *>(&p) : static_cast<OpTileParams *>(const_cast<OpVTileParams *>(&p))};
+  cudaLaunchKernel(fn, dim3(unsigned(grid)), dim3(kOpThreads), args, op_tile_smem(R, es, p.k.nf), stream);
   return 1;
 }
 
-int launch_op_cells(const OpCellParams &p, int es, int grid, cudaStream_t stream) {
+int launch_op_cells(const OpVCellParams &p, int es, bool has_coef, int grid, cudaStream_t stream) {
   if (grid <= 0 || p.n <= 0) return 0;
-  if (es == 4)
-    op_cell_kernel<float><<<unsigned(grid), 256, 0, stream>>>(p);
+  const OpCellParams &b = p;
+  if (es == 4 && has_coef)
+    op_cell_kernel<float, true><<<unsigned(grid), 256, 0, stream>>>(p);
+  else if (es == 4)
+    op_cell_kernel<float, false><<<unsigned(grid), 256, 0, stream>>>(b);
+  else if (has_coef)
+    op_cell_kernel<double, true><<<unsigned(grid), 256, 0, stream>>>(p);
   else
-    op_cell_kernel<double><<<unsigned(grid), 256, 0, stream>>>(p);
+    op_cell_kernel<double, false><<<unsigned(grid), 256, 0, stream>>>(b);
   return 1;
 }
 

@@ -1,4 +1,5 @@
-// Constant-coefficient linear stencil operators (include/stencil_b200.h, sb_stencil_*; DESIGN.md section 2.7).
+// Linear stencil operators, constant and variable coefficients (include/stencil_b200.h, sb_stencil_*; DESIGN.md
+// section 2.7).
 #pragma once
 
 #include <cstdint>
@@ -50,11 +51,38 @@ struct OpCellParams {
 __host__ __device__ constexpr int op_tile_sw(int R) { return kOpTileX + 2 * R; }
 __host__ __device__ constexpr int op_tile_plane(int R) { return (kOpTileX + 2 * R) * (kOpTileY + 2 * R); }
 
+// Coefficient fields (sb_stencil_vplan_create).  The plan numbers the fields the op references 0 .. nf - 1 (in order of
+// their C ABI index).  In the tile kernel each one has a ring of kOpCoefSlots planes of op_tile_plane(1) elements after
+// the src ring, filled by cp.async one plane ahead (slot of plane z: (z - z0 + 1) % kOpCoefSlots), each field's window
+// limited to its own reach crm / crp.  cfield[t]: the field of term t, or -1.
+constexpr int kOpMaxCoefs = 4;
+constexpr int kOpCoefSlots = 4; // planes z - 1 .. z + 1 being read, and z + 2 landing
+struct OpCoefTile {
+  const char *coef[kOpMaxCoefs];
+  int nf;
+  int crm[kOpMaxCoefs][3], crp[kOpMaxCoefs][3];
+  signed char cfield[kOpMaxTerms];
+  short coff[kOpCoefSlots][kOpMaxTerms]; // shared-memory element offset of term t's coefficient from the cell's own
+                                         // position in field 0's ring, while the centre plane sits in slot c
+};
+struct OpVTileParams : OpTileParams {
+  OpCoefTile k;
+};
+static_assert(sizeof(OpVTileParams) <= 4096, "the tile kernel's parameters fit the classic 4 KB limit");
+
+// the cell kernel's coefficient reads: field cfield[t] (-1: none) at byte offset cgoff[t] from the cell
+struct OpVCellParams : OpCellParams {
+  const char *coef[kOpMaxCoefs];
+  signed char cfield[kOpMaxTerms];
+  long long cgoff[kOpMaxTerms];
+};
+
 // Host: dynamic shared memory of the tile kernel; one-time attribute setup; the number of CTAs of the tile kernel that
-// fit on one SM (0 on error).  launch_* return the number of launches issued.
-size_t op_tile_smem(int R, int es);
-int op_tile_prepare(int R, int es, int device);
-int launch_op_tile(const OpTileParams &p, int R, int es, int grid, cudaStream_t stream);
-int launch_op_cells(const OpCellParams &p, int es, int grid, cudaStream_t stream);
+// fit on one SM (0 on error).  launch_* return the number of launches issued.  nf: coefficient fields (0: the plain
+// kernel).
+size_t op_tile_smem(int R, int es, int nf = 0);
+int op_tile_prepare(int R, int es, int device, int nf = 0);
+int launch_op_tile(const OpVTileParams &p, int R, int es, int grid, cudaStream_t stream);
+int launch_op_cells(const OpVCellParams &p, int es, bool has_coef, int grid, cudaStream_t stream);
 
 } // namespace sb

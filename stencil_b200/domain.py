@@ -1145,11 +1145,15 @@ class DistributedDomain:
         return _lib.ReduceItem(kind, bc_dtype(self.dtypes_[qs[0]]), (Pitched * 3)(*srcs), i3(d.accessor_origin()), i3(lo), i3(hi))
 
     # -- linear stencil operators
-    def apply(self, op, dst, src, aux=None, exchange: bool = True) -> None:
-        """dst = op(src, aux) over the whole compute region of every local subdomain (DESIGN.md section 2.7).
+    def apply(self, op, dst, src, aux=None, exchange: bool = True, coefs=None) -> None:
+        """dst = op(src, aux, coefs) over the whole compute region of every local subdomain (DESIGN.md section 2.7).
 
         Buffers are (DataHandle, "curr" | "next"); a bare handle means "next" for dst and "curr" for src and aux.  src is
         always a curr buffer (the one exchange() fills); dst may be aux, never src; all share op's element type.
+        coefs: one DataHandle per coefficient field the op names (op.ncoef of them, field k = coefs[k]), read from their
+        curr buffers, which exchange() fills like src's (with the quantity's own BC on a wall); a coefficient must not be
+        dst.  swap() turns every quantity's buffers, coefficients included, so a static coefficient must hold the same
+        compute cells in curr and next.
         exchange=True: the interior runs on its own stream while exchange() fills the ghost cells, then the exterior slabs
         of each subdomain run as one launch; exchange=False: one launch over the whole region, and the caller guarantees
         the ghost cells are current.  Returns when the update is complete.  The plans are built on first use and kept,
@@ -1181,15 +1185,27 @@ class DistributedDomain:
         a = buf(aux, "curr", "aux") if aux is not None else None
         if op.has_aux and a is None:
             raise _lib.StencilError("apply: the op has a term on aux, but no aux buffer was given")
+        cs = list(coefs) if coefs is not None else []
+        if len(cs) != op.ncoef:
+            raise _lib.StencilError(f"apply: the op reads {op.ncoef} coefficient fields, but {len(cs)} were given")
+        c_q = []
+        for k, c in enumerate(cs):
+            q, w = buf(c, "curr", f"coefficient {k}")
+            if w != "curr":
+                raise _lib.StencilError(f"apply: coefficient {k} must be a curr buffer (the one exchange() fills)")
+            if (q, w) == (d_q, d_w):
+                raise _lib.StencilError(f"apply: coefficient {k} must not be dst")
+            c_q.append(q)
         op.check(self.radius_)
-        key = (op.key(), (d_q, d_w), s_q, a if op.has_aux else None, bool(exchange), self._parity)
+        key = (op.key(), (d_q, d_w), s_q, a if op.has_aux else None, tuple(c_q), bool(exchange), self._parity)
         plans = self._stencil_plans.get(key)
         if plans is None:
             plans = []
             interiors, exteriors = (self.get_interior(), self.get_exterior()) if exchange else (None, None)
             for di, d in enumerate(self.domains_):
                 P = (d.pitched(d_q, d_w), d.pitched(s_q, "curr"), d.pitched(a[0], a[1]) if a is not None and op.has_aux else Pitched(None, 0, 0))
-                mk = lambda boxes: StencilPlan(d.gpu(), op, *P, d.accessor_origin(), d.raw_size()[2], boxes)  # noqa: E731
+                K = [d.pitched(q, "curr") for q in c_q] if op.has_coef else None
+                mk = lambda boxes: StencilPlan(d.gpu(), op, *P, d.accessor_origin(), d.raw_size()[2], boxes, K)  # noqa: E731
                 if exchange:
                     plans.append((mk([interiors[di]]), mk(exteriors[di])))
                 else:

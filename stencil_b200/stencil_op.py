@@ -1,4 +1,4 @@
-"""Constant-coefficient linear stencil operators over the C ABI (sb_stencil_*, DESIGN.md section 2.7).
+"""Linear stencil operators, constant and variable coefficients, over the C ABI (sb_stencil_*, DESIGN.md section 2.7).
 
     op = StencilOp.laplacian(4, (hx, hy, hz), np.float64)          # or StencilOp([(source, (dx, dy, dz), w), ...], dtype)
     heat = StencilOp([(s, o, dt * w) for s, o, w in op.terms] + [(0, (0, 0, 0), 1.0)], np.float64)
@@ -6,20 +6,28 @@
     dd.swap()
 
 A term reads src (source 0) at p + offset or aux (source 1) at p.  Per cell, in the quantity's type with every multiply
-and add rounded separately: acc = T(w_0) * S_0; acc = acc + T(w_k) * S_k in list order; dst[p] = acc.  The rule, the
-reach check against a domain's radius and the Laplacian table live in the C library; this module only carries them.
+and add rounded separately: acc = T(w_0) * S_0; acc = acc + T(w_k) * S_k in list order; dst[p] = acc.  A coefficient term
+(source, offset, weight, k, coef_offset) also reads coefficient field k (0..3) at p + coef_offset (|c_a| <= 1) and
+contributes (T(w) * C_k) * S instead:
+
+    kdt = StencilOp.div_grad((hx, hy, hz), np.float64).scaled(dt)    # dt div(kappa grad u), kappa on faces in 3 fields
+    heat = StencilOp(list(kdt.terms) + [(0, (0, 0, 0), 1.0)], np.float64)
+    dd.apply(heat, h, h, coefs=[kx, ky, kz])
+
+The rule, the reach check against a domain's radius and the Laplacian and div-grad tables live in the C library; this
+module only carries them.
 """
 from __future__ import annotations
 
 import ctypes as C
-from typing import Iterable, List, Sequence, Tuple
+from typing import Iterable, List, Optional, Sequence, Tuple
 
 import numpy as np
 
 from . import _lib
-from ._lib import I27, Pitched, StencilTerm, check, i3, lib, stream_ptr
+from ._lib import I27, Pitched, StencilTerm, StencilVTerm, check, i3, lib, stream_ptr
 
-Term = Tuple[int, Tuple[int, int, int], float]
+Term = Tuple  # (source, offset, weight) or (source, offset, weight, coef, coef_offset)
 
 
 def _dtype_code(dtype) -> int:
@@ -32,18 +40,34 @@ def _dtype_code(dtype) -> int:
 
 
 class StencilOp:
-    """An operator: terms (source, (dx, dy, dz), weight) applied in list order, in dtype (float32 or float64)."""
+    """An operator: terms (source, (dx, dy, dz), weight) or coefficient terms (source, (dx, dy, dz), weight, coef,
+    (cx, cy, cz)) applied in list order, in dtype (float32 or float64).  A 5-tuple with coef -1 is a plain term and is
+    kept as the 3-tuple."""
 
     def __init__(self, terms: Iterable[Sequence], dtype):
         out: List[Term] = []
         for t in terms:
-            s, o, w = t
+            if len(t) == 5 and int(t[3]) != -1:
+                s, o, w, k, c = t
+                out.append((int(s), (int(o[0]), int(o[1]), int(o[2])), float(w), int(k), (int(c[0]), int(c[1]), int(c[2]))))
+                continue
+            if len(t) == 5 and any(int(v) for v in t[4]):
+                raise _lib.StencilError(f"term {t!r}: a term without a coefficient field has coefficient offset (0, 0, 0)")
+            if len(t) not in (3, 5):
+                raise _lib.StencilError(f"term {t!r}: (source, offset, weight) or (source, offset, weight, coef, coef_offset)")
+            s, o, w = t[:3]
             out.append((int(s), (int(o[0]), int(o[1]), int(o[2])), float(w)))
         self.terms: Tuple[Term, ...] = tuple(out)
         self.dtype = np.dtype(dtype)
         self.dtype_code = _dtype_code(self.dtype)
         # the limits of a term list, whatever the domain: every ghost box at the largest radius
-        check(lib().sb_stencil_check(self.c_terms(), len(self.terms), I27(*([_lib.STENCIL_MAX_REACH] * 27))))
+        self._check(I27(*([_lib.STENCIL_MAX_REACH] * 27)))
+
+    def _check(self, r27) -> None:
+        if self.has_coef:
+            check(lib().sb_stencil_vcheck(self.c_vterms(), len(self.terms), r27))
+        else:
+            check(lib().sb_stencil_check(self.c_terms(), len(self.terms), r27))
 
     @staticmethod
     def laplacian(order: int, spacing: Sequence[float], dtype) -> "StencilOp":
@@ -55,22 +79,53 @@ class StencilOp:
         check(lib().sb_stencil_laplacian(int(order), h, buf, n))
         return StencilOp([(t.source, tuple(t.offset), t.weight) for t in buf], dtype)
 
+    @staticmethod
+    def div_grad(spacing: Sequence[float], dtype) -> "StencilOp":
+        """The conservative second-order div(kappa grad u) (sb_stencil_div_grad): 12 terms; coefficient field a holds
+        kappa on the faces normal to axis a, C_a(p) on the face between p - e_a and p."""
+        h = (C.c_double * 3)(*[float(v) for v in spacing])
+        n = check(lib().sb_stencil_div_grad(h, None, 0))
+        buf = (StencilVTerm * n)()
+        check(lib().sb_stencil_div_grad(h, buf, n))
+        return StencilOp([(t.source, tuple(t.offset), t.weight, t.coef, tuple(t.coef_offset)) for t in buf], dtype)
+
+    def scaled(self, f: float) -> "StencilOp":
+        """The same op with every weight multiplied by f (in double)."""
+        return StencilOp([(t[0], t[1], t[2] * float(f)) + tuple(t[3:]) for t in self.terms], self.dtype)
+
     def c_terms(self):
         arr = (StencilTerm * max(1, len(self.terms)))()
-        for k, (s, o, w) in enumerate(self.terms):
-            arr[k] = StencilTerm(s, (C.c_int32 * 3)(*o), w)
+        for k, t in enumerate(self.terms):
+            arr[k] = StencilTerm(t[0], (C.c_int32 * 3)(*t[1]), t[2])
+        return arr
+
+    def c_vterms(self):
+        arr = (StencilVTerm * max(1, len(self.terms)))()
+        for k, t in enumerate(self.terms):
+            coef, co = (t[3], t[4]) if len(t) == 5 else (-1, (0, 0, 0))
+            arr[k] = StencilVTerm(t[0], (C.c_int32 * 3)(*t[1]), coef, (C.c_int32 * 3)(*co), t[2])
         return arr
 
     @property
     def has_aux(self) -> bool:
-        return any(s == 1 for s, _, _ in self.terms)
+        return any(t[0] == 1 for t in self.terms)
+
+    @property
+    def has_coef(self) -> bool:
+        return any(len(t) == 5 for t in self.terms)
+
+    @property
+    def ncoef(self) -> int:
+        """The number of coefficient fields apply() takes: the highest field a term names, plus one (0: none)."""
+        return max([t[3] + 1 for t in self.terms if len(t) == 5] + [0])
 
     def reach(self) -> int:
-        return max(max(abs(c) for c in o) for _, o, _ in self.terms)
+        return max(max(abs(c) for c in t[1]) for t in self.terms)
 
     def check(self, radius) -> None:
-        """Raise StencilError unless a domain with this Radius exchanges every ghost cell the op reads."""
-        check(lib().sb_stencil_check(self.c_terms(), len(self.terms), radius.c27()))
+        """Raise StencilError unless a domain with this Radius exchanges every ghost cell the op reads (src cells and
+        coefficient cells alike)."""
+        self._check(radius.c27())
 
     def key(self) -> tuple:
         return (self.terms, self.dtype.str)
@@ -89,13 +144,20 @@ class StencilPlan:
     """sb_stencil_plan: the op over a list of boxes [lo, hi) (global coordinates) of three allocations of one subdomain."""
 
     def __init__(self, device: int, op: StencilOp, dst: Pitched, src: Pitched, aux: Pitched, acc_origin, zsize: int,
-                 boxes: Sequence[Tuple[Sequence[int], Sequence[int]]]):
+                 boxes: Sequence[Tuple[Sequence[int], Sequence[int]]], coefs: Optional[Sequence[Pitched]] = None):
+        """coefs: the coefficient allocations (sb_stencil_vplan_create), field k = coefs[k]; None for a plain op."""
         nb = len(boxes)
         lo = (C.c_int64 * (3 * max(1, nb)))(*[int(v) for b in boxes for v in b[0]])
         hi = (C.c_int64 * (3 * max(1, nb)))(*[int(v) for b in boxes for v in b[1]])
         h = C.c_void_p()
-        check(lib().sb_stencil_plan_create(C.byref(h), device, op.dtype_code, op.c_terms(), len(op.terms), dst, src, aux,
-                                           i3(acc_origin), int(zsize), nb, lo, hi))
+        if coefs is None and not op.has_coef:
+            check(lib().sb_stencil_plan_create(C.byref(h), device, op.dtype_code, op.c_terms(), len(op.terms), dst, src, aux,
+                                               i3(acc_origin), int(zsize), nb, lo, hi))
+        else:
+            cs = list(coefs or [])
+            carr = (Pitched * max(1, len(cs)))(*cs)
+            check(lib().sb_stencil_vplan_create(C.byref(h), device, op.dtype_code, op.c_vterms(), len(op.terms), dst, src, aux, carr,
+                                                len(cs), i3(acc_origin), int(zsize), nb, lo, hi))
         self._h = h
         self.device = device
         self.bytes = int(lib().sb_stencil_plan_bytes(h))
