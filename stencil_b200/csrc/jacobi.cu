@@ -1061,14 +1061,7 @@ int launch_jacobi(const JacobiParams &p_in, int dtype_size, cudaStream_t stream)
 
   static const int allow_shift = env_int("SB_JACOBI_SHIFT", 1);
   bool shift = false;
-  int vx = pick_vectors(p, dtype_size, allow_shift != 0, &shift);
-  // Unshifted rows: a vector that holds compute cells but hangs over the end of its row is replaced by a stand-in load
-  // (march_body, xin), which would feed wrong values to those cells.  Such a region (e.g. 30 floats with one ghost cell
-  // behind a 12-byte lead) takes the scalar path.  A vector that holds only the ghost cell is handled in march_body.
-  if (!shift && vx > 1 && p.x0a + ((p.hi[0] - 1 - p.x0a) / vx) * vx + vx > p.raw[0]) {
-    vx = 1;
-    p.x0a = p.lo[0];
-  }
+  const int vx = pick_vectors(p, dtype_size, allow_shift != 0, &shift);
   if (dtype_size == 8) {
     if (vx == 2) return shift ? launch_march<double, 2, true>(p, ry, mb, stream) : launch_march<double, 2, false>(p, ry, mb, stream);
     return launch_march<double, 1, false>(p, ry, mb, stream);
@@ -1082,6 +1075,10 @@ int launch_jacobi(const JacobiParams &p_in, int dtype_size, cudaStream_t stream)
 // of the allocation base: LocalDomain places the base so that the first COMPUTE cell is 16-byte aligned (the whole
 // compute region of 512 cells is then exactly 8 strips of 32 lanes x 2 doubles); any other common phase of src and dst
 // works as well.  Returns VX (1 = scalar fallback) and sets p.x0a; `shift` reports the alternating-phase case.
+// Unshifted rows: a vector that holds compute cells but hangs over the end of its row is replaced by a stand-in load
+// (march_body, xin), which would feed wrong values to those cells.  Such a region (e.g. 30 or 130 floats with one ghost
+// cell behind a 12-byte lead) takes the scalar path, in launch_jacobi and launch_jacobi_fused alike.  A vector that holds
+// only the ghost cell is handled in march_body (tail_lane), unless the lane before it is lane 0 of a strip (below).
 static int pick_vectors(JacobiParams &p, int dtype_size, bool allow_shift, bool *shift) {
   const unsigned long long s = (unsigned long long)(uintptr_t)p.src, d = (unsigned long long)(uintptr_t)p.dst;
   const int full = 16 / dtype_size;
@@ -1093,17 +1090,25 @@ static int pick_vectors(JacobiParams &p, int dtype_size, bool allow_shift, bool 
     p.x0a = p.lo[0] - r;
     return vx;
   };
+  int vx;
   if (p.pitch % 16 == 0 && p.slice % 16 == 0 && (s & 15) == (d & 15) && (s & 15) % dtype_size == 0) {
     // with a non-zero phase the first vector may start before x = 0: still inside the (256-byte aligned) allocation,
     // whose first `phase` bytes are the lead pad
-    return origin(full, unsigned(s & 15));
-  }
-  if (allow_shift && (s & 15) == 0 && (d & 15) == 0 && p.slice % 16 == 0 && p.pitch % 16 == 8) {
+    vx = origin(full, unsigned(s & 15));
+  } else if (allow_shift && (s & 15) == 0 && (d & 15) == 0 && p.slice % 16 == 0 && p.pitch % 16 == 8) {
     *shift = true;
-    return origin(full, 0);
+    return origin(full, 0); // (shifted rows may hang over either end of a row: march_body xin)
+  } else if (dtype_size == 4 && ((s | d | (unsigned long long)p.pitch | (unsigned long long)p.slice) % 8 == 0)) {
+    vx = origin(2, 0);
+  } else {
+    return origin(1, 0);
   }
-  if (dtype_size == 4 && ((s | d | (unsigned long long)p.pitch | (unsigned long long)p.slice) % 8 == 0)) return origin(2, 0);
-  return origin(1, 0);
+  const int last = p.x0a + ((p.hi[0] - 1 - p.x0a) / vx) * vx; // first cell of the last vector holding compute cells
+  if (last + vx > p.raw[0]) return origin(1, 0);               // the overhang above
+  // march_body's tail_lane takes the ghost cell as the right neighbour through the lane's one edge scalar; lane 0 of a strip
+  // needs that scalar for its left neighbour (e.g. 66 or 130 doubles with one ghost cell behind an 8-byte lead)
+  if (last + vx == p.hi[0] && last + 2 * vx > p.raw[0] && (last - p.x0a) / vx % 32 == 0) return origin(1, 0);
+  return vx;
 }
 
 int launch_jacobi_fused(const JacobiParams &p_in, const FusedSync &sync_in, int dtype_size, cudaStream_t stream) {
