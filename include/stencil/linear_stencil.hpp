@@ -91,6 +91,82 @@ public:
   }
 };
 
+// A system (DESIGN.md section 2.8): terms (output, input, offset, weight), each of which may also read an input as its
+// coefficient at an offset of reach 1, over nin() inputs and nout() outputs; each output sums its own terms in list order
+// by the operator rule.  One launch per box computes every output.
+//
+//     // E = E + (dt / eps) curl- H in place: inputs Hx, Hy, Hz, Ex, Ey, Ez; outputs Ex, Ey, Ez
+//     stencil::LinearSystem e = stencil::LinearSystem().add(0, 3, 0, 0, 0, 1.0).add(1, 4, 0, 0, 0, 1.0).add(2, 5, 0, 0, 0, 1.0) +
+//                               stencil::LinearSystem::curl(-1, h, h, h).scaled(dt / eps);
+//     dd.apply(e, {curr(ex), curr(ey), curr(ez)}, {curr(hx), curr(hy), curr(hz), curr(ex), curr(ey), curr(ez)});
+class LinearSystem {
+  std::vector<sb_stencil_sys_term> terms_;
+  int nin_ = 0, nout_ = 0;
+
+  template <typename Fn> static LinearSystem table(Fn fn, const char *name, int stagger, double hx, double hy, double hz) {
+    const double h[3] = {hx, hy, hz};
+    const int n = fn(stagger, h, nullptr, 0);
+    if (n < 0) LOG_FATAL("LinearSystem::" << name << ": " << sb_last_error());
+    std::vector<sb_stencil_sys_term> terms(static_cast<size_t>(n));
+    fn(stagger, h, terms.data(), n);
+    LinearSystem s;
+    for (const sb_stencil_sys_term &t : terms) s.push(t);
+    return s;
+  }
+  void push(const sb_stencil_sys_term &t) {
+    terms_.push_back(t);
+    nout_ = t.output + 1 > nout_ ? t.output + 1 : nout_;
+    nin_ = t.input + 1 > nin_ ? t.input + 1 : nin_;
+    nin_ = t.coef + 1 > nin_ ? t.coef + 1 : nin_;
+  }
+
+public:
+  LinearSystem &add(int out, int in, int dx, int dy, int dz, double w) {
+    push(sb_stencil_sys_term{out, in, {dx, dy, dz}, -1, {0, 0, 0}, w});
+    return *this;
+  }
+  // a coefficient term: also reads input coef (-1: none) at (cx, cy, cz)
+  LinearSystem &add(int out, int in, int dx, int dy, int dz, double w, int coef, int cx, int cy, int cz) {
+    push(sb_stencil_sys_term{out, in, {dx, dy, dz}, coef, {cx, cy, cz}, w});
+    return *this;
+  }
+  // every weight multiplied by f (in double)
+  LinearSystem scaled(double f) const {
+    LinearSystem out(*this);
+    for (sb_stencil_sys_term &t : out.terms_) t.weight *= f;
+    return out;
+  }
+  // the same system reading inputs input_base + i (coefficients included) and writing outputs output_base + j
+  LinearSystem shifted(int input_base, int output_base) const {
+    LinearSystem out;
+    for (sb_stencil_sys_term t : terms_) {
+      t.output += output_base;
+      t.input += input_base;
+      if (t.coef >= 0) t.coef += input_base;
+      out.push(t);
+    }
+    out.nin_ = nin_ + input_base > out.nin_ ? nin_ + input_base : out.nin_;
+    out.nout_ = nout_ + output_base > out.nout_ ? nout_ + output_base : out.nout_;
+    return out;
+  }
+  // concatenation: this system's terms, then o's
+  LinearSystem operator+(const LinearSystem &o) const {
+    LinearSystem out(*this);
+    for (const sb_stencil_sys_term &t : o.terms_) out.push(t);
+    out.nin_ = o.nin_ > out.nin_ ? o.nin_ : out.nin_;
+    out.nout_ = o.nout_ > out.nout_ ? o.nout_ : out.nout_;
+    return out;
+  }
+  // difference tables (sb_stencil_grad / div / curl): stagger +1 forward, -1 backward, 0 central
+  static LinearSystem grad(int stagger, double hx, double hy, double hz) { return table(sb_stencil_grad, "grad", stagger, hx, hy, hz); }
+  static LinearSystem div(int stagger, double hx, double hy, double hz) { return table(sb_stencil_div, "div", stagger, hx, hy, hz); }
+  static LinearSystem curl(int stagger, double hx, double hy, double hz) { return table(sb_stencil_curl, "curl", stagger, hx, hy, hz); }
+
+  const std::vector<sb_stencil_sys_term> &terms() const noexcept { return terms_; }
+  int nin() const noexcept { return nin_; }
+  int nout() const noexcept { return nout_; }
+};
+
 // A buffer of a quantity for DistributedDomain::apply: its curr or next allocation.
 template <typename T> struct Buffer {
   DataHandle<T> h;

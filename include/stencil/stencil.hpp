@@ -10,9 +10,11 @@
 #include <cassert>
 #include <cstdlib>
 #include <fstream>
+#include <functional>
 #include <map>
 #include <set>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include <mpi.h>
@@ -132,6 +134,13 @@ private:
   void destroy_stencil_plans();
   void apply_op(const stencil::LinearStencil &op, int dtype, size_t dq, stencil::Which dw, size_t sq, int64_t aq, stencil::Which aw,
                 const std::vector<size_t> &cq, bool exchange);
+  void apply_sys(const stencil::LinearSystem &sys, int dtype, const std::vector<std::pair<size_t, stencil::Which>> &outs,
+                 const std::vector<std::pair<size_t, stencil::Which>> &ins, bool exchange);
+  // the schedule apply_op and apply_sys share: the cached per-domain plans of key (built by make(domain, boxes) on first
+  // use), then the interior plans on their own streams while exchange() runs and the exterior plans after it, or the one
+  // whole-region plan per domain; returns when every launch is complete
+  void run_stencil_plans(const std::vector<int64_t> &key, bool exchange,
+                         const std::function<sb_stencil_plan *(size_t, const std::vector<Rect3> &)> &make);
 
   std::string outputPrefix_;
 
@@ -287,6 +296,19 @@ public:
   void apply(const stencil::LinearStencil &op, const stencil::Buffer<T> &dst, const DataHandle<T> &src, const stencil::Buffer<T> &aux,
              const std::vector<DataHandle<T>> &coefs, bool exchange = true) {
     apply_op(op, stencil::bc_dtype<T>(), dst.h.id(), dst.which, src.id(), int64_t(aux.h.id()), aux.which, ids_of(coefs), exchange);
+  }
+  // outputs = sys(inputs) over the whole compute region of every local subdomain (DESIGN.md section 2.8): sys.nout()
+  // outputs and sys.nin() inputs, each the curr or next buffer of a quantity of the system's type.  An input read at a
+  // non-zero offset must be a curr buffer (the one exchange() fills); outputs are pairwise distinct; an output may be an
+  // input only if every read of that input is at offset 0 (an in-place update).  Schedule, plan cache and failure rules
+  // are the operator apply's.
+  template <typename T>
+  void apply(const stencil::LinearSystem &sys, const std::vector<stencil::Buffer<T>> &outputs, const std::vector<stencil::Buffer<T>> &inputs,
+             bool exchange = true) {
+    std::vector<std::pair<size_t, stencil::Which>> o, i;
+    for (const stencil::Buffer<T> &b : outputs) o.emplace_back(b.h.id(), b.which);
+    for (const stencil::Buffer<T> &b : inputs) i.emplace_back(b.h.id(), b.which);
+    apply_sys(sys, stencil::bc_dtype<T>(), o, i, exchange);
   }
   template <typename T> static std::vector<size_t> ids_of(const std::vector<DataHandle<T>> &hs) {
     std::vector<size_t> ids;

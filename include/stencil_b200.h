@@ -356,6 +356,60 @@ int sb_stencil_vplan_create(sb_stencil_plan **out, int device, int dtype, const 
                             int64_t zsize, int nbox, const int64_t *lo, const int64_t *hi);
 
 /* ---------------------------------------------------------------------------------------------
+ * Linear stencil systems: one launch over nin input and nout output allocations.  A term of output j reads input
+ * `input` at p + o (|o_a| <= SB_STENCIL_MAX_REACH) and, if coef >= 0, input `coef` at p + c (|c_a| <=
+ * SB_STENCIL_COEF_REACH) as its coefficient.  For each output j, over the terms with output == j in list order (terms of
+ * different outputs may interleave), in T with every multiply and add rounded separately (no FMA contraction):
+ *   coefficient term  m = (T(w) * I_coef(p + c)) * I_in(p + o)
+ *   plain term        m = T(w) * I_in(p + o)
+ *   acc = m_first;  acc = acc + m for each later term;  O_j[p] = acc
+ * A system with one output, src as input 0, aux as input 1 and coefficient field k as input 2 + k gives the bits of
+ * sb_stencil_vplan_create.  Aliasing: outputs are pairwise distinct buffers; an output may be an input only if every
+ * read of that input (as a source or a coefficient, by any output's terms) is at offset 0; every read of a cell happens
+ * before any output of that cell is written.  An input no term reads may be NULL; it is neither checked nor counted.
+ * ------------------------------------------------------------------------------------------- */
+#define SB_STENCIL_SYS_MAX_INPUTS 8
+#define SB_STENCIL_SYS_MAX_OUTPUTS 4
+#define SB_STENCIL_SYS_MAX_TERMS 128
+typedef struct sb_stencil_sys_term {
+  int32_t output;         /* 0 .. nout-1 */
+  int32_t input;          /* the source read: 0 .. nin-1 */
+  int32_t offset[3];      /* |o_a| <= SB_STENCIL_MAX_REACH */
+  int32_t coef;           /* an input read as coefficient, or -1 */
+  int32_t coef_offset[3]; /* |c_a| <= SB_STENCIL_COEF_REACH; (0,0,0) when coef = -1 */
+  double weight;
+} sb_stencil_sys_term;
+
+/* Host only.  The limits (1 .. SB_STENCIL_SYS_MAX_TERMS terms, 1 .. 8 inputs, 1 .. 4 outputs, indices in range, the
+ * offset limits above) and the reach test of sb_stencil_check on every source and coefficient offset. */
+int sb_stencil_sys_check(const sb_stencil_sys_term *terms, int n, int nin, int nout, const int64_t radius27[27]);
+/* Host only.  Difference tables on a grid of spacing[3] (weights in double).  stagger +1: forward, D_a u = (u(p + e_a) -
+ * u(p)) / h_a, terms (+e_a, 1/h_a) then (0, -1/h_a); -1: backward, (0, 1/h_a) then (-e_a, -1/h_a); 0: central,
+ * (+e_a, 0.5/h_a) then (-e_a, -0.5/h_a).
+ *   grad: input 0 -> outputs 0, 1, 2 (D_x, D_y, D_z); 6 terms
+ *   div:  inputs 0, 1, 2 -> output 0 (D_x in 0 + D_y in 1 + D_z in 2, in that order); 6 terms
+ *   curl: output 0 = D_y in 2 - D_z in 1, output 1 = D_z in 0 - D_x in 2, output 2 = D_x in 1 - D_y in 0, the positive
+ *         part first; 12 terms
+ * Each writes at most cap terms (out may be NULL with cap 0) and returns the term count, or SB_ERR_INVALID for a
+ * stagger outside -1 .. 1 or a spacing that is not finite and > 0.  A forward curl for H and a backward curl for E are
+ * the Yee scheme (DESIGN.md section 2.8). */
+int sb_stencil_grad(int stagger, const double spacing[3], sb_stencil_sys_term *out, int cap);
+int sb_stencil_div(int stagger, const double spacing[3], sb_stencil_sys_term *out, int cap);
+int sb_stencil_curl(int stagger, const double spacing[3], sb_stencil_sys_term *out, int cap);
+/* A persistent plan of the system over nbox boxes [lo, hi) (global coordinates; acc_origin as for sb_stencil_plan_create)
+ * of nout outputs[] and nin inputs[] that share pitch, row count and zsize.  Boxes of at least 8 cells on every axis go
+ * to the z-marching tile kernel, one launch each; thinner boxes share one-thread-per-cell launches.  Launch, bytes (per
+ * cell one element read of each input a term reads and one written per output) and destroy through sb_stencil_plan_*.
+ * Errors (SB_ERR_INVALID with a message, checked before anything is allocated): an unknown dtype, an invalid term list,
+ * an output without terms, a NULL output or read input, two equal outputs, an output that is an input read at a
+ * non-zero offset, mismatched pitches or row counts, a pointer or pitch that is not a multiple of the element size,
+ * lo > hi, a box whose reads leave an allocation, and a system whose tile kernel needs more shared memory than the
+ * device allows a block. */
+int sb_stencil_sys_plan_create(sb_stencil_plan **out, int device, int dtype, const sb_stencil_sys_term *terms, int n,
+                               const sb_pitched *outputs, int nout, const sb_pitched *inputs, int nin,
+                               const int64_t acc_origin[3], int64_t zsize, int nbox, const int64_t *lo, const int64_t *hi);
+
+/* ---------------------------------------------------------------------------------------------
  * 7-point jacobi step (the reference's user kernel, bin/jacobi3d.cu:40-85) over a region.
  * dtype_size 4 = float, 8 = double.  acc_origin = global coordinate of allocation element (0,0,0)
  * (Accessor origin, include/stencil/local_domain.cuh:153-173).  [lo,hi) = region to update,

@@ -678,35 +678,99 @@ void DistributedDomain::apply_op(const stencil::LinearStencil &op, int dtype, si
     std::memcpy(&wbits, &t.weight, 8);
     key.insert(key.end(), {t.source, t.offset[0], t.offset[1], t.offset[2], t.coef, t.coef_offset[0], t.coef_offset[1], t.coef_offset[2], wbits});
   }
+  run_stencil_plans(key, exchange, [&](size_t di, const std::vector<Rect3> &boxes) {
+    LocalDomain &d = domains_[di];
+    const sb_pitched dst = as_sb(dw == Which::curr ? d.curr_data(dq) : d.next_data(dq)), src = as_sb(d.curr_data(sq));
+    const sb_pitched aux = aq < 0 ? sb_pitched{nullptr, 0, 0} : as_sb(aw == Which::curr ? d.curr_data(size_t(aq)) : d.next_data(size_t(aq)));
+    std::vector<sb_pitched> coef;
+    for (const size_t q : cq) coef.push_back(as_sb(d.curr_data(q)));
+    int64_t acc[3];
+    set3(acc, d.origin() - Dim3(radius_.x(-1), radius_.y(-1), radius_.z(-1)));
+    std::vector<int64_t> lo, hi;
+    for (const Rect3 &b : boxes) {
+      lo.insert(lo.end(), {b.lo.x, b.lo.y, b.lo.z});
+      hi.insert(hi.end(), {b.hi.x, b.hi.y, b.hi.z});
+    }
+    sb_stencil_plan *p = nullptr;
+    if (SB_OK != sb_stencil_vplan_create(&p, d.gpu(), dtype, terms.data(), int(terms.size()), dst, src, aux, coef.data(), int(coef.size()), acc,
+                                         d.raw_size().z, int(boxes.size()), lo.data(), hi.data()))
+      LOG_FATAL("apply: " << sb_last_error());
+    return p;
+  });
+}
+
+void DistributedDomain::apply_sys(const stencil::LinearSystem &sys, int dtype, const std::vector<std::pair<size_t, stencil::Which>> &outs,
+                                  const std::vector<std::pair<size_t, stencil::Which>> &ins, bool exchange) {
+  using stencil::Which;
+  if (domains_.empty() || plans_[0].size() != domains_.size()) LOG_FATAL("apply: call realize() first");
+  if (dtype != SB_DTYPE_F32 && dtype != SB_DTYPE_F64) LOG_FATAL("apply: a stencil system computes in float or double");
+  if (int(outs.size()) != sys.nout() || int(ins.size()) != sys.nin())
+    LOG_FATAL("apply: the system has " << sys.nin() << " inputs and " << sys.nout() << " outputs, but " << ins.size() << " inputs and "
+                                       << outs.size() << " outputs were given");
+  for (const auto *v : {&outs, &ins})
+    for (const auto &b : *v)
+      if (b.first >= dataDtype_.size() || dataDtype_[b.first] != dtype) LOG_FATAL("apply: unknown data handle or type for " << b.first);
+  const std::vector<sb_stencil_sys_term> &terms = sys.terms();
+  std::vector<bool> moved(ins.size(), false);
+  for (const sb_stencil_sys_term &t : terms) {
+    if (t.input >= 0 && size_t(t.input) < ins.size() && (t.offset[0] || t.offset[1] || t.offset[2])) moved[size_t(t.input)] = true;
+    if (t.coef >= 0 && size_t(t.coef) < ins.size() && (t.coef_offset[0] || t.coef_offset[1] || t.coef_offset[2])) moved[size_t(t.coef)] = true;
+  }
+  for (size_t i = 0; i < ins.size(); ++i)
+    if (moved[i] && ins[i].second != Which::curr)
+      LOG_FATAL("apply: input " << i << " is read at a non-zero offset, so it must be a curr buffer (the one exchange() fills)");
+  for (size_t j = 0; j < outs.size(); ++j) {
+    for (size_t k = 0; k < j; ++k)
+      if (outs[k] == outs[j]) LOG_FATAL("apply: outputs " << k << " and " << j << " are the same buffer");
+    for (size_t i = 0; i < ins.size(); ++i)
+      if (moved[i] && ins[i] == outs[j]) LOG_FATAL("apply: output " << j << " is input " << i << ", which is read at a non-zero offset");
+  }
+  int64_t r27[27];
+  for (int z = -1, i = 0; z <= 1; ++z)
+    for (int y = -1; y <= 1; ++y)
+      for (int x = -1; x <= 1; ++x) r27[i++] = int64_t(radius_.dir(x, y, z));
+  if (SB_OK != sb_stencil_sys_check(terms.data(), int(terms.size()), sys.nin(), sys.nout(), r27)) LOG_FATAL("apply: " << sb_last_error());
+  // -1 first: a system's key never equals an operator's, whose first entry is a dtype code
+  std::vector<int64_t> key = {-1, dtype, int64_t(exchange), parity_, sys.nin(), sys.nout()};
+  for (const auto *v : {&outs, &ins})
+    for (const auto &b : *v) key.insert(key.end(), {int64_t(b.first), int64_t(b.second == Which::next)});
+  for (const sb_stencil_sys_term &t : terms) {
+    int64_t wbits;
+    std::memcpy(&wbits, &t.weight, 8);
+    key.insert(key.end(), {t.output, t.input, t.offset[0], t.offset[1], t.offset[2], t.coef, t.coef_offset[0], t.coef_offset[1], t.coef_offset[2], wbits});
+  }
+  run_stencil_plans(key, exchange, [&](size_t di, const std::vector<Rect3> &boxes) {
+    LocalDomain &d = domains_[di];
+    std::vector<sb_pitched> o, i;
+    for (const auto &b : outs) o.push_back(as_sb(b.second == Which::curr ? d.curr_data(b.first) : d.next_data(b.first)));
+    for (const auto &b : ins) i.push_back(as_sb(b.second == Which::curr ? d.curr_data(b.first) : d.next_data(b.first)));
+    int64_t acc[3];
+    set3(acc, d.origin() - Dim3(radius_.x(-1), radius_.y(-1), radius_.z(-1)));
+    std::vector<int64_t> lo, hi;
+    for (const Rect3 &b : boxes) {
+      lo.insert(lo.end(), {b.lo.x, b.lo.y, b.lo.z});
+      hi.insert(hi.end(), {b.hi.x, b.hi.y, b.hi.z});
+    }
+    sb_stencil_plan *p = nullptr;
+    if (SB_OK != sb_stencil_sys_plan_create(&p, d.gpu(), dtype, terms.data(), int(terms.size()), o.data(), int(o.size()), i.data(), int(i.size()),
+                                            acc, d.raw_size().z, int(boxes.size()), lo.data(), hi.data()))
+      LOG_FATAL("apply: " << sb_last_error());
+    return p;
+  });
+}
+
+void DistributedDomain::run_stencil_plans(const std::vector<int64_t> &key, bool exchange,
+                                          const std::function<sb_stencil_plan *(size_t, const std::vector<Rect3> &)> &make) {
   auto found = stencilPlans_.find(key);
   if (found == stencilPlans_.end()) {
     const std::vector<Rect3> interiors = exchange ? get_interior() : std::vector<Rect3>();
     const std::vector<std::vector<Rect3>> exteriors = exchange ? get_exterior() : std::vector<std::vector<Rect3>>();
     std::vector<std::vector<sb_stencil_plan *>> per_dom;
     for (size_t di = 0; di < domains_.size(); ++di) {
-      LocalDomain &d = domains_[di];
-      const sb_pitched dst = as_sb(dw == Which::curr ? d.curr_data(dq) : d.next_data(dq)), src = as_sb(d.curr_data(sq));
-      const sb_pitched aux = aq < 0 ? sb_pitched{nullptr, 0, 0} : as_sb(aw == Which::curr ? d.curr_data(size_t(aq)) : d.next_data(size_t(aq)));
-      std::vector<sb_pitched> coef;
-      for (const size_t q : cq) coef.push_back(as_sb(d.curr_data(q)));
-      int64_t acc[3];
-      set3(acc, d.origin() - Dim3(radius_.x(-1), radius_.y(-1), radius_.z(-1)));
-      auto make = [&](const std::vector<Rect3> &boxes) {
-        std::vector<int64_t> lo, hi;
-        for (const Rect3 &b : boxes) {
-          lo.insert(lo.end(), {b.lo.x, b.lo.y, b.lo.z});
-          hi.insert(hi.end(), {b.hi.x, b.hi.y, b.hi.z});
-        }
-        sb_stencil_plan *p = nullptr;
-        if (SB_OK != sb_stencil_vplan_create(&p, d.gpu(), dtype, terms.data(), int(terms.size()), dst, src, aux, coef.data(), int(coef.size()),
-                                             acc, d.raw_size().z, int(boxes.size()), lo.data(), hi.data()))
-          LOG_FATAL("apply: " << sb_last_error());
-        return p;
-      };
       if (exchange)
-        per_dom.push_back({make({interiors[di]}), make(exteriors[di])});
+        per_dom.push_back({make(di, {interiors[di]}), make(di, exteriors[di])});
       else
-        per_dom.push_back({make({d.get_compute_region()})});
+        per_dom.push_back({make(di, {domains_[di].get_compute_region()})});
     }
     found = stencilPlans_.emplace(key, std::move(per_dom)).first;
   }

@@ -33,6 +33,6 @@ from .domain import (  # noqa: F401
     raw_size,
     reduce_combine,
 )
-from .stencil_op import StencilOp, StencilPlan  # noqa: F401
+from .stencil_op import StencilOp, StencilPlan, StencilSystem, SystemPlan  # noqa: F401
 
 __all__ = [n for n in dir() if not n.startswith("_")]

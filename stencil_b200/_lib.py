@@ -132,6 +132,17 @@ class StencilVTerm(C.Structure):
 
 STENCIL_MAX_COEFS, STENCIL_COEF_REACH = 4, 1  # SB_STENCIL_MAX_COEFS, SB_STENCIL_COEF_REACH
 
+
+class StencilSysTerm(C.Structure):
+    """sb_stencil_sys_term: a term of a system: output, input read at offset, coefficient input (-1: none) at coef_offset."""
+
+    _fields_ = [("output", C.c_int32), ("input", C.c_int32), ("offset", C.c_int32 * 3), ("coef", C.c_int32), ("coef_offset", C.c_int32 * 3),
+                ("weight", C.c_double)]
+
+
+# SB_STENCIL_SYS_MAX_INPUTS, SB_STENCIL_SYS_MAX_OUTPUTS, SB_STENCIL_SYS_MAX_TERMS
+STENCIL_SYS_MAX_INPUTS, STENCIL_SYS_MAX_OUTPUTS, STENCIL_SYS_MAX_TERMS = 8, 4, 128
+
 I6 = C.c_int32 * 6
 
 FUSED_MAX_GROUPS = 4096  # SB_FUSED_MAX_GROUPS
@@ -191,6 +202,15 @@ _SIGS = {
     "sb_stencil_vplan_create": (
         C.c_int,
         [C.POINTER(C.c_void_p), C.c_int, C.c_int, C.POINTER(StencilVTerm), C.c_int, Pitched, Pitched, Pitched, C.POINTER(Pitched), C.c_int,
+         I3, C.c_int64, C.c_int, C.POINTER(C.c_int64), C.POINTER(C.c_int64)],
+    ),
+    "sb_stencil_sys_check": (C.c_int, [C.POINTER(StencilSysTerm), C.c_int, C.c_int, C.c_int, I27]),
+    "sb_stencil_grad": (C.c_int, [C.c_int, C.c_double * 3, C.POINTER(StencilSysTerm), C.c_int]),
+    "sb_stencil_div": (C.c_int, [C.c_int, C.c_double * 3, C.POINTER(StencilSysTerm), C.c_int]),
+    "sb_stencil_curl": (C.c_int, [C.c_int, C.c_double * 3, C.POINTER(StencilSysTerm), C.c_int]),
+    "sb_stencil_sys_plan_create": (
+        C.c_int,
+        [C.POINTER(C.c_void_p), C.c_int, C.c_int, C.POINTER(StencilSysTerm), C.c_int, C.POINTER(Pitched), C.c_int, C.POINTER(Pitched), C.c_int,
          I3, C.c_int64, C.c_int, C.POINTER(C.c_int64), C.POINTER(C.c_int64)],
     ),
     "sb_stencil_plan_launch": (C.c_int, [C.c_void_p, C.c_void_p]),

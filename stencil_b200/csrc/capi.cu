@@ -22,6 +22,7 @@
 #include "astaroth.cuh"
 #include "jacobi.cuh"
 #include "stencil_op.cuh"
+#include "stencil_sys.cuh"
 
 #include "stencil/exchange_plan.hpp"
 #include "stencil/geometry.hpp"
@@ -561,6 +562,11 @@ struct sb_stencil_plan {
   std::vector<int> tile_grids;
   std::vector<sb::OpVCellParams> cells; // one cell-kernel launch per group of thin boxes
   std::vector<int> cell_grids;
+  std::vector<sb::SysTileParams> sys_tiles; // a system (sb_stencil_sys_plan_create): one tile launch per thick box
+  std::vector<int> sys_tile_grids;
+  size_t sys_smem = 0;
+  std::vector<sb::SysCellParams> sys_cells;
+  std::vector<int> sys_cell_grids;
   int64_t bytes = 0;
 };
 
@@ -1328,29 +1334,52 @@ int sb_reduce_combine(const sb_reduce_result *parts, int64_t n, sb_reduce_result
 // ----------------------------------------------------------------------------------------- linear stencil operators
 // The limits every term list obeys, whatever the domain: n, sources, |o_a| <= 4, aux terms without offset, coefficient
 // fields 0 .. 3 (or -1) read within reach 1, plain terms without a coefficient offset.
+// |o_a| <= 4 for the source offset of term t (operators and systems alike)
+static int stencil_offset_ok(int t, const int32_t o[3]) {
+  for (int a = 0; a < 3; ++a)
+    if (o[a] < -SB_STENCIL_MAX_REACH || o[a] > SB_STENCIL_MAX_REACH)
+      return fail(SB_ERR_INVALID, "term %d: offset (%d, %d, %d) reaches beyond %d cells", t, int(o[0]), int(o[1]), int(o[2]),
+                  SB_STENCIL_MAX_REACH);
+  return SB_OK;
+}
+
+// The coefficient of term t (operators and systems alike): -1 or 0 .. ncoef - 1 (what: "field" or "input"), read within
+// reach 1, and no coefficient offset without a coefficient.
+static int stencil_coef_ok(int t, int32_t coef, const int32_t c[3], int ncoef, const char *what) {
+  if (coef < -1 || coef >= ncoef) return fail(SB_ERR_INVALID, "term %d: coefficient %s %d must be -1 (none) or 0 .. %d", t, what, int(coef), ncoef - 1);
+  if (coef == -1 && (c[0] || c[1] || c[2]))
+    return fail(SB_ERR_INVALID, "term %d: a term without a coefficient field has coefficient offset (0, 0, 0), not (%d, %d, %d)", t,
+                int(c[0]), int(c[1]), int(c[2]));
+  for (int a = 0; a < 3; ++a)
+    if (c[a] < -SB_STENCIL_COEF_REACH || c[a] > SB_STENCIL_COEF_REACH)
+      return fail(SB_ERR_INVALID, "term %d: coefficient offset (%d, %d, %d) reaches beyond %d cell", t, int(c[0]), int(c[1]), int(c[2]),
+                  SB_STENCIL_COEF_REACH);
+  return SB_OK;
+}
+
 static int stencil_terms_ok(const sb_stencil_vterm *terms, int n) {
   if (!terms || n < 1 || n > SB_STENCIL_MAX_TERMS) return fail(SB_ERR_INVALID, "an op has 1 to %d terms, not %d", SB_STENCIL_MAX_TERMS, terms ? n : 0);
   for (int t = 0; t < n; ++t) {
     const sb_stencil_vterm &T = terms[t];
     if (T.source != 0 && T.source != 1) return fail(SB_ERR_INVALID, "term %d: source %d must be 0 (src) or 1 (aux)", t, int(T.source));
-    for (int a = 0; a < 3; ++a)
-      if (T.offset[a] < -SB_STENCIL_MAX_REACH || T.offset[a] > SB_STENCIL_MAX_REACH)
-        return fail(SB_ERR_INVALID, "term %d: offset (%d, %d, %d) reaches beyond %d cells", t, int(T.offset[0]), int(T.offset[1]),
-                    int(T.offset[2]), SB_STENCIL_MAX_REACH);
+    int rc = stencil_offset_ok(t, T.offset);
+    if (rc != SB_OK) return rc;
     if (T.source == 1 && (T.offset[0] || T.offset[1] || T.offset[2]))
       return fail(SB_ERR_INVALID, "term %d: an aux term has offset (0, 0, 0), not (%d, %d, %d)", t, int(T.offset[0]), int(T.offset[1]),
                   int(T.offset[2]));
-    if (T.coef < -1 || T.coef >= SB_STENCIL_MAX_COEFS)
-      return fail(SB_ERR_INVALID, "term %d: coefficient field %d must be -1 (none) or 0 .. %d", t, int(T.coef), SB_STENCIL_MAX_COEFS - 1);
-    const int32_t *c = T.coef_offset;
-    if (T.coef == -1 && (c[0] || c[1] || c[2]))
-      return fail(SB_ERR_INVALID, "term %d: a term without a coefficient field has coefficient offset (0, 0, 0), not (%d, %d, %d)", t,
-                  int(c[0]), int(c[1]), int(c[2]));
-    for (int a = 0; a < 3; ++a)
-      if (c[a] < -SB_STENCIL_COEF_REACH || c[a] > SB_STENCIL_COEF_REACH)
-        return fail(SB_ERR_INVALID, "term %d: coefficient offset (%d, %d, %d) reaches beyond %d cell", t, int(c[0]), int(c[1]), int(c[2]),
-                    SB_STENCIL_COEF_REACH);
+    if ((rc = stencil_coef_ok(t, T.coef, T.coef_offset, SB_STENCIL_MAX_COEFS, "field")) != SB_OK) return rc;
   }
+  return SB_OK;
+}
+
+// Whether box b (allocation-relative lo l, extent e), read rm cells below and rp above on each axis, stays inside an
+// allocation of size[3]; who: what reads ("the op reads", "input 2 is read at", ...).
+static int stencil_box_reads_ok(int b, const int64_t l[3], const int64_t e[3], const int rm[3], const int rp[3], const int64_t size[3],
+                                const std::string &who) {
+  for (int a = 0; a < 3; ++a)
+    if (l[a] - rm[a] < 0 || l[a] + e[a] + rp[a] > size[a])
+      return fail(SB_ERR_INVALID, "box %d: %s cells %lld .. %lld on axis %c, outside the allocation's 0 .. %lld", b, who.c_str(),
+                  (long long)(l[a] - rm[a]), (long long)(l[a] + e[a] + rp[a] - 1), "xyz"[a], (long long)(size[a] - 1));
   return SB_OK;
 }
 
@@ -1371,6 +1400,20 @@ static int stencil_offset_in_reach(int t, const char *what, const int32_t o[3], 
     if (int64_t(o[a] < 0 ? -o[a] : o[a]) > face)
       return fail(SB_ERR_INVALID, "term %d: %s (%d, %d, %d) reaches %d cells on side %c%c, whose face radius is %lld", t, what,
                   int(o[0]), int(o[1]), int(o[2]), int(o[a] < 0 ? -o[a] : o[a]), s[a] < 0 ? '-' : '+', "xyz"[a], (long long)face);
+  }
+  return SB_OK;
+}
+
+// Every buffer shares ref's pitch and row count (ref_name: what ref is called), and its pointer and pitch are positive
+// multiples of the es-byte element.
+static int stencil_buffers_ok(const std::vector<const sb_pitched *> &bufs, const std::vector<std::string> &names, const sb_pitched &ref,
+                              const char *ref_name, int es) {
+  for (size_t b = 0; b < bufs.size(); ++b) {
+    const sb_pitched &P = *bufs[b];
+    if (P.pitch != ref.pitch || P.ysize != ref.ysize)
+      return fail(SB_ERR_INVALID, "%s has another pitch or row count than %s", names[b].c_str(), ref_name);
+    if ((uintptr_t(P.ptr) % uintptr_t(es)) || P.pitch <= 0 || (P.pitch % es) || P.ysize <= 0)
+      return fail(SB_ERR_INVALID, "%s: pointer and pitch must be positive multiples of the %d-byte element", names[b].c_str(), es);
   }
   return SB_OK;
 }
@@ -1522,12 +1565,7 @@ int sb_stencil_vplan_create(sb_stencil_plan **out, int device, int dtype, const 
     bufs.push_back(&coef[fsrc[f]]);
     names.push_back("coefficient field " + std::to_string(fsrc[f]));
   }
-  for (size_t b = 0; b < bufs.size(); ++b) {
-    const sb_pitched &P = *bufs[b];
-    if (P.pitch != src.pitch || P.ysize != src.ysize) return fail(SB_ERR_INVALID, "%s has another pitch or row count than src", names[b].c_str());
-    if ((uintptr_t(P.ptr) % uintptr_t(es)) || P.pitch <= 0 || (P.pitch % es) || P.ysize <= 0)
-      return fail(SB_ERR_INVALID, "%s: pointer and pitch must be positive multiples of the %d-byte element", names[b].c_str(), es);
-  }
+  if ((rc = stencil_buffers_ok(bufs, names, src, "src", es)) != SB_OK) return rc;
   if (!acc_origin || zsize < 1) return fail(SB_ERR_INVALID, "sb_stencil_plan_create needs acc_origin and zsize >= 1");
   if (nbox < 0 || (nbox > 0 && (!lo || !hi))) return fail(SB_ERR_INVALID, "nbox %d: needs nbox >= 0 and lo / hi arrays", nbox);
   const int64_t size[3] = {src.pitch / es, src.ysize, zsize};
@@ -1543,15 +1581,10 @@ int sb_stencil_vplan_create(sb_stencil_plan **out, int device, int dtype, const 
       empty = empty || e[a] == 0;
     }
     if (empty) continue;
-    for (int a = 0; a < 3; ++a)
-      if (l[a] - rm[a] < 0 || l[a] + e[a] + rp[a] > size[a])
-        return fail(SB_ERR_INVALID, "box %d: the op reads cells %lld .. %lld on axis %c, outside the allocation's 0 .. %lld", b,
-                    (long long)(l[a] - rm[a]), (long long)(l[a] + e[a] + rp[a] - 1), "xyz"[a], (long long)(size[a] - 1));
+    if ((rc = stencil_box_reads_ok(b, l, e, rm, rp, size, "the op reads")) != SB_OK) return rc;
     for (int f = 0; f < nf; ++f)
-      for (int a = 0; a < 3; ++a)
-        if (l[a] - crm[f][a] < 0 || l[a] + e[a] + crp[f][a] > size[a])
-          return fail(SB_ERR_INVALID, "box %d: coefficient field %d is read at cells %lld .. %lld on axis %c, outside the allocation's 0 .. %lld",
-                      b, fsrc[f], (long long)(l[a] - crm[f][a]), (long long)(l[a] + e[a] + crp[f][a] - 1), "xyz"[a], (long long)(size[a] - 1));
+      if ((rc = stencil_box_reads_ok(b, l, e, crm[f], crp[f], size, "coefficient field " + std::to_string(fsrc[f]) + " is read at")) != SB_OK)
+        return rc;
     if (e[0] * e[1] * e[2] >= (1ll << 32)) return fail(SB_ERR_INVALID, "box %d: more than 2^32 cells", b);
     const std::array<int, 6> bx = {int(l[0]), int(l[1]), int(l[2]), int(e[0]), int(e[1]), int(e[2])};
     (e[0] >= 8 && e[1] >= 8 && e[2] >= 8 ? thick : thin).push_back(bx);
@@ -1664,6 +1697,305 @@ int sb_stencil_vplan_create(sb_stencil_plan **out, int device, int dtype, const 
   return SB_OK;
 }
 
+// ----------------------------------------------------------------------------------------- linear stencil systems
+// The limits every system obeys, whatever the domain: counts, indices, and each term's offsets as for an operator.
+static int stencil_sys_terms_ok(const sb_stencil_sys_term *terms, int n, int nin, int nout) {
+  if (nin < 1 || nin > SB_STENCIL_SYS_MAX_INPUTS) return fail(SB_ERR_INVALID, "a system has 1 to %d inputs, not %d", SB_STENCIL_SYS_MAX_INPUTS, nin);
+  if (nout < 1 || nout > SB_STENCIL_SYS_MAX_OUTPUTS) return fail(SB_ERR_INVALID, "a system has 1 to %d outputs, not %d", SB_STENCIL_SYS_MAX_OUTPUTS, nout);
+  if (!terms || n < 1 || n > SB_STENCIL_SYS_MAX_TERMS)
+    return fail(SB_ERR_INVALID, "a system has 1 to %d terms, not %d", SB_STENCIL_SYS_MAX_TERMS, terms ? n : 0);
+  for (int t = 0; t < n; ++t) {
+    const sb_stencil_sys_term &T = terms[t];
+    if (T.output < 0 || T.output >= nout) return fail(SB_ERR_INVALID, "term %d: output %d must be 0 .. %d", t, int(T.output), nout - 1);
+    if (T.input < 0 || T.input >= nin) return fail(SB_ERR_INVALID, "term %d: input %d must be 0 .. %d", t, int(T.input), nin - 1);
+    int rc = stencil_offset_ok(t, T.offset);
+    if (rc != SB_OK || (rc = stencil_coef_ok(t, T.coef, T.coef_offset, nin, "input")) != SB_OK) return rc;
+  }
+  return SB_OK;
+}
+
+int sb_stencil_sys_check(const sb_stencil_sys_term *terms, int n, int nin, int nout, const int64_t radius27[27]) {
+  if (!radius27) return fail(SB_ERR_INVALID, "sb_stencil_sys_check needs radius27");
+  int rc = stencil_sys_terms_ok(terms, n, nin, nout);
+  if (rc != SB_OK) return rc;
+  for (int t = 0; t < n; ++t) {
+    if ((rc = stencil_offset_in_reach(t, "offset", terms[t].offset, radius27)) != SB_OK) return rc;
+    if (terms[t].coef >= 0 && (rc = stencil_offset_in_reach(t, "coefficient offset", terms[t].coef_offset, radius27)) != SB_OK) return rc;
+  }
+  return SB_OK;
+}
+
+// The difference D_a of input `in` into output `out` with the given stagger, times sign (+1 or -1, exact): two terms.
+static void stencil_diff_terms(int stagger, int a, double h, int out, int in, double sign, std::vector<sb_stencil_sys_term> &v) {
+  const double w = stagger == 0 ? 0.5 / h : 1.0 / h;
+  const int hi = stagger >= 0 ? 1 : 0, lo = stagger <= 0 ? -1 : 0; // the offsets along a of the + and the - term
+  sb_stencil_sys_term t{out, in, {0, 0, 0}, -1, {0, 0, 0}, sign * w};
+  t.offset[a] = hi;
+  v.push_back(t);
+  t.offset[a] = lo;
+  t.weight = -(sign * w);
+  v.push_back(t);
+}
+
+static int stencil_table_ok(const char *name, int stagger, const double spacing[3], const sb_stencil_sys_term *out, int cap) {
+  if (stagger < -1 || stagger > 1) return fail(SB_ERR_INVALID, "%s: stagger %d must be -1 (backward), 0 (central) or +1 (forward)", name, stagger);
+  if (!spacing) return fail(SB_ERR_INVALID, "%s needs spacing[3]", name);
+  for (int a = 0; a < 3; ++a)
+    if (!(spacing[a] > 0.0) || !std::isfinite(spacing[a])) return fail(SB_ERR_INVALID, "spacing[%d] = %g must be finite and > 0", a, spacing[a]);
+  if (cap < 0 || (cap > 0 && !out)) return fail(SB_ERR_INVALID, "%s: bad output buffer", name);
+  return SB_OK;
+}
+
+static int stencil_table_put(const std::vector<sb_stencil_sys_term> &v, sb_stencil_sys_term *out, int cap) {
+  for (int i = 0; i < int(v.size()) && i < cap; ++i) out[i] = v[size_t(i)];
+  return int(v.size());
+}
+
+int sb_stencil_grad(int stagger, const double spacing[3], sb_stencil_sys_term *out, int cap) {
+  int rc = stencil_table_ok("sb_stencil_grad", stagger, spacing, out, cap);
+  if (rc != SB_OK) return rc;
+  std::vector<sb_stencil_sys_term> v;
+  for (int a = 0; a < 3; ++a) stencil_diff_terms(stagger, a, spacing[a], a, 0, 1.0, v);
+  return stencil_table_put(v, out, cap);
+}
+
+int sb_stencil_div(int stagger, const double spacing[3], sb_stencil_sys_term *out, int cap) {
+  int rc = stencil_table_ok("sb_stencil_div", stagger, spacing, out, cap);
+  if (rc != SB_OK) return rc;
+  std::vector<sb_stencil_sys_term> v;
+  for (int a = 0; a < 3; ++a) stencil_diff_terms(stagger, a, spacing[a], 0, a, 1.0, v);
+  return stencil_table_put(v, out, cap);
+}
+
+int sb_stencil_curl(int stagger, const double spacing[3], sb_stencil_sys_term *out, int cap) {
+  int rc = stencil_table_ok("sb_stencil_curl", stagger, spacing, out, cap);
+  if (rc != SB_OK) return rc;
+  std::vector<sb_stencil_sys_term> v;
+  for (int j = 0; j < 3; ++j) { // output j = D_{j+1} in_{j+2} - D_{j+2} in_{j+1}
+    const int a = (j + 1) % 3, b = (j + 2) % 3;
+    stencil_diff_terms(stagger, a, spacing[a], j, b, 1.0, v);
+    stencil_diff_terms(stagger, b, spacing[b], j, a, -1.0, v);
+  }
+  return stencil_table_put(v, out, cap);
+}
+
+int sb_stencil_sys_plan_create(sb_stencil_plan **out, int device, int dtype, const sb_stencil_sys_term *terms, int n,
+                               const sb_pitched *outputs, int nout, const sb_pitched *inputs, int nin, const int64_t acc_origin[3],
+                               int64_t zsize, int nbox, const int64_t *lo, const int64_t *hi) {
+  constexpr int NI = SB_STENCIL_SYS_MAX_INPUTS, NO = SB_STENCIL_SYS_MAX_OUTPUTS;
+  static_assert(NI == sb::kSysMaxInputs && NO == sb::kSysMaxOutputs && SB_STENCIL_SYS_MAX_TERMS == sb::kSysMaxTerms, "one set of limits");
+  if (!out) return fail(SB_ERR_INVALID, "sb_stencil_sys_plan_create needs an output handle");
+  if (dtype != SB_DTYPE_F32 && dtype != SB_DTYPE_F64) return fail(SB_ERR_INVALID, "dtype %d must be SB_DTYPE_F32 or SB_DTYPE_F64", dtype);
+  const int es = dtype == SB_DTYPE_F32 ? 4 : 8;
+  int rc = stencil_sys_terms_ok(terms, n, nin, nout);
+  if (rc != SB_OK) return rc;
+  if (!outputs || !inputs) return fail(SB_ERR_INVALID, "sb_stencil_sys_plan_create needs the output and input arrays");
+  // the inputs the terms read, each with its reach per axis and side, and whether any read has a non-zero offset
+  bool used[NI] = {}, moved[NI] = {};
+  int rm[NI][3] = {}, rp[NI][3] = {}, count[NO] = {};
+  auto reads = [&](int i, const int32_t o[3]) {
+    used[i] = true;
+    for (int a = 0; a < 3; ++a) {
+      rm[i][a] = std::max(rm[i][a], -o[a]);
+      rp[i][a] = std::max(rp[i][a], o[a]);
+      moved[i] = moved[i] || o[a] != 0;
+    }
+  };
+  for (int t = 0; t < n; ++t) {
+    ++count[terms[t].output];
+    reads(terms[t].input, terms[t].offset);
+    if (terms[t].coef >= 0) reads(terms[t].coef, terms[t].coef_offset);
+  }
+  for (int j = 0; j < nout; ++j) {
+    if (!count[j]) return fail(SB_ERR_INVALID, "output %d has no terms", j);
+    if (!outputs[j].ptr) return fail(SB_ERR_INVALID, "output %d is NULL", j);
+    for (int k = 0; k < j; ++k)
+      if (outputs[k].ptr == outputs[j].ptr) return fail(SB_ERR_INVALID, "outputs %d and %d are the same buffer", k, j);
+  }
+  for (int i = 0; i < nin; ++i) {
+    if (!used[i]) continue;
+    if (!inputs[i].ptr) return fail(SB_ERR_INVALID, "input %d is read by a term, but it is NULL", i);
+    for (int j = 0; j < nout && moved[i]; ++j)
+      if (outputs[j].ptr == inputs[i].ptr)
+        return fail(SB_ERR_INVALID, "output %d is input %d, which a term reads at a non-zero offset (an output may be an input read only at offset 0)", j, i);
+  }
+  std::vector<const sb_pitched *> bufs;
+  std::vector<std::string> names;
+  for (int j = 0; j < nout; ++j) {
+    bufs.push_back(&outputs[j]);
+    names.push_back("output " + std::to_string(j));
+  }
+  for (int i = 0; i < nin; ++i)
+    if (used[i]) {
+      bufs.push_back(&inputs[i]);
+      names.push_back("input " + std::to_string(i));
+    }
+  if ((rc = stencil_buffers_ok(bufs, names, outputs[0], "output 0", es)) != SB_OK) return rc;
+  if (!acc_origin || zsize < 1) return fail(SB_ERR_INVALID, "sb_stencil_sys_plan_create needs acc_origin and zsize >= 1");
+  if (nbox < 0 || (nbox > 0 && (!lo || !hi))) return fail(SB_ERR_INVALID, "nbox %d: needs nbox >= 0 and lo / hi arrays", nbox);
+  const int64_t pitch = outputs[0].pitch, slice = pitch * outputs[0].ysize;
+  const int64_t size[3] = {pitch / es, outputs[0].ysize, zsize};
+  std::vector<std::array<int, 6>> thick, thin; // allocation-relative lo, ext
+  int64_t cells = 0;
+  for (int b = 0; b < nbox; ++b) {
+    int64_t l[3], e[3];
+    bool empty = false;
+    for (int a = 0; a < 3; ++a) {
+      if (lo[3 * b + a] > hi[3 * b + a]) return fail(SB_ERR_INVALID, "box %d: lo > hi on axis %d", b, a);
+      l[a] = lo[3 * b + a] - acc_origin[a];
+      e[a] = hi[3 * b + a] - lo[3 * b + a];
+      empty = empty || e[a] == 0;
+    }
+    if (empty) continue;
+    for (int i = 0; i < nin; ++i)
+      if (used[i] && (rc = stencil_box_reads_ok(b, l, e, rm[i], rp[i], size, "input " + std::to_string(i) + " is read at")) != SB_OK) return rc;
+    if (e[0] * e[1] * e[2] >= (1ll << 32)) return fail(SB_ERR_INVALID, "box %d: more than 2^32 cells", b);
+    const std::array<int, 6> bx = {int(l[0]), int(l[1]), int(l[2]), int(e[0]), int(e[1]), int(e[2])};
+    (e[0] >= 8 && e[1] >= 8 && e[2] >= 8 ? thick : thin).push_back(bx);
+    cells += e[0] * e[1] * e[2];
+  }
+
+  // the read inputs renumbered 0 .. nr - 1 (ring r of the tile kernel); each ring's plane size; the shared row width fits
+  // the widest window shifted onto 16-byte phase
+  int ri[NI], src_of[NI], nr = 0, rx = 0;
+  for (int i = 0; i < nin; ++i) {
+    ri[i] = used[i] ? nr : -1;
+    if (used[i]) {
+      src_of[nr++] = i;
+      rx = std::max(rx, rm[i][0] + rp[i][0]);
+    }
+  }
+  const int V = 16 / es;
+  const int sw = (V - 1 + sb::kOpTileX + rx + V - 1) / V * V;
+  int base[NI] = {}, ns[NI] = {};
+  size_t ring_elems = 0;
+  for (int r = 0; r < nr; ++r) {
+    const int i = src_of[r];
+    ns[r] = rm[i][2] + rp[i][2] + 2;
+    base[r] = int(ring_elems);
+    ring_elems += size_t(ns[r]) * size_t(sb::kOpTileY + rm[i][1] + rp[i][1]) * size_t(sw);
+  }
+  const size_t smem = size_t(sb::kSysTableBytes) + ring_elems * size_t(es);
+  DeviceGuard guard(device);
+  if (!guard.ok) return fail(SB_ERR_NOGPU, "cannot select CUDA device %d", device);
+  int sms = 0, optin = 0;
+  SB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
+  SB_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device));
+  if (!thick.empty() && smem > size_t(optin))
+    return fail(SB_ERR_INVALID, "the system's tile kernel needs %zu bytes of shared memory per block, the device allows %d", smem, optin);
+
+  // the terms sorted by output (stable): the rule sums each output's terms in list order
+  std::vector<int> order;
+  sb::SysTerms com{};
+  for (int j = 0; j < nout; ++j) {
+    com.first[j] = int(order.size());
+    for (int t = 0; t < n; ++t)
+      if (terms[t].output == j) order.push_back(t);
+    com.out[j] = static_cast<char *>(outputs[j].ptr);
+  }
+  com.first[nout] = n;
+  com.pitch = pitch;
+  com.slice = slice;
+  com.n = n;
+  com.nout = nout;
+  for (int k = 0; k < n; ++k) {
+    const sb_stencil_sys_term &T = terms[order[size_t(k)]];
+    com.in[k] = (signed char)ri[T.input];
+    com.cin[k] = (signed char)(T.coef < 0 ? -1 : ri[T.coef]);
+    com.w[k] = T.weight;
+    com.wf[k] = float(T.weight); // round to nearest
+  }
+
+  sb_stencil_plan *p = new sb_stencil_plan();
+  p->device = device;
+  p->es = es;
+  p->bytes = cells * es * (nr + nout);
+  p->sys_smem = smem;
+  if (!thick.empty()) {
+    const int per_sm = sb::sys_tile_prepare(es, device, smem);
+    if (per_sm <= 0) {
+      delete p;
+      return fail(SB_ERR_CUDA, "the system tile kernel cannot be configured: %s", cudaGetErrorString(cudaGetLastError()));
+    }
+    for (const auto &b : thick) {
+      sb::SysTileParams tp{};
+      tp.c = com;
+      tp.nr = nr;
+      tp.sw = sw;
+      int shift[NI] = {};
+      for (int r = 0; r < nr; ++r) {
+        const int i = src_of[r];
+        tp.in[r] = static_cast<const char *>(inputs[i].ptr);
+        tp.vec[r] = pitch % 16 == 0; // else rows alternate between 16-byte phases: elements one by one
+        shift[r] = tp.vec[r] ? int((uintptr_t(tp.in[r]) + uintptr_t(int64_t(b[0] - rm[i][0]) * es)) % 16) / es : 0;
+        tp.shift[r] = shift[r];
+        tp.ns[r] = ns[r];
+        tp.base[r] = base[r];
+        for (int a = 0; a < 3; ++a) {
+          tp.rm[r][a] = rm[i][a];
+          tp.rp[r][a] = rp[i][a];
+        }
+      }
+      // a read's shared offset within its plane, from the cell's own slot position wy * sw + lane
+      auto inplane = [&](int r, const int32_t o[3]) { return (tp.rm[r][1] + o[1]) * sw + tp.rm[r][0] + shift[r] + o[0]; };
+      for (int k = 0; k < n; ++k) {
+        const sb_stencil_sys_term &T = terms[order[size_t(k)]];
+        tp.oz[k] = (signed char)T.offset[2];
+        tp.inpl[k] = inplane(com.in[k], T.offset);
+        if (com.cin[k] >= 0) {
+          tp.coz[k] = (signed char)T.coef_offset[2];
+          tp.cinpl[k] = inplane(com.cin[k], T.coef_offset);
+        }
+      }
+      for (int a = 0; a < 3; ++a) {
+        tp.lo[a] = b[a];
+        tp.ext[a] = b[3 + a];
+      }
+      tp.tiles_x = (tp.ext[0] + sb::kOpTileX - 1) / sb::kOpTileX;
+      tp.tiles_y = (tp.ext[1] + sb::kOpTileY - 1) / sb::kOpTileY;
+      // z chunks as for an operator: at least two waves of resident CTAs, chunks no shorter than 16 planes
+      const long long cols = (long long)tp.tiles_x * tp.tiles_y;
+      const long long want = (2ll * sms * per_sm + cols - 1) / cols;
+      int zc = int((tp.ext[2] + want - 1) / want);
+      zc = std::max(zc, std::min(16, tp.ext[2]));
+      tp.zchunk = zc;
+      const long long grid = cols * ((tp.ext[2] + zc - 1) / zc);
+      if (grid >= (1ll << 31)) {
+        delete p;
+        return fail(SB_ERR_INVALID, "box too large for the tile kernel");
+      }
+      p->sys_tiles.push_back(tp);
+      p->sys_tile_grids.push_back(int(grid));
+    }
+  }
+  for (size_t b0 = 0; b0 < thin.size(); b0 += sb::kOpMaxBoxes) {
+    sb::SysCellParams cp{};
+    cp.c = com;
+    for (int r = 0; r < nr; ++r) cp.in[r] = static_cast<const char *>(inputs[src_of[r]].ptr);
+    for (int k = 0; k < n; ++k) {
+      const sb_stencil_sys_term &T = terms[order[size_t(k)]];
+      for (int a = 0; a < 3; ++a) {
+        cp.o[k][a] = (signed char)T.offset[a];
+        cp.co[k][a] = (signed char)T.coef_offset[a];
+      }
+    }
+    cp.first[0] = 0;
+    for (size_t b = b0; b < thin.size() && b < b0 + sb::kOpMaxBoxes; ++b) {
+      const int m = cp.nb++;
+      for (int a = 0; a < 3; ++a) {
+        cp.lo[m][a] = thin[b][a];
+        cp.ext[m][a] = thin[b][3 + a];
+      }
+      cp.first[m + 1] = cp.first[m] + (long long)thin[b][3] * thin[b][4] * thin[b][5];
+    }
+    const long long total = cp.first[cp.nb];
+    p->sys_cells.push_back(cp);
+    p->sys_cell_grids.push_back(int(std::min<long long>((total + 255) / 256, 32ll * sms)));
+  }
+  *out = p;
+  return SB_OK;
+}
+
 int sb_stencil_plan_launch(sb_stencil_plan *p, void *stream) {
   if (!p) return fail(SB_ERR_INVALID, "null plan");
   DeviceGuard guard(p->device);
@@ -1671,6 +2003,8 @@ int sb_stencil_plan_launch(sb_stencil_plan *p, void *stream) {
   const cudaStream_t s = static_cast<cudaStream_t>(stream);
   for (size_t i = 0; i < p->tiles.size(); ++i) g_launches += uint64_t(sb::launch_op_tile(p->tiles[i], p->R, p->es, p->tile_grids[i], s));
   for (size_t i = 0; i < p->cells.size(); ++i) g_launches += uint64_t(sb::launch_op_cells(p->cells[i], p->es, p->has_coef, p->cell_grids[i], s));
+  for (size_t i = 0; i < p->sys_tiles.size(); ++i) g_launches += uint64_t(sb::launch_sys_tile(p->sys_tiles[i], p->es, p->sys_smem, p->sys_tile_grids[i], s));
+  for (size_t i = 0; i < p->sys_cells.size(); ++i) g_launches += uint64_t(sb::launch_sys_cells(p->sys_cells[i], p->es, p->sys_cell_grids[i], s));
   SB_CUDA(cudaGetLastError());
   return SB_OK;
 }

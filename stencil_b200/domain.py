@@ -1159,8 +1159,6 @@ class DistributedDomain:
         the ghost cells are current.  Returns when the update is complete.  The plans are built on first use and kept,
         per (op, buffers, exchange, swap parity), until close().  Under torchrun every rank calls it (exchange() is
         collective)."""
-        import torch
-
         from .stencil_op import StencilOp, StencilPlan
 
         if not isinstance(op, StencilOp):
@@ -1198,19 +1196,91 @@ class DistributedDomain:
             c_q.append(q)
         op.check(self.radius_)
         key = (op.key(), (d_q, d_w), s_q, a if op.has_aux else None, tuple(c_q), bool(exchange), self._parity)
+
+        def make(di, d, boxes):
+            P = (d.pitched(d_q, d_w), d.pitched(s_q, "curr"), d.pitched(a[0], a[1]) if a is not None and op.has_aux else Pitched(None, 0, 0))
+            K = [d.pitched(q, "curr") for q in c_q] if op.has_coef else None
+            return StencilPlan(d.gpu(), op, *P, d.accessor_origin(), d.raw_size()[2], boxes, K)
+
+        self._run_plans(self._plans_for(key, exchange, make), exchange)
+
+    def apply_system(self, system, outputs, inputs, exchange: bool = True) -> None:
+        """outputs = system(inputs) over the whole compute region of every local subdomain (DESIGN.md section 2.8).
+
+        outputs: system.nout buffers, inputs: system.nin buffers, each (DataHandle, "curr" | "next"); a bare handle means
+        "next" for an output and "curr" for an input; an input no term reads may be None.  All share the system's element
+        type.  An input read at a non-zero offset (as a source or a coefficient) must be a curr buffer, the one
+        exchange() fills.  Outputs are pairwise distinct; an output may be an input only if every read of that input is
+        at offset 0 (an in-place update such as E = E + dt curl H).
+        The schedule, the plan cache (per system, buffers, exchange and swap parity) and the torchrun rule are apply()'s."""
+        from .stencil_op import StencilSystem, SystemPlan
+
+        if not isinstance(system, StencilSystem):
+            raise _lib.StencilError(f"{system!r} is not a StencilSystem")
+        if self.partition_ is None or not self._plans:
+            raise _lib.StencilError("apply_system: call realize() first")
+        outputs, inputs = list(outputs), list(inputs)
+        if len(outputs) != system.nout or len(inputs) != system.nin:
+            raise _lib.StencilError(f"apply_system: the system has {system.nin} inputs and {system.nout} outputs, "
+                                    f"but {len(inputs)} inputs and {len(outputs)} outputs were given")
+
+        def buf(arg, default, role):
+            h, which = (arg, default) if isinstance(arg, DataHandle) else tuple(arg)
+            if not isinstance(h, DataHandle) or which not in ("curr", "next"):
+                raise _lib.StencilError(f"apply_system: {role} must be a DataHandle or (DataHandle, 'curr' | 'next'), not {arg!r}")
+            if self.dtypes_[h.id] != system.dtype:
+                raise _lib.StencilError(f"apply_system: {role} is {self.dtypes_[h.id]}, the system computes in {system.dtype}")
+            return h.id, which
+
+        outs = [buf(o, "next", f"output {j}") for j, o in enumerate(outputs)]
+        reads, moved = system.read_inputs(), system.moved_inputs()
+        ins = []
+        for i, a in enumerate(inputs):
+            if a is None:
+                if i in reads:
+                    raise _lib.StencilError(f"apply_system: input {i} is read by a term, but it is None")
+                ins.append(None)
+                continue
+            q = buf(a, "curr", f"input {i}")
+            if i in moved and q[1] != "curr":
+                raise _lib.StencilError(f"apply_system: input {i} is read at a non-zero offset, so it must be a curr buffer (the one exchange() fills)")
+            ins.append(q if i in reads else None)
+        if len(set(outs)) != len(outs):
+            raise _lib.StencilError("apply_system: the outputs must be distinct buffers")
+        for j, o in enumerate(outs):
+            for i in moved:
+                if ins[i] == o:
+                    raise _lib.StencilError(f"apply_system: output {j} is input {i}, which is read at a non-zero offset")
+        system.check(self.radius_)
+        key = ("system", system.key(), tuple(outs), tuple(ins), bool(exchange), self._parity)
+
+        def make(di, d, boxes):
+            O = [d.pitched(q, w) for q, w in outs]
+            I = [d.pitched(q[0], q[1]) if q is not None else Pitched(None, 0, 0) for q in ins]
+            return SystemPlan(d.gpu(), system, O, I, d.accessor_origin(), d.raw_size()[2], boxes)
+
+        self._run_plans(self._plans_for(key, exchange, make), exchange)
+
+    def _plans_for(self, key, exchange: bool, make):
+        """The cached per-domain plans of key: (interior, exterior) pairs with exchange, else one plan over the whole
+        compute region; make(di, d, boxes) builds one plan."""
         plans = self._stencil_plans.get(key)
         if plans is None:
             plans = []
             interiors, exteriors = (self.get_interior(), self.get_exterior()) if exchange else (None, None)
             for di, d in enumerate(self.domains_):
-                P = (d.pitched(d_q, d_w), d.pitched(s_q, "curr"), d.pitched(a[0], a[1]) if a is not None and op.has_aux else Pitched(None, 0, 0))
-                K = [d.pitched(q, "curr") for q in c_q] if op.has_coef else None
-                mk = lambda boxes: StencilPlan(d.gpu(), op, *P, d.accessor_origin(), d.raw_size()[2], boxes, K)  # noqa: E731
                 if exchange:
-                    plans.append((mk([interiors[di]]), mk(exteriors[di])))
+                    plans.append((make(di, d, [interiors[di]]), make(di, d, exteriors[di])))
                 else:
-                    plans.append((mk([d.get_compute_region()]),))
+                    plans.append((make(di, d, [d.get_compute_region()]),))
             self._stencil_plans[key] = plans
+        return plans
+
+    def _run_plans(self, plans, exchange: bool) -> None:
+        """The schedule of apply and apply_system: with exchange, every interior plan on its own stream while exchange()
+        fills the ghost cells, then every exterior plan; without, the one plan per domain.  Returns when all are done."""
+        import torch
+
         if not self._apply_streams:
             self._apply_streams = [(torch.cuda.Stream(device=d.gpu()), torch.cuda.Stream(device=d.gpu())) for d in self.domains_]
         for d, (si, se) in zip(self.domains_, self._apply_streams):  # after the work queued on the caller's stream

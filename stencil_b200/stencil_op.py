@@ -14,8 +14,17 @@ contributes (T(w) * C_k) * S instead:
     heat = StencilOp(list(kdt.terms) + [(0, (0, 0, 0), 1.0)], np.float64)
     dd.apply(heat, h, h, coefs=[kx, ky, kz])
 
-The rule, the reach check against a domain's radius and the Laplacian and div-grad tables live in the C library; this
-module only carries them.
+A system (DESIGN.md section 2.8) has several outputs over several inputs, one launch for all of them.  A term
+(output, input, offset, weight) or (output, input, offset, weight, coef, coef_offset) adds to output `output`; each
+output sums its own terms in list order by the same rule:
+
+    curl_h = StencilSystem.curl(-1, (h, h, h), np.float64).scaled(dt / eps)    # inputs 0-2: H, outputs 0-2
+    ident = StencilSystem([(j, 3 + j, (0, 0, 0), 1.0) for j in range(3)], np.float64, nin=6)   # inputs 3-5: E
+    E = [(q, "curr") for q in (ex, ey, ez)]
+    dd.apply_system(ident + curl_h, E, [hx, hy, hz] + E)                       # E = E + dt/eps curl H, in place
+
+The rule, the reach check against a domain's radius and the Laplacian, div-grad, grad, div and curl tables live in the
+C library; this module only carries them.
 """
 from __future__ import annotations
 
@@ -25,7 +34,7 @@ from typing import Iterable, List, Optional, Sequence, Tuple
 import numpy as np
 
 from . import _lib
-from ._lib import I27, Pitched, StencilTerm, StencilVTerm, check, i3, lib, stream_ptr
+from ._lib import I27, Pitched, StencilSysTerm, StencilTerm, StencilVTerm, check, i3, lib, stream_ptr
 
 Term = Tuple  # (source, offset, weight) or (source, offset, weight, coef, coef_offset)
 
@@ -175,3 +184,127 @@ class StencilPlan:
             self.destroy()
         except Exception:
             pass
+
+
+SysTerm = Tuple  # (output, input, offset, weight) or (output, input, offset, weight, coef, coef_offset)
+
+
+class StencilSystem:
+    """A system: terms (output, input, (dx, dy, dz), weight) or (output, input, (dx, dy, dz), weight, coef, (cx, cy, cz)),
+    in dtype (float32 or float64), over nin inputs and nout outputs (by default one more than the highest index a term
+    names).  A 6-tuple with coef -1 is a plain term and is kept as the 4-tuple."""
+
+    def __init__(self, terms: Iterable[Sequence], dtype, nin: Optional[int] = None, nout: Optional[int] = None):
+        out: List[SysTerm] = []
+        for t in terms:
+            if len(t) not in (4, 6):
+                raise _lib.StencilError(f"term {t!r}: (output, input, offset, weight) or (output, input, offset, weight, coef, coef_offset)")
+            j, i, o, w = int(t[0]), int(t[1]), (int(t[2][0]), int(t[2][1]), int(t[2][2])), float(t[3])
+            if len(t) == 6 and int(t[4]) != -1:
+                c = t[5]
+                out.append((j, i, o, w, int(t[4]), (int(c[0]), int(c[1]), int(c[2]))))
+                continue
+            if len(t) == 6 and any(int(v) for v in t[5]):
+                raise _lib.StencilError(f"term {t!r}: a term without a coefficient field has coefficient offset (0, 0, 0)")
+            out.append((j, i, o, w))
+        self.terms: Tuple[SysTerm, ...] = tuple(out)
+        self.dtype = np.dtype(dtype)
+        self.dtype_code = _dtype_code(self.dtype)
+        reads = [t[1] for t in out] + [t[4] for t in out if len(t) == 6]
+        self.nin = int(nin) if nin is not None else max(reads, default=-1) + 1
+        self.nout = int(nout) if nout is not None else max([t[0] for t in out], default=-1) + 1
+        self._check(I27(*([_lib.STENCIL_MAX_REACH] * 27)))
+
+    def _check(self, r27) -> None:
+        check(lib().sb_stencil_sys_check(self.c_terms(), len(self.terms), self.nin, self.nout, r27))
+
+    @staticmethod
+    def _table(fn, stagger: int, spacing: Sequence[float], dtype) -> "StencilSystem":
+        h = (C.c_double * 3)(*[float(v) for v in spacing])
+        n = check(fn(int(stagger), h, None, 0))
+        buf = (StencilSysTerm * n)()
+        check(fn(int(stagger), h, buf, n))
+        return StencilSystem([(t.output, t.input, tuple(t.offset), t.weight) for t in buf], dtype)
+
+    @staticmethod
+    def grad(stagger: int, spacing: Sequence[float], dtype) -> "StencilSystem":
+        """Input 0 -> outputs x, y, z (sb_stencil_grad).  stagger +1: forward differences, -1: backward, 0: central."""
+        return StencilSystem._table(lib().sb_stencil_grad, stagger, spacing, dtype)
+
+    @staticmethod
+    def div(stagger: int, spacing: Sequence[float], dtype) -> "StencilSystem":
+        """Inputs 0, 1, 2 -> output 0 (sb_stencil_div)."""
+        return StencilSystem._table(lib().sb_stencil_div, stagger, spacing, dtype)
+
+    @staticmethod
+    def curl(stagger: int, spacing: Sequence[float], dtype) -> "StencilSystem":
+        """Inputs 0, 1, 2 -> outputs 0, 1, 2 (sb_stencil_curl)."""
+        return StencilSystem._table(lib().sb_stencil_curl, stagger, spacing, dtype)
+
+    def scaled(self, f: float) -> "StencilSystem":
+        """The same system with every weight multiplied by f (in double)."""
+        return StencilSystem([t[:3] + (t[3] * float(f),) + tuple(t[4:]) for t in self.terms], self.dtype, self.nin, self.nout)
+
+    def shifted(self, input_base: int = 0, output_base: int = 0) -> "StencilSystem":
+        """The same system reading inputs input_base + i (coefficients included) and writing outputs output_base + j."""
+        ib, ob = int(input_base), int(output_base)
+        out = []
+        for t in self.terms:
+            u = (t[0] + ob, t[1] + ib) + t[2:4]
+            out.append(u + (t[4] + ib, t[5]) if len(t) == 6 else u)
+        return StencilSystem(out, self.dtype, self.nin + ib, self.nout + ob)
+
+    def __add__(self, o: "StencilSystem") -> "StencilSystem":
+        """Concatenation: self's terms, then o's; each output still sums its terms in this order."""
+        if not isinstance(o, StencilSystem) or o.dtype != self.dtype:
+            raise _lib.StencilError(f"cannot concatenate {self!r} and {o!r}")
+        return StencilSystem(self.terms + o.terms, self.dtype, max(self.nin, o.nin), max(self.nout, o.nout))
+
+    def c_terms(self):
+        arr = (StencilSysTerm * max(1, len(self.terms)))()
+        for k, t in enumerate(self.terms):
+            coef, co = (t[4], t[5]) if len(t) == 6 else (-1, (0, 0, 0))
+            arr[k] = StencilSysTerm(t[0], t[1], (C.c_int32 * 3)(*t[2]), coef, (C.c_int32 * 3)(*co), t[3])
+        return arr
+
+    def moved_inputs(self) -> set:
+        """The inputs some term reads at a non-zero offset (as a source or a coefficient)."""
+        return {t[1] for t in self.terms if any(t[2])} | {t[4] for t in self.terms if len(t) == 6 and any(t[5])}
+
+    def read_inputs(self) -> set:
+        return {t[1] for t in self.terms} | {t[4] for t in self.terms if len(t) == 6}
+
+    def check(self, radius) -> None:
+        """Raise StencilError unless a domain with this Radius exchanges every ghost cell the system reads."""
+        self._check(radius.c27())
+
+    def key(self) -> tuple:
+        return (self.terms, self.dtype.str, self.nin, self.nout)
+
+    def __eq__(self, o) -> bool:
+        return isinstance(o, StencilSystem) and self.key() == o.key()
+
+    def __hash__(self) -> int:
+        return hash(self.key())
+
+    def __repr__(self) -> str:
+        return f"StencilSystem({len(self.terms)} terms, {self.nin} -> {self.nout}, {self.dtype})"
+
+
+class SystemPlan(StencilPlan):
+    """sb_stencil_sys_plan_create: the system over a list of boxes [lo, hi) (global coordinates) of one subdomain's output
+    and input allocations (an input no term reads may be Pitched(None, 0, 0))."""
+
+    def __init__(self, device: int, system: StencilSystem, outputs: Sequence[Pitched], inputs: Sequence[Pitched], acc_origin, zsize: int,
+                 boxes: Sequence[Tuple[Sequence[int], Sequence[int]]]):
+        nb = len(boxes)
+        lo = (C.c_int64 * (3 * max(1, nb)))(*[int(v) for b in boxes for v in b[0]])
+        hi = (C.c_int64 * (3 * max(1, nb)))(*[int(v) for b in boxes for v in b[1]])
+        outs = (Pitched * max(1, len(outputs)))(*outputs)
+        ins = (Pitched * max(1, len(inputs)))(*inputs)
+        h = C.c_void_p()
+        check(lib().sb_stencil_sys_plan_create(C.byref(h), device, system.dtype_code, system.c_terms(), len(system.terms), outs, len(outputs), ins,
+                                               len(inputs), i3(acc_origin), int(zsize), nb, lo, hi))
+        self._h = h
+        self.device = device
+        self.bytes = int(lib().sb_stencil_plan_bytes(h))
