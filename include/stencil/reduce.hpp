@@ -6,6 +6,7 @@
 //     double res = dd.reduce_diff(h).l2();                       // ||curr - next||_2
 //     double urms = dd.reduce_norm(hx, hy, hz).rms();            // sqrt(sum |u|^2 / N)
 //     auto rs = dd.reduce_many({stencil::ReduceItem::scalar(h), stencil::ReduceItem::diff(h)});  // one launch per subdomain
+//     double total = dd.reduce(h, stencil::Which::curr, stencil::Sum::exact).sum;  // correctly rounded, any partition
 #include <cmath>
 #include <cstddef>
 #include <cstdint>
@@ -27,6 +28,11 @@ struct Reduction {
 };
 
 enum class Which { curr, next };
+
+// How sum and sumsq are formed.  ordered: the fixed trees of sb_reduce_plan_* (the faster path; the bits depend on the
+// partition).  exact: sb_reduce_exact_plan_* -- the exact sums rounded once, the same bits for every partition and rank
+// count (DESIGN.md section 2.6.1).  min, max and count are the same either way on one subdomain.
+enum class Sum { ordered, exact };
 
 // One item of DistributedDomain::reduce_many: a SCALAR (curr or next buffer), a DIFF (curr - next) or a NORM3
 // (|(x, y, z)| of three quantities' curr buffers) over the whole compute region.

@@ -47,6 +47,7 @@
 struct sb_copy_plan;
 struct sb_bc_plan;
 struct sb_reduce_plan;
+struct sb_reduce_exact_plan;
 struct sb_stencil_plan;
 
 class DistributedDomain {
@@ -121,8 +122,10 @@ private:
 
   // reductions: per (item list, swap parity), one plan and one device result buffer per local domain
   struct ReduceCache {
-    std::vector<sb_reduce_plan *> plans;
+    std::vector<sb_reduce_plan *> plans; // Sum::ordered
     std::vector<sb_reduce_result *> out;
+    std::vector<sb_reduce_exact_plan *> xplans; // Sum::exact
+    std::vector<sb_reduce_exact_part *> xout;
   };
   std::map<std::vector<int64_t>, ReduceCache> reducePlans_;
   void destroy_reduce_plans();
@@ -258,14 +261,28 @@ public:
   // (x fastest).  Collective: every rank must call it with the same items.  The plans (tile tables, scratch, result
   // buffer) are built once per item list and swap parity and kept until the domain is destroyed, so a program should
   // reduce a fixed set of item lists rather than build new ones every iteration.
+  // With stencil::Sum::exact the per-subdomain exact parts are gathered with MPI_Allgatherv, combined with
+  // sb_reduce_exact_combine and rounded once with sb_reduce_exact_round on every rank: sum and sumsq are correctly rounded
+  // and the same bits for every partition and rank count.  Plans are cached per item list, exactness and swap parity.
   template <typename T> stencil::Reduction reduce(const DataHandle<T> &h, stencil::Which which = stencil::Which::curr) {
     return reduce_many(std::vector<stencil::ReduceItem>(1, stencil::ReduceItem::scalar(h, which)))[0];
   }
+  template <typename T> stencil::Reduction reduce(const DataHandle<T> &h, stencil::Which which, stencil::Sum sum) {
+    return reduce_many(std::vector<stencil::ReduceItem>(1, stencil::ReduceItem::scalar(h, which)), sum)[0];
+  }
   template <typename T> stencil::Reduction reduce_diff(const DataHandle<T> &h) { return reduce_many(std::vector<stencil::ReduceItem>(1, stencil::ReduceItem::diff(h)))[0]; }
+  template <typename T> stencil::Reduction reduce_diff(const DataHandle<T> &h, stencil::Sum sum) {
+    return reduce_many(std::vector<stencil::ReduceItem>(1, stencil::ReduceItem::diff(h)), sum)[0];
+  }
   template <typename T> stencil::Reduction reduce_norm(const DataHandle<T> &x, const DataHandle<T> &y, const DataHandle<T> &z) {
     return reduce_many(std::vector<stencil::ReduceItem>(1, stencil::ReduceItem::norm(x, y, z)))[0];
   }
-  std::vector<stencil::Reduction> reduce_many(const std::vector<stencil::ReduceItem> &items);
+  template <typename T>
+  stencil::Reduction reduce_norm(const DataHandle<T> &x, const DataHandle<T> &y, const DataHandle<T> &z, stencil::Sum sum) {
+    return reduce_many(std::vector<stencil::ReduceItem>(1, stencil::ReduceItem::norm(x, y, z)), sum)[0];
+  }
+  std::vector<stencil::Reduction> reduce_many(const std::vector<stencil::ReduceItem> &items) { return reduce_many(items, stencil::Sum::ordered); }
+  std::vector<stencil::Reduction> reduce_many(const std::vector<stencil::ReduceItem> &items, stencil::Sum sum);
 
   // dst = op(src, aux) over the whole compute region of every local subdomain (DESIGN.md section 2.7).  src is the curr
   // buffer (the one exchange() fills); dst is curr or next of any quantity of the same type, never src itself; aux is curr

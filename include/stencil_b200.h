@@ -268,6 +268,55 @@ int sb_reduce_plan_destroy(sb_reduce_plan *plan);
 int sb_reduce_combine(const sb_reduce_result *parts, int64_t n, sb_reduce_result *out);
 
 /* ---------------------------------------------------------------------------------------------
+ * Exact reductions (DESIGN.md section 2.6.1): the same items and per-cell v and q as above, with
+ *   min, max, count  the plain plan's, bit for bit (the same NaN rule and empty-box values); across parts,
+ *                    sb_reduce_exact_combine's order-independent rule below, which may pick other bits than
+ *                    sb_reduce_combine's tree only between +0 and -0 or between two NaNs;
+ *   sum (sumsq)      the exact real sum of every v (q), rounded once to double, to nearest, ties to even.
+ * Special values, for both sums: a NaN term gives NaN; +inf and -inf among the terms give NaN; otherwise an infinite
+ * term gives that infinity; an exact sum beyond the double range rounds to +-inf as IEEE round-to-nearest does; an
+ * exact zero is +0.0.  A q that overflowed to inf when it was formed is an infinite term.
+ * The sums depend only on the multiset of per-cell terms: not on the partition, the tiling, the allocation layout, the
+ * SM count or the order in which parts are combined.
+ *
+ * sb_exact_sum is the canonical accumulator: the exact sum of the finite terms as a 2176-bit two's complement integer
+ * in units of 2^-1074, word[0] least significant, fully carried (equal multisets give byte-identical accumulators),
+ * plus the flags of the non-finite terms.  A finite term is below 2^1024 = 2^2098 units, so any sum of fewer than 2^77
+ * terms (every cell count the library can form, and any combine of such parts) fits without overflow.
+ * ------------------------------------------------------------------------------------------- */
+#define SB_EXACT_WORDS 34
+#define SB_EXACT_NAN 1u     /* some term is NaN */
+#define SB_EXACT_POS_INF 2u /* some term is +inf */
+#define SB_EXACT_NEG_INF 4u /* some term is -inf */
+typedef struct sb_exact_sum {
+  uint64_t word[SB_EXACT_WORDS];
+  uint64_t flags;
+} sb_exact_sum;
+
+typedef struct sb_reduce_exact_part {
+  double min, max;
+  int64_t count;
+  sb_exact_sum sum, sumsq;
+} sb_reduce_exact_part;
+
+/* A persistent plan with the contract of sb_reduce_plan_*: the same items and the same errors and messages, plus one:
+ * a box with rows of more than 2^27 cells.  sb_reduce_exact_plan_launch writes one sb_reduce_exact_part per item, in
+ * item order, to out_dev (device memory); it allocates nothing, never synchronises the host, may be captured in a CUDA
+ * graph, and at most one launch of a plan may be in flight at a time. */
+typedef struct sb_reduce_exact_plan sb_reduce_exact_plan;
+int sb_reduce_exact_plan_create(sb_reduce_exact_plan **out, int device, const sb_reduce_item *items, int64_t n);
+int sb_reduce_exact_plan_launch(sb_reduce_exact_plan *plan, sb_reduce_exact_part *out_dev, void *stream);
+int64_t sb_reduce_exact_plan_bytes(const sb_reduce_exact_plan *plan); /* source bytes read per launch */
+int sb_reduce_exact_plan_destroy(sb_reduce_exact_plan *plan);
+/* Host only.  parts[0..n) (n >= 1, e.g. one per subdomain) merged: accumulators added, flags or-ed, counts added, min
+ * and max by a rule that does not depend on the order of parts (a NaN operand wins, the larger bit pattern of two
+ * NaNs; of +0 and -0 min takes -0 and max +0).  Combine parts, then round: rounding each part first would make the
+ * result depend on the partition again. */
+int sb_reduce_exact_combine(const sb_reduce_exact_part *parts, int64_t n, sb_reduce_exact_part *out);
+/* Host only.  The one place that rounds: min, max and count copied, sum and sumsq rounded by the rule above. */
+int sb_reduce_exact_round(const sb_reduce_exact_part *part, sb_reduce_result *out);
+
+/* ---------------------------------------------------------------------------------------------
  * Constant-coefficient linear stencil operators (not in the reference; DESIGN.md section 2.7).
  * An operator is a list of 1 <= n <= SB_STENCIL_MAX_TERMS terms (source s, offset o, weight w): s = 0 reads src at
  * p + o, s = 1 reads aux at p (aux terms have offset 0: a previous time level, a right-hand side, a blend);

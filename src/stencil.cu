@@ -633,6 +633,11 @@ void DistributedDomain::destroy_reduce_plans() {
       cudaSetDevice(domains_[di].gpu());
       cudaFree(kv.second.out[di]);
     }
+    for (size_t di = 0; di < kv.second.xplans.size(); ++di) {
+      sb_reduce_exact_plan_destroy(kv.second.xplans[di]);
+      cudaSetDevice(domains_[di].gpu());
+      cudaFree(kv.second.xout[di]);
+    }
   }
   reducePlans_.clear();
 }
@@ -800,8 +805,9 @@ void DistributedDomain::run_stencil_plans(const std::vector<int64_t> &key, bool 
   }
 }
 
-std::vector<stencil::Reduction> DistributedDomain::reduce_many(const std::vector<stencil::ReduceItem> &items) {
+std::vector<stencil::Reduction> DistributedDomain::reduce_many(const std::vector<stencil::ReduceItem> &items, stencil::Sum sum) {
   using stencil::Which;
+  const bool exact = sum == stencil::Sum::exact;
   const size_t n = items.size();
   if (0 == n) return {};
   std::vector<int64_t> key;
@@ -817,6 +823,7 @@ std::vector<stencil::Reduction> DistributedDomain::reduce_many(const std::vector
                            int64_t(it.kind == SB_REDUCE_SCALAR && it.which == Which::next)});
   }
   key.push_back(parity_);
+  key.push_back(int64_t(exact));
   auto found = reducePlans_.find(key);
   if (found == reducePlans_.end()) {
     ReduceCache c;
@@ -841,13 +848,23 @@ std::vector<stencil::Reduction> DistributedDomain::reduce_many(const std::vector
           r.hi[a] = hi[a];
         }
       }
-      sb_reduce_plan *plan = nullptr;
-      if (SB_OK != sb_reduce_plan_create(&plan, d.gpu(), its.data(), int64_t(n))) LOG_FATAL("reduce: " << sb_last_error());
-      sb_reduce_result *out = nullptr;
-      d.set_device();
-      CUDA_RUNTIME(cudaMalloc(&out, n * sizeof(sb_reduce_result)));
-      c.plans.push_back(plan);
-      c.out.push_back(out);
+      if (exact) {
+        sb_reduce_exact_plan *plan = nullptr;
+        if (SB_OK != sb_reduce_exact_plan_create(&plan, d.gpu(), its.data(), int64_t(n))) LOG_FATAL("reduce: " << sb_last_error());
+        sb_reduce_exact_part *out = nullptr;
+        d.set_device();
+        CUDA_RUNTIME(cudaMalloc(&out, n * sizeof(sb_reduce_exact_part)));
+        c.xplans.push_back(plan);
+        c.xout.push_back(out);
+      } else {
+        sb_reduce_plan *plan = nullptr;
+        if (SB_OK != sb_reduce_plan_create(&plan, d.gpu(), its.data(), int64_t(n))) LOG_FATAL("reduce: " << sb_last_error());
+        sb_reduce_result *out = nullptr;
+        d.set_device();
+        CUDA_RUNTIME(cudaMalloc(&out, n * sizeof(sb_reduce_result)));
+        c.plans.push_back(plan);
+        c.out.push_back(out);
+      }
     }
     found = reducePlans_.emplace(key, std::move(c)).first;
   }
@@ -859,15 +876,19 @@ std::vector<stencil::Reduction> DistributedDomain::reduce_many(const std::vector
   }
   // 2. one launch sequence per local subdomain on its exchange stream; records: global index, then n results
   const Dim3 dim = placement_->dim();
-  const size_t rec = sizeof(int64_t) + n * sizeof(sb_reduce_result);
+  //    (exact: n sb_reduce_exact_parts, gathered unrounded)
+  const size_t res_size = exact ? sizeof(sb_reduce_exact_part) : sizeof(sb_reduce_result);
+  const size_t rec = sizeof(int64_t) + n * res_size;
   std::vector<unsigned char> mine(domains_.size() * rec);
   for (size_t di = 0; di < domains_.size(); ++di) {
     domains_[di].set_device();
-    if (SB_OK != sb_reduce_plan_launch(c.plans[di], c.out[di], streams_[di])) LOG_FATAL("reduce: " << sb_last_error());
+    const int rc = exact ? sb_reduce_exact_plan_launch(c.xplans[di], c.xout[di], streams_[di]) : sb_reduce_plan_launch(c.plans[di], c.out[di], streams_[di]);
+    if (SB_OK != rc) LOG_FATAL("reduce: " << sb_last_error());
     const Dim3 &idx = domainIdx_[di];
     const int64_t lin = idx.x + dim.x * (idx.y + dim.y * idx.z);
     std::memcpy(&mine[di * rec], &lin, sizeof(lin));
-    CUDA_RUNTIME(cudaMemcpyAsync(&mine[di * rec + sizeof(int64_t)], c.out[di], n * sizeof(sb_reduce_result), cudaMemcpyDeviceToHost, streams_[di]));
+    const void *src = exact ? static_cast<const void *>(c.xout[di]) : static_cast<const void *>(c.out[di]);
+    CUDA_RUNTIME(cudaMemcpyAsync(&mine[di * rec + sizeof(int64_t)], src, n * res_size, cudaMemcpyDeviceToHost, streams_[di]));
   }
   for (size_t di = 0; di < domains_.size(); ++di) {
     domains_[di].set_device();
@@ -896,6 +917,19 @@ std::vector<stencil::Reduction> DistributedDomain::reduce_many(const std::vector
   }
   std::sort(order.begin(), order.end());
   std::vector<stencil::Reduction> result(n);
+  if (exact) { // combined (in any order: the sums are exact), then rounded once
+    std::vector<sb_reduce_exact_part> xparts(nrec);
+    for (size_t i = 0; i < n; ++i) {
+      for (size_t k = 0; k < nrec; ++k)
+        std::memcpy(&xparts[k], &all[order[k].second * rec + sizeof(int64_t) + i * res_size], sizeof(sb_reduce_exact_part));
+      sb_reduce_exact_part tot;
+      sb_reduce_result r;
+      if (SB_OK != sb_reduce_exact_combine(xparts.data(), int64_t(nrec), &tot) || SB_OK != sb_reduce_exact_round(&tot, &r))
+        LOG_FATAL("reduce: " << sb_last_error());
+      result[i] = stencil::Reduction{r.min, r.max, r.sum, r.sumsq, r.count};
+    }
+    return result;
+  }
   std::vector<sb_reduce_result> parts(nrec);
   for (size_t i = 0; i < n; ++i) {
     for (size_t k = 0; k < nrec; ++k)

@@ -16,6 +16,7 @@ from .domain import (  # noqa: F401
     bc_regions,
     DataHandle,
     DistributedDomain,
+    ExactReducePlan,
     LocalDomain,
     Method,
     Partition,
@@ -32,6 +33,8 @@ from .domain import (  # noqa: F401
     prime_factors,
     raw_size,
     reduce_combine,
+    reduce_exact_combine,
+    reduce_exact_round,
 )
 from .stencil_op import StencilOp, StencilPlan, StencilSystem, SystemPlan  # noqa: F401
 

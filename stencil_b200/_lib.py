@@ -114,6 +114,22 @@ class ReduceResult(C.Structure):
 
 REDUCE_SCALAR, REDUCE_DIFF, REDUCE_NORM3 = 0, 1, 2  # sb_reduce_kind
 
+EXACT_WORDS = 34  # SB_EXACT_WORDS
+EXACT_NAN, EXACT_POS_INF, EXACT_NEG_INF = 1, 2, 4  # SB_EXACT_NAN, SB_EXACT_POS_INF, SB_EXACT_NEG_INF
+
+
+class ExactSum(C.Structure):
+    """sb_exact_sum: the exact sum of the finite terms, 2176-bit two's complement in units of 2^-1074 (word[0] least
+    significant), and the flags of the non-finite terms."""
+
+    _fields_ = [("word", C.c_uint64 * EXACT_WORDS), ("flags", C.c_uint64)]
+
+
+class ReduceExactPart(C.Structure):
+    """sb_reduce_exact_part"""
+
+    _fields_ = [("min", C.c_double), ("max", C.c_double), ("count", C.c_int64), ("sum", ExactSum), ("sumsq", ExactSum)]
+
 
 class StencilTerm(C.Structure):
     """sb_stencil_term: one term of a linear stencil operator (source 0 = src, 1 = aux; offset; weight)."""
@@ -190,6 +206,12 @@ _SIGS = {
     "sb_reduce_plan_bytes": (C.c_int64, [C.c_void_p]),
     "sb_reduce_plan_destroy": (C.c_int, [C.c_void_p]),
     "sb_reduce_combine": (C.c_int, [C.POINTER(ReduceResult), C.c_int64, C.POINTER(ReduceResult)]),
+    "sb_reduce_exact_plan_create": (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.POINTER(ReduceItem), C.c_int64]),
+    "sb_reduce_exact_plan_launch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
+    "sb_reduce_exact_plan_bytes": (C.c_int64, [C.c_void_p]),
+    "sb_reduce_exact_plan_destroy": (C.c_int, [C.c_void_p]),
+    "sb_reduce_exact_combine": (C.c_int, [C.POINTER(ReduceExactPart), C.c_int64, C.POINTER(ReduceExactPart)]),
+    "sb_reduce_exact_round": (C.c_int, [C.POINTER(ReduceExactPart), C.POINTER(ReduceResult)]),
     "sb_stencil_check": (C.c_int, [C.POINTER(StencilTerm), C.c_int, I27]),
     "sb_stencil_laplacian": (C.c_int, [C.c_int, C.c_double * 3, C.POINTER(StencilTerm), C.c_int]),
     "sb_stencil_plan_create": (

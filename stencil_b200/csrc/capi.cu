@@ -554,6 +554,17 @@ struct sb_reduce_plan {
   int64_t bytes = 0;
 };
 
+struct sb_reduce_exact_plan {
+  int device = 0;
+  sb::RedItem *items_dev = nullptr;
+  sb::RedTile *tiles_dev = nullptr;
+  sb::RedExactPartial *scratch = nullptr; // one partial per tile, rewritten by every launch
+  unsigned nitems = 0, ntiles = 0;
+  unsigned class_tiles[sb::kRedClasses][2] = {};
+  int grids[sb::kRedClasses] = {};
+  int64_t bytes = 0;
+};
+
 struct sb_stencil_plan {
   int device = 0;
   int es = 8, R = 1;
@@ -1203,12 +1214,20 @@ int sb_sqdiff(sb_pitched a, sb_pitched b, int dtype_size, const int64_t acc_orig
 }
 
 // ----------------------------------------------------------------------------------------- reductions
-int sb_reduce_plan_create(sb_reduce_plan **out, int device, const sb_reduce_item *items, int64_t n) {
-  if (!out || !items || n < 1) return fail(SB_ERR_INVALID, "sb_reduce_plan_create needs an output handle and n >= 1 items");
-  if (n > (1 << 20)) return fail(SB_ERR_INVALID, "at most 2^20 items per plan");
+namespace {
+// The checks, items and tile table of a reduction plan, ordered or exact (`fn` names the entry point in the messages).
+struct RedTables {
   std::vector<sb::RedItem> its;
   std::vector<sb::RedTile> tiles;
+  unsigned class_tiles[sb::kRedClasses][2];
   int64_t bytes = 0;
+};
+int reduce_tables(const char *fn, bool out_ok, const sb_reduce_item *items, int64_t n, RedTables &T) {
+  if (!out_ok || !items || n < 1) return fail(SB_ERR_INVALID, "%s needs an output handle and n >= 1 items", fn);
+  if (n > (1 << 20)) return fail(SB_ERR_INVALID, "at most 2^20 items per plan");
+  std::vector<sb::RedItem> &its = T.its;
+  std::vector<sb::RedTile> &tiles = T.tiles;
+  int64_t &bytes = T.bytes;
   for (int64_t i = 0; i < n; ++i) {
     const sb_reduce_item &I = items[i];
     const long long li = (long long)i;
@@ -1253,7 +1272,7 @@ int sb_reduce_plan_create(sb_reduce_plan **out, int device, const sb_reduce_item
     bytes += r.count * es * ns;
   }
   // the tile table, class by class; inside a class item by item
-  unsigned class_tiles[sb::kRedClasses][2];
+  unsigned(&class_tiles)[sb::kRedClasses][2] = T.class_tiles;
   for (int c = 0; c < sb::kRedClasses; ++c) {
     class_tiles[c][0] = unsigned(tiles.size());
     for (size_t i = 0; i < its.size(); ++i) {
@@ -1274,6 +1293,18 @@ int sb_reduce_plan_create(sb_reduce_plan **out, int device, const sb_reduce_item
     }
     class_tiles[c][1] = unsigned(tiles.size());
   }
+  return SB_OK;
+}
+} // namespace
+
+int sb_reduce_plan_create(sb_reduce_plan **out, int device, const sb_reduce_item *items, int64_t n) {
+  RedTables T;
+  const int rc = reduce_tables("sb_reduce_plan_create", out != nullptr, items, n, T);
+  if (rc != SB_OK) return rc;
+  const std::vector<sb::RedItem> &its = T.its;
+  const std::vector<sb::RedTile> &tiles = T.tiles;
+  const unsigned(&class_tiles)[sb::kRedClasses][2] = T.class_tiles;
+  const int64_t bytes = T.bytes;
   DeviceGuard guard(device);
   if (!guard.ok) return fail(SB_ERR_NOGPU, "cannot select CUDA device %d", device);
   sb_reduce_plan *p = new sb_reduce_plan();
@@ -1328,6 +1359,145 @@ int sb_reduce_combine(const sb_reduce_result *parts, int64_t n, sb_reduce_result
   for (int64_t s = 1; s < n; s *= 2)
     for (int64_t i = 0; i + s < n; i += 2 * s) a[size_t(i)] = sb::red_merge(a[size_t(i)], a[size_t(i + s)]);
   *out = a[0];
+  return SB_OK;
+}
+
+// ----------------------------------------------------------------------------------------- exact reductions
+int sb_reduce_exact_plan_create(sb_reduce_exact_plan **out, int device, const sb_reduce_item *items, int64_t n) {
+  RedTables T;
+  const int rc = reduce_tables("sb_reduce_exact_plan_create", out != nullptr, items, n, T);
+  if (rc != SB_OK) return rc;
+  // a tile then holds at most 2^30 cells, and the kernel's per-tile digit counters cannot overflow (reduce.cuh)
+  for (size_t i = 0; i < T.its.size(); ++i)
+    if (T.its[i].ext[0] > (1 << 27)) return fail(SB_ERR_INVALID, "item %lld: rows of more than 2^27 cells", (long long)i);
+  DeviceGuard guard(device);
+  if (!guard.ok) return fail(SB_ERR_NOGPU, "cannot select CUDA device %d", device);
+  sb_reduce_exact_plan *p = new sb_reduce_exact_plan();
+  p->device = device;
+  p->bytes = T.bytes;
+  p->nitems = unsigned(T.its.size());
+  p->ntiles = unsigned(T.tiles.size());
+  cudaError_t e = cudaMalloc(&p->items_dev, T.its.size() * sizeof(sb::RedItem));
+  if (e == cudaSuccess) e = cudaMalloc(&p->tiles_dev, std::max<size_t>(1, T.tiles.size()) * sizeof(sb::RedTile));
+  if (e == cudaSuccess) e = cudaMalloc(&p->scratch, std::max<size_t>(1, T.tiles.size()) * sizeof(sb::RedExactPartial));
+  if (e == cudaSuccess) e = cudaMemcpy(p->items_dev, T.its.data(), T.its.size() * sizeof(sb::RedItem), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess && !T.tiles.empty())
+    e = cudaMemcpy(p->tiles_dev, T.tiles.data(), T.tiles.size() * sizeof(sb::RedTile), cudaMemcpyHostToDevice);
+  if (e != cudaSuccess) {
+    sb_reduce_exact_plan_destroy(p);
+    return fail(SB_ERR_CUDA, "reduction plan upload: %s", cudaGetErrorString(e));
+  }
+  for (int c = 0; c < sb::kRedClasses; ++c) {
+    p->class_tiles[c][0] = T.class_tiles[c][0];
+    p->class_tiles[c][1] = T.class_tiles[c][1];
+    p->grids[c] = sb::reduce_exact_grid(device, c, T.class_tiles[c][1] - T.class_tiles[c][0]);
+  }
+  *out = p;
+  return SB_OK;
+}
+
+int sb_reduce_exact_plan_launch(sb_reduce_exact_plan *p, sb_reduce_exact_part *out_dev, void *stream) {
+  if (!p) return fail(SB_ERR_INVALID, "null plan");
+  if (!out_dev) return fail(SB_ERR_INVALID, "null output buffer");
+  DeviceGuard guard(p->device);
+  if (!guard.ok) return fail(SB_ERR_NOGPU, "cannot select CUDA device %d", p->device);
+  g_launches += uint64_t(sb::launch_reduce_exact(p->items_dev, p->nitems, p->tiles_dev, p->class_tiles, p->grids, p->scratch, out_dev,
+                                                 static_cast<cudaStream_t>(stream)));
+  SB_CUDA(cudaGetLastError());
+  return SB_OK;
+}
+
+int64_t sb_reduce_exact_plan_bytes(const sb_reduce_exact_plan *p) { return p ? p->bytes : 0; }
+
+int sb_reduce_exact_plan_destroy(sb_reduce_exact_plan *p) {
+  if (!p) return SB_OK;
+  DeviceGuard guard(p->device);
+  if (p->items_dev) cudaFree(p->items_dev);
+  if (p->tiles_dev) cudaFree(p->tiles_dev);
+  if (p->scratch) cudaFree(p->scratch);
+  delete p;
+  return SB_OK;
+}
+
+namespace {
+uint64_t bits_of(double x) {
+  uint64_t b;
+  std::memcpy(&b, &x, sizeof b);
+  return b;
+}
+// min / max whose result does not depend on the operand order: a NaN wins (of two, the larger bit pattern); of +0 and
+// -0 min takes -0, max +0
+double exact_min(double a, double b) {
+  if (a != a || b != b) return (a != a && b != b) ? (bits_of(a) > bits_of(b) ? a : b) : (a != a ? a : b);
+  if (a != b) return a < b ? a : b;
+  return std::signbit(a) ? a : b;
+}
+double exact_max(double a, double b) {
+  if (a != a || b != b) return (a != a && b != b) ? (bits_of(a) > bits_of(b) ? a : b) : (a != a ? a : b);
+  if (a != b) return a > b ? a : b;
+  return std::signbit(a) ? b : a;
+}
+void exact_add(sb_exact_sum &a, const sb_exact_sum &b) {
+  unsigned carry = 0;
+  for (int k = 0; k < SB_EXACT_WORDS; ++k) {
+    const uint64_t s = a.word[k] + b.word[k];
+    const unsigned c1 = s < a.word[k];
+    a.word[k] = s + carry;
+    carry = c1 | (a.word[k] < s);
+  }
+  a.flags |= b.flags;
+}
+// the exact sum rounded to nearest, ties to even, with the special-value rule of include/stencil_b200.h
+double exact_round(const sb_exact_sum &e) {
+  if ((e.flags & SB_EXACT_NAN) || ((e.flags & SB_EXACT_POS_INF) && (e.flags & SB_EXACT_NEG_INF))) return std::nan("");
+  if (e.flags & SB_EXACT_POS_INF) return HUGE_VAL;
+  if (e.flags & SB_EXACT_NEG_INF) return -HUGE_VAL;
+  uint64_t m[SB_EXACT_WORDS];
+  const bool neg = e.word[SB_EXACT_WORDS - 1] >> 63;
+  unsigned carry = 1;
+  for (int k = 0; k < SB_EXACT_WORDS; ++k) { // magnitude: two's complement negation for a negative sum
+    m[k] = neg ? ~e.word[k] + carry : e.word[k];
+    if (neg) carry = carry && m[k] == 0;
+  }
+  int top = -1; // highest set bit, in units of 2^-1074
+  for (int k = SB_EXACT_WORDS - 1; k >= 0 && top < 0; --k)
+    if (m[k]) top = 64 * k + 63 - __builtin_clzll(m[k]);
+  if (top < 0) return 0.0;
+  auto bit = [&](int i) { return i >= 0 ? int((m[i / 64] >> (i % 64)) & 1u) : 0; };
+  double r;
+  if (top < 53) {
+    r = std::ldexp(double(m[0]), -1074); // below 2^53 units: exact (subnormal or the smallest normal binade)
+  } else {
+    const int lsb = top - 52; // the 53 kept bits are [lsb, top]
+    uint64_t mant = 0;
+    for (int i = top; i >= lsb; --i) mant = (mant << 1) | uint64_t(bit(i));
+    bool sticky = false;
+    for (int i = 0; i < lsb - 1 && !sticky; ++i) sticky = bit(i);
+    if (bit(lsb - 1) && (sticky || (mant & 1u))) ++mant; // 2^53 stays exact: ldexp scales it
+    r = std::ldexp(double(mant), lsb - 1074);            // beyond the double range: inf
+  }
+  return neg ? -r : r;
+}
+} // namespace
+
+int sb_reduce_exact_combine(const sb_reduce_exact_part *parts, int64_t n, sb_reduce_exact_part *out) {
+  if (!parts || !out || n < 1) return fail(SB_ERR_INVALID, "sb_reduce_exact_combine needs n >= 1 parts and an output");
+  sb_reduce_exact_part r = parts[0];
+  for (int64_t i = 1; i < n; ++i) {
+    const sb_reduce_exact_part &b = parts[i];
+    r.min = exact_min(r.min, b.min);
+    r.max = exact_max(r.max, b.max);
+    r.count += b.count;
+    exact_add(r.sum, b.sum);
+    exact_add(r.sumsq, b.sumsq);
+  }
+  *out = r;
+  return SB_OK;
+}
+
+int sb_reduce_exact_round(const sb_reduce_exact_part *part, sb_reduce_result *out) {
+  if (!part || !out) return fail(SB_ERR_INVALID, "sb_reduce_exact_round needs a part and an output");
+  *out = sb_reduce_result{part->min, part->max, exact_round(part->sum), exact_round(part->sumsq), part->count};
   return SB_OK;
 }
 

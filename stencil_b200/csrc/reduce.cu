@@ -4,18 +4,12 @@
 namespace sb {
 namespace {
 
-template <typename T, int N> struct Vec { using type = T; };
-template <> struct Vec<float, 4> { using type = float4; };
-template <> struct Vec<double, 2> { using type = double2; };
-
-__device__ __forceinline__ double pos_inf() { return __longlong_as_double(0x7ff0000000000000ll); }
-
 struct Acc {
   double mn, mx, s, q;
 };
 
-// One cell: v and its squared term q, formed with separately rounded operations (no FMA contraction), then one step of
-// each chain.  `v < mn || v != v` keeps a NaN once it is in and lets a NaN in.
+// One cell: v and q (the operations of cell_terms, written out so that the SASS stays as it is), then one step of each
+// chain.  `v < mn || v != v` keeps a NaN once it is in and lets a NaN in.
 template <int KIND> __device__ __forceinline__ void add(Acc &a, double x, double y, double z) {
   double v, q;
   if (KIND == SB_REDUCE_SCALAR) {
@@ -34,73 +28,7 @@ template <int KIND> __device__ __forceinline__ void add(Acc &a, double x, double
   a.q = __dadd_rn(a.q, q);
 }
 
-template <int KIND> __host__ __device__ constexpr int num_sources() { return KIND == SB_REDUCE_SCALAR ? 1 : KIND == SB_REDUCE_DIFF ? 2 : 3; }
-
-template <typename T, int KIND> __device__ __forceinline__ void add_cell(Acc &a, const char *const *p, unsigned j) {
-  constexpr int NS = num_sources<KIND>();
-  double x[3] = {0, 0, 0};
-#pragma unroll
-  for (int s = 0; s < NS; ++s) x[s] = double(__ldg(reinterpret_cast<const T *>(p[s]) + j));
-  add<KIND>(a, x[0], x[1], x[2]);
-}
-
-// The rows of one tile.  WIDE: cells [0, head) and [tail0, nx) of a row are read one by one (head brings the address to
-// a 16-byte boundary), the body in 16-byte vectors; otherwise every access is one element.  Lane l of a row's group
-// reads head / tail cells l, l + G, ... and body vectors l, l + G, ..., four per source in flight.
-template <typename T, int KIND, bool WIDE> __device__ void reduce_rows(const RedItem &it, const RedTile &t, Acc &a) {
-  constexpr int NS = num_sources<KIND>();
-  constexpr int N = WIDE ? 16 / int(sizeof(T)) : 1;
-  using V = typename Vec<T, N>::type;
-  const unsigned lg = unsigned(it.lg_group), G = 1u << lg;
-  const unsigned lane = threadIdx.x & (G - 1), per_pass = unsigned(kRedThreads) >> lg;
-  const unsigned nx = unsigned(it.ext[0]), ey = unsigned(it.ext[1]);
-#pragma unroll 1
-  for (unsigned r = threadIdx.x >> lg; r < t.nrows; r += per_pass) {
-    const unsigned row = t.row0 + r;
-    const long long off = (long long)(row / ey) * it.slice + (long long)(row % ey) * it.pitch;
-    const char *p[NS];
-#pragma unroll
-    for (int s = 0; s < NS; ++s) p[s] = it.src[s] + off;
-    unsigned head = 0;
-    if (WIDE) {
-      head = unsigned((16 - (reinterpret_cast<uintptr_t>(p[0]) & 15)) & 15) / unsigned(sizeof(T));
-      head = head < nx ? head : nx;
-    }
-    const unsigned nvec = (nx - head) / unsigned(N);
-    if (WIDE) {
-#pragma unroll 1
-      for (unsigned j = lane; j < head; j += G) add_cell<T, KIND>(a, p, j);
-#pragma unroll 1
-      for (unsigned j = head + nvec * unsigned(N) + lane; j < nx; j += G) add_cell<T, KIND>(a, p, j);
-    }
-    const V *vp[NS];
-#pragma unroll
-    for (int s = 0; s < NS; ++s) vp[s] = reinterpret_cast<const V *>(p[s] + size_t(head) * sizeof(T));
-#pragma unroll 1
-    for (unsigned c = lane; c < nvec; c += 4 * G) {
-      V w[4][NS];
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        const unsigned i = c + unsigned(k) * G;
-#pragma unroll
-        for (int s = 0; s < NS; ++s)
-          if (i < nvec) w[k][s] = __ldg(vp[s] + i);
-      }
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        if (c + unsigned(k) * G < nvec) {
-#pragma unroll
-          for (int e = 0; e < N; ++e) {
-            double x[3] = {0, 0, 0};
-#pragma unroll
-            for (int s = 0; s < NS; ++s) x[s] = double(reinterpret_cast<const T *>(&w[k][s])[e]);
-            add<KIND>(a, x[0], x[1], x[2]);
-          }
-        }
-      }
-    }
-  }
-}
+#include "reduce_rows.cuh"
 
 __device__ __forceinline__ sb_reduce_result as_result(const Acc &a) { return sb_reduce_result{a.mn, a.mx, a.s, a.q, 0}; }
 __device__ __forceinline__ Acc as_acc(const sb_reduce_result &r) { return Acc{r.min, r.max, r.sum, r.sumsq}; }
@@ -121,7 +49,7 @@ __global__ void __launch_bounds__(kRedThreads) reduce_tiles_kernel(const RedItem
     }
     __syncthreads();
     Acc a{pos_inf(), -pos_inf(), 0.0, 0.0};
-    reduce_rows<T, KIND, WIDE>(it, t, a);
+    reduce_rows<T, KIND, WIDE, Acc>(it, t, a);
     // the block's 256 chains: a fixed tree, lane l + o into lane l for o = 16, 8, 4, 2, 1, then warps 2i + 1 into 2i,
     // 4i + 2 into 4i, 4 into 0
 #pragma unroll
@@ -184,16 +112,18 @@ ClassKernel class_kernel(int c) {
 
 int reduce_class(const RedItem &it) { return 6 * (it.dtype == SB_DTYPE_F64) + 2 * it.kind + (it.vec == 16); }
 
-int reduce_grid(int device, int cls, unsigned ntiles) {
+int persistent_grid(int device, const void *kernel, unsigned ntiles) {
   int sms = 132, per_sm = 1;
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, class_kernel(cls), kRedThreads, 0) != cudaSuccess || per_sm < 1) {
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kRedThreads, 0) != cudaSuccess || per_sm < 1) {
     cudaGetLastError();
     per_sm = 1;
   }
   const long long cap = (long long)sms * per_sm;
   return int(ntiles < cap ? ntiles : cap);
 }
+
+int reduce_grid(int device, int cls, unsigned ntiles) { return persistent_grid(device, reinterpret_cast<const void *>(class_kernel(cls)), ntiles); }
 
 int launch_reduce(const RedItem *items_dev, unsigned nitems, const RedTile *tiles_dev, const unsigned (*class_tiles)[2], const int *grids,
                   RedPartial *scratch, sb_reduce_result *out, cudaStream_t stream) {

@@ -421,6 +421,69 @@ class ReducePlan:
             pass
 
 
+def reduce_exact_combine(parts: Sequence[_lib.ReduceExactPart]) -> _lib.ReduceExactPart:
+    """sb_reduce_exact_combine: parts (e.g. one per subdomain) merged; the result does not depend on their order."""
+    arr = (_lib.ReduceExactPart * max(1, len(parts)))(*parts)
+    out = _lib.ReduceExactPart()
+    check(lib().sb_reduce_exact_combine(arr, len(parts), C.byref(out)))
+    return out
+
+
+def reduce_exact_round(part: _lib.ReduceExactPart) -> Reduction:
+    """sb_reduce_exact_round: min, max and count as they are, sum and sumsq correctly rounded."""
+    out = _lib.ReduceResult()
+    check(lib().sb_reduce_exact_round(C.byref(part), C.byref(out)))
+    return Reduction.of(out)
+
+
+class ExactReducePlan:
+    """sb_reduce_exact_plan: the items of a ReducePlan with exact sums; results are sb_reduce_exact_parts, to be
+    combined across subdomains and then rounded.  One launch in flight at a time."""
+
+    def __init__(self, device: int, items: Sequence[_lib.ReduceItem]):
+        arr = (_lib.ReduceItem * len(items))(*items)
+        h = C.c_void_p()
+        check(lib().sb_reduce_exact_plan_create(C.byref(h), device, arr, len(items)))
+        self._h = h
+        self.device = device
+        self.n = len(items)
+        self.bytes = int(lib().sb_reduce_exact_plan_bytes(h))
+        out = C.c_void_p()
+        nbytes = self.n * C.sizeof(_lib.ReduceExactPart)
+        if lib().sb_malloc(C.byref(out), nbytes, device) != 0:
+            self.destroy()
+            raise _lib.StencilError(f"reduction output buffer: {lib().sb_last_error().decode()}")
+        self.out_dev = out.value
+
+    def launch(self, stream=None) -> None:
+        check(lib().sb_reduce_exact_plan_launch(self._h, C.c_void_p(self.out_dev), stream_ptr(stream)))
+
+    def parts(self, stream=None) -> List[_lib.ReduceExactPart]:
+        """Copy the last launch's parts (ordered after it on `stream`) to the host."""
+        host = (_lib.ReduceExactPart * self.n)()
+        check(lib().sb_memcpy(C.addressof(host), C.c_void_p(self.out_dev), C.sizeof(host), self.device, stream_ptr(stream)))
+        check(lib().sb_stream_sync(self.device, stream_ptr(stream)))
+        return list(host)
+
+    def results(self, stream=None) -> List[Reduction]:
+        """The last launch's parts, each rounded: the whole result when the plan covers the whole region."""
+        return [reduce_exact_round(p) for p in self.parts(stream)]
+
+    def destroy(self) -> None:
+        if getattr(self, "out_dev", None):
+            lib().sb_free(C.c_void_p(self.out_dev), self.device)
+            self.out_dev = None
+        if self._h:
+            lib().sb_reduce_exact_plan_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.destroy()
+        except Exception:
+            pass
+
+
 # ------------------------------------------------------------------------------------------ LocalDomain
 class LocalDomain:
     """One subdomain on one GPU: curr/next allocation per quantity (local_domain.cuh:34-276,
@@ -1065,53 +1128,63 @@ class DistributedDomain:
     # -- reductions
     _REDUCE_KINDS = {"scalar": (_lib.REDUCE_SCALAR, 1), "diff": (_lib.REDUCE_DIFF, 1), "norm": (_lib.REDUCE_NORM3, 3)}
 
-    def reduce(self, h: DataHandle, which: str = "curr") -> Reduction:
-        """min, max, sum and sum of squares of quantity h (its curr or next buffer) over the whole compute region."""
-        return self.reduce_many([("scalar", h, which)])[0]
+    def reduce(self, h: DataHandle, which: str = "curr", exact: bool = False) -> Reduction:
+        """min, max, sum and sum of squares of quantity h (its curr or next buffer) over the whole compute region.
+        exact=True: sum and sumsq correctly rounded, the same bits for every partition (sb_reduce_exact_*)."""
+        return self.reduce_many([("scalar", h, which)], exact=exact)[0]
 
-    def reduce_diff(self, h: DataHandle) -> Reduction:
+    def reduce_diff(self, h: DataHandle, exact: bool = False) -> Reduction:
         """The same statistics of curr - next of quantity h; .l2() is the 2-norm of the last update after a swap."""
-        return self.reduce_many([("diff", h)])[0]
+        return self.reduce_many([("diff", h)], exact=exact)[0]
 
-    def reduce_norm(self, hx: DataHandle, hy: DataHandle, hz: DataHandle) -> Reduction:
+    def reduce_norm(self, hx: DataHandle, hy: DataHandle, hz: DataHandle, exact: bool = False) -> Reduction:
         """Statistics of |u| = sqrt(hx^2 + hy^2 + hz^2) (curr buffers); .rms() is sqrt(sum |u|^2 / N)."""
-        return self.reduce_many([("norm", hx, hy, hz)])[0]
+        return self.reduce_many([("norm", hx, hy, hz)], exact=exact)[0]
 
-    def reduce_plans(self, items: Sequence[tuple]) -> List[ReducePlan]:
-        """The plans reduce_many(items) launches, one per local subdomain, for the current swap parity.  They are built
-        on first use and kept, per item list and parity, until close(): a program should reduce a fixed set of item
-        lists rather than build a new list every iteration, or each new list holds device memory until close()."""
+    def reduce_plans(self, items: Sequence[tuple], exact: bool = False) -> list:
+        """The plans reduce_many(items, exact) launches, one per local subdomain, for the current swap parity
+        (ReducePlan, or ExactReducePlan with exact=True).  They are built on first use and kept, per item list,
+        exactness and parity, until close(): a program should reduce a fixed set of item lists rather than build a new
+        list every iteration, or each new list holds device memory until close()."""
         keys = [self._reduce_key(it) for it in items]
         if not keys:
             raise _lib.StencilError("reduce_plans: no items")
-        ck = (tuple(keys), self._parity)
+        ck = (tuple(keys), self._parity, bool(exact))
         plans = self._reduce_plans.get(ck)
         if plans is None:
-            plans = [ReducePlan(d.gpu(), [self._reduce_item(di, k) for k in keys]) for di, d in enumerate(self.domains_)]
+            cls = ExactReducePlan if exact else ReducePlan
+            plans = [cls(d.gpu(), [self._reduce_item(di, k) for k in keys]) for di, d in enumerate(self.domains_)]
             self._reduce_plans[ck] = plans
         return plans
 
-    def reduce_many(self, items: Sequence[tuple]) -> List[Reduction]:
+    def reduce_many(self, items: Sequence[tuple], exact: bool = False) -> List[Reduction]:
         """Several reductions, one launch sequence per local subdomain.  Items: ("scalar", h[, "curr" | "next"]),
         ("diff", h) (curr - next), ("norm", hx, hy, hz).  Waits for all work queued on the local devices, reduces on
         the exchange streams, gathers every rank's per-subdomain results and merges them with sb_reduce_combine in
-        global subdomain-index order (x fastest), so every rank returns the same bits.  Collective under torchrun.  The
-        plans are cached as reduce_plans() describes."""
+        global subdomain-index order (x fastest), so every rank returns the same bits.  exact=True: the per-subdomain
+        exact parts are gathered, combined by sb_reduce_exact_combine and rounded once, so sum and sumsq are correctly
+        rounded and the same bits for every partition and rank count.  Collective under torchrun.  The plans are cached
+        as reduce_plans() describes."""
         from . import dist as _dist
 
         if not items:
             return []
         n = len(items)
-        plans = self.reduce_plans(items)
+        plans = self.reduce_plans(items, exact)
         for dev in sorted({d.gpu() for d in self.domains_}):
             check(lib().sb_device_sync(dev))
         for plan, s in zip(plans, self._streams):
             plan.launch(s)
         dim = self.partition_.dim
-        mine = [(idx, [(r.min, r.max, r.sum, r.sumsq, r.count) for r in plan.results(s)])
-                for idx, plan, s in zip(self.domain_idx_, plans, self._streams)]  # fmt: skip
+        if exact:
+            mine = [(idx, [bytes(p) for p in plan.parts(s)]) for idx, plan, s in zip(self.domain_idx_, plans, self._streams)]
+        else:
+            mine = [(idx, [(r.min, r.max, r.sum, r.sumsq, r.count) for r in plan.results(s)])
+                    for idx, plan, s in zip(self.domain_idx_, plans, self._streams)]  # fmt: skip
         everyone = _dist.all_gather_object(mine) if self._world.size > 1 else [mine]
         parts = sorted((p for rank_parts in everyone for p in rank_parts), key=lambda p: p[0][0] + dim[0] * (p[0][1] + dim[1] * p[0][2]))
+        if exact:
+            return [reduce_exact_round(reduce_exact_combine([_lib.ReduceExactPart.from_buffer_copy(p[1][i]) for p in parts])) for i in range(n)]
         return [reduce_combine([Reduction(*p[1][i]) for p in parts]) for i in range(n)]
 
     def _reduce_key(self, it: tuple) -> tuple:
