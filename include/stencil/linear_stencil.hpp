@@ -10,6 +10,10 @@
 //     // u + dt div(kappa grad u), kappa on the x / y / z faces in three quantities (their curr buffers)
 //     stencil::LinearStencil kheat = stencil::LinearStencil::div_grad(hx, hy, hz).scaled(dt).add(stencil::Source::src, 0, 0, 0, 1.0);
 //     dd.apply(kheat, stencil::next(h), h, {kx, ky, kz});
+//
+//     // Gauss-Seidel / SOR for A u = f (DESIGN.md section 2.9): one coloured apply per colour, in place, f on aux
+//     stencil::LinearStencil sor = stencil::LinearStencil::laplacian(2, h, h, h).scaled(-1.0).relax(omega);
+//     for (int c = 0; c < 2; ++c) dd.apply(sor, stencil::curr(u), u, stencil::curr(f), stencil::Colour{2, c});
 #include <cstdint>
 #include <vector>
 
@@ -21,6 +25,12 @@
 namespace stencil {
 
 enum class Source { src = 0, aux = 1 };
+
+// A colouring m (1, 2 or 8) and one of its colours c (0 .. m-1), from global coordinates: m = 2 is red-black,
+// (x + y + z) mod 2; m = 8 is (x mod 2) + 2 (y mod 2) + 4 (z mod 2).  A coloured apply writes the cells of colour c only.
+struct Colour {
+  int m = 1, c = 0;
+};
 
 // An operator: terms (source, offset, weight) applied in list order, each of which may also read a coefficient field k at
 // an offset of reach 1 (then it contributes (T(w) * C_k) * S).  Terms on aux have offset 0.
@@ -65,6 +75,19 @@ public:
     std::vector<sb_stencil_vterm> terms(static_cast<size_t>(n));
     sb_stencil_div_grad(h, terms.data(), n);
     return LinearStencil(terms);
+  }
+  // the SOR update of A u = f for this op A (constant coefficients, one centre term, no aux term), f on aux:
+  // u + omega (f - A u) / a_c (sb_stencil_relax).  omega = 1 in a coloured sweep is Gauss-Seidel; omega outside (0, 2)
+  // diverges for a symmetric positive definite A.
+  LinearStencil relax(double omega) const {
+    for (const sb_stencil_vterm &t : vterms_)
+      if (t.coef >= 0) LOG_FATAL("LinearStencil::relax: the op has coefficient terms; the relaxation table takes constant coefficients");
+    const int n = int(terms_.size());
+    std::vector<sb_stencil_term> out(static_cast<size_t>(n + 1));
+    const int m = sb_stencil_relax(terms_.data(), n, omega, out.data(), n + 1);
+    if (m < 0) LOG_FATAL("LinearStencil::relax: " << sb_last_error());
+    out.resize(static_cast<size_t>(m));
+    return LinearStencil(std::move(out));
   }
   // the central-difference Laplacian of order 2, 4, 6 or 8 on a grid of spacing (hx, hy, hz): sb_stencil_laplacian
   static LinearStencil laplacian(int order, double hx, double hy, double hz) {

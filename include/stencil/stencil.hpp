@@ -136,13 +136,15 @@ private:
   std::vector<cudaStream_t> applyStreams_;
   void destroy_stencil_plans();
   void apply_op(const stencil::LinearStencil &op, int dtype, size_t dq, stencil::Which dw, size_t sq, int64_t aq, stencil::Which aw,
-                const std::vector<size_t> &cq, bool exchange);
+                const std::vector<size_t> &cq, bool exchange, stencil::Colour colour = stencil::Colour{});
   void apply_sys(const stencil::LinearSystem &sys, int dtype, const std::vector<std::pair<size_t, stencil::Which>> &outs,
                  const std::vector<std::pair<size_t, stencil::Which>> &ins, bool exchange);
   // the schedule apply_op and apply_sys share: the cached per-domain plans of key (built by make(domain, boxes) on first
   // use), then the interior plans on their own streams while exchange() runs and the exterior plans after it, or the one
-  // whole-region plan per domain; returns when every launch is complete
-  void run_stencil_plans(const std::vector<int64_t> &key, bool exchange,
+  // whole-region plan per domain; returns when every launch is complete.  writes_src: the launch writes src (a coloured
+  // apply in place), so the interior also keeps clear of the slabs exchange() sends, which are as wide as the radius on
+  // the opposite side.
+  void run_stencil_plans(const std::vector<int64_t> &key, bool exchange, bool writes_src,
                          const std::function<sb_stencil_plan *(size_t, const std::vector<Rect3> &)> &make);
 
   std::string outputPrefix_;
@@ -313,6 +315,31 @@ public:
   void apply(const stencil::LinearStencil &op, const stencil::Buffer<T> &dst, const DataHandle<T> &src, const stencil::Buffer<T> &aux,
              const std::vector<DataHandle<T>> &coefs, bool exchange = true) {
     apply_op(op, stencil::bc_dtype<T>(), dst.h.id(), dst.which, src.id(), int64_t(aux.h.id()), aux.which, ids_of(coefs), exchange);
+  }
+  // Coloured applies (DESIGN.md section 2.9): only the cells of colour colour.c of the colouring colour.m are written,
+  // each from the buffers as they were before the call; with m > 1 dst may be src (curr(src)), and every src term with a
+  // non-zero offset must read another colour (sb_stencil_ccheck).  A Gauss-Seidel / SOR sweep is one call per colour:
+  //     for (int c = 0; c < 2; ++c) dd.apply(sor, stencil::curr(u), u, stencil::curr(f), stencil::Colour{2, c});
+  // Schedule, plan cache (with the colouring in its key) and failure rules are the uncoloured apply's.
+  template <typename T>
+  void apply(const stencil::LinearStencil &op, const stencil::Buffer<T> &dst, const DataHandle<T> &src, stencil::Colour colour,
+             bool exchange = true) {
+    apply_op(op, stencil::bc_dtype<T>(), dst.h.id(), dst.which, src.id(), -1, stencil::Which::curr, {}, exchange, colour);
+  }
+  template <typename T>
+  void apply(const stencil::LinearStencil &op, const stencil::Buffer<T> &dst, const DataHandle<T> &src, const stencil::Buffer<T> &aux,
+             stencil::Colour colour, bool exchange = true) {
+    apply_op(op, stencil::bc_dtype<T>(), dst.h.id(), dst.which, src.id(), int64_t(aux.h.id()), aux.which, {}, exchange, colour);
+  }
+  template <typename T>
+  void apply(const stencil::LinearStencil &op, const stencil::Buffer<T> &dst, const DataHandle<T> &src, const std::vector<DataHandle<T>> &coefs,
+             stencil::Colour colour, bool exchange = true) {
+    apply_op(op, stencil::bc_dtype<T>(), dst.h.id(), dst.which, src.id(), -1, stencil::Which::curr, ids_of(coefs), exchange, colour);
+  }
+  template <typename T>
+  void apply(const stencil::LinearStencil &op, const stencil::Buffer<T> &dst, const DataHandle<T> &src, const stencil::Buffer<T> &aux,
+             const std::vector<DataHandle<T>> &coefs, stencil::Colour colour, bool exchange = true) {
+    apply_op(op, stencil::bc_dtype<T>(), dst.h.id(), dst.which, src.id(), int64_t(aux.h.id()), aux.which, ids_of(coefs), exchange, colour);
   }
   // outputs = sys(inputs) over the whole compute region of every local subdomain (DESIGN.md section 2.8): sys.nout()
   // outputs and sys.nin() inputs, each the curr or next buffer of a quantity of the system's type.  An input read at a

@@ -405,6 +405,45 @@ int sb_stencil_vplan_create(sb_stencil_plan **out, int device, int dtype, const 
                             int64_t zsize, int nbox, const int64_t *lo, const int64_t *hi);
 
 /* ---------------------------------------------------------------------------------------------
+ * Coloured application (DESIGN.md section 2.9): Gauss-Seidel and SOR sweeps in place.  A colouring m is 1, 2 or 8 and a
+ * colour c is 0 .. m-1, taken from the GLOBAL compute coordinates (x, y, z) of a cell:
+ *   m = 1: every cell has colour 0 (the uncoloured rule)
+ *   m = 2: colour (x + y + z) mod 2 (red-black)
+ *   m = 8: colour (x mod 2) + 2 (y mod 2) + 4 (z mod 2)
+ * A coloured launch evaluates the op rule above (plain or coefficient terms) on the buffers AS THEY WERE BEFORE THE
+ * LAUNCH and writes dst[p] = op(p) for the cells p of the boxes of colour c only; every other cell of dst keeps its bits.
+ * With m > 1, dst may be src (in place).  The colour condition: every src term with o != 0 reads a cell of another colour
+ * than its own, for every cell, that is o_x + o_y + o_z odd for m = 2 and some o_a odd for m = 8.  It is checked
+ * whenever m > 1, in place or not: a coloured op that reads its own colour is not a Gauss-Seidel sweep.  Aux terms keep
+ * offset 0 and aux may be dst (so src as well); coefficient fields must not be dst, so in place they cannot be src.
+ * Coefficient reads need no colour condition: nothing writes them.  On a periodic axis of odd length a cell and its
+ * wrapped neighbour can share a colour; that read goes through a ghost cell and sees the old value, as the rule says.
+ * Consequence: in place, "before the launch" and "in any order" give the same bits.  Every value a cell uses is its own
+ * old value (read before its own write), a cell of another colour (which nothing writes) or a ghost cell (which nothing
+ * writes), so a kernel races only on values it never uses.  A sweep is one launch per colour, each after an exchange:
+ *   for c in 0 .. m-1:  exchange();  apply the op with colouring (m, c), dst = src = u
+ * and it gives the same bits on every partition.
+ * ------------------------------------------------------------------------------------------- */
+/* Host only.  sb_stencil_vcheck plus, for ncolours > 1, the colour condition.  SB_ERR_INVALID with a message for
+ * ncolours not 1, 2 or 8, or a term that reads its own colour (naming the term and its offset). */
+int sb_stencil_ccheck(const sb_stencil_vterm *terms, int n, const int64_t radius27[27], int ncolours);
+/* Host only.  The SOR update of A u = f (f on aux): u <- u + omega (f - A u) / a_c, for a constant-coefficient op A with
+ * exactly one src term at offset 0 (weight a_c != 0) and no aux term.  Terms, in order, weights in double with exactly
+ * this association: the centre (src, 0, 1 - omega); each off-centre src term (src, o, w) of A, in A's order, as
+ * (src, o, (-omega * w) / a_c); then (aux, 0, omega / a_c).  omega = 1 is Gauss-Seidel (in a coloured sweep) or Jacobi
+ * (out of place); 0 < omega < 2 is over- / under-relaxation.  omega outside (0, 2) is accepted but diverges for a
+ * symmetric positive definite A.  Writes at most cap terms (out may be NULL with cap 0) and returns n + 1, or
+ * SB_ERR_INVALID for an invalid term list, no centre term, two centre terms, a_c = 0, an aux term or omega not finite. */
+int sb_stencil_relax(const sb_stencil_term *A, int n, double omega, sb_stencil_term *out, int cap);
+/* sb_stencil_vplan_create with a colouring: ncolours m and colour c.  sb_stencil_vplan_create is this call with m = 1,
+ * c = 0.  Errors beyond sb_stencil_vplan_create's (SB_ERR_INVALID with a message, before anything is allocated): m not 1,
+ * 2 or 8, c outside 0 .. m-1, a term that reads its own colour; dst == src only when m = 1.  sb_stencil_plan_bytes of a
+ * coloured plan counts the reads of every cell of the boxes and one element written per cell of the colour. */
+int sb_stencil_cplan_create(sb_stencil_plan **out, int device, int dtype, const sb_stencil_vterm *terms, int n, sb_pitched dst,
+                            sb_pitched src, sb_pitched aux, const sb_pitched *coef, int ncoef, int ncolours, int colour,
+                            const int64_t acc_origin[3], int64_t zsize, int nbox, const int64_t *lo, const int64_t *hi);
+
+/* ---------------------------------------------------------------------------------------------
  * Linear stencil systems: one launch over nin input and nout output allocations.  A term of output j reads input
  * `input` at p + o (|o_a| <= SB_STENCIL_MAX_REACH) and, if coef >= 0, input `coef` at p + c (|c_a| <=
  * SB_STENCIL_COEF_REACH) as its coefficient.  For each output j, over the terms with output == j in list order (terms of

@@ -655,13 +655,15 @@ void DistributedDomain::destroy_stencil_plans() {
 }
 
 void DistributedDomain::apply_op(const stencil::LinearStencil &op, int dtype, size_t dq, stencil::Which dw, size_t sq, int64_t aq,
-                                 stencil::Which aw, const std::vector<size_t> &cq, bool exchange) {
+                                 stencil::Which aw, const std::vector<size_t> &cq, bool exchange, stencil::Colour colour) {
   using stencil::Which;
   if (domains_.empty() || plans_[0].size() != domains_.size()) LOG_FATAL("apply: call realize() first");
   if (dtype != SB_DTYPE_F32 && dtype != SB_DTYPE_F64) LOG_FATAL("apply: a stencil operator computes in float or double");
   for (const int64_t q : {int64_t(dq), int64_t(sq), aq})
     if (q >= 0 && (size_t(q) >= dataDtype_.size() || dataDtype_[size_t(q)] != dtype)) LOG_FATAL("apply: unknown data handle " << q);
-  if (dq == sq && dw == Which::curr) LOG_FATAL("apply: dst must not be src");
+  if ((colour.m != 1 && colour.m != 2 && colour.m != 8) || colour.c < 0 || colour.c >= colour.m)
+    LOG_FATAL("apply: colour (" << colour.m << ", " << colour.c << ") must have m = 1, 2 or 8 and 0 <= c < m");
+  if (dq == sq && dw == Which::curr && colour.m == 1) LOG_FATAL("apply: dst must not be src");
   if (op.has_aux() && aq < 0) LOG_FATAL("apply: the op has a term on aux, but no aux buffer was given");
   if (int(cq.size()) != op.ncoef()) LOG_FATAL("apply: the op reads " << op.ncoef() << " coefficient fields, but " << cq.size() << " were given");
   for (size_t k = 0; k < cq.size(); ++k) {
@@ -673,17 +675,17 @@ void DistributedDomain::apply_op(const stencil::LinearStencil &op, int dtype, si
     for (int y = -1; y <= 1; ++y)
       for (int x = -1; x <= 1; ++x) r27[i++] = int64_t(radius_.dir(x, y, z));
   const std::vector<sb_stencil_vterm> &terms = op.vterms();
-  if (SB_OK != sb_stencil_vcheck(terms.data(), int(terms.size()), r27)) LOG_FATAL("apply: " << sb_last_error());
+  if (SB_OK != sb_stencil_ccheck(terms.data(), int(terms.size()), r27, colour.m)) LOG_FATAL("apply: " << sb_last_error());
   if (!op.has_aux()) aq = -1;
   std::vector<int64_t> key = {dtype, int64_t(dq), int64_t(dw == Which::next), int64_t(sq), aq, int64_t(aw == Which::next), int64_t(exchange), parity_,
-                              int64_t(cq.size())};
+                              colour.m, colour.c, int64_t(cq.size())};
   for (const size_t q : cq) key.push_back(int64_t(q));
   for (const sb_stencil_vterm &t : terms) {
     int64_t wbits;
     std::memcpy(&wbits, &t.weight, 8);
     key.insert(key.end(), {t.source, t.offset[0], t.offset[1], t.offset[2], t.coef, t.coef_offset[0], t.coef_offset[1], t.coef_offset[2], wbits});
   }
-  run_stencil_plans(key, exchange, [&](size_t di, const std::vector<Rect3> &boxes) {
+  run_stencil_plans(key, exchange, dq == sq && dw == Which::curr, [&](size_t di, const std::vector<Rect3> &boxes) {
     LocalDomain &d = domains_[di];
     const sb_pitched dst = as_sb(dw == Which::curr ? d.curr_data(dq) : d.next_data(dq)), src = as_sb(d.curr_data(sq));
     const sb_pitched aux = aq < 0 ? sb_pitched{nullptr, 0, 0} : as_sb(aw == Which::curr ? d.curr_data(size_t(aq)) : d.next_data(size_t(aq)));
@@ -697,8 +699,8 @@ void DistributedDomain::apply_op(const stencil::LinearStencil &op, int dtype, si
       hi.insert(hi.end(), {b.hi.x, b.hi.y, b.hi.z});
     }
     sb_stencil_plan *p = nullptr;
-    if (SB_OK != sb_stencil_vplan_create(&p, d.gpu(), dtype, terms.data(), int(terms.size()), dst, src, aux, coef.data(), int(coef.size()), acc,
-                                         d.raw_size().z, int(boxes.size()), lo.data(), hi.data()))
+    if (SB_OK != sb_stencil_cplan_create(&p, d.gpu(), dtype, terms.data(), int(terms.size()), dst, src, aux, coef.data(), int(coef.size()),
+                                         colour.m, colour.c, acc, d.raw_size().z, int(boxes.size()), lo.data(), hi.data()))
       LOG_FATAL("apply: " << sb_last_error());
     return p;
   });
@@ -744,7 +746,7 @@ void DistributedDomain::apply_sys(const stencil::LinearSystem &sys, int dtype, c
     std::memcpy(&wbits, &t.weight, 8);
     key.insert(key.end(), {t.output, t.input, t.offset[0], t.offset[1], t.offset[2], t.coef, t.coef_offset[0], t.coef_offset[1], t.coef_offset[2], wbits});
   }
-  run_stencil_plans(key, exchange, [&](size_t di, const std::vector<Rect3> &boxes) {
+  run_stencil_plans(key, exchange, false, [&](size_t di, const std::vector<Rect3> &boxes) {
     LocalDomain &d = domains_[di];
     std::vector<sb_pitched> o, i;
     for (const auto &b : outs) o.push_back(as_sb(b.second == Which::curr ? d.curr_data(b.first) : d.next_data(b.first)));
@@ -764,16 +766,22 @@ void DistributedDomain::apply_sys(const stencil::LinearSystem &sys, int dtype, c
   });
 }
 
-void DistributedDomain::run_stencil_plans(const std::vector<int64_t> &key, bool exchange,
+void DistributedDomain::run_stencil_plans(const std::vector<int64_t> &key, bool exchange, bool writes_src,
                                           const std::function<sb_stencil_plan *(size_t, const std::vector<Rect3> &)> &make) {
   auto found = stencilPlans_.find(key);
   if (found == stencilPlans_.end()) {
-    const std::vector<Rect3> interiors = exchange ? get_interior() : std::vector<Rect3>();
-    const std::vector<std::vector<Rect3>> exteriors = exchange ? get_exterior() : std::vector<std::vector<Rect3>>();
+    // exchange() sends from side s of a subdomain a slab as wide as the radius on side -s; an apply that writes src
+    // (a coloured one in place) keeps its interior clear of both, so the interior writes no cell exchange() reads
+    Radius cut = radius_;
+    if (writes_src)
+      for (int z = -1; z <= 1; ++z)
+        for (int y = -1; y <= 1; ++y)
+          for (int x = -1; x <= 1; ++x) cut.dir(x, y, z) = std::max(radius_.dir(x, y, z), radius_.dir(-x, -y, -z));
     std::vector<std::vector<sb_stencil_plan *>> per_dom;
     for (size_t di = 0; di < domains_.size(); ++di) {
+      const Rect3 compute = domains_[di].get_compute_region();
       if (exchange)
-        per_dom.push_back({make(di, {interiors[di]}), make(di, exteriors[di])});
+        per_dom.push_back({make(di, {stencil::geom::interior(compute, cut)}), make(di, stencil::geom::exterior(compute, cut))});
       else
         per_dom.push_back({make(di, {domains_[di].get_compute_region()})});
     }

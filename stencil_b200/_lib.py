@@ -226,6 +226,13 @@ _SIGS = {
         [C.POINTER(C.c_void_p), C.c_int, C.c_int, C.POINTER(StencilVTerm), C.c_int, Pitched, Pitched, Pitched, C.POINTER(Pitched), C.c_int,
          I3, C.c_int64, C.c_int, C.POINTER(C.c_int64), C.POINTER(C.c_int64)],
     ),
+    "sb_stencil_ccheck": (C.c_int, [C.POINTER(StencilVTerm), C.c_int, I27, C.c_int]),
+    "sb_stencil_relax": (C.c_int, [C.POINTER(StencilTerm), C.c_int, C.c_double, C.POINTER(StencilTerm), C.c_int]),
+    "sb_stencil_cplan_create": (
+        C.c_int,
+        [C.POINTER(C.c_void_p), C.c_int, C.c_int, C.POINTER(StencilVTerm), C.c_int, Pitched, Pitched, Pitched, C.POINTER(Pitched), C.c_int,
+         C.c_int, C.c_int, I3, C.c_int64, C.c_int, C.POINTER(C.c_int64), C.POINTER(C.c_int64)],
+    ),
     "sb_stencil_sys_check": (C.c_int, [C.POINTER(StencilSysTerm), C.c_int, C.c_int, C.c_int, I27]),
     "sb_stencil_grad": (C.c_int, [C.c_int, C.c_double * 3, C.POINTER(StencilSysTerm), C.c_int]),
     "sb_stencil_div": (C.c_int, [C.c_int, C.c_double * 3, C.POINTER(StencilSysTerm), C.c_int]),

@@ -569,9 +569,9 @@ struct sb_stencil_plan {
   int device = 0;
   int es = 8, R = 1;
   bool has_coef = false;                // some term reads a coefficient field: the HAS_COEF kernels
-  std::vector<sb::OpVTileParams> tiles; // one tile-kernel launch per thick box
+  std::vector<sb::OpCTileParams> tiles; // one tile-kernel launch per thick box
   std::vector<int> tile_grids;
-  std::vector<sb::OpVCellParams> cells; // one cell-kernel launch per group of thin boxes
+  std::vector<sb::OpCCellParams> cells; // one cell-kernel launch per group of thin boxes
   std::vector<int> cell_grids;
   std::vector<sb::SysTileParams> sys_tiles; // a system (sb_stencil_sys_plan_create): one tile launch per thick box
   std::vector<int> sys_tile_grids;
@@ -1617,6 +1617,74 @@ int sb_stencil_check(const sb_stencil_term *terms, int n, const int64_t radius27
   return sb_stencil_vcheck(terms ? v.data() : nullptr, n, radius27);
 }
 
+// The colouring m (1, 2 or 8) and the colour condition on every src term with o != 0 (DESIGN.md section 2.9): under
+// m = 2 the cell at p + o has another colour than p's iff o_x + o_y + o_z is odd, under m = 8 iff some o_a is odd.
+static int stencil_colours_ok(const sb_stencil_vterm *terms, int n, int m) {
+  if (m != 1 && m != 2 && m != 8) return fail(SB_ERR_INVALID, "ncolours %d: a colouring has 1, 2 or 8 colours", m);
+  for (int t = 0; t < n && m > 1; ++t) {
+    const int32_t *o = terms[t].offset;
+    if (terms[t].source != 0 || (!o[0] && !o[1] && !o[2])) continue;
+    const bool other = m == 2 ? ((o[0] + o[1] + o[2]) & 1) != 0 : ((o[0] | o[1] | o[2]) & 1) != 0;
+    if (!other)
+      return fail(SB_ERR_INVALID, "term %d: offset (%d, %d, %d) reads a cell of its own colour under %d colours", t, int(o[0]), int(o[1]),
+                  int(o[2]), m);
+  }
+  return SB_OK;
+}
+
+// The cells of colour c under the colouring m in the box [lo, lo + e) (global coordinates).
+static int64_t stencil_colour_cells(const int64_t lo[3], const int64_t e[3], int m, int c) {
+  if (m == 1) return e[0] * e[1] * e[2];
+  int64_t n[3][2]; // n[a][q]: the coordinates of the box on axis a of parity q
+  for (int a = 0; a < 3; ++a) {
+    const int q0 = int(((lo[a] % 2) + 2) % 2);
+    n[a][q0] = (e[a] + 1) / 2;
+    n[a][q0 ^ 1] = e[a] / 2;
+  }
+  if (m == 8) return n[0][c & 1] * n[1][(c >> 1) & 1] * n[2][(c >> 2) & 1];
+  int64_t total = 0;
+  for (int qx = 0; qx < 2; ++qx)
+    for (int qy = 0; qy < 2; ++qy) total += n[0][qx] * n[1][qy] * n[2][(c - qx - qy) & 1];
+  return total;
+}
+
+int sb_stencil_ccheck(const sb_stencil_vterm *terms, int n, const int64_t radius27[27], int ncolours) {
+  int rc = sb_stencil_vcheck(terms, n, radius27);
+  if (rc != SB_OK) return rc;
+  return stencil_colours_ok(terms, n, ncolours);
+}
+
+int sb_stencil_relax(const sb_stencil_term *A, int n, double omega, sb_stencil_term *out, int cap) {
+  const std::vector<sb_stencil_vterm> v = stencil_vterms_of(A, n);
+  int rc = stencil_terms_ok(A ? v.data() : nullptr, n);
+  if (rc != SB_OK) return rc;
+  if (!std::isfinite(omega)) return fail(SB_ERR_INVALID, "sb_stencil_relax: omega = %g must be finite", omega);
+  if (cap < 0 || (cap > 0 && !out)) return fail(SB_ERR_INVALID, "sb_stencil_relax: bad output buffer");
+  int centre = -1;
+  for (int t = 0; t < n; ++t) {
+    const sb_stencil_term &T = A[t];
+    if (T.source == 1) return fail(SB_ERR_INVALID, "sb_stencil_relax: term %d reads aux; A reads src only (f goes on aux)", t);
+    if (T.offset[0] || T.offset[1] || T.offset[2]) continue;
+    if (centre >= 0) return fail(SB_ERR_INVALID, "sb_stencil_relax: terms %d and %d are both at offset (0, 0, 0); A needs one centre term", centre, t);
+    centre = t;
+  }
+  if (centre < 0) return fail(SB_ERR_INVALID, "sb_stencil_relax: A has no term at offset (0, 0, 0)");
+  const double ac = A[centre].weight;
+  if (ac == 0.0) return fail(SB_ERR_INVALID, "sb_stencil_relax: the centre weight of A is 0");
+  if (n + 1 > SB_STENCIL_MAX_TERMS)
+    return fail(SB_ERR_INVALID, "sb_stencil_relax: A has %d terms, so the update would have %d (at most %d)", n, n + 1, SB_STENCIL_MAX_TERMS);
+  std::vector<sb_stencil_term> r;
+  r.push_back(sb_stencil_term{0, {0, 0, 0}, 1.0 - omega});
+  for (int t = 0; t < n; ++t)
+    if (t != centre) {
+      const double num = -omega * A[t].weight;
+      r.push_back(sb_stencil_term{0, {A[t].offset[0], A[t].offset[1], A[t].offset[2]}, num / ac});
+    }
+  r.push_back(sb_stencil_term{1, {0, 0, 0}, omega / ac});
+  for (int i = 0; i < int(r.size()) && i < cap; ++i) out[i] = r[size_t(i)];
+  return int(r.size());
+}
+
 int sb_stencil_div_grad(const double spacing[3], sb_stencil_vterm *out, int cap) {
   if (!spacing) return fail(SB_ERR_INVALID, "sb_stencil_div_grad needs spacing[3]");
   for (int a = 0; a < 3; ++a)
@@ -1684,11 +1752,19 @@ int sb_stencil_plan_create(sb_stencil_plan **out, int device, int dtype, const s
 int sb_stencil_vplan_create(sb_stencil_plan **out, int device, int dtype, const sb_stencil_vterm *terms, int n, sb_pitched dst,
                             sb_pitched src, sb_pitched aux, const sb_pitched *coef, int ncoef, const int64_t acc_origin[3],
                             int64_t zsize, int nbox, const int64_t *lo, const int64_t *hi) {
+  return sb_stencil_cplan_create(out, device, dtype, terms, n, dst, src, aux, coef, ncoef, 1, 0, acc_origin, zsize, nbox, lo, hi);
+}
+
+int sb_stencil_cplan_create(sb_stencil_plan **out, int device, int dtype, const sb_stencil_vterm *terms, int n, sb_pitched dst,
+                            sb_pitched src, sb_pitched aux, const sb_pitched *coef, int ncoef, int ncolours, int colour,
+                            const int64_t acc_origin[3], int64_t zsize, int nbox, const int64_t *lo, const int64_t *hi) {
   if (!out) return fail(SB_ERR_INVALID, "sb_stencil_plan_create needs an output handle");
   if (dtype != SB_DTYPE_F32 && dtype != SB_DTYPE_F64) return fail(SB_ERR_INVALID, "dtype %d must be SB_DTYPE_F32 or SB_DTYPE_F64", dtype);
   const int es = dtype == SB_DTYPE_F32 ? 4 : 8;
   int rc = stencil_terms_ok(terms, n);
   if (rc != SB_OK) return rc;
+  if ((rc = stencil_colours_ok(terms, n, ncolours)) != SB_OK) return rc;
+  if (colour < 0 || colour >= ncolours) return fail(SB_ERR_INVALID, "colour %d: 0 .. %d under %d colours", colour, ncolours - 1, ncolours);
   if (ncoef < 0 || ncoef > SB_STENCIL_MAX_COEFS) return fail(SB_ERR_INVALID, "ncoef %d: 0 to %d coefficient fields", ncoef, SB_STENCIL_MAX_COEFS);
   if (ncoef > 0 && !coef) return fail(SB_ERR_INVALID, "ncoef %d, but the coefficient array is NULL", ncoef);
   bool has_aux = false;
@@ -1722,7 +1798,7 @@ int sb_stencil_vplan_create(sb_stencil_plan **out, int device, int dtype, const 
       }
   if (has_aux && !aux.ptr) return fail(SB_ERR_INVALID, "the op has a term on aux, but aux is NULL");
   if (!dst.ptr || !src.ptr) return fail(SB_ERR_INVALID, "dst and src must not be NULL");
-  if (dst.ptr == src.ptr) return fail(SB_ERR_INVALID, "dst must not be src (dst may be aux)");
+  if (dst.ptr == src.ptr && ncolours == 1) return fail(SB_ERR_INVALID, "dst must not be src (dst may be aux)");
   for (int f = 0; f < nf; ++f)
     if (coef[fsrc[f]].ptr == dst.ptr) return fail(SB_ERR_INVALID, "coefficient field %d is dst (coefficients are read only)", fsrc[f]);
   std::vector<const sb_pitched *> bufs = {&dst, &src};
@@ -1740,7 +1816,7 @@ int sb_stencil_vplan_create(sb_stencil_plan **out, int device, int dtype, const 
   if (nbox < 0 || (nbox > 0 && (!lo || !hi))) return fail(SB_ERR_INVALID, "nbox %d: needs nbox >= 0 and lo / hi arrays", nbox);
   const int64_t size[3] = {src.pitch / es, src.ysize, zsize};
   std::vector<std::array<int, 6>> thick, thin; // allocation-relative lo, ext
-  int64_t cells = 0;
+  int64_t cells = 0, written = 0;
   for (int b = 0; b < nbox; ++b) {
     int64_t l[3], e[3];
     bool empty = false;
@@ -1759,7 +1835,10 @@ int sb_stencil_vplan_create(sb_stencil_plan **out, int device, int dtype, const 
     const std::array<int, 6> bx = {int(l[0]), int(l[1]), int(l[2]), int(e[0]), int(e[1]), int(e[2])};
     (e[0] >= 8 && e[1] >= 8 && e[2] >= 8 ? thick : thin).push_back(bx);
     cells += e[0] * e[1] * e[2];
+    written += stencil_colour_cells(&lo[3 * b], e, ncolours, colour);
   }
+  sb::OpColour col{ncolours, colour, {}};
+  for (int a = 0; a < 3; ++a) col.par[a] = int(((acc_origin[a] % 2) + 2) % 2);
 
   sb::OpCommon com{};
   com.dst = static_cast<char *>(dst.ptr);
@@ -1784,9 +1863,9 @@ int sb_stencil_vplan_create(sb_stencil_plan **out, int device, int dtype, const 
   p->es = es;
   p->R = R;
   p->has_coef = nf > 0;
-  p->bytes = cells * es * ((has_aux ? 3 : 2) + nf);
+  p->bytes = cells * es * ((has_aux ? 2 : 1) + nf) + written * es;
   if (!thick.empty()) {
-    const int per_sm = sb::op_tile_prepare(R, es, device, nf);
+    const int per_sm = sb::op_tile_prepare(R, es, device, nf, ncolours > 1);
     if (per_sm <= 0) {
       delete p;
       return fail(SB_ERR_CUDA, "the R = %d tile kernel cannot be configured: %s", R, cudaGetErrorString(cudaGetLastError()));
@@ -1794,8 +1873,9 @@ int sb_stencil_vplan_create(sb_stencil_plan **out, int device, int dtype, const 
     const int SW = sb::op_tile_sw(R), P = sb::op_tile_plane(R), NS = 2 * R + 1;
     const int CSW = sb::op_tile_sw(1), CP = sb::op_tile_plane(1), CS = sb::kOpCoefSlots;
     for (const auto &b : thick) {
-      sb::OpVTileParams tp{};
+      sb::OpCTileParams tp{};
       tp.c = com;
+      tp.col = col;
       tp.k.nf = nf;
       for (int f = 0; f < nf; ++f) {
         tp.k.coef[f] = static_cast<const char *>(coef[fsrc[f]].ptr);
@@ -1840,8 +1920,9 @@ int sb_stencil_vplan_create(sb_stencil_plan **out, int device, int dtype, const 
     }
   }
   for (size_t b0 = 0; b0 < thin.size(); b0 += sb::kOpMaxBoxes) {
-    sb::OpVCellParams cp{};
+    sb::OpCCellParams cp{};
     cp.c = com;
+    cp.col = col;
     for (int t = 0; t < n; ++t)
       cp.goff[t] = (long long)terms[t].offset[2] * com.slice + (long long)terms[t].offset[1] * com.pitch + (long long)terms[t].offset[0] * es;
     for (int f = 0; f < nf; ++f) cp.coef[f] = static_cast<const char *>(coef[fsrc[f]].ptr);

@@ -20,6 +20,11 @@
 // kOpCoefSlots halo'd planes per referenced field behind the src ring, filled one plane ahead by cp.async (no register
 // staging), each field's window cut to its own reach; the term table carries each term's coefficient offset per slot.
 // The cell kernel reads coefficients through __ldg at per-term byte offsets.
+//
+// Coloured application (COL, DESIGN.md section 2.9; again a compile-time switch): only the cells of colour c of the
+// colouring m (2 or 8, from global coordinates) are written, and dst may be src.  In a tile row the cells of a colour
+// alternate along x, so each lane computes one of them (cell 2 * lane + s); the cell kernel skips the other cells.
+// src is read with plain loads, since the launch may write it.
 #include "stencil_op.cuh"
 
 #include <cstring>
@@ -47,10 +52,20 @@ template <typename T> __device__ __forceinline__ void cp_async_elem(T *dst, cons
 }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;\n" ::: "memory"); }
 
-template <bool HAS_COEF> using OpTileParamsOf = typename std::conditional<HAS_COEF, OpVTileParams, OpTileParams>::type;
+// A load of src.  The coloured kernels may run in place (dst == src), so they read src with plain loads: the
+// non-coherent path may not see what this launch writes.  What they then race on is only what they never use.
+template <bool COL, typename V> __device__ __forceinline__ V src_load(const V *a) {
+  if constexpr (COL) return *a;
+  else return __ldg(a);
+}
 
-template <typename T, int R, bool HAS_COEF>
-__global__ void __launch_bounds__(kOpThreads, 2) op_tile_kernel(const __grid_constant__ OpTileParamsOf<HAS_COEF> p) {
+template <bool HAS_COEF, bool COL>
+using OpTileParamsOf = typename std::conditional<COL, OpCTileParams, typename std::conditional<HAS_COEF, OpVTileParams, OpTileParams>::type>::type;
+
+// COL: the coloured kernel.  Each warp row holds 32 cells of the colour at most (one colour of two alternates along x),
+// so each lane computes one of them: the cell 2 * lane + s of the row, with s the row's colour phase.
+template <typename T, int R, bool HAS_COEF, bool COL>
+__global__ void __launch_bounds__(kOpThreads, 2) op_tile_kernel(const __grid_constant__ OpTileParamsOf<HAS_COEF, COL> p) {
   extern __shared__ __align__(16) unsigned char op_smem[];
   T *ring = reinterpret_cast<T *>(op_smem);
   constexpr int SW = op_tile_sw(R), P = op_tile_plane(R), NS = 2 * R + 1;
@@ -87,13 +102,13 @@ __global__ void __launch_bounds__(kOpThreads, 2) op_tile_kernel(const __grid_con
         if (ca < wb) {
           xc[i] = int((ca - row) / ES);
           if (ca >= p.c.src && ca + 16 <= p.src_end) {
-            buf[i] = __ldg(reinterpret_cast<const uint4 *>(ca));
+            buf[i] = src_load<COL>(reinterpret_cast<const uint4 *>(ca));
           } else { // a chunk that would leave the allocation: its wanted elements one by one
             T e[V];
 #pragma unroll
             for (int v = 0; v < V; ++v) {
               const char *a = ca + v * ES;
-              e[v] = (a >= wa && a < wb) ? __ldg(reinterpret_cast<const T *>(a)) : T(0);
+              e[v] = (a >= wa && a < wb) ? src_load<COL>(reinterpret_cast<const T *>(a)) : T(0);
             }
             memcpy(&buf[i], e, 16);
           }
@@ -152,6 +167,33 @@ __global__ void __launch_bounds__(kOpThreads, 2) op_tile_kernel(const __grid_con
   const bool okA = y < ye && xA < xe, okB = y < ye && xB < xe;
   const T *own = ring + (wy + R) * SW + lane + R;
   const T *const cown = cring + (wy + 1) * CSW + lane + 1;
+  // the coloured kernel's plane zc (cell: the byte offset of this warp's row): this lane's cell of the colour, if any
+  auto coloured_row = [&](int zc, long long cell) {
+    if constexpr (COL) {
+      const int gx = x0 + p.col.par[0], gy = y + p.col.par[1], gz = zc + p.col.par[2], c = p.col.c;
+      const bool on = p.col.m == 2 || (((gy ^ (c >> 1)) | (gz ^ (c >> 2))) & 1) == 0; // m = 8: the row's y and z parities
+      const int s = (p.col.m == 2 ? c - gx - gy - gz : c - gx) & 1;                   // the x parity of the colour's cells
+      const int xl = 2 * lane + s, x = x0 + xl;
+      if (!on || y >= ye || x >= xe) return;
+      const long long at = cell + x * ES;
+      const T a = p.c.has_aux ? *reinterpret_cast<const T *>(p.c.aux + at) : T(0); // before the write: dst may be aux
+      const T *const o1 = ring + (wy + R) * SW + R + xl;
+      const int sl = slot_of(zc);
+      T acc = T(0);
+      for (int t = 0; t < p.c.n; ++t) {
+        const T v = p.c.source[t] == 0 ? o1[p.toff[sl][t]] : a;
+        T w = OpNum<T>::w(p.c, t);
+        if constexpr (HAS_COEF) {
+          const T *const co1 = cring + (wy + 1) * CSW + 1 + xl;
+          const int cs = (zc - z0 + 1) & (kOpCoefSlots - 1);
+          if (p.k.cfield[t] >= 0) w = OpNum<T>::mul(w, co1[p.k.coff[cs][t]]);
+        }
+        const T m = OpNum<T>::mul(w, v);
+        acc = t == 0 ? m : OpNum<T>::add(acc, m);
+      }
+      *reinterpret_cast<T *>(p.c.dst + at) = acc;
+    }
+  };
   for (int zc = z0; zc < z1; ++zc) {
     store(slot_of(zc + p.rp[2])); // the slot of plane zc + rp - (2R + 1), which no cell of plane zc reads
     if constexpr (HAS_COEF) cp_async_wait_all(); // this thread's coefficient planes up to zc + crp have landed
@@ -162,6 +204,11 @@ __global__ void __launch_bounds__(kOpThreads, 2) op_tile_kernel(const __grid_con
         for (int f = 0; f < p.k.nf; ++f) coef_plane(f, zc + 1 + p.k.crp[f][2]);
     }
     const long long cell = (long long)zc * p.c.slice + (long long)y * p.c.pitch;
+    if constexpr (COL) {
+      coloured_row(zc, cell);
+      __syncthreads();
+      continue;
+    }
     T auxA = T(0), auxB = T(0);
     if (p.c.has_aux) { // read before the cell is written: dst may be aux
       if (okA) auxA = *reinterpret_cast<const T *>(p.c.aux + cell + xA * ES);
@@ -205,10 +252,12 @@ __global__ void __launch_bounds__(kOpThreads, 2) op_tile_kernel(const __grid_con
   }
 }
 
-template <bool HAS_COEF> using OpCellParamsOf = typename std::conditional<HAS_COEF, OpVCellParams, OpCellParams>::type;
+template <bool HAS_COEF, bool COL>
+using OpCellParamsOf = typename std::conditional<COL, OpCCellParams, typename std::conditional<HAS_COEF, OpVCellParams, OpCellParams>::type>::type;
 
-template <typename T, bool HAS_COEF>
-__global__ void __launch_bounds__(256) op_cell_kernel(const __grid_constant__ OpCellParamsOf<HAS_COEF> p) {
+// COL: the coloured kernel; a thread whose cell is of another colour does nothing
+template <typename T, bool HAS_COEF, bool COL>
+__global__ void __launch_bounds__(256) op_cell_kernel(const __grid_constant__ OpCellParamsOf<HAS_COEF, COL> p) {
   const long long total = p.first[p.n];
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     int k = 0;
@@ -227,13 +276,18 @@ __global__ void __launch_bounds__(256) op_cell_kernel(const __grid_constant__ Op
       xx = t % ex;
       zz = t / ex;
     }
+    if constexpr (COL) {
+      const int gx = p.lo[k][0] + int(xx) + p.col.par[0], gy = p.lo[k][1] + int(yy) + p.col.par[1], gz = p.lo[k][2] + int(zz) + p.col.par[2];
+      const int colour = p.col.m == 2 ? (gx + gy + gz) & 1 : (gx & 1) | (gy & 1) << 1 | (gz & 1) << 2;
+      if (colour != p.col.c) continue;
+    }
     const long long off = (long long)(p.lo[k][2] + (int)zz) * p.c.slice + (long long)(p.lo[k][1] + (int)yy) * p.c.pitch +
                           (long long)(p.lo[k][0] + (int)xx) * (long long)sizeof(T);
     const char *s = p.c.src + off;
     const T a = p.c.has_aux ? *reinterpret_cast<const T *>(p.c.aux + off) : T(0); // before the write: dst may be aux
     T acc = T(0);
     for (int t = 0; t < p.c.n; ++t) {
-      const T v = p.c.source[t] == 0 ? __ldg(reinterpret_cast<const T *>(s + p.goff[t])) : a;
+      const T v = p.c.source[t] == 0 ? src_load<COL>(reinterpret_cast<const T *>(s + p.goff[t])) : a;
       T w = OpNum<T>::w(p.c, t);
       if constexpr (HAS_COEF) {
         const int f = p.cfield[t];
@@ -246,20 +300,21 @@ __global__ void __launch_bounds__(256) op_cell_kernel(const __grid_constant__ Op
   }
 }
 
-template <typename T, int R> const void *tile_fn(bool coef) {
-  return coef ? reinterpret_cast<const void *>(&op_tile_kernel<T, R, true>) : reinterpret_cast<const void *>(&op_tile_kernel<T, R, false>);
+template <typename T, int R, bool COL> const void *tile_fn(bool coef) {
+  return coef ? reinterpret_cast<const void *>(&op_tile_kernel<T, R, true, COL>) : reinterpret_cast<const void *>(&op_tile_kernel<T, R, false, COL>);
 }
+template <typename T, int R> const void *tile_fn(bool coef, bool col) { return col ? tile_fn<T, R, true>(coef) : tile_fn<T, R, false>(coef); }
 
-const void *tile_kernel(int R, int es, bool coef) {
+const void *tile_kernel(int R, int es, bool coef, bool col) {
   switch (R * 10 + es) {
-  case 14: return tile_fn<float, 1>(coef);
-  case 24: return tile_fn<float, 2>(coef);
-  case 34: return tile_fn<float, 3>(coef);
-  case 44: return tile_fn<float, 4>(coef);
-  case 18: return tile_fn<double, 1>(coef);
-  case 28: return tile_fn<double, 2>(coef);
-  case 38: return tile_fn<double, 3>(coef);
-  case 48: return tile_fn<double, 4>(coef);
+  case 14: return tile_fn<float, 1>(coef, col);
+  case 24: return tile_fn<float, 2>(coef, col);
+  case 34: return tile_fn<float, 3>(coef, col);
+  case 44: return tile_fn<float, 4>(coef, col);
+  case 18: return tile_fn<double, 1>(coef, col);
+  case 28: return tile_fn<double, 2>(coef, col);
+  case 38: return tile_fn<double, 3>(coef, col);
+  case 48: return tile_fn<double, 4>(coef, col);
   default: return nullptr;
   }
 }
@@ -270,8 +325,8 @@ size_t op_tile_smem(int R, int es, int nf) {
   return (size_t(2 * R + 1) * size_t(op_tile_plane(R)) + size_t(nf) * kOpCoefSlots * size_t(op_tile_plane(1))) * size_t(es);
 }
 
-int op_tile_prepare(int R, int es, int device, int nf) {
-  const void *fn = tile_kernel(R, es, nf > 0);
+int op_tile_prepare(int R, int es, int device, int nf, bool col) {
+  const void *fn = tile_kernel(R, es, nf > 0, col);
   if (!fn) return 0;
   // the coefficient kernel's limit covers every field count, so plans with different counts can share it
   const int limit = int(op_tile_smem(R, es, nf > 0 ? kOpMaxCoefs : 0));
@@ -282,28 +337,40 @@ int op_tile_prepare(int R, int es, int device, int nf) {
   return ctas;
 }
 
-int launch_op_tile(const OpVTileParams &p, int R, int es, int grid, cudaStream_t stream) {
+int launch_op_tile(const OpCTileParams &p, int R, int es, int grid, cudaStream_t stream) {
   if (grid <= 0) return 0;
-  const bool coef = p.k.nf > 0;
-  const void *fn = tile_kernel(R, es, coef);
+  const bool coef = p.k.nf > 0, col = p.col.m > 1;
+  const void *fn = tile_kernel(R, es, coef, col);
   if (!fn) return 0;
-  // the plain kernel takes the OpTileParams part only
-  void *args[] = {coef ? const_cast<OpVTileParams *>(&p) : static_cast<OpTileParams *>(const_cast<OpVTileParams *>(&p))};
+  // the uncoloured kernels take the OpVTileParams part, the plain one the OpTileParams part only
+  OpCTileParams *const q = const_cast<OpCTileParams *>(&p);
+  void *args[] = {col ? static_cast<void *>(q) : coef ? static_cast<void *>(static_cast<OpVTileParams *>(q)) : static_cast<void *>(static_cast<OpTileParams *>(q))};
   cudaLaunchKernel(fn, dim3(unsigned(grid)), dim3(kOpThreads), args, op_tile_smem(R, es, p.k.nf), stream);
   return 1;
 }
 
-int launch_op_cells(const OpVCellParams &p, int es, bool has_coef, int grid, cudaStream_t stream) {
+int launch_op_cells(const OpCCellParams &p, int es, bool has_coef, int grid, cudaStream_t stream) {
   if (grid <= 0 || p.n <= 0) return 0;
+  const OpVCellParams &v = p;
   const OpCellParams &b = p;
-  if (es == 4 && has_coef)
-    op_cell_kernel<float, true><<<unsigned(grid), 256, 0, stream>>>(p);
+  const unsigned g = unsigned(grid);
+  if (p.col.m > 1) {
+    if (es == 4 && has_coef)
+      op_cell_kernel<float, true, true><<<g, 256, 0, stream>>>(p);
+    else if (es == 4)
+      op_cell_kernel<float, false, true><<<g, 256, 0, stream>>>(p);
+    else if (has_coef)
+      op_cell_kernel<double, true, true><<<g, 256, 0, stream>>>(p);
+    else
+      op_cell_kernel<double, false, true><<<g, 256, 0, stream>>>(p);
+  } else if (es == 4 && has_coef)
+    op_cell_kernel<float, true, false><<<g, 256, 0, stream>>>(v);
   else if (es == 4)
-    op_cell_kernel<float, false><<<unsigned(grid), 256, 0, stream>>>(b);
+    op_cell_kernel<float, false, false><<<g, 256, 0, stream>>>(b);
   else if (has_coef)
-    op_cell_kernel<double, true><<<unsigned(grid), 256, 0, stream>>>(p);
+    op_cell_kernel<double, true, false><<<g, 256, 0, stream>>>(v);
   else
-    op_cell_kernel<double, false><<<unsigned(grid), 256, 0, stream>>>(b);
+    op_cell_kernel<double, false, false><<<g, 256, 0, stream>>>(b);
   return 1;
 }
 

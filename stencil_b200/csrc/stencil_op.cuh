@@ -77,12 +77,27 @@ struct OpVCellParams : OpCellParams {
   long long cgoff[kOpMaxTerms];
 };
 
+// Coloured application (sb_stencil_cplan_create; DESIGN.md section 2.9): only the cells of colour c under the colouring
+// m (1, 2 or 8) are written.  par[a]: the parity of the global coordinate of allocation element 0 on axis a, so a cell's
+// colour follows from its allocation coordinates.  m = 1 launches the uncoloured kernels, which take the base parameters.
+struct OpColour {
+  int m, c;
+  int par[3];
+};
+struct OpCTileParams : OpVTileParams {
+  OpColour col;
+};
+static_assert(sizeof(OpCTileParams) <= 4096, "the coloured tile kernel's parameters fit the classic 4 KB limit");
+struct OpCCellParams : OpVCellParams {
+  OpColour col;
+};
+
 // Host: dynamic shared memory of the tile kernel; one-time attribute setup; the number of CTAs of the tile kernel that
 // fit on one SM (0 on error).  launch_* return the number of launches issued.  nf: coefficient fields (0: the plain
-// kernel).
+// kernel); col: the coloured kernel.
 size_t op_tile_smem(int R, int es, int nf = 0);
-int op_tile_prepare(int R, int es, int device, int nf = 0);
-int launch_op_tile(const OpVTileParams &p, int R, int es, int grid, cudaStream_t stream);
-int launch_op_cells(const OpVCellParams &p, int es, bool has_coef, int grid, cudaStream_t stream);
+int op_tile_prepare(int R, int es, int device, int nf = 0, bool col = false);
+int launch_op_tile(const OpCTileParams &p, int R, int es, int grid, cudaStream_t stream);
+int launch_op_cells(const OpCCellParams &p, int es, bool has_coef, int grid, cudaStream_t stream);
 
 } // namespace sb

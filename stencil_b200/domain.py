@@ -778,21 +778,23 @@ class DistributedDomain:
     def get_origin(self, i: int) -> Vec:
         return self.domains_[i].origin()
 
-    def get_interior(self) -> List[Tuple[Vec, Vec]]:
+    def get_interior(self, r27=None) -> List[Tuple[Vec, Vec]]:
+        """r27: the 27 radii to cut by (default: the domain's)."""
         out = []
         for d in self.domains_:
             lo, hi = d.get_compute_region()
             ilo, ihi = o3(), o3()
-            check(lib().sb_interior(i3(lo), i3(hi), self.radius_.c27(), ilo, ihi))
+            check(lib().sb_interior(i3(lo), i3(hi), self.radius_.c27() if r27 is None else r27, ilo, ihi))
             out.append((t3(ilo), t3(ihi)))
         return out
 
-    def get_exterior(self) -> List[List[Tuple[Vec, Vec]]]:
+    def get_exterior(self, r27=None) -> List[List[Tuple[Vec, Vec]]]:
+        """r27: the 27 radii to cut by (default: the domain's)."""
         out = []
         for d in self.domains_:
             lo, hi = d.get_compute_region()
             elo, ehi = (C.c_int64 * 18)(), (C.c_int64 * 18)()
-            n = check(lib().sb_exterior(i3(lo), i3(hi), self.radius_.c27(), elo, ehi))
+            n = check(lib().sb_exterior(i3(lo), i3(hi), self.radius_.c27() if r27 is None else r27, elo, ehi))
             out.append([(tuple(elo[3 * k : 3 * k + 3]), tuple(ehi[3 * k : 3 * k + 3])) for k in range(n)])
         return out
 
@@ -1218,7 +1220,7 @@ class DistributedDomain:
         return _lib.ReduceItem(kind, bc_dtype(self.dtypes_[qs[0]]), (Pitched * 3)(*srcs), i3(d.accessor_origin()), i3(lo), i3(hi))
 
     # -- linear stencil operators
-    def apply(self, op, dst, src, aux=None, exchange: bool = True, coefs=None) -> None:
+    def apply(self, op, dst, src, aux=None, exchange: bool = True, coefs=None, colour=None) -> None:
         """dst = op(src, aux, coefs) over the whole compute region of every local subdomain (DESIGN.md section 2.7).
 
         Buffers are (DataHandle, "curr" | "next"); a bare handle means "next" for dst and "curr" for src and aux.  src is
@@ -1230,8 +1232,17 @@ class DistributedDomain:
         exchange=True: the interior runs on its own stream while exchange() fills the ghost cells, then the exterior slabs
         of each subdomain run as one launch; exchange=False: one launch over the whole region, and the caller guarantees
         the ghost cells are current.  Returns when the update is complete.  The plans are built on first use and kept,
-        per (op, buffers, exchange, swap parity), until close().  Under torchrun every rank calls it (exchange() is
-        collective)."""
+        per (op, buffers, exchange, swap parity, colour), until close().  Under torchrun every rank calls it (exchange() is
+        collective).
+        colour=(m, c), m in 1, 2, 8 (DESIGN.md section 2.9): only the cells of colour c of the colouring m (taken from global
+        coordinates) are written, each from the buffers as they were before the call, and with m > 1 dst may be src, so
+        a Gauss-Seidel / SOR sweep is one call per colour:
+            sor = op.relax(omega)                         # op: A of A u = f
+            for c in range(2):
+                dd.apply(sor, (u, "curr"), u, f, colour=(2, c))
+        Every src term with a non-zero offset must read another colour (op.check(radius, colours=m)).  In place the
+        schedule is the same, with the interior cut by the larger radius of both sides of each axis, so that it writes
+        no cell exchange() sends (a slab as wide as the opposite side's radius); the exterior runs after exchange()."""
         from .stencil_op import StencilOp, StencilPlan
 
         if not isinstance(op, StencilOp):
@@ -1251,7 +1262,10 @@ class DistributedDomain:
         s_q, s_w = buf(src, "curr", "src")
         if s_w != "curr":
             raise _lib.StencilError("apply: src must be a curr buffer (the one exchange() fills)")
-        if (d_q, d_w) == (s_q, s_w):
+        ncol, col = (1, 0) if colour is None else (int(colour[0]), int(colour[1]))
+        if ncol not in (1, 2, 8) or not 0 <= col < ncol:
+            raise _lib.StencilError(f"apply: colour {colour!r} must be (m, c) with m in 1, 2, 8 and 0 <= c < m")
+        if (d_q, d_w) == (s_q, s_w) and ncol == 1:
             raise _lib.StencilError("apply: dst must not be src")
         a = buf(aux, "curr", "aux") if aux is not None else None
         if op.has_aux and a is None:
@@ -1267,15 +1281,15 @@ class DistributedDomain:
             if (q, w) == (d_q, d_w):
                 raise _lib.StencilError(f"apply: coefficient {k} must not be dst")
             c_q.append(q)
-        op.check(self.radius_)
-        key = (op.key(), (d_q, d_w), s_q, a if op.has_aux else None, tuple(c_q), bool(exchange), self._parity)
+        op.check(self.radius_, colours=ncol)
+        key = (op.key(), (d_q, d_w), s_q, a if op.has_aux else None, tuple(c_q), bool(exchange), self._parity, (ncol, col))
 
         def make(di, d, boxes):
             P = (d.pitched(d_q, d_w), d.pitched(s_q, "curr"), d.pitched(a[0], a[1]) if a is not None and op.has_aux else Pitched(None, 0, 0))
             K = [d.pitched(q, "curr") for q in c_q] if op.has_coef else None
-            return StencilPlan(d.gpu(), op, *P, d.accessor_origin(), d.raw_size()[2], boxes, K)
+            return StencilPlan(d.gpu(), op, *P, d.accessor_origin(), d.raw_size()[2], boxes, K, (ncol, col) if ncol > 1 else None)
 
-        self._run_plans(self._plans_for(key, exchange, make), exchange)
+        self._run_plans(self._plans_for(key, exchange, make, writes_src=(d_q, d_w) == (s_q, s_w)), exchange)
 
     def apply_system(self, system, outputs, inputs, exchange: bool = True) -> None:
         """outputs = system(inputs) over the whole compute region of every local subdomain (DESIGN.md section 2.8).
@@ -1334,13 +1348,17 @@ class DistributedDomain:
 
         self._run_plans(self._plans_for(key, exchange, make), exchange)
 
-    def _plans_for(self, key, exchange: bool, make):
+    def _plans_for(self, key, exchange: bool, make, writes_src: bool = False):
         """The cached per-domain plans of key: (interior, exterior) pairs with exchange, else one plan over the whole
-        compute region; make(di, d, boxes) builds one plan."""
+        compute region; make(di, d, boxes) builds one plan.  writes_src: the plans write src (a coloured apply in place).
+        exchange() sends from side s of a subdomain a slab as wide as the radius on side -s, so such an interior also
+        keeps clear of that: it is cut by max(radius(d), radius(-d)) in every direction d."""
         plans = self._stencil_plans.get(key)
         if plans is None:
             plans = []
-            interiors, exteriors = (self.get_interior(), self.get_exterior()) if exchange else (None, None)
+            r = list(self.radius_.c27())
+            r27 = I27(*[max(r[i], r[26 - i]) for i in range(27)]) if writes_src else None
+            interiors, exteriors = (self.get_interior(r27), self.get_exterior(r27)) if exchange else (None, None)
             for di, d in enumerate(self.domains_):
                 if exchange:
                     plans.append((make(di, d, [interiors[di]]), make(di, d, exteriors[di])))

@@ -23,8 +23,15 @@ output sums its own terms in list order by the same rule:
     E = [(q, "curr") for q in (ex, ey, ez)]
     dd.apply_system(ident + curl_h, E, [hx, hy, hz] + E)                       # E = E + dt/eps curl H, in place
 
-The rule, the reach check against a domain's radius and the Laplacian, div-grad, grad, div and curl tables live in the
-C library; this module only carries them.
+A coloured apply (DESIGN.md section 2.9) writes only the cells of one colour and may run in place; one apply per colour
+is a Gauss-Seidel or SOR sweep.  For A u = f with f in the quantity f:
+
+    sor = StencilOp.laplacian(2, (h, h, h), np.float64).scaled(-1.0).relax(omega)   # u + omega (f - A u) / a_c
+    for c in range(2):                                                               # red, then black
+        dd.apply(sor, (u, "curr"), u, f, colour=(2, c))
+
+The rule, the reach and colour checks against a domain's radius and the Laplacian, div-grad, relaxation, grad, div and
+curl tables live in the C library; this module only carries them.
 """
 from __future__ import annotations
 
@@ -72,8 +79,10 @@ class StencilOp:
         # the limits of a term list, whatever the domain: every ghost box at the largest radius
         self._check(I27(*([_lib.STENCIL_MAX_REACH] * 27)))
 
-    def _check(self, r27) -> None:
-        if self.has_coef:
+    def _check(self, r27, colours: int = 1) -> None:
+        if colours != 1:
+            check(lib().sb_stencil_ccheck(self.c_vterms(), len(self.terms), r27, int(colours)))
+        elif self.has_coef:
             check(lib().sb_stencil_vcheck(self.c_vterms(), len(self.terms), r27))
         else:
             check(lib().sb_stencil_check(self.c_terms(), len(self.terms), r27))
@@ -97,6 +106,18 @@ class StencilOp:
         buf = (StencilVTerm * n)()
         check(lib().sb_stencil_div_grad(h, buf, n))
         return StencilOp([(t.source, tuple(t.offset), t.weight, t.coef, tuple(t.coef_offset)) for t in buf], dtype)
+
+    def relax(self, omega: float) -> "StencilOp":
+        """The SOR update of A u = f for this op A, f on aux (sb_stencil_relax): u + omega (f - A u) / a_c, with a_c the
+        weight of A's one centre term.  Terms: (src, 0, 1 - omega), each off-centre term of A as (src, o, (-omega w) / a_c),
+        then (aux, 0, omega / a_c).  omega = 1 in a coloured sweep is Gauss-Seidel, out of place Jacobi; omega outside
+        (0, 2) diverges for a symmetric positive definite A.  A must have constant coefficients and no aux term."""
+        if self.has_coef:
+            raise _lib.StencilError("relax: the op has coefficient terms; the relaxation table takes constant coefficients")
+        n = len(self.terms)
+        buf = (StencilTerm * (n + 1))()
+        n = check(lib().sb_stencil_relax(self.c_terms(), n, float(omega), buf, n + 1))
+        return StencilOp([(t.source, tuple(t.offset), t.weight) for t in buf[:n]], self.dtype)
 
     def scaled(self, f: float) -> "StencilOp":
         """The same op with every weight multiplied by f (in double)."""
@@ -131,10 +152,11 @@ class StencilOp:
     def reach(self) -> int:
         return max(max(abs(c) for c in t[1]) for t in self.terms)
 
-    def check(self, radius) -> None:
+    def check(self, radius, colours: int = 1) -> None:
         """Raise StencilError unless a domain with this Radius exchanges every ghost cell the op reads (src cells and
-        coefficient cells alike)."""
-        self._check(radius.c27())
+        coefficient cells alike) and, for colours 2 or 8, every src term with a non-zero offset reads a cell of another
+        colour (sb_stencil_ccheck)."""
+        self._check(radius.c27(), colours)
 
     def key(self) -> tuple:
         return (self.terms, self.dtype.str)
@@ -153,13 +175,21 @@ class StencilPlan:
     """sb_stencil_plan: the op over a list of boxes [lo, hi) (global coordinates) of three allocations of one subdomain."""
 
     def __init__(self, device: int, op: StencilOp, dst: Pitched, src: Pitched, aux: Pitched, acc_origin, zsize: int,
-                 boxes: Sequence[Tuple[Sequence[int], Sequence[int]]], coefs: Optional[Sequence[Pitched]] = None):
-        """coefs: the coefficient allocations (sb_stencil_vplan_create), field k = coefs[k]; None for a plain op."""
+                 boxes: Sequence[Tuple[Sequence[int], Sequence[int]]], coefs: Optional[Sequence[Pitched]] = None,
+                 colour: Optional[Tuple[int, int]] = None):
+        """coefs: the coefficient allocations (sb_stencil_vplan_create), field k = coefs[k]; None for a plain op.
+        colour: (m, c), write only the cells of colour c under the colouring m (sb_stencil_cplan_create); dst may then be
+        src."""
         nb = len(boxes)
         lo = (C.c_int64 * (3 * max(1, nb)))(*[int(v) for b in boxes for v in b[0]])
         hi = (C.c_int64 * (3 * max(1, nb)))(*[int(v) for b in boxes for v in b[1]])
         h = C.c_void_p()
-        if coefs is None and not op.has_coef:
+        if colour is not None:
+            cs = list(coefs or [])
+            carr = (Pitched * max(1, len(cs)))(*cs)
+            check(lib().sb_stencil_cplan_create(C.byref(h), device, op.dtype_code, op.c_vterms(), len(op.terms), dst, src, aux, carr,
+                                                len(cs), int(colour[0]), int(colour[1]), i3(acc_origin), int(zsize), nb, lo, hi))
+        elif coefs is None and not op.has_coef:
             check(lib().sb_stencil_plan_create(C.byref(h), device, op.dtype_code, op.c_terms(), len(op.terms), dst, src, aux,
                                                i3(acc_origin), int(zsize), nb, lo, hi))
         else:
