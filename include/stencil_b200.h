@@ -21,7 +21,7 @@
 extern "C" {
 #endif
 
-#define SB_VERSION 1
+#define SB_VERSION 2
 
 typedef enum sb_status {
   SB_OK = 0,
@@ -106,9 +106,6 @@ int sb_copy_plan_create(sb_copy_plan **out, int device, const sb_box_copy *copie
 int sb_copy_plan_launch(sb_copy_plan *plan, void *stream);
 int64_t sb_copy_plan_bytes(const sb_copy_plan *plan);     /* payload bytes per launch */
 int64_t sb_copy_plan_num_tiles(const sb_copy_plan *plan); /* work items per launch */
-/* how many of the plan's copies are carried by the TMA (cp.async.bulk.tensor) path: wide rows whose source
- * and destination are 16-byte aligned in base and strides; the rest use the LDG/STG path.  SB_TMA=0 disables. */
-int64_t sb_copy_plan_num_tma_segments(const sb_copy_plan *plan);
 int sb_copy_plan_destroy(sb_copy_plan *plan);
 
 /* Cross-GPU completion flags for the fused exchange when source and destination GPUs are driven

@@ -46,7 +46,6 @@ def timeit(fn, reps=reps):
     return e0.elapsed_time(e1) / reps
 
 
-tag = os.environ.get("SB_AC_SHAPE", "0") + "/" + os.environ.get("SB_AC_ZCHUNK", "auto")
 for variant, name in ((ac.TEAM3_TMA, "team3-tma"), (ac.TEAM_TMA, "team2-tma"), (ac.TEAM, "team"), (ac.TILE, "tile"), (ac.CELL, "cell")):
     if variant in (ac.TEAM3_TMA, ac.TEAM_TMA) and dtype != np.float64:
         continue
@@ -55,7 +54,7 @@ for variant, name in ((ac.TEAM3_TMA, "team3-tma"), (ac.TEAM_TMA, "team2-tma"), (
     for step in range(3):
         ms = timeit(lambda: ac.substep(step, cur, nxt, es, (m, m, m), (3, 3, 3), (m - 3, m - 3, m - 3), params, variant, stream), reps if variant != ac.CELL else 2)
         alg = (16 if step == 0 else 24) * es * cells
-        print(f"[{np.dtype(dtype).name} n={n} shape/zc={tag}] {name} substep {step}: {ms:.4f} ms  {cells/ms/1e6:.1f} Gcell/s  {alg/ms/1e6:.0f} GB/s algorithmic = {alg/ms/1e6/peak*100:.1f}% of HBM peak", flush=True)
+        print(f"[{np.dtype(dtype).name} n={n}] {name} substep {step}: {ms:.4f} ms  {cells/ms/1e6:.1f} Gcell/s  {alg/ms/1e6:.0f} GB/s algorithmic = {alg/ms/1e6/peak*100:.1f}% of HBM peak", flush=True)
 if not os.environ.get("SKIP_ITER"):
     for overlap in (True, False):
         sim = ac.Astaroth(dd, handles, params, overlap=overlap)

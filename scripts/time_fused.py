@@ -52,31 +52,11 @@ if only:
     run(int(only), f"fused (default variant) subdomains={only}")
     sys.exit(0)
 run(1, "plain whole-region kernel (calibration)", fused=False)
-if os.environ.get("F32VARIANTS"):
-    # FP32 rows alternate between two 16-byte phases: what the pieces of the fused kernel cost on one GPU
-    for env, what in (({}, "fused, defaults (tail-column tiles)"), ({"SB_JACOBI_COLUMN": "0"}, "fused, fifth strip instead of column tiles"),
-                      ({"SB_JACOBI_SHIFT": "0"}, "fused, 64-bit vectors instead of phase-shifted rows"), ({"SB_DEBUG_FUSED": "64"}, "fused, every tile runs the plain loop (wrong halos)"),
-                      ({"SB_DEBUG_FUSED": str(64 + (3 << 8))}, "  only the x-face tiles run the boundary loop"), ({"SB_DEBUG_FUSED": str(64 + (12 << 8))}, "  only the y-face tiles"),
-                      ({"SB_DEBUG_FUSED": str(64 + (48 << 8))}, "  only the z-face tiles"), ({"SB_DEBUG_FUSED": "65536"}, "fused, patch scalar from the lane's own vector (wrong halos)"),
-                      ({"SB_DEBUG_FUSED": "131072"}, "fused, no patch at all (wrong halos)"), ({"SB_DEBUG_FUSED": "131072", "SB_JACOBI_PREFETCH": "0"}, "  same, no L2 prefetch")):
-        os.environ.update(env)
-        run(1, what)
-        for k in env:
-            del os.environ[k]
-    sys.exit(0)
 if os.environ.get("SPLITS", "1") == "1":
     # which face direction costs what: two 512^3 subdomains on this GPU, cut along x / y / z (the other two axes wrap in place)
     run(2, "fused, 2 x 512^3 cut along x (dense x lines)", shape=(2 * n, n, n))
-    for dbg, what in ((16, "ghost column instead of the dense array"), (32, "no x parking"), (48, "both")):
-        os.environ["SB_DEBUG_FUSED"] = str(dbg)
-        run(2, "  same, " + what, shape=(2 * n, n, n))
-    del os.environ["SB_DEBUG_FUSED"]
     run(2, "fused, 2 x 512^3 cut along y", shape=(n, 2 * n, n))
     run(2, "fused, 2 x 512^3 cut along z", shape=(n, n, 2 * n))
     run(8, "fused, 8 x 512^3 cut along x, y and z", shape=(2 * n, 2 * n, 2 * n))
-    os.environ["SB_DEBUG_NOPUSH"] = "1"
-    run(2, "fused, 2 x 512^3 cut along x NOPUSH", shape=(2 * n, n, n))
-    run(8, "fused, 8 x 512^3 cut along x, y and z NOPUSH", shape=(2 * n, 2 * n, 2 * n))
-    del os.environ["SB_DEBUG_NOPUSH"]
     sys.exit(0)
 run(1, "fused, one 512^3 subdomain (every neighbour is the subdomain itself)")

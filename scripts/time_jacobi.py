@@ -1,4 +1,4 @@
-"""Time the jacobi kernels alone (CUDA events) for the current SB_JACOBI_* environment.
+"""Time the jacobi kernels alone (CUDA events) at one size and precision.
 usage: python scripts/time_jacobi.py [n] [dtype] [reps]"""
 import os
 import sys
@@ -39,7 +39,7 @@ def timeit(fn, cells):
     return ms, 2 * es * cells / (ms * 1e-3) / 1e9
 
 
-cfg = {k: v for k, v in os.environ.items() if k.startswith("SB_")}
+cfg = f"{np.dtype(dtype).name} {n}^3"
 ms, gbs = timeit(jac.launch_interior, jac.interior_cells)
 print(f"{cfg} interior {ms:.4f} ms {gbs:.0f} GB/s", flush=True)
 ms, gbs = timeit(jac.launch_whole, n**3)

@@ -3,11 +3,11 @@
   * the card: name, power limit and max SM clock (read-only nvidia-smi query);
   * the copy ceiling on two 514^3 FP64 buffers (the 512^3 subdomain with its ghost layer, 1.086 GB each):
     dst.copy_(src) (a device-to-device memcpy) and one torch elementwise kernel with out=; bytes = read + write;
-  * the fused step (Jacobi3D.step_fused) on 512^3 FP64 at the defaults and at other z-chunk / L2-prefetch settings.
+  * the fused step (Jacobi3D.step_fused) on 512^3 FP64.
 
 Times are CUDA events around each call, reduced to the trimean of --reps samples.  With --ab LIB the script then
 alternates bench.py between this tree's library and LIB (SB_LIB_PATH, e.g. a parent-commit build) for --pairs FP64
-pairs, one FP32 pair, and scripts/time_fused.py's 2- and 8-subdomain one-GPU stand-ins.
+and --pairs FP32 pairs, then scripts/time_fused.py's 2- and 8-subdomain one-GPU stand-ins.
 
 usage: python scripts/time_jacobi_feed.py [--reps 40] [--ab stencil_b200/_alt/libstencil_b200_parent.so] [--pairs 3]"""
 import argparse
@@ -68,33 +68,24 @@ def ceiling(reps):
     return res
 
 
-def fused(reps, env, label):
+def fused(reps):
     import stencil_b200 as sb
     from stencil_b200.jacobi import Jacobi3D, jacobi_radius
 
-    saved = {k: os.environ.get(k) for k in env}
-    os.environ.update(env)  # read by launch_jacobi_fused at every launch
-    try:
-        n = 512
-        dd = sb.DistributedDomain(n, n, n)
-        dd.set_gpus([0])
-        dd.set_radius(jacobi_radius())
-        h = dd.add_data(np.float64)
-        dd.realize()
-        jac = Jacobi3D(dd, h)
-        jac.init(0.5)
-        ms = event_trimean(jac.step_fused, jac.streams[0], reps)
-        gbs = 16 * n**3 / (ms * 1e-3) / 1e9
-        print(f"  fused 512^3 FP64 {label:36s} {ms:.4f} ms  {gbs:.0f} GB/s algorithmic", flush=True)
-        jac.close()
-        dd.close()
-        return {"ms": ms, "gbs": gbs}
-    finally:
-        for k, v in saved.items():
-            if v is None:
-                os.environ.pop(k, None)
-            else:
-                os.environ[k] = v
+    n = 512
+    dd = sb.DistributedDomain(n, n, n)
+    dd.set_gpus([0])
+    dd.set_radius(jacobi_radius())
+    h = dd.add_data(np.float64)
+    dd.realize()
+    jac = Jacobi3D(dd, h)
+    jac.init(0.5)
+    ms = event_trimean(jac.step_fused, jac.streams[0], reps)
+    gbs = 16 * n**3 / (ms * 1e-3) / 1e9
+    print(f"  fused 512^3 FP64 {ms:.4f} ms  {gbs:.0f} GB/s algorithmic", flush=True)
+    jac.close()
+    dd.close()
+    return {"ms": ms, "gbs": gbs}
 
 
 def bench(lib, extra=()):
@@ -138,34 +129,24 @@ def main():
     ap.add_argument("--reps", type=int, default=40)
     ap.add_argument("--ab", default=None, help="library to alternate with this tree's (SB_LIB_PATH)")
     ap.add_argument("--pairs", type=int, default=3)
-    ap.add_argument("--no-variants", action="store_true", help="only the defaults of the fused step")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "needs a CUDA device"
     print(f"card: {card()}", flush=True)
     print("copy ceiling, 2 x 514^3 FP64:", flush=True)
     ceil = ceiling(args.reps)
     top = max(v["gbs"] for v in ceil.values())
-    variants = [({}, "defaults")]
-    if not args.no_variants:
-        variants += [({"SB_JACOBI_ZCHUNK": "16", "SB_JACOBI_PREFETCH": "2"}, "16-plane chunks, prefetch 2"),
-                     ({"SB_JACOBI_ZCHUNK": "16", "SB_JACOBI_PREFETCH": "3"}, "16-plane chunks, prefetch 3"),
-                     ({"SB_JACOBI_ZCHUNK": "8"}, "8-plane chunks"), ({"SB_JACOBI_ZCHUNK": "8", "SB_JACOBI_PREFETCH": "0"}, "8-plane chunks, no prefetch"),
-                     ({"SB_JACOBI_ZCHUNK": "8", "SB_JACOBI_PREFETCH": "2"}, "8-plane chunks, prefetch 2"),
-                     ({"SB_JACOBI_ZCHUNK": "12"}, "12-plane chunks"), ({"SB_JACOBI_ZCHUNK": "16"}, "16-plane chunks"), ({}, "defaults again")]
-    for env, label in variants:
-        r = fused(args.reps, env, label)
-        print(f"    = {r['gbs'] / top:.3f} of the copy ceiling ({top:.0f} GB/s)", flush=True)
+    r = fused(args.reps)
+    print(f"    = {r['gbs'] / top:.3f} of the copy ceiling ({top:.0f} GB/s)", flush=True)
     if not args.ab:
         return
     print(f"A/B: bench.py --steps 200 --warmup 20, this tree ('new') vs {args.ab} ('alt'), alternating", flush=True)
-    new, alt = [], []
-    for _ in range(args.pairs):
-        alt.append(bench(args.ab)[0])
-        new.append(bench(None)[0])
-    print(f"  FP64 median new {np.median(new):.4f} alt {np.median(alt):.4f} ms/step ({np.median(new) / np.median(alt) - 1:+.1%}); "
-          f"slowest new {max(new):.4f} vs fastest alt {min(alt):.4f}", flush=True)
-    bench(args.ab, ("--dtype", "f32"))
-    bench(None, ("--dtype", "f32"))
+    for name, extra in (("FP64", ()), ("FP32", ("--dtype", "f32"))):
+        new, alt = [], []
+        for _ in range(args.pairs):
+            alt.append(bench(args.ab, extra)[0])
+            new.append(bench(None, extra)[0])
+        print(f"  {name} median new {np.median(new):.4f} alt {np.median(alt):.4f} ms/step ({np.median(new) / np.median(alt) - 1:+.1%}); "
+              f"new {min(new):.4f}..{max(new):.4f}, alt {min(alt):.4f}..{max(alt):.4f}", flush=True)
     stand_ins(args.ab)
     stand_ins(None)
     print("copy ceiling again:", flush=True)

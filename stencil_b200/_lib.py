@@ -192,7 +192,6 @@ _SIGS = {
     "sb_copy_plan_launch": (C.c_int, [C.c_void_p, C.c_void_p]),
     "sb_copy_plan_bytes": (C.c_int64, [C.c_void_p]),
     "sb_copy_plan_num_tiles": (C.c_int64, [C.c_void_p]),
-    "sb_copy_plan_num_tma_segments": (C.c_int64, [C.c_void_p]),
     "sb_copy_plan_destroy": (C.c_int, [C.c_void_p]),
     "sb_bc_regions": (C.c_int, [I3, I27, I6, C.POINTER(BcRegion), C.c_int]),
     "sb_exchange_messages": (C.c_int, [I3, I3, I3, C.c_int32 * 3, I27, I3, C.POINTER(Message), C.c_int]),

@@ -281,10 +281,10 @@ template <int BYTES> __device__ __forceinline__ void cp_async(void *smem, const 
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 
-template <int STEP, typename T, int TX, int TY, int NSLOT>
+template <int STEP, typename T, int TX, int TY>
 __global__ void __launch_bounds__(TX *TY, 1) ac_tile_kernel(const __grid_constant__ AcArgs<T> A) {
+  constexpr int NSLOT = 8; // ring of 8 planes: 7 in use + 1 in flight (the refill overlaps the computation)
   constexpr int W = TX + 6, H = TY + 6, PL = W * H, NT = TX * TY, NL = (PL + NT - 1) / NT;
-  static_assert(NSLOT == 7 || NSLOT == 8, "ring of 7 (synchronous refill) or 8 (refill overlaps the computation) planes");
   extern __shared__ __align__(16) unsigned char ac_smem[];
   T *ring = reinterpret_cast<T *>(ac_smem); // [field][slot][H][W]
 
@@ -328,11 +328,8 @@ __global__ void __launch_bounds__(TX *TY, 1) ac_tile_kernel(const __grid_constan
 
   for (int z = z0; z < z1; ++z, idx += mxy) {
     const int zi = z - z0;
-    const bool more = z + 1 < z1;
-    if (NSLOT == 8) {
-      if (more) load_plane(z + 4, (zi + 7) % NSLOT);
-      cp_async_commit();
-    }
+    if (z + 1 < z1) load_plane(z + 4, (zi + 7) % NSLOT);
+    cp_async_commit();
     if (valid) {
       const T *b[7]; // plane z-3+k of field 0 at this thread's cell
 #pragma unroll
@@ -342,22 +339,10 @@ __global__ void __launch_bounds__(TX *TY, 1) ac_tile_kernel(const __grid_constan
       };
       solve_cell<STEP>(atf, A, idx);
     }
-    if (NSLOT == 8) {
-      cp_async_wait_all();
-      __syncthreads();
-    } else {
-      __syncthreads(); // everyone is done with plane z-3 before its slot is refilled
-      if (more) {
-        load_plane(z + 4, (zi + 7) % NSLOT);
-        cp_async_commit();
-        cp_async_wait_all();
-        __syncthreads();
-      }
-    }
+    cp_async_wait_all();
+    __syncthreads();
   }
 }
-
-int env_int(const char *name, int dflt);
 
 // ---------------------------------------------------------------------------------------------- team kernel
 // Two threads per cell.  The tile kernel above keeps value + gradient + hessian of all 8 fields live until the physics
@@ -377,7 +362,7 @@ __device__ __forceinline__ void bar_sync(int id, int n) { asm volatile("bar.sync
 
 // One plane of the two-team scheme (see ac_team_kernel): team A (induction) or team U (continuity, momentum, entropy) of
 // the cell at shared-memory offset o0 of ring plane `zi`, global index idx.  Shared by the cp.async-fed and the TMA-fed kernel.
-template <int STEP, typename T, int W, int PL, int NSLOT, int NC, bool PACED>
+template <int STEP, typename T, int W, int PL, int NSLOT, int NC>
 __device__ __forceinline__ void team_plane(const AcArgs<T> &A, const T *ring, T *xb, int zi, int o0, int cell, bool teamA, bool valid, long long idx) {
   constexpr int NT = 2 * NC;
   const AcConst<T> &P = A.P;
@@ -397,21 +382,21 @@ __device__ __forceinline__ void team_plane(const AcArgs<T> &A, const T *ring, T 
       // curl A, laplacian A, grad div A, folded field by field
       T Bx, By, Bz, lax, lay, laz, gx, gy, gz, av[3];
       {
-        const Dv<T> d = derive<T, true, true, false, PACED>(atf(AX), P);
+        const Dv<T> d = derive<T, true, true, false, true>(atf(AX), P);
         av[0] = d.v;
         By = d.gz, Bz = -d.gy;
         lax = d.xx + d.yy + d.zz;
         gx = d.xx, gy = d.xy, gz = d.xz;
       }
       {
-        const Dv<T> d = derive<T, true, false, true, PACED>(atf(AY), P);
+        const Dv<T> d = derive<T, true, false, true, true>(atf(AY), P);
         av[1] = d.v;
         Bx = -d.gz, Bz += d.gx;
         lay = d.xx + d.yy + d.zz;
         gx += d.xy, gy += d.yy, gz += d.yz;
       }
       {
-        const Dv<T> d = derive<T, false, true, true, PACED>(atf(AZ), P);
+        const Dv<T> d = derive<T, false, true, true, true>(atf(AZ), P);
         av[2] = d.v;
         Bx += d.gy, By -= d.gx;
         laz = d.xx + d.yy + d.zz;
@@ -446,14 +431,14 @@ __device__ __forceinline__ void team_plane(const AcArgs<T> &A, const T *ring, T 
       }
       T llr;
       {
-        const Dv<T> d = derive<T, false, false, false, PACED>(atf(LNRHO), P);
+        const Dv<T> d = derive<T, false, false, false, true>(atf(LNRHO), P);
         lrv = d.v;
         lg[0] = d.gx, lg[1] = d.gy, lg[2] = d.gz;
         llr = d.xx + d.yy + d.zz;
         cont = -(ux * d.gx + uy * d.gy + uz * d.gz);
       }
       {
-        const Dv<T> d = derive<T, false, false, false, PACED>(atf(ENTROPY), P);
+        const Dv<T> d = derive<T, false, false, false, true>(atf(ENTROPY), P);
         sv = d.v;
         const T ls = d.xx + d.yy + d.zz;
         const T sg[3] = {d.gx, d.gy, d.gz};
@@ -471,7 +456,7 @@ __device__ __forceinline__ void team_plane(const AcArgs<T> &A, const T *ring, T 
         arg = P.gam * d.v * P.icp + (P.gam - T(1.0)) * (lrv - P.lnrho0);
       }
       {
-        const Dv<T> d = derive<T, true, true, false, PACED>(atf(UUX), P);
+        const Dv<T> d = derive<T, true, true, false, true>(atf(UUX), P);
         madv[0] = -(d.gx * ux + d.gy * uy + d.gz * uz);
         divu = d.gx;
         lu[0] = d.xx + d.yy + d.zz;
@@ -480,7 +465,7 @@ __device__ __forceinline__ void team_plane(const AcArgs<T> &A, const T *ring, T 
         S01 = half * d.gy, S02 = half * d.gz;
       }
       {
-        const Dv<T> d = derive<T, true, false, true, PACED>(atf(UUY), P);
+        const Dv<T> d = derive<T, true, false, true, true>(atf(UUY), P);
         madv[1] = -(d.gx * ux + d.gy * uy + d.gz * uz);
         divu += d.gy;
         lu[1] = d.xx + d.yy + d.zz;
@@ -489,7 +474,7 @@ __device__ __forceinline__ void team_plane(const AcArgs<T> &A, const T *ring, T 
         S01 += half * d.gx, S12 = half * d.gz;
       }
       {
-        const Dv<T> d = derive<T, false, true, true, PACED>(atf(UUZ), P);
+        const Dv<T> d = derive<T, false, true, true, true>(atf(UUZ), P);
         madv[2] = -(d.gx * ux + d.gy * uy + d.gz * uz);
         divu += d.gz;
         lu[2] = d.xx + d.yy + d.zz;
@@ -528,7 +513,7 @@ __device__ __forceinline__ void team_plane(const AcArgs<T> &A, const T *ring, T 
   }
 }
 
-template <int STEP, typename T, int TX, int TY, int NSLOT, bool PACED>
+template <int STEP, typename T, int TX, int TY, int NSLOT>
 __global__ void __launch_bounds__(2 * TX *TY, 1) ac_team_kernel(const __grid_constant__ AcArgs<T> A) {
   constexpr int W = TX + 6, H = TY + 6, PL = W * H, NC = TX * TY, NT = 2 * NC, NL = (PL + NT - 1) / NT;
   static_assert(NSLOT == 8, "ring of 8 planes: 7 in use + 1 in flight");
@@ -577,7 +562,7 @@ __global__ void __launch_bounds__(2 * TX *TY, 1) ac_team_kernel(const __grid_con
     const int zi = z - z0;
     if (z + 1 < z1) load_plane(z + 4, (zi + 7) % NSLOT);
     cp_async_commit();
-    team_plane<STEP, T, W, PL, NSLOT, NC, PACED>(A, ring, xb, zi, o0, cell, teamA, valid, idx);
+    team_plane<STEP, T, W, PL, NSLOT, NC>(A, ring, xb, zi, o0, cell, teamA, valid, idx);
     cp_async_wait_all();
     __syncthreads();
   }
@@ -593,7 +578,7 @@ __global__ void __launch_bounds__(2 * TX *TY, 1) ac_team_kernel(const __grid_con
 // What one equation needs from another team's fields crosses through 14 words of shared memory per cell:
 //   A -> V: j x B (3)   A -> T: |j|^2 (1)   T -> V: cs2, G = grad s / cp + grad lnrho (3), grad lnrho (3), 1 / rho   V -> T: div u, S : S
 // ordered by three named barriers (the producer arrives, the consumers wait; no cycle: T publishes before it waits for V).
-template <int STEP, typename T, int W, int PL, int NSLOT, int NC, bool PACED>
+template <int STEP, typename T, int W, int PL, int NSLOT, int NC>
 __device__ __forceinline__ void team3_plane(const AcArgs<T> &A, const T *ring, T *xb, int zi, int o0, int cell, int team, bool valid, long long idx) {
   const AcConst<T> &P = A.P;
   const T third = T(1.0) / T(3.0), half = T(0.5);
@@ -616,21 +601,21 @@ __device__ __forceinline__ void team3_plane(const AcArgs<T> &A, const T *ring, T
       }
       T gx, gy, gz;
       {
-        const Dv<T> d = derive<T, true, true, false, PACED>(atf(AX), P);
+        const Dv<T> d = derive<T, true, true, false, true>(atf(AX), P);
         av[0] = d.v;
         By = d.gz, Bz = -d.gy;
         lax = d.xx + d.yy + d.zz;
         gx = d.xx, gy = d.xy, gz = d.xz;
       }
       {
-        const Dv<T> d = derive<T, true, false, true, PACED>(atf(AY), P);
+        const Dv<T> d = derive<T, true, false, true, true>(atf(AY), P);
         av[1] = d.v;
         Bx = -d.gz, Bz += d.gx;
         lay = d.xx + d.yy + d.zz;
         gx += d.xy, gy += d.yy, gz += d.yz;
       }
       {
-        const Dv<T> d = derive<T, false, true, true, PACED>(atf(AZ), P);
+        const Dv<T> d = derive<T, false, true, true, true>(atf(AZ), P);
         av[2] = d.v;
         Bx += d.gy, By -= d.gx;
         laz = d.xx + d.yy + d.zz;
@@ -663,7 +648,7 @@ __device__ __forceinline__ void team3_plane(const AcArgs<T> &A, const T *ring, T
       }
       T divu;
       {
-        const Dv<T> d = derive<T, true, true, false, PACED>(atf(UUX), P);
+        const Dv<T> d = derive<T, true, true, false, true>(atf(UUX), P);
         madv[0] = -(d.gx * ux + d.gy * uy + d.gz * uz);
         divu = d.gx;
         lu[0] = d.xx + d.yy + d.zz;
@@ -672,7 +657,7 @@ __device__ __forceinline__ void team3_plane(const AcArgs<T> &A, const T *ring, T
         S01 = half * d.gy, S02 = half * d.gz;
       }
       {
-        const Dv<T> d = derive<T, true, false, true, PACED>(atf(UUY), P);
+        const Dv<T> d = derive<T, true, false, true, true>(atf(UUY), P);
         madv[1] = -(d.gx * ux + d.gy * uy + d.gz * uz);
         divu += d.gy;
         lu[1] = d.xx + d.yy + d.zz;
@@ -681,7 +666,7 @@ __device__ __forceinline__ void team3_plane(const AcArgs<T> &A, const T *ring, T
         S01 += half * d.gx, S12 = half * d.gz;
       }
       {
-        const Dv<T> d = derive<T, false, true, true, PACED>(atf(UUZ), P);
+        const Dv<T> d = derive<T, false, true, true, true>(atf(UUZ), P);
         madv[2] = -(d.gx * ux + d.gy * uy + d.gz * uz);
         divu += d.gz;
         lu[2] = d.xx + d.yy + d.zz;
@@ -716,7 +701,7 @@ __device__ __forceinline__ void team3_plane(const AcArgs<T> &A, const T *ring, T
       if (STEP != 0) pl = A.out[LNRHO][idx], ps = A.out[ENTROPY][idx];
       T llr, lg[3];
       {
-        const Dv<T> d = derive<T, false, false, false, PACED>(atf(LNRHO), P);
+        const Dv<T> d = derive<T, false, false, false, true>(atf(LNRHO), P);
         lrv = d.v;
         lg[0] = d.gx, lg[1] = d.gy, lg[2] = d.gz;
         llr = d.xx + d.yy + d.zz;
@@ -727,7 +712,7 @@ __device__ __forceinline__ void team3_plane(const AcArgs<T> &A, const T *ring, T
 #pragma unroll
       for (int i = 0; i < 3; ++i) xb[(LG + i) * NC + cell] = lg[i];
       {
-        const Dv<T> d = derive<T, false, false, false, PACED>(atf(ENTROPY), P);
+        const Dv<T> d = derive<T, false, false, false, true>(atf(ENTROPY), P);
         sv = d.v;
         const T ls = d.xx + d.yy + d.zz;
         const T sg[3] = {d.gx, d.gy, d.gz};
@@ -805,7 +790,7 @@ __device__ __forceinline__ void ac_tma_load_3d(void *smem, const void *map, unsi
                : "memory");
 }
 
-template <int STEP, int TX, int TY, int NTEAM, bool PACED>
+template <int STEP, int TX, int TY, int NTEAM>
 __global__ void __launch_bounds__(NTEAM *TX *TY, 1) ac_team_tma_kernel(const __grid_constant__ AcArgs<double> A, const __grid_constant__ AcMaps maps, int xshift) {
   using T = double;
   constexpr int NSLOT = 8, W = TX + 8, H = TY + 6, PL = W * H, NC = TX * TY;
@@ -850,8 +835,8 @@ __global__ void __launch_bounds__(NTEAM *TX *TY, 1) ac_team_tma_kernel(const __g
     const int zi = z - z0;
     const bool more = z + 1 < z1;
     if (more && tid == 0) issue_plane(z + 4, (zi + 7) % NSLOT); // that slot held plane z - 4: nobody reads it any more
-    if (NTEAM == 2) team_plane<STEP, T, W, PL, NSLOT, NC, PACED>(A, ring, xb, zi, o0, cell, team == 1, valid, idx);
-    else team3_plane<STEP, T, W, PL, NSLOT, NC, PACED>(A, ring, xb, zi, o0, cell, team, valid, idx);
+    if (NTEAM == 2) team_plane<STEP, T, W, PL, NSLOT, NC>(A, ring, xb, zi, o0, cell, team == 1, valid, idx);
+    else team3_plane<STEP, T, W, PL, NSLOT, NC>(A, ring, xb, zi, o0, cell, team, valid, idx);
     if (more) ac_mbar_wait(&bars[(zi + 7) % NSLOT], unsigned((zi + 7) / NSLOT) & 1u);
     __syncthreads(); // everyone is done with plane z - 3 (and with xb) before the next iteration overwrites them
   }
@@ -861,13 +846,11 @@ template <int STEP, typename T, int TX, int TY> int launch_team(AcArgs<T> &A, cu
   constexpr int NSLOT = 8;
   constexpr size_t smem = (size_t(kAcFields) * NSLOT * (TX + 6) * (TY + 6) + 4 * TX * TY) * sizeof(T);
   static unsigned long long configured = 0;
-  static const bool paced = env_int("SB_AC_PACE", 1) != 0;
-  auto kern = paced ? ac_team_kernel<STEP, T, TX, TY, NSLOT, true> : ac_team_kernel<STEP, T, TX, TY, NSLOT, false>;
+  auto kern = ac_team_kernel<STEP, T, TX, TY, NSLOT>;
   int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   if (!(configured >> (dev & 63) & 1)) {
-    if (cudaFuncSetAttribute(ac_team_kernel<STEP, T, TX, TY, NSLOT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)) != cudaSuccess) return -1;
-    if (cudaFuncSetAttribute(ac_team_kernel<STEP, T, TX, TY, NSLOT, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)) != cudaSuccess) return -1;
+    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)) != cudaSuccess) return -1;
     configured |= 1ull << (dev & 63);
   }
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
@@ -881,22 +864,16 @@ template <int STEP, typename T, int TX, int TY> int launch_team(AcArgs<T> &A, cu
     const long long cost = ((ctas + sms - 1) / sms) * (len + 4);
     if (best_cost < 0 || cost < best_cost) best_cost = cost, best_len = len;
   }
-  const int forced = env_int("SB_AC_ZCHUNK", 0);
-  A.zchunk = forced > 0 ? (forced < ez ? forced : ez) : best_len;
+  A.zchunk = best_len;
   dim3 grid(gx, gy, (ez + A.zchunk - 1) / A.zchunk);
   kern<<<grid, 2 * TX * TY, smem, stream>>>(A);
   return 1;
 }
 
-int env_int(const char *name, int dflt) {
-  const char *s = getenv(name);
-  return (s && *s) ? atoi(s) : dflt;
-}
-
-template <int STEP, typename T, int TX, int TY, int NSLOT> int launch_tile(AcArgs<T> &A, cudaStream_t stream) {
-  constexpr size_t smem = size_t(kAcFields) * NSLOT * (TX + 6) * (TY + 6) * sizeof(T);
+template <int STEP, typename T, int TX, int TY> int launch_tile(AcArgs<T> &A, cudaStream_t stream) {
+  constexpr size_t smem = size_t(kAcFields) * 8 * (TX + 6) * (TY + 6) * sizeof(T); // a ring of 8 planes
   static unsigned long long configured = 0; // bit per device: the opt-in is per function and per context
-  auto kern = ac_tile_kernel<STEP, T, TX, TY, NSLOT>;
+  auto kern = ac_tile_kernel<STEP, T, TX, TY>;
   int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   if (!(configured >> (dev & 63) & 1)) {
@@ -916,8 +893,7 @@ template <int STEP, typename T, int TX, int TY, int NSLOT> int launch_tile(AcArg
     const long long cost = ((ctas + sms - 1) / sms) * (len + 7);
     if (best_cost < 0 || cost < best_cost) best_cost = cost, best_len = len;
   }
-  const int forced = env_int("SB_AC_ZCHUNK", 0);
-  A.zchunk = forced > 0 ? (forced < ez ? forced : ez) : best_len;
+  A.zchunk = best_len;
   dim3 grid(gx, gy, (ez + A.zchunk - 1) / A.zchunk);
   kern<<<grid, TX * TY, smem, stream>>>(A);
   return 1;
@@ -983,14 +959,12 @@ template <int STEP, int TX, int TY, int NTEAM> int launch_team_tma(AcArgs<double
     if ((reinterpret_cast<uintptr_t>(A.in[f]) & 15u) != phase) return 0; // one box origin for all fields
     if (!ac_field_map(A.in[f], A.mx, A.my, mz, W, H, maps.m[f])) return 0;
   }
-  static const bool paced = env_int("SB_AC_PACE", 1) != 0;
-  auto kern = paced ? ac_team_tma_kernel<STEP, TX, TY, NTEAM, true> : ac_team_tma_kernel<STEP, TX, TY, NTEAM, false>;
+  auto kern = ac_team_tma_kernel<STEP, TX, TY, NTEAM>;
   static unsigned long long configured = 0;
   int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   if (!(configured >> (dev & 63) & 1)) {
-    if (cudaFuncSetAttribute(ac_team_tma_kernel<STEP, TX, TY, NTEAM, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)) != cudaSuccess) return 0;
-    if (cudaFuncSetAttribute(ac_team_tma_kernel<STEP, TX, TY, NTEAM, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)) != cudaSuccess) return 0;
+    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(smem)) != cudaSuccess) return 0;
     configured |= 1ull << (dev & 63);
   }
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
@@ -1004,8 +978,7 @@ template <int STEP, int TX, int TY, int NTEAM> int launch_team_tma(AcArgs<double
     const long long cost = ((ctas + sms - 1) / sms) * (len + 3);
     if (best_cost < 0 || cost < best_cost) best_cost = cost, best_len = len;
   }
-  const int forced = env_int("SB_AC_ZCHUNK", 0);
-  A.zchunk = forced > 0 ? (forced < ez ? forced : ez) : best_len;
+  A.zchunk = best_len;
   dim3 grid(gx, gy, (ez + A.zchunk - 1) / A.zchunk);
   kern<<<grid, NTEAM * TX * TY, smem, stream>>>(A, maps, int(phase / 8));
   return 1;
@@ -1031,28 +1004,20 @@ template <int STEP, typename T> int launch_step(AcArgs<T> &A, long long mz, int 
   if (variant == AC_CELL) return launch_cell<STEP>(A, stream);
   if (variant == AC_TEAM || variant == AC_TEAM_TMA || variant == AC_TEAM3_TMA) {
     if constexpr (sizeof(T) == 8) {
-      if (variant != AC_TEAM || env_int("SB_AC_TMA", 1) != 0) {
-        // two teams by default; SB_AC_TEAMS=3 or variant 5 = three teams
-        const bool three = variant == AC_TEAM3_TMA || (variant == AC_TEAM && env_int("SB_AC_TEAMS", 2) == 3);
-        const int n = three ? launch_team_tma<STEP, 16, 10, 3>(A, mz, stream) : launch_team_tma<STEP, 16, 12, 2>(A, mz, stream);
-        if (n > 0) return n;
-        if (variant != AC_TEAM) return -4; // asked for explicitly and not applicable
-      }
+      // two teams, or three with variant AC_TEAM3_TMA
+      const int n = variant == AC_TEAM3_TMA ? launch_team_tma<STEP, 16, 10, 3>(A, mz, stream) : launch_team_tma<STEP, 16, 12, 2>(A, mz, stream);
+      if (n > 0) return n;
+      if (variant != AC_TEAM) return -4; // asked for explicitly and not applicable
       return launch_team<STEP, T, 16, 12>(A, stream);
     } else {
       if (variant != AC_TEAM) return -4;
       return launch_team<STEP, T, 32, 8>(A, stream);
     }
   }
-  const int shape = env_int("SB_AC_SHAPE", 0);
-  if constexpr (sizeof(T) == 8) {
-    if (shape == 1) return launch_tile<STEP, T, 16, 16, 7>(A, stream);
-    return launch_tile<STEP, T, 16, 14, 8>(A, stream);
-  } else {
-    // 32x8 tiles (256 threads) by default, SB_AC_SHAPE=1 for 32x16 (512 threads)
-    if (shape == 1) return launch_tile<STEP, T, 32, 16, 8>(A, stream);
-    return launch_tile<STEP, T, 32, 8, 8>(A, stream);
-  }
+  if constexpr (sizeof(T) == 8)
+    return launch_tile<STEP, T, 16, 14>(A, stream);
+  else
+    return launch_tile<STEP, T, 32, 8>(A, stream);
 }
 
 template <typename T>

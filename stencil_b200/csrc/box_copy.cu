@@ -95,224 +95,17 @@ __device__ __forceinline__ void copy_tile_dispatch(const Seg &s, unsigned row0, 
   }
 }
 
-// ------------------------------------------------------------------------------------------- TMA tiles
-constexpr int kTmaStages = 4;
-constexpr unsigned kTmaStageBytes = 8192;
-
-__device__ __forceinline__ unsigned smem_u32(const void *p) { return (unsigned)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(unsigned long long *bar, unsigned count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(unsigned long long *bar, unsigned bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(unsigned long long *bar, unsigned parity) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "SB_WAIT_%=:\n"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-      "@p bra SB_DONE_%=;\n"
-      "bra SB_WAIT_%=;\n"
-      "SB_DONE_%=:\n"
-      "}\n" ::"r"(smem_u32(bar)),
-      "r"(parity)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_3d(void *smem, const void *map, unsigned long long *bar, int x, int y, int z) {
-  asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(
-                   smem_u32(smem)),
-               "l"(map), "r"(smem_u32(bar)), "r"(x), "r"(y), "r"(z)
-               : "memory");
-}
-__device__ __forceinline__ void tma_store_3d(const void *map, const void *smem, int x, int y, int z) {
-  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.tile.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(map), "r"(smem_u32(smem)),
-               "r"(x), "r"(y), "r"(z)
-               : "memory");
-}
-
-// executed by ONE thread of the CTA
-__device__ void tma_tile(const TmaSeg &t, const void *smap, const void *dmap, unsigned row0, unsigned nrows, unsigned char *ring,
-                         unsigned long long *bars, unsigned &phases) {
-  const unsigned per_group = kTmaStageBytes / t.cstride; // chunks per ring stage (>= 4: chunks are <= 2 KiB)
-  const unsigned total = nrows * t.chunks_per_row;
-  const unsigned ngroups = (total + per_group - 1) / per_group;
-
-  auto coords = [&](unsigned c, int &cx, int &y, int &z) {
-    const unsigned r = row0 + c / t.chunks_per_row;
-    const unsigned zz = (unsigned)(((unsigned long long)r * t.ny_magic) >> t.ny_shift);
-    cx = (int)((c % t.chunks_per_row) * t.bx);
-    y = (int)(r - zz * t.ny);
-    z = (int)zz;
-  };
-  auto issue_loads = [&](unsigned g) {
-    const unsigned s = g % kTmaStages;
-    const unsigned first = g * per_group;
-    const unsigned n = (total - first < per_group) ? total - first : per_group;
-    mbar_expect_tx(&bars[s], n * t.chunk_bytes);
-    for (unsigned k = 0; k < n; ++k) {
-      int cx, y, z;
-      coords(first + k, cx, y, z);
-      tma_load_3d(ring + s * kTmaStageBytes + k * t.cstride, smap, &bars[s], t.sx0 + cx, t.sy0 + y, t.sz0 + z);
-    }
-  };
-
-  for (unsigned g = 0; g < ngroups && g < kTmaStages - 1; ++g) issue_loads(g);
-  for (unsigned g = 0; g < ngroups; ++g) {
-    const unsigned s = g % kTmaStages;
-    mbar_wait(&bars[s], (phases >> s) & 1u);
-    phases ^= 1u << s;
-    const unsigned first = g * per_group;
-    const unsigned n = (total - first < per_group) ? total - first : per_group;
-    for (unsigned k = 0; k < n; ++k) {
-      int cx, y, z;
-      coords(first + k, cx, y, z);
-      tma_store_3d(dmap, ring + s * kTmaStageBytes + k * t.cstride, t.dx0 + cx, t.dy0 + y, t.dz0 + z);
-    }
-    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-    const unsigned gn = g + kTmaStages - 1;
-    if (gn < ngroups) {
-      // the ring slot of group gn was last used by group g-1: its stores must have finished READING it
-      asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
-      issue_loads(gn);
-    }
-  }
-  asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-}
-
 // Persistent walk over the tile table: grid is a multiple of the SM count, tiles are taken
 // round-robin so consecutive CTAs stream consecutive rows of the same segment.
-// kind 2: one thread feeds the ring with TMA loads, all threads drain it with vector stores
-__device__ void tma_ld_tile(const TmaSeg &t, const void *smap, unsigned row0, unsigned nrows, unsigned char *ring, unsigned long long *bars,
-                            unsigned &phases) {
-  const unsigned per_group = kTmaStageBytes / t.cstride;
-  const unsigned total = nrows * t.chunks_per_row;
-  const unsigned ngroups = (total + per_group - 1) / per_group;
-  const unsigned box_bytes = t.bxa * t.es;
-  const unsigned po = t.pre * t.es;        // payload offset inside a chunk image
-  const unsigned pay = t.chunk_bytes;      // payload bytes per chunk
-
-  auto coords = [&](unsigned c, unsigned &cxe, unsigned &y, unsigned &z) {
-    const unsigned r = row0 + c / t.chunks_per_row;
-    z = (unsigned)(((unsigned long long)r * t.ny_magic) >> t.ny_shift);
-    y = r - z * t.ny;
-    cxe = (c % t.chunks_per_row) * t.bx; // payload element offset of this chunk inside its row
-  };
-  auto issue_loads = [&](unsigned g) { // thread 0 only
-    const unsigned s = g % kTmaStages;
-    const unsigned first = g * per_group;
-    const unsigned n = (total - first < per_group) ? total - first : per_group;
-    mbar_expect_tx(&bars[s], n * box_bytes);
-    for (unsigned k = 0; k < n; ++k) {
-      unsigned cxe, y, z;
-      coords(first + k, cxe, y, z);
-      tma_load_3d(ring + s * kTmaStageBytes + k * t.cstride, smap, &bars[s], t.sx0 - (int)t.pre + (int)cxe, t.sy0 + (int)y, t.sz0 + (int)z);
-    }
-  };
-
-  if (threadIdx.x == 0)
-    for (unsigned g = 0; g < ngroups && g < kTmaStages - 1; ++g) issue_loads(g);
-
-  const unsigned lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  for (unsigned g = 0; g < ngroups; ++g) {
-    // everybody has finished reading the slot that is refilled next (group g-1's)
-    __syncthreads();
-    if (threadIdx.x == 0 && g + kTmaStages - 1 < ngroups) issue_loads(g + kTmaStages - 1);
-    const unsigned s = g % kTmaStages;
-    mbar_wait(&bars[s], (phases >> s) & 1u);
-    phases ^= 1u << s;
-    const unsigned first = g * per_group;
-    const unsigned n = (total - first < per_group) ? total - first : per_group;
-    // one warp per chunk
-    for (unsigned k = warp; k < n; k += kCopyThreads / 32) {
-      unsigned cxe, y, z;
-      coords(first + k, cxe, y, z);
-      const unsigned char *img = ring + s * kTmaStageBytes + k * t.cstride;
-      char *d = t.dst + (long long)z * t.dst_slice + (long long)y * t.dst_pitch + (long long)cxe * t.es;
-      if (t.same_phase) {
-        // 16-byte vectors of the aligned image; the first and last may hold ghost / trailing bytes
-        char *dal = d - po;
-        const unsigned nv = box_bytes / 16;
-        for (unsigned j = lane; j < nv; j += 32) {
-          const uint4 v = *reinterpret_cast<const uint4 *>(img + 16 * j);
-          const unsigned lo = (16 * j < po) ? po : 16 * j;
-          const unsigned hi = (16 * j + 16 > po + pay) ? po + pay : 16 * j + 16;
-          if (hi - lo == 16) {
-            *reinterpret_cast<uint4 *>(dal + 16 * j) = v;
-          } else if (hi > lo) {
-            const unsigned char *vb = reinterpret_cast<const unsigned char *>(&v);
-            if (t.es == 8) {
-              for (unsigned b = lo; b < hi; b += 8)
-                *reinterpret_cast<unsigned long long *>(dal + b) = *reinterpret_cast<const unsigned long long *>(vb + (b - 16 * j));
-            } else {
-              for (unsigned b = lo; b < hi; b += 4)
-                *reinterpret_cast<unsigned *>(dal + b) = *reinterpret_cast<const unsigned *>(vb + (b - 16 * j));
-            }
-          }
-        }
-      } else if (t.vec == 8) {
-        for (unsigned j = lane; j < pay / 8; j += 32)
-          reinterpret_cast<unsigned long long *>(d)[j] = *reinterpret_cast<const unsigned long long *>(img + po + 8 * j);
-      } else {
-        for (unsigned j = lane; j < pay / 4; j += 32) reinterpret_cast<unsigned *>(d)[j] = *reinterpret_cast<const unsigned *>(img + po + 4 * j);
-      }
-    }
-  }
-}
-
-template <bool TMA> struct CopyShared {
-  Seg seg;
-  Tile tile;
-};
-template <> struct CopyShared<true> {
-  alignas(128) unsigned char ring[kTmaStages * kTmaStageBytes];
-  alignas(8) unsigned long long bars[kTmaStages];
-  Seg seg;
-  Tile tile;
-};
-
-template <bool TMA>
-__device__ __forceinline__ void box_copy_body(CopyShared<TMA> &sh, const Seg *__restrict__ segs, const TmaSeg *__restrict__ tsegs,
-                                              const TmaMaps *maps, const Tile *__restrict__ tiles, unsigned ntiles) {
-  Seg &seg = sh.seg;
-  Tile &tile = sh.tile;
+__global__ void __launch_bounds__(kCopyThreads, 3)
+    box_copy_kernel(const Seg *__restrict__ segs, const Tile *__restrict__ tiles, unsigned ntiles) {
+  __shared__ Seg seg;
+  __shared__ Tile tile;
   unsigned cached = 0xFFFFFFFFu;
-  unsigned phases = 0; // parity of each ring barrier (thread 0)
-  if constexpr (TMA) {
-    if (threadIdx.x == 0) {
-      for (int i = 0; i < kTmaStages; ++i) mbar_init(&sh.bars[i], 1);
-      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    }
-  }
   for (unsigned t = blockIdx.x; t < ntiles; t += gridDim.x) {
     __syncthreads(); // previous tile done before the descriptors are replaced
     if (threadIdx.x == 0) tile = tiles[t];
     __syncthreads();
-    if constexpr (TMA) {
-      if (tile.kind == 1) { // TMA tile: one elected thread drives the copy engine
-        __shared__ TmaSeg ts1;
-        if (threadIdx.x == 0) ts1 = tsegs[tile.seg];
-        __syncthreads();
-        unsigned mine = phases;
-        if (threadIdx.x == 0) tma_tile(ts1, &maps->m[ts1.smap][0], &maps->m[ts1.dmap][0], tile.row0, tile.nrows, sh.ring, sh.bars, mine);
-        // every thread keeps the ring-barrier parities in step (kind-2 tiles wait on them with all threads)
-        const unsigned per_group = kTmaStageBytes / ts1.cstride;
-        const unsigned ngroups = (tile.nrows * ts1.chunks_per_row + per_group - 1) / per_group;
-#pragma unroll
-        for (unsigned st = 0; st < kTmaStages; ++st)
-          if (((ngroups + kTmaStages - 1 - st) / kTmaStages) & 1u) phases ^= 1u << st;
-        continue;
-      }
-      if (tile.kind == 2) { // TMA loads by one thread, vector stores by all
-        __shared__ TmaSeg ts2;
-        if (threadIdx.x == 0) ts2 = tsegs[tile.seg];
-        __syncthreads();
-        tma_ld_tile(ts2, &maps->m[ts2.smap][0], tile.row0, tile.nrows, sh.ring, sh.bars, phases);
-        continue;
-      }
-    }
     if (tile.seg != cached) {
       // cooperative 80-byte descriptor fetch
       if (threadIdx.x < sizeof(Seg) / 4)
@@ -322,20 +115,6 @@ __device__ __forceinline__ void box_copy_body(CopyShared<TMA> &sh, const Seg *__
     }
     copy_tile_dispatch(seg, tile.row0, tile.nrows);
   }
-}
-
-__global__ void __launch_bounds__(kCopyThreads, 3)
-    box_copy_kernel(const Seg *__restrict__ segs, const Tile *__restrict__ tiles, unsigned ntiles) {
-  __shared__ CopyShared<false> sh;
-  box_copy_body<false>(sh, segs, nullptr, nullptr, tiles, ntiles);
-}
-
-// Same walk, plus TMA tiles; the tensor maps are a __grid_constant__ parameter.
-__global__ void __launch_bounds__(kCopyThreads, 3)
-    box_copy_tma_kernel(const Seg *__restrict__ segs, const TmaSeg *__restrict__ tsegs, const __grid_constant__ TmaMaps maps,
-                        const Tile *__restrict__ tiles, unsigned ntiles) {
-  __shared__ CopyShared<true> sh;
-  box_copy_body<true>(sh, segs, tsegs, &maps, tiles, ntiles);
 }
 
 // One segment passed by value: the pack_kernel / unpack_kernel / translate one-shots.
@@ -355,12 +134,8 @@ __global__ void __launch_bounds__(kCopyThreads, 3) box_copy_single_kernel(const 
 
 } // namespace
 
-void launch_box_copy(const Seg *segs_dev, const TmaSeg *tsegs_dev, const TmaMaps *maps_host, const Tile *tiles_dev, unsigned ntiles, int grid,
-                     cudaStream_t stream) {
-  if (tsegs_dev != nullptr && maps_host != nullptr)
-    box_copy_tma_kernel<<<grid, kCopyThreads, 0, stream>>>(segs_dev, tsegs_dev, *maps_host, tiles_dev, ntiles);
-  else
-    box_copy_kernel<<<grid, kCopyThreads, 0, stream>>>(segs_dev, tiles_dev, ntiles);
+void launch_box_copy(const Seg *segs_dev, const Tile *tiles_dev, unsigned ntiles, int grid, cudaStream_t stream) {
+  box_copy_kernel<<<grid, kCopyThreads, 0, stream>>>(segs_dev, tiles_dev, ntiles);
 }
 
 unsigned rows_per_tile_for(unsigned row_bytes) {
@@ -375,7 +150,6 @@ void preload_box_copy_kernels() {
   // the module load (bench_pack of the reference has no warm-up iteration)
   cudaFuncAttributes a;
   cudaFuncGetAttributes(&a, box_copy_kernel);
-  cudaFuncGetAttributes(&a, box_copy_tma_kernel);
   cudaFuncGetAttributes(&a, box_copy_single_kernel);
 }
 

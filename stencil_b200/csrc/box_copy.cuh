@@ -36,62 +36,17 @@ struct Seg {
   unsigned long long ny_magic;
 };
 
-// Opt-in (SB_TMA=1) TMA tile kinds for wide segments.  Constraints (probed with scripts/exp/tma_probe3.cu):
-// a box's global START address must be 16-byte aligned (element-granular coordinates do NOT absorb an 8-byte row
-// phase: UTMALDG/UTMASTG raise "illegal instruction"), and its shared-memory address must be 128-byte aligned.
-//   kind 1  both sides TMA-legal (16-byte aligned base, strides and box start, e.g. r=2 FP64): cp.async.bulk.tensor
-//           global -> shared (mbarrier complete_tx) then shared -> global (bulk_group), ONE elected thread per CTA,
-//           4-stage shared-memory ring, a row cut into chunks of `bx` elements (box = bx x 1 x 1).
-//   kind 2  source rows start off a 16-byte boundary (r=1 FP64): aligned-down TMA load, vector stores by all threads.
-// Result on the B200 they were written on (not re-timed on the H100): for halo-sized messages (2-4 MB, <1 tile per
-// SM) both kinds were slower than the LSU path below, which is why they are off by default.
-constexpr int kMaxTmaMaps = 16;
-
-// The CUtensorMap descriptors travel as a __grid_constant__ kernel parameter (the documented-safe home
-// of a host-encoded tensor map); 128 bytes each, opaque here so that this header needs no <cuda.h>.
-struct alignas(64) TmaMaps {
-  unsigned long long m[kMaxTmaMaps][16];
-};
-
-struct TmaSeg {
-  int smap; // index into TmaMaps: tensor map of the source allocation
-  int dmap;
-  int sx0, sy0, sz0; // region start inside the source tensor (elements / rows / planes)
-  int dx0, dy0, dz0;
-  unsigned bx;             // chunk width (elements)
-  unsigned chunks_per_row; // ext.x / bx
-  unsigned chunk_bytes;
-  unsigned ny, nz;
-  unsigned ny_shift;
-  unsigned long long ny_magic;
-  // kind 2 ("TMA load, vector store"): the halo rows of an FP64 r=1 subdomain start 8 bytes into a
-  // 16-byte vector, and a TMA box must START on a 16-byte boundary (measured: UTMALDG raises an illegal
-  // instruction otherwise).  The load therefore begins `pre` elements early (box = bxa elements, a
-  // multiple of 16 bytes covering pre + bx), the payload sits `pre * es` bytes into each shared-memory
-  // chunk, and all threads of the CTA store it to the destination -- 128-bit stores when source and
-  // destination rows have the same phase (peeling the first / last element), else the widest aligned.
-  char *dst;              // destination of the box's first payload byte
-  long long dst_pitch, dst_slice;
-  unsigned pre;           // elements loaded before the payload in every chunk
-  unsigned bxa;           // box width (elements) of the source map
-  unsigned cstride;       // bytes a chunk occupies in the ring (multiple of 128)
-  unsigned es;            // element size
-  unsigned vec;           // store width when the phases differ
-  unsigned same_phase;    // 1: (dst - pre*es) is 16-byte aligned for every row
-};
-
 struct Tile {
-  unsigned seg; // index into the Seg table (kind 0) or the TmaSeg table (kinds 1, 2)
+  unsigned seg; // index into the Seg table
   unsigned row0;
   unsigned nrows;
-  unsigned kind;
 };
 
 constexpr int kCopyThreads = 256;
 constexpr unsigned kTileBytes = 16384;
+constexpr int kCopyCtasPerSm = 8; // persistent grid of a copy plan: CTAs per SM
 
-void launch_box_copy(const Seg *segs_dev, const TmaSeg *tsegs_dev, const TmaMaps *maps_host, const Tile *tiles_dev, unsigned ntiles, int grid,
-                     cudaStream_t stream);
+void launch_box_copy(const Seg *segs_dev, const Tile *tiles_dev, unsigned ntiles, int grid, cudaStream_t stream);
 void launch_box_copy_single(const Seg &seg, cudaStream_t stream);
 unsigned rows_per_tile_for(unsigned row_bytes); // tile height for a segment
 void preload_box_copy_kernels();

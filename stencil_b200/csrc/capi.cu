@@ -13,7 +13,6 @@
 #include <string>
 #include <vector>
 
-#include <cuda.h> // CUtensorMap types only: the driver entry point is resolved at run time, libcuda is not linked
 #include <cuda_runtime.h>
 
 #include "box_copy.cuh"
@@ -198,226 +197,6 @@ int build_segments(const sb_box_copy &c, std::vector<sb::Seg> &out) {
   return emit(src, dst, row_bytes, ny, nz, sp, ss, dp, ds);
 }
 
-int env_int(const char *name, int dflt);
-
-// ------------------------------------------------------------------------------------------- TMA segments
-typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *,
-                                  const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-EncodeTiledFn encode_tiled_fn() {
-  static EncodeTiledFn fn = []() -> EncodeTiledFn {
-    void *p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess) {
-      cudaGetLastError();
-      return nullptr;
-    }
-    return reinterpret_cast<EncodeTiledFn>(p);
-  }();
-  return fn;
-}
-
-struct MapKey {
-  void *ptr;
-  int64_t pitch, ysize, es;
-  unsigned bx;
-  bool operator==(const MapKey &o) const { return ptr == o.ptr && pitch == o.pitch && ysize == o.ysize && es == o.es && bx == o.bx; }
-};
-
-struct TmaBuild {
-  std::vector<CUtensorMap> maps;
-  std::vector<MapKey> keys;
-  std::vector<sb::TmaSeg> segs; // smap/dmap are indices into maps
-  std::vector<int> kinds;       // 1 = TMA load + TMA store, 2 = TMA load + vector stores
-};
-
-// tensor map of a whole allocation, box = bx x 1 x 1 elements
-int tma_map_index(TmaBuild &tb, const sb_pitched &a, int64_t es, unsigned bx) {
-  const MapKey key{a.ptr, a.pitch, a.ysize, es, bx};
-  for (size_t i = 0; i < tb.keys.size(); ++i)
-    if (tb.keys[i] == key) return int(i);
-  if (tb.maps.size() >= size_t(sb::kMaxTmaMaps)) return -1; // parameter space holds kMaxTmaMaps descriptors
-  CUtensorMapDataType dt = es == 8 ? CU_TENSOR_MAP_DATA_TYPE_UINT64
-                           : es == 4 ? CU_TENSOR_MAP_DATA_TYPE_UINT32
-                                     : es == 2 ? CU_TENSOR_MAP_DATA_TYPE_UINT16 : CU_TENSOR_MAP_DATA_TYPE_UINT8;
-  const cuuint64_t dims[3] = {cuuint64_t(a.pitch / es), cuuint64_t(a.ysize), cuuint64_t(1) << 20};
-  const cuuint64_t strides[2] = {cuuint64_t(a.pitch), cuuint64_t(a.pitch) * cuuint64_t(a.ysize)};
-  const cuuint32_t box[3] = {bx, 1, 1};
-  const cuuint32_t estr[3] = {1, 1, 1};
-  CUtensorMap m;
-  const CUresult r = encode_tiled_fn()(&m, dt, 3, a.ptr, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                                       CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return -1;
-  tb.maps.push_back(m);
-  tb.keys.push_back(key);
-  return int(tb.maps.size()) - 1;
-}
-
-// returns true if the copy was taken over by the TMA path
-bool try_tma_segment(const sb_box_copy &c, TmaBuild &tb, int plan_device) {
-  const int enabled = env_int("SB_TMA", 0); // opt-in: slower than the LSU path for halo-sized messages
-  static const int peer_ok = env_int("SB_TMA_PEER", 1); // TMA stores into peer-mapped (NVLink) memory
-  if (!enabled || !encode_tiled_fn()) return false;
-  if (!peer_ok) {
-    cudaPointerAttributes at;
-    if (cudaPointerGetAttributes(&at, c.dst.ptr) != cudaSuccess) {
-      cudaGetLastError();
-      return false;
-    }
-    if (at.type == cudaMemoryTypeDevice && at.device != plan_device) return false;
-  }
-  const int64_t es = c.elem_size;
-  if (es != 1 && es != 2 && es != 4 && es != 8) return false;
-  const int64_t row_bytes = c.extent[0] * es;
-  if (row_bytes < 512) return false; // thin rows stay on the LSU path
-  for (const sb_pitched *a : {&c.src, &c.dst}) {
-    if ((uintptr_t(a->ptr) & 15) || (a->pitch & 15) || ((a->pitch * a->ysize) & 15) || (a->pitch % es)) return false;
-    if (a->pitch * a->ysize >= (int64_t(1) << 40)) return false;
-  }
-  // Probed with scripts/exp/tma_probe3.cu: the global address a box starts at must itself be 16-byte
-  // aligned -- a UINT64 box at x = 1 (or an INT32 box at x = 1..3) raises "illegal instruction" at the
-  // UTMALDG, x = 2 (x = 4) is fine.  Rows of an FP64 r=1 halo start 8 bytes into the row, so they are NOT
-  // directly TMA-addressable; such segments take the LSU path (or the aligned-down TMA-load kind).
-  if ((c.src_pos[0] * es) & 15 || (c.dst_pos[0] * es) & 15) return false;
-  // chunk width: the whole row if it fits a box, else its largest divisor that does
-  unsigned bx = 0;
-  for (int64_t d = std::min<int64_t>(256, c.extent[0]); d >= 1; --d) {
-    if (c.extent[0] % d == 0 && (d * es) % 16 == 0 && d * es >= 256) {
-      bx = unsigned(d);
-      break;
-    }
-  }
-  if (0 == bx) return false;
-  const int64_t rows = c.extent[1] * c.extent[2];
-  if (rows >= (1 << 24) || c.extent[1] >= (1 << 24)) return false;
-  for (int a = 0; a < 3; ++a)
-    if (c.src_pos[a] + c.extent[a] >= (int64_t(1) << 20) && a == 2) return false;
-  const int si = tma_map_index(tb, c.src, es, bx), di = tma_map_index(tb, c.dst, es, bx);
-  if (si < 0 || di < 0) return false;
-  sb::TmaSeg t{};
-  t.sx0 = int(c.src_pos[0]);
-  t.sy0 = int(c.src_pos[1]);
-  t.sz0 = int(c.src_pos[2]);
-  t.dx0 = int(c.dst_pos[0]);
-  t.dy0 = int(c.dst_pos[1]);
-  t.dz0 = int(c.dst_pos[2]);
-  t.bx = bx;
-  t.chunks_per_row = unsigned(c.extent[0] / bx);
-  t.chunk_bytes = unsigned(bx * es);
-  t.ny = unsigned(c.extent[1]);
-  t.nz = unsigned(c.extent[2]);
-  const unsigned bits = ceil_log2(t.ny);
-  t.ny_shift = 24 + bits;
-  t.ny_magic = ((1ull << t.ny_shift) + t.ny - 1) / t.ny;
-  t.smap = si;
-  t.dmap = di;
-  t.cstride = (t.chunk_bytes + 127u) & ~127u; // shared-memory box addresses must be 128-byte aligned
-  t.es = unsigned(es);
-  tb.segs.push_back(t);
-  tb.kinds.push_back(1);
-  return true;
-}
-
-// kind 2: TMA loads from an aligned-down start + vector stores by the CTA (see box_copy.cuh).  Applies to
-// wide rows of 4- or 8-byte elements whose SOURCE allocation is TMA-legal; the destination can be anything.
-bool try_tma_load_segment(const sb_box_copy &c, TmaBuild &tb) {
-  const int enabled = env_int("SB_TMA", 0) && env_int("SB_TMA_LOAD", 1);
-  if (!enabled || !encode_tiled_fn()) return false;
-  const int64_t es = c.elem_size;
-  if (es != 4 && es != 8) return false;
-  if (c.extent[0] * es < 512) return false;
-  const sb_pitched &a = c.src;
-  if ((uintptr_t(a.ptr) & 15) || (a.pitch & 15) || ((a.pitch * a.ysize) & 15) || (a.pitch % es)) return false;
-  if (a.pitch * a.ysize >= (int64_t(1) << 40)) return false;
-  const int64_t po = (c.src_pos[0] * es) & 15; // bytes between the aligned-down start and the payload
-  const int64_t pre = po / es;
-  if (c.src_pos[0] - pre < 0) return false;
-  // payload chunk: a divisor of the row, a multiple of 16 bytes, box (pre + bx rounded up to 16 B) <= 256 elements
-  unsigned bx = 0, bxa = 0;
-  for (int64_t d = std::min<int64_t>(256, c.extent[0]); d >= 1; --d) {
-    if (c.extent[0] % d || (d * es) % 16 || d * es < 256) continue;
-    const int64_t box_bytes = (po + d * es + 15) & ~int64_t(15);
-    if (box_bytes / es > 256) continue;
-    bx = unsigned(d);
-    bxa = unsigned(box_bytes / es);
-    break;
-  }
-  if (0 == bx) return false;
-  if (c.src_pos[0] - pre + c.extent[0] - bx + bxa > a.pitch / es) return false; // the last box must stay inside the row
-  const int64_t rows = c.extent[1] * c.extent[2];
-  if (rows >= (1 << 24) || c.extent[1] >= (1 << 24) || c.src_pos[2] + c.extent[2] >= (int64_t(1) << 20)) return false;
-  const int si = tma_map_index(tb, c.src, es, bxa);
-  if (si < 0) return false;
-  sb::TmaSeg t{};
-  t.smap = si;
-  t.dmap = -1;
-  t.sx0 = int(c.src_pos[0]);
-  t.sy0 = int(c.src_pos[1]);
-  t.sz0 = int(c.src_pos[2]);
-  t.bx = bx;
-  t.chunks_per_row = unsigned(c.extent[0] / bx);
-  t.chunk_bytes = unsigned(bx * es); // payload bytes per chunk
-  t.ny = unsigned(c.extent[1]);
-  t.nz = unsigned(c.extent[2]);
-  const unsigned bits = ceil_log2(t.ny);
-  t.ny_shift = 24 + bits;
-  t.ny_magic = ((1ull << t.ny_shift) + t.ny - 1) / t.ny;
-  t.dst = static_cast<char *>(c.dst.ptr) + (c.dst_pos[2] * c.dst.ysize + c.dst_pos[1]) * c.dst.pitch + c.dst_pos[0] * es;
-  t.dst_pitch = c.dst.pitch;
-  t.dst_slice = c.dst.pitch * c.dst.ysize;
-  t.pre = unsigned(pre);
-  t.bxa = bxa;
-  t.cstride = unsigned((bxa * es + 127) & ~int64_t(127));
-  t.es = unsigned(es);
-  unsigned long long align = (unsigned long long)(uintptr_t)t.dst | (unsigned long long)po | (unsigned long long)(bx * es);
-  if (t.ny > 1) align |= (unsigned long long)t.dst_pitch;
-  if (t.nz > 1) align |= (unsigned long long)t.dst_slice;
-  t.vec = (align % 8 == 0 && es == 8) ? 8 : ((align % 8 == 0) ? 8 : 4);
-  if (t.vec > 4 && (align % 8)) t.vec = 4;
-  unsigned long long ph = ((unsigned long long)(uintptr_t)t.dst - (unsigned long long)po);
-  if (t.ny > 1) ph |= (unsigned long long)t.dst_pitch;
-  if (t.nz > 1) ph |= (unsigned long long)t.dst_slice;
-  t.same_phase = (ph % 16 == 0) ? 1u : 0u;
-  tb.segs.push_back(t);
-  tb.kinds.push_back(2);
-  return true;
-}
-
-void build_tma_tiles(const std::vector<sb::TmaSeg> &segs, const std::vector<int> &kinds, std::vector<sb::Tile> &tiles) {
-  for (size_t si = 0; si < segs.size(); ++si) {
-    const sb::TmaSeg &g = segs[si];
-    if (kinds[si] == 2) {
-      // all threads work on these: normal tile size
-      const unsigned row_bytes = g.chunk_bytes * g.chunks_per_row;
-      unsigned rows_per_tile = (2 * sb::kTileBytes) / row_bytes;
-      if (rows_per_tile < 1) rows_per_tile = 1;
-      const unsigned total = g.ny * g.nz;
-      for (unsigned r = 0; r < total; r += rows_per_tile) {
-        sb::Tile t{};
-        t.seg = unsigned(si);
-        t.row0 = r;
-        t.nrows = (total - r < rows_per_tile) ? total - r : rows_per_tile;
-        t.kind = 2;
-        tiles.push_back(t);
-      }
-      continue;
-    }
-    const unsigned row_bytes = g.chunk_bytes * g.chunks_per_row;
-    unsigned rows_per_tile = 65536u / row_bytes; // one thread drives a tile: make it big
-    if (rows_per_tile < 1) rows_per_tile = 1;
-    const unsigned total = g.ny * g.nz;
-    for (unsigned r = 0; r < total; r += rows_per_tile) {
-      sb::Tile t{};
-      t.seg = unsigned(si);
-      t.row0 = r;
-      t.nrows = (total - r < rows_per_tile) ? total - r : rows_per_tile;
-      t.kind = 1;
-      tiles.push_back(t);
-    }
-  }
-}
-
 void build_tiles(const std::vector<sb::Seg> &segs, std::vector<sb::Tile> &tiles) {
   for (size_t si = 0; si < segs.size(); ++si) {
     const sb::Seg &g = segs[si];
@@ -428,15 +207,9 @@ void build_tiles(const std::vector<sb::Seg> &segs, std::vector<sb::Tile> &tiles)
       t.seg = unsigned(si);
       t.row0 = r;
       t.nrows = (total - r < rows_per_tile) ? total - r : rows_per_tile;
-      t.kind = 0;
       tiles.push_back(t);
     }
   }
-}
-
-int env_int(const char *name, int dflt) {
-  const char *s = getenv(name);
-  return (s && *s) ? atoi(s) : dflt;
 }
 
 struct SlotTable {
@@ -584,9 +357,6 @@ struct sb_stencil_plan {
 struct sb_copy_plan {
   int device = 0;
   sb::Seg *segs_dev = nullptr;
-  sb::TmaSeg *tsegs_dev = nullptr;
-  sb::TmaMaps *maps_host = nullptr; // passed by value as a __grid_constant__ kernel parameter
-  unsigned ntma = 0;
   sb::Tile *tiles_dev = nullptr;
   unsigned ntiles = 0;
   unsigned nsegs = 0;
@@ -721,17 +491,13 @@ int sb_translate(sb_pitched dst, const int64_t dst_pos[3], sb_pitched src, const
 int sb_copy_plan_create(sb_copy_plan **out, int device, const sb_box_copy *copies, int64_t n) {
   if (!out || (n > 0 && !copies) || n < 0) return fail(SB_ERR_INVALID, "bad arguments to sb_copy_plan_create");
   std::vector<sb::Seg> segs;
-  TmaBuild tb;
   int64_t bytes = 0;
   for (int64_t i = 0; i < n; ++i) {
     bytes += copies[i].extent[0] * copies[i].extent[1] * copies[i].extent[2] * copies[i].elem_size;
-    if (try_tma_segment(copies[i], tb, device)) continue;
-    if (try_tma_load_segment(copies[i], tb)) continue;
     int rc = build_segments(copies[i], segs);
     if (rc != SB_OK) return rc;
   }
   std::vector<sb::Tile> tiles;
-  build_tma_tiles(tb.segs, tb.kinds, tiles); // big tiles first: they take longest
   build_tiles(segs, tiles);
 
   DeviceGuard guard(device);
@@ -742,24 +508,14 @@ int sb_copy_plan_create(sb_copy_plan **out, int device, const sb_box_copy *copie
   p->bytes = bytes;
   p->nsegs = unsigned(segs.size());
   p->ntiles = unsigned(tiles.size());
-  p->ntma = unsigned(tb.segs.size());
   if (p->ntiles) {
-    if (!tb.segs.empty()) {
-      static_assert(sizeof(CUtensorMap) == 128, "CUtensorMap is 128 bytes");
-      p->maps_host = new sb::TmaMaps();
-      std::memset(p->maps_host, 0, sizeof(sb::TmaMaps));
-      for (size_t i = 0; i < tb.maps.size(); ++i) std::memcpy(&p->maps_host->m[i][0], &tb.maps[i], sizeof(CUtensorMap));
-      SB_CUDA(cudaMalloc(&p->tsegs_dev, tb.segs.size() * sizeof(sb::TmaSeg)));
-      SB_CUDA(cudaMemcpy(p->tsegs_dev, tb.segs.data(), tb.segs.size() * sizeof(sb::TmaSeg), cudaMemcpyHostToDevice));
-    }
     SB_CUDA(cudaMalloc(&p->segs_dev, (segs.size() + 1) * sizeof(sb::Seg)));
     SB_CUDA(cudaMalloc(&p->tiles_dev, tiles.size() * sizeof(sb::Tile)));
     SB_CUDA(cudaMemcpy(p->segs_dev, segs.data(), segs.size() * sizeof(sb::Seg), cudaMemcpyHostToDevice));
     SB_CUDA(cudaMemcpy(p->tiles_dev, tiles.data(), tiles.size() * sizeof(sb::Tile), cudaMemcpyHostToDevice));
     int sms = 132;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
-    const int per_sm = env_int("SB_COPY_CTAS_PER_SM", 8);
-    const long long cap = (long long)sms * per_sm;
+    const long long cap = (long long)sms * sb::kCopyCtasPerSm;
     p->grid = int(p->ntiles < cap ? p->ntiles : cap);
   }
   *out = p;
@@ -771,7 +527,7 @@ int sb_copy_plan_launch(sb_copy_plan *p, void *stream) {
   if (0 == p->ntiles) return SB_OK;
   DeviceGuard guard(p->device);
   if (!guard.ok) return fail(SB_ERR_NOGPU, "cannot select CUDA device %d", p->device);
-  sb::launch_box_copy(p->segs_dev, p->tsegs_dev, p->maps_host, p->tiles_dev, p->ntiles, p->grid, static_cast<cudaStream_t>(stream));
+  sb::launch_box_copy(p->segs_dev, p->tiles_dev, p->ntiles, p->grid, static_cast<cudaStream_t>(stream));
   ++g_launches;
   SB_CUDA(cudaGetLastError());
   return SB_OK;
@@ -779,14 +535,11 @@ int sb_copy_plan_launch(sb_copy_plan *p, void *stream) {
 
 int64_t sb_copy_plan_bytes(const sb_copy_plan *p) { return p ? p->bytes : 0; }
 int64_t sb_copy_plan_num_tiles(const sb_copy_plan *p) { return p ? p->ntiles : 0; }
-int64_t sb_copy_plan_num_tma_segments(const sb_copy_plan *p) { return p ? p->ntma : 0; }
 
 int sb_copy_plan_destroy(sb_copy_plan *p) {
   if (!p) return SB_OK;
   DeviceGuard guard(p->device);
   if (p->segs_dev) cudaFree(p->segs_dev);
-  if (p->tsegs_dev) cudaFree(p->tsegs_dev);
-  delete p->maps_host;
   if (p->tiles_dev) cudaFree(p->tiles_dev);
   delete p;
   return SB_OK;

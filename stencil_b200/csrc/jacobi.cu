@@ -94,7 +94,7 @@ __shared__ uint4 g_zstage[8 * 32];
 // The kernel is latency- and issue-bound at once (53 % issue utilisation with 8 warps per scheduler): every instruction
 // added to the loop shows in the run time, so each boundary CTA runs the leanest variant that serves its faces.
 template <typename T, int VX, int RY, bool SHIFT, int MODE>
-__device__ __forceinline__ void march_body(const JacobiParams &p, const int bx, const int by, const int bz, const bool wait_barrier = false, const int debug = 0) {
+__device__ __forceinline__ void march_body(const JacobiParams &p, const int bx, const int by, const int bz, const bool wait_barrier = false) {
   static_assert(!SHIFT || (RY == 1 && VX >= 2), "the phase-shifted variant handles one row per warp");
   static_assert(!MODE || RY == 1, "the boundary variants handle one row per warp");
   static_assert(MODE == 0 || (MODE & 1), "XPUSH / YPUSH imply EDGE");
@@ -154,7 +154,7 @@ __device__ __forceinline__ void march_body(const JacobiParams &p, const int bx, 
     ph[j] = src + (long long)z0 * S + yo(y + j) + (long long)hx * (long long)sizeof(T);
     if (XP) { // the x neighbour of the first / last compute cell may come from a dense received array [y][z]
       const int side = (lane == 0 && x == p.lo[0]) ? 0 : ((lane == 31 && x + VX == p.hi[0]) ? 1 : -1);
-      if (side >= 0 && p.xghost_ptr[side] && !(debug & 16)) {
+      if (side >= 0 && p.xghost_ptr[side]) {
         ph[j] = p.xghost_ptr[side] + (long long)(y + j) * p.xghost_pitch[side] + (long long)z0 * (long long)sizeof(T);
         phstep = (long long)sizeof(T);
       }
@@ -177,8 +177,8 @@ __device__ __forceinline__ void march_body(const JacobiParams &p, const int bx, 
   // asked for the rows above and below: two memory latencies per step, the x-face tiles of FP32 512^3 ran at half speed.)
   // Every lane loads a scalar (its own first element where nothing is patched): no divergent branch around a load.
   int wrap_i = -1;
-  const bool xpatch = EDGE && SHIFT && p.xwrap && !(debug & 131072); // kernel-uniform (131072: experiment, no patch at all)
-  const char *wrap_p = xpatch ? pc[0] : nullptr; // the scalar of plane z+1
+  const bool xpatch = EDGE && SHIFT && p.xwrap; // kernel-uniform
+  const char *wrap_p = pc[0]; // the scalar of plane z+1
   if (xpatch) {
 #pragma unroll
     for (int i = 0; i < VX; ++i) {
@@ -186,7 +186,6 @@ __device__ __forceinline__ void march_body(const JacobiParams &p, const int bx, 
       const int xw = xi == p.lo[0] - 1 ? p.hi[0] - 1 : (xi == p.hi[0] ? p.lo[0] : -1);
       if (xw >= 0) wrap_i = i, wrap_p = src + (long long)(z0 + 1) * S + yo(y) + (long long)xw * (long long)sizeof(T);
     }
-    if (debug & 65536) wrap_p = pc[0]; // experiment: the patch scalar from the lane's own vector (wrong halos)
   }
   T wA = T(0), wB = T(0), wC = T(0); // the scalar that belongs into each register plane's vector (loaded with it; no copies:
                                      // a copy right behind the load would make the warp wait for it)
@@ -227,7 +226,6 @@ __device__ __forceinline__ void march_body(const JacobiParams &p, const int bx, 
       if (x + i == p.lo[0] && p.push_ptr[0]) xsi = i, xsp = xstage_row<T>(0, warp);
       if (x + i == p.hi[0] - 1 && p.push_ptr[1]) xsi = i, xsp = xstage_row<T>(1, warp);
     }
-    if (debug & 32) xsi = -1;
   }
   if (YP && sizeof(V) == 16 && row_ok[0]) {
     // (a tile on both y faces -- a subdomain of at most 8 rows -- parks the -y row; finish_tile copies the other one)
@@ -253,7 +251,8 @@ __device__ __forceinline__ void march_body(const JacobiParams &p, const int bx, 
   // loop): also store the result into the z neighbours named by zmask (bit 0: -z, bit 1: +z).
   auto step = [&](auto zp_tag, const unsigned zmask, const V(&prev)[RY], const V(&cur)[RY], V(&nxt)[RY], const T &wcur, T &wnext) {
     constexpr bool ZP = decltype(zp_tag)::value;
-    if (xpatch && wrap_i >= 0) wnext = *reinterpret_cast<const T *>(wrap_p);
+    if (EDGE && SHIFT && wrap_i >= 0) wnext = *reinterpret_cast<const T *>(wrap_p); // (wrap_i >= 0 only with xpatch;
+                                                                                   // testing xpatch too made ptxas spill in the FP32 x-face loop)
 #pragma unroll
     for (int j = 0; j < RY; ++j) nxt[j] = *reinterpret_cast<const V *>(pc[j]);
     if (EDGE && SHIFT) wrap_p += S;
@@ -425,12 +424,16 @@ __device__ __forceinline__ void march_body(const JacobiParams &p, const int bx, 
   }
 }
 
-template <typename T, int VX, int RY, int MB, bool SHIFT>
-__global__ void __launch_bounds__(256, MB) jacobi_march_kernel(const __grid_constant__ JacobiParams p, int tiles_x, int tiles_y) {
+// Rows per warp and minimum CTAs per SM of the march kernel: fewer rows -> fewer registers -> more warps in flight.
+constexpr int kMarchRows = 1;
+constexpr int kMarchCtasPerSm = 4;
+
+template <typename T, int VX, bool SHIFT>
+__global__ void __launch_bounds__(256, kMarchCtasPerSm) jacobi_march_kernel(const __grid_constant__ JacobiParams p, int tiles_x, int tiles_y) {
   int b = blockIdx.x;
   const int bx = b % tiles_x;
   b /= tiles_x;
-  march_body<T, VX, RY, SHIFT, 0>(p, bx, b % tiles_y, b / tiles_y);
+  march_body<T, VX, kMarchRows, SHIFT, 0>(p, bx, b % tiles_y, b / tiles_y);
 }
 
 // The tail column of phase-shifted rows (fused kernel).  FP32 rows of 514 floats alternate between two 16-byte phases, so
@@ -599,7 +602,6 @@ __device__ __forceinline__ void fused_body(const JacobiParams &p, const FusedSyn
   if (by == ny - 1) touch |= 8u;
   if (bz == 0) touch |= 16u;
   if (bz == nz - 1) touch |= 32u;
-  if (s.debug & 64) touch &= (unsigned)(s.debug >> 8); // experiment: only tiles on the faces in bits 8.. run a boundary variant (wrong halos)
   if (!touch) { // CTAs that touch no face take the plain loop
     march_body<T, VX, 1, SHIFT, 0>(p, bx, by, bz);
     return;
@@ -636,9 +638,9 @@ __device__ __forceinline__ void fused_body(const JacobiParams &p, const FusedSyn
   if (needy)
     march_body<T, VX, 1, SHIFT, 7>(p, bx, by, bz, waits);
   else if (needx)
-    march_body<T, VX, 1, SHIFT, 3>(p, bx, by, bz, waits, s.debug);
+    march_body<T, VX, 1, SHIFT, 3>(p, bx, by, bz, waits);
   else
-    march_body<T, VX, 1, SHIFT, 1>(p, bx, by, bz, waits, s.debug);
+    march_body<T, VX, 1, SHIFT, 1>(p, bx, by, bz, waits);
   if (EDGE >= 2) finish_tile<T, VX, SHIFT>(p, s, nx, ny, nz);
 }
 
@@ -908,8 +910,6 @@ __global__ void __launch_bounds__(256) sqdiff_kernel(const char *a, const char *
   }
 }
 
-int env_int(const char *name, int dflt);
-
 template <typename T, int VX, bool SHIFT> int launch_fused(const JacobiParams &p, FusedSync s, cudaStream_t stream) {
   const int x0a = p.x0a;
   int tiles_x = (p.hi[0] - x0a + (SHIFT ? VX / 2 : 0) + 32 * VX - 1) / (32 * VX);
@@ -921,7 +921,7 @@ template <typename T, int VX, bool SHIFT> int launch_fused(const JacobiParams &p
   // vector becomes tail-column tiles (march_column), the strips before it the main grid.  Not when the +x face is pushed:
   // its cells would have to be parked by the column tiles.
   s.col_cy = s.col_x = 0;
-  if (SHIFT && tiles_x >= 2 && !p.push_ptr[1] && env_int("SB_JACOBI_COLUMN", 1)) {
+  if (SHIFT && tiles_x >= 2 && !p.push_ptr[1]) {
     const int xcol = x0a + (tiles_x - 1) * 32 * VX; // first cell of the last strip on rows of phase 0
     if (p.hi[0] - (xcol - VX / 2) <= VX && xcol - VX / 2 >= p.lo[0]) {
       s.col_cy = (ny + 255) / 256;
@@ -930,7 +930,6 @@ template <typename T, int VX, bool SHIFT> int launch_fused(const JacobiParams &p
     }
   }
   const long long blocks = (long long)tiles_x * tiles_y * tiles_z + (long long)s.col_cy * tiles_z;
-  s.xrot = s.yrot = s.zrot = 0;
   s.any_wait = s.any_signal = 0;
   for (int f = 0; f < 6; ++f) {
     if (s.wait_row[f]) s.any_wait = 1;
@@ -943,11 +942,9 @@ template <typename T, int VX, bool SHIFT> int launch_fused(const JacobiParams &p
   // ones (pushes after the march, three extra plane loads in the top chunk), so the walk should not end with them, and z
   // starts in the middle, which keeps the z-face tiles out of the first wave, where every boundary tile waits for the
   // neighbour rank's kernel to start.  (Measured on and off, one and two ranks: within the run-to-run noise.)
-  if (env_int("SB_FUSED_ROTATE", 1)) {
-    s.xrot = tiles_x - 1;
-    s.yrot = tiles_y - 1;
-    s.zrot = tiles_z / 2;
-  }
+  s.xrot = tiles_x - 1;
+  s.yrot = tiles_y - 1;
+  s.zrot = tiles_z / 2;
   if (!any_push && !dense_ghosts) // every face is a periodic self-neighbour read in place (one GPU)
     jacobi_fused_kernel<T, VX, SHIFT, 1><<<(unsigned)blocks, 256, 0, stream>>>(p, s, tiles_x, tiles_y, tiles_z);
   else
@@ -955,53 +952,22 @@ template <typename T, int VX, bool SHIFT> int launch_fused(const JacobiParams &p
   return 1;
 }
 
-template <typename T, int VX, bool SHIFT> int launch_march(const JacobiParams &p, int ry, int mb, cudaStream_t stream) {
+template <typename T, int VX, bool SHIFT> int launch_march(const JacobiParams &p, cudaStream_t stream) {
   const int x0a = p.x0a;
   // a shifted row starts VX/2 cells early, so the last tile must reach VX/2 cells further
   const int tiles_x = (p.hi[0] - x0a + (SHIFT ? VX / 2 : 0) + 32 * VX - 1) / (32 * VX);
   const int ny = p.hi[1] - p.lo[1], nz = p.hi[2] - p.lo[2];
   const int tiles_z = (nz + p.zchunk - 1) / p.zchunk;
-  auto go = [&](auto kern, int RY) {
-    const int tiles_y = (ny + 8 * RY - 1) / (8 * RY);
-    const long long blocks = (long long)tiles_x * tiles_y * tiles_z;
-    kern<<<(unsigned)blocks, 256, 0, stream>>>(p, tiles_x, tiles_y);
-  };
-  // (rows per warp, min CTAs/SM): fewer rows -> fewer registers -> more warps in flight
-  if (SHIFT) {
-    if (mb == 5)
-      go(jacobi_march_kernel<T, VX, 1, 5, SHIFT>, 1);
-    else
-      go(jacobi_march_kernel<T, VX, 1, 4, SHIFT>, 1);
-    return 1;
-  }
-  const int key = ry * 10 + mb;
-  switch (key) {
-  case 14:
-    go(jacobi_march_kernel<T, VX, 1, 4, false>, 1);
-    break;
-  case 15:
-    go(jacobi_march_kernel<T, VX, 1, 5, false>, 1);
-    break;
-  case 16:
-    go(jacobi_march_kernel<T, VX, 1, 6, false>, 1);
-    break;
-  case 24:
-    go(jacobi_march_kernel<T, VX, 2, 4, false>, 2);
-    break;
-  case 42:
-    go(jacobi_march_kernel<T, VX, 4, 2, false>, 4);
-    break;
-  default:
-    go(jacobi_march_kernel<T, VX, 2, 3, false>, 2);
-    break;
-  }
+  const int tiles_y = (ny + 8 * kMarchRows - 1) / (8 * kMarchRows);
+  const long long blocks = (long long)tiles_x * tiles_y * tiles_z;
+  jacobi_march_kernel<T, VX, SHIFT><<<(unsigned)blocks, 256, 0, stream>>>(p, tiles_x, tiles_y);
   return 1;
 }
 
-int env_int(const char *name, int dflt) {
-  const char *s = getenv(name);
-  return (s && *s) ? atoi(s) : dflt;
-}
+// regions narrower than this in x take the one-thread-per-cell kernel
+constexpr int kThinX = 16;
+// grid cap of the exterior-slab kernel
+constexpr int kRegionsCtasPerSm = 32;
 
 // SMs of the current device: the grid-stride kernels below cap their grids at a few CTAs per SM
 long long sm_count() {
@@ -1017,8 +983,7 @@ int launch_jacobi_regions(const JacobiParams &p, const JacobiRegions &r, int dty
   const long long total = r.first[r.n];
   if (r.n <= 0 || total <= 0) return 0;
   long long blocks = (total + 255) / 256;
-  static const int per_sm = env_int("SB_JACOBI_EXT_CTAS_PER_SM", 32);
-  if (blocks > sm_count() * per_sm) blocks = sm_count() * per_sm;
+  if (blocks > sm_count() * kRegionsCtasPerSm) blocks = sm_count() * kRegionsCtasPerSm;
   if (dtype_size == 4)
     jacobi_regions_kernel<float><<<(unsigned)blocks, 256, 0, stream>>>(p, r);
   else
@@ -1026,20 +991,14 @@ int launch_jacobi_regions(const JacobiParams &p, const JacobiRegions &r, int dty
   return 1;
 }
 
-static int pick_vectors(JacobiParams &p, int dtype_size, bool allow_shift, bool *shift);
+static int pick_vectors(JacobiParams &p, int dtype_size, bool *shift);
 
 int launch_jacobi(const JacobiParams &p_in, int dtype_size, cudaStream_t stream) {
   JacobiParams p = p_in;
   const int ex = p.hi[0] - p.lo[0], ey = p.hi[1] - p.lo[1], ez = p.hi[2] - p.lo[2];
   if (ex <= 0 || ey <= 0 || ez <= 0) return 0;
 
-  static const int ry = env_int("SB_JACOBI_RY", 1);
-  static const int mb = env_int("SB_JACOBI_MB", 4);
-  static const int zchunk_env = env_int("SB_JACOBI_ZCHUNK", 0);
-  static const int pf = env_int("SB_JACOBI_PREFETCH", 2);
-  static const int thin = env_int("SB_JACOBI_THIN_X", 16);
-
-  if (ex < thin) {
+  if (ex < kThinX) {
     const long long total = (long long)ex * ey * ez;
     long long blocks = (total + 255) / 256;
     if (blocks > sm_count() * 16) blocks = sm_count() * 16;
@@ -1050,25 +1009,20 @@ int launch_jacobi(const JacobiParams &p_in, int dtype_size, cudaStream_t stream)
     return 1;
   }
 
-  // z chunk: enough CTAs for several waves of 4 resident CTAs per SM, but chunks no shorter than 16 planes
-  if (zchunk_env > 0) {
-    p.zchunk = zchunk_env;
-  } else if (p.zchunk <= 0) {
-    p.zchunk = 32;
-  }
+  // z chunk: the caller's, else 32 planes
+  if (p.zchunk <= 0) p.zchunk = 32;
   if (p.zchunk > ez) p.zchunk = ez;
-  p.prefetch = pf;
+  p.prefetch = 2;
 
-  static const int allow_shift = env_int("SB_JACOBI_SHIFT", 1);
   bool shift = false;
-  const int vx = pick_vectors(p, dtype_size, allow_shift != 0, &shift);
+  const int vx = pick_vectors(p, dtype_size, &shift);
   if (dtype_size == 8) {
-    if (vx == 2) return shift ? launch_march<double, 2, true>(p, ry, mb, stream) : launch_march<double, 2, false>(p, ry, mb, stream);
-    return launch_march<double, 1, false>(p, ry, mb, stream);
+    if (vx == 2) return shift ? launch_march<double, 2, true>(p, stream) : launch_march<double, 2, false>(p, stream);
+    return launch_march<double, 1, false>(p, stream);
   }
-  if (vx == 4) return shift ? launch_march<float, 4, true>(p, ry, mb, stream) : launch_march<float, 4, false>(p, ry, mb, stream);
-  if (vx == 2) return launch_march<float, 2, false>(p, ry, mb, stream);
-  return launch_march<float, 1, false>(p, ry, mb, stream);
+  if (vx == 4) return shift ? launch_march<float, 4, true>(p, stream) : launch_march<float, 4, false>(p, stream);
+  if (vx == 2) return launch_march<float, 2, false>(p, stream);
+  return launch_march<float, 1, false>(p, stream);
 }
 
 // Vector width and strip origin for a launch.  Rows whose pitch and slice are multiples of 16 bytes all have the phase
@@ -1079,7 +1033,7 @@ int launch_jacobi(const JacobiParams &p_in, int dtype_size, cudaStream_t stream)
 // (march_body, xin), which would feed wrong values to those cells.  Such a region (e.g. 30 or 130 floats with one ghost
 // cell behind a 12-byte lead) takes the scalar path, in launch_jacobi and launch_jacobi_fused alike.  A vector that holds
 // only the ghost cell is handled in march_body (tail_lane), unless the lane before it is lane 0 of a strip (below).
-static int pick_vectors(JacobiParams &p, int dtype_size, bool allow_shift, bool *shift) {
+static int pick_vectors(JacobiParams &p, int dtype_size, bool *shift) {
   const unsigned long long s = (unsigned long long)(uintptr_t)p.src, d = (unsigned long long)(uintptr_t)p.dst;
   const int full = 16 / dtype_size;
   *shift = false;
@@ -1095,7 +1049,7 @@ static int pick_vectors(JacobiParams &p, int dtype_size, bool allow_shift, bool 
     // with a non-zero phase the first vector may start before x = 0: still inside the (256-byte aligned) allocation,
     // whose first `phase` bytes are the lead pad
     vx = origin(full, unsigned(s & 15));
-  } else if (allow_shift && (s & 15) == 0 && (d & 15) == 0 && p.slice % 16 == 0 && p.pitch % 16 == 8) {
+  } else if ((s & 15) == 0 && (d & 15) == 0 && p.slice % 16 == 0 && p.pitch % 16 == 8) {
     *shift = true;
     return origin(full, 0); // (shifted rows may hang over either end of a row: march_body xin)
   } else if (dtype_size == 4 && ((s | d | (unsigned long long)p.pitch | (unsigned long long)p.slice) % 8 == 0)) {
@@ -1111,35 +1065,21 @@ static int pick_vectors(JacobiParams &p, int dtype_size, bool allow_shift, bool 
   return vx;
 }
 
-int launch_jacobi_fused(const JacobiParams &p_in, const FusedSync &sync_in, int dtype_size, cudaStream_t stream) {
+int launch_jacobi_fused(const JacobiParams &p_in, const FusedSync &sync, int dtype_size, cudaStream_t stream) {
   JacobiParams p = p_in;
   const int ex = p.hi[0] - p.lo[0], ey = p.hi[1] - p.lo[1], ez = p.hi[2] - p.lo[2];
   if (ex <= 0 || ey <= 0 || ez <= 0) return 0;
-  const int zchunk_env = env_int("SB_JACOBI_ZCHUNK", 0);
   // H100 80GB HBM3 (400 W), 512^3 FP64, one GPU, 1-plane L2 prefetch: 8-plane chunks take 0.78 ms per iteration, 16-plane
   // chunks 0.80 ms, 32 planes with a 2-plane prefetch 0.88 ms; deeper prefetch is slower (DESIGN.md section 2.2)
-  const int pf = env_int("SB_JACOBI_PREFETCH", 1);
-  const int allow_shift = env_int("SB_JACOBI_SHIFT", 1);
-  p.prefetch = pf;
-  FusedSync sync = sync_in;
-  const int dbg = env_int("SB_DEBUG_FUSED", 0); // timing diagnostics only (results may be wrong): 1 no waits, 2 no signals
-  for (int f = 0; f < 6; ++f) {
-    if (dbg & 1) sync.wait_row[f] = nullptr;
-    if (dbg & 2) sync.signal_row[f] = nullptr;
-  }
-  sync.debug = dbg;
+  p.prefetch = 1;
   bool shift = false;
-  const int vx = pick_vectors(p, dtype_size, allow_shift != 0, &shift);
+  const int vx = pick_vectors(p, dtype_size, &shift);
   // z chunk (the x faces are staged at most 32 planes at a time): 8 planes by default, 16 or 32 where shorter chunks would
   // give a face more tiles than launch_fused's group limit (8: subdomains up to 512 cells in z at 512 cells in y; 16: up to
   // ~720 cells in y and z)
-  if (zchunk_env > 0 && zchunk_env <= 32) {
-    p.zchunk = zchunk_env;
-  } else {
-    const long long tiles_x = (p.hi[0] - p.x0a + (shift ? vx / 2 : 0) + 32 * vx - 1) / (32 * vx), tiles_y = (ey + 7) / 8;
-    const long long across = tiles_x > tiles_y ? tiles_x : tiles_y;
-    p.zchunk = ((ez + 7) / 8) * across <= kMaxGroups ? 8 : (((ez + 15) / 16) * across <= kMaxGroups ? 16 : 32);
-  }
+  const long long tiles_x = (p.hi[0] - p.x0a + (shift ? vx / 2 : 0) + 32 * vx - 1) / (32 * vx), tiles_y = (ey + 7) / 8;
+  const long long across = tiles_x > tiles_y ? tiles_x : tiles_y;
+  p.zchunk = ((ez + 7) / 8) * across <= kMaxGroups ? 8 : (((ez + 15) / 16) * across <= kMaxGroups ? 16 : 32);
   if (p.zchunk > ez) p.zchunk = ez;
   // x wrap (periodic self-neighbour read in place) works through the edge lanes' scalar load, so the first compute cell
   // must open lane 0 of the first strip and the last one must close lane 31 of the last strip; otherwise the ghost

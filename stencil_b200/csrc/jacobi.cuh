@@ -59,7 +59,6 @@ struct FusedSync {
   int xrot, yrot, zrot;    // set by the launcher: where the walk over the tiles starts on each axis
   int any_wait, any_signal; // set by the launcher
   int col_cy, col_x;        // set by the launcher: tail-column tiles of phase-shifted rows (march_column): CTAs per z chunk (0: none), first cell
-  int debug;                // timing experiments (SB_DEBUG_FUSED bits 16, 32; wrong results)
 };
 
 // Up to 8 thin regions (the exterior slabs of one subdomain) updated by ONE launch.

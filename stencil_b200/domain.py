@@ -646,7 +646,6 @@ class CopyPlan:
         self.device = device
         self.bytes = int(lib().sb_copy_plan_bytes(h))
         self.num_tiles = int(lib().sb_copy_plan_num_tiles(h))
-        self.num_tma_segments = int(lib().sb_copy_plan_num_tma_segments(h))
 
     def launch(self, stream=None) -> None:
         check(lib().sb_copy_plan_launch(self._h, stream_ptr(stream)))

@@ -40,13 +40,13 @@ def scaled_size(x: int, y: int, z: int, num_subdoms: int) -> Tuple[int, int, int
 FACE_DIRS = ((-1, 0, 0), (1, 0, 0), (0, -1, 0), (0, 1, 0), (0, 0, -1), (0, 0, 1))
 
 
-def fused_x_mode(part, owner, elem_size: int, radius: Radius, mode: str = "") -> str:
+def fused_x_mode(part, owner, elem_size: int, radius: Radius) -> str:
     """How the fused schedule moves x faces for a given partition / ownership (pure: every rank computes the same).
 
     "direct": no x face crosses ranks -- the kernel stores boundary cells into the neighbour's ghost cells (own memory or
               a peer GPU of this process) or reads a periodic self-neighbour in place;
     "dense":  x faces cross ranks and travel as 256-byte lines into dense receive arrays (kernel mode XPUSH): needs whole warp
-              strips along x and rows of one 16-byte phase (mode "0" = SB_FUSED_IPC=0 switches it off);
+              strips along x and rows of one 16-byte phase;
     "queued": fall back to the queued schedule (Jacobi3D.step_async)."""
     from .domain import get_neighbor
 
@@ -60,10 +60,10 @@ def fused_x_mode(part, owner, elem_size: int, radius: Radius, mode: str = "") ->
         part.subdomain_size(i)[0] % strip == 0 and ((part.subdomain_size(i)[0] + radius.x(-1) + radius.x(1)) * elem_size) % 16 == 0
         for i in part.indices()
     )
-    return "dense" if (layout and mode != "0") else "queued"
+    return "dense" if layout else "queued"
 
 
-def fused_schedule(dd, elem_size: int, mode: str = "") -> str:
+def fused_schedule(dd, elem_size: int) -> str:
     """Which schedule Jacobi3D.step_fused runs -- "fused" or "queued" -- as a pure function of the GLOBAL partition,
     radius and transport, so that every rank takes the same one (a rank on another schedule would wait on flags the
     others never write)."""
@@ -75,7 +75,7 @@ def fused_schedule(dd, elem_size: int, mode: str = "") -> str:
     part = dd.partition_
     if any(part.subdomain_size(i)[0] < 16 for i in part.indices()):
         return "queued"
-    return "queued" if fused_x_mode(part, dd._owner, elem_size, r, mode) == "queued" else "fused"
+    return "queued" if fused_x_mode(part, dd._owner, elem_size, r) == "queued" else "fused"
 
 
 class Jacobi3D:
@@ -122,10 +122,6 @@ class Jacobi3D:
         self._devs = [d.gpu() for d in dd.domains()]
         self._multi_dev = len(set(self._devs)) > 1
         self._set_device = torch.cuda.set_device
-        import os
-
-        dbg = os.environ.get("SB_DEBUG_SKIP", "")
-        self._debug_skip = {"both": ("ext", "xchg")}.get(dbg, (dbg,) if dbg else ())
         self._ghosts_current = False  # step_fused: do the ghost cells of curr hold the neighbours' current values?
         self._ev_ext = None  # step_async: exterior-done events of the previous iteration (one per subdomain)
         self._ev_int = None
@@ -194,7 +190,6 @@ class Jacobi3D:
         if getattr(self, "_ev_fused", None) is not None:
             self.synchronize()
             self._ev_fused = None
-        skip = self._debug_skip  # timing diagnostics only (SB_DEBUG_SKIP=ext|xchg|both): results are wrong when set
         nd = len(self._devs)
         prev_ext, prev_int = self._ev_ext, self._ev_int
         xs = dd.exchange_streams()
@@ -217,8 +212,7 @@ class Jacobi3D:
             for x in xs:
                 for e in prev_ext:
                     x.wait_event(e)
-        if "xchg" not in skip:
-            dd.exchange_async()
+        dd.exchange_async()
         ev_x = []
         for di, x in enumerate(xs):
             if self._multi_dev:
@@ -235,8 +229,7 @@ class Jacobi3D:
                 s.wait_event(e)
             if prev_int is not None:
                 s.wait_event(prev_int[di])
-            if "ext" not in skip:
-                check(self._fn_regions(*a[1]))
+            check(self._fn_regions(*a[1]))
             e = torch.cuda.Event()
             e.record(s)
             ev_ext.append(e)
@@ -249,8 +242,6 @@ class Jacobi3D:
         output allocations (own memory, a peer GPU of this process, or another rank's IPC mapping), the dense x arrays and
         the mailboxes of the in-kernel handshake.  Returns False (on every rank alike) if the fused schedule does not
         apply after all."""
-        import os
-
         from . import dist as _dist
         from ._lib import FUSED_MAX_GROUPS, StepSync
         from .domain import CopyPlan, box_copy, get_neighbor
@@ -278,7 +269,7 @@ class Jacobi3D:
         layout = all(part.subdomain_size(i)[0] % strip == 0 and ((part.subdomain_size(i)[0] + r.x(-1) + r.x(1)) * es) % 16 == 0 for i in part.indices())
         aligned = all((d.pitched(h.id, w).ptr + r.x(-1) * es) % 16 == 0 for d in dd.domains() for w in ("curr", "next"))
         dense = layout and all(gather(bool(aligned)))
-        x_crosses_ranks = fused_x_mode(part, dd._owner, es, r, os.environ.get("SB_FUSED_IPC", "")) != "direct"
+        x_crosses_ranks = fused_x_mode(part, dd._owner, es, r) != "direct"
         if x_crosses_ranks and not dense:
             return False
 
@@ -311,7 +302,7 @@ class Jacobi3D:
                     if nidx != idx:
                         recv[(idx, side)] = [dev_alloc(raw[1] * raw[2] * es, d.gpu()) for _ in range(2)]
         # mailboxes of the in-kernel handshake: one subdomain per rank (the torchrun layout) with neighbours on other ranks
-        inkernel = multi_rank and len(dd.domains()) == 1 and os.environ.get("SB_FUSED_INKERNEL", "1") != "0"
+        inkernel = multi_rank and len(dd.domains()) == 1
         mailbox = dev_alloc(6 * FUSED_MAX_GROUPS * 4, dd.domains()[0].gpu()) if inkernel else 0
         for _, gpu in self._xbuf:
             check(L.sb_device_sync(gpu))
@@ -380,8 +371,6 @@ class Jacobi3D:
                         for zz in range(lo3[2], lo3[2] + sz3[2]):
                             col = Pitched(target[rel] + zz * es, myraw[2] * es, myraw[1])  # element (0, y, 0) -> [y][zz]
                             init_copies.append(box_copy(col, (0, lo3[1], 0), src, (xcol, lo3[1], zz), (1, sz3[1], 1), es))
-                    if os.environ.get("SB_DEBUG_NOPUSH"):  # timing diagnostics only: results are wrong
-                        push.nbr[k] = Pitched(None, 0, 0)
                 creg = d.get_compute_region()
                 clo, chi = i3(self.creg[0]), i3(self.creg[1])
                 pack = (dst, src, d.elem_size(h.id), i3(d.accessor_origin()), i3(creg[0]), i3(creg[1]), clo, chi, push, stream_ptr(self.streams[di]))
@@ -423,12 +412,10 @@ class Jacobi3D:
         import torch
 
         if not hasattr(self, "_fused_calls"):
-            import os
-
             es = self.dd.domains()[0].elem_size(self.h.id)
             self._fused_calls = []
             # a pure function of the global partition; _build_fused adds one all-gathered layout check (the same everywhere)
-            self.fused_supported = fused_schedule(self.dd, es, os.environ.get("SB_FUSED_IPC", "")) == "fused" and self._build_fused()
+            self.fused_supported = fused_schedule(self.dd, es) == "fused" and self._build_fused()
         if not self.fused_supported:  # the queued schedule computes the same iteration
             return self.step_async(timing=timing)
         dd = self.dd
@@ -439,7 +426,7 @@ class Jacobi3D:
             self.synchronize()
             dd.exchange()  # ghost cells of curr, once; afterwards every iteration leaves them filled for the next
             rel0 = (dd._parity - self._parity0) & 1
-            for di, plan in enumerate(self._init_plans[rel0]):  # dense x columns for neighbour ranks (SB_FUSED_IPC=1)
+            for di, plan in enumerate(self._init_plans[rel0]):  # dense x columns for neighbour ranks
                 if plan is not None:
                     plan.launch(self.streams[di])
             self.synchronize()

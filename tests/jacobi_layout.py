@@ -18,11 +18,11 @@ from dataclasses import dataclass, field
 from typing import Dict, List, Optional, Tuple
 
 MAX_GROUPS = 4096  # SB_FUSED_MAX_GROUPS
-THIN_X = 16  # launch_jacobi: regions narrower than this take jacobi_cell_kernel (SB_JACOBI_THIN_X)
+THIN_X = 16  # launch_jacobi: regions narrower than this take jacobi_cell_kernel (kThinX)
 FACES = ("-x", "+x", "-y", "+y", "-z", "+z")
 
 
-def pick_vectors(s_lead: int, d_lead: int, pitch: int, slice_: int, es: int, lo0: int, hi0: int, raw0: int, allow_shift: bool = True):
+def pick_vectors(s_lead: int, d_lead: int, pitch: int, slice_: int, es: int, lo0: int, hi0: int, raw0: int):
     """jacobi.cu pick_vectors -> (vx, x0a, kind).  kind: "phase0" / "phase" (full 16-byte vectors, rows of one phase, equal
     src and dst phase 0 / not 0), "shift" (full vectors on rows alternating between two phases), "pairs" (FP32 8-byte pairs),
     "scalar", "overhang" (unshifted vectors where the last one holding compute cells would hang over the end of its row:
@@ -38,7 +38,7 @@ def pick_vectors(s_lead: int, d_lead: int, pitch: int, slice_: int, es: int, lo0
 
     if pitch % 16 == 0 and slice_ % 16 == 0 and s == d and s % es == 0:
         vx, x0a, kind = full, origin(full, s), ("phase0" if s == 0 else "phase")
-    elif allow_shift and s == 0 and d == 0 and slice_ % 16 == 0 and pitch % 16 == 8:
+    elif s == 0 and d == 0 and slice_ % 16 == 0 and pitch % 16 == 8:
         return full, origin(full, 0), "shift"
     elif es == 4 and (s_lead | d_lead | pitch | slice_) % 8 == 0:
         vx, x0a, kind = 2, origin(2, 0), "pairs"

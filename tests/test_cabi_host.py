@@ -40,7 +40,7 @@ def test_library_exports_every_declared_symbol():
         assert hasattr(L, name), name
     # and the ctypes table covers exactly the header
     assert declared == set(_lib._SIGS), declared ^ set(_lib._SIGS)
-    assert sb.lib().sb_version() == 1
+    assert sb.lib().sb_version() == 2
 
 
 def test_missing_library_fails_loudly(monkeypatch):
@@ -139,18 +139,16 @@ def test_fused_schedule_choice_per_partition():
     assert tuple(two.dim) == (2, 1, 1)
     assert fused_x_mode(two, owners(two, 2), 8, r) == "direct"  # one process x 2 GPUs: peer access
     assert fused_x_mode(two, owners(two, 1), 8, r) == "dense"  # torchrun, 2 ranks
-    assert fused_x_mode(two, owners(two, 1), 8, r, "0") == "queued"
     four = Partition((1024, 1024, 512), r, 1, 4)
     assert tuple(four.dim) == (2, 2, 1) and fused_x_mode(four, owners(four, 1), 8, r) == "dense"
     eight = Partition((1024, 1024, 1024), r, 1, 8)
     assert tuple(eight.dim) == (2, 2, 2)
     assert fused_x_mode(eight, owners(eight, 1), 8, r) == "dense"
-    assert fused_x_mode(eight, owners(eight, 1), 8, r, "0") == "queued"
     # 48 cells along x per rank are not whole warp strips (64 FP64 cells): never dense
     small = Partition((96, 48, 48), r, 1, 2)
-    assert fused_x_mode(small, owners(small, 1), 8, r, "1") == "queued"
+    assert fused_x_mode(small, owners(small, 1), 8, r) == "queued"
     # FP32: strips of 128 cells, and 514-float rows alternate between two 16-byte phases
-    assert fused_x_mode(two, owners(two, 1), 4, r, "1") == "queued"
+    assert fused_x_mode(two, owners(two, 1), 4, r) == "queued"
     # bench.py's default shapes grow along y and z only: x never crosses ranks, either precision runs the fused schedule
     for size, n, dim in (((512, 512, 1024), 2, (1, 1, 2)), ((512, 1024, 1024), 4, (1, 2, 2)), ((512, 1024, 2048), 8, (1, 2, 4))):
         part = Partition(size, r, 1, n)

@@ -76,18 +76,27 @@ def test_substeps_match_oracle(dtype, variant, box):
     run_substeps(fields, ref, lo, hi, ac.conf_params(dt=1e-3), variant)
 
 
-@pytest.mark.parametrize("variant", [ac.CELL, ac.TILE, ac.TEAM, ac.TEAM_TMA, ac.TEAM3_TMA])
-@pytest.mark.parametrize("shape", [0, 1])
-def test_tile_shapes_and_zchunks(variant, shape, monkeypatch):
-    """Both tile shapes per precision (SB_AC_SHAPE) and a forced short z chunk (ring warm-up at every chunk start)."""
-    monkeypatch.setenv("SB_AC_SHAPE", str(shape))
-    monkeypatch.setenv("SB_AC_ZCHUNK", "5")
-    for dtype in (np.float64, np.float32):
-        if variant in (ac.TEAM_TMA, ac.TEAM3_TMA) and dtype == np.float32:
-            continue
-        raw, lo, hi = (50, 45, 29), (3, 3, 3), (47, 42, 26)
-        fields, ref = cached_reference(raw, lo, hi, 11, np.dtype(dtype).name, "conf")
-        run_substeps(fields, ref, lo, hi, ac.conf_params(dt=1e-3), variant)
+# every variant that applies to the precision, at the allocation lead LocalDomain gives it (FP64 8 bytes, FP32 4) and at 0
+CHUNK_CASES = [(dt, lead, v) for dt, leads, vs in ((np.float64, (0, 8), (ac.CELL, ac.TILE, ac.TEAM, ac.TEAM_TMA, ac.TEAM3_TMA)),
+                                                  (np.float32, (0, 4), (ac.CELL, ac.TILE, ac.TEAM)))
+               for lead in leads for v in vs]
+VARIANT_NAMES = {ac.CELL: "cell", ac.TILE: "tile", ac.TEAM: "team", ac.TEAM_TMA: "team_tma", ac.TEAM3_TMA: "team3_tma"}
+
+
+@pytest.mark.parametrize("dtype,lead,variant", CHUNK_CASES, ids=[f"{np.dtype(d).name}-lead{l}-{VARIANT_NAMES[v]}" for d, l, v in CHUNK_CASES])
+def test_tile_shapes_and_zchunks(dtype, lead, variant):
+    """A 44 x 39 x 23 compute box cut into many short z chunks (ring warm-up at every chunk start, a partial last chunk).
+    The launchers pick the chunk length that minimises (waves of CTAs) x (chunk cost) for one CTA per SM; with 132 SMs
+    (H100 SXM) that is:
+      tile kernel, FP64 16 x 14 tiles: 3 x 3 CTAs per chunk, cost len + 7  -> 2 planes (12 chunks, 108 CTAs, one wave)
+      tile kernel, FP32 32 x 8 tiles:  2 x 5 CTAs per chunk, cost len + 7  -> 2 planes (12 chunks, 120 CTAs)
+      team kernel, FP64 16 x 12:       3 x 4 CTAs per chunk, cost len + 4  -> 3 planes (8 chunks, 96 CTAs; 2 planes
+                                                                              would take two waves)
+      team kernel, FP32 32 x 8:        2 x 5 CTAs per chunk, cost len + 4  -> 2 planes (12 chunks)
+      TMA team kernels, 16 x 12 / 16 x 10 (FP64): 3 x 4 CTAs, cost len + 3  -> 3 planes (8 chunks)."""
+    raw, lo, hi = (50, 45, 29), (3, 3, 3), (47, 42, 26)
+    fields, ref = cached_reference(raw, lo, hi, 11, np.dtype(dtype).name, "conf")
+    run_substeps(fields, ref, lo, hi, ac.conf_params(dt=1e-3), variant, lead=lead)
 
 
 @pytest.mark.skipif(not os.path.exists(GOLDEN), reason="golden vectors not generated yet (oracle/ref/make_astaroth_golden.py)")

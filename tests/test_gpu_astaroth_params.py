@@ -1,5 +1,5 @@
-"""The astaroth solve<step> kernels with parameters that cannot stand in for one another, on non-cubic boxes, at
-shifted allocations and with the unpaced kernel instantiations.
+"""The astaroth solve<step> kernels with parameters that cannot stand in for one another, on non-cubic boxes and at
+shifted allocations.
 
 The conf parameter set has inv_dsx == inv_dsy == inv_dsz, nu_visc == eta and cs2_sound == cp_sound == 1: a kernel that
 swaps two of those or drops a 1 / cp computes the same numbers there.  Here the distinct set (stencil_b200.astaroth.
@@ -7,8 +7,6 @@ distinct_params, anisotropic spacing) is used, and every result is compared with
 rounding budget of astaroth_util, which is tight enough that such a mistake fails at FP32 as well as FP64
 (tests/test_oracle_astaroth.py::test_distinct_params_discriminate)."""
 import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -79,32 +77,6 @@ def test_tma_not_applicable(lead):
         fields, ref = cached_reference(raw, lo, hi, 7, np.dtype(dtype).name, "distinct")
         for variant in (ac.AUTO, ac.TEAM):
             run_substeps(fields, ref, lo, hi, ac.distinct_params(1e-3), variant, lead=lead)
-
-
-UNPACED = """
-import os, sys
-import numpy as np
-from astaroth_util import cached_reference
-from stencil_b200 import astaroth as ac
-from test_gpu_astaroth import run_substeps
-raw, lo, hi = (44, 27, 33), (3, 3, 3), (41, 24, 30)
-for dtype, variant, tma in ((np.float64, ac.TEAM, "0"), (np.float32, ac.TEAM, "1"), (np.float64, ac.TEAM_TMA, "1"),
-                            (np.float64, ac.TEAM3_TMA, "1"), (np.float64, ac.TEAM, "1")):
-    os.environ["SB_AC_TMA"] = tma
-    fields, ref = cached_reference(raw, lo, hi, 7, np.dtype(dtype).name, "distinct")
-    run_substeps(fields, ref, lo, hi, ac.distinct_params(1e-3), variant, lead=8 if dtype == np.float64 else 0)
-print("unpaced ok")
-"""
-
-
-def test_unpaced_kernels():
-    """SB_AC_PACE=0 selects the team kernels without the scheduling fences between pencils (PACED = false).  The value
-    is read once per process, so the cp.async-fed team kernel (FP64 and FP32) and both TMA-fed ones run in a fresh
-    interpreter."""
-    here = os.path.dirname(os.path.abspath(__file__))
-    env = dict(os.environ, SB_AC_PACE="0", PYTHONPATH=os.pathsep.join([here, os.path.dirname(here), os.environ.get("PYTHONPATH", "")]))
-    r = subprocess.run([sys.executable, "-c", UNPACED], cwd=here, env=env, capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0 and "unpaced ok" in r.stdout, r.stdout[-3000:] + r.stderr[-3000:]
 
 
 @pytest.mark.parametrize("dtype", [np.float64, np.float32])

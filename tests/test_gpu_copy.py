@@ -196,50 +196,3 @@ def test_full_size_face_roundtrip_512():
         ext = g.halo_extent(g.neg(d), (n, n, n), ro)
         got = dev_pack(src, pos, ext).get().reshape(-1)
         assert np.array_equal(got, no.pack(a, pos, ext)), d
-
-
-@pytest.mark.parametrize("dtype,n,r", [(np.float64, 124, 2), (np.float32, 248, 4), (np.float64, 508, 2), (np.float64, 64, 1), (np.float64, 510, 1), (np.float32, 252, 2), (np.float64, 126, 3)])
-def test_tma_path_is_taken_and_exact(dtype, n, r, monkeypatch):
-    """Wide rows with 16-byte aligned bases/strides are moved by the TMA tile kind (cp.async.bulk.tensor load +
-    store through a shared-memory ring).  Halo regions of every wide class (y face, z face, yz edge) + pack +
-    unpack, byte-compared with the oracle; the plan must report TMA segments.  The path is opt-in (SB_TMA=1): it is slower than the LSU path for halo-sized
-    messages, but it stays parity-tested."""
-    monkeypatch.setenv("SB_TMA", "1")  # opt-in path: slower than the LSU path for halo-sized messages
-    ro = g.Radius.constant(r)
-    sz = (n, n, n)
-    raw = g.raw_size(sz, ro)
-    es = np.dtype(dtype).itemsize
-    assert (raw[0] * es) % 16 == 0, "test shape must be TMA-legal"
-    rng = np.random.default_rng(23)
-    a = rng.integers(0, 1 << 20, size=raw[::-1]).astype(dtype)
-    src, dst = DevArray(a), DevArray(np.zeros_like(a))
-    want = np.zeros_like(a)
-    copies = []
-    for d in [(0, 1, 0), (0, -1, 0), (0, 0, 1), (0, 0, -1), (0, 1, 1), (0, -1, 1)]:
-        spos, ext = g.halo_pos(d, sz, ro, False), g.halo_extent(g.neg(d), sz, ro)
-        dpos = g.halo_pos(g.neg(d), sz, ro, True)
-        copies.append(sb.box_copy(dst.pitched(), dpos, src.pitched(), spos, ext, es))
-        no.translate(want, dpos, a, spos, ext)
-    plan = sb.CopyPlan(0, copies)
-    # TMA boxes must START on a 16-byte boundary (measured, scripts/exp/tma_probe3.cu).  When r * es is a multiple
-    # of 16 (r=2 FP64, r=4 FP32) the rows are moved by TMA load + TMA store (kind 1); otherwise (r=1 FP64) by an
-    # aligned-down TMA load + vector stores (kind 2).  Either way every wide copy of this plan is a TMA segment.
-    assert plan.num_tma_segments == len(copies)
-    plan.launch()
-    plan.launch()  # idempotent, and exercises the mbarrier phase bookkeeping across launches
-    assert np.array_equal(dst.get(), want)
-    # pack into / unpack from a dense buffer through TMA as well
-    d = (0, 0, 1)
-    spos, ext = g.halo_pos(d, sz, ro, False), g.halo_extent(g.neg(d), sz, ro)
-    nel = ext[0] * ext[1] * ext[2]
-    buf = DevArray(np.zeros((1, 1, nel), dtype=dtype))
-    dense = Pitched(buf.ptr, ext[0] * es, ext[1])
-    p1 = sb.CopyPlan(0, [sb.box_copy(dense, (0, 0, 0), src.pitched(), spos, ext, es)])
-    p1.launch()
-    assert np.array_equal(buf.get().reshape(-1), no.pack(a, spos, ext))
-    dst2 = DevArray(np.zeros_like(a))
-    p2 = sb.CopyPlan(0, [sb.box_copy(dst2.pitched(), spos, dense, (0, 0, 0), ext, es)])
-    p2.launch()
-    want2 = np.zeros_like(a)
-    no.unpack(want2, no.pack(a, spos, ext), spos, ext)
-    assert np.array_equal(dst2.get(), want2)

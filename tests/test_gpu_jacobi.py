@@ -241,40 +241,41 @@ def test_step_async_is_bitwise_step(dtype, ndom):
     assert float(np.ptp(fields[0][0])) > 0  # the hot/cold spheres made the field non-trivial
 
 
-@pytest.mark.parametrize("rotate", [0, 1])
+TILE_WALK_SHAPES = [((40, 24, 70), 1), ((200, 20, 40), 1), ((256, 40, 100), 1), ((384, 30, 66), 2), ((130, 17, 33), 1), ((64, 40, 65), 2), ((128, 7, 1), 1),
+                    ((128, 300, 40), 2), ((129, 40, 300), 2), ((256, 600, 9), 2),  # FP32: tail-column tiles that push y / z faces
+                    ((64, 768, 768), 1), ((64, 768, 1536), 2)]
+
+
+@pytest.mark.parametrize("size,ndom", TILE_WALK_SHAPES, ids=[f"{'x'.join(map(str, s))}-{n}" for s, n in TILE_WALK_SHAPES])
 @pytest.mark.parametrize("dtype", [np.float32, np.float64])
-def test_fused_kernel_tile_walks(monkeypatch, rotate, dtype):
-    """jacobi_fused_kernel walks its tiles from a rotated origin on every axis (SB_FUSED_ROTATE, default on) so that the
-    walk does not end with tiles that push; inner tiles take the plain loop, boundary tiles the variant their faces need.
-    Either walk, on shapes with 1..N tiles per axis (also fewer than the two boundary tiles, partial tiles, one-plane
-    chunks, and subdomains 768 cells tall in y and z, whose 16-plane chunks would exceed the face-group limit), must
-    reproduce Jacobi3D.step bit for bit."""
+def test_fused_kernel_tile_walks(dtype, size, ndom):
+    """jacobi_fused_kernel walks its tiles from a rotated origin on every axis so that the walk does not end with tiles
+    that push; inner tiles take the plain loop, boundary tiles the variant their faces need.  The walk, on shapes with
+    1..N tiles per axis (also fewer than the two boundary tiles, partial tiles, one-plane chunks, and subdomains 768
+    cells tall in y and z, whose 16-plane chunks would exceed the face-group limit), must reproduce Jacobi3D.step bit
+    for bit."""
     from stencil_b200.jacobi import Jacobi3D, jacobi_radius
 
-    monkeypatch.setenv("SB_FUSED_ROTATE", str(rotate))
-    for size, ndom in [((40, 24, 70), 1), ((200, 20, 40), 1), ((256, 40, 100), 1), ((384, 30, 66), 2), ((130, 17, 33), 1), ((64, 40, 65), 2), ((128, 7, 1), 1),
-                       ((128, 300, 40), 2), ((129, 40, 300), 2), ((256, 600, 9), 2),  # FP32: tail-column tiles that push y / z faces
-                       ((64, 768, 768), 1), ((64, 768, 1536), 2)]:
-        fields = []
-        for mode in ("sync", "fused"):
-            dd = sb.DistributedDomain(*size)
-            dd.set_gpus([0] * ndom)
-            dd.set_radius(jacobi_radius())
-            h = dd.add_data(dtype, "d")
-            dd.realize()
-            try:
-                jac = Jacobi3D(dd, h)
-                jac.init(0.5)
-                for it in range(7):
-                    jac.step() if mode == "sync" else jac.step_fused()
-                jac.synchronize()
-                if mode == "fused":
-                    assert jac.fused_supported
-                fields.append([d.interior_to_host(0) for d in dd.domains()])
-            finally:
-                dd.close()
-        for a, b in zip(*fields):
-            assert np.array_equal(a, b), (size, ndom)
+    fields = []
+    for mode in ("sync", "fused"):
+        dd = sb.DistributedDomain(*size)
+        dd.set_gpus([0] * ndom)
+        dd.set_radius(jacobi_radius())
+        h = dd.add_data(dtype, "d")
+        dd.realize()
+        try:
+            jac = Jacobi3D(dd, h)
+            jac.init(0.5)
+            for it in range(7):
+                jac.step() if mode == "sync" else jac.step_fused()
+            jac.synchronize()
+            if mode == "fused":
+                assert jac.fused_supported
+            fields.append([d.interior_to_host(0) for d in dd.domains()])
+        finally:
+            dd.close()
+    for a, b in zip(*fields):
+        assert np.array_equal(a, b), (size, ndom)
 
 
 @pytest.mark.parametrize("schedule", ["host-sync", "queued", "fused"])
