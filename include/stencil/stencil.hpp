@@ -49,6 +49,7 @@ struct sb_bc_plan;
 struct sb_reduce_plan;
 struct sb_reduce_exact_plan;
 struct sb_stencil_plan;
+struct sb_transfer_plan;
 
 class DistributedDomain {
 private:
@@ -146,6 +147,17 @@ private:
   // the opposite side.
   void run_stencil_plans(const std::vector<int64_t> &key, bool exchange, bool writes_src,
                          const std::function<sb_stencil_plan *(size_t, const std::vector<Rect3> &)> &make);
+
+  // multigrid transfers: per (coarse domain, kind, buffers, the swap parity of both domains), one plan per local domain.
+  // serial_ names a domain for the lifetime of the process (an address can be reused by a later domain)
+  uint64_t serial_;
+  std::map<std::vector<int64_t>, std::vector<sb_transfer_plan *>> transferPlans_;
+  std::set<std::pair<uint64_t, bool>> paired_; // (coarse serial, with ghosts) that passed the pairing check
+  void transfer(DistributedDomain &coarse, bool prolong, int dtype, size_t dq, stencil::Which dw, size_t sq, stencil::Which sw, int64_t aq,
+                stencil::Which aw, bool exchange);
+  void check_pairing(DistributedDomain &coarse, bool ghosts);
+  void destroy_transfer_plans();
+  void create_apply_streams(); // two per local domain (interior, exterior), on first use
 
   std::string outputPrefix_;
 
@@ -358,6 +370,32 @@ public:
     std::vector<size_t> ids;
     for (const DataHandle<T> &h : hs) ids.push_back(h.id());
     return ids;
+  }
+
+  // Multigrid transfers (DESIGN.md section 2.10) between this domain and `coarse`, a realized domain twice as coarse on
+  // every axis: the same partition dim, every subdomain's origin and size exactly half of this one's, on the same rank and
+  // GPU (sb_transfer_check over every subdomain index, checked once per coarse domain), quantities of the same type.
+  // restrict_to: dst (a quantity of coarse) = the 8-cell average of src (a quantity of this domain), curr or next, over
+  // every coarse compute cell; no ghost cells are read.
+  // prolong_from: dst = aux + P src (or P src) over every fine compute cell, P trilinear; dst and aux are quantities of
+  // this domain and aux may be dst (the in-place correction u <- u + P e); src is a curr buffer of coarse, whose radius
+  // must be >= 1 in all 26 directions.  exchange = true runs coarse.exchange() first (collective), exchange = false
+  // leaves the coarse ghost cells to the caller.
+  // One launch per local subdomain on the apply streams; returns when complete.  Plans are kept, per (coarse domain,
+  // kind, buffers, swap parity of both domains), until this domain is destroyed.
+  //     fine.restrict_to(coarse, stencil::curr(f2), stencil::curr(r));
+  //     fine.prolong_from(coarse, stencil::curr(u), stencil::curr(e), stencil::curr(u));
+  template <typename T> void restrict_to(DistributedDomain &coarse, const stencil::Buffer<T> &dst, const stencil::Buffer<T> &src) {
+    transfer(coarse, false, stencil::bc_dtype<T>(), dst.h.id(), dst.which, src.h.id(), src.which, -1, stencil::Which::curr, false);
+  }
+  template <typename T>
+  void prolong_from(DistributedDomain &coarse, const stencil::Buffer<T> &dst, const stencil::Buffer<T> &src, bool exchange = true) {
+    transfer(coarse, true, stencil::bc_dtype<T>(), dst.h.id(), dst.which, src.h.id(), src.which, -1, stencil::Which::curr, exchange);
+  }
+  template <typename T>
+  void prolong_from(DistributedDomain &coarse, const stencil::Buffer<T> &dst, const stencil::Buffer<T> &src, const stencil::Buffer<T> &aux,
+                    bool exchange = true) {
+    transfer(coarse, true, stencil::bc_dtype<T>(), dst.h.id(), dst.which, src.h.id(), src.which, int64_t(aux.h.id()), aux.which, exchange);
   }
 
   // one CSV file per subdomain: Z,Y,X,<quantities...>

@@ -495,6 +495,55 @@ int sb_stencil_sys_plan_create(sb_stencil_plan **out, int device, int dtype, con
                                const int64_t acc_origin[3], int64_t zsize, int nbox, const int64_t *lo, const int64_t *hi);
 
 /* ---------------------------------------------------------------------------------------------
+ * Multigrid transfers (DESIGN.md section 2.10) between a cell-centred grid and the grid twice as coarse on every axis.
+ * Coarse cell I covers the fine cells 2I + d, d in {0,1}^3; all coordinates are global compute coordinates.  In the
+ * quantity's type T with every multiply and add rounded separately (no FMA contraction); every weight is exact in T.
+ *   Restriction, the 8-cell average, for each coarse cell I of a box:
+ *     acc = F(2I + (0,0,0));  acc = acc + F(2I + d) for d = (1,0,0), (0,1,0), (1,1,0), (0,0,1), (1,0,1), (0,1,1), (1,1,1)
+ *     C[I] = T(0.125) * acc
+ *   It reads only fine cells inside the coarse cells' footprint: no fine ghost cells, no exchange.
+ *   Prolongation, trilinear, for each fine cell p of a box: parent P = floor(p / 2) per axis, side s_a = +1 if p_a is
+ *   odd, else -1, and
+ *     acc = T(27/64) * E[P]
+ *     acc = acc + T(9/64) * E[P + s_x e_x];  acc = acc + T(9/64) * E[P + s_y e_y];  acc = acc + T(9/64) * E[P + s_z e_z]
+ *     acc = acc + T(3/64) * E[P + s_x e_x + s_y e_y];  then (x, z), then (y, z)
+ *     acc = acc + T(1/64) * E[P + s]
+ *     dst[p] = aux[p] + acc, or dst[p] = acc without aux
+ *   aux may be dst (each cell's aux value is read before that cell is written, by the same thread): u <- u + P e in
+ *   place.  dst must not be src.  It reads coarse cells within +-1 of the parent box on every axis, corners included,
+ *   so the coarse quantity needs one exchanged ghost layer in all 26 directions.
+ * Walls need nothing special: the coarse ghost cells come from the coarse domain's own BC.  ODD(c) and EVEN mirror about
+ * the wall face, which is the same plane on both grids, so trilinear interpolation reproduces the linear extrapolation
+ * to the wall.  VALUE(c) pins the ghost cell's centre, h/2 beyond the face, and h differs between the grids, so a cycle
+ * with VALUE walls on every level is not consistent.
+ * ------------------------------------------------------------------------------------------- */
+typedef enum sb_transfer_kind { SB_TRANSFER_RESTRICT = 0, SB_TRANSFER_PROLONG = 1 } sb_transfer_kind;
+/* Host only.  Whether a fine and a coarse partition pair for transfers that stay on each subdomain's GPU: the same dim,
+ * and for every subdomain index (x fastest, fine_dim[0] * fine_dim[1] * fine_dim[2] of them, 3 int64 each) fine origin
+ * = 2 * coarse origin and fine size = 2 * coarse size.  coarse_radius27 (the coarse ghost widths) may be NULL, for
+ * restriction only; otherwise every one of the 26 directions needs a radius >= 1, as prolongation reads one ghost layer.
+ * SB_ERR_INVALID with a message naming the subdomain index and axis, or the missing ghost direction. */
+int sb_transfer_check(const int64_t fine_dim[3], const int64_t coarse_dim[3], const int64_t *fine_origin, const int64_t *fine_size,
+                      const int64_t *coarse_origin, const int64_t *coarse_size, const int64_t coarse_radius27[27]);
+/* A persistent plan of one transfer over the box [lo, hi) of dst, in dst's global coordinates: coarse cells for
+ * SB_TRANSFER_RESTRICT (dst coarse, src fine), fine cells for SB_TRANSFER_PROLONG (dst fine, src coarse).  Each
+ * allocation has its own pitch, row count, zsize and acc_origin (the global coordinate of its element (0,0,0), as for
+ * sb_jacobi3d); aux (prolongation only; ptr NULL: none) shares dst's.  dtype SB_DTYPE_F32 or SB_DTYPE_F64.  Errors
+ * (SB_ERR_INVALID with a message, before anything is allocated): an unknown dtype or kind, a NULL dst or src, dst == src,
+ * aux given to a restriction, aux with another pitch or row count than dst, a pointer or pitch that is not a multiple of
+ * the element size, lo > hi, a box outside dst's allocation, and reads that leave src's allocation (restriction: fine
+ * [2 lo, 2 hi); prolongation: coarse [floor(lo / 2) - 1, floor((hi - 1) / 2) + 2) on every axis).
+ * sb_transfer_plan_launch allocates nothing and never synchronises the host.  sb_transfer_plan_bytes: the algorithmic
+ * bytes of a launch, every element the rule reads counted once and one element written per cell of the box. */
+typedef struct sb_transfer_plan sb_transfer_plan;
+int sb_transfer_plan_create(sb_transfer_plan **out, int device, int dtype, int kind, sb_pitched dst, const int64_t dst_acc_origin[3],
+                            int64_t dst_zsize, sb_pitched src, const int64_t src_acc_origin[3], int64_t src_zsize, sb_pitched aux,
+                            const int64_t lo[3], const int64_t hi[3]);
+int sb_transfer_plan_launch(sb_transfer_plan *plan, void *stream);
+int64_t sb_transfer_plan_bytes(const sb_transfer_plan *plan);
+int sb_transfer_plan_destroy(sb_transfer_plan *plan);
+
+/* ---------------------------------------------------------------------------------------------
  * 7-point jacobi step (the reference's user kernel, bin/jacobi3d.cu:40-85) over a region.
  * dtype_size 4 = float, 8 = double.  acc_origin = global coordinate of allocation element (0,0,0)
  * (Accessor origin, include/stencil/local_domain.cuh:153-173).  [lo,hi) = region to update,

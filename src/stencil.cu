@@ -11,6 +11,7 @@
 
 #include "stencil_b200.h"
 
+#include <atomic>
 #include <cmath>
 #include <cstdio>
 #include <cstring>
@@ -38,6 +39,8 @@ DistributedDomain::DistributedDomain(size_t x, size_t y, size_t z)
 #ifdef STENCIL_EXCHANGE_STATS
   timeExchange_ = timeSwap_ = 0;
 #endif
+  static std::atomic<uint64_t> domains_made{0};
+  serial_ = ++domains_made;
   MPI_Comm_rank(MPI_COMM_WORLD, &rank_);
   MPI_Comm_size(MPI_COMM_WORLD, &worldSize_);
   if (const char *s = std::getenv("STENCIL_OUTPUT_PREFIX")) outputPrefix_ = s;
@@ -76,6 +79,7 @@ DistributedDomain::~DistributedDomain() {
 
 void DistributedDomain::destroy_plans() {
   destroy_reduce_plans();
+  destroy_transfer_plans();
   destroy_stencil_plans();
   for (auto *sides : {&plans_, &unpackPlans_}) {
     for (int parity = 0; parity < 2; ++parity) {
@@ -787,17 +791,7 @@ void DistributedDomain::run_stencil_plans(const std::vector<int64_t> &key, bool 
     }
     found = stencilPlans_.emplace(key, std::move(per_dom)).first;
   }
-  if (applyStreams_.empty()) {
-    // blocking streams: ordered after the work the caller queued on the legacy default stream
-    for (LocalDomain &d : domains_) {
-      d.set_device();
-      for (int k = 0; k < 2; ++k) {
-        cudaStream_t s;
-        CUDA_RUNTIME(cudaStreamCreate(&s));
-        applyStreams_.push_back(s);
-      }
-    }
-  }
+  create_apply_streams();
   const std::vector<std::vector<sb_stencil_plan *>> &plans = found->second;
   for (size_t di = 0; di < domains_.size(); ++di)
     if (SB_OK != sb_stencil_plan_launch(plans[di][0], applyStreams_[2 * di])) LOG_FATAL("apply: " << sb_last_error());
@@ -810,6 +804,110 @@ void DistributedDomain::run_stencil_plans(const std::vector<int64_t> &key, bool 
     domains_[di].set_device();
     CUDA_RUNTIME(cudaStreamSynchronize(applyStreams_[2 * di]));
     CUDA_RUNTIME(cudaStreamSynchronize(applyStreams_[2 * di + 1]));
+  }
+}
+
+void DistributedDomain::create_apply_streams() {
+  if (!applyStreams_.empty()) return;
+  // blocking streams: ordered after the work the caller queued on the legacy default stream
+  for (LocalDomain &d : domains_) {
+    d.set_device();
+    for (int k = 0; k < 2; ++k) {
+      cudaStream_t s;
+      CUDA_RUNTIME(cudaStreamCreate(&s));
+      applyStreams_.push_back(s);
+    }
+  }
+}
+
+// ---- multigrid transfers (DESIGN.md section 2.10) ------------------------------------------------------------------------
+void DistributedDomain::destroy_transfer_plans() {
+  for (auto &kv : transferPlans_)
+    for (sb_transfer_plan *p : kv.second) sb_transfer_plan_destroy(p);
+  transferPlans_.clear();
+  paired_.clear();
+}
+
+void DistributedDomain::check_pairing(DistributedDomain &coarse, bool ghosts) {
+  if (paired_.count(std::make_pair(coarse.serial_, ghosts))) return;
+  const Dim3 fdim = placement_->dim(), cdim = coarse.placement_->dim();
+  int64_t fd[3], cd[3];
+  set3(fd, fdim);
+  set3(cd, cdim);
+  // every subdomain index, x fastest: global information, so every rank reaches the same verdict
+  std::vector<Dim3> idx;
+  for (int64_t z = 0; z < fdim.z; ++z)
+    for (int64_t y = 0; y < fdim.y; ++y)
+      for (int64_t x = 0; x < fdim.x; ++x) idx.push_back(Dim3(x, y, z));
+  std::vector<int64_t> fo(3 * idx.size()), fs(3 * idx.size()), co(3 * idx.size()), cs(3 * idx.size());
+  for (size_t k = 0; k < idx.size(); ++k) {
+    set3(&fo[3 * k], placement_->subdomain_origin(idx[k]));
+    set3(&fs[3 * k], placement_->subdomain_size(idx[k]));
+    if (fdim == cdim) { // otherwise sb_transfer_check stops at the dims
+      set3(&co[3 * k], coarse.placement_->subdomain_origin(idx[k]));
+      set3(&cs[3 * k], coarse.placement_->subdomain_size(idx[k]));
+    }
+  }
+  int64_t r27[27];
+  for (int z = -1, i = 0; z <= 1; ++z)
+    for (int y = -1; y <= 1; ++y)
+      for (int x = -1; x <= 1; ++x) r27[i++] = int64_t(coarse.radius_.dir(x, y, z));
+  if (SB_OK != sb_transfer_check(fd, cd, fo.data(), fs.data(), co.data(), cs.data(), ghosts ? r27 : nullptr))
+    LOG_FATAL("transfer: " << sb_last_error());
+  for (const Dim3 &i : idx) {
+    if (placement_->get_rank(i) != coarse.placement_->get_rank(i) || placement_->get_subdomain_id(i) != coarse.placement_->get_subdomain_id(i))
+      LOG_FATAL("transfer: subdomain " << i << " belongs to another rank or local slot on the coarse level");
+    if (placement_->get_cuda(i) != coarse.placement_->get_cuda(i))
+      LOG_FATAL("transfer: subdomain " << i << " is on GPU " << placement_->get_cuda(i) << " on the fine level and GPU " << coarse.placement_->get_cuda(i)
+                                       << " on the coarse one");
+  }
+  paired_.insert(std::make_pair(coarse.serial_, ghosts));
+}
+
+void DistributedDomain::transfer(DistributedDomain &coarse, bool prolong, int dtype, size_t dq, stencil::Which dw, size_t sq, stencil::Which sw,
+                                 int64_t aq, stencil::Which aw, bool exchange) {
+  using stencil::Which;
+  const char *name = prolong ? "prolong_from" : "restrict_to";
+  if (&coarse == this) LOG_FATAL(name << ": coarse must be another DistributedDomain");
+  if (domains_.empty() || plans_[0].size() != domains_.size() || coarse.domains_.empty() || coarse.plans_[0].size() != coarse.domains_.size())
+    LOG_FATAL(name << ": call realize() on both domains first");
+  if (dtype != SB_DTYPE_F32 && dtype != SB_DTYPE_F64) LOG_FATAL(name << ": a transfer computes in float or double");
+  DistributedDomain &D = prolong ? *this : coarse, &S = prolong ? coarse : *this;
+  if (dq >= D.dataDtype_.size() || D.dataDtype_[dq] != dtype) LOG_FATAL(name << ": dst " << dq << " is not a quantity of that type");
+  if (sq >= S.dataDtype_.size() || S.dataDtype_[sq] != dtype) LOG_FATAL(name << ": src " << sq << " is not a quantity of that type");
+  if (aq >= 0 && (size_t(aq) >= dataDtype_.size() || dataDtype_[size_t(aq)] != dtype)) LOG_FATAL(name << ": aux " << aq << " is not a quantity of that type");
+  if (prolong && sw != Which::curr) LOG_FATAL(name << ": src must be a curr buffer (the one coarse.exchange() fills)");
+  check_pairing(coarse, prolong);
+  const std::vector<int64_t> key = {int64_t(coarse.serial_), int64_t(prolong), int64_t(dq), int64_t(dw == Which::next), int64_t(sq),
+                                    int64_t(sw == Which::next), aq, int64_t(aw == Which::next), parity_, coarse.parity_};
+  auto found = transferPlans_.find(key);
+  if (found == transferPlans_.end()) {
+    auto pick = [](LocalDomain &d, size_t q, Which w) { return as_sb(w == Which::curr ? d.curr_data(q) : d.next_data(q)); };
+    std::vector<sb_transfer_plan *> per_dom;
+    for (size_t di = 0; di < domains_.size(); ++di) {
+      LocalDomain &f = domains_[di], &dd = prolong ? f : coarse.domains_[di], &sd = prolong ? coarse.domains_[di] : f;
+      int64_t dacc[3], sacc[3], lo[3], hi[3];
+      set3(dacc, dd.origin() - Dim3(D.radius_.x(-1), D.radius_.y(-1), D.radius_.z(-1)));
+      set3(sacc, sd.origin() - Dim3(S.radius_.x(-1), S.radius_.y(-1), S.radius_.z(-1)));
+      const Rect3 box = dd.get_compute_region();
+      set3(lo, box.lo);
+      set3(hi, box.hi);
+      const sb_pitched aux = aq < 0 ? sb_pitched{nullptr, 0, 0} : pick(f, size_t(aq), aw);
+      sb_transfer_plan *p = nullptr;
+      if (SB_OK != sb_transfer_plan_create(&p, f.gpu(), dtype, prolong ? SB_TRANSFER_PROLONG : SB_TRANSFER_RESTRICT, pick(dd, dq, dw), dacc,
+                                           dd.raw_size().z, pick(sd, sq, sw), sacc, sd.raw_size().z, aux, lo, hi))
+        LOG_FATAL(name << ": " << sb_last_error());
+      per_dom.push_back(p);
+    }
+    found = transferPlans_.emplace(key, std::move(per_dom)).first;
+  }
+  if (prolong && exchange) coarse.exchange();
+  create_apply_streams();
+  for (size_t di = 0; di < domains_.size(); ++di)
+    if (SB_OK != sb_transfer_plan_launch(found->second[di], applyStreams_[2 * di])) LOG_FATAL(name << ": " << sb_last_error());
+  for (size_t di = 0; di < domains_.size(); ++di) {
+    domains_[di].set_device();
+    CUDA_RUNTIME(cudaStreamSynchronize(applyStreams_[2 * di]));
   }
 }
 

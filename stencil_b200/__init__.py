@@ -24,6 +24,7 @@ from .domain import (  # noqa: F401
     Radius,
     Reduction,
     ReducePlan,
+    TransferPlan,
     box_copy,
     fill,
     get_neighbor,
@@ -35,6 +36,7 @@ from .domain import (  # noqa: F401
     reduce_combine,
     reduce_exact_combine,
     reduce_exact_round,
+    transfer_check,
 )
 from .stencil_op import StencilOp, StencilPlan, StencilSystem, SystemPlan  # noqa: F401
 

@@ -161,6 +161,8 @@ STENCIL_SYS_MAX_INPUTS, STENCIL_SYS_MAX_OUTPUTS, STENCIL_SYS_MAX_TERMS = 8, 4, 1
 
 I6 = C.c_int32 * 6
 
+TRANSFER_RESTRICT, TRANSFER_PROLONG = 0, 1  # sb_transfer_kind
+
 FUSED_MAX_GROUPS = 4096  # SB_FUSED_MAX_GROUPS
 
 
@@ -244,6 +246,14 @@ _SIGS = {
     "sb_stencil_plan_launch": (C.c_int, [C.c_void_p, C.c_void_p]),
     "sb_stencil_plan_bytes": (C.c_int64, [C.c_void_p]),
     "sb_stencil_plan_destroy": (C.c_int, [C.c_void_p]),
+    "sb_transfer_check": (C.c_int, [I3, I3, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
+    "sb_transfer_plan_create": (
+        C.c_int,
+        [C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, Pitched, I3, C.c_int64, Pitched, I3, C.c_int64, Pitched, I3, I3],
+    ),
+    "sb_transfer_plan_launch": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "sb_transfer_plan_bytes": (C.c_int64, [C.c_void_p]),
+    "sb_transfer_plan_destroy": (C.c_int, [C.c_void_p]),
     "sb_signal": (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.c_uint32, C.c_int, C.c_void_p]),
     "sb_wait": (C.c_int, [C.c_void_p, C.c_int, C.c_uint32, C.c_int, C.c_void_p]),
     "sb_jacobi3d": (C.c_int, [Pitched, Pitched, C.c_int, I3, I3, I3, I3, I3, C.c_void_p]),

@@ -22,6 +22,7 @@
 #include "jacobi.cuh"
 #include "stencil_op.cuh"
 #include "stencil_sys.cuh"
+#include "transfer.cuh"
 
 #include "stencil/exchange_plan.hpp"
 #include "stencil/geometry.hpp"
@@ -351,6 +352,16 @@ struct sb_stencil_plan {
   size_t sys_smem = 0;
   std::vector<sb::SysCellParams> sys_cells;
   std::vector<int> sys_cell_grids;
+  int64_t bytes = 0;
+};
+
+struct sb_transfer_plan {
+  int device = 0;
+  int es = 8, kind = SB_TRANSFER_RESTRICT;
+  int launches = 0; // 0: an empty box
+  sb::RestrictParams r{};
+  sb::ProlongParams pr{};
+  int grid = 0; // prolongation CTAs
   int64_t bytes = 0;
 };
 
@@ -2016,6 +2027,185 @@ int sb_stencil_plan_launch(sb_stencil_plan *p, void *stream) {
 int64_t sb_stencil_plan_bytes(const sb_stencil_plan *p) { return p ? p->bytes : 0; }
 
 int sb_stencil_plan_destroy(sb_stencil_plan *p) {
+  delete p;
+  return SB_OK;
+}
+
+// ----------------------------------------------------------------------------------------- multigrid transfers
+static int64_t floor_half(int64_t v) { return v >= 0 ? v / 2 : -((1 - v) / 2); }
+
+int sb_transfer_check(const int64_t fine_dim[3], const int64_t coarse_dim[3], const int64_t *fine_origin, const int64_t *fine_size,
+                      const int64_t *coarse_origin, const int64_t *coarse_size, const int64_t coarse_radius27[27]) {
+  if (!fine_dim || !coarse_dim || !fine_origin || !fine_size || !coarse_origin || !coarse_size)
+    return fail(SB_ERR_INVALID, "sb_transfer_check needs both dims and the origin and size arrays");
+  for (int a = 0; a < 3; ++a) {
+    if (fine_dim[a] < 1 || coarse_dim[a] < 1) return fail(SB_ERR_INVALID, "a partition has at least one subdomain on every axis");
+    if (fine_dim[a] != coarse_dim[a])
+      return fail(SB_ERR_INVALID, "the fine partition is %lld x %lld x %lld subdomains, the coarse one %lld x %lld x %lld: they must be the same",
+                  (long long)fine_dim[0], (long long)fine_dim[1], (long long)fine_dim[2], (long long)coarse_dim[0], (long long)coarse_dim[1],
+                  (long long)coarse_dim[2]);
+  }
+  const int64_t n = fine_dim[0] * fine_dim[1] * fine_dim[2];
+  for (int64_t k = 0; k < n; ++k) {
+    const long long i = (long long)(k % fine_dim[0]), j = (long long)((k / fine_dim[0]) % fine_dim[1]),
+                    l = (long long)(k / (fine_dim[0] * fine_dim[1]));
+    for (int a = 0; a < 3; ++a) {
+      const int64_t fo = fine_origin[3 * k + a], co = coarse_origin[3 * k + a], fs = fine_size[3 * k + a], cs = coarse_size[3 * k + a];
+      if (fo != 2 * co)
+        return fail(SB_ERR_INVALID, "subdomain (%lld, %lld, %lld): fine origin %lld on axis %c is not twice the coarse origin %lld", i, j, l,
+                    (long long)fo, "xyz"[a], (long long)co);
+      if (fs != 2 * cs)
+        return fail(SB_ERR_INVALID, "subdomain (%lld, %lld, %lld): fine size %lld on axis %c is not twice the coarse size %lld", i, j, l,
+                    (long long)fs, "xyz"[a], (long long)cs);
+    }
+  }
+  if (coarse_radius27)
+    for (int z = -1; z <= 1; ++z)
+      for (int y = -1; y <= 1; ++y)
+        for (int x = -1; x <= 1; ++x)
+          if ((x || y || z) && coarse_radius27[(z + 1) * 9 + (y + 1) * 3 + (x + 1)] < 1)
+            return fail(SB_ERR_INVALID, "the coarse radius in direction (%d, %d, %d) is 0: prolongation reads one ghost layer in all 26 directions",
+                        x, y, z);
+  return SB_OK;
+}
+
+int sb_transfer_plan_create(sb_transfer_plan **out, int device, int dtype, int kind, sb_pitched dst, const int64_t dst_acc_origin[3],
+                            int64_t dst_zsize, sb_pitched src, const int64_t src_acc_origin[3], int64_t src_zsize, sb_pitched aux,
+                            const int64_t lo[3], const int64_t hi[3]) {
+  if (!out) return fail(SB_ERR_INVALID, "sb_transfer_plan_create needs an output handle");
+  if (dtype != SB_DTYPE_F32 && dtype != SB_DTYPE_F64) return fail(SB_ERR_INVALID, "dtype %d must be SB_DTYPE_F32 or SB_DTYPE_F64", dtype);
+  if (kind != SB_TRANSFER_RESTRICT && kind != SB_TRANSFER_PROLONG)
+    return fail(SB_ERR_INVALID, "kind %d must be SB_TRANSFER_RESTRICT or SB_TRANSFER_PROLONG", kind);
+  const int es = dtype == SB_DTYPE_F32 ? 4 : 8;
+  const bool prolong = kind == SB_TRANSFER_PROLONG, has_aux = aux.ptr != nullptr;
+  if (!dst.ptr || !src.ptr) return fail(SB_ERR_INVALID, "dst and src must not be NULL");
+  if (dst.ptr == src.ptr) return fail(SB_ERR_INVALID, "dst must not be src");
+  if (has_aux && !prolong) return fail(SB_ERR_INVALID, "a restriction takes no aux");
+  if (!dst_acc_origin || !src_acc_origin || !lo || !hi) return fail(SB_ERR_INVALID, "sb_transfer_plan_create needs both acc_origins, lo and hi");
+  if (dst_zsize < 1 || src_zsize < 1) return fail(SB_ERR_INVALID, "dst_zsize and src_zsize must be >= 1");
+  int rc = stencil_buffers_ok({&dst}, {"dst"}, dst, "dst", es);
+  if (rc == SB_OK) rc = stencil_buffers_ok({&src}, {"src"}, src, "src", es);
+  if (rc == SB_OK && has_aux) rc = stencil_buffers_ok({&aux}, {"aux"}, dst, "dst", es);
+  if (rc != SB_OK) return rc;
+  const int64_t dsize[3] = {dst.pitch / es, dst.ysize, dst_zsize}, ssize[3] = {src.pitch / es, src.ysize, src_zsize};
+  int64_t l[3], e[3];
+  bool empty = false;
+  for (int a = 0; a < 3; ++a) {
+    if (lo[a] > hi[a]) return fail(SB_ERR_INVALID, "lo > hi on axis %c", "xyz"[a]);
+    l[a] = lo[a] - dst_acc_origin[a];
+    e[a] = hi[a] - lo[a];
+    empty = empty || e[a] == 0;
+  }
+  sb_transfer_plan *p = nullptr;
+  if (empty) {
+    p = new sb_transfer_plan();
+    p->device = device;
+    p->es = es;
+    *out = p;
+    return SB_OK;
+  }
+  const int zero[3] = {0, 0, 0};
+  if ((rc = stencil_box_reads_ok(0, l, e, zero, zero, dsize, "dst is written at")) != SB_OK) return rc;
+  // src reads [rl, rl + re) (allocation coordinates) that the checks cover
+  int64_t rl[3], re[3];
+  for (int a = 0; a < 3; ++a) {
+    if (prolong) {
+      rl[a] = floor_half(lo[a]) - 1 - src_acc_origin[a];
+      re[a] = floor_half(hi[a] - 1) + 2 - floor_half(lo[a]) + 1;
+    } else {
+      rl[a] = 2 * lo[a] - src_acc_origin[a];
+      re[a] = 2 * e[a];
+    }
+  }
+  if ((rc = stencil_box_reads_ok(0, rl, re, zero, zero, ssize, prolong ? "the prolongation reads coarse" : "the restriction reads fine")) != SB_OK)
+    return rc;
+  if (e[0] * e[1] * e[2] >= (1ll << 32)) return fail(SB_ERR_INVALID, "a box of more than 2^32 cells");
+
+  DeviceGuard guard(device);
+  if (!guard.ok) return fail(SB_ERR_NOGPU, "cannot select CUDA device %d", device);
+  int sms = 0;
+  SB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
+  p = new sb_transfer_plan();
+  p->device = device;
+  p->es = es;
+  p->kind = kind;
+  const int64_t cells = e[0] * e[1] * e[2];
+  if (!prolong) {
+    sb::RestrictParams &r = p->r;
+    r.dst = static_cast<char *>(dst.ptr);
+    r.src = static_cast<const char *>(src.ptr);
+    r.dpitch = dst.pitch;
+    r.dslice = dst.pitch * dst.ysize;
+    r.spitch = src.pitch;
+    r.sslice = src.pitch * src.ysize;
+    for (int a = 0; a < 3; ++a) {
+      r.lo[a] = int(l[a]);
+      r.ext[a] = int(e[a]);
+      r.flo[a] = int(rl[a]);
+    }
+    p->bytes = (8 + 1) * cells * es;
+    p->launches = 1;
+  } else {
+    sb::ProlongParams &q = p->pr;
+    q.dst = static_cast<char *>(dst.ptr);
+    q.aux = has_aux ? static_cast<const char *>(aux.ptr) : nullptr;
+    q.src = static_cast<const char *>(src.ptr);
+    q.dpitch = dst.pitch;
+    q.dslice = dst.pitch * dst.ysize;
+    q.spitch = src.pitch;
+    q.sslice = src.pitch * src.ysize;
+    int64_t reads = 1;
+    for (int a = 0; a < 3; ++a) {
+      q.lo[a] = int(l[a]);
+      q.ext[a] = int(e[a]);
+      q.off[a] = int(2 * src_acc_origin[a] - dst_acc_origin[a]);
+      q.plo[a] = int(floor_half(lo[a]) - src_acc_origin[a]);
+      q.pext[a] = int(floor_half(hi[a] - 1) - floor_half(lo[a]) + 1);
+      // the cells the rule reads: a child at an even coordinate reads its parent's lower neighbour, at an odd one the upper
+      q.rlo[a] = int(floor_half(lo[a] - 1) - src_acc_origin[a]);
+      q.rhi[a] = int(floor_half(hi[a]) + 1 - src_acc_origin[a]);
+      reads *= q.rhi[a] - q.rlo[a];
+    }
+    p->bytes = reads * es + cells * es * (has_aux ? 2 : 1);
+    const int per_sm = sb::prolong_ctas_per_sm(es);
+    if (per_sm <= 0) {
+      delete p;
+      return fail(SB_ERR_CUDA, "the prolongation kernel cannot be configured: %s", cudaGetErrorString(cudaGetLastError()));
+    }
+    q.tiles_x = (q.pext[0] + sb::kProlongX - 1) / sb::kProlongX;
+    q.tiles_y = (q.pext[1] + sb::kProlongY - 1) / sb::kProlongY;
+    // z chunks: at least two waves of resident CTAs, no shorter than 8 parent planes (each chunk reloads 2 planes)
+    const long long cols = (long long)q.tiles_x * q.tiles_y;
+    const long long want = (2ll * sms * per_sm + cols - 1) / cols;
+    int zc = int((q.pext[2] + want - 1) / want);
+    zc = std::max(zc, std::min(8, q.pext[2]));
+    q.zchunk = zc;
+    const long long grid = cols * ((q.pext[2] + zc - 1) / zc);
+    if (grid >= (1ll << 31)) {
+      delete p;
+      return fail(SB_ERR_INVALID, "box too large for the prolongation kernel");
+    }
+    p->grid = int(grid);
+    p->launches = 1;
+  }
+  *out = p;
+  return SB_OK;
+}
+
+int sb_transfer_plan_launch(sb_transfer_plan *p, void *stream) {
+  if (!p) return fail(SB_ERR_INVALID, "null plan");
+  if (!p->launches) return SB_OK;
+  DeviceGuard guard(p->device);
+  if (!guard.ok) return fail(SB_ERR_NOGPU, "cannot select CUDA device %d", p->device);
+  const cudaStream_t s = static_cast<cudaStream_t>(stream);
+  g_launches += uint64_t(p->kind == SB_TRANSFER_PROLONG ? sb::launch_prolong(p->pr, p->es, p->grid, s) : sb::launch_restrict(p->r, p->es, s));
+  SB_CUDA(cudaGetLastError());
+  return SB_OK;
+}
+
+int64_t sb_transfer_plan_bytes(const sb_transfer_plan *p) { return p ? p->bytes : 0; }
+
+int sb_transfer_plan_destroy(sb_transfer_plan *p) {
   delete p;
   return SB_OK;
 }

@@ -339,6 +339,48 @@ class BCPlan:
             pass
 
 
+# ------------------------------------------------------------------------------------------ multigrid transfers
+def transfer_check(fine_dim: Vec, coarse_dim: Vec, fine_origins: Sequence[Vec], fine_sizes: Sequence[Vec], coarse_origins: Sequence[Vec],
+                   coarse_sizes: Sequence[Vec], coarse_radius: Optional[Radius] = None) -> None:
+    """sb_transfer_check: whether a fine and a coarse partition pair for transfers (pure geometry, host only).  Per
+    subdomain index in partition order (x fastest): origins and sizes.  coarse_radius=None checks restriction only;
+    with a radius, prolongation's one ghost layer in all 26 directions as well.  Raises StencilError."""
+
+    def arr(vs):
+        return (C.c_int64 * (3 * max(1, len(vs))))(*[int(v) for t in vs for v in t])
+
+    r = coarse_radius.c27() if coarse_radius is not None else None
+    check(lib().sb_transfer_check(i3(fine_dim), i3(coarse_dim), arr(fine_origins), arr(fine_sizes), arr(coarse_origins), arr(coarse_sizes), r))
+
+
+class TransferPlan:
+    """sb_transfer_plan: one restriction (kind 0; dst coarse, src fine) or prolongation (kind 1; dst fine, src coarse,
+    optional aux with dst's layout) over the box [lo, hi) of dst (global coordinates); one launch."""
+
+    def __init__(self, device: int, dtype, kind: int, dst: Pitched, dst_origin: Vec, dst_zsize: int, src: Pitched, src_origin: Vec,
+                 src_zsize: int, aux: Optional[Pitched], lo: Vec, hi: Vec):
+        h = C.c_void_p()
+        check(lib().sb_transfer_plan_create(C.byref(h), device, bc_dtype(dtype), int(kind), dst, i3(dst_origin), int(dst_zsize), src,
+                                            i3(src_origin), int(src_zsize), aux if aux is not None else Pitched(None, 0, 0), i3(lo), i3(hi)))
+        self._h = h
+        self.device = device
+        self.bytes = int(lib().sb_transfer_plan_bytes(h))
+
+    def launch(self, stream=None) -> None:
+        check(lib().sb_transfer_plan_launch(self._h, stream_ptr(stream)))
+
+    def destroy(self) -> None:
+        if self._h:
+            lib().sb_transfer_plan_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.destroy()
+        except Exception:
+            pass
+
+
 # ------------------------------------------------------------------------------------------ reductions
 @dataclasses.dataclass(frozen=True)
 class Reduction:
@@ -697,6 +739,8 @@ class DistributedDomain:
         self._reduce_plans: Dict[tuple, List[ReducePlan]] = {}  # (item keys, parity) -> one plan per local domain
         self._stencil_plans: Dict[tuple, list] = {}  # (op, buffers, exchange, parity) -> per local domain: plans
         self._apply_streams: list = []  # per local domain: (interior stream, exterior stream)
+        self._transfer_plans: Dict[tuple, list] = {}  # (coarse domain, kind, buffers, both parities) -> per local domain
+        self._paired: set = set()  # (coarse domain, with ghosts) that passed the pairing check
 
     # -- configuration (call before realize)
     def set_radius(self, r) -> None:
@@ -1396,7 +1440,94 @@ class DistributedDomain:
             si.synchronize()
             se.synchronize()
 
+    # -- multigrid transfers
+    def restrict_to(self, coarse: "DistributedDomain", dst, src) -> None:
+        """dst (a quantity of coarse) = the 8-cell average of src (a quantity of this domain) over every coarse compute
+        cell (DESIGN.md section 2.10).  Buffers follow apply(): a bare handle means "next" for dst and "curr" for src;
+        src may be curr or next, as restriction reads no ghost cells.  coarse must pair with this domain: the same
+        partition dim, every subdomain exactly twice as coarse, on the same rank and GPU (sb_transfer_check; checked
+        once per coarse domain).  One launch per local subdomain on the apply streams, after the work queued on the
+        caller's stream; returns when it is complete.  Plans are cached as prolong_from() describes.
+            fine.restrict_to(coarse, (f2, "curr"), (r, "curr"))"""
+        self._transfer(coarse, _lib.TRANSFER_RESTRICT, dst, src, None, False)
+
+    def prolong_from(self, coarse: "DistributedDomain", dst, src, aux=None, exchange: bool = True) -> None:
+        """dst = aux + P src (or P src without aux) over every fine compute cell, P the trilinear interpolation from the
+        coarse grid (DESIGN.md section 2.10).  dst and aux are quantities of this domain (bare handles: "next" and
+        "curr"); aux may be dst, which gives the in-place correction u <- u + P e.  src is a quantity of coarse and must
+        be a curr buffer: its ghost cells are read.  exchange=True runs coarse.exchange() first (collective: every rank
+        calls it), with exchange=False the caller guarantees the coarse ghost cells.  The coarse radius must be >= 1 in
+        all 26 directions.  Plans are built on first use and kept, per (coarse domain, kind, buffers, the swap parity
+        of both domains), until close().
+            fine.prolong_from(coarse, (u, "curr"), (e, "curr"), aux=(u, "curr"))"""
+        self._transfer(coarse, _lib.TRANSFER_PROLONG, dst, src, aux, exchange)
+
+    def _transfer(self, coarse, kind: int, dst, src, aux, exchange: bool) -> None:
+        name = "restrict_to" if kind == _lib.TRANSFER_RESTRICT else "prolong_from"
+        if not isinstance(coarse, DistributedDomain) or coarse is self:
+            raise _lib.StencilError(f"{name}: coarse must be another DistributedDomain, not {coarse!r}")
+        if self.partition_ is None or not self._plans or coarse.partition_ is None or not coarse._plans:
+            raise _lib.StencilError(f"{name}: call realize() on both domains first")
+        restrict = kind == _lib.TRANSFER_RESTRICT
+        dst_dom, src_dom = (coarse, self) if restrict else (self, coarse)
+
+        def buf(dom, arg, default, role):
+            h, which = (arg, default) if isinstance(arg, DataHandle) else tuple(arg)
+            if not isinstance(h, DataHandle) or which not in ("curr", "next") or not 0 <= h.id < len(dom.dtypes_):
+                raise _lib.StencilError(f"{name}: {role} must be a DataHandle of the {'coarse' if dom is coarse else 'fine'} domain "
+                                        f"or (DataHandle, 'curr' | 'next'), not {arg!r}")
+            return h.id, which
+
+        d = buf(dst_dom, dst, "next", "dst")
+        s = buf(src_dom, src, "curr", "src")
+        a = buf(self, aux, "curr", "aux") if aux is not None else None
+        dtype = dst_dom.dtypes_[d[0]]
+        if src_dom.dtypes_[s[0]] != dtype or (a is not None and self.dtypes_[a[0]] != dtype) or bc_dtype(dtype) == 0:
+            raise _lib.StencilError(f"{name}: dst, src and aux must all be float32 or all float64")
+        if not restrict and s[1] != "curr":
+            raise _lib.StencilError(f"{name}: src must be a curr buffer (the one coarse.exchange() fills)")
+        self._check_pairing(coarse, not restrict)
+        key = (coarse, kind, d, s, a, self._parity, coarse._parity)
+        plans = self._transfer_plans.get(key)
+        if plans is None:
+            plans = []
+            for fd, cd in zip(self.domains_, coarse.domains_):
+                dd, sd = (cd, fd) if restrict else (fd, cd)
+                lo, hi = dd.get_compute_region()
+                plans.append((TransferPlan(fd.gpu(), dtype, kind, dd.pitched(*d), dd.accessor_origin(), dd.raw_size()[2], sd.pitched(*s),
+                                           sd.accessor_origin(), sd.raw_size()[2], fd.pitched(*a) if a is not None else None, lo, hi),))
+            self._transfer_plans[key] = plans
+        if not restrict and exchange:
+            coarse.exchange()
+        self._run_plans(plans, False)
+
+    def _check_pairing(self, coarse, ghosts: bool) -> None:
+        """The pairing of sb_transfer_check over every subdomain index (global information, so every rank reaches the same
+        verdict), plus the same owner rank and GPU for every index; ghosts: prolongation's coarse radius as well."""
+        if (coarse, ghosts) in self._paired:
+            return
+        fp, cp = self.partition_, coarse.partition_
+        if fp.dim != cp.dim:
+            raise _lib.StencilError(f"transfer: the fine partition is {fp.dim} subdomains, the coarse one {cp.dim}: they must be the same")
+        idx = fp.indices()
+        transfer_check(fp.dim, cp.dim, [fp.subdomain_origin(i) for i in idx], [fp.subdomain_size(i) for i in idx],
+                       [cp.subdomain_origin(i) for i in idx], [cp.subdomain_size(i) for i in idx], coarse.radius_ if ghosts else None)
+        for i in idx:
+            if self._owner[i] != coarse._owner[i]:
+                raise _lib.StencilError(f"transfer: subdomain {i} belongs to rank / slot {self._owner[i]} on the fine level and "
+                                        f"{coarse._owner[i]} on the coarse one")
+        for i, fd, cd in zip(self.domain_idx_, self.domains_, coarse.domains_):
+            if fd.gpu() != cd.gpu():
+                raise _lib.StencilError(f"transfer: subdomain {i} is on GPU {fd.gpu()} on the fine level and GPU {cd.gpu()} on the coarse one")
+        self._paired.add((coarse, ghosts))
+
     def close(self) -> None:
+        for plans in self._transfer_plans.values():
+            for per_dom in plans:
+                for p in per_dom:
+                    p.destroy()
+        self._transfer_plans = {}
+        self._paired = set()
         for plans in self._stencil_plans.values():
             for per_dom in plans:
                 for p in per_dom:
