@@ -1,0 +1,196 @@
+// Geometric multigrid for A u = f on a DistributedDomain (DESIGN.md section 2.11), the C++ twin of
+// stencil_b200.Multigrid: V(nu1, nu2) cycles over coarsenings by 2, built from the coloured sweeps (section 2.9), the
+// fused residual-restriction and the prolongation, queued on CUDA events with one host wait per cycle.
+//
+//     stencil::Multigrid<double> mg(dd, u, f, r, [&](int l) { return A(l); });   // A on level l, l = 0 finest
+//     std::vector<double> history = mg.solve(1e-8, 20);                          // ||f - A u||_2 per cycle
+//
+// u, f and r are quantities of the realized domain dd (r: scratch for the residual norm).  Each coarse level is a
+// DistributedDomain of u and f on the same GPUs, placement and boundary kinds, with dd's radius raised to >= 1 in all 26
+// directions; the grid is halved while every subdomain extent is even and its half >= 2, at most `levels` grids (0: no
+// cap).  Coarse u takes ODD(0) where u has ODD(c) and EVEN where u has EVEN; VALUE, a FIXED face without a BC on u, a
+// grid that cannot be coarsened once, an op with coefficient or aux terms or of reach > 1 are refused (LOG_FATAL) before
+// any domain is built.  The smoother is red-black Gauss-Seidel if every level's A passes the red-black colour check,
+// else 8-colour.  Building, cycle() and solve() are collective under MPI.  Periodic Poisson needs f of zero mean.
+#pragma once
+
+#include <cmath>
+#include <functional>
+#include <memory>
+#include <vector>
+
+#include "stencil/linear_stencil.hpp"
+#include "stencil/stencil.hpp"
+#include "stencil_b200.h"
+
+namespace stencil {
+
+template <typename T> class Multigrid {
+public:
+  Multigrid(DistributedDomain &dd, DataHandle<T> u, DataHandle<T> f, DataHandle<T> r, const std::function<LinearStencil(int)> &op_at, int nu1 = 2,
+            int nu2 = 2, int coarse_sweeps = 30, int levels = 0)
+      : nu1_(nu1), nu2_(nu2), coarse_sweeps_(coarse_sweeps), r_(r) {
+    const int dtype = bc_dtype<T>();
+    if (dtype != SB_DTYPE_F32 && dtype != SB_DTYPE_F64) LOG_FATAL("Multigrid: u, f and r must be float or double");
+    if (dd.domains_.empty()) LOG_FATAL("Multigrid: dd must be realized");
+    if (u.id() == f.id() || u.id() == r.id() || f.id() == r.id()) LOG_FATAL("Multigrid: u, f and r must be three different quantities");
+    if (nu1 < 0 || nu2 < 0 || coarse_sweeps < 1) LOG_FATAL("Multigrid: nu1 and nu2 must be >= 0 and coarse_sweeps >= 1");
+    if (levels == 1 || levels < 0) LOG_FATAL("Multigrid: levels must be >= 2 (or 0: no cap)");
+    // the coarse BCs of u
+    std::vector<std::pair<int, BC>> walls;
+    for (int fc = 0; fc < 6; ++fc) {
+      if (dd.boundary_[fc / 2] != Topology::Boundary::FIXED) continue;
+      auto it = dd.bcs_.find(std::make_pair(u.id(), fc));
+      const int kind = it == dd.bcs_.end() ? SB_BC_NONE : int(it->second.kind);
+      if (kind == SB_BC_VALUE) LOG_FATAL("Multigrid: VALUE walls are not consistent across levels (DESIGN.md section 2.10); use ODD(c)");
+      if (kind == SB_BC_NONE) LOG_FATAL("Multigrid: u needs a boundary condition (ODD or EVEN) on every FIXED face");
+      walls.push_back(std::make_pair(fc, kind == SB_BC_ODD ? BC::ODD(0.0) : BC::EVEN()));
+    }
+    // the number of grids: every subdomain extent (global information, the same verdict on every rank)
+    const Dim3 dim = dd.placement_->dim();
+    int nlev = 1;
+    for (int64_t step = 1; levels == 0 || nlev < levels; step *= 2, ++nlev) {
+      bool ok = true;
+      for (int64_t z = 0; z < dim.z && ok; ++z)
+        for (int64_t y = 0; y < dim.y && ok; ++y)
+          for (int64_t x = 0; x < dim.x && ok; ++x) {
+            const Dim3 s = dd.placement_->subdomain_size(Dim3(x, y, z));
+            for (int64_t v : {s.x, s.y, s.z}) ok = ok && v % (2 * step) == 0 && v / (2 * step) >= 2;
+          }
+      if (!ok) break;
+    }
+    if (nlev < 2) LOG_FATAL("Multigrid: the grid cannot be coarsened once: every subdomain extent must be even and >= 4");
+    Radius cr = dd.radius_;
+    for (int z = -1; z <= 1; ++z)
+      for (int y = -1; y <= 1; ++y)
+        for (int x = -1; x <= 1; ++x)
+          if (x || y || z) cr.dir(x, y, z) = std::max<size_t>(cr.dir(x, y, z), 1);
+    std::vector<LinearStencil> ops;
+    for (int l = 0; l < nlev; ++l) {
+      ops.push_back(op_at(l));
+      const LinearStencil &A = ops.back();
+      if (A.ncoef() > 0 || A.has_aux()) LOG_FATAL("Multigrid: op_at(" << l << ") has coefficient or aux terms");
+      for (const sb_stencil_term &t : A.terms())
+        for (int a = 0; a < 3; ++a)
+          if (t.offset[a] < -1 || t.offset[a] > 1) LOG_FATAL("Multigrid: op_at(" << l << ") reaches beyond 1 cell");
+    }
+    for (int m : {2, 8}) {
+      bool ok = true;
+      for (int l = 0; l < nlev && ok; ++l) {
+        int64_t r27[27];
+        const Radius &rad = l == 0 ? dd.radius_ : cr;
+        for (int z = -1, i = 0; z <= 1; ++z)
+          for (int y = -1; y <= 1; ++y)
+            for (int x = -1; x <= 1; ++x) r27[i++] = int64_t(rad.dir(x, y, z));
+        ok = SB_OK == sb_stencil_ccheck(ops[l].vterms().data(), int(ops[l].vterms().size()), r27, m);
+      }
+      if (ok) {
+        colours_ = m;
+        break;
+      }
+    }
+    if (!colours_) LOG_FATAL("Multigrid: no Gauss-Seidel colouring applies to A (or it leaves the radius)");
+    dd.create_apply_streams();
+    levels_.push_back(Level{&dd, nullptr, u, f, ops[0].relax(1.0), residual(ops[0])});
+    Dim3 size = dd.size_;
+    for (int l = 1; l < nlev; ++l) {
+      size = Dim3(size.x / 2, size.y / 2, size.z / 2);
+      std::unique_ptr<DistributedDomain> cd(new DistributedDomain(size.x, size.y, size.z));
+      if (!dd.gpus_.empty()) cd->set_gpus(dd.gpus_);
+      cd->set_placement(dd.strategy_);
+      cd->set_radius(cr);
+      DataHandle<T> cu = cd->template add_data<T>("u"), cf = cd->template add_data<T>("f");
+      cd->set_boundary(dd.boundary_[0], dd.boundary_[1], dd.boundary_[2]);
+      for (const auto &w : walls) cd->set_boundary_condition(cu, Dim3(w.first / 2 == 0 ? (w.first % 2 ? 1 : -1) : 0, w.first / 2 == 1 ? (w.first % 2 ? 1 : -1) : 0,
+                                                                       w.first / 2 == 2 ? (w.first % 2 ? 1 : -1) : 0), w.second);
+      cd->realize();
+      // every level queues on dd's apply streams, so stream order alone orders consecutive levels
+      cd->applyStreams_ = dd.applyStreams_;
+      cd->sharedApplyStreams_ = true;
+      levels_.push_back(Level{cd.get(), std::move(cd), cu, cf, ops[size_t(l)].relax(1.0), residual(ops[size_t(l)])});
+    }
+    for (size_t l = 0; l + 1 < levels_.size(); ++l) levels_[l].dd->check_pairing(*levels_[l + 1].dd, true);
+  }
+
+  size_t num_levels() const { return levels_.size(); }
+  int colours() const { return colours_; }
+
+  // One V(nu1, nu2) cycle, queued after the work on the legacy default stream; returns when it is complete.
+  void cycle() {
+    for (Level &L : levels_) L.dd->queued_ = true;
+    vcycle(0);
+    for (Level &L : levels_) L.dd->queued_ = false;
+    DistributedDomain &dd = *levels_[0].dd;
+    for (size_t i = 0; i < dd.applyStreams_.size(); ++i) {
+      CUDA_RUNTIME(cudaSetDevice(dd.domains_[i / 2].gpu()));
+      CUDA_RUNTIME(cudaStreamSynchronize(dd.applyStreams_[i]));
+    }
+    for (Level &L : levels_) L.dd->exchange_wait();
+  }
+
+  // ||f - A u||_2: the residual into r and an exact reduction, the same on every rank and partition
+  double residual_norm() {
+    Level &L = levels_[0];
+    L.dd->apply(L.res, curr(r_), L.u, curr(L.f));
+    return std::sqrt(L.dd->reduce(r_, Which::curr, Sum::exact).sumsq);
+  }
+
+  // cycles until ||f - A u||_2 <= rtol ||f||_2 or max_cycles; the norm before the first cycle and after each
+  std::vector<double> solve(double rtol, int max_cycles) {
+    Level &L = levels_[0];
+    const double target = rtol * std::sqrt(L.dd->reduce(L.f, Which::curr, Sum::exact).sumsq);
+    std::vector<double> hist{residual_norm()};
+    while (hist.back() > target && int(hist.size()) - 1 < max_cycles) {
+      cycle();
+      hist.push_back(residual_norm());
+    }
+    return hist;
+  }
+
+private:
+  struct Level {
+    DistributedDomain *dd;
+    std::unique_ptr<DistributedDomain> owned; // the coarse levels
+    DataHandle<T> u, f;
+    LinearStencil gs, res;
+  };
+  int nu1_, nu2_, coarse_sweeps_, colours_ = 0;
+  DataHandle<T> r_;
+  std::vector<Level> levels_;
+
+  static LinearStencil residual(const LinearStencil &A) {
+    LinearStencil res;
+    res.add(Source::aux, 0, 0, 0, 1.0);
+    for (const sb_stencil_term &t : A.terms()) res.add(Source::src, t.offset[0], t.offset[1], t.offset[2], -t.weight);
+    return res;
+  }
+
+  void smooth(Level &L, int sweeps) {
+    for (int k = 0; k < sweeps; ++k)
+      for (int c = 0; c < colours_; ++c) L.dd->apply(L.gs, curr(L.u), L.u, curr(L.f), Colour{colours_, c});
+  }
+
+  void vcycle(size_t l) {
+    Level &L = levels_[l];
+    if (l + 1 == levels_.size()) {
+      smooth(L, coarse_sweeps_);
+      return;
+    }
+    smooth(L, nu1_);
+    Level &C = levels_[l + 1];
+    L.dd->restrict_to(*C.dd, curr(C.f), L.res, L.u, curr(L.f));
+    // coarse u <- +0: a memset of the curr allocation (an exchange refills the ghost cells before any read)
+    C.dd->queue_after_exterior();
+    for (size_t di = 0; di < C.dd->domains_.size(); ++di) {
+      LocalDomain &d = C.dd->domains_[di];
+      d.set_device();
+      const cudaPitchedPtr p = d.curr_data(C.u.id());
+      CUDA_RUNTIME(cudaMemsetAsync(p.ptr, 0, p.pitch * p.ysize * size_t(d.raw_size().z), C.dd->applyStreams_[2 * di]));
+    }
+    vcycle(l + 1);
+    L.dd->prolong_from(*C.dd, curr(L.u), curr(C.u), curr(L.u));
+    smooth(L, nu2_);
+  }
+};
+
+} // namespace stencil

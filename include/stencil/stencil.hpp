@@ -51,7 +51,13 @@ struct sb_reduce_exact_plan;
 struct sb_stencil_plan;
 struct sb_transfer_plan;
 
+namespace stencil {
+template <typename T> class Multigrid;
+}
+
 class DistributedDomain {
+  template <typename T> friend class stencil::Multigrid;
+
 private:
   Dim3 size_; // compute extent of the whole grid
 
@@ -148,13 +154,31 @@ private:
   void run_stencil_plans(const std::vector<int64_t> &key, bool exchange, bool writes_src,
                          const std::function<sb_stencil_plan *(size_t, const std::vector<Rect3> &)> &make);
 
+  // The queued schedule (the multigrid solver's, DESIGN.md section 2.11): while queued_ is set, run_stencil_plans and
+  // transfer issue the same launches but return at once, ordered by CUDA events only.  Each interior (or whole-region
+  // launch) waits for the previous exterior of its subdomain; queue_exchange() makes every exchange stream wait for every
+  // local apply stream before exchange_async(), so an exchange neither sends a value still being written nor overwrites
+  // a ghost cell an earlier launch still reads (and, across ranks, signals its neighbours only after those waits);
+  // wait_exchange(other, interior) makes this domain's exterior (and interior) apply streams wait for other's exchange.
+  bool queued_ = false;
+  bool sharedApplyStreams_ = false; // applyStreams_ belong to another domain (a solver's finer level)
+  std::vector<cudaEvent_t> applyEvents_, exchangeEvents_; // one per apply / exchange stream, recorded again on each use
+  void queue_after_exterior();
+  void queue_exchange();
+  void wait_exchange(DistributedDomain &other, bool interior);
+  void ensure_queue_events();
+  // the queued form of the interior / exchange / exterior schedule: launch(domain, part, stream), part 0 the interior (or
+  // the whole region without exchange), 1 the exterior
+  void queued_schedule(const std::function<void(size_t, int, cudaStream_t)> &launch, bool exchange);
+
   // multigrid transfers: per (coarse domain, kind, buffers, the swap parity of both domains), one plan per local domain.
   // serial_ names a domain for the lifetime of the process (an address can be reused by a later domain)
   uint64_t serial_;
   std::map<std::vector<int64_t>, std::vector<sb_transfer_plan *>> transferPlans_;
   std::set<std::pair<uint64_t, bool>> paired_; // (coarse serial, with ghosts) that passed the pairing check
+  // op: the fused residual-restriction (sb_transfer_oplan_create; restriction only), with apply's schedule when exchange
   void transfer(DistributedDomain &coarse, bool prolong, int dtype, size_t dq, stencil::Which dw, size_t sq, stencil::Which sw, int64_t aq,
-                stencil::Which aw, bool exchange);
+                stencil::Which aw, bool exchange, const stencil::LinearStencil *op = nullptr);
   void check_pairing(DistributedDomain &coarse, bool ghosts);
   void destroy_transfer_plans();
   void create_apply_streams(); // two per local domain (interior, exterior), on first use
@@ -387,6 +411,21 @@ public:
   //     fine.prolong_from(coarse, stencil::curr(u), stencil::curr(e), stencil::curr(u));
   template <typename T> void restrict_to(DistributedDomain &coarse, const stencil::Buffer<T> &dst, const stencil::Buffer<T> &src) {
     transfer(coarse, false, stencil::bc_dtype<T>(), dst.h.id(), dst.which, src.h.id(), src.which, -1, stencil::Which::curr, false);
+  }
+  // restrict_to with an op (DESIGN.md section 2.11): dst = the 8-cell average of op(src, aux), the fine values never
+  // stored; op has plain terms of reach <= 1, src is a curr buffer (its ghost cells are read).  exchange = true: the
+  // coarse interior (the compute region cut by 1) runs while exchange() fills the ghost cells, then the exterior slabs;
+  // exchange = false: one launch, the caller guarantees the ghost cells.  The op is part of the plan key.
+  //     fine.restrict_to(coarse, stencil::curr(f2), residual, u, stencil::curr(f));   // f2 = R (f - A u)
+  template <typename T>
+  void restrict_to(DistributedDomain &coarse, const stencil::Buffer<T> &dst, const stencil::LinearStencil &op, const DataHandle<T> &src,
+                   const stencil::Buffer<T> &aux, bool exchange = true) {
+    transfer(coarse, false, stencil::bc_dtype<T>(), dst.h.id(), dst.which, src.id(), stencil::Which::curr, int64_t(aux.h.id()), aux.which, exchange, &op);
+  }
+  template <typename T>
+  void restrict_to(DistributedDomain &coarse, const stencil::Buffer<T> &dst, const stencil::LinearStencil &op, const DataHandle<T> &src,
+                   bool exchange = true) {
+    transfer(coarse, false, stencil::bc_dtype<T>(), dst.h.id(), dst.which, src.id(), stencil::Which::curr, -1, stencil::Which::curr, exchange, &op);
   }
   template <typename T>
   void prolong_from(DistributedDomain &coarse, const stencil::Buffer<T> &dst, const stencil::Buffer<T> &src, bool exchange = true) {

@@ -542,6 +542,26 @@ int sb_transfer_plan_create(sb_transfer_plan **out, int device, int dtype, int k
 int sb_transfer_plan_launch(sb_transfer_plan *plan, void *stream);
 int64_t sb_transfer_plan_bytes(const sb_transfer_plan *plan);
 int sb_transfer_plan_destroy(sb_transfer_plan *plan);
+/* Fused residual-restriction (DESIGN.md section 2.11): a plain op (the rule of sb_stencil_plan_create, terms on src and
+ * aux) of reach <= 1 on every axis, evaluated on the fine grid and restricted without storing the fine values.  For
+ * each coarse cell I of the boxes:
+ *   v(p) = op(p) for the eight fine cells p = 2I + d, by the linear stencil rule above, in T, no FMA contraction
+ *   C[I] = the restriction above of those eight values, in its order, times T(0.125)
+ * The result is the bits of sb_stencil_plan over the fine footprint into a scratch allocation followed by
+ * SB_TRANSFER_RESTRICT.  For multigrid the op is the residual: (aux, 0, 1), then (src, o, -w) for each term of A.
+ * dst is coarse; src and aux (ptr NULL: none; needed when a term reads aux) are fine and share src's pitch and row
+ * count; each acc_origin is the global coordinate of its allocation's element (0,0,0).  nbox boxes [lo, hi) of coarse
+ * global coordinates (nbox * 3 int64 each).  Boxes of at least 4 coarse cells on every axis go to a z-marching tile
+ * kernel, one launch each; thinner boxes share one-thread-per-coarse-cell launches of up to 16 boxes.  Launch, bytes
+ * (per coarse cell of the boxes: 8 x (one src element, plus one aux element if a term reads aux), plus one coarse
+ * element written) and destroy go through sb_transfer_plan_*.  Errors (SB_ERR_INVALID with a message, before anything
+ * is allocated): an unknown dtype, an invalid term list, an offset beyond 1 cell, an aux term without aux, a NULL dst
+ * or src, dst equal to src or aux, aux with another pitch or row count than src, a pointer or pitch that is not a
+ * multiple of the element size, lo > hi, a box outside dst's allocation, and fine reads [2 lo - 1, 2 hi + 1) that leave
+ * src's allocation on some axis. */
+int sb_transfer_oplan_create(sb_transfer_plan **out, int device, int dtype, const sb_stencil_term *terms, int n, sb_pitched dst,
+                             const int64_t dst_acc_origin[3], int64_t dst_zsize, sb_pitched src, const int64_t src_acc_origin[3],
+                             int64_t src_zsize, sb_pitched aux, int nbox, const int64_t *lo, const int64_t *hi);
 
 /* ---------------------------------------------------------------------------------------------
  * 7-point jacobi step (the reference's user kernel, bin/jacobi3d.cu:40-85) over a region.

@@ -651,11 +651,21 @@ void DistributedDomain::destroy_stencil_plans() {
     for (auto &per_dom : kv.second)
       for (sb_stencil_plan *p : per_dom) sb_stencil_plan_destroy(p);
   stencilPlans_.clear();
-  for (size_t i = 0; i < applyStreams_.size(); ++i) {
+  for (size_t i = 0; i < applyStreams_.size() && !sharedApplyStreams_; ++i) {
     cudaSetDevice(domains_[i / 2].gpu());
     cudaStreamDestroy(applyStreams_[i]);
   }
   applyStreams_.clear();
+  for (size_t i = 0; i < applyEvents_.size(); ++i) {
+    cudaSetDevice(domains_[i / 2].gpu());
+    cudaEventDestroy(applyEvents_[i]);
+  }
+  applyEvents_.clear();
+  for (size_t i = 0; i < exchangeEvents_.size(); ++i) {
+    cudaSetDevice(domains_[i].gpu());
+    cudaEventDestroy(exchangeEvents_[i]);
+  }
+  exchangeEvents_.clear();
 }
 
 void DistributedDomain::apply_op(const stencil::LinearStencil &op, int dtype, size_t dq, stencil::Which dw, size_t sq, int64_t aq,
@@ -793,6 +803,12 @@ void DistributedDomain::run_stencil_plans(const std::vector<int64_t> &key, bool 
   }
   create_apply_streams();
   const std::vector<std::vector<sb_stencil_plan *>> &plans = found->second;
+  if (queued_) {
+    queued_schedule([&](size_t di, int part, cudaStream_t s) {
+      if (SB_OK != sb_stencil_plan_launch(plans[di][size_t(part)], s)) LOG_FATAL("apply: " << sb_last_error());
+    }, exchange);
+    return;
+  }
   for (size_t di = 0; di < domains_.size(); ++di)
     if (SB_OK != sb_stencil_plan_launch(plans[di][0], applyStreams_[2 * di])) LOG_FATAL("apply: " << sb_last_error());
   if (exchange) {
@@ -804,6 +820,76 @@ void DistributedDomain::run_stencil_plans(const std::vector<int64_t> &key, bool 
     domains_[di].set_device();
     CUDA_RUNTIME(cudaStreamSynchronize(applyStreams_[2 * di]));
     CUDA_RUNTIME(cudaStreamSynchronize(applyStreams_[2 * di + 1]));
+  }
+}
+
+void DistributedDomain::ensure_queue_events() {
+  create_apply_streams();
+  for (size_t i = applyEvents_.size(); i < applyStreams_.size(); ++i) {
+    CUDA_RUNTIME(cudaSetDevice(domains_[i / 2].gpu()));
+    cudaEvent_t e;
+    CUDA_RUNTIME(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    applyEvents_.push_back(e);
+  }
+  for (size_t i = exchangeEvents_.size(); i < streams_.size(); ++i) {
+    CUDA_RUNTIME(cudaSetDevice(domains_[i].gpu()));
+    cudaEvent_t e;
+    CUDA_RUNTIME(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    exchangeEvents_.push_back(e);
+  }
+}
+
+void DistributedDomain::queue_after_exterior() {
+  ensure_queue_events();
+  for (size_t di = 0; di < domains_.size(); ++di) {
+    CUDA_RUNTIME(cudaSetDevice(domains_[di].gpu()));
+    CUDA_RUNTIME(cudaEventRecord(applyEvents_[2 * di + 1], applyStreams_[2 * di + 1]));
+    CUDA_RUNTIME(cudaStreamWaitEvent(applyStreams_[2 * di], applyEvents_[2 * di + 1], 0));
+  }
+}
+
+void DistributedDomain::queue_exchange() {
+  ensure_queue_events();
+  for (size_t i = 0; i < applyStreams_.size(); ++i) {
+    CUDA_RUNTIME(cudaSetDevice(domains_[i / 2].gpu()));
+    CUDA_RUNTIME(cudaEventRecord(applyEvents_[i], applyStreams_[i]));
+  }
+  for (size_t di = 0; di < streams_.size(); ++di) {
+    CUDA_RUNTIME(cudaSetDevice(domains_[di].gpu()));
+    for (cudaEvent_t e : applyEvents_) CUDA_RUNTIME(cudaStreamWaitEvent(streams_[di], e, 0));
+  }
+  exchange_async();
+}
+
+void DistributedDomain::wait_exchange(DistributedDomain &other, bool interior) {
+  ensure_queue_events();
+  other.ensure_queue_events();
+  for (size_t di = 0; di < other.streams_.size(); ++di) {
+    CUDA_RUNTIME(cudaSetDevice(other.domains_[di].gpu()));
+    CUDA_RUNTIME(cudaEventRecord(other.exchangeEvents_[di], other.streams_[di]));
+  }
+  for (size_t di = 0; di < domains_.size(); ++di) {
+    CUDA_RUNTIME(cudaSetDevice(domains_[di].gpu()));
+    for (cudaEvent_t e : other.exchangeEvents_) {
+      CUDA_RUNTIME(cudaStreamWaitEvent(applyStreams_[2 * di + 1], e, 0));
+      if (interior) CUDA_RUNTIME(cudaStreamWaitEvent(applyStreams_[2 * di], e, 0));
+    }
+  }
+}
+
+void DistributedDomain::queued_schedule(const std::function<void(size_t, int, cudaStream_t)> &launch, bool exchange) {
+  queue_after_exterior();
+  if (exchange) queue_exchange(); // waits for the apply streams as they are before this interior
+  for (size_t di = 0; di < domains_.size(); ++di) {
+    domains_[di].set_device();
+    launch(di, 0, applyStreams_[2 * di]);
+  }
+  if (exchange) {
+    wait_exchange(*this, false);
+    for (size_t di = 0; di < domains_.size(); ++di) {
+      domains_[di].set_device();
+      launch(di, 1, applyStreams_[2 * di + 1]);
+    }
   }
 }
 
@@ -865,7 +951,7 @@ void DistributedDomain::check_pairing(DistributedDomain &coarse, bool ghosts) {
 }
 
 void DistributedDomain::transfer(DistributedDomain &coarse, bool prolong, int dtype, size_t dq, stencil::Which dw, size_t sq, stencil::Which sw,
-                                 int64_t aq, stencil::Which aw, bool exchange) {
+                                 int64_t aq, stencil::Which aw, bool exchange, const stencil::LinearStencil *op) {
   using stencil::Which;
   const char *name = prolong ? "prolong_from" : "restrict_to";
   if (&coarse == this) LOG_FATAL(name << ": coarse must be another DistributedDomain");
@@ -877,14 +963,63 @@ void DistributedDomain::transfer(DistributedDomain &coarse, bool prolong, int dt
   if (sq >= S.dataDtype_.size() || S.dataDtype_[sq] != dtype) LOG_FATAL(name << ": src " << sq << " is not a quantity of that type");
   if (aq >= 0 && (size_t(aq) >= dataDtype_.size() || dataDtype_[size_t(aq)] != dtype)) LOG_FATAL(name << ": aux " << aq << " is not a quantity of that type");
   if (prolong && sw != Which::curr) LOG_FATAL(name << ": src must be a curr buffer (the one coarse.exchange() fills)");
+  const bool split = op && exchange; // the fused restriction with apply's schedule: interior and exterior plans
+  std::vector<int64_t> key = {int64_t(coarse.serial_), int64_t(prolong), int64_t(dq), int64_t(dw == Which::next), int64_t(sq),
+                              int64_t(sw == Which::next), aq, int64_t(aw == Which::next), parity_, coarse.parity_};
+  if (op) {
+    if (prolong) LOG_FATAL(name << ": only a restriction takes an op");
+    if (op->ncoef() > 0) LOG_FATAL(name << ": the op has coefficient terms; the fused restriction takes plain terms");
+    if (sw != Which::curr) LOG_FATAL(name << ": with an op, src must be a curr buffer (the one exchange() fills)");
+    if (op->has_aux() && aq < 0) LOG_FATAL(name << ": the op has a term on aux, but no aux buffer was given");
+    int64_t r27[27];
+    for (int z = -1, i = 0; z <= 1; ++z)
+      for (int y = -1; y <= 1; ++y)
+        for (int x = -1; x <= 1; ++x) r27[i++] = int64_t(radius_.dir(x, y, z));
+    if (SB_OK != sb_stencil_check(op->terms().data(), int(op->terms().size()), r27)) LOG_FATAL(name << ": " << sb_last_error());
+    if (!op->has_aux()) {
+      aq = -1;
+      key[6] = -1;
+      key[7] = 0;
+    }
+    key.push_back(int64_t(exchange));
+    for (const sb_stencil_term &t : op->terms()) {
+      int64_t wbits;
+      std::memcpy(&wbits, &t.weight, 8);
+      key.insert(key.end(), {t.source, t.offset[0], t.offset[1], t.offset[2], wbits});
+    }
+  }
   check_pairing(coarse, prolong);
-  const std::vector<int64_t> key = {int64_t(coarse.serial_), int64_t(prolong), int64_t(dq), int64_t(dw == Which::next), int64_t(sq),
-                                    int64_t(sw == Which::next), aq, int64_t(aw == Which::next), parity_, coarse.parity_};
   auto found = transferPlans_.find(key);
   if (found == transferPlans_.end()) {
     auto pick = [](LocalDomain &d, size_t q, Which w) { return as_sb(w == Which::curr ? d.curr_data(q) : d.next_data(q)); };
-    std::vector<sb_transfer_plan *> per_dom;
-    for (size_t di = 0; di < domains_.size(); ++di) {
+    std::vector<sb_transfer_plan *> per_dom; // per local domain: one plan, or (interior, exterior) when split
+    Radius one = Radius::constant(1);
+    for (size_t di = 0; di < domains_.size() && op; ++di) {
+      LocalDomain &f = domains_[di], &cd = coarse.domains_[di];
+      int64_t dacc[3], sacc[3];
+      set3(dacc, cd.origin() - Dim3(coarse.radius_.x(-1), coarse.radius_.y(-1), coarse.radius_.z(-1)));
+      set3(sacc, f.origin() - Dim3(radius_.x(-1), radius_.y(-1), radius_.z(-1)));
+      const sb_pitched aux = aq < 0 ? sb_pitched{nullptr, 0, 0} : pick(f, size_t(aq), aw);
+      const Rect3 compute = cd.get_compute_region();
+      std::vector<std::vector<Rect3>> parts;
+      if (split)
+        parts = {{stencil::geom::interior(compute, one)}, stencil::geom::exterior(compute, one)};
+      else
+        parts = {{compute}};
+      for (const std::vector<Rect3> &boxes : parts) {
+        std::vector<int64_t> lo, hi;
+        for (const Rect3 &b : boxes) {
+          lo.insert(lo.end(), {b.lo.x, b.lo.y, b.lo.z});
+          hi.insert(hi.end(), {b.hi.x, b.hi.y, b.hi.z});
+        }
+        sb_transfer_plan *p = nullptr;
+        if (SB_OK != sb_transfer_oplan_create(&p, f.gpu(), dtype, op->terms().data(), int(op->terms().size()), pick(cd, dq, dw), dacc,
+                                              cd.raw_size().z, pick(f, sq, sw), sacc, f.raw_size().z, aux, int(boxes.size()), lo.data(), hi.data()))
+          LOG_FATAL(name << ": " << sb_last_error());
+        per_dom.push_back(p);
+      }
+    }
+    for (size_t di = 0; di < domains_.size() && !op; ++di) {
       LocalDomain &f = domains_[di], &dd = prolong ? f : coarse.domains_[di], &sd = prolong ? coarse.domains_[di] : f;
       int64_t dacc[3], sacc[3], lo[3], hi[3];
       set3(dacc, dd.origin() - Dim3(D.radius_.x(-1), D.radius_.y(-1), D.radius_.z(-1)));
@@ -901,13 +1036,30 @@ void DistributedDomain::transfer(DistributedDomain &coarse, bool prolong, int dt
     }
     found = transferPlans_.emplace(key, std::move(per_dom)).first;
   }
-  if (prolong && exchange) coarse.exchange();
   create_apply_streams();
-  for (size_t di = 0; di < domains_.size(); ++di)
-    if (SB_OK != sb_transfer_plan_launch(found->second[di], applyStreams_[2 * di])) LOG_FATAL(name << ": " << sb_last_error());
+  const std::vector<sb_transfer_plan *> &plans = found->second;
+  const size_t per = split ? 2 : 1;
+  auto launch = [&](size_t di, int part, cudaStream_t s) {
+    if (SB_OK != sb_transfer_plan_launch(plans[per * di + size_t(part)], s)) LOG_FATAL(name << ": " << sb_last_error());
+  };
+  if (queued_) {
+    if (prolong && exchange) {
+      coarse.queue_exchange();
+      wait_exchange(coarse, true);
+    }
+    queued_schedule(launch, split);
+    return;
+  }
+  if (prolong && exchange) coarse.exchange();
+  for (size_t di = 0; di < domains_.size(); ++di) launch(di, 0, applyStreams_[2 * di]);
+  if (split) {
+    this->exchange(); // returns when every ghost cell of this rank is filled
+    for (size_t di = 0; di < domains_.size(); ++di) launch(di, 1, applyStreams_[2 * di + 1]);
+  }
   for (size_t di = 0; di < domains_.size(); ++di) {
     domains_[di].set_device();
     CUDA_RUNTIME(cudaStreamSynchronize(applyStreams_[2 * di]));
+    CUDA_RUNTIME(cudaStreamSynchronize(applyStreams_[2 * di + 1]));
   }
 }
 

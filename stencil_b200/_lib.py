@@ -251,6 +251,11 @@ _SIGS = {
         C.c_int,
         [C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, Pitched, I3, C.c_int64, Pitched, I3, C.c_int64, Pitched, I3, I3],
     ),
+    "sb_transfer_oplan_create": (
+        C.c_int,
+        [C.POINTER(C.c_void_p), C.c_int, C.c_int, C.POINTER(StencilTerm), C.c_int, Pitched, I3, C.c_int64, Pitched, I3, C.c_int64, Pitched,
+         C.c_int, C.POINTER(C.c_int64), C.POINTER(C.c_int64)],
+    ),
     "sb_transfer_plan_launch": (C.c_int, [C.c_void_p, C.c_void_p]),
     "sb_transfer_plan_bytes": (C.c_int64, [C.c_void_p]),
     "sb_transfer_plan_destroy": (C.c_int, [C.c_void_p]),

@@ -362,6 +362,11 @@ struct sb_transfer_plan {
   sb::RestrictParams r{};
   sb::ProlongParams pr{};
   int grid = 0; // prolongation CTAs
+  bool fused = false; // sb_transfer_oplan_create: the launches below instead
+  std::vector<sb::RopTileParams> rop_tiles; // one tile-kernel launch per thick box
+  std::vector<int> rop_tile_grids;
+  std::vector<sb::RopCellParams> rop_cells; // one cell-kernel launch per group of thin boxes
+  std::vector<int> rop_cell_grids;
   int64_t bytes = 0;
 };
 
@@ -2192,13 +2197,165 @@ int sb_transfer_plan_create(sb_transfer_plan **out, int device, int dtype, int k
   return SB_OK;
 }
 
+int sb_transfer_oplan_create(sb_transfer_plan **out, int device, int dtype, const sb_stencil_term *terms, int n, sb_pitched dst,
+                             const int64_t dst_acc_origin[3], int64_t dst_zsize, sb_pitched src, const int64_t src_acc_origin[3],
+                             int64_t src_zsize, sb_pitched aux, int nbox, const int64_t *lo, const int64_t *hi) {
+  if (!out) return fail(SB_ERR_INVALID, "sb_transfer_oplan_create needs an output handle");
+  if (dtype != SB_DTYPE_F32 && dtype != SB_DTYPE_F64) return fail(SB_ERR_INVALID, "dtype %d must be SB_DTYPE_F32 or SB_DTYPE_F64", dtype);
+  const int es = dtype == SB_DTYPE_F32 ? 4 : 8;
+  const std::vector<sb_stencil_vterm> vt = stencil_vterms_of(terms, n);
+  int rc = stencil_terms_ok(terms ? vt.data() : nullptr, n);
+  if (rc != SB_OK) return rc;
+  bool aux_term = false;
+  for (int t = 0; t < n; ++t) {
+    aux_term = aux_term || terms[t].source == 1;
+    for (int a = 0; a < 3; ++a)
+      if (terms[t].offset[a] < -1 || terms[t].offset[a] > 1)
+        return fail(SB_ERR_INVALID, "term %d: offset (%d, %d, %d) reaches beyond 1 cell, the fused restriction's limit", t,
+                    int(terms[t].offset[0]), int(terms[t].offset[1]), int(terms[t].offset[2]));
+  }
+  if (aux_term && !aux.ptr) return fail(SB_ERR_INVALID, "a term reads aux, but aux is NULL");
+  if (!dst.ptr || !src.ptr) return fail(SB_ERR_INVALID, "dst and src must not be NULL");
+  if (dst.ptr == src.ptr) return fail(SB_ERR_INVALID, "dst must not be src");
+  if (aux_term && dst.ptr == aux.ptr) return fail(SB_ERR_INVALID, "dst must not be aux");
+  if (!dst_acc_origin || !src_acc_origin) return fail(SB_ERR_INVALID, "sb_transfer_oplan_create needs both acc_origins");
+  if (nbox < 0 || (nbox > 0 && (!lo || !hi))) return fail(SB_ERR_INVALID, "nbox %d boxes need lo and hi arrays", nbox);
+  if (dst_zsize < 1 || src_zsize < 1) return fail(SB_ERR_INVALID, "dst_zsize and src_zsize must be >= 1");
+  rc = stencil_buffers_ok({&dst}, {"dst"}, dst, "dst", es);
+  if (rc == SB_OK) rc = stencil_buffers_ok({&src}, {"src"}, src, "src", es);
+  if (rc == SB_OK && aux_term) rc = stencil_buffers_ok({&aux}, {"aux"}, src, "src", es);
+  if (rc != SB_OK) return rc;
+  const int64_t dsize[3] = {dst.pitch / es, dst.ysize, dst_zsize}, ssize[3] = {src.pitch / es, src.ysize, src_zsize};
+  const int zero[3] = {0, 0, 0}, one[3] = {1, 1, 1};
+  // per box: coarse lo, extent (dst allocation coordinates), fine 2 * lo (src allocation coordinates)
+  std::vector<std::array<int, 9>> thick, thin;
+  int64_t cells = 0;
+  for (int b = 0; b < nbox; ++b) {
+    int64_t l[3], e[3], fl[3], fe[3];
+    bool empty = false;
+    for (int a = 0; a < 3; ++a) {
+      if (lo[3 * b + a] > hi[3 * b + a]) return fail(SB_ERR_INVALID, "box %d: lo > hi on axis %c", b, "xyz"[a]);
+      l[a] = lo[3 * b + a] - dst_acc_origin[a];
+      e[a] = hi[3 * b + a] - lo[3 * b + a];
+      fl[a] = 2 * lo[3 * b + a] - src_acc_origin[a];
+      fe[a] = 2 * e[a];
+      empty = empty || e[a] == 0;
+    }
+    if (empty) continue;
+    if ((rc = stencil_box_reads_ok(b, l, e, zero, zero, dsize, "dst is written at")) != SB_OK) return rc;
+    if ((rc = stencil_box_reads_ok(b, fl, fe, one, one, ssize, "the fused restriction reads fine")) != SB_OK) return rc;
+    if (e[0] * e[1] * e[2] >= (1ll << 32)) return fail(SB_ERR_INVALID, "box %d: more than 2^32 cells", b);
+    cells += e[0] * e[1] * e[2];
+    const std::array<int, 9> B = {int(l[0]), int(l[1]), int(l[2]), int(e[0]), int(e[1]), int(e[2]), int(fl[0]), int(fl[1]), int(fl[2])};
+    (e[0] >= 4 && e[1] >= 4 && e[2] >= 4 ? thick : thin).push_back(B);
+  }
+
+  sb::RopCommon com{};
+  com.dst = static_cast<char *>(dst.ptr);
+  com.src = static_cast<const char *>(src.ptr);
+  com.aux = aux_term ? static_cast<const char *>(aux.ptr) : nullptr;
+  com.dpitch = dst.pitch;
+  com.dslice = dst.pitch * dst.ysize;
+  com.spitch = src.pitch;
+  com.sslice = src.pitch * src.ysize;
+  com.n = n;
+  for (int t = 0; t < n; ++t) {
+    com.source[t] = (signed char)terms[t].source;
+    for (int a = 0; a < 3; ++a) com.off[t][a] = (signed char)terms[t].offset[a];
+    com.w[t] = terms[t].weight;
+    com.wf[t] = float(terms[t].weight); // round to nearest
+  }
+  sb_transfer_plan *p = new sb_transfer_plan();
+  p->device = device;
+  p->es = es;
+  p->kind = SB_TRANSFER_RESTRICT;
+  p->fused = true;
+  p->bytes = cells * es * (8 * (aux_term ? 2 : 1) + 1);
+  if (cells == 0) {
+    *out = p;
+    return SB_OK;
+  }
+  DeviceGuard guard(device);
+  if (!guard.ok) {
+    delete p;
+    return fail(SB_ERR_NOGPU, "cannot select CUDA device %d", device);
+  }
+  int sms = 0;
+  if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device) != cudaSuccess) {
+    delete p;
+    return fail(SB_ERR_CUDA, "cudaDeviceGetAttribute: %s", cudaGetErrorString(cudaGetLastError()));
+  }
+  if (!thick.empty()) {
+    const int per_sm = sb::rop_tile_ctas_per_sm(es);
+    if (per_sm <= 0) {
+      delete p;
+      return fail(SB_ERR_CUDA, "the fused restriction's tile kernel cannot be configured: %s", cudaGetErrorString(cudaGetLastError()));
+    }
+    for (const auto &B : thick) {
+      sb::RopTileParams tp{};
+      tp.c = com;
+      for (int a = 0; a < 3; ++a) {
+        tp.lo[a] = B[a];
+        tp.ext[a] = B[3 + a];
+        tp.flo[a] = B[6 + a];
+        tp.rlo[a] = B[6 + a] - 1;
+        tp.rhi[a] = B[6 + a] + 2 * B[3 + a] + 1;
+      }
+      for (int c = 0; c < 3; ++c)
+        for (int t = 0; t < n; ++t) {
+          const int32_t *o = terms[t].offset;
+          tp.toff[c][t] = ((c + o[2] + 3) % 3) * sb::kRopPlane + o[1] * sb::kRopSW + o[0];
+        }
+      tp.tiles_x = (tp.ext[0] + sb::kRestrictX - 1) / sb::kRestrictX;
+      tp.tiles_y = (tp.ext[1] + sb::kRestrictY - 1) / sb::kRestrictY;
+      // z chunks: at least two waves of resident CTAs, no shorter than 4 coarse planes (each chunk reloads 2 fine planes)
+      const long long cols = (long long)tp.tiles_x * tp.tiles_y;
+      const long long want = (2ll * sms * per_sm + cols - 1) / cols;
+      int zc = int((tp.ext[2] + want - 1) / want);
+      zc = std::max(zc, std::min(4, tp.ext[2]));
+      tp.zchunk = zc;
+      const long long grid = cols * ((tp.ext[2] + zc - 1) / zc);
+      if (grid >= (1ll << 31)) {
+        delete p;
+        return fail(SB_ERR_INVALID, "box too large for the fused restriction's tile kernel");
+      }
+      p->rop_tiles.push_back(tp);
+      p->rop_tile_grids.push_back(int(grid));
+    }
+  }
+  for (size_t b0 = 0; b0 < thin.size(); b0 += sb::kRopMaxBoxes) {
+    sb::RopCellParams cp{};
+    cp.c = com;
+    cp.first[0] = 0;
+    for (size_t b = b0; b < thin.size() && b < b0 + sb::kRopMaxBoxes; ++b) {
+      const int m = cp.n++;
+      for (int a = 0; a < 3; ++a) {
+        cp.lo[m][a] = thin[b][a];
+        cp.ext[m][a] = thin[b][3 + a];
+        cp.flo[m][a] = thin[b][6 + a];
+      }
+      cp.first[m + 1] = cp.first[m] + (long long)thin[b][3] * thin[b][4] * thin[b][5];
+    }
+    p->rop_cells.push_back(cp);
+    p->rop_cell_grids.push_back(int(std::min<long long>((cp.first[cp.n] + 255) / 256, 32ll * sms)));
+  }
+  p->launches = int(p->rop_tiles.size() + p->rop_cells.size());
+  *out = p;
+  return SB_OK;
+}
+
 int sb_transfer_plan_launch(sb_transfer_plan *p, void *stream) {
   if (!p) return fail(SB_ERR_INVALID, "null plan");
   if (!p->launches) return SB_OK;
   DeviceGuard guard(p->device);
   if (!guard.ok) return fail(SB_ERR_NOGPU, "cannot select CUDA device %d", p->device);
   const cudaStream_t s = static_cast<cudaStream_t>(stream);
-  g_launches += uint64_t(p->kind == SB_TRANSFER_PROLONG ? sb::launch_prolong(p->pr, p->es, p->grid, s) : sb::launch_restrict(p->r, p->es, s));
+  if (p->fused) {
+    for (size_t i = 0; i < p->rop_tiles.size(); ++i) g_launches += uint64_t(sb::launch_rop_tile(p->rop_tiles[i], p->es, p->rop_tile_grids[i], s));
+    for (size_t i = 0; i < p->rop_cells.size(); ++i) g_launches += uint64_t(sb::launch_rop_cells(p->rop_cells[i], p->es, p->rop_cell_grids[i], s));
+  } else {
+    g_launches += uint64_t(p->kind == SB_TRANSFER_PROLONG ? sb::launch_prolong(p->pr, p->es, p->grid, s) : sb::launch_restrict(p->r, p->es, s));
+  }
   SB_CUDA(cudaGetLastError());
   return SB_OK;
 }

@@ -12,6 +12,17 @@
 // dst written as one 2-element vector when both children lie in the box and the pair is aligned, element by element
 // otherwise.  Only coarse cells the rule reads for a child of the box are loaded.
 //
+// rop_tile_kernel<T>: the fused residual-restriction (sb_transfer_oplan_create) over a thick box.  A CTA owns 32 x 8
+// coarse cells of a z chunk, one per thread, and marches the fine planes of their 64 x 16 footprint: planes z - 1 .. z + 1
+// of the footprint and its one-cell ring sit in a 3-slot shared ring, filled one plane ahead through registers (only
+// cells inside the checked read box [2 lo - 1, 2 hi + 1) are loaded).  On each fine plane a thread evaluates the op on
+// its coarse cell's four fine cells of that plane and adds them to its running sum in the rule's order, so the two
+// planes of a coarse cell give the eight values in order and the fine values are never stored.  A chunk starts at an
+// even fine plane.  aux is read from global memory as one pair per fine row (a vector where aligned), one plane ahead.
+//
+// rop_cell_kernel<T>: one thread per coarse cell over up to 16 thin boxes (the exterior slabs, one coarse cell thick),
+// every term read through the read-only path.
+//
 // Numerics: every multiply and add rounded separately (__fmul_rn / __fadd_rn, __dmul_rn / __dadd_rn; no FMA), in the
 // order of the rule in include/stencil_b200.h, so a cell's value does not depend on the launch shape or the partition.
 #include "transfer.cuh"
@@ -24,11 +35,13 @@ template <> struct TNum<float> {
   using V2 = float2;
   static __device__ __forceinline__ float mul(float a, float b) { return __fmul_rn(a, b); }
   static __device__ __forceinline__ float add(float a, float b) { return __fadd_rn(a, b); }
+  static __device__ __forceinline__ float w(const RopCommon &c, int t) { return c.wf[t]; }
 };
 template <> struct TNum<double> {
   using V2 = double2;
   static __device__ __forceinline__ double mul(double a, double b) { return __dmul_rn(a, b); }
   static __device__ __forceinline__ double add(double a, double b) { return __dadd_rn(a, b); }
+  static __device__ __forceinline__ double w(const RopCommon &c, int t) { return c.w[t]; }
 };
 
 template <typename T> __device__ __forceinline__ bool pair_aligned(const void *a) {
@@ -200,7 +213,176 @@ template <typename T> __global__ void __launch_bounds__(kProlongThreads) prolong
   }
 }
 
+template <typename T> __global__ void __launch_bounds__(kRestrictX * kRestrictY) rop_tile_kernel(const __grid_constant__ RopTileParams p) {
+  using N = TNum<T>;
+  constexpr long long ES = sizeof(T);
+  constexpr int NT = kRestrictX * kRestrictY;
+  constexpr int PER = (kRopPlane + NT - 1) / NT; // ring elements per thread and plane
+  __shared__ T ring[3][kRopPlane];
+
+  const int tid = threadIdx.x, lane = tid & 31, wy = tid >> 5;
+  int b = blockIdx.x;
+  const int bx = b % p.tiles_x;
+  b /= p.tiles_x;
+  const int by = b % p.tiles_y, bz = b / p.tiles_y;
+  const int k0 = bz * p.zchunk, k1 = min(k0 + p.zchunk, p.ext[2]); // the chunk's coarse planes, box-relative
+  if (k0 >= k1) return;
+  const int Z0 = p.flo[2] + 2 * k0, Z1 = p.flo[2] + 2 * k1;        // its fine planes, src allocation coordinates
+  const int WX = p.flo[0] + 2 * kRestrictX * bx - 1, WY = p.flo[1] + 2 * kRestrictY * by - 1; // ring window origin
+
+  T buf[PER];
+  auto fetch = [&](int z) {
+    const char *plane = p.c.src + (long long)z * p.c.sslice;
+#pragma unroll
+    for (int e = 0; e < PER; ++e) {
+      const int q = tid + e * NT;
+      const int r = q / kRopSW, col = q - r * kRopSW;
+      const int x = WX + col, y = WY + r;
+      buf[e] = T(0);
+      if (q < kRopPlane && x >= p.rlo[0] && x < p.rhi[0] && y >= p.rlo[1] && y < p.rhi[1])
+        buf[e] = __ldg(reinterpret_cast<const T *>(plane + y * p.c.spitch + x * ES));
+    }
+  };
+  auto store = [&](int z) {
+    T *pl = ring[(z - Z0 + 1) % 3];
+#pragma unroll
+    for (int e = 0; e < PER; ++e) {
+      const int q = tid + e * NT;
+      if (q < kRopPlane) pl[q] = buf[e];
+    }
+  };
+  fetch(Z0 - 1);
+  store(Z0 - 1);
+  fetch(Z0);
+  store(Z0);
+  fetch(Z0 + 1);
+
+  const int i = kRestrictX * bx + lane, j = kRestrictY * by + wy; // this thread's coarse cell, box-relative
+  const bool mine = i < p.ext[0] && j < p.ext[1];
+  const int fx = p.flo[0] + 2 * i, fy = p.flo[1] + 2 * j;
+  const int s00 = (2 * wy + 1) * kRopSW + 2 * lane + 1; // the fine cell (0, 0, .) in a ring slot
+  // aux of this thread's two fine rows, one plane ahead like the ring, so its latency hides behind a plane's work
+  T ax[2][2] = {{T(0), T(0)}, {T(0), T(0)}};
+  auto fetch_aux = [&](int z) {
+    if (mine && p.c.aux)
+#pragma unroll
+      for (int dy = 0; dy < 2; ++dy)
+        load_pair<T>(p.c.aux + (long long)z * p.c.sslice + (long long)(fy + dy) * p.c.spitch + fx * ES, ax[dy][0], ax[dy][1]);
+  };
+  fetch_aux(Z0);
+  T acc = T(0);
+  for (int zc = Z0; zc < Z1; ++zc) {
+    store(zc + 1);
+    __syncthreads();
+    if (zc + 1 < Z1) fetch(zc + 2);
+    const T a[2][2] = {{ax[0][0], ax[0][1]}, {ax[1][0], ax[1][1]}};
+    if (zc + 1 < Z1) fetch_aux(zc + 1);
+    if (mine) {
+      // the op on the four fine cells (dx, dy) of this plane, term by term (each term's table entry read once for all
+      // four), each cell's sum in list order; v[2 dy + dx]
+      const T *q0 = &ring[0][0] + s00;
+      const int *toff = p.toff[(zc - Z0 + 1) % 3];
+      T v[4];
+      for (int t = 0; t < p.c.n; ++t) {
+        const T w = N::w(p.c, t);
+        T m[4];
+        if (p.c.source[t] == 0) {
+          const T *q = q0 + toff[t];
+          m[0] = N::mul(w, q[0]);
+          m[1] = N::mul(w, q[1]);
+          m[2] = N::mul(w, q[kRopSW]);
+          m[3] = N::mul(w, q[kRopSW + 1]);
+        } else {
+#pragma unroll
+          for (int k = 0; k < 4; ++k) m[k] = N::mul(w, a[k >> 1][k & 1]);
+        }
+#pragma unroll
+        for (int k = 0; k < 4; ++k) v[k] = t == 0 ? m[k] : N::add(v[k], m[k]);
+      }
+      const bool first = ((zc - Z0) & 1) == 0;
+      acc = first ? v[0] : N::add(acc, v[0]);
+#pragma unroll
+      for (int k = 1; k < 4; ++k) acc = N::add(acc, v[k]);
+      if (!first)
+        *reinterpret_cast<T *>(p.c.dst + (long long)(p.lo[2] + (zc - p.flo[2]) / 2) * p.c.dslice + (long long)(p.lo[1] + j) * p.c.dpitch +
+                               (long long)(p.lo[0] + i) * ES) = N::mul(T(0.125), acc);
+    }
+    __syncthreads();
+  }
+}
+
+template <typename T> __global__ void __launch_bounds__(256) rop_cell_kernel(const __grid_constant__ RopCellParams p) {
+  using N = TNum<T>;
+  constexpr long long ES = sizeof(T);
+  const long long total = p.first[p.n];
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    int k = 0;
+    while (k + 1 < p.n && i >= p.first[k + 1]) ++k;
+    const unsigned li = (unsigned)(i - p.first[k]);
+    const unsigned ex = p.ext[k][0], ey = p.ext[k][1];
+    unsigned xx, yy, zz;
+    if (ex >= 32) { // x fastest
+      xx = li % ex;
+      const unsigned t = li / ex;
+      yy = t % ey;
+      zz = t / ey;
+    } else { // y fastest: an x slab is one column per row
+      yy = li % ey;
+      const unsigned t = li / ey;
+      xx = t % ex;
+      zz = t / ex;
+    }
+    const long long f0 = (long long)(p.flo[k][2] + 2 * (int)zz) * p.c.sslice + (long long)(p.flo[k][1] + 2 * (int)yy) * p.c.spitch +
+                         (long long)(p.flo[k][0] + 2 * (int)xx) * ES;
+    T acc = T(0);
+#pragma unroll
+    for (int d = 0; d < 8; ++d) { // the rule's order: x fastest, then y, then z
+      const long long f = f0 + (d >> 2) * p.c.sslice + ((d >> 1) & 1) * p.c.spitch + (d & 1) * ES;
+      const T a = p.c.aux ? __ldg(reinterpret_cast<const T *>(p.c.aux + f)) : T(0);
+      T v = T(0);
+      for (int t = 0; t < p.c.n; ++t) {
+        const signed char *o = p.c.off[t];
+        const T x = p.c.source[t] == 0 ? __ldg(reinterpret_cast<const T *>(p.c.src + f + o[2] * p.c.sslice + o[1] * p.c.spitch + o[0] * ES)) : a;
+        const T m = N::mul(N::w(p.c, t), x);
+        v = t == 0 ? m : N::add(v, m);
+      }
+      acc = d == 0 ? v : N::add(acc, v);
+    }
+    *reinterpret_cast<T *>(p.c.dst + (long long)(p.lo[k][2] + (int)zz) * p.c.dslice + (long long)(p.lo[k][1] + (int)yy) * p.c.dpitch +
+                           (long long)(p.lo[k][0] + (int)xx) * ES) = N::mul(T(0.125), acc);
+  }
+}
+
 } // namespace
+
+int rop_tile_ctas_per_sm(int es) {
+  int ctas = 0;
+  const void *fn = es == 4 ? reinterpret_cast<const void *>(&rop_tile_kernel<float>) : reinterpret_cast<const void *>(&rop_tile_kernel<double>);
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctas, fn, kRestrictX * kRestrictY, 0) != cudaSuccess) return 0;
+  return ctas;
+}
+
+int launch_rop_tile(const RopTileParams &p, int es, int grid, cudaStream_t stream) {
+  if (grid <= 0) return 0;
+  if (es == 4)
+    rop_tile_kernel<float><<<unsigned(grid), kRestrictX * kRestrictY, 0, stream>>>(p);
+  else if (es == 8)
+    rop_tile_kernel<double><<<unsigned(grid), kRestrictX * kRestrictY, 0, stream>>>(p);
+  else
+    return 0;
+  return 1;
+}
+
+int launch_rop_cells(const RopCellParams &p, int es, int grid, cudaStream_t stream) {
+  if (grid <= 0 || p.n <= 0) return 0;
+  if (es == 4)
+    rop_cell_kernel<float><<<unsigned(grid), 256, 0, stream>>>(p);
+  else if (es == 8)
+    rop_cell_kernel<double><<<unsigned(grid), 256, 0, stream>>>(p);
+  else
+    return 0;
+  return 1;
+}
 
 int launch_restrict(const RestrictParams &p, int es, cudaStream_t stream) {
   if (p.ext[0] <= 0 || p.ext[1] <= 0 || p.ext[2] <= 0) return 0;

@@ -38,9 +38,48 @@ struct ProlongParams {
 };
 static_assert(sizeof(ProlongParams) <= 4096, "the prolongation's parameters fit the classic 4 KB limit");
 
+// Fused residual-restriction (sb_transfer_oplan_create): a plain op of reach <= 1 evaluated on the eight fine cells of
+// each coarse cell and restricted, the fine values never stored.  Weights already rounded to T; off[t]: term t's offset.
+constexpr int kRopMaxTerms = 64;
+constexpr int kRopMaxBoxes = 16; // thin boxes per cell-kernel launch
+// tile kernel: a CTA of kRestrictX x kRestrictY threads owns as many coarse cells of a z chunk; the fine planes of its
+// 2kRestrictX x 2kRestrictY footprint and a one-cell ring pass through a 3-slot shared ring
+constexpr int kRopSW = 2 * kRestrictX + 2, kRopPlane = kRopSW * (2 * kRestrictY + 2);
+struct RopCommon {
+  char *dst;                  // coarse
+  const char *src, *aux;      // fine; aux shares src's pitch and rows (NULL: no aux term)
+  long long dpitch, dslice;   // dst
+  long long spitch, sslice;   // src and aux
+  int n;
+  signed char source[kRopMaxTerms];
+  signed char off[kRopMaxTerms][3];
+  double w[kRopMaxTerms];     // T(w) for T = double
+  float wf[kRopMaxTerms];     // T(w) for T = float
+};
+struct RopTileParams {
+  RopCommon c;
+  int lo[3], ext[3];          // the coarse box in dst's allocation coordinates
+  int flo[3];                 // the fine cell 2 * (global lo) in src's allocation coordinates
+  int rlo[3], rhi[3];         // the fine cells the plan checked, [flo - 1, flo + 2 ext + 1), in src's allocation coordinates
+  int zchunk, tiles_x, tiles_y;
+  int toff[3][kRopMaxTerms];  // shared-memory element offset of term t's src cell from the ring base, relative to the
+                              // cell's place in a slot, while the centre plane occupies ring slot c (precomputed by the plan)
+};
+static_assert(sizeof(RopTileParams) <= 4096, "the fused restriction's tile parameters fit the classic 4 KB limit");
+struct RopCellParams {
+  RopCommon c;
+  int n;                      // boxes
+  int lo[kRopMaxBoxes][3], ext[kRopMaxBoxes][3], flo[kRopMaxBoxes][3];
+  long long first[kRopMaxBoxes + 1];
+};
+static_assert(sizeof(RopCellParams) <= 4096, "the fused restriction's cell parameters fit the classic 4 KB limit");
+
 // Host: launch_* return the number of launches issued (0 on an empty box or an unknown element size).
 int launch_restrict(const RestrictParams &p, int es, cudaStream_t stream);
 int prolong_ctas_per_sm(int es);
 int launch_prolong(const ProlongParams &p, int es, int grid, cudaStream_t stream);
+int rop_tile_ctas_per_sm(int es);
+int launch_rop_tile(const RopTileParams &p, int es, int grid, cudaStream_t stream);
+int launch_rop_cells(const RopCellParams &p, int es, int grid, cudaStream_t stream);
 
 } // namespace sb

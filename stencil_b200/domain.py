@@ -366,6 +366,24 @@ class TransferPlan:
         self.device = device
         self.bytes = int(lib().sb_transfer_plan_bytes(h))
 
+    @classmethod
+    def fused(cls, device: int, op, dst: Pitched, dst_origin: Vec, dst_zsize: int, src: Pitched, src_origin: Vec, src_zsize: int,
+              aux: Optional[Pitched], boxes: Sequence[Tuple[Vec, Vec]]) -> "TransferPlan":
+        """sb_transfer_oplan_create: the fused residual-restriction, dst (coarse) = the restriction of op(src, aux) (fine;
+        aux shares src's layout) over the coarse boxes [lo, hi) (global coordinates); op is a StencilOp without
+        coefficient terms and of reach <= 1."""
+        nb = len(boxes)
+        lo = (C.c_int64 * (3 * max(1, nb)))(*[int(v) for b in boxes for v in b[0]])
+        hi = (C.c_int64 * (3 * max(1, nb)))(*[int(v) for b in boxes for v in b[1]])
+        h = C.c_void_p()
+        check(lib().sb_transfer_oplan_create(C.byref(h), device, op.dtype_code, op.c_terms(), len(op.terms), dst, i3(dst_origin), int(dst_zsize),
+                                             src, i3(src_origin), int(src_zsize), aux if aux is not None else Pitched(None, 0, 0), nb, lo, hi))
+        self = cls.__new__(cls)
+        self._h = h
+        self.device = device
+        self.bytes = int(lib().sb_transfer_plan_bytes(h))
+        return self
+
     def launch(self, stream=None) -> None:
         check(lib().sb_transfer_plan_launch(self._h, stream_ptr(stream)))
 
@@ -1286,6 +1304,10 @@ class DistributedDomain:
         Every src term with a non-zero offset must read another colour (op.check(radius, colours=m)).  In place the
         schedule is the same, with the interior cut by the larger radius of both sides of each axis, so that it writes
         no cell exchange() sends (a slab as wide as the opposite side's radius); the exterior runs after exchange()."""
+        self._run_plans(*self._apply_plans(op, dst, src, aux, exchange, coefs, colour))
+
+    def _apply_plans(self, op, dst, src, aux=None, exchange: bool = True, coefs=None, colour=None):
+        """apply()'s checks and cached plans, returned with its schedule as the arguments of _run_plans."""
         from .stencil_op import StencilOp, StencilPlan
 
         if not isinstance(op, StencilOp):
@@ -1332,7 +1354,7 @@ class DistributedDomain:
             K = [d.pitched(q, "curr") for q in c_q] if op.has_coef else None
             return StencilPlan(d.gpu(), op, *P, d.accessor_origin(), d.raw_size()[2], boxes, K, (ncol, col) if ncol > 1 else None)
 
-        self._run_plans(self._plans_for(key, exchange, make, writes_src=(d_q, d_w) == (s_q, s_w)), exchange)
+        return self._plans_for(key, exchange, make, writes_src=(d_q, d_w) == (s_q, s_w)), exchange
 
     def apply_system(self, system, outputs, inputs, exchange: bool = True) -> None:
         """outputs = system(inputs) over the whole compute region of every local subdomain (DESIGN.md section 2.8).
@@ -1410,13 +1432,17 @@ class DistributedDomain:
             self._stencil_plans[key] = plans
         return plans
 
-    def _run_plans(self, plans, exchange: bool) -> None:
+    def _run_plans(self, plans, exchange: bool, queued: bool = False) -> None:
         """The schedule of apply and apply_system: with exchange, every interior plan on its own stream while exchange()
-        fills the ghost cells, then every exterior plan; without, the one plan per domain.  Returns when all are done."""
+        fills the ghost cells, then every exterior plan; without, the one plan per domain.  Returns when all are done.
+        queued: the same launches, ordered by events only, and returns at once (_queue_plans)."""
         import torch
 
         if not self._apply_streams:
             self._apply_streams = [(torch.cuda.Stream(device=d.gpu()), torch.cuda.Stream(device=d.gpu())) for d in self.domains_]
+        if queued:
+            self._queue_plans(plans, exchange)
+            return
         for d, (si, se) in zip(self.domains_, self._apply_streams):  # after the work queued on the caller's stream
             si.wait_stream(torch.cuda.current_stream(d.gpu()))
             se.wait_stream(torch.cuda.current_stream(d.gpu()))
@@ -1440,16 +1466,90 @@ class DistributedDomain:
             si.synchronize()
             se.synchronize()
 
+    # -- the queued schedule (the multigrid solver's): nothing waits on the host, CUDA events order the launches
+    def _queue_plans(self, plans, exchange: bool) -> None:
+        """_run_plans without a host wait.  Each interior (or the one plan without exchange) waits for the previous
+        exterior on its subdomain's apply streams; with exchange, the exchange waits for every apply stream as they were
+        before this interior (_queue_exchange), and each exterior waits for the exchange."""
+        import torch
+
+        multi = len({d.gpu() for d in self.domains_}) > 1
+        apply_ev, _ = self._queue_events()
+        for (si, se), pair in zip(self._apply_streams, apply_ev):
+            pair[1].record(se)
+            si.wait_event(pair[1])
+        if exchange:
+            self._queue_exchange()
+        for d, p, (si, _) in zip(self.domains_, plans, self._apply_streams):
+            if multi:
+                _set_current_device(d.gpu())
+            p[0].launch(si)
+        if exchange:
+            self._wait_exchange(self, interior=False)
+            for d, p, (_, se) in zip(self.domains_, plans, self._apply_streams):
+                if multi:
+                    _set_current_device(d.gpu())
+                p[1].launch(se)
+
+    def _queue_events(self):
+        """The events of the queued schedule, created once and recorded again on each use (a wait takes the record made
+        before it): per local domain a pair for its apply streams, and one per exchange stream."""
+        import torch
+
+        ev = getattr(self, "_queue_ev", None)
+        if ev is None or len(ev[0]) != len(self._apply_streams):
+            ev = ([(torch.cuda.Event(), torch.cuda.Event()) for _ in self._apply_streams], [torch.cuda.Event() for _ in self._streams])
+            self._queue_ev = ev
+        return ev
+
+    def _queue_exchange(self) -> None:
+        """exchange() without a host wait.  Every exchange stream first waits for every local apply stream, on every GPU
+        of the process: the exchange then neither sends a value still being written nor overwrites a ghost cell an
+        earlier launch still reads, and across ranks the exchange signals its neighbours only after those waits."""
+        apply_ev, _ = self._queue_events()
+        for pair, evs in zip(self._apply_streams, apply_ev):
+            for st, ev in zip(pair, evs):
+                ev.record(st)
+        for x in self._streams:
+            for evs in apply_ev:
+                for ev in evs:
+                    x.wait_event(ev)
+        self.exchange_async()
+
+    def _wait_exchange(self, other: "DistributedDomain", interior: bool = True) -> None:
+        """Every exterior apply stream of this domain (and every interior one with interior=True) waits for the
+        exchange queued last on other's exchange streams."""
+        _, evs = other._queue_events()
+        for x, ev in zip(other._streams, evs):
+            ev.record(x)
+        for si, se in self._apply_streams:
+            for ev in evs:
+                se.wait_event(ev)
+                if interior:
+                    si.wait_event(ev)
+
     # -- multigrid transfers
-    def restrict_to(self, coarse: "DistributedDomain", dst, src) -> None:
+    def restrict_to(self, coarse: "DistributedDomain", dst, src, op=None, aux=None, exchange: bool = True) -> None:
         """dst (a quantity of coarse) = the 8-cell average of src (a quantity of this domain) over every coarse compute
         cell (DESIGN.md section 2.10).  Buffers follow apply(): a bare handle means "next" for dst and "curr" for src;
         src may be curr or next, as restriction reads no ghost cells.  coarse must pair with this domain: the same
         partition dim, every subdomain exactly twice as coarse, on the same rank and GPU (sb_transfer_check; checked
         once per coarse domain).  One launch per local subdomain on the apply streams, after the work queued on the
         caller's stream; returns when it is complete.  Plans are cached as prolong_from() describes.
-            fine.restrict_to(coarse, (f2, "curr"), (r, "curr"))"""
-        self._transfer(coarse, _lib.TRANSFER_RESTRICT, dst, src, None, False)
+            fine.restrict_to(coarse, (f2, "curr"), (r, "curr"))
+        op: a StencilOp (plain terms, reach <= 1): dst = the 8-cell average of op(src, aux), the fine values never
+        stored (DESIGN.md section 2.11), the same bits as apply() into a scratch quantity followed by restrict_to().
+        src must then be a curr buffer, as op reads its ghost cells; aux (a bare handle means "curr") is needed when a
+        term reads it.  exchange=True follows apply(): the coarse interior (the coarse compute region cut by 1, which
+        reads no fine ghost cell) runs while exchange() fills the ghost cells, then the exterior slabs; exchange=False:
+        one launch over the whole region, the caller guarantees the ghost cells.  The op is part of the plan key.
+            fine.restrict_to(coarse, (f2, "curr"), u, op=residual, aux=(f, "curr"))   # f2 = R (f - A u)"""
+        if op is None:
+            if aux is not None:
+                raise _lib.StencilError("restrict_to: aux is read only by an op")
+            self._transfer(coarse, _lib.TRANSFER_RESTRICT, dst, src, None, False)
+        else:
+            self._transfer(coarse, _lib.TRANSFER_RESTRICT, dst, src, aux, exchange, op)
 
     def prolong_from(self, coarse: "DistributedDomain", dst, src, aux=None, exchange: bool = True) -> None:
         """dst = aux + P src (or P src without aux) over every fine compute cell, P the trilinear interpolation from the
@@ -1462,7 +1562,10 @@ class DistributedDomain:
             fine.prolong_from(coarse, (u, "curr"), (e, "curr"), aux=(u, "curr"))"""
         self._transfer(coarse, _lib.TRANSFER_PROLONG, dst, src, aux, exchange)
 
-    def _transfer(self, coarse, kind: int, dst, src, aux, exchange: bool) -> None:
+    def _transfer(self, coarse, kind: int, dst, src, aux, exchange: bool, op=None, queued: bool = False) -> None:
+        """restrict_to / prolong_from; queued: the schedule of _run_plans(queued=True), for a solver that owns the cycle."""
+        from .stencil_op import StencilOp
+
         name = "restrict_to" if kind == _lib.TRANSFER_RESTRICT else "prolong_from"
         if not isinstance(coarse, DistributedDomain) or coarse is self:
             raise _lib.StencilError(f"{name}: coarse must be another DistributedDomain, not {coarse!r}")
@@ -1486,20 +1589,47 @@ class DistributedDomain:
             raise _lib.StencilError(f"{name}: dst, src and aux must all be float32 or all float64")
         if not restrict and s[1] != "curr":
             raise _lib.StencilError(f"{name}: src must be a curr buffer (the one coarse.exchange() fills)")
+        if op is not None:
+            if not isinstance(op, StencilOp) or op.has_coef:
+                raise _lib.StencilError(f"{name}: op must be a StencilOp without coefficient terms, not {op!r}")
+            if op.dtype != dtype:
+                raise _lib.StencilError(f"{name}: the op computes in {op.dtype}, the quantities are {dtype}")
+            if s[1] != "curr":
+                raise _lib.StencilError(f"{name}: with an op, src must be a curr buffer (the one exchange() fills)")
+            if op.has_aux and a is None:
+                raise _lib.StencilError(f"{name}: the op has a term on aux, but no aux buffer was given")
+            op.check(self.radius_)
+            a = a if op.has_aux else None
         self._check_pairing(coarse, not restrict)
-        key = (coarse, kind, d, s, a, self._parity, coarse._parity)
+        fused_exchange = op is not None and bool(exchange)
+        key = (coarse, kind, d, s, a, self._parity, coarse._parity) + ((op.key(), fused_exchange) if op is not None else ())
         plans = self._transfer_plans.get(key)
         if plans is None:
             plans = []
-            for fd, cd in zip(self.domains_, coarse.domains_):
+            if op is not None:
+                one = Radius.constant(1).c27()
+                boxes = list(zip(coarse.get_interior(one), coarse.get_exterior(one))) if fused_exchange else None
+            for di, (fd, cd) in enumerate(zip(self.domains_, coarse.domains_)):
                 dd, sd = (cd, fd) if restrict else (fd, cd)
+                if op is not None:
+                    args = (fd.gpu(), op, cd.pitched(*d), cd.accessor_origin(), cd.raw_size()[2], fd.pitched(*s), fd.accessor_origin(),
+                            fd.raw_size()[2], fd.pitched(*a) if a is not None else None)
+                    if fused_exchange:
+                        plans.append((TransferPlan.fused(*args, [boxes[di][0]]), TransferPlan.fused(*args, boxes[di][1])))
+                    else:
+                        plans.append((TransferPlan.fused(*args, [cd.get_compute_region()]),))
+                    continue
                 lo, hi = dd.get_compute_region()
                 plans.append((TransferPlan(fd.gpu(), dtype, kind, dd.pitched(*d), dd.accessor_origin(), dd.raw_size()[2], sd.pitched(*s),
                                            sd.accessor_origin(), sd.raw_size()[2], fd.pitched(*a) if a is not None else None, lo, hi),))
             self._transfer_plans[key] = plans
         if not restrict and exchange:
-            coarse.exchange()
-        self._run_plans(plans, False)
+            if queued:
+                coarse._queue_exchange()
+                self._wait_exchange(coarse)
+            else:
+                coarse.exchange()
+        self._run_plans(plans, fused_exchange, queued)
 
     def _check_pairing(self, coarse, ghosts: bool) -> None:
         """The pairing of sb_transfer_check over every subdomain index (global information, so every rank reaches the same

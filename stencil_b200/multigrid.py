@@ -1,0 +1,242 @@
+"""Geometric multigrid for A u = f on a DistributedDomain (DESIGN.md section 2.11): V(nu1, nu2) cycles over a hierarchy
+of coarsenings by 2, built from the coloured sweeps (section 2.9), the fused residual-restriction and the prolongation
+(sections 2.10, 2.11), with no host synchronisation inside a cycle.
+
+    A = sb.StencilOp.laplacian(2, (h, h, h), np.float64).scaled(-1.0)          # -lap u = f
+    mg = sb.Multigrid(dd, u, f, r, lambda l: A if l == 0 else coarse_A(l))     # A on level l, l = 0 finest
+    history = mg.solve(1e-8, 20)                                                # ||f - A u||_2 per cycle
+    mg.close()
+
+Periodic Poisson (A singular) needs f of zero mean; the solver does not project."""
+from __future__ import annotations
+
+import ctypes as C
+from typing import Callable, List, Optional
+
+import numpy as np
+
+from . import _lib
+from ._lib import check, lib, stream_ptr
+from .domain import FACES, BC, BCKind, Boundary, DataHandle, DistributedDomain, Partition, PlacementStrategy, Radius
+from .stencil_op import StencilOp
+
+
+def residual_op(A: StencilOp) -> StencilOp:
+    """r = f - A u as one op on src u and aux f: (aux, 0, 1), then each term of A with its weight negated."""
+    return StencilOp([(1, (0, 0, 0), 1.0)] + [(0, t[1], -t[2]) for t in A.terms], A.dtype)
+
+
+def coarse_bc(bc: BC) -> BC:
+    """The coarse correction's BC for a wall BC of u: ODD(c) -> ODD(0) (the correction of a solution pinned to c at the
+    wall vanishes there), EVEN -> EVEN.  VALUE and NONE have none (StencilError)."""
+    if bc.kind == BCKind.ODD:
+        return BC.ODD(0.0)
+    if bc.kind == BCKind.EVEN:
+        return BC.EVEN()
+    if bc.kind == BCKind.VALUE:
+        raise _lib.StencilError("Multigrid: VALUE walls are not consistent across levels (DESIGN.md section 2.10); use ODD(c), "
+                                "which pins the same value at the wall face")
+    raise _lib.StencilError("Multigrid: u needs a boundary condition (ODD or EVEN) on every FIXED face")
+
+
+def level_count(sizes, levels: Optional[int] = None) -> int:
+    """The number of grids: halve while every subdomain extent is even and its half is >= 2, capped at levels."""
+    n, cur = 1, [tuple(s) for s in sizes]
+    while (levels is None or n < levels) and all(v % 2 == 0 and v // 2 >= 2 for s in cur for v in s):
+        cur = [tuple(v // 2 for v in s) for s in cur]
+        n += 1
+    return n
+
+
+class _Clear:
+    """A one-launch plan that sets a quantity's whole curr allocation to +0 (ghost cells included; an exchange refills
+    them before any read)."""
+
+    def __init__(self, d, q: int):
+        raw = d.raw_size()
+        self.gpu, self.ptr, self.nbytes = d.gpu(), d.curr_[q], raw[0] * raw[1] * raw[2] * d.elem_size(q)
+
+    def launch(self, stream=None) -> None:
+        check(lib().sb_memset(C.c_void_p(self.ptr), 0, self.nbytes, self.gpu, stream_ptr(stream)))
+
+
+class _Level:
+    def __init__(self, dd: DistributedDomain, u: DataHandle, f: DataHandle, A: StencilOp):
+        self.dd, self.u, self.f, self.A = dd, u, f, A
+        self.gs = A.relax(1.0)
+        self.res = residual_op(A)
+
+
+class Multigrid:
+    """V(nu1, nu2) cycles for A u = f on the realized domain dd.  u, f and r are float32 or float64 quantities of dd
+    (curr buffers); r is scratch for the residual norm of solve().  op_at(l) returns A on level l (0 = dd): a StencilOp
+    of dd's type with plain src terms of reach <= 1 and one centre term.  Each coarse level is a DistributedDomain of u
+    and f on the same GPUs, placement and boundary kinds as dd, with dd's radius raised to >= 1 in all 26 directions;
+    the grid is halved while every subdomain extent is even and its half >= 2, at most `levels` grids.  The smoother is
+    red-black Gauss-Seidel if every level's A passes check(radius, colours=2), else 8-colour Gauss-Seidel.  Building the
+    hierarchy is collective under torchrun, and so are cycle() and solve().  The solver never calls dd.swap()."""
+
+    def __init__(self, dd: DistributedDomain, u: DataHandle, f: DataHandle, r: DataHandle, op_at: Callable[[int], StencilOp], nu1: int = 2,
+                 nu2: int = 2, coarse_sweeps: int = 30, levels: Optional[int] = None):
+        if not isinstance(dd, DistributedDomain) or dd.partition_ is None or not dd._plans:
+            raise _lib.StencilError("Multigrid: dd must be a realized DistributedDomain")
+        for name, h in (("u", u), ("f", f), ("r", r)):
+            if not isinstance(h, DataHandle) or not 0 <= h.id < len(dd.dtypes_):
+                raise _lib.StencilError(f"Multigrid: {name} must be a DataHandle of dd, not {h!r}")
+        if len({u.id, f.id, r.id}) != 3:
+            raise _lib.StencilError("Multigrid: u, f and r must be three different quantities")
+        dtype = dd.dtypes_[u.id]
+        if dtype not in (np.dtype(np.float32), np.dtype(np.float64)) or dd.dtypes_[f.id] != dtype or dd.dtypes_[r.id] != dtype:
+            raise _lib.StencilError("Multigrid: u, f and r must all be float32 or all float64")
+        if int(nu1) < 0 or int(nu2) < 0 or int(coarse_sweeps) < 1:
+            raise _lib.StencilError("Multigrid: nu1 and nu2 must be >= 0 and coarse_sweeps >= 1")
+        if levels is not None and int(levels) < 2:
+            raise _lib.StencilError("Multigrid: levels must be >= 2 (or None)")
+        self.nu1, self.nu2, self.coarse_sweeps = int(nu1), int(nu2), int(coarse_sweeps)
+        walls = {}
+        for fc in range(6):
+            if dd.boundary_[fc // 2] == Boundary.FIXED:
+                walls[fc] = coarse_bc(dd.bcs_.get((u.id, fc), BC.NONE()))
+        part = dd.partition_
+        nlev = level_count([part.subdomain_size(i) for i in part.indices()], levels)
+        if nlev < 2:
+            raise _lib.StencilError(f"Multigrid: the grid cannot be coarsened once: every subdomain extent must be even and >= 4, "
+                                    f"not {[part.subdomain_size(i) for i in part.indices()]}")
+        coarse_radius = Radius()
+        for d in coarse_radius._r:
+            coarse_radius.set_dir(d, dd.radius_.dir(d) if d == (0, 0, 0) else max(1, dd.radius_.dir(d)))
+        # each coarse domain partitions its own grid: check now, before any domain is built, that it splits as dd does
+        n_sub = len(dd.gpus_) * dd._world.size
+        trivial = dd.strategy_ == PlacementStrategy.Trivial
+        for l in range(1, nlev):
+            size_l = tuple(v >> l for v in dd.size())
+            cp = Partition(size_l, coarse_radius, 1, n_sub, trivial=trivial)
+            if cp.dim != part.dim or any(tuple(v * (1 << l) for v in cp.subdomain_size(i)) != tuple(part.subdomain_size(i)) for i in part.indices()):
+                raise _lib.StencilError(f"Multigrid: the {size_l} grid of level {l} is split as {cp.dim} subdomains, not as dd's {part.dim} "
+                                        f"halved {l} times; pass levels={l} or choose a grid whose coarsenings split alike")
+        ops = []
+        for l in range(nlev):
+            A = op_at(l)
+            if not isinstance(A, StencilOp) or A.dtype != dtype:
+                raise _lib.StencilError(f"Multigrid: op_at({l}) must be a StencilOp in {dtype}, not {A!r}")
+            if A.has_coef or A.has_aux:
+                raise _lib.StencilError(f"Multigrid: op_at({l}) has coefficient or aux terms; the smoother takes constant-coefficient src terms")
+            if A.reach() > 1:
+                raise _lib.StencilError(f"Multigrid: op_at({l}) reaches {A.reach()} cells; the fused residual-restriction takes reach <= 1")
+            ops.append(A)
+        self.colours = 0
+        for m in (2, 8):
+            try:
+                for l, A in enumerate(ops):
+                    A.check(dd.radius_ if l == 0 else coarse_radius, colours=m)
+            except _lib.StencilError:
+                continue
+            self.colours = m
+            break
+        if not self.colours:
+            raise _lib.StencilError("Multigrid: A reads its own colour under both red-black and 8-colour orderings (or leaves the "
+                                    "radius); no Gauss-Seidel smoother applies")
+        self.levels: List[_Level] = [_Level(dd, u, f, ops[0])]
+        self.r = r
+        # every level queues on dd's apply streams, so stream order alone orders the work of consecutive levels
+        if not dd._apply_streams:
+            import torch
+
+            dd._apply_streams = [(torch.cuda.Stream(device=d.gpu()), torch.cuda.Stream(device=d.gpu())) for d in dd.domains_]
+        size = dd.size()
+        try:
+            for l in range(1, nlev):
+                size = tuple(v // 2 for v in size)
+                cd = DistributedDomain(*size)
+                if dd.gpus_ is not None:
+                    cd.set_gpus(dd.gpus_)
+                cd.set_placement(dd.strategy_)
+                cd.set_methods(dd.flags_)
+                cd.set_radius(coarse_radius)
+                cu, cf = cd.add_data(dtype, "u"), cd.add_data(dtype, "f")
+                cd.set_boundary(*dd.boundary_)
+                for fc, bc in walls.items():
+                    cd.set_boundary_condition(cu, FACES[fc], bc)
+                cd.realize()
+                cd._apply_streams = dd._apply_streams
+                self.levels.append(_Level(cd, cu, cf, ops[l]))
+            for l in range(nlev - 1):
+                self.levels[l].dd._check_pairing(self.levels[l + 1].dd, True)
+        except Exception:
+            self.close()
+            raise
+
+    def _smooth(self, L: _Level, sweeps: int) -> None:
+        for _ in range(sweeps):
+            for c in range(self.colours):
+                L.dd._run_plans(*L.dd._apply_plans(L.gs, (L.u, "curr"), L.u, (L.f, "curr"), colour=(self.colours, c)), queued=True)
+
+    def _vcycle(self, l: int) -> None:
+        L = self.levels[l]
+        if l == len(self.levels) - 1:
+            self._smooth(L, self.coarse_sweeps)
+            return
+        self._smooth(L, self.nu1)
+        Cl = self.levels[l + 1]
+        L.dd._transfer(Cl.dd, _lib.TRANSFER_RESTRICT, (Cl.f, "curr"), (L.u, "curr"), (L.f, "curr"), True, op=L.res, queued=True)
+        Cl.dd._run_plans([(_Clear(d, Cl.u.id),) for d in Cl.dd.domains_], False, queued=True)
+        self._vcycle(l + 1)
+        L.dd._transfer(Cl.dd, _lib.TRANSFER_PROLONG, (L.u, "curr"), (Cl.u, "curr"), (L.u, "curr"), True, queued=True)
+        self._smooth(L, self.nu2)
+
+    def cycle(self, wait: bool = True) -> None:
+        """One V(nu1, nu2) cycle: per level nu1 sweeps, the fused residual-restriction into the coarse f, the coarse u set
+        to +0, the recursion, the in-place prolongation u <- u + P e and nu2 sweeps; coarse_sweeps sweeps on the coarsest
+        level.  Queued after the work on the caller's stream; returns when the cycle is complete (one host wait), or,
+        with wait=False, as soon as it is queued (call wait() before touching u)."""
+        import torch
+
+        dd = self.levels[0].dd
+        for d, (si, se) in zip(dd.domains_, dd._apply_streams):
+            si.wait_stream(torch.cuda.current_stream(d.gpu()))
+            se.wait_stream(torch.cuda.current_stream(d.gpu()))
+        self._vcycle(0)
+        if wait:
+            self.wait()
+
+    def wait(self) -> None:
+        """Return when every queued cycle is complete."""
+        dd = self.levels[0].dd
+        for si, se in dd._apply_streams:
+            si.synchronize()
+            se.synchronize()
+        for L in self.levels:
+            for x in L.dd._streams:
+                x.synchronize()
+
+    def residual_norm(self) -> float:
+        """||f - A u||_2 over dd's compute region: the residual into r (apply) and an exact reduction, so every rank and
+        every partition reach the same value."""
+        L = self.levels[0]
+        L.dd.apply(L.res, (self.r, "curr"), L.u, (L.f, "curr"))
+        return L.dd.reduce(self.r, "curr", exact=True).l2()
+
+    def solve(self, rtol: float, max_cycles: int) -> List[float]:
+        """Cycles until ||f - A u||_2 <= rtol ||f||_2 or max_cycles cycles; returns the residual norm before the first
+        cycle and after each.  Every rank calls it."""
+        L = self.levels[0]
+        target = float(rtol) * L.dd.reduce(L.f, "curr", exact=True).l2()
+        hist = [self.residual_norm()]
+        while hist[-1] > target and len(hist) - 1 < int(max_cycles):
+            self.cycle()
+            hist.append(self.residual_norm())
+        return hist
+
+    def close(self) -> None:
+        """Release the coarse domains and dd's transfer plans to them."""
+        dd = self.levels[0].dd
+        coarse = [L.dd for L in self.levels[1:]]
+        for fine in [dd] + coarse[:-1]:
+            for key in [k for k in fine._transfer_plans if any(k[0] is cd for cd in coarse)]:
+                for per_dom in fine._transfer_plans.pop(key):
+                    for p in per_dom:
+                        p.destroy()
+            fine._paired = {k for k in fine._paired if not any(k[0] is cd for cd in coarse)}
+        for cd in coarse:
+            cd.close()
+        self.levels = self.levels[:1]
