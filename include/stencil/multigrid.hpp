@@ -9,14 +9,24 @@
 // DistributedDomain of u and f on the same GPUs, placement and boundary kinds, with dd's radius raised to >= 1 in all 26
 // directions; the grid is halved while every subdomain extent is even and its half >= 2, at most `levels` grids (0: no
 // cap).  Coarse u takes ODD(0) where u has ODD(c) and EVEN where u has EVEN; VALUE, a FIXED face without a BC on u, a
-// grid that cannot be coarsened once, an op with coefficient or aux terms or of reach > 1 are refused (LOG_FATAL) before
+// grid that cannot be coarsened once, an op with aux terms (or coefficient terms without coefs) or of reach > 1 are
+// refused (LOG_FATAL) before
 // any domain is built.  The smoother is red-black Gauss-Seidel if every level's A passes the red-black colour check,
 // else 8-colour.  Building, cycle() and solve() are collective under MPI.  Periodic Poisson needs f of zero mean.
+//
+// Variable coefficients (DESIGN.md section 2.12): the constructor taking coefs and coef_kinds accepts ops with
+// coefficient terms, such as -div(kappa grad u) with kappa on faces in three quantities.  Kind "x", "y" or "z" marks a
+// face field (coarsened by the face restriction), "cell" a cell-centred one (the 8-cell restriction).  Each coarse level
+// holds one quantity per field with the fine field's BC on every FIXED face (a field without one is refused).
+// Coefficient ops are smoothed by the diagonal relaxation (DistributedDomain::relax, omega = 1) and their residual goes
+// through the fused coefficient restriction; update_coefficients() re-coarsens every level from the fine fields.
+//     stencil::Multigrid<double> mg(dd, u, f, r, [&](int l) { return A(l); }, {kx, ky, kz}, {"x", "y", "z"});
 #pragma once
 
 #include <cmath>
 #include <functional>
 #include <memory>
+#include <string>
 #include <vector>
 
 #include "stencil/linear_stencil.hpp"
@@ -30,12 +40,97 @@ public:
   Multigrid(DistributedDomain &dd, DataHandle<T> u, DataHandle<T> f, DataHandle<T> r, const std::function<LinearStencil(int)> &op_at, int nu1 = 2,
             int nu2 = 2, int coarse_sweeps = 30, int levels = 0)
       : nu1_(nu1), nu2_(nu2), coarse_sweeps_(coarse_sweeps), r_(r) {
+    init(dd, u, f, op_at, levels, {}, {});
+  }
+  Multigrid(DistributedDomain &dd, DataHandle<T> u, DataHandle<T> f, DataHandle<T> r, const std::function<LinearStencil(int)> &op_at,
+            const std::vector<DataHandle<T>> &coefs, const std::vector<std::string> &coef_kinds, int nu1 = 2, int nu2 = 2, int coarse_sweeps = 30,
+            int levels = 0)
+      : nu1_(nu1), nu2_(nu2), coarse_sweeps_(coarse_sweeps), r_(r) {
+    init(dd, u, f, op_at, levels, coefs, coef_kinds);
+  }
+
+  size_t num_levels() const { return levels_.size(); }
+  int colours() const { return colours_; }
+
+  // One V(nu1, nu2) cycle, queued after the work on the legacy default stream; returns when it is complete.
+  void cycle() {
+    for (Level &L : levels_) L.dd->queued_ = true;
+    vcycle(0);
+    finish();
+  }
+
+  // Re-coarsen every level's coefficient fields from the current fine ones, level by level, queued like a cycle with one
+  // host wait.  The constructor calls it once; call it again whenever the fine fields change.
+  void update_coefficients() {
+    for (Level &L : levels_) L.dd->queued_ = true;
+    for (size_t l = 0; l + 1 < levels_.size(); ++l)
+      for (size_t k = 0; k < axes_.size(); ++k) {
+        Level &F = levels_[l], &C = levels_[l + 1];
+        if (axes_[k] >= 0)
+          F.dd->restrict_to(*C.dd, curr(C.coefs[k]), curr(F.coefs[k]), axes_[k]);
+        else
+          F.dd->restrict_to(*C.dd, curr(C.coefs[k]), curr(F.coefs[k]));
+      }
+    finish();
+  }
+
+  // ||f - A u||_2: the residual into r and an exact reduction, the same on every rank and partition
+  double residual_norm() {
+    Level &L = levels_[0];
+    if (L.coefs.empty())
+      L.dd->apply(L.res, curr(r_), L.u, curr(L.f));
+    else
+      L.dd->apply(L.res, curr(r_), L.u, curr(L.f), L.coefs);
+    return std::sqrt(L.dd->reduce(r_, Which::curr, Sum::exact).sumsq);
+  }
+
+  // cycles until ||f - A u||_2 <= rtol ||f||_2 or max_cycles; the norm before the first cycle and after each
+  std::vector<double> solve(double rtol, int max_cycles) {
+    Level &L = levels_[0];
+    const double target = rtol * std::sqrt(L.dd->reduce(L.f, Which::curr, Sum::exact).sumsq);
+    std::vector<double> hist{residual_norm()};
+    while (hist.back() > target && int(hist.size()) - 1 < max_cycles) {
+      cycle();
+      hist.push_back(residual_norm());
+    }
+    return hist;
+  }
+
+private:
+  struct Level {
+    DistributedDomain *dd;
+    std::unique_ptr<DistributedDomain> owned; // the coarse levels
+    DataHandle<T> u, f;
+    LinearStencil A, gs, res; // gs: the SOR table of a plain op (a coefficient op is smoothed by relax)
+    std::vector<DataHandle<T>> coefs;
+  };
+  int nu1_, nu2_, coarse_sweeps_, colours_ = 0;
+  DataHandle<T> r_;
+  std::vector<Level> levels_;
+  std::vector<int> axes_; // per coefficient field: the face axis, or -1 for a cell field
+
+  void init(DistributedDomain &dd, DataHandle<T> u, DataHandle<T> f, const std::function<LinearStencil(int)> &op_at, int levels,
+            const std::vector<DataHandle<T>> &coefs, const std::vector<std::string> &coef_kinds) {
+    const DataHandle<T> r = r_;
+    const int nu1 = nu1_, nu2 = nu2_, coarse_sweeps = coarse_sweeps_;
     const int dtype = bc_dtype<T>();
     if (dtype != SB_DTYPE_F32 && dtype != SB_DTYPE_F64) LOG_FATAL("Multigrid: u, f and r must be float or double");
     if (dd.domains_.empty()) LOG_FATAL("Multigrid: dd must be realized");
     if (u.id() == f.id() || u.id() == r.id() || f.id() == r.id()) LOG_FATAL("Multigrid: u, f and r must be three different quantities");
     if (nu1 < 0 || nu2 < 0 || coarse_sweeps < 1) LOG_FATAL("Multigrid: nu1 and nu2 must be >= 0 and coarse_sweeps >= 1");
     if (levels == 1 || levels < 0) LOG_FATAL("Multigrid: levels must be >= 2 (or 0: no cap)");
+    if (coefs.size() > 4) LOG_FATAL("Multigrid: at most 4 coefficient fields");
+    if (coef_kinds.size() != coefs.size()) LOG_FATAL("Multigrid: coef_kinds must name one of x, y, z, cell per coefficient field");
+    for (size_t k = 0; k < coefs.size(); ++k) {
+      const std::string &kind = coef_kinds[k];
+      if (kind != "x" && kind != "y" && kind != "z" && kind != "cell")
+        LOG_FATAL("Multigrid: coef_kinds must name one of x, y, z, cell per coefficient field, not " << kind);
+      axes_.push_back(kind == "cell" ? -1 : kind[0] - 'x');
+      const size_t q = coefs[k].id();
+      if (q == u.id() || q == f.id() || q == r.id()) LOG_FATAL("Multigrid: coefficient " << k << " must be a quantity other than u, f and r");
+      for (size_t j = 0; j < k; ++j)
+        if (coefs[j].id() == q) LOG_FATAL("Multigrid: the coefficient fields must be different quantities");
+    }
     // the coarse BCs of u
     std::vector<std::pair<int, BC>> walls;
     for (int fc = 0; fc < 6; ++fc) {
@@ -45,6 +140,17 @@ public:
       if (kind == SB_BC_VALUE) LOG_FATAL("Multigrid: VALUE walls are not consistent across levels (DESIGN.md section 2.10); use ODD(c)");
       if (kind == SB_BC_NONE) LOG_FATAL("Multigrid: u needs a boundary condition (ODD or EVEN) on every FIXED face");
       walls.push_back(std::make_pair(fc, kind == SB_BC_ODD ? BC::ODD(0.0) : BC::EVEN()));
+    }
+    // every coefficient field's BCs, kept on every level
+    std::vector<std::vector<std::pair<int, BC>>> coef_walls(coefs.size());
+    for (int fc = 0; fc < 6; ++fc) {
+      if (dd.boundary_[fc / 2] != Topology::Boundary::FIXED) continue;
+      for (size_t k = 0; k < coefs.size(); ++k) {
+        auto it = dd.bcs_.find(std::make_pair(coefs[k].id(), fc));
+        if (it == dd.bcs_.end() || it->second.kind == BC::Kind::NONE)
+          LOG_FATAL("Multigrid: coefficient " << k << " needs a boundary condition on every FIXED face");
+        coef_walls[k].push_back(std::make_pair(fc, it->second));
+      }
     }
     // the number of grids: every subdomain extent (global information, the same verdict on every rank)
     const Dim3 dim = dd.placement_->dim();
@@ -69,10 +175,16 @@ public:
     for (int l = 0; l < nlev; ++l) {
       ops.push_back(op_at(l));
       const LinearStencil &A = ops.back();
-      if (A.ncoef() > 0 || A.has_aux()) LOG_FATAL("Multigrid: op_at(" << l << ") has coefficient or aux terms");
-      for (const sb_stencil_term &t : A.terms())
+      if (A.has_aux() || (A.ncoef() > 0 && coefs.empty())) LOG_FATAL("Multigrid: op_at(" << l << ") has coefficient or aux terms");
+      if (!coefs.empty() && size_t(A.ncoef()) != coefs.size())
+        LOG_FATAL("Multigrid: op_at(" << l << ") reads " << A.ncoef() << " coefficient fields, but " << coefs.size() << " were given");
+      bool centre = false;
+      for (const sb_stencil_vterm &t : A.vterms()) {
+        centre = centre || (!t.offset[0] && !t.offset[1] && !t.offset[2]);
         for (int a = 0; a < 3; ++a)
           if (t.offset[a] < -1 || t.offset[a] > 1) LOG_FATAL("Multigrid: op_at(" << l << ") reaches beyond 1 cell");
+      }
+      if (A.ncoef() > 0 && !centre) LOG_FATAL("Multigrid: op_at(" << l << ") has no term at offset (0, 0, 0)");
     }
     for (int m : {2, 8}) {
       bool ok = true;
@@ -91,7 +203,7 @@ public:
     }
     if (!colours_) LOG_FATAL("Multigrid: no Gauss-Seidel colouring applies to A (or it leaves the radius)");
     dd.create_apply_streams();
-    levels_.push_back(Level{&dd, nullptr, u, f, ops[0].relax(1.0), residual(ops[0])});
+    levels_.push_back(Level{&dd, nullptr, u, f, ops[0], smoother(ops[0]), residual(ops[0]), coefs});
     Dim3 size = dd.size_;
     for (int l = 1; l < nlev; ++l) {
       size = Dim3(size.x / 2, size.y / 2, size.z / 2);
@@ -100,25 +212,31 @@ public:
       cd->set_placement(dd.strategy_);
       cd->set_radius(cr);
       DataHandle<T> cu = cd->template add_data<T>("u"), cf = cd->template add_data<T>("f");
+      std::vector<DataHandle<T>> ck;
+      for (size_t k = 0; k < coefs.size(); ++k) ck.push_back(cd->template add_data<T>("coef" + std::to_string(k)));
       cd->set_boundary(dd.boundary_[0], dd.boundary_[1], dd.boundary_[2]);
-      for (const auto &w : walls) cd->set_boundary_condition(cu, Dim3(w.first / 2 == 0 ? (w.first % 2 ? 1 : -1) : 0, w.first / 2 == 1 ? (w.first % 2 ? 1 : -1) : 0,
-                                                                       w.first / 2 == 2 ? (w.first % 2 ? 1 : -1) : 0), w.second);
+      for (const auto &w : walls) cd->set_boundary_condition(cu, face_dir(w.first), w.second);
+      for (size_t k = 0; k < coefs.size(); ++k)
+        for (const auto &w : coef_walls[k]) cd->set_boundary_condition(ck[k], face_dir(w.first), w.second);
       cd->realize();
       // every level queues on dd's apply streams, so stream order alone orders consecutive levels
       cd->applyStreams_ = dd.applyStreams_;
       cd->sharedApplyStreams_ = true;
-      levels_.push_back(Level{cd.get(), std::move(cd), cu, cf, ops[size_t(l)].relax(1.0), residual(ops[size_t(l)])});
+      levels_.push_back(Level{cd.get(), std::move(cd), cu, cf, ops[size_t(l)], smoother(ops[size_t(l)]), residual(ops[size_t(l)]), ck});
     }
     for (size_t l = 0; l + 1 < levels_.size(); ++l) levels_[l].dd->check_pairing(*levels_[l + 1].dd, true);
+    if (!coefs.empty()) update_coefficients();
   }
 
-  size_t num_levels() const { return levels_.size(); }
-  int colours() const { return colours_; }
+  static Dim3 face_dir(int fc) {
+    const int s = fc % 2 ? 1 : -1;
+    return Dim3(fc / 2 == 0 ? s : 0, fc / 2 == 1 ? s : 0, fc / 2 == 2 ? s : 0);
+  }
 
-  // One V(nu1, nu2) cycle, queued after the work on the legacy default stream; returns when it is complete.
-  void cycle() {
-    for (Level &L : levels_) L.dd->queued_ = true;
-    vcycle(0);
+  static LinearStencil smoother(const LinearStencil &A) { return A.ncoef() > 0 ? LinearStencil() : A.relax(1.0); }
+
+  // the end of a queued cycle: every apply stream and exchange of every level complete
+  void finish() {
     for (Level &L : levels_) L.dd->queued_ = false;
     DistributedDomain &dd = *levels_[0].dd;
     for (size_t i = 0; i < dd.applyStreams_.size(); ++i) {
@@ -128,46 +246,23 @@ public:
     for (Level &L : levels_) L.dd->exchange_wait();
   }
 
-  // ||f - A u||_2: the residual into r and an exact reduction, the same on every rank and partition
-  double residual_norm() {
-    Level &L = levels_[0];
-    L.dd->apply(L.res, curr(r_), L.u, curr(L.f));
-    return std::sqrt(L.dd->reduce(r_, Which::curr, Sum::exact).sumsq);
-  }
-
-  // cycles until ||f - A u||_2 <= rtol ||f||_2 or max_cycles; the norm before the first cycle and after each
-  std::vector<double> solve(double rtol, int max_cycles) {
-    Level &L = levels_[0];
-    const double target = rtol * std::sqrt(L.dd->reduce(L.f, Which::curr, Sum::exact).sumsq);
-    std::vector<double> hist{residual_norm()};
-    while (hist.back() > target && int(hist.size()) - 1 < max_cycles) {
-      cycle();
-      hist.push_back(residual_norm());
-    }
-    return hist;
-  }
-
-private:
-  struct Level {
-    DistributedDomain *dd;
-    std::unique_ptr<DistributedDomain> owned; // the coarse levels
-    DataHandle<T> u, f;
-    LinearStencil gs, res;
-  };
-  int nu1_, nu2_, coarse_sweeps_, colours_ = 0;
-  DataHandle<T> r_;
-  std::vector<Level> levels_;
-
+  // r = f - A u: (aux, 0, 1), then each term of A with its weight negated (a coefficient term keeps its field)
   static LinearStencil residual(const LinearStencil &A) {
     LinearStencil res;
     res.add(Source::aux, 0, 0, 0, 1.0);
-    for (const sb_stencil_term &t : A.terms()) res.add(Source::src, t.offset[0], t.offset[1], t.offset[2], -t.weight);
+    for (const sb_stencil_vterm &t : A.vterms())
+      res.add(Source::src, t.offset[0], t.offset[1], t.offset[2], -t.weight, t.coef, t.coef_offset[0], t.coef_offset[1], t.coef_offset[2]);
     return res;
   }
 
   void smooth(Level &L, int sweeps) {
     for (int k = 0; k < sweeps; ++k)
-      for (int c = 0; c < colours_; ++c) L.dd->apply(L.gs, curr(L.u), L.u, curr(L.f), Colour{colours_, c});
+      for (int c = 0; c < colours_; ++c) {
+        if (L.coefs.empty())
+          L.dd->apply(L.gs, curr(L.u), L.u, curr(L.f), Colour{colours_, c});
+        else
+          L.dd->relax(L.A, curr(L.u), L.u, curr(L.f), L.coefs, Colour{colours_, c}, 1.0);
+      }
   }
 
   void vcycle(size_t l) {
@@ -178,7 +273,10 @@ private:
     }
     smooth(L, nu1_);
     Level &C = levels_[l + 1];
-    L.dd->restrict_to(*C.dd, curr(C.f), L.res, L.u, curr(L.f));
+    if (L.coefs.empty())
+      L.dd->restrict_to(*C.dd, curr(C.f), L.res, L.u, curr(L.f));
+    else
+      L.dd->restrict_to(*C.dd, curr(C.f), L.res, L.u, curr(L.f), L.coefs);
     // coarse u <- +0: a memset of the curr allocation (an exchange refills the ghost cells before any read)
     C.dd->queue_after_exterior();
     for (size_t di = 0; di < C.dd->domains_.size(); ++di) {

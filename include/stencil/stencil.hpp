@@ -142,8 +142,9 @@ private:
   std::map<std::vector<int64_t>, std::vector<std::vector<sb_stencil_plan *>>> stencilPlans_;
   std::vector<cudaStream_t> applyStreams_;
   void destroy_stencil_plans();
+  // omega non-NULL: relax()'s diagonal relaxation (sb_stencil_dplan_create), aq the right-hand side f
   void apply_op(const stencil::LinearStencil &op, int dtype, size_t dq, stencil::Which dw, size_t sq, int64_t aq, stencil::Which aw,
-                const std::vector<size_t> &cq, bool exchange, stencil::Colour colour = stencil::Colour{});
+                const std::vector<size_t> &cq, bool exchange, stencil::Colour colour = stencil::Colour{}, const double *omega = nullptr);
   void apply_sys(const stencil::LinearSystem &sys, int dtype, const std::vector<std::pair<size_t, stencil::Which>> &outs,
                  const std::vector<std::pair<size_t, stencil::Which>> &ins, bool exchange);
   // the schedule apply_op and apply_sys share: the cached per-domain plans of key (built by make(domain, boxes) on first
@@ -176,9 +177,11 @@ private:
   uint64_t serial_;
   std::map<std::vector<int64_t>, std::vector<sb_transfer_plan *>> transferPlans_;
   std::set<std::pair<uint64_t, bool>> paired_; // (coarse serial, with ghosts) that passed the pairing check
-  // op: the fused residual-restriction (sb_transfer_oplan_create; restriction only), with apply's schedule when exchange
+  // op: the fused residual-restriction (sb_transfer_oplan_create, or sb_transfer_voplan_create over the fine coefficient
+  // quantities cq; restriction only), with apply's schedule when exchange.  face >= 0: the face-coefficient restriction
+  // of the faces normal to that axis (sb_transfer_fplan_create).
   void transfer(DistributedDomain &coarse, bool prolong, int dtype, size_t dq, stencil::Which dw, size_t sq, stencil::Which sw, int64_t aq,
-                stencil::Which aw, bool exchange, const stencil::LinearStencil *op = nullptr);
+                stencil::Which aw, bool exchange, const stencil::LinearStencil *op = nullptr, const std::vector<size_t> &cq = {}, int face = -1);
   void check_pairing(DistributedDomain &coarse, bool ghosts);
   void destroy_transfer_plans();
   void create_apply_streams(); // two per local domain (interior, exterior), on first use
@@ -377,6 +380,27 @@ public:
              const std::vector<DataHandle<T>> &coefs, stencil::Colour colour, bool exchange = true) {
     apply_op(op, stencil::bc_dtype<T>(), dst.h.id(), dst.which, src.id(), int64_t(aux.h.id()), aux.which, ids_of(coefs), exchange, colour);
   }
+  // One relaxation pass of A u = f that divides by A's own diagonal (DESIGN.md section 2.12, sb_stencil_dplan_create):
+  // dst = u + omega (f - A u) / d, d the sum of the factors of A's offset-0 terms, on the cells of the colour (none: every
+  // cell, weighted Jacobi, dst must not be u).  A has src terms only (plain or coefficient) and a term at offset 0; f is a
+  // buffer of A's type; coefs as apply's.  Schedule, plan cache (omega in its key) and failure rules are apply's.
+  //     for (int c = 0; c < 2; ++c) dd.relax(A, stencil::curr(u), u, stencil::curr(f), {kx, ky, kz}, stencil::Colour{2, c});
+  template <typename T>
+  void relax(const stencil::LinearStencil &A, const stencil::Buffer<T> &dst, const DataHandle<T> &u, const stencil::Buffer<T> &f,
+             const std::vector<DataHandle<T>> &coefs, stencil::Colour colour, double omega = 1.0, bool exchange = true) {
+    apply_op(A, stencil::bc_dtype<T>(), dst.h.id(), dst.which, u.id(), int64_t(f.h.id()), f.which, ids_of(coefs), exchange, colour, &omega);
+  }
+  template <typename T>
+  void relax(const stencil::LinearStencil &A, const stencil::Buffer<T> &dst, const DataHandle<T> &u, const stencil::Buffer<T> &f,
+             const std::vector<DataHandle<T>> &coefs, double omega = 1.0, bool exchange = true) {
+    apply_op(A, stencil::bc_dtype<T>(), dst.h.id(), dst.which, u.id(), int64_t(f.h.id()), f.which, ids_of(coefs), exchange, stencil::Colour{}, &omega);
+  }
+  template <typename T>
+  void relax(const stencil::LinearStencil &A, const stencil::Buffer<T> &dst, const DataHandle<T> &u, const stencil::Buffer<T> &f,
+             stencil::Colour colour, double omega = 1.0, bool exchange = true) {
+    apply_op(A, stencil::bc_dtype<T>(), dst.h.id(), dst.which, u.id(), int64_t(f.h.id()), f.which, {}, exchange, colour, &omega);
+  }
+
   // outputs = sys(inputs) over the whole compute region of every local subdomain (DESIGN.md section 2.8): sys.nout()
   // outputs and sys.nin() inputs, each the curr or next buffer of a quantity of the system's type.  An input read at a
   // non-zero offset must be a curr buffer (the one exchange() fills); outputs are pairwise distinct; an output may be an
@@ -426,6 +450,22 @@ public:
   void restrict_to(DistributedDomain &coarse, const stencil::Buffer<T> &dst, const stencil::LinearStencil &op, const DataHandle<T> &src,
                    bool exchange = true) {
     transfer(coarse, false, stencil::bc_dtype<T>(), dst.h.id(), dst.which, src.id(), stencil::Which::curr, -1, stencil::Which::curr, exchange, &op);
+  }
+  // restrict_to with a coefficient op (DESIGN.md section 2.12): coefs are op.ncoef() fine quantities (curr buffers,
+  // exchanged like src); the result is the bits of apply() into a scratch quantity followed by restrict_to().
+  //     fine.restrict_to(coarse, stencil::curr(f2), residual, u, stencil::curr(f), {kx, ky, kz});
+  template <typename T>
+  void restrict_to(DistributedDomain &coarse, const stencil::Buffer<T> &dst, const stencil::LinearStencil &op, const DataHandle<T> &src,
+                   const stencil::Buffer<T> &aux, const std::vector<DataHandle<T>> &coefs, bool exchange = true) {
+    transfer(coarse, false, stencil::bc_dtype<T>(), dst.h.id(), dst.which, src.id(), stencil::Which::curr, int64_t(aux.h.id()), aux.which, exchange, &op,
+             ids_of(coefs));
+  }
+  // the face-coefficient restriction (DESIGN.md section 2.12): src holds values on the faces normal to axis (0, 1, 2),
+  // C_a(p) on the face between p - e_a and p; dst = the average of the four fine faces of each coarse face.
+  //     fine.restrict_to(coarse, stencil::curr(kx2), stencil::curr(kx), 0);
+  template <typename T> void restrict_to(DistributedDomain &coarse, const stencil::Buffer<T> &dst, const stencil::Buffer<T> &src, int axis) {
+    if (axis < 0 || axis > 2) LOG_FATAL("restrict_to: face axis " << axis << " must be 0, 1 or 2");
+    transfer(coarse, false, stencil::bc_dtype<T>(), dst.h.id(), dst.which, src.h.id(), src.which, -1, stencil::Which::curr, false, nullptr, {}, axis);
   }
   template <typename T>
   void prolong_from(DistributedDomain &coarse, const stencil::Buffer<T> &dst, const stencil::Buffer<T> &src, bool exchange = true) {

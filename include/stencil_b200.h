@@ -439,6 +439,21 @@ int sb_stencil_relax(const sb_stencil_term *A, int n, double omega, sb_stencil_t
 int sb_stencil_cplan_create(sb_stencil_plan **out, int device, int dtype, const sb_stencil_vterm *terms, int n, sb_pitched dst,
                             sb_pitched src, sb_pitched aux, const sb_pitched *coef, int ncoef, int ncolours, int colour,
                             const int64_t acc_origin[3], int64_t zsize, int nbox, const int64_t *lo, const int64_t *hi);
+/* Diagonal relaxation (DESIGN.md section 2.12): a relaxation sweep of A u = f for an op A whose diagonal varies from
+ * cell to cell, such as div(kappa grad u).  A is an op of src terms only (plain or coefficient terms, no aux term, at
+ * least one term at offset 0); f is on aux (the `f` argument); omega is the relaxation factor.  For every cell p of
+ * colour c under the colouring m, in T with every operation rounded separately (no FMA contraction):
+ *   for each term t in list order: k_t = T(w_t), or T(w_t) * C_k(p + c_t) for a coefficient term; m_t = k_t * u(p + o_t);
+ *     a = m_0, then a = a + m_t (the op rule above, unchanged)
+ *   d = the sum of the factors k_t of the terms with o_t = 0, in list order (the first, then d = d + k_t)
+ *   dst[p] = u(p) + T(omega) * ((f(p) - a) / d), with an IEEE round-to-nearest divide
+ * With m > 1 dst may be src (in place) and the colour condition applies; with m = 1 and dst != src it is weighted
+ * Jacobi.  d = 0 or a non-finite d gives whatever IEEE arithmetic gives; it is not checked.  Errors beyond
+ * sb_stencil_cplan_create's (SB_ERR_INVALID with a message, before anything is allocated): an aux term in A, no term
+ * at offset 0, omega not finite, f NULL.  sb_stencil_plan_bytes counts as for a coloured plan, f as the aux read. */
+int sb_stencil_dplan_create(sb_stencil_plan **out, int device, int dtype, const sb_stencil_vterm *terms, int n, sb_pitched dst,
+                            sb_pitched src, sb_pitched f, const sb_pitched *coef, int ncoef, double omega, int ncolours, int colour,
+                            const int64_t acc_origin[3], int64_t zsize, int nbox, const int64_t *lo, const int64_t *hi);
 
 /* ---------------------------------------------------------------------------------------------
  * Linear stencil systems: one launch over nin input and nout output allocations.  A term of output j reads input
@@ -562,6 +577,28 @@ int sb_transfer_plan_destroy(sb_transfer_plan *plan);
 int sb_transfer_oplan_create(sb_transfer_plan **out, int device, int dtype, const sb_stencil_term *terms, int n, sb_pitched dst,
                              const int64_t dst_acc_origin[3], int64_t dst_zsize, sb_pitched src, const int64_t src_acc_origin[3],
                              int64_t src_zsize, sb_pitched aux, int nbox, const int64_t *lo, const int64_t *hi);
+/* sb_transfer_oplan_create for an op with coefficient terms (DESIGN.md section 2.12): the same rule, the factor of a
+ * coefficient term being T(w) * C_k(p + c) as in sb_stencil_vplan_create, so the result is the bits of
+ * sb_stencil_vplan_create over the fine footprint into a scratch allocation followed by SB_TRANSFER_RESTRICT.  coef:
+ * ncoef (<= 4) fine fields that share src's pitch, row count, zsize and acc_origin; coefficient offsets reach at most 1.
+ * Boxes go to the kernels of sb_transfer_oplan_create, which read the fields through the read-only cache at each term's
+ * coefficient offset.  Bytes as sb_transfer_oplan_create's plus 8 elements per
+ * coarse cell of each field a term reads.  Errors: sb_transfer_oplan_create's, plus a field index out of range, a NULL
+ * field a term names, a field that is dst, and a field with another pitch or row count than src. */
+int sb_transfer_voplan_create(sb_transfer_plan **out, int device, int dtype, const sb_stencil_vterm *terms, int n, sb_pitched dst,
+                              const int64_t dst_acc_origin[3], int64_t dst_zsize, sb_pitched src, const int64_t src_acc_origin[3],
+                              int64_t src_zsize, sb_pitched aux, const sb_pitched *coef, int ncoef, int nbox, const int64_t *lo,
+                              const int64_t *hi);
+/* Face-coefficient restriction (DESIGN.md section 2.12): a field of values on the faces normal to axis `axis` (C_a(p) on
+ * the face between p - e_a and p, the convention of sb_stencil_div_grad) to the coarse grid.  With b < c the two other
+ * axes, for each coarse cell I of the box [lo, hi) of dst (coarse global coordinates), in T:
+ *   C[I] = T(0.25) * (((F(2I) + F(2I + e_b)) + F(2I + e_c)) + F(2I + e_b + e_c))
+ * the four fine faces that make up coarse face I.  It reads only inside the footprint (no fine ghost cells).  Buffers,
+ * launch, bytes (4 fine elements read and one written per coarse cell) and destroy as for SB_TRANSFER_RESTRICT, whose
+ * errors it shares, plus an axis outside 0 .. 2. */
+int sb_transfer_fplan_create(sb_transfer_plan **out, int device, int dtype, int axis, sb_pitched dst, const int64_t dst_acc_origin[3],
+                             int64_t dst_zsize, sb_pitched src, const int64_t src_acc_origin[3], int64_t src_zsize,
+                             const int64_t lo[3], const int64_t hi[3]);
 
 /* ---------------------------------------------------------------------------------------------
  * 7-point jacobi step (the reference's user kernel, bin/jacobi3d.cu:40-85) over a region.

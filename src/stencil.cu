@@ -669,31 +669,44 @@ void DistributedDomain::destroy_stencil_plans() {
 }
 
 void DistributedDomain::apply_op(const stencil::LinearStencil &op, int dtype, size_t dq, stencil::Which dw, size_t sq, int64_t aq,
-                                 stencil::Which aw, const std::vector<size_t> &cq, bool exchange, stencil::Colour colour) {
+                                 stencil::Which aw, const std::vector<size_t> &cq, bool exchange, stencil::Colour colour, const double *omega) {
   using stencil::Which;
-  if (domains_.empty() || plans_[0].size() != domains_.size()) LOG_FATAL("apply: call realize() first");
-  if (dtype != SB_DTYPE_F32 && dtype != SB_DTYPE_F64) LOG_FATAL("apply: a stencil operator computes in float or double");
+  const char *name = omega ? "relax" : "apply";
+  if (domains_.empty() || plans_[0].size() != domains_.size()) LOG_FATAL(name << ": call realize() first");
+  if (dtype != SB_DTYPE_F32 && dtype != SB_DTYPE_F64) LOG_FATAL(name << ": a stencil operator computes in float or double");
   for (const int64_t q : {int64_t(dq), int64_t(sq), aq})
-    if (q >= 0 && (size_t(q) >= dataDtype_.size() || dataDtype_[size_t(q)] != dtype)) LOG_FATAL("apply: unknown data handle " << q);
+    if (q >= 0 && (size_t(q) >= dataDtype_.size() || dataDtype_[size_t(q)] != dtype)) LOG_FATAL(name << ": unknown data handle " << q);
   if ((colour.m != 1 && colour.m != 2 && colour.m != 8) || colour.c < 0 || colour.c >= colour.m)
-    LOG_FATAL("apply: colour (" << colour.m << ", " << colour.c << ") must have m = 1, 2 or 8 and 0 <= c < m");
-  if (dq == sq && dw == Which::curr && colour.m == 1) LOG_FATAL("apply: dst must not be src");
-  if (op.has_aux() && aq < 0) LOG_FATAL("apply: the op has a term on aux, but no aux buffer was given");
-  if (int(cq.size()) != op.ncoef()) LOG_FATAL("apply: the op reads " << op.ncoef() << " coefficient fields, but " << cq.size() << " were given");
+    LOG_FATAL(name << ": colour (" << colour.m << ", " << colour.c << ") must have m = 1, 2 or 8 and 0 <= c < m");
+  if (dq == sq && dw == Which::curr && colour.m == 1) LOG_FATAL(name << ": dst must not be src");
+  if (op.has_aux() && aq < 0) LOG_FATAL(name << ": the op has a term on aux, but no aux buffer was given");
+  if (omega) {
+    if (op.has_aux()) LOG_FATAL("relax: A has a term on aux; A reads u only (f is the right-hand side)");
+    bool centre = false;
+    for (const sb_stencil_vterm &t : op.vterms()) centre = centre || (t.source == 0 && !t.offset[0] && !t.offset[1] && !t.offset[2]);
+    if (!centre) LOG_FATAL("relax: A has no term at offset (0, 0, 0), so no diagonal");
+    if (!std::isfinite(*omega)) LOG_FATAL("relax: omega = " << *omega << " must be finite");
+  }
+  if (int(cq.size()) != op.ncoef()) LOG_FATAL(name << ": the op reads " << op.ncoef() << " coefficient fields, but " << cq.size() << " were given");
   for (size_t k = 0; k < cq.size(); ++k) {
-    if (cq[k] >= dataDtype_.size() || dataDtype_[cq[k]] != dtype) LOG_FATAL("apply: coefficient " << k << " is not a quantity of the op's type");
-    if (cq[k] == dq && dw == Which::curr) LOG_FATAL("apply: coefficient " << k << " must not be dst");
+    if (cq[k] >= dataDtype_.size() || dataDtype_[cq[k]] != dtype) LOG_FATAL(name << ": coefficient " << k << " is not a quantity of the op's type");
+    if (cq[k] == dq && dw == Which::curr) LOG_FATAL(name << ": coefficient " << k << " must not be dst");
   }
   int64_t r27[27];
   for (int z = -1, i = 0; z <= 1; ++z)
     for (int y = -1; y <= 1; ++y)
       for (int x = -1; x <= 1; ++x) r27[i++] = int64_t(radius_.dir(x, y, z));
   const std::vector<sb_stencil_vterm> &terms = op.vterms();
-  if (SB_OK != sb_stencil_ccheck(terms.data(), int(terms.size()), r27, colour.m)) LOG_FATAL("apply: " << sb_last_error());
-  if (!op.has_aux()) aq = -1;
+  if (SB_OK != sb_stencil_ccheck(terms.data(), int(terms.size()), r27, colour.m)) LOG_FATAL(name << ": " << sb_last_error());
+  if (!op.has_aux() && !omega) aq = -1;
   std::vector<int64_t> key = {dtype, int64_t(dq), int64_t(dw == Which::next), int64_t(sq), aq, int64_t(aw == Which::next), int64_t(exchange), parity_,
                               colour.m, colour.c, int64_t(cq.size())};
   for (const size_t q : cq) key.push_back(int64_t(q));
+  if (omega) { // the diagonal mode and omega's bits (the plain key ends with a term's 9 entries, so the two never collide)
+    int64_t obits;
+    std::memcpy(&obits, omega, 8);
+    key.insert(key.end(), {-2, obits});
+  }
   for (const sb_stencil_vterm &t : terms) {
     int64_t wbits;
     std::memcpy(&wbits, &t.weight, 8);
@@ -713,9 +726,11 @@ void DistributedDomain::apply_op(const stencil::LinearStencil &op, int dtype, si
       hi.insert(hi.end(), {b.hi.x, b.hi.y, b.hi.z});
     }
     sb_stencil_plan *p = nullptr;
-    if (SB_OK != sb_stencil_cplan_create(&p, d.gpu(), dtype, terms.data(), int(terms.size()), dst, src, aux, coef.data(), int(coef.size()),
-                                         colour.m, colour.c, acc, d.raw_size().z, int(boxes.size()), lo.data(), hi.data()))
-      LOG_FATAL("apply: " << sb_last_error());
+    const int rc = omega ? sb_stencil_dplan_create(&p, d.gpu(), dtype, terms.data(), int(terms.size()), dst, src, aux, coef.data(), int(coef.size()),
+                                                   *omega, colour.m, colour.c, acc, d.raw_size().z, int(boxes.size()), lo.data(), hi.data())
+                         : sb_stencil_cplan_create(&p, d.gpu(), dtype, terms.data(), int(terms.size()), dst, src, aux, coef.data(), int(coef.size()),
+                                                   colour.m, colour.c, acc, d.raw_size().z, int(boxes.size()), lo.data(), hi.data());
+    if (SB_OK != rc) LOG_FATAL(name << ": " << sb_last_error());
     return p;
   });
 }
@@ -951,7 +966,7 @@ void DistributedDomain::check_pairing(DistributedDomain &coarse, bool ghosts) {
 }
 
 void DistributedDomain::transfer(DistributedDomain &coarse, bool prolong, int dtype, size_t dq, stencil::Which dw, size_t sq, stencil::Which sw,
-                                 int64_t aq, stencil::Which aw, bool exchange, const stencil::LinearStencil *op) {
+                                 int64_t aq, stencil::Which aw, bool exchange, const stencil::LinearStencil *op, const std::vector<size_t> &cq, int face) {
   using stencil::Which;
   const char *name = prolong ? "prolong_from" : "restrict_to";
   if (&coarse == this) LOG_FATAL(name << ": coarse must be another DistributedDomain");
@@ -968,25 +983,41 @@ void DistributedDomain::transfer(DistributedDomain &coarse, bool prolong, int dt
                               int64_t(sw == Which::next), aq, int64_t(aw == Which::next), parity_, coarse.parity_};
   if (op) {
     if (prolong) LOG_FATAL(name << ": only a restriction takes an op");
-    if (op->ncoef() > 0) LOG_FATAL(name << ": the op has coefficient terms; the fused restriction takes plain terms");
+    if (int(cq.size()) != op->ncoef()) LOG_FATAL(name << ": the op reads " << op->ncoef() << " coefficient fields, but " << cq.size() << " were given");
+    for (size_t k = 0; k < cq.size(); ++k)
+      if (cq[k] >= dataDtype_.size() || dataDtype_[cq[k]] != dtype) LOG_FATAL(name << ": coefficient " << k << " is not a quantity of that type");
     if (sw != Which::curr) LOG_FATAL(name << ": with an op, src must be a curr buffer (the one exchange() fills)");
     if (op->has_aux() && aq < 0) LOG_FATAL(name << ": the op has a term on aux, but no aux buffer was given");
     int64_t r27[27];
     for (int z = -1, i = 0; z <= 1; ++z)
       for (int y = -1; y <= 1; ++y)
         for (int x = -1; x <= 1; ++x) r27[i++] = int64_t(radius_.dir(x, y, z));
-    if (SB_OK != sb_stencil_check(op->terms().data(), int(op->terms().size()), r27)) LOG_FATAL(name << ": " << sb_last_error());
+    if (SB_OK != sb_stencil_vcheck(op->vterms().data(), int(op->vterms().size()), r27)) LOG_FATAL(name << ": " << sb_last_error());
     if (!op->has_aux()) {
       aq = -1;
       key[6] = -1;
       key[7] = 0;
     }
     key.push_back(int64_t(exchange));
-    for (const sb_stencil_term &t : op->terms()) {
-      int64_t wbits;
-      std::memcpy(&wbits, &t.weight, 8);
-      key.insert(key.end(), {t.source, t.offset[0], t.offset[1], t.offset[2], wbits});
+    if (cq.empty()) {
+      for (const sb_stencil_term &t : op->terms()) {
+        int64_t wbits;
+        std::memcpy(&wbits, &t.weight, 8);
+        key.insert(key.end(), {t.source, t.offset[0], t.offset[1], t.offset[2], wbits});
+      }
+    } else { // a coefficient op: a marker, the fields, then every term with its coefficient
+      key.insert(key.end(), {-2, int64_t(cq.size())});
+      for (const size_t q : cq) key.push_back(int64_t(q));
+      for (const sb_stencil_vterm &t : op->vterms()) {
+        int64_t wbits;
+        std::memcpy(&wbits, &t.weight, 8);
+        key.insert(key.end(), {t.source, t.offset[0], t.offset[1], t.offset[2], t.coef, t.coef_offset[0], t.coef_offset[1], t.coef_offset[2], wbits});
+      }
     }
+  }
+  if (face >= 0) {
+    if (op || prolong) LOG_FATAL(name << ": a face restriction takes no op");
+    key.insert(key.end(), {-3, int64_t(face)});
   }
   check_pairing(coarse, prolong);
   auto found = transferPlans_.find(key);
@@ -1013,9 +1044,15 @@ void DistributedDomain::transfer(DistributedDomain &coarse, bool prolong, int dt
           hi.insert(hi.end(), {b.hi.x, b.hi.y, b.hi.z});
         }
         sb_transfer_plan *p = nullptr;
-        if (SB_OK != sb_transfer_oplan_create(&p, f.gpu(), dtype, op->terms().data(), int(op->terms().size()), pick(cd, dq, dw), dacc,
-                                              cd.raw_size().z, pick(f, sq, sw), sacc, f.raw_size().z, aux, int(boxes.size()), lo.data(), hi.data()))
-          LOG_FATAL(name << ": " << sb_last_error());
+        std::vector<sb_pitched> coef;
+        for (const size_t q : cq) coef.push_back(as_sb(f.curr_data(q)));
+        const int rc = cq.empty() ? sb_transfer_oplan_create(&p, f.gpu(), dtype, op->terms().data(), int(op->terms().size()), pick(cd, dq, dw), dacc,
+                                                             cd.raw_size().z, pick(f, sq, sw), sacc, f.raw_size().z, aux, int(boxes.size()), lo.data(),
+                                                             hi.data())
+                                  : sb_transfer_voplan_create(&p, f.gpu(), dtype, op->vterms().data(), int(op->vterms().size()), pick(cd, dq, dw), dacc,
+                                                              cd.raw_size().z, pick(f, sq, sw), sacc, f.raw_size().z, aux, coef.data(), int(coef.size()),
+                                                              int(boxes.size()), lo.data(), hi.data());
+        if (SB_OK != rc) LOG_FATAL(name << ": " << sb_last_error());
         per_dom.push_back(p);
       }
     }
@@ -1029,9 +1066,11 @@ void DistributedDomain::transfer(DistributedDomain &coarse, bool prolong, int dt
       set3(hi, box.hi);
       const sb_pitched aux = aq < 0 ? sb_pitched{nullptr, 0, 0} : pick(f, size_t(aq), aw);
       sb_transfer_plan *p = nullptr;
-      if (SB_OK != sb_transfer_plan_create(&p, f.gpu(), dtype, prolong ? SB_TRANSFER_PROLONG : SB_TRANSFER_RESTRICT, pick(dd, dq, dw), dacc,
-                                           dd.raw_size().z, pick(sd, sq, sw), sacc, sd.raw_size().z, aux, lo, hi))
-        LOG_FATAL(name << ": " << sb_last_error());
+      const int rc = face >= 0 ? sb_transfer_fplan_create(&p, f.gpu(), dtype, face, pick(dd, dq, dw), dacc, dd.raw_size().z, pick(sd, sq, sw), sacc,
+                                                          sd.raw_size().z, lo, hi)
+                               : sb_transfer_plan_create(&p, f.gpu(), dtype, prolong ? SB_TRANSFER_PROLONG : SB_TRANSFER_RESTRICT, pick(dd, dq, dw), dacc,
+                                                         dd.raw_size().z, pick(sd, sq, sw), sacc, sd.raw_size().z, aux, lo, hi);
+      if (SB_OK != rc) LOG_FATAL(name << ": " << sb_last_error());
       per_dom.push_back(p);
     }
     found = transferPlans_.emplace(key, std::move(per_dom)).first;

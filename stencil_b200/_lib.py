@@ -234,6 +234,11 @@ _SIGS = {
         [C.POINTER(C.c_void_p), C.c_int, C.c_int, C.POINTER(StencilVTerm), C.c_int, Pitched, Pitched, Pitched, C.POINTER(Pitched), C.c_int,
          C.c_int, C.c_int, I3, C.c_int64, C.c_int, C.POINTER(C.c_int64), C.POINTER(C.c_int64)],
     ),
+    "sb_stencil_dplan_create": (
+        C.c_int,
+        [C.POINTER(C.c_void_p), C.c_int, C.c_int, C.POINTER(StencilVTerm), C.c_int, Pitched, Pitched, Pitched, C.POINTER(Pitched), C.c_int,
+         C.c_double, C.c_int, C.c_int, I3, C.c_int64, C.c_int, C.POINTER(C.c_int64), C.POINTER(C.c_int64)],
+    ),
     "sb_stencil_sys_check": (C.c_int, [C.POINTER(StencilSysTerm), C.c_int, C.c_int, C.c_int, I27]),
     "sb_stencil_grad": (C.c_int, [C.c_int, C.c_double * 3, C.POINTER(StencilSysTerm), C.c_int]),
     "sb_stencil_div": (C.c_int, [C.c_int, C.c_double * 3, C.POINTER(StencilSysTerm), C.c_int]),
@@ -255,6 +260,15 @@ _SIGS = {
         C.c_int,
         [C.POINTER(C.c_void_p), C.c_int, C.c_int, C.POINTER(StencilTerm), C.c_int, Pitched, I3, C.c_int64, Pitched, I3, C.c_int64, Pitched,
          C.c_int, C.POINTER(C.c_int64), C.POINTER(C.c_int64)],
+    ),
+    "sb_transfer_voplan_create": (
+        C.c_int,
+        [C.POINTER(C.c_void_p), C.c_int, C.c_int, C.POINTER(StencilVTerm), C.c_int, Pitched, I3, C.c_int64, Pitched, I3, C.c_int64, Pitched,
+         C.POINTER(Pitched), C.c_int, C.c_int, C.POINTER(C.c_int64), C.POINTER(C.c_int64)],
+    ),
+    "sb_transfer_fplan_create": (
+        C.c_int,
+        [C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, Pitched, I3, C.c_int64, Pitched, I3, C.c_int64, I3, I3],
     ),
     "sb_transfer_plan_launch": (C.c_int, [C.c_void_p, C.c_void_p]),
     "sb_transfer_plan_bytes": (C.c_int64, [C.c_void_p]),

@@ -343,9 +343,9 @@ struct sb_stencil_plan {
   int device = 0;
   int es = 8, R = 1;
   bool has_coef = false;                // some term reads a coefficient field: the HAS_COEF kernels
-  std::vector<sb::OpCTileParams> tiles; // one tile-kernel launch per thick box
+  std::vector<sb::OpDTileParams> tiles; // one tile-kernel launch per thick box
   std::vector<int> tile_grids;
-  std::vector<sb::OpCCellParams> cells; // one cell-kernel launch per group of thin boxes
+  std::vector<sb::OpDCellParams> cells; // one cell-kernel launch per group of thin boxes
   std::vector<int> cell_grids;
   std::vector<sb::SysTileParams> sys_tiles; // a system (sb_stencil_sys_plan_create): one tile launch per thick box
   std::vector<int> sys_tile_grids;
@@ -367,6 +367,11 @@ struct sb_transfer_plan {
   std::vector<int> rop_tile_grids;
   std::vector<sb::RopCellParams> rop_cells; // one cell-kernel launch per group of thin boxes
   std::vector<int> rop_cell_grids;
+  std::vector<sb::RopVTileParams> rop_vtiles; // sb_transfer_voplan_create: the same launches with coefficient fields
+  std::vector<int> rop_vtile_grids;
+  std::vector<sb::RopVCellParams> rop_vcells;
+  std::vector<int> rop_vcell_grids;
+  int face = -1; // sb_transfer_fplan_create: the face axis of the restriction r
   int64_t bytes = 0;
 };
 
@@ -1509,6 +1514,11 @@ int sb_stencil_laplacian(int order, const double spacing[3], sb_stencil_term *ou
   return total;
 }
 
+static int stencil_plan_build(sb_stencil_plan **out, int device, int dtype, const sb_stencil_vterm *terms, int n, sb_pitched dst,
+                              sb_pitched src, sb_pitched aux, const sb_pitched *coef, int ncoef, int ncolours, int colour,
+                              const int64_t acc_origin[3], int64_t zsize, int nbox, const int64_t *lo, const int64_t *hi,
+                              const double *omega);
+
 int sb_stencil_plan_create(sb_stencil_plan **out, int device, int dtype, const sb_stencil_term *terms, int n, sb_pitched dst,
                            sb_pitched src, sb_pitched aux, const int64_t acc_origin[3], int64_t zsize, int nbox, const int64_t *lo,
                            const int64_t *hi) {
@@ -1527,16 +1537,41 @@ int sb_stencil_vplan_create(sb_stencil_plan **out, int device, int dtype, const 
 int sb_stencil_cplan_create(sb_stencil_plan **out, int device, int dtype, const sb_stencil_vterm *terms, int n, sb_pitched dst,
                             sb_pitched src, sb_pitched aux, const sb_pitched *coef, int ncoef, int ncolours, int colour,
                             const int64_t acc_origin[3], int64_t zsize, int nbox, const int64_t *lo, const int64_t *hi) {
+  return stencil_plan_build(out, device, dtype, terms, n, dst, src, aux, coef, ncoef, ncolours, colour, acc_origin, zsize, nbox, lo, hi, nullptr);
+}
+
+int sb_stencil_dplan_create(sb_stencil_plan **out, int device, int dtype, const sb_stencil_vterm *terms, int n, sb_pitched dst,
+                            sb_pitched src, sb_pitched f, const sb_pitched *coef, int ncoef, double omega, int ncolours, int colour,
+                            const int64_t acc_origin[3], int64_t zsize, int nbox, const int64_t *lo, const int64_t *hi) {
+  return stencil_plan_build(out, device, dtype, terms, n, dst, src, f, coef, ncoef, ncolours, colour, acc_origin, zsize, nbox, lo, hi, &omega);
+}
+
+// sb_stencil_cplan_create, and with omega non-NULL sb_stencil_dplan_create (aux is f)
+static int stencil_plan_build(sb_stencil_plan **out, int device, int dtype, const sb_stencil_vterm *terms, int n, sb_pitched dst,
+                              sb_pitched src, sb_pitched aux, const sb_pitched *coef, int ncoef, int ncolours, int colour,
+                              const int64_t acc_origin[3], int64_t zsize, int nbox, const int64_t *lo, const int64_t *hi,
+                              const double *omega) {
   if (!out) return fail(SB_ERR_INVALID, "sb_stencil_plan_create needs an output handle");
   if (dtype != SB_DTYPE_F32 && dtype != SB_DTYPE_F64) return fail(SB_ERR_INVALID, "dtype %d must be SB_DTYPE_F32 or SB_DTYPE_F64", dtype);
   const int es = dtype == SB_DTYPE_F32 ? 4 : 8;
   int rc = stencil_terms_ok(terms, n);
   if (rc != SB_OK) return rc;
+  const bool diag = omega != nullptr;
+  unsigned long long centre = 0;
+  if (diag) {
+    for (int t = 0; t < n; ++t) {
+      if (terms[t].source == 1) return fail(SB_ERR_INVALID, "sb_stencil_dplan_create: term %d reads aux; A reads src only (f goes on aux)", t);
+      if (!terms[t].offset[0] && !terms[t].offset[1] && !terms[t].offset[2]) centre |= 1ull << t;
+    }
+    if (!centre) return fail(SB_ERR_INVALID, "sb_stencil_dplan_create: A has no term at offset (0, 0, 0), so no diagonal");
+    if (!std::isfinite(*omega)) return fail(SB_ERR_INVALID, "sb_stencil_dplan_create: omega = %g must be finite", *omega);
+    if (!aux.ptr) return fail(SB_ERR_INVALID, "sb_stencil_dplan_create: f is NULL");
+  }
   if ((rc = stencil_colours_ok(terms, n, ncolours)) != SB_OK) return rc;
   if (colour < 0 || colour >= ncolours) return fail(SB_ERR_INVALID, "colour %d: 0 .. %d under %d colours", colour, ncolours - 1, ncolours);
   if (ncoef < 0 || ncoef > SB_STENCIL_MAX_COEFS) return fail(SB_ERR_INVALID, "ncoef %d: 0 to %d coefficient fields", ncoef, SB_STENCIL_MAX_COEFS);
   if (ncoef > 0 && !coef) return fail(SB_ERR_INVALID, "ncoef %d, but the coefficient array is NULL", ncoef);
-  bool has_aux = false;
+  bool has_aux = diag; // the diagonal mode reads f on aux
   int rm[3] = {0, 0, 0}, rp[3] = {0, 0, 0}, R = 1;
   // coefficient fields the op references, renumbered 0 .. nf - 1 in order of their index, with their reach per axis
   int fmap[SB_STENCIL_MAX_COEFS] = {-1, -1, -1, -1}, fsrc[SB_STENCIL_MAX_COEFS] = {}, nf = 0;
@@ -1567,7 +1602,7 @@ int sb_stencil_cplan_create(sb_stencil_plan **out, int device, int dtype, const 
       }
   if (has_aux && !aux.ptr) return fail(SB_ERR_INVALID, "the op has a term on aux, but aux is NULL");
   if (!dst.ptr || !src.ptr) return fail(SB_ERR_INVALID, "dst and src must not be NULL");
-  if (dst.ptr == src.ptr && ncolours == 1) return fail(SB_ERR_INVALID, "dst must not be src (dst may be aux)");
+  if (dst.ptr == src.ptr && ncolours == 1) return fail(SB_ERR_INVALID, "dst must not be src (dst may be %s)", diag ? "f" : "aux");
   for (int f = 0; f < nf; ++f)
     if (coef[fsrc[f]].ptr == dst.ptr) return fail(SB_ERR_INVALID, "coefficient field %d is dst (coefficients are read only)", fsrc[f]);
   std::vector<const sb_pitched *> bufs = {&dst, &src};
@@ -1608,6 +1643,7 @@ int sb_stencil_cplan_create(sb_stencil_plan **out, int device, int dtype, const 
   }
   sb::OpColour col{ncolours, colour, {}};
   for (int a = 0; a < 3; ++a) col.par[a] = int(((acc_origin[a] % 2) + 2) % 2);
+  sb::OpDiag dg{diag ? 1 : 0, centre, diag ? *omega : 0.0, diag ? float(*omega) : 0.0f};
 
   sb::OpCommon com{};
   com.dst = static_cast<char *>(dst.ptr);
@@ -1634,7 +1670,7 @@ int sb_stencil_cplan_create(sb_stencil_plan **out, int device, int dtype, const 
   p->has_coef = nf > 0;
   p->bytes = cells * es * ((has_aux ? 2 : 1) + nf) + written * es;
   if (!thick.empty()) {
-    const int per_sm = sb::op_tile_prepare(R, es, device, nf, ncolours > 1);
+    const int per_sm = sb::op_tile_prepare(R, es, device, nf, ncolours > 1, diag);
     if (per_sm <= 0) {
       delete p;
       return fail(SB_ERR_CUDA, "the R = %d tile kernel cannot be configured: %s", R, cudaGetErrorString(cudaGetLastError()));
@@ -1642,9 +1678,10 @@ int sb_stencil_cplan_create(sb_stencil_plan **out, int device, int dtype, const 
     const int SW = sb::op_tile_sw(R), P = sb::op_tile_plane(R), NS = 2 * R + 1;
     const int CSW = sb::op_tile_sw(1), CP = sb::op_tile_plane(1), CS = sb::kOpCoefSlots;
     for (const auto &b : thick) {
-      sb::OpCTileParams tp{};
+      sb::OpDTileParams tp{};
       tp.c = com;
       tp.col = col;
+      tp.dg = dg;
       tp.k.nf = nf;
       for (int f = 0; f < nf; ++f) {
         tp.k.coef[f] = static_cast<const char *>(coef[fsrc[f]].ptr);
@@ -1689,9 +1726,10 @@ int sb_stencil_cplan_create(sb_stencil_plan **out, int device, int dtype, const 
     }
   }
   for (size_t b0 = 0; b0 < thin.size(); b0 += sb::kOpMaxBoxes) {
-    sb::OpCCellParams cp{};
+    sb::OpDCellParams cp{};
     cp.c = com;
     cp.col = col;
+    cp.dg = dg;
     for (int t = 0; t < n; ++t)
       cp.goff[t] = (long long)terms[t].offset[2] * com.slice + (long long)terms[t].offset[1] * com.pitch + (long long)terms[t].offset[0] * es;
     for (int f = 0; f < nf; ++f) cp.coef[f] = static_cast<const char *>(coef[fsrc[f]].ptr);
@@ -2074,19 +2112,39 @@ int sb_transfer_check(const int64_t fine_dim[3], const int64_t coarse_dim[3], co
   return SB_OK;
 }
 
+// sb_transfer_plan_create, and with face >= 0 (a restriction) sb_transfer_fplan_create
+static int transfer_plan_build(sb_transfer_plan **out, int device, int dtype, int kind, sb_pitched dst, const int64_t dst_acc_origin[3],
+                               int64_t dst_zsize, sb_pitched src, const int64_t src_acc_origin[3], int64_t src_zsize, sb_pitched aux,
+                               const int64_t lo[3], const int64_t hi[3], int face, const char *fn);
+
 int sb_transfer_plan_create(sb_transfer_plan **out, int device, int dtype, int kind, sb_pitched dst, const int64_t dst_acc_origin[3],
                             int64_t dst_zsize, sb_pitched src, const int64_t src_acc_origin[3], int64_t src_zsize, sb_pitched aux,
                             const int64_t lo[3], const int64_t hi[3]) {
-  if (!out) return fail(SB_ERR_INVALID, "sb_transfer_plan_create needs an output handle");
-  if (dtype != SB_DTYPE_F32 && dtype != SB_DTYPE_F64) return fail(SB_ERR_INVALID, "dtype %d must be SB_DTYPE_F32 or SB_DTYPE_F64", dtype);
   if (kind != SB_TRANSFER_RESTRICT && kind != SB_TRANSFER_PROLONG)
     return fail(SB_ERR_INVALID, "kind %d must be SB_TRANSFER_RESTRICT or SB_TRANSFER_PROLONG", kind);
+  return transfer_plan_build(out, device, dtype, kind, dst, dst_acc_origin, dst_zsize, src, src_acc_origin, src_zsize, aux, lo, hi, -1,
+                             "sb_transfer_plan_create");
+}
+
+int sb_transfer_fplan_create(sb_transfer_plan **out, int device, int dtype, int axis, sb_pitched dst, const int64_t dst_acc_origin[3],
+                             int64_t dst_zsize, sb_pitched src, const int64_t src_acc_origin[3], int64_t src_zsize,
+                             const int64_t lo[3], const int64_t hi[3]) {
+  if (axis < 0 || axis > 2) return fail(SB_ERR_INVALID, "sb_transfer_fplan_create: axis %d must be 0, 1 or 2", axis);
+  return transfer_plan_build(out, device, dtype, SB_TRANSFER_RESTRICT, dst, dst_acc_origin, dst_zsize, src, src_acc_origin, src_zsize,
+                             sb_pitched{nullptr, 0, 0}, lo, hi, axis, "sb_transfer_fplan_create");
+}
+
+static int transfer_plan_build(sb_transfer_plan **out, int device, int dtype, int kind, sb_pitched dst, const int64_t dst_acc_origin[3],
+                               int64_t dst_zsize, sb_pitched src, const int64_t src_acc_origin[3], int64_t src_zsize, sb_pitched aux,
+                               const int64_t lo[3], const int64_t hi[3], int face, const char *fn) {
+  if (!out) return fail(SB_ERR_INVALID, "%s needs an output handle", fn);
+  if (dtype != SB_DTYPE_F32 && dtype != SB_DTYPE_F64) return fail(SB_ERR_INVALID, "dtype %d must be SB_DTYPE_F32 or SB_DTYPE_F64", dtype);
   const int es = dtype == SB_DTYPE_F32 ? 4 : 8;
   const bool prolong = kind == SB_TRANSFER_PROLONG, has_aux = aux.ptr != nullptr;
   if (!dst.ptr || !src.ptr) return fail(SB_ERR_INVALID, "dst and src must not be NULL");
   if (dst.ptr == src.ptr) return fail(SB_ERR_INVALID, "dst must not be src");
   if (has_aux && !prolong) return fail(SB_ERR_INVALID, "a restriction takes no aux");
-  if (!dst_acc_origin || !src_acc_origin || !lo || !hi) return fail(SB_ERR_INVALID, "sb_transfer_plan_create needs both acc_origins, lo and hi");
+  if (!dst_acc_origin || !src_acc_origin || !lo || !hi) return fail(SB_ERR_INVALID, "%s needs both acc_origins, lo and hi", fn);
   if (dst_zsize < 1 || src_zsize < 1) return fail(SB_ERR_INVALID, "dst_zsize and src_zsize must be >= 1");
   int rc = stencil_buffers_ok({&dst}, {"dst"}, dst, "dst", es);
   if (rc == SB_OK) rc = stencil_buffers_ok({&src}, {"src"}, src, "src", es);
@@ -2134,6 +2192,7 @@ int sb_transfer_plan_create(sb_transfer_plan **out, int device, int dtype, int k
   p->device = device;
   p->es = es;
   p->kind = kind;
+  p->face = face;
   const int64_t cells = e[0] * e[1] * e[2];
   if (!prolong) {
     sb::RestrictParams &r = p->r;
@@ -2148,7 +2207,7 @@ int sb_transfer_plan_create(sb_transfer_plan **out, int device, int dtype, int k
       r.ext[a] = int(e[a]);
       r.flo[a] = int(rl[a]);
     }
-    p->bytes = (8 + 1) * cells * es;
+    p->bytes = (face >= 0 ? 4 + 1 : 8 + 1) * cells * es;
     p->launches = 1;
   } else {
     sb::ProlongParams &q = p->pr;
@@ -2197,34 +2256,67 @@ int sb_transfer_plan_create(sb_transfer_plan **out, int device, int dtype, int k
   return SB_OK;
 }
 
+static int transfer_oplan_build(const char *fn, sb_transfer_plan **out, int device, int dtype, const sb_stencil_vterm *terms, int n,
+                                sb_pitched dst, const int64_t dst_acc_origin[3], int64_t dst_zsize, sb_pitched src,
+                                const int64_t src_acc_origin[3], int64_t src_zsize, sb_pitched aux, const sb_pitched *coef, int ncoef,
+                                int nbox, const int64_t *lo, const int64_t *hi);
+
 int sb_transfer_oplan_create(sb_transfer_plan **out, int device, int dtype, const sb_stencil_term *terms, int n, sb_pitched dst,
                              const int64_t dst_acc_origin[3], int64_t dst_zsize, sb_pitched src, const int64_t src_acc_origin[3],
                              int64_t src_zsize, sb_pitched aux, int nbox, const int64_t *lo, const int64_t *hi) {
-  if (!out) return fail(SB_ERR_INVALID, "sb_transfer_oplan_create needs an output handle");
+  const std::vector<sb_stencil_vterm> vt = stencil_vterms_of(terms, n);
+  return transfer_oplan_build("sb_transfer_oplan_create", out, device, dtype, terms ? vt.data() : nullptr, n, dst, dst_acc_origin, dst_zsize,
+                              src, src_acc_origin, src_zsize, aux, nullptr, 0, nbox, lo, hi);
+}
+
+int sb_transfer_voplan_create(sb_transfer_plan **out, int device, int dtype, const sb_stencil_vterm *terms, int n, sb_pitched dst,
+                              const int64_t dst_acc_origin[3], int64_t dst_zsize, sb_pitched src, const int64_t src_acc_origin[3],
+                              int64_t src_zsize, sb_pitched aux, const sb_pitched *coef, int ncoef, int nbox, const int64_t *lo,
+                              const int64_t *hi) {
+  return transfer_oplan_build("sb_transfer_voplan_create", out, device, dtype, terms, n, dst, dst_acc_origin, dst_zsize, src, src_acc_origin,
+                              src_zsize, aux, coef, ncoef, nbox, lo, hi);
+}
+
+static int transfer_oplan_build(const char *fn, sb_transfer_plan **out, int device, int dtype, const sb_stencil_vterm *terms, int n,
+                                sb_pitched dst, const int64_t dst_acc_origin[3], int64_t dst_zsize, sb_pitched src,
+                                const int64_t src_acc_origin[3], int64_t src_zsize, sb_pitched aux, const sb_pitched *coef, int ncoef,
+                                int nbox, const int64_t *lo, const int64_t *hi) {
+  if (!out) return fail(SB_ERR_INVALID, "%s needs an output handle", fn);
   if (dtype != SB_DTYPE_F32 && dtype != SB_DTYPE_F64) return fail(SB_ERR_INVALID, "dtype %d must be SB_DTYPE_F32 or SB_DTYPE_F64", dtype);
   const int es = dtype == SB_DTYPE_F32 ? 4 : 8;
-  const std::vector<sb_stencil_vterm> vt = stencil_vterms_of(terms, n);
-  int rc = stencil_terms_ok(terms ? vt.data() : nullptr, n);
+  int rc = stencil_terms_ok(terms, n);
   if (rc != SB_OK) return rc;
-  bool aux_term = false;
+  if (ncoef < 0 || ncoef > SB_STENCIL_MAX_COEFS) return fail(SB_ERR_INVALID, "ncoef %d: 0 to %d coefficient fields", ncoef, SB_STENCIL_MAX_COEFS);
+  if (ncoef > 0 && !coef) return fail(SB_ERR_INVALID, "ncoef %d, but the coefficient array is NULL", ncoef);
+  bool aux_term = false, used[SB_STENCIL_MAX_COEFS] = {};
   for (int t = 0; t < n; ++t) {
     aux_term = aux_term || terms[t].source == 1;
     for (int a = 0; a < 3; ++a)
       if (terms[t].offset[a] < -1 || terms[t].offset[a] > 1)
         return fail(SB_ERR_INVALID, "term %d: offset (%d, %d, %d) reaches beyond 1 cell, the fused restriction's limit", t,
                     int(terms[t].offset[0]), int(terms[t].offset[1]), int(terms[t].offset[2]));
+    const int k = terms[t].coef;
+    if (k >= ncoef) return fail(SB_ERR_INVALID, "term %d names coefficient field %d, but ncoef is %d", t, k, ncoef);
+    if (k >= 0 && !coef[k].ptr) return fail(SB_ERR_INVALID, "coefficient field %d is NULL", k);
+    if (k >= 0) used[k] = true;
   }
   if (aux_term && !aux.ptr) return fail(SB_ERR_INVALID, "a term reads aux, but aux is NULL");
   if (!dst.ptr || !src.ptr) return fail(SB_ERR_INVALID, "dst and src must not be NULL");
   if (dst.ptr == src.ptr) return fail(SB_ERR_INVALID, "dst must not be src");
   if (aux_term && dst.ptr == aux.ptr) return fail(SB_ERR_INVALID, "dst must not be aux");
-  if (!dst_acc_origin || !src_acc_origin) return fail(SB_ERR_INVALID, "sb_transfer_oplan_create needs both acc_origins");
+  for (int k = 0; k < ncoef; ++k)
+    if (used[k] && coef[k].ptr == dst.ptr) return fail(SB_ERR_INVALID, "coefficient field %d is dst (coefficients are read only)", k);
+  if (!dst_acc_origin || !src_acc_origin) return fail(SB_ERR_INVALID, "%s needs both acc_origins", fn);
   if (nbox < 0 || (nbox > 0 && (!lo || !hi))) return fail(SB_ERR_INVALID, "nbox %d boxes need lo and hi arrays", nbox);
   if (dst_zsize < 1 || src_zsize < 1) return fail(SB_ERR_INVALID, "dst_zsize and src_zsize must be >= 1");
   rc = stencil_buffers_ok({&dst}, {"dst"}, dst, "dst", es);
   if (rc == SB_OK) rc = stencil_buffers_ok({&src}, {"src"}, src, "src", es);
   if (rc == SB_OK && aux_term) rc = stencil_buffers_ok({&aux}, {"aux"}, src, "src", es);
+  for (int k = 0; k < ncoef && rc == SB_OK; ++k)
+    if (used[k]) rc = stencil_buffers_ok({&coef[k]}, {"coefficient field " + std::to_string(k)}, src, "src", es);
   if (rc != SB_OK) return rc;
+  int nf = 0;
+  for (int k = 0; k < ncoef; ++k) nf += used[k] ? 1 : 0;
   const int64_t dsize[3] = {dst.pitch / es, dst.ysize, dst_zsize}, ssize[3] = {src.pitch / es, src.ysize, src_zsize};
   const int zero[3] = {0, 0, 0}, one[3] = {1, 1, 1};
   // per box: coarse lo, extent (dst allocation coordinates), fine 2 * lo (src allocation coordinates)
@@ -2270,7 +2362,7 @@ int sb_transfer_oplan_create(sb_transfer_plan **out, int device, int dtype, cons
   p->es = es;
   p->kind = SB_TRANSFER_RESTRICT;
   p->fused = true;
-  p->bytes = cells * es * (8 * (aux_term ? 2 : 1) + 1);
+  p->bytes = cells * es * (8 * ((aux_term ? 2 : 1) + nf) + 1);
   if (cells == 0) {
     *out = p;
     return SB_OK;
@@ -2286,7 +2378,7 @@ int sb_transfer_oplan_create(sb_transfer_plan **out, int device, int dtype, cons
     return fail(SB_ERR_CUDA, "cudaDeviceGetAttribute: %s", cudaGetErrorString(cudaGetLastError()));
   }
   if (!thick.empty()) {
-    const int per_sm = sb::rop_tile_ctas_per_sm(es);
+    const int per_sm = sb::rop_tile_ctas_per_sm(es, nf > 0);
     if (per_sm <= 0) {
       delete p;
       return fail(SB_ERR_CUDA, "the fused restriction's tile kernel cannot be configured: %s", cudaGetErrorString(cudaGetLastError()));
@@ -2319,8 +2411,21 @@ int sb_transfer_oplan_create(sb_transfer_plan **out, int device, int dtype, cons
         delete p;
         return fail(SB_ERR_INVALID, "box too large for the fused restriction's tile kernel");
       }
-      p->rop_tiles.push_back(tp);
-      p->rop_tile_grids.push_back(int(grid));
+      if (nf == 0) {
+        p->rop_tiles.push_back(tp);
+        p->rop_tile_grids.push_back(int(grid));
+        continue;
+      }
+      sb::RopVTileParams vp{};
+      static_cast<sb::RopTileParams &>(vp) = tp;
+      for (int k = 0; k < ncoef; ++k) vp.coef[k] = static_cast<const char *>(coef[k].ptr);
+      for (int t = 0; t < n; ++t) {
+        const int32_t *c = terms[t].coef_offset;
+        vp.cfield[t] = (signed char)terms[t].coef;
+        vp.cgoff[t] = (long long)c[2] * com.sslice + (long long)c[1] * com.spitch + (long long)c[0] * es;
+      }
+      p->rop_vtiles.push_back(vp);
+      p->rop_vtile_grids.push_back(int(grid));
     }
   }
   for (size_t b0 = 0; b0 < thin.size(); b0 += sb::kRopMaxBoxes) {
@@ -2336,10 +2441,23 @@ int sb_transfer_oplan_create(sb_transfer_plan **out, int device, int dtype, cons
       }
       cp.first[m + 1] = cp.first[m] + (long long)thin[b][3] * thin[b][4] * thin[b][5];
     }
-    p->rop_cells.push_back(cp);
-    p->rop_cell_grids.push_back(int(std::min<long long>((cp.first[cp.n] + 255) / 256, 32ll * sms)));
+    const int grid = int(std::min<long long>((cp.first[cp.n] + 255) / 256, 32ll * sms));
+    if (nf == 0) {
+      p->rop_cells.push_back(cp);
+      p->rop_cell_grids.push_back(grid);
+      continue;
+    }
+    sb::RopVCellParams vp{};
+    static_cast<sb::RopCellParams &>(vp) = cp;
+    for (int k = 0; k < ncoef; ++k) vp.coef[k] = static_cast<const char *>(coef[k].ptr);
+    for (int t = 0; t < n; ++t) {
+      vp.cfield[t] = (signed char)terms[t].coef;
+      for (int a = 0; a < 3; ++a) vp.coff[t][a] = (signed char)terms[t].coef_offset[a];
+    }
+    p->rop_vcells.push_back(vp);
+    p->rop_vcell_grids.push_back(grid);
   }
-  p->launches = int(p->rop_tiles.size() + p->rop_cells.size());
+  p->launches = int(p->rop_tiles.size() + p->rop_cells.size() + p->rop_vtiles.size() + p->rop_vcells.size());
   *out = p;
   return SB_OK;
 }
@@ -2353,8 +2471,12 @@ int sb_transfer_plan_launch(sb_transfer_plan *p, void *stream) {
   if (p->fused) {
     for (size_t i = 0; i < p->rop_tiles.size(); ++i) g_launches += uint64_t(sb::launch_rop_tile(p->rop_tiles[i], p->es, p->rop_tile_grids[i], s));
     for (size_t i = 0; i < p->rop_cells.size(); ++i) g_launches += uint64_t(sb::launch_rop_cells(p->rop_cells[i], p->es, p->rop_cell_grids[i], s));
+    for (size_t i = 0; i < p->rop_vtiles.size(); ++i) g_launches += uint64_t(sb::launch_rop_vtile(p->rop_vtiles[i], p->es, p->rop_vtile_grids[i], s));
+    for (size_t i = 0; i < p->rop_vcells.size(); ++i) g_launches += uint64_t(sb::launch_rop_vcells(p->rop_vcells[i], p->es, p->rop_vcell_grids[i], s));
   } else {
-    g_launches += uint64_t(p->kind == SB_TRANSFER_PROLONG ? sb::launch_prolong(p->pr, p->es, p->grid, s) : sb::launch_restrict(p->r, p->es, s));
+    g_launches += uint64_t(p->kind == SB_TRANSFER_PROLONG ? sb::launch_prolong(p->pr, p->es, p->grid, s)
+                           : p->face >= 0             ? sb::launch_face_restrict(p->r, p->es, p->face, s)
+                                                      : sb::launch_restrict(p->r, p->es, s));
   }
   SB_CUDA(cudaGetLastError());
   return SB_OK;

@@ -25,6 +25,9 @@
 // colouring m (2 or 8, from global coordinates) are written, and dst may be src.  In a tile row the cells of a colour
 // alternate along x, so each lane computes one of them (cell 2 * lane + s); the cell kernel skips the other cells.
 // src is read with plain loads, since the launch may write it.
+//
+// Diagonal relaxation (DIAG, DESIGN.md section 2.12; with COL, a compile-time switch): a cell of the colour gets
+// u + omega ((f - A u) / d), f on aux and d the sum of the offset-0 terms' factors, formed in the same term loop.
 #include "stencil_op.cuh"
 
 #include <cstring>
@@ -38,11 +41,15 @@ template <> struct OpNum<float> {
   static __device__ __forceinline__ float mul(float a, float b) { return __fmul_rn(a, b); }
   static __device__ __forceinline__ float add(float a, float b) { return __fadd_rn(a, b); }
   static __device__ __forceinline__ float w(const OpCommon &c, int t) { return c.wf[t]; }
+  static __device__ __forceinline__ float sub(float a, float b) { return __fsub_rn(a, b); }
+  static __device__ __forceinline__ float div(float a, float b) { return __fdiv_rn(a, b); }
 };
 template <> struct OpNum<double> {
   static __device__ __forceinline__ double mul(double a, double b) { return __dmul_rn(a, b); }
   static __device__ __forceinline__ double add(double a, double b) { return __dadd_rn(a, b); }
   static __device__ __forceinline__ double w(const OpCommon &c, int t) { return c.w[t]; }
+  static __device__ __forceinline__ double sub(double a, double b) { return __dsub_rn(a, b); }
+  static __device__ __forceinline__ double div(double a, double b) { return __ddiv_rn(a, b); }
 };
 
 // one element global -> shared, asynchronously (cp.async, sm_80+); completion by cp_async_wait_all
@@ -59,13 +66,16 @@ template <bool COL, typename V> __device__ __forceinline__ V src_load(const V *a
   else return __ldg(a);
 }
 
-template <bool HAS_COEF, bool COL>
-using OpTileParamsOf = typename std::conditional<COL, OpCTileParams, typename std::conditional<HAS_COEF, OpVTileParams, OpTileParams>::type>::type;
+template <bool HAS_COEF, bool COL, bool DIAG = false>
+using OpTileParamsOf = typename std::conditional<
+    DIAG, OpDTileParams,
+    typename std::conditional<COL, OpCTileParams, typename std::conditional<HAS_COEF, OpVTileParams, OpTileParams>::type>::type>::type;
 
 // COL: the coloured kernel.  Each warp row holds 32 cells of the colour at most (one colour of two alternates along x),
-// so each lane computes one of them: the cell 2 * lane + s of the row, with s the row's colour phase.
-template <typename T, int R, bool HAS_COEF, bool COL>
-__global__ void __launch_bounds__(kOpThreads, 2) op_tile_kernel(const __grid_constant__ OpTileParamsOf<HAS_COEF, COL> p) {
+// so each lane computes one of them: the cell 2 * lane + s of the row, with s the row's colour phase.  DIAG (always with
+// COL): the diagonal relaxation; under m = 1 each lane computes the cells 2 * lane and 2 * lane + 1.
+template <typename T, int R, bool HAS_COEF, bool COL, bool DIAG = false>
+__global__ void __launch_bounds__(kOpThreads, 2) op_tile_kernel(const __grid_constant__ OpTileParamsOf<HAS_COEF, COL, DIAG> p) {
   extern __shared__ __align__(16) unsigned char op_smem[];
   T *ring = reinterpret_cast<T *>(op_smem);
   constexpr int SW = op_tile_sw(R), P = op_tile_plane(R), NS = 2 * R + 1;
@@ -194,6 +204,42 @@ __global__ void __launch_bounds__(kOpThreads, 2) op_tile_kernel(const __grid_con
       *reinterpret_cast<T *>(p.c.dst + at) = acc;
     }
   };
+  // DIAG: the cells of the colour in this warp's row of plane zc, each u + omega ((f - A u) / d); f is aux
+  auto diag_row = [&](int zc, long long cell) {
+    if constexpr (DIAG) {
+      const int gx = x0 + p.col.par[0], gy = y + p.col.par[1], gz = zc + p.col.par[2], c = p.col.c, m = p.col.m;
+      const bool on = m <= 2 || (((gy ^ (c >> 1)) | (gz ^ (c >> 2))) & 1) == 0;
+      const int s = m == 1 ? 0 : (m == 2 ? c - gx - gy - gz : c - gx) & 1;
+      if (!on || y >= ye) return;
+      const int sl = slot_of(zc);
+      for (int k = 0; k < (m == 1 ? 2 : 1); ++k) {
+        const int xl = 2 * lane + s + k, x = x0 + xl;
+        if (x >= xe) break;
+        const long long at = cell + x * ES;
+        const T f = *reinterpret_cast<const T *>(p.c.aux + at); // before the write: dst may be aux
+        const T *const o1 = ring + (wy + R) * SW + R + xl;
+        T acc = T(0), d = T(0);
+        bool first = true;
+        for (int t = 0; t < p.c.n; ++t) {
+          T w = OpNum<T>::w(p.c, t);
+          if constexpr (HAS_COEF) {
+            const T *const co1 = cring + (wy + 1) * CSW + 1 + xl;
+            const int cs = (zc - z0 + 1) & (kOpCoefSlots - 1);
+            if (p.k.cfield[t] >= 0) w = OpNum<T>::mul(w, co1[p.k.coff[cs][t]]);
+          }
+          const T mt = OpNum<T>::mul(w, o1[p.toff[sl][t]]);
+          acc = t == 0 ? mt : OpNum<T>::add(acc, mt);
+          if ((p.dg.centre >> t) & 1ull) {
+            d = first ? w : OpNum<T>::add(d, w);
+            first = false;
+          }
+        }
+        const T u = o1[sl * P];
+        const T om = sizeof(T) == 4 ? T(p.dg.omegaf) : T(p.dg.omega);
+        *reinterpret_cast<T *>(p.c.dst + at) = OpNum<T>::add(u, OpNum<T>::mul(om, OpNum<T>::div(OpNum<T>::sub(f, acc), d)));
+      }
+    }
+  };
   for (int zc = z0; zc < z1; ++zc) {
     store(slot_of(zc + p.rp[2])); // the slot of plane zc + rp - (2R + 1), which no cell of plane zc reads
     if constexpr (HAS_COEF) cp_async_wait_all(); // this thread's coefficient planes up to zc + crp have landed
@@ -204,7 +250,11 @@ __global__ void __launch_bounds__(kOpThreads, 2) op_tile_kernel(const __grid_con
         for (int f = 0; f < p.k.nf; ++f) coef_plane(f, zc + 1 + p.k.crp[f][2]);
     }
     const long long cell = (long long)zc * p.c.slice + (long long)y * p.c.pitch;
-    if constexpr (COL) {
+    if constexpr (DIAG) {
+      diag_row(zc, cell);
+      __syncthreads();
+      continue;
+    } else if constexpr (COL) {
       coloured_row(zc, cell);
       __syncthreads();
       continue;
@@ -252,12 +302,15 @@ __global__ void __launch_bounds__(kOpThreads, 2) op_tile_kernel(const __grid_con
   }
 }
 
-template <bool HAS_COEF, bool COL>
-using OpCellParamsOf = typename std::conditional<COL, OpCCellParams, typename std::conditional<HAS_COEF, OpVCellParams, OpCellParams>::type>::type;
+template <bool HAS_COEF, bool COL, bool DIAG = false>
+using OpCellParamsOf = typename std::conditional<
+    DIAG, OpDCellParams,
+    typename std::conditional<COL, OpCCellParams, typename std::conditional<HAS_COEF, OpVCellParams, OpCellParams>::type>::type>::type;
 
-// COL: the coloured kernel; a thread whose cell is of another colour does nothing
-template <typename T, bool HAS_COEF, bool COL>
-__global__ void __launch_bounds__(256) op_cell_kernel(const __grid_constant__ OpCellParamsOf<HAS_COEF, COL> p) {
+// COL: the coloured kernel; a thread whose cell is of another colour does nothing.  DIAG (always with COL): the
+// diagonal relaxation, every cell under m = 1.
+template <typename T, bool HAS_COEF, bool COL, bool DIAG = false>
+__global__ void __launch_bounds__(256) op_cell_kernel(const __grid_constant__ OpCellParamsOf<HAS_COEF, COL, DIAG> p) {
   const long long total = p.first[p.n];
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     int k = 0;
@@ -276,7 +329,11 @@ __global__ void __launch_bounds__(256) op_cell_kernel(const __grid_constant__ Op
       xx = t % ex;
       zz = t / ex;
     }
-    if constexpr (COL) {
+    if constexpr (DIAG) {
+      const int gx = p.lo[k][0] + int(xx) + p.col.par[0], gy = p.lo[k][1] + int(yy) + p.col.par[1], gz = p.lo[k][2] + int(zz) + p.col.par[2];
+      const int colour = p.col.m == 1 ? 0 : p.col.m == 2 ? (gx + gy + gz) & 1 : (gx & 1) | (gy & 1) << 1 | (gz & 1) << 2;
+      if (colour != p.col.c) continue;
+    } else if constexpr (COL) {
       const int gx = p.lo[k][0] + int(xx) + p.col.par[0], gy = p.lo[k][1] + int(yy) + p.col.par[1], gz = p.lo[k][2] + int(zz) + p.col.par[2];
       const int colour = p.col.m == 2 ? (gx + gy + gz) & 1 : (gx & 1) | (gy & 1) << 1 | (gz & 1) << 2;
       if (colour != p.col.c) continue;
@@ -284,6 +341,28 @@ __global__ void __launch_bounds__(256) op_cell_kernel(const __grid_constant__ Op
     const long long off = (long long)(p.lo[k][2] + (int)zz) * p.c.slice + (long long)(p.lo[k][1] + (int)yy) * p.c.pitch +
                           (long long)(p.lo[k][0] + (int)xx) * (long long)sizeof(T);
     const char *s = p.c.src + off;
+    if constexpr (DIAG) { // u + omega ((f - A u) / d); f is aux, read before the write (dst may be aux)
+      const T f = *reinterpret_cast<const T *>(p.c.aux + off);
+      T acc = T(0), d = T(0);
+      bool first = true;
+      for (int t = 0; t < p.c.n; ++t) {
+        T w = OpNum<T>::w(p.c, t);
+        if constexpr (HAS_COEF) {
+          const int fi = p.cfield[t];
+          if (fi >= 0) w = OpNum<T>::mul(w, __ldg(reinterpret_cast<const T *>(p.coef[fi] + off + p.cgoff[t])));
+        }
+        const T m = OpNum<T>::mul(w, *reinterpret_cast<const T *>(s + p.goff[t]));
+        acc = t == 0 ? m : OpNum<T>::add(acc, m);
+        if ((p.dg.centre >> t) & 1ull) {
+          d = first ? w : OpNum<T>::add(d, w);
+          first = false;
+        }
+      }
+      const T u = *reinterpret_cast<const T *>(s);
+      const T om = sizeof(T) == 4 ? T(p.dg.omegaf) : T(p.dg.omega);
+      *reinterpret_cast<T *>(p.c.dst + off) = OpNum<T>::add(u, OpNum<T>::mul(om, OpNum<T>::div(OpNum<T>::sub(f, acc), d)));
+      continue;
+    }
     const T a = p.c.has_aux ? *reinterpret_cast<const T *>(p.c.aux + off) : T(0); // before the write: dst may be aux
     T acc = T(0);
     for (int t = 0; t < p.c.n; ++t) {
@@ -303,18 +382,23 @@ __global__ void __launch_bounds__(256) op_cell_kernel(const __grid_constant__ Op
 template <typename T, int R, bool COL> const void *tile_fn(bool coef) {
   return coef ? reinterpret_cast<const void *>(&op_tile_kernel<T, R, true, COL>) : reinterpret_cast<const void *>(&op_tile_kernel<T, R, false, COL>);
 }
-template <typename T, int R> const void *tile_fn(bool coef, bool col) { return col ? tile_fn<T, R, true>(coef) : tile_fn<T, R, false>(coef); }
+template <typename T, int R> const void *tile_fn(bool coef, bool col, bool diag) {
+  if (diag)
+    return coef ? reinterpret_cast<const void *>(&op_tile_kernel<T, R, true, true, true>)
+                : reinterpret_cast<const void *>(&op_tile_kernel<T, R, false, true, true>);
+  return col ? tile_fn<T, R, true>(coef) : tile_fn<T, R, false>(coef);
+}
 
-const void *tile_kernel(int R, int es, bool coef, bool col) {
+const void *tile_kernel(int R, int es, bool coef, bool col, bool diag) {
   switch (R * 10 + es) {
-  case 14: return tile_fn<float, 1>(coef, col);
-  case 24: return tile_fn<float, 2>(coef, col);
-  case 34: return tile_fn<float, 3>(coef, col);
-  case 44: return tile_fn<float, 4>(coef, col);
-  case 18: return tile_fn<double, 1>(coef, col);
-  case 28: return tile_fn<double, 2>(coef, col);
-  case 38: return tile_fn<double, 3>(coef, col);
-  case 48: return tile_fn<double, 4>(coef, col);
+  case 14: return tile_fn<float, 1>(coef, col, diag);
+  case 24: return tile_fn<float, 2>(coef, col, diag);
+  case 34: return tile_fn<float, 3>(coef, col, diag);
+  case 44: return tile_fn<float, 4>(coef, col, diag);
+  case 18: return tile_fn<double, 1>(coef, col, diag);
+  case 28: return tile_fn<double, 2>(coef, col, diag);
+  case 38: return tile_fn<double, 3>(coef, col, diag);
+  case 48: return tile_fn<double, 4>(coef, col, diag);
   default: return nullptr;
   }
 }
@@ -325,8 +409,8 @@ size_t op_tile_smem(int R, int es, int nf) {
   return (size_t(2 * R + 1) * size_t(op_tile_plane(R)) + size_t(nf) * kOpCoefSlots * size_t(op_tile_plane(1))) * size_t(es);
 }
 
-int op_tile_prepare(int R, int es, int device, int nf, bool col) {
-  const void *fn = tile_kernel(R, es, nf > 0, col);
+int op_tile_prepare(int R, int es, int device, int nf, bool col, bool diag) {
+  const void *fn = tile_kernel(R, es, nf > 0, col, diag);
   if (!fn) return 0;
   // the coefficient kernel's limit covers every field count, so plans with different counts can share it
   const int limit = int(op_tile_smem(R, es, nf > 0 ? kOpMaxCoefs : 0));
@@ -337,32 +421,46 @@ int op_tile_prepare(int R, int es, int device, int nf, bool col) {
   return ctas;
 }
 
-int launch_op_tile(const OpCTileParams &p, int R, int es, int grid, cudaStream_t stream) {
+int launch_op_tile(const OpDTileParams &p, int R, int es, int grid, cudaStream_t stream) {
   if (grid <= 0) return 0;
-  const bool coef = p.k.nf > 0, col = p.col.m > 1;
-  const void *fn = tile_kernel(R, es, coef, col);
+  const bool coef = p.k.nf > 0, diag = p.dg.on != 0, col = p.col.m > 1;
+  const void *fn = tile_kernel(R, es, coef, col, diag);
   if (!fn) return 0;
-  // the uncoloured kernels take the OpVTileParams part, the plain one the OpTileParams part only
-  OpCTileParams *const q = const_cast<OpCTileParams *>(&p);
-  void *args[] = {col ? static_cast<void *>(q) : coef ? static_cast<void *>(static_cast<OpVTileParams *>(q)) : static_cast<void *>(static_cast<OpTileParams *>(q))};
+  // the coloured kernels take the OpCTileParams part, the uncoloured ones the OpVTileParams part, the plain one the
+  // OpTileParams part only
+  OpDTileParams *const q = const_cast<OpDTileParams *>(&p);
+  void *args[] = {diag  ? static_cast<void *>(q)
+                  : col ? static_cast<void *>(static_cast<OpCTileParams *>(q))
+                  : coef ? static_cast<void *>(static_cast<OpVTileParams *>(q))
+                         : static_cast<void *>(static_cast<OpTileParams *>(q))};
   cudaLaunchKernel(fn, dim3(unsigned(grid)), dim3(kOpThreads), args, op_tile_smem(R, es, p.k.nf), stream);
   return 1;
 }
 
-int launch_op_cells(const OpCCellParams &p, int es, bool has_coef, int grid, cudaStream_t stream) {
+int launch_op_cells(const OpDCellParams &p, int es, bool has_coef, int grid, cudaStream_t stream) {
   if (grid <= 0 || p.n <= 0) return 0;
+  const OpCCellParams &cc = p;
   const OpVCellParams &v = p;
   const OpCellParams &b = p;
   const unsigned g = unsigned(grid);
-  if (p.col.m > 1) {
+  if (p.dg.on) {
     if (es == 4 && has_coef)
-      op_cell_kernel<float, true, true><<<g, 256, 0, stream>>>(p);
+      op_cell_kernel<float, true, true, true><<<g, 256, 0, stream>>>(p);
     else if (es == 4)
-      op_cell_kernel<float, false, true><<<g, 256, 0, stream>>>(p);
+      op_cell_kernel<float, false, true, true><<<g, 256, 0, stream>>>(p);
     else if (has_coef)
-      op_cell_kernel<double, true, true><<<g, 256, 0, stream>>>(p);
+      op_cell_kernel<double, true, true, true><<<g, 256, 0, stream>>>(p);
     else
-      op_cell_kernel<double, false, true><<<g, 256, 0, stream>>>(p);
+      op_cell_kernel<double, false, true, true><<<g, 256, 0, stream>>>(p);
+  } else if (p.col.m > 1) {
+    if (es == 4 && has_coef)
+      op_cell_kernel<float, true, true><<<g, 256, 0, stream>>>(cc);
+    else if (es == 4)
+      op_cell_kernel<float, false, true><<<g, 256, 0, stream>>>(cc);
+    else if (has_coef)
+      op_cell_kernel<double, true, true><<<g, 256, 0, stream>>>(cc);
+    else
+      op_cell_kernel<double, false, true><<<g, 256, 0, stream>>>(cc);
   } else if (es == 4 && has_coef)
     op_cell_kernel<float, true, false><<<g, 256, 0, stream>>>(v);
   else if (es == 4)

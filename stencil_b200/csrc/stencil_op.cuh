@@ -92,12 +92,30 @@ struct OpCCellParams : OpVCellParams {
   OpColour col;
 };
 
+// Diagonal relaxation (sb_stencil_dplan_create; DESIGN.md section 2.12): the op is A (src terms only), aux holds f, and
+// a cell of the colour gets u + T(omega) * ((f - A u) / d), d the sum of the factors T(w) (times C) of the terms at
+// offset 0 (bit t of centre: term t is one).  The diagonal kernels are the coloured ones with this flag (DIAG, a
+// compile-time switch); with m = 1 they write every cell of the boxes.
+struct OpDiag {
+  int on;
+  unsigned long long centre;
+  double omega;
+  float omegaf;
+};
+struct OpDTileParams : OpCTileParams {
+  OpDiag dg;
+};
+static_assert(sizeof(OpDTileParams) <= 4096, "the diagonal tile kernel's parameters fit the classic 4 KB limit");
+struct OpDCellParams : OpCCellParams {
+  OpDiag dg;
+};
+
 // Host: dynamic shared memory of the tile kernel; one-time attribute setup; the number of CTAs of the tile kernel that
 // fit on one SM (0 on error).  launch_* return the number of launches issued.  nf: coefficient fields (0: the plain
-// kernel); col: the coloured kernel.
+// kernel); col: the coloured kernel; diag: the diagonal one (p.dg.on in the launches).
 size_t op_tile_smem(int R, int es, int nf = 0);
-int op_tile_prepare(int R, int es, int device, int nf = 0, bool col = false);
-int launch_op_tile(const OpCTileParams &p, int R, int es, int grid, cudaStream_t stream);
-int launch_op_cells(const OpCCellParams &p, int es, bool has_coef, int grid, cudaStream_t stream);
+int op_tile_prepare(int R, int es, int device, int nf = 0, bool col = false, bool diag = false);
+int launch_op_tile(const OpDTileParams &p, int R, int es, int grid, cudaStream_t stream);
+int launch_op_cells(const OpDCellParams &p, int es, bool has_coef, int grid, cudaStream_t stream);
 
 } // namespace sb

@@ -23,9 +23,17 @@
 // rop_cell_kernel<T>: one thread per coarse cell over up to 16 thin boxes (the exterior slabs, one coarse cell thick),
 // every term read through the read-only path.
 //
+// Coefficient terms (HAS_COEF on both fused kernels, sb_transfer_voplan_create): a term's factor T(w) * C reads its field
+// through the read-only path at the term's coefficient offset from each fine cell.
+//
+// face_restrict_kernel<T, AX>: the face-coefficient restriction (sb_transfer_fplan_create), restrict_kernel's walk over
+// the four fine faces normal to AX under each coarse cell.
+//
 // Numerics: every multiply and add rounded separately (__fmul_rn / __fadd_rn, __dmul_rn / __dadd_rn; no FMA), in the
 // order of the rule in include/stencil_b200.h, so a cell's value does not depend on the launch shape or the partition.
 #include "transfer.cuh"
+
+#include <type_traits>
 
 namespace sb {
 namespace {
@@ -84,6 +92,36 @@ template <typename T> __global__ void __launch_bounds__(kRestrictX * kRestrictY)
     acc = N::add(acc, a11); // (0,1,1)
     acc = N::add(acc, b11); // (1,1,1)
     *reinterpret_cast<T *>(p.dst + (p.lo[2] + (long long)k) * p.dslice + cy * p.dpitch + cx * ES) = N::mul(T(0.125), acc);
+  }
+}
+
+// face_restrict_kernel<T, AX>: restrict_kernel's walk, one thread per coarse cell, reading the four fine faces normal to
+// axis AX under it (the fine plane 2I_AX only): on AX = 0 every other element of two rows in two planes, on AX = 1 a
+// pair in each of two planes, on AX = 2 a pair in each of two rows
+template <typename T, int AX> __global__ void __launch_bounds__(kRestrictX * kRestrictY) face_restrict_kernel(const __grid_constant__ RestrictParams p) {
+  using N = TNum<T>;
+  constexpr long long ES = sizeof(T);
+  const int i = blockIdx.x * kRestrictX + threadIdx.x, j = blockIdx.y * kRestrictY + threadIdx.y;
+  if (i >= p.ext[0] || j >= p.ext[1]) return;
+  const long long fx = p.flo[0] + 2 * i, fy = p.flo[1] + 2 * j;
+  const long long cx = p.lo[0] + i, cy = p.lo[1] + j;
+  for (int k = blockIdx.z; k < p.ext[2]; k += gridDim.z) {
+    const char *r00 = p.src + (p.flo[2] + 2ll * k) * p.sslice + fy * p.spitch + fx * ES; // fine row y0 of plane z0
+    T f0, f1, f2, f3; // F(2I), F(2I + e_b), F(2I + e_c), F(2I + e_b + e_c)
+    if constexpr (AX == 0) { // b = y, c = z
+      f0 = __ldg(reinterpret_cast<const T *>(r00));
+      f1 = __ldg(reinterpret_cast<const T *>(r00 + p.spitch));
+      f2 = __ldg(reinterpret_cast<const T *>(r00 + p.sslice));
+      f3 = __ldg(reinterpret_cast<const T *>(r00 + p.sslice + p.spitch));
+    } else if constexpr (AX == 1) { // b = x, c = z
+      load_pair<T>(r00, f0, f1);
+      load_pair<T>(r00 + p.sslice, f2, f3);
+    } else { // b = x, c = y
+      load_pair<T>(r00, f0, f1);
+      load_pair<T>(r00 + p.spitch, f2, f3);
+    }
+    const T acc = N::add(N::add(N::add(f0, f1), f2), f3);
+    *reinterpret_cast<T *>(p.dst + (p.lo[2] + (long long)k) * p.dslice + cy * p.dpitch + cx * ES) = N::mul(T(0.25), acc);
   }
 }
 
@@ -213,7 +251,11 @@ template <typename T> __global__ void __launch_bounds__(kProlongThreads) prolong
   }
 }
 
-template <typename T> __global__ void __launch_bounds__(kRestrictX * kRestrictY) rop_tile_kernel(const __grid_constant__ RopTileParams p) {
+// HAS_COEF: the coefficient variant (sb_transfer_voplan_create), a compile-time switch, so the plain instantiations are
+// the code they were; a coefficient term's factor reads its field through the read-only path
+template <typename T, bool HAS_COEF = false>
+__global__ void __launch_bounds__(kRestrictX * kRestrictY)
+    rop_tile_kernel(const __grid_constant__ typename std::conditional<HAS_COEF, RopVTileParams, RopTileParams>::type p) {
   using N = TNum<T>;
   constexpr long long ES = sizeof(T);
   constexpr int NT = kRestrictX * kRestrictY;
@@ -286,7 +328,25 @@ template <typename T> __global__ void __launch_bounds__(kRestrictX * kRestrictY)
       for (int t = 0; t < p.c.n; ++t) {
         const T w = N::w(p.c, t);
         T m[4];
-        if (p.c.source[t] == 0) {
+        if constexpr (HAS_COEF) { // (T(w) * C) * S, C at the term's coefficient offset from each fine cell
+          T wk[4] = {w, w, w, w};
+          const int cf = p.cfield[t];
+          if (cf >= 0) {
+            const char *c0 = p.coef[cf] + (long long)zc * p.c.sslice + (long long)fy * p.c.spitch + fx * ES + p.cgoff[t];
+#pragma unroll
+            for (int k = 0; k < 4; ++k) wk[k] = N::mul(w, __ldg(reinterpret_cast<const T *>(c0 + (k >> 1) * p.c.spitch + (k & 1) * ES)));
+          }
+          if (p.c.source[t] == 0) {
+            const T *q = q0 + toff[t];
+            m[0] = N::mul(wk[0], q[0]);
+            m[1] = N::mul(wk[1], q[1]);
+            m[2] = N::mul(wk[2], q[kRopSW]);
+            m[3] = N::mul(wk[3], q[kRopSW + 1]);
+          } else {
+#pragma unroll
+            for (int k = 0; k < 4; ++k) m[k] = N::mul(wk[k], a[k >> 1][k & 1]);
+          }
+        } else if (p.c.source[t] == 0) {
           const T *q = q0 + toff[t];
           m[0] = N::mul(w, q[0]);
           m[1] = N::mul(w, q[1]);
@@ -311,7 +371,10 @@ template <typename T> __global__ void __launch_bounds__(kRestrictX * kRestrictY)
   }
 }
 
-template <typename T> __global__ void __launch_bounds__(256) rop_cell_kernel(const __grid_constant__ RopCellParams p) {
+// HAS_COEF: the coefficient variant (sb_transfer_voplan_create), a compile-time switch, so the plain instantiations are
+// the code they were
+template <typename T, bool HAS_COEF = false>
+__global__ void __launch_bounds__(256) rop_cell_kernel(const __grid_constant__ typename std::conditional<HAS_COEF, RopVCellParams, RopCellParams>::type p) {
   using N = TNum<T>;
   constexpr long long ES = sizeof(T);
   const long long total = p.first[p.n];
@@ -343,7 +406,15 @@ template <typename T> __global__ void __launch_bounds__(256) rop_cell_kernel(con
       for (int t = 0; t < p.c.n; ++t) {
         const signed char *o = p.c.off[t];
         const T x = p.c.source[t] == 0 ? __ldg(reinterpret_cast<const T *>(p.c.src + f + o[2] * p.c.sslice + o[1] * p.c.spitch + o[0] * ES)) : a;
-        const T m = N::mul(N::w(p.c, t), x);
+        T w = N::w(p.c, t);
+        if constexpr (HAS_COEF) {
+          const int cf = p.cfield[t];
+          if (cf >= 0) {
+            const signed char *c = p.coff[t];
+            w = N::mul(w, __ldg(reinterpret_cast<const T *>(p.coef[cf] + f + c[2] * p.c.sslice + c[1] * p.c.spitch + c[0] * ES)));
+          }
+        }
+        const T m = N::mul(w, x);
         v = t == 0 ? m : N::add(v, m);
       }
       acc = d == 0 ? v : N::add(acc, v);
@@ -355,9 +426,10 @@ template <typename T> __global__ void __launch_bounds__(256) rop_cell_kernel(con
 
 } // namespace
 
-int rop_tile_ctas_per_sm(int es) {
+int rop_tile_ctas_per_sm(int es, bool coef) {
   int ctas = 0;
-  const void *fn = es == 4 ? reinterpret_cast<const void *>(&rop_tile_kernel<float>) : reinterpret_cast<const void *>(&rop_tile_kernel<double>);
+  const void *fn = coef ? (es == 4 ? reinterpret_cast<const void *>(&rop_tile_kernel<float, true>) : reinterpret_cast<const void *>(&rop_tile_kernel<double, true>))
+                        : (es == 4 ? reinterpret_cast<const void *>(&rop_tile_kernel<float>) : reinterpret_cast<const void *>(&rop_tile_kernel<double>));
   if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctas, fn, kRestrictX * kRestrictY, 0) != cudaSuccess) return 0;
   return ctas;
 }
@@ -381,6 +453,40 @@ int launch_rop_cells(const RopCellParams &p, int es, int grid, cudaStream_t stre
     rop_cell_kernel<double><<<unsigned(grid), 256, 0, stream>>>(p);
   else
     return 0;
+  return 1;
+}
+
+int launch_rop_vtile(const RopVTileParams &p, int es, int grid, cudaStream_t stream) {
+  if (grid <= 0) return 0;
+  if (es == 4)
+    rop_tile_kernel<float, true><<<unsigned(grid), kRestrictX * kRestrictY, 0, stream>>>(p);
+  else if (es == 8)
+    rop_tile_kernel<double, true><<<unsigned(grid), kRestrictX * kRestrictY, 0, stream>>>(p);
+  else
+    return 0;
+  return 1;
+}
+
+int launch_rop_vcells(const RopVCellParams &p, int es, int grid, cudaStream_t stream) {
+  if (grid <= 0 || p.n <= 0) return 0;
+  if (es == 4)
+    rop_cell_kernel<float, true><<<unsigned(grid), 256, 0, stream>>>(p);
+  else if (es == 8)
+    rop_cell_kernel<double, true><<<unsigned(grid), 256, 0, stream>>>(p);
+  else
+    return 0;
+  return 1;
+}
+
+int launch_face_restrict(const RestrictParams &p, int es, int axis, cudaStream_t stream) {
+  if (p.ext[0] <= 0 || p.ext[1] <= 0 || p.ext[2] <= 0 || axis < 0 || axis > 2 || (es != 4 && es != 8)) return 0;
+  const dim3 grid(unsigned((p.ext[0] + kRestrictX - 1) / kRestrictX), unsigned((p.ext[1] + kRestrictY - 1) / kRestrictY),
+                  unsigned(p.ext[2] < 65535 ? p.ext[2] : 65535));
+  const dim3 block(kRestrictX, kRestrictY);
+  using K = void (*)(const RestrictParams);
+  static const K fn[2][3] = {{face_restrict_kernel<float, 0>, face_restrict_kernel<float, 1>, face_restrict_kernel<float, 2>},
+                             {face_restrict_kernel<double, 0>, face_restrict_kernel<double, 1>, face_restrict_kernel<double, 2>}};
+  fn[es == 8][axis]<<<grid, block, 0, stream>>>(p);
   return 1;
 }
 

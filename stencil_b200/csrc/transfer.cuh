@@ -73,13 +73,34 @@ struct RopCellParams {
   long long first[kRopMaxBoxes + 1];
 };
 static_assert(sizeof(RopCellParams) <= 4096, "the fused restriction's cell parameters fit the classic 4 KB limit");
+// With coefficient terms (sb_transfer_voplan_create): term t's factor is T(w) * C_f(p + coff[t]), f = cfield[t] (-1:
+// none); the fields share src's pitch and rows.  The tile kernel reads them through the read-only path at the byte
+// offset cgoff[t] from the fine cell.
+constexpr int kRopMaxCoefs = 4;
+struct RopVTileParams : RopTileParams {
+  const char *coef[kRopMaxCoefs];
+  signed char cfield[kRopMaxTerms];
+  long long cgoff[kRopMaxTerms];
+};
+static_assert(sizeof(RopVTileParams) <= 4096, "the coefficient fused restriction's tile parameters fit the classic 4 KB limit");
+struct RopVCellParams : RopCellParams {
+  const char *coef[kRopMaxCoefs];
+  signed char cfield[kRopMaxTerms];
+  signed char coff[kRopMaxTerms][3];
+};
+static_assert(sizeof(RopVCellParams) <= 4096, "the coefficient fused restriction's cell parameters fit the classic 4 KB limit");
 
 // Host: launch_* return the number of launches issued (0 on an empty box or an unknown element size).
 int launch_restrict(const RestrictParams &p, int es, cudaStream_t stream);
+// face-coefficient restriction (sb_transfer_fplan_create) of the faces normal to axis 0, 1 or 2: RestrictParams' box
+// and allocations, the same grid
+int launch_face_restrict(const RestrictParams &p, int es, int axis, cudaStream_t stream);
 int prolong_ctas_per_sm(int es);
 int launch_prolong(const ProlongParams &p, int es, int grid, cudaStream_t stream);
-int rop_tile_ctas_per_sm(int es);
+int rop_tile_ctas_per_sm(int es, bool coef = false);
 int launch_rop_tile(const RopTileParams &p, int es, int grid, cudaStream_t stream);
 int launch_rop_cells(const RopCellParams &p, int es, int grid, cudaStream_t stream);
+int launch_rop_vcells(const RopVCellParams &p, int es, int grid, cudaStream_t stream);
+int launch_rop_vtile(const RopVTileParams &p, int es, int grid, cudaStream_t stream);
 
 } // namespace sb

@@ -368,16 +368,37 @@ class TransferPlan:
 
     @classmethod
     def fused(cls, device: int, op, dst: Pitched, dst_origin: Vec, dst_zsize: int, src: Pitched, src_origin: Vec, src_zsize: int,
-              aux: Optional[Pitched], boxes: Sequence[Tuple[Vec, Vec]]) -> "TransferPlan":
+              aux: Optional[Pitched], boxes: Sequence[Tuple[Vec, Vec]], coefs: Optional[Sequence[Pitched]] = None) -> "TransferPlan":
         """sb_transfer_oplan_create: the fused residual-restriction, dst (coarse) = the restriction of op(src, aux) (fine;
-        aux shares src's layout) over the coarse boxes [lo, hi) (global coordinates); op is a StencilOp without
-        coefficient terms and of reach <= 1."""
+        aux shares src's layout) over the coarse boxes [lo, hi) (global coordinates); op is a StencilOp of reach <= 1.
+        An op with coefficient terms takes coefs, its fine coefficient allocations (sb_transfer_voplan_create)."""
         nb = len(boxes)
         lo = (C.c_int64 * (3 * max(1, nb)))(*[int(v) for b in boxes for v in b[0]])
         hi = (C.c_int64 * (3 * max(1, nb)))(*[int(v) for b in boxes for v in b[1]])
         h = C.c_void_p()
-        check(lib().sb_transfer_oplan_create(C.byref(h), device, op.dtype_code, op.c_terms(), len(op.terms), dst, i3(dst_origin), int(dst_zsize),
-                                             src, i3(src_origin), int(src_zsize), aux if aux is not None else Pitched(None, 0, 0), nb, lo, hi))
+        a = aux if aux is not None else Pitched(None, 0, 0)
+        if op.has_coef:
+            cs = list(coefs or [])
+            carr = (Pitched * max(1, len(cs)))(*cs)
+            check(lib().sb_transfer_voplan_create(C.byref(h), device, op.dtype_code, op.c_vterms(), len(op.terms), dst, i3(dst_origin),
+                                                  int(dst_zsize), src, i3(src_origin), int(src_zsize), a, carr, len(cs), nb, lo, hi))
+        else:
+            check(lib().sb_transfer_oplan_create(C.byref(h), device, op.dtype_code, op.c_terms(), len(op.terms), dst, i3(dst_origin),
+                                                 int(dst_zsize), src, i3(src_origin), int(src_zsize), a, nb, lo, hi))
+        return cls._wrap(h, device)
+
+    @classmethod
+    def face(cls, device: int, dtype, axis: int, dst: Pitched, dst_origin: Vec, dst_zsize: int, src: Pitched, src_origin: Vec, src_zsize: int,
+             lo: Vec, hi: Vec) -> "TransferPlan":
+        """sb_transfer_fplan_create: dst (coarse) = the face-coefficient restriction of src (fine), faces normal to axis,
+        over the coarse box [lo, hi)."""
+        h = C.c_void_p()
+        check(lib().sb_transfer_fplan_create(C.byref(h), device, bc_dtype(dtype), int(axis), dst, i3(dst_origin), int(dst_zsize), src,
+                                             i3(src_origin), int(src_zsize), i3(lo), i3(hi)))
+        return cls._wrap(h, device)
+
+    @classmethod
+    def _wrap(cls, h, device: int) -> "TransferPlan":
         self = cls.__new__(cls)
         self._h = h
         self.device = device
@@ -1306,53 +1327,81 @@ class DistributedDomain:
         no cell exchange() sends (a slab as wide as the opposite side's radius); the exterior runs after exchange()."""
         self._run_plans(*self._apply_plans(op, dst, src, aux, exchange, coefs, colour))
 
-    def _apply_plans(self, op, dst, src, aux=None, exchange: bool = True, coefs=None, colour=None):
-        """apply()'s checks and cached plans, returned with its schedule as the arguments of _run_plans."""
+    def relax(self, A, dst, u, f, coefs=None, colour=None, omega: float = 1.0, exchange: bool = True) -> None:
+        """One relaxation pass of A u = f that divides by A's own diagonal (DESIGN.md section 2.12): dst[p] = u(p) +
+        omega ((f(p) - (A u)(p)) / d(p)), d(p) the sum of the factors (weight, times the coefficient for a coefficient
+        term) of A's terms at offset 0, for the cells of colour c of colour=(m, c) (None: every cell, weighted Jacobi,
+        dst must not be u).  A has src terms only (plain or coefficient terms) and at least one term at offset 0; for
+        div(kappa grad u) the diagonal differs from cell to cell, which A.relax(omega) cannot express.  Buffers, coefs,
+        the colour condition, the schedule, the in-place interior cut and the plan cache are apply()'s, with u as src and
+        f as aux; omega joins the plan key.  A red-black Gauss-Seidel sweep of -div(kappa grad u) = f:
+            A = StencilOp.div_grad((h, h, h), np.float64).scaled(-1.0)
+            for c in range(2):
+                dd.relax(A, (u, "curr"), u, f, coefs=[kx, ky, kz], colour=(2, c))
+        A zero or non-finite diagonal gives whatever IEEE arithmetic gives."""
+        if not np.isfinite(float(omega)):
+            raise _lib.StencilError(f"relax: omega = {omega} must be finite")
+        self._run_plans(*self._apply_plans(A, dst, u, f, exchange, coefs, colour, omega=float(omega)))
+
+    def _apply_plans(self, op, dst, src, aux=None, exchange: bool = True, coefs=None, colour=None, omega=None):
+        """apply()'s checks and cached plans, returned with its schedule as the arguments of _run_plans.  omega: relax()'s
+        plans (aux is f)."""
         from .stencil_op import StencilOp, StencilPlan
 
+        name = "apply" if omega is None else "relax"
         if not isinstance(op, StencilOp):
             raise _lib.StencilError(f"{op!r} is not a StencilOp")
         if self.partition_ is None or not self._plans:
-            raise _lib.StencilError("apply: call realize() first")
+            raise _lib.StencilError(f"{name}: call realize() first")
 
         def buf(arg, default, role):
             h, which = (arg, default) if isinstance(arg, DataHandle) else tuple(arg)
             if not isinstance(h, DataHandle) or which not in ("curr", "next"):
-                raise _lib.StencilError(f"apply: {role} must be a DataHandle or (DataHandle, 'curr' | 'next'), not {arg!r}")
+                raise _lib.StencilError(f"{name}: {role} must be a DataHandle or (DataHandle, 'curr' | 'next'), not {arg!r}")
             if self.dtypes_[h.id] != op.dtype:
-                raise _lib.StencilError(f"apply: {role} is {self.dtypes_[h.id]}, the op computes in {op.dtype}")
+                raise _lib.StencilError(f"{name}: {role} is {self.dtypes_[h.id]}, the op computes in {op.dtype}")
             return h.id, which
 
         d_q, d_w = buf(dst, "next", "dst")
         s_q, s_w = buf(src, "curr", "src")
         if s_w != "curr":
-            raise _lib.StencilError("apply: src must be a curr buffer (the one exchange() fills)")
+            raise _lib.StencilError(f"{name}: src must be a curr buffer (the one exchange() fills)")
         ncol, col = (1, 0) if colour is None else (int(colour[0]), int(colour[1]))
         if ncol not in (1, 2, 8) or not 0 <= col < ncol:
-            raise _lib.StencilError(f"apply: colour {colour!r} must be (m, c) with m in 1, 2, 8 and 0 <= c < m")
+            raise _lib.StencilError(f"{name}: colour {colour!r} must be (m, c) with m in 1, 2, 8 and 0 <= c < m")
         if (d_q, d_w) == (s_q, s_w) and ncol == 1:
-            raise _lib.StencilError("apply: dst must not be src")
-        a = buf(aux, "curr", "aux") if aux is not None else None
+            raise _lib.StencilError(f"{name}: dst must not be src")
+        a = buf(aux, "curr", "aux" if omega is None else "f") if aux is not None else None
         if op.has_aux and a is None:
-            raise _lib.StencilError("apply: the op has a term on aux, but no aux buffer was given")
+            raise _lib.StencilError(f"{name}: the op has a term on aux, but no aux buffer was given")
+        if omega is not None:
+            if op.has_aux:
+                raise _lib.StencilError("relax: A has a term on aux; A reads u only (f is the right-hand side)")
+            if not any(t[0] == 0 and t[1] == (0, 0, 0) for t in op.terms):
+                raise _lib.StencilError("relax: A has no term at offset (0, 0, 0), so no diagonal")
+            if a is None:
+                raise _lib.StencilError("relax: f is needed")
         cs = list(coefs) if coefs is not None else []
         if len(cs) != op.ncoef:
-            raise _lib.StencilError(f"apply: the op reads {op.ncoef} coefficient fields, but {len(cs)} were given")
+            raise _lib.StencilError(f"{name}: the op reads {op.ncoef} coefficient fields, but {len(cs)} were given")
         c_q = []
         for k, c in enumerate(cs):
             q, w = buf(c, "curr", f"coefficient {k}")
             if w != "curr":
-                raise _lib.StencilError(f"apply: coefficient {k} must be a curr buffer (the one exchange() fills)")
+                raise _lib.StencilError(f"{name}: coefficient {k} must be a curr buffer (the one exchange() fills)")
             if (q, w) == (d_q, d_w):
-                raise _lib.StencilError(f"apply: coefficient {k} must not be dst")
+                raise _lib.StencilError(f"{name}: coefficient {k} must not be dst")
             c_q.append(q)
         op.check(self.radius_, colours=ncol)
-        key = (op.key(), (d_q, d_w), s_q, a if op.has_aux else None, tuple(c_q), bool(exchange), self._parity, (ncol, col))
+        reads_aux = op.has_aux or omega is not None
+        key = (op.key(), (d_q, d_w), s_q, a if reads_aux else None, tuple(c_q), bool(exchange), self._parity, (ncol, col))
+        if omega is not None:
+            key += ("diag", omega)
 
         def make(di, d, boxes):
-            P = (d.pitched(d_q, d_w), d.pitched(s_q, "curr"), d.pitched(a[0], a[1]) if a is not None and op.has_aux else Pitched(None, 0, 0))
+            P = (d.pitched(d_q, d_w), d.pitched(s_q, "curr"), d.pitched(a[0], a[1]) if a is not None and reads_aux else Pitched(None, 0, 0))
             K = [d.pitched(q, "curr") for q in c_q] if op.has_coef else None
-            return StencilPlan(d.gpu(), op, *P, d.accessor_origin(), d.raw_size()[2], boxes, K, (ncol, col) if ncol > 1 else None)
+            return StencilPlan(d.gpu(), op, *P, d.accessor_origin(), d.raw_size()[2], boxes, K, (ncol, col) if ncol > 1 else None, omega)
 
         return self._plans_for(key, exchange, make, writes_src=(d_q, d_w) == (s_q, s_w)), exchange
 
@@ -1529,7 +1578,7 @@ class DistributedDomain:
                     si.wait_event(ev)
 
     # -- multigrid transfers
-    def restrict_to(self, coarse: "DistributedDomain", dst, src, op=None, aux=None, exchange: bool = True) -> None:
+    def restrict_to(self, coarse: "DistributedDomain", dst, src, op=None, aux=None, exchange: bool = True, coefs=None, face=None) -> None:
         """dst (a quantity of coarse) = the 8-cell average of src (a quantity of this domain) over every coarse compute
         cell (DESIGN.md section 2.10).  Buffers follow apply(): a bare handle means "next" for dst and "curr" for src;
         src may be curr or next, as restriction reads no ghost cells.  coarse must pair with this domain: the same
@@ -1543,13 +1592,26 @@ class DistributedDomain:
         term reads it.  exchange=True follows apply(): the coarse interior (the coarse compute region cut by 1, which
         reads no fine ghost cell) runs while exchange() fills the ghost cells, then the exterior slabs; exchange=False:
         one launch over the whole region, the caller guarantees the ghost cells.  The op is part of the plan key.
-            fine.restrict_to(coarse, (f2, "curr"), u, op=residual, aux=(f, "curr"))   # f2 = R (f - A u)"""
-        if op is None:
-            if aux is not None:
-                raise _lib.StencilError("restrict_to: aux is read only by an op")
+            fine.restrict_to(coarse, (f2, "curr"), u, op=residual, aux=(f, "curr"))   # f2 = R (f - A u)
+        An op with coefficient terms takes coefs, as apply() does (op.ncoef DataHandles of this domain, curr buffers,
+        exchanged like src); the result is the bits of apply() into a scratch quantity followed by restrict_to()
+        (sb_transfer_voplan_create; DESIGN.md section 2.12).
+        face=a (0, 1 or 2): src holds values on the faces normal to axis a (C_a(p) on the face between p - e_a and p, as
+        div_grad's coefficient field a), and dst = the average of the four fine faces that make up each coarse face
+        (sb_transfer_fplan_create); no op.
+            fine.restrict_to(coarse, (kx2, "curr"), (kx, "curr"), face=0)"""
+        if face is not None:
+            if op is not None or aux is not None or coefs is not None:
+                raise _lib.StencilError("restrict_to: a face restriction takes no op, aux or coefs")
+            if int(face) not in (0, 1, 2):
+                raise _lib.StencilError(f"restrict_to: face {face!r} must be the axis 0, 1 or 2")
+            self._transfer(coarse, _lib.TRANSFER_RESTRICT, dst, src, None, False, face=int(face))
+        elif op is None:
+            if aux is not None or coefs is not None:
+                raise _lib.StencilError("restrict_to: aux and coefs are read only by an op")
             self._transfer(coarse, _lib.TRANSFER_RESTRICT, dst, src, None, False)
         else:
-            self._transfer(coarse, _lib.TRANSFER_RESTRICT, dst, src, aux, exchange, op)
+            self._transfer(coarse, _lib.TRANSFER_RESTRICT, dst, src, aux, exchange, op, coefs=coefs)
 
     def prolong_from(self, coarse: "DistributedDomain", dst, src, aux=None, exchange: bool = True) -> None:
         """dst = aux + P src (or P src without aux) over every fine compute cell, P the trilinear interpolation from the
@@ -1562,8 +1624,9 @@ class DistributedDomain:
             fine.prolong_from(coarse, (u, "curr"), (e, "curr"), aux=(u, "curr"))"""
         self._transfer(coarse, _lib.TRANSFER_PROLONG, dst, src, aux, exchange)
 
-    def _transfer(self, coarse, kind: int, dst, src, aux, exchange: bool, op=None, queued: bool = False) -> None:
-        """restrict_to / prolong_from; queued: the schedule of _run_plans(queued=True), for a solver that owns the cycle."""
+    def _transfer(self, coarse, kind: int, dst, src, aux, exchange: bool, op=None, queued: bool = False, coefs=None, face=None) -> None:
+        """restrict_to / prolong_from; queued: the schedule of _run_plans(queued=True), for a solver that owns the cycle;
+        coefs: the fine coefficient quantities of a coefficient op; face: the axis of a face restriction."""
         from .stencil_op import StencilOp
 
         name = "restrict_to" if kind == _lib.TRANSFER_RESTRICT else "prolong_from"
@@ -1589,9 +1652,18 @@ class DistributedDomain:
             raise _lib.StencilError(f"{name}: dst, src and aux must all be float32 or all float64")
         if not restrict and s[1] != "curr":
             raise _lib.StencilError(f"{name}: src must be a curr buffer (the one coarse.exchange() fills)")
+        c_q = []
         if op is not None:
-            if not isinstance(op, StencilOp) or op.has_coef:
-                raise _lib.StencilError(f"{name}: op must be a StencilOp without coefficient terms, not {op!r}")
+            if not isinstance(op, StencilOp):
+                raise _lib.StencilError(f"{name}: op must be a StencilOp, not {op!r}")
+            cs = list(coefs) if coefs is not None else []
+            if len(cs) != op.ncoef:
+                raise _lib.StencilError(f"{name}: the op reads {op.ncoef} coefficient fields, but {len(cs)} were given")
+            for k, c in enumerate(cs):
+                q = buf(self, c, "curr", f"coefficient {k}")
+                if q[1] != "curr" or self.dtypes_[q[0]] != dtype:
+                    raise _lib.StencilError(f"{name}: coefficient {k} must be a curr buffer (the one exchange() fills) of the quantities' type")
+                c_q.append(q[0])
             if op.dtype != dtype:
                 raise _lib.StencilError(f"{name}: the op computes in {op.dtype}, the quantities are {dtype}")
             if s[1] != "curr":
@@ -1602,7 +1674,9 @@ class DistributedDomain:
             a = a if op.has_aux else None
         self._check_pairing(coarse, not restrict)
         fused_exchange = op is not None and bool(exchange)
-        key = (coarse, kind, d, s, a, self._parity, coarse._parity) + ((op.key(), fused_exchange) if op is not None else ())
+        key = (coarse, kind, d, s, a, self._parity, coarse._parity) + ((op.key(), fused_exchange, tuple(c_q)) if op is not None else ())
+        if face is not None:
+            key += (("face", face),)
         plans = self._transfer_plans.get(key)
         if plans is None:
             plans = []
@@ -1614,12 +1688,17 @@ class DistributedDomain:
                 if op is not None:
                     args = (fd.gpu(), op, cd.pitched(*d), cd.accessor_origin(), cd.raw_size()[2], fd.pitched(*s), fd.accessor_origin(),
                             fd.raw_size()[2], fd.pitched(*a) if a is not None else None)
+                    K = [fd.pitched(q, "curr") for q in c_q]
                     if fused_exchange:
-                        plans.append((TransferPlan.fused(*args, [boxes[di][0]]), TransferPlan.fused(*args, boxes[di][1])))
+                        plans.append((TransferPlan.fused(*args, [boxes[di][0]], K), TransferPlan.fused(*args, boxes[di][1], K)))
                     else:
-                        plans.append((TransferPlan.fused(*args, [cd.get_compute_region()]),))
+                        plans.append((TransferPlan.fused(*args, [cd.get_compute_region()], K),))
                     continue
                 lo, hi = dd.get_compute_region()
+                if face is not None:
+                    plans.append((TransferPlan.face(fd.gpu(), dtype, face, dd.pitched(*d), dd.accessor_origin(), dd.raw_size()[2], sd.pitched(*s),
+                                                    sd.accessor_origin(), sd.raw_size()[2], lo, hi),))
+                    continue
                 plans.append((TransferPlan(fd.gpu(), dtype, kind, dd.pitched(*d), dd.accessor_origin(), dd.raw_size()[2], sd.pitched(*s),
                                            sd.accessor_origin(), sd.raw_size()[2], fd.pitched(*a) if a is not None else None, lo, hi),))
             self._transfer_plans[key] = plans

@@ -7,11 +7,20 @@ of coarsenings by 2, built from the coloured sweeps (section 2.9), the fused res
     history = mg.solve(1e-8, 20)                                                # ||f - A u||_2 per cycle
     mg.close()
 
-Periodic Poisson (A singular) needs f of zero mean; the solver does not project."""
+Periodic Poisson (A singular) needs f of zero mean; the solver does not project.
+
+Variable coefficients (DESIGN.md section 2.12): with coefs= the ops may have coefficient terms, such as -div(kappa grad u)
+with kappa on faces in three fields; each level gets its own coarsened copy of every field and is smoothed by the
+diagonal relaxation (DistributedDomain.relax) instead of A.relax(1):
+
+    A_at = lambda l: sb.StencilOp.div_grad((h * 2**l,) * 3, np.float64).scaled(-1.0)
+    mg = sb.Multigrid(dd, u, f, r, A_at, coefs=[kx, ky, kz], coef_kinds=("x", "y", "z"))
+    ...                                    # kappa changes (a variable-density projection: kappa = 1 / rho)
+    mg.update_coefficients()               # every coarse level re-coarsened from kx, ky, kz"""
 from __future__ import annotations
 
 import ctypes as C
-from typing import Callable, List, Optional
+from typing import Callable, List, Optional, Sequence
 
 import numpy as np
 
@@ -22,8 +31,12 @@ from .stencil_op import StencilOp
 
 
 def residual_op(A: StencilOp) -> StencilOp:
-    """r = f - A u as one op on src u and aux f: (aux, 0, 1), then each term of A with its weight negated."""
-    return StencilOp([(1, (0, 0, 0), 1.0)] + [(0, t[1], -t[2]) for t in A.terms], A.dtype)
+    """r = f - A u as one op on src u and aux f: (aux, 0, 1), then each term of A with its weight negated (a coefficient
+    term keeps its field and coefficient offset)."""
+    return StencilOp([(1, (0, 0, 0), 1.0)] + [(0, t[1], -t[2]) + tuple(t[3:]) for t in A.terms], A.dtype)
+
+
+COEF_KINDS = {"x": 0, "y": 1, "z": 2, "cell": None}  # a face field's axis; None: a cell-centred field
 
 
 def coarse_bc(bc: BC) -> BC:
@@ -61,9 +74,10 @@ class _Clear:
 
 
 class _Level:
-    def __init__(self, dd: DistributedDomain, u: DataHandle, f: DataHandle, A: StencilOp):
-        self.dd, self.u, self.f, self.A = dd, u, f, A
-        self.gs = A.relax(1.0)
+    def __init__(self, dd: DistributedDomain, u: DataHandle, f: DataHandle, A: StencilOp, coefs: List[DataHandle]):
+        self.dd, self.u, self.f, self.A, self.coefs = dd, u, f, A, coefs
+        # coefficient ops: the diagonal relaxation (relax); plain ops: the SOR table, as before
+        self.gs = None if A.has_coef else A.relax(1.0)
         self.res = residual_op(A)
 
 
@@ -73,11 +87,21 @@ class Multigrid:
     of dd's type with plain src terms of reach <= 1 and one centre term.  Each coarse level is a DistributedDomain of u
     and f on the same GPUs, placement and boundary kinds as dd, with dd's radius raised to >= 1 in all 26 directions;
     the grid is halved while every subdomain extent is even and its half >= 2, at most `levels` grids.  The smoother is
-    red-black Gauss-Seidel if every level's A passes check(radius, colours=2), else 8-colour Gauss-Seidel.  Building the
-    hierarchy is collective under torchrun, and so are cycle() and solve().  The solver never calls dd.swap()."""
+    red-black Gauss-Seidel if every level's A passes check(radius, colours=2), else 8-colour Gauss-Seidel.  With coefs=
+    the ops may have coefficient terms (DESIGN.md section 2.12): each level holds its own coarsened fields, the smoother
+    is the diagonal relaxation and the residual goes through the fused coefficient kernel.  Building the hierarchy is
+    collective under torchrun, and so are cycle(), update_coefficients() and solve().  The solver never calls
+    dd.swap()."""
 
     def __init__(self, dd: DistributedDomain, u: DataHandle, f: DataHandle, r: DataHandle, op_at: Callable[[int], StencilOp], nu1: int = 2,
-                 nu2: int = 2, coarse_sweeps: int = 30, levels: Optional[int] = None):
+                 nu2: int = 2, coarse_sweeps: int = 30, levels: Optional[int] = None, coefs: Optional[Sequence[DataHandle]] = None,
+                 coef_kinds: Optional[Sequence[str]] = None):
+        """coefs: the coefficient quantities of dd the ops read (field k = coefs[k], every op_at(l) with ncoef equal to
+        len(coefs)); coef_kinds: one per field, "x", "y" or "z" for a field on the faces normal to that axis (coarsened by
+        the face restriction) or "cell" for a cell-centred field (the 8-cell restriction); by default ("x", "y", "z")
+        for three fields.  Each coarse level holds one quantity per field with the fine field's BC on every FIXED face,
+        which must be set.  Coefficient ops are smoothed by the diagonal relaxation with omega = 1 and their residual is
+        restricted by the fused coefficient kernel; plain ops run as without coefs."""
         if not isinstance(dd, DistributedDomain) or dd.partition_ is None or not dd._plans:
             raise _lib.StencilError("Multigrid: dd must be a realized DistributedDomain")
         for name, h in (("u", u), ("f", f), ("r", r)):
@@ -88,15 +112,35 @@ class Multigrid:
         dtype = dd.dtypes_[u.id]
         if dtype not in (np.dtype(np.float32), np.dtype(np.float64)) or dd.dtypes_[f.id] != dtype or dd.dtypes_[r.id] != dtype:
             raise _lib.StencilError("Multigrid: u, f and r must all be float32 or all float64")
+        coefs = list(coefs) if coefs is not None else []
+        if coef_kinds is None:
+            coef_kinds = ("x", "y", "z") if len(coefs) == 3 else ()
+        coef_kinds = tuple(coef_kinds)
+        if len(coefs) > 4:
+            raise _lib.StencilError(f"Multigrid: at most 4 coefficient fields, not {len(coefs)}")
+        if len(coef_kinds) != len(coefs) or any(k not in COEF_KINDS for k in coef_kinds):
+            raise _lib.StencilError(f"Multigrid: coef_kinds must name one of 'x', 'y', 'z', 'cell' per coefficient field, not {coef_kinds!r}")
+        for k, h in enumerate(coefs):
+            if not isinstance(h, DataHandle) or not 0 <= h.id < len(dd.dtypes_):
+                raise _lib.StencilError(f"Multigrid: coefficient {k} must be a DataHandle of dd, not {h!r}")
+            if h.id in (u.id, f.id, r.id) or dd.dtypes_[h.id] != dtype:
+                raise _lib.StencilError(f"Multigrid: coefficient {k} must be a quantity of u's type other than u, f and r")
+        if len({h.id for h in coefs}) != len(coefs):
+            raise _lib.StencilError("Multigrid: the coefficient fields must be different quantities")
         if int(nu1) < 0 or int(nu2) < 0 or int(coarse_sweeps) < 1:
             raise _lib.StencilError("Multigrid: nu1 and nu2 must be >= 0 and coarse_sweeps >= 1")
         if levels is not None and int(levels) < 2:
             raise _lib.StencilError("Multigrid: levels must be >= 2 (or None)")
         self.nu1, self.nu2, self.coarse_sweeps = int(nu1), int(nu2), int(coarse_sweeps)
-        walls = {}
+        walls, coef_walls = {}, [{} for _ in coefs]
         for fc in range(6):
             if dd.boundary_[fc // 2] == Boundary.FIXED:
                 walls[fc] = coarse_bc(dd.bcs_.get((u.id, fc), BC.NONE()))
+                for k, h in enumerate(coefs):
+                    bc = dd.bcs_.get((h.id, fc), BC.NONE())
+                    if bc.kind == BCKind.NONE:
+                        raise _lib.StencilError(f"Multigrid: coefficient {k} needs a boundary condition on every FIXED face (face {FACES[fc]})")
+                    coef_walls[k][fc] = bc
         part = dd.partition_
         nlev = level_count([part.subdomain_size(i) for i in part.indices()], levels)
         if nlev < 2:
@@ -119,8 +163,13 @@ class Multigrid:
             A = op_at(l)
             if not isinstance(A, StencilOp) or A.dtype != dtype:
                 raise _lib.StencilError(f"Multigrid: op_at({l}) must be a StencilOp in {dtype}, not {A!r}")
-            if A.has_coef or A.has_aux:
-                raise _lib.StencilError(f"Multigrid: op_at({l}) has coefficient or aux terms; the smoother takes constant-coefficient src terms")
+            if A.has_aux or (A.has_coef and not coefs):
+                raise _lib.StencilError(f"Multigrid: op_at({l}) has coefficient or aux terms; the smoother takes src terms, and coefficient "
+                                        "terms only with coefs=")
+            if coefs and A.ncoef != len(coefs):
+                raise _lib.StencilError(f"Multigrid: op_at({l}) reads {A.ncoef} coefficient fields, but {len(coefs)} were given")
+            if A.has_coef and not any(t[0] == 0 and t[1] == (0, 0, 0) for t in A.terms):
+                raise _lib.StencilError(f"Multigrid: op_at({l}) has no term at offset (0, 0, 0)")
             if A.reach() > 1:
                 raise _lib.StencilError(f"Multigrid: op_at({l}) reaches {A.reach()} cells; the fused residual-restriction takes reach <= 1")
             ops.append(A)
@@ -136,8 +185,9 @@ class Multigrid:
         if not self.colours:
             raise _lib.StencilError("Multigrid: A reads its own colour under both red-black and 8-colour orderings (or leaves the "
                                     "radius); no Gauss-Seidel smoother applies")
-        self.levels: List[_Level] = [_Level(dd, u, f, ops[0])]
+        self.levels: List[_Level] = [_Level(dd, u, f, ops[0], coefs)]
         self.r = r
+        self.coef_kinds = coef_kinds
         # every level queues on dd's apply streams, so stream order alone orders the work of consecutive levels
         if not dd._apply_streams:
             import torch
@@ -154,14 +204,20 @@ class Multigrid:
                 cd.set_methods(dd.flags_)
                 cd.set_radius(coarse_radius)
                 cu, cf = cd.add_data(dtype, "u"), cd.add_data(dtype, "f")
+                ck = [cd.add_data(dtype, f"coef{k}") for k in range(len(coefs))]
                 cd.set_boundary(*dd.boundary_)
                 for fc, bc in walls.items():
                     cd.set_boundary_condition(cu, FACES[fc], bc)
+                for h, w in zip(ck, coef_walls):
+                    for fc, bc in w.items():
+                        cd.set_boundary_condition(h, FACES[fc], bc)
                 cd.realize()
                 cd._apply_streams = dd._apply_streams
-                self.levels.append(_Level(cd, cu, cf, ops[l]))
+                self.levels.append(_Level(cd, cu, cf, ops[l], ck))
             for l in range(nlev - 1):
                 self.levels[l].dd._check_pairing(self.levels[l + 1].dd, True)
+            if coefs:
+                self.update_coefficients()
         except Exception:
             self.close()
             raise
@@ -169,7 +225,28 @@ class Multigrid:
     def _smooth(self, L: _Level, sweeps: int) -> None:
         for _ in range(sweeps):
             for c in range(self.colours):
-                L.dd._run_plans(*L.dd._apply_plans(L.gs, (L.u, "curr"), L.u, (L.f, "curr"), colour=(self.colours, c)), queued=True)
+                if L.gs is None:
+                    plans = L.dd._apply_plans(L.A, (L.u, "curr"), L.u, (L.f, "curr"), coefs=L.coefs, colour=(self.colours, c), omega=1.0)
+                else:
+                    plans = L.dd._apply_plans(L.gs, (L.u, "curr"), L.u, (L.f, "curr"), colour=(self.colours, c))
+                L.dd._run_plans(*plans, queued=True)
+
+    def update_coefficients(self, wait: bool = True) -> None:
+        """Re-coarsen every level's coefficient fields from the current fine ones, level by level: face fields by the
+        face restriction, cell fields by the 8-cell restriction.  Queued like a cycle, after the work on the caller's
+        stream, with one host wait (none with wait=False).  The constructor calls it once; call it again whenever the
+        fine fields change.  The coarse ghost cells are filled by the exchanges of the next cycle."""
+        import torch
+
+        dd = self.levels[0].dd
+        for d, (si, se) in zip(dd.domains_, dd._apply_streams):
+            si.wait_stream(torch.cuda.current_stream(d.gpu()))
+            se.wait_stream(torch.cuda.current_stream(d.gpu()))
+        for F, Cl in zip(self.levels[:-1], self.levels[1:]):
+            for kf, kc, kind in zip(F.coefs, Cl.coefs, self.coef_kinds):
+                F.dd._transfer(Cl.dd, _lib.TRANSFER_RESTRICT, (kc, "curr"), (kf, "curr"), None, False, queued=True, face=COEF_KINDS[kind])
+        if wait:
+            self.wait()
 
     def _vcycle(self, l: int) -> None:
         L = self.levels[l]
@@ -178,7 +255,8 @@ class Multigrid:
             return
         self._smooth(L, self.nu1)
         Cl = self.levels[l + 1]
-        L.dd._transfer(Cl.dd, _lib.TRANSFER_RESTRICT, (Cl.f, "curr"), (L.u, "curr"), (L.f, "curr"), True, op=L.res, queued=True)
+        L.dd._transfer(Cl.dd, _lib.TRANSFER_RESTRICT, (Cl.f, "curr"), (L.u, "curr"), (L.f, "curr"), True, op=L.res, queued=True,
+                       coefs=L.coefs if L.res.has_coef else None)
         Cl.dd._run_plans([(_Clear(d, Cl.u.id),) for d in Cl.dd.domains_], False, queued=True)
         self._vcycle(l + 1)
         L.dd._transfer(Cl.dd, _lib.TRANSFER_PROLONG, (L.u, "curr"), (Cl.u, "curr"), (L.u, "curr"), True, queued=True)
@@ -213,7 +291,7 @@ class Multigrid:
         """||f - A u||_2 over dd's compute region: the residual into r (apply) and an exact reduction, so every rank and
         every partition reach the same value."""
         L = self.levels[0]
-        L.dd.apply(L.res, (self.r, "curr"), L.u, (L.f, "curr"))
+        L.dd.apply(L.res, (self.r, "curr"), L.u, (L.f, "curr"), coefs=L.coefs if L.res.has_coef else None)
         return L.dd.reduce(self.r, "curr", exact=True).l2()
 
     def solve(self, rtol: float, max_cycles: int) -> List[float]:

@@ -176,15 +176,22 @@ class StencilPlan:
 
     def __init__(self, device: int, op: StencilOp, dst: Pitched, src: Pitched, aux: Pitched, acc_origin, zsize: int,
                  boxes: Sequence[Tuple[Sequence[int], Sequence[int]]], coefs: Optional[Sequence[Pitched]] = None,
-                 colour: Optional[Tuple[int, int]] = None):
+                 colour: Optional[Tuple[int, int]] = None, omega: Optional[float] = None):
         """coefs: the coefficient allocations (sb_stencil_vplan_create), field k = coefs[k]; None for a plain op.
         colour: (m, c), write only the cells of colour c under the colouring m (sb_stencil_cplan_create); dst may then be
-        src."""
+        src.  omega: the diagonal relaxation u + omega ((f - A u) / d) of the op A with f on aux (sb_stencil_dplan_create;
+        colour None means m = 1)."""
         nb = len(boxes)
         lo = (C.c_int64 * (3 * max(1, nb)))(*[int(v) for b in boxes for v in b[0]])
         hi = (C.c_int64 * (3 * max(1, nb)))(*[int(v) for b in boxes for v in b[1]])
         h = C.c_void_p()
-        if colour is not None:
+        if omega is not None:
+            cs = list(coefs or [])
+            carr = (Pitched * max(1, len(cs)))(*cs)
+            m, c = colour if colour is not None else (1, 0)
+            check(lib().sb_stencil_dplan_create(C.byref(h), device, op.dtype_code, op.c_vterms(), len(op.terms), dst, src, aux, carr, len(cs),
+                                                float(omega), int(m), int(c), i3(acc_origin), int(zsize), nb, lo, hi))
+        elif colour is not None:
             cs = list(coefs or [])
             carr = (Pitched * max(1, len(cs)))(*cs)
             check(lib().sb_stencil_cplan_create(C.byref(h), device, op.dtype_code, op.c_vterms(), len(op.terms), dst, src, aux, carr,
