@@ -12,7 +12,7 @@ NVCCFLAGS := -O3 -std=c++17 $(ARCH) -lineinfo -Xcompiler -fPIC -Xcompiler -Wall 
 INC       := -Iinclude -Istencil_b200/csrc
 
 # ---- core: kernels + C ABI (shared library, loaded by python and linked by the C++ API)
-CSRC      := stencil_b200/csrc/box_copy.cu stencil_b200/csrc/boundary.cu stencil_b200/csrc/reduce.cu stencil_b200/csrc/reduce_exact.cu stencil_b200/csrc/jacobi.cu stencil_b200/csrc/astaroth.cu stencil_b200/csrc/stencil_op.cu stencil_b200/csrc/stencil_sys.cu stencil_b200/csrc/transfer.cu stencil_b200/csrc/capi.cu
+CSRC      := stencil_b200/csrc/box_copy.cu stencil_b200/csrc/boundary.cu stencil_b200/csrc/reduce.cu stencil_b200/csrc/reduce_exact.cu stencil_b200/csrc/jacobi.cu stencil_b200/csrc/astaroth.cu stencil_b200/csrc/stencil_op.cu stencil_b200/csrc/stencil_sys.cu stencil_b200/csrc/transfer.cu stencil_b200/csrc/krylov.cu stencil_b200/csrc/capi.cu
 COBJ      := $(patsubst stencil_b200/csrc/%.cu,build/csrc/%.o,$(CSRC))
 SO        := stencil_b200/libstencil_b200.so
 
@@ -35,7 +35,8 @@ LIBMPI    := lib/libmpi_shim.a
 
 all: $(SO) $(LIBA) $(LIBMPI) bin/sb_mpirun bin/jacobi3d_b200 bin/test_exchange_multigpu bin/test_boundary_multigpu \
           bin/test_reduce_multigpu bin/test_stencil_multigpu bin/test_vstencil_multigpu bin/test_system_multigpu \
-          bin/test_reduce_exact_multigpu bin/test_colour_multigpu bin/test_mg_multigpu bin/test_multigrid_multigpu bin/test_vmultigrid_multigpu
+          bin/test_reduce_exact_multigpu bin/test_colour_multigpu bin/test_mg_multigpu bin/test_multigrid_multigpu bin/test_vmultigrid_multigpu \
+          bin/test_krylov_multigpu
 
 build/mpi_shim.o: src/mpi_shim.cpp include/mpi_shim/mpi.h
 	@mkdir -p build
@@ -179,6 +180,12 @@ build/drv/test_vmultigrid_multigpu.o: tests/cpp/test_vmultigrid_multigpu.cu $(wi
 	@mkdir -p $(dir $@)
 	$(NVCC) $(OWNDRVFLAGS) -c $< -o $@
 bin/test_vmultigrid_multigpu: build/drv/test_vmultigrid_multigpu.o $(LIBA) $(LIBMPI)
+	@mkdir -p bin
+	$(NVCC) $(DRVLINK) -o $@ $< $(LIBA) $(LIBMPI)
+build/drv/test_krylov_multigpu.o: tests/cpp/test_krylov_multigpu.cu $(wildcard include/stencil/*) include/stencil_b200.h
+	@mkdir -p $(dir $@)
+	$(NVCC) $(OWNDRVFLAGS) -c $< -o $@
+bin/test_krylov_multigpu: build/drv/test_krylov_multigpu.o $(LIBA) $(LIBMPI)
 	@mkdir -p bin
 	$(NVCC) $(DRVLINK) -o $@ $< $(LIBA) $(LIBMPI)
 build/drv/test_system_multigpu.o: tests/cpp/test_system_multigpu.cu $(wildcard include/stencil/*) include/stencil_b200.h

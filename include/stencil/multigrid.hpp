@@ -36,6 +36,8 @@
 namespace stencil {
 
 template <typename T> class Multigrid {
+  friend class PCG<T>; // queues this solver's cycle as its preconditioner
+
 public:
   Multigrid(DistributedDomain &dd, DataHandle<T> u, DataHandle<T> f, DataHandle<T> r, const std::function<LinearStencil(int)> &op_at, int nu1 = 2,
             int nu2 = 2, int coarse_sweeps = 30, int levels = 0)

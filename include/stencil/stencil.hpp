@@ -48,15 +48,18 @@ struct sb_copy_plan;
 struct sb_bc_plan;
 struct sb_reduce_plan;
 struct sb_reduce_exact_plan;
+struct sb_krylov_plan;
 struct sb_stencil_plan;
 struct sb_transfer_plan;
 
 namespace stencil {
 template <typename T> class Multigrid;
+template <typename T> class PCG;
 }
 
 class DistributedDomain {
   template <typename T> friend class stencil::Multigrid;
+  template <typename T> friend class stencil::PCG;
 
 private:
   Dim3 size_; // compute extent of the whole grid
@@ -136,6 +139,25 @@ private:
   };
   std::map<std::vector<int64_t>, ReduceCache> reducePlans_;
   void destroy_reduce_plans();
+  // every rank's byte records (MPI_Allgatherv, in rank order), the gather of reduce(..., Sum::exact) and of the Krylov sums
+  std::vector<unsigned char> allgather_records(const std::vector<unsigned char> &mine) const;
+
+  // Krylov vector passes (DESIGN.md section 2.13): per (mode, quantities, swap parity), one sb_krylov_plan over the
+  // compute region and one device buffer of its exact parts per local domain
+  struct KrylovCache {
+    std::vector<sb_krylov_plan *> plans;
+    std::vector<sb_reduce_exact_part *> out;
+    int nparts = 0;
+  };
+  std::map<std::vector<int64_t>, KrylovCache> krylovPlans_;
+  void destroy_krylov_plans();
+  KrylovCache &krylov_plans(int mode, const std::vector<size_t> &qs);
+  // one launch per local domain with the scalar s: queued (after the previous exterior, on the interior apply stream) or
+  // on the exchange streams after all work queued on the local devices
+  void krylov_launch(KrylovCache &c, double s, bool queued);
+  // the host wait: the parts of the last launch (on the streams krylov_launch used), gathered from every rank with
+  // MPI_Allgatherv, combined and rounded once; one sum per part
+  std::vector<double> krylov_sums(KrylovCache &c, bool queued);
 
   // linear stencil operators: per (op, buffers, exchange, swap parity), per local domain the interior and exterior plans
   // (exchange = true) or the whole-region plan; two streams per local domain (interior, exterior)
@@ -324,6 +346,16 @@ public:
   }
   std::vector<stencil::Reduction> reduce_many(const std::vector<stencil::ReduceItem> &items) { return reduce_many(items, stencil::Sum::ordered); }
   std::vector<stencil::Reduction> reduce_many(const std::vector<stencil::ReduceItem> &items, stencil::Sum sum);
+  // The exact inner product <a, b> of the curr buffers of two float or double quantities over the whole compute region
+  // (DESIGN.md section 2.13): the exact sum over the cells of fl64(double(a) * double(b)), rounded once, so the bits do
+  // not depend on the partition or the rank count (a may be b).  Like reduce(..., Sum::exact): waits for all work queued
+  // on the local devices, runs on the exchange streams, gathers the parts with MPI_Allgatherv; collective.  Plans are
+  // cached per pair and swap parity.
+  template <typename T> double dot(const DataHandle<T> &a, const DataHandle<T> &b) {
+    KrylovCache &c = krylov_plans(SB_KRYLOV_DOT, {a.id(), b.id()});
+    krylov_launch(c, 0.0, false);
+    return krylov_sums(c, false)[0];
+  }
 
   // dst = op(src, aux) over the whole compute region of every local subdomain (DESIGN.md section 2.7).  src is the curr
   // buffer (the one exchange() fills); dst is curr or next of any quantity of the same type, never src itself; aux is curr

@@ -314,6 +314,43 @@ int sb_reduce_exact_combine(const sb_reduce_exact_part *parts, int64_t n, sb_red
 int sb_reduce_exact_round(const sb_reduce_exact_part *part, sb_reduce_result *out);
 
 /* ---------------------------------------------------------------------------------------------
+ * Krylov vector kernels (DESIGN.md section 2.13): the vector algebra between operator applications of a conjugate-gradient
+ * iteration, one elementwise pass over a box [lo, hi) (global coordinates) of buffers that share dtype, pitch and row
+ * count.  T(s) is the double s rounded to the buffers' type; every per-cell multiply and add is rounded to nearest on
+ * its own (no FMA contraction).  An exact dot <a, b> is the exact real sum over the cells of v = fl64(double(a) *
+ * double(b)) (exact for float; one rounded multiply for double), written as an sb_reduce_exact_part with sum = the
+ * exact sum of v, sumsq = an exact zero, count = the cells and min / max of v by sb_reduce_exact_combine's
+ * order-independent rule; so parts of several boxes, subdomains or ranks merge by sb_reduce_exact_combine and round once
+ * by sb_reduce_exact_round, and the result does not depend on the partition.
+ *   SB_KRYLOV_DOT     buffers a, b[, c]: part 0 = <a, b>, part 1 = <a, c> (with c).  Sources may alias.
+ *   SB_KRYLOV_XPBY    buffers p, z:      p = z + T(s) * p; where T(s) is +0 or -0, p = z without reading p.  p and z
+ *                                      must not overlap.
+ *   SB_KRYLOV_UPDATE  buffers x, p, r, q: x = x + T(s) * p, r = r - T(s) * q, part 0 = <r, r> of the stored new r.
+ *                     Four buffers, no two overlapping.
+ * Cells outside the box are neither read nor written.
+ * ------------------------------------------------------------------------------------------- */
+typedef enum sb_krylov_mode { SB_KRYLOV_DOT = 0, SB_KRYLOV_XPBY = 1, SB_KRYLOV_UPDATE = 2 } sb_krylov_mode;
+
+/* A persistent plan of one mode over one box.  bufs: nbuf buffers in the order above (DOT 2 or 3, XPBY 2, UPDATE 4),
+ * acc_origin the global coordinate of their element (0,0,0).  dtype SB_DTYPE_F32 or SB_DTYPE_F64.  Errors
+ * (SB_ERR_INVALID with a message, before anything is allocated): an unknown mode or dtype, a wrong buffer count, a NULL
+ * buffer, buffers with different pitches or row counts, a pointer or pitch that is not a multiple of the element size,
+ * lo > hi, a box outside the allocation, rows of more than 2^27 cells or more than 2^31 rows, and forbidden aliasing:
+ * XPBY's p equal to z, UPDATE's buffers not distinct, and for XPBY and UPDATE any two buffers whose bytes from the box's
+ * first cell to its last overlap (DOT sources may alias).  16-byte accesses are used when every buffer has the same address modulo 16.
+ * sb_krylov_plan_launch runs the mode with the scalar s (ignored by DOT) and writes its parts (DOT: nbuf - 1, UPDATE: 1,
+ * XPBY: none, parts_dev may be NULL) to parts_dev (device memory) in the order of `stream`; it allocates nothing, never
+ * synchronises the host, may be captured in a CUDA graph, and at most one launch of a plan may be in flight at a time.
+ * sb_krylov_plan_bytes: the algorithmic bytes of a launch, per cell one element per distinct buffer read (XPBY counts p)
+ * and one per buffer written. */
+typedef struct sb_krylov_plan sb_krylov_plan;
+int sb_krylov_plan_create(sb_krylov_plan **out, int device, int mode, int dtype, const sb_pitched *bufs, int nbuf, const int64_t acc_origin[3],
+                          const int64_t lo[3], const int64_t hi[3]);
+int sb_krylov_plan_launch(sb_krylov_plan *plan, double s, sb_reduce_exact_part *parts_dev, void *stream);
+int64_t sb_krylov_plan_bytes(const sb_krylov_plan *plan);
+int sb_krylov_plan_destroy(sb_krylov_plan *plan);
+
+/* ---------------------------------------------------------------------------------------------
  * Constant-coefficient linear stencil operators (not in the reference; DESIGN.md section 2.7).
  * An operator is a list of 1 <= n <= SB_STENCIL_MAX_TERMS terms (source s, offset o, weight w): s = 0 reads src at
  * p + o, s = 1 reads aux at p (aux terms have offset 0: a previous time level, a right-hand side, a blend);

@@ -79,6 +79,7 @@ DistributedDomain::~DistributedDomain() {
 
 void DistributedDomain::destroy_plans() {
   destroy_reduce_plans();
+  destroy_krylov_plans();
   destroy_transfer_plans();
   destroy_stencil_plans();
   for (auto *sides : {&plans_, &unpackPlans_}) {
@@ -1102,6 +1103,21 @@ void DistributedDomain::transfer(DistributedDomain &coarse, bool prolong, int dt
   }
 }
 
+std::vector<unsigned char> DistributedDomain::allgather_records(const std::vector<unsigned char> &mine) const {
+  if (worldSize_ <= 1) return mine;
+  const int count = int(mine.size());
+  std::vector<int> counts(static_cast<size_t>(worldSize_)), displs(static_cast<size_t>(worldSize_));
+  MPI_Allgather(&count, 1, MPI_INT, counts.data(), 1, MPI_INT, MPI_COMM_WORLD);
+  int total = 0;
+  for (int r = 0; r < worldSize_; ++r) {
+    displs[size_t(r)] = total;
+    total += counts[size_t(r)];
+  }
+  std::vector<unsigned char> all(size_t(total), 0);
+  MPI_Allgatherv(mine.data(), count, MPI_BYTE, all.data(), counts.data(), displs.data(), MPI_BYTE, MPI_COMM_WORLD);
+  return all;
+}
+
 std::vector<stencil::Reduction> DistributedDomain::reduce_many(const std::vector<stencil::ReduceItem> &items, stencil::Sum sum) {
   using stencil::Which;
   const bool exact = sum == stencil::Sum::exact;
@@ -1192,19 +1208,7 @@ std::vector<stencil::Reduction> DistributedDomain::reduce_many(const std::vector
     CUDA_RUNTIME(cudaStreamSynchronize(streams_[di]));
   }
   // 3. every rank's records
-  std::vector<unsigned char> all = mine;
-  if (worldSize_ > 1) {
-    const int count = int(mine.size());
-    std::vector<int> counts(static_cast<size_t>(worldSize_)), displs(static_cast<size_t>(worldSize_));
-    MPI_Allgather(&count, 1, MPI_INT, counts.data(), 1, MPI_INT, MPI_COMM_WORLD);
-    int total = 0;
-    for (int r = 0; r < worldSize_; ++r) {
-      displs[size_t(r)] = total;
-      total += counts[size_t(r)];
-    }
-    all.assign(size_t(total), 0);
-    MPI_Allgatherv(mine.data(), count, MPI_BYTE, all.data(), counts.data(), displs.data(), MPI_BYTE, MPI_COMM_WORLD);
-  }
+  const std::vector<unsigned char> all = allgather_records(mine);
   // 4. merge in global subdomain-index order, the same on every rank
   const size_t nrec = all.size() / rec;
   std::vector<std::pair<int64_t, size_t>> order(nrec);
@@ -1236,6 +1240,103 @@ std::vector<stencil::Reduction> DistributedDomain::reduce_many(const std::vector
     result[i] = stencil::Reduction{r.min, r.max, r.sum, r.sumsq, r.count};
   }
   return result;
+}
+
+// ---- Krylov vector passes (DESIGN.md section 2.13) -----------------------------------------------------------------------
+void DistributedDomain::destroy_krylov_plans() {
+  for (auto &kv : krylovPlans_)
+    for (size_t di = 0; di < kv.second.plans.size(); ++di) {
+      sb_krylov_plan_destroy(kv.second.plans[di]);
+      cudaSetDevice(domains_[di].gpu());
+      if (kv.second.out[di]) cudaFree(kv.second.out[di]);
+    }
+  krylovPlans_.clear();
+}
+
+DistributedDomain::KrylovCache &DistributedDomain::krylov_plans(int mode, const std::vector<size_t> &qs) {
+  if (domains_.empty()) LOG_FATAL("krylov: call realize() first");
+  std::vector<int64_t> key{int64_t(mode)};
+  for (size_t q : qs) {
+    if (q >= dataDtype_.size()) LOG_FATAL("krylov: unknown data handle " << q);
+    if (dataDtype_[q] != SB_DTYPE_F32 && dataDtype_[q] != SB_DTYPE_F64) LOG_FATAL("krylov: quantity " << q << " is not float or double");
+    if (dataDtype_[q] != dataDtype_[qs[0]]) LOG_FATAL("krylov: the quantities must share one type");
+    key.push_back(int64_t(q));
+  }
+  key.push_back(parity_);
+  auto found = krylovPlans_.find(key);
+  if (found != krylovPlans_.end()) return found->second;
+  KrylovCache c;
+  c.nparts = mode == SB_KRYLOV_DOT ? int(qs.size()) - 1 : mode == SB_KRYLOV_UPDATE ? 1 : 0;
+  for (LocalDomain &d : domains_) {
+    const Rect3 cr = d.get_compute_region();
+    const Dim3 ao = d.origin() - Dim3(radius_.x(-1), radius_.y(-1), radius_.z(-1));
+    std::vector<sb_pitched> bufs;
+    for (size_t q : qs) {
+      const cudaPitchedPtr p = d.curr_data(q);
+      bufs.push_back(sb_pitched{p.ptr, int64_t(p.pitch), int64_t(p.ysize)});
+    }
+    const int64_t acc[3] = {ao.x, ao.y, ao.z}, lo[3] = {cr.lo.x, cr.lo.y, cr.lo.z}, hi[3] = {cr.hi.x, cr.hi.y, cr.hi.z};
+    sb_krylov_plan *plan = nullptr;
+    if (SB_OK != sb_krylov_plan_create(&plan, d.gpu(), mode, dataDtype_[qs[0]], bufs.data(), int(bufs.size()), acc, lo, hi))
+      LOG_FATAL("krylov: " << sb_last_error());
+    sb_reduce_exact_part *out = nullptr;
+    if (c.nparts) {
+      d.set_device();
+      CUDA_RUNTIME(cudaMalloc(&out, size_t(c.nparts) * sizeof(sb_reduce_exact_part)));
+    }
+    c.plans.push_back(plan);
+    c.out.push_back(out);
+  }
+  return krylovPlans_.emplace(key, std::move(c)).first->second;
+}
+
+void DistributedDomain::krylov_launch(KrylovCache &c, double s, bool queued) {
+  if (queued) {
+    create_apply_streams();
+    queue_after_exterior();
+  } else {
+    for (const int dev : std::set<int>(gpus_.begin(), gpus_.end())) {
+      CUDA_RUNTIME(cudaSetDevice(dev));
+      CUDA_RUNTIME(cudaDeviceSynchronize());
+    }
+  }
+  for (size_t di = 0; di < domains_.size(); ++di) {
+    domains_[di].set_device();
+    if (SB_OK != sb_krylov_plan_launch(c.plans[di], s, c.out[di], queued ? applyStreams_[2 * di] : cudaStream_t(streams_[di])))
+      LOG_FATAL("krylov: " << sb_last_error());
+  }
+}
+
+std::vector<double> DistributedDomain::krylov_sums(KrylovCache &c, bool queued) {
+  const size_t n = size_t(c.nparts), rec = sizeof(int64_t) + n * sizeof(sb_reduce_exact_part);
+  const Dim3 dim = placement_->dim();
+  std::vector<unsigned char> mine(domains_.size() * rec);
+  for (size_t di = 0; di < domains_.size(); ++di) {
+    domains_[di].set_device();
+    const Dim3 &idx = domainIdx_[di];
+    const int64_t lin = idx.x + dim.x * (idx.y + dim.y * idx.z);
+    std::memcpy(&mine[di * rec], &lin, sizeof(lin));
+    const cudaStream_t st = queued ? applyStreams_[2 * di] : cudaStream_t(streams_[di]);
+    CUDA_RUNTIME(cudaMemcpyAsync(&mine[di * rec + sizeof(int64_t)], c.out[di], n * sizeof(sb_reduce_exact_part), cudaMemcpyDeviceToHost, st));
+  }
+  for (size_t di = 0; di < domains_.size(); ++di) {
+    domains_[di].set_device();
+    CUDA_RUNTIME(cudaStreamSynchronize(queued ? applyStreams_[2 * di] : cudaStream_t(streams_[di])));
+  }
+  const std::vector<unsigned char> all = allgather_records(mine);
+  // exact sums: combined in any order, then rounded once, the same on every rank
+  const size_t nrec = all.size() / rec;
+  std::vector<double> out(n);
+  std::vector<sb_reduce_exact_part> parts(nrec);
+  for (size_t i = 0; i < n; ++i) {
+    for (size_t k = 0; k < nrec; ++k) std::memcpy(&parts[k], &all[k * rec + sizeof(int64_t) + i * sizeof(sb_reduce_exact_part)], sizeof(sb_reduce_exact_part));
+    sb_reduce_exact_part tot;
+    sb_reduce_result r;
+    if (SB_OK != sb_reduce_exact_combine(parts.data(), int64_t(nrec), &tot) || SB_OK != sb_reduce_exact_round(&tot, &r))
+      LOG_FATAL("krylov: " << sb_last_error());
+    out[i] = r.sum;
+  }
+  return out;
 }
 
 std::vector<Rect3> DistributedDomain::get_interior() const {

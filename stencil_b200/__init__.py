@@ -17,6 +17,7 @@ from .domain import (  # noqa: F401
     DataHandle,
     DistributedDomain,
     ExactReducePlan,
+    KrylovPlan,
     LocalDomain,
     Method,
     Partition,
@@ -40,5 +41,6 @@ from .domain import (  # noqa: F401
 )
 from .stencil_op import StencilOp, StencilPlan, StencilSystem, SystemPlan  # noqa: F401
 from .multigrid import Multigrid  # noqa: F401
+from .krylov import PCG  # noqa: F401
 
 __all__ = [n for n in dir() if not n.startswith("_")]

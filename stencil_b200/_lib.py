@@ -163,6 +163,8 @@ I6 = C.c_int32 * 6
 
 TRANSFER_RESTRICT, TRANSFER_PROLONG = 0, 1  # sb_transfer_kind
 
+KRYLOV_DOT, KRYLOV_XPBY, KRYLOV_UPDATE = 0, 1, 2  # sb_krylov_mode
+
 FUSED_MAX_GROUPS = 4096  # SB_FUSED_MAX_GROUPS
 
 
@@ -213,6 +215,10 @@ _SIGS = {
     "sb_reduce_exact_plan_destroy": (C.c_int, [C.c_void_p]),
     "sb_reduce_exact_combine": (C.c_int, [C.POINTER(ReduceExactPart), C.c_int64, C.POINTER(ReduceExactPart)]),
     "sb_reduce_exact_round": (C.c_int, [C.POINTER(ReduceExactPart), C.POINTER(ReduceResult)]),
+    "sb_krylov_plan_create": (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, C.POINTER(Pitched), C.c_int, I3, I3, I3]),
+    "sb_krylov_plan_launch": (C.c_int, [C.c_void_p, C.c_double, C.c_void_p, C.c_void_p]),
+    "sb_krylov_plan_bytes": (C.c_int64, [C.c_void_p]),
+    "sb_krylov_plan_destroy": (C.c_int, [C.c_void_p]),
     "sb_stencil_check": (C.c_int, [C.POINTER(StencilTerm), C.c_int, I27]),
     "sb_stencil_laplacian": (C.c_int, [C.c_int, C.c_double * 3, C.POINTER(StencilTerm), C.c_int]),
     "sb_stencil_plan_create": (

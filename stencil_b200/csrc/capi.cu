@@ -20,6 +20,7 @@
 #include "reduce.cuh"
 #include "astaroth.cuh"
 #include "jacobi.cuh"
+#include "krylov.cuh"
 #include "stencil_op.cuh"
 #include "stencil_sys.cuh"
 #include "transfer.cuh"
@@ -336,6 +337,16 @@ struct sb_reduce_exact_plan {
   unsigned nitems = 0, ntiles = 0;
   unsigned class_tiles[sb::kRedClasses][2] = {};
   int grids[sb::kRedClasses] = {};
+  int64_t bytes = 0;
+};
+
+struct sb_krylov_plan {
+  int device = 0;
+  int dtype = SB_DTYPE_F64, mode = 0; // mode: the kernel mode (krylov.cuh)
+  bool wide = false;
+  sb::KryParams params{};
+  sb::KryPartial *scratch = nullptr; // one partial per tile, rewritten by every launch (modes with dots)
+  int grid = 0, copy_grid = 0;
   int64_t bytes = 0;
 };
 
@@ -1272,6 +1283,130 @@ int sb_reduce_exact_combine(const sb_reduce_exact_part *parts, int64_t n, sb_red
 int sb_reduce_exact_round(const sb_reduce_exact_part *part, sb_reduce_result *out) {
   if (!part || !out) return fail(SB_ERR_INVALID, "sb_reduce_exact_round needs a part and an output");
   *out = sb_reduce_result{part->min, part->max, exact_round(part->sum), exact_round(part->sumsq), part->count};
+  return SB_OK;
+}
+
+// ----------------------------------------------------------------------------------------- krylov vector kernels
+int sb_krylov_plan_create(sb_krylov_plan **out, int device, int mode, int dtype, const sb_pitched *bufs, int nbuf, const int64_t acc_origin[3],
+                          const int64_t lo[3], const int64_t hi[3]) {
+  if (!out || !acc_origin || !lo || !hi) return fail(SB_ERR_INVALID, "sb_krylov_plan_create needs an output handle, acc_origin, lo and hi");
+  if (mode < SB_KRYLOV_DOT || mode > SB_KRYLOV_UPDATE) return fail(SB_ERR_INVALID, "unknown krylov mode %d", mode);
+  if (dtype != SB_DTYPE_F32 && dtype != SB_DTYPE_F64) return fail(SB_ERR_INVALID, "dtype %d must be SB_DTYPE_F32 or SB_DTYPE_F64", dtype);
+  static const char *const names[3][4] = {{"a", "b", "c", ""}, {"p", "z", "", ""}, {"x", "p", "r", "q"}};
+  const bool count_ok = mode == SB_KRYLOV_DOT ? (nbuf == 2 || nbuf == 3) : mode == SB_KRYLOV_XPBY ? nbuf == 2 : nbuf == 4;
+  if (!bufs || !count_ok)
+    return fail(SB_ERR_INVALID, "%s takes %s buffers, not %d", mode == SB_KRYLOV_DOT ? "SB_KRYLOV_DOT" : mode == SB_KRYLOV_XPBY ? "SB_KRYLOV_XPBY" : "SB_KRYLOV_UPDATE",
+                mode == SB_KRYLOV_DOT ? "2 or 3" : mode == SB_KRYLOV_XPBY ? "2" : "4", nbuf);
+  const int es = dtype == SB_DTYPE_F32 ? 4 : 8;
+  for (int a = 0; a < 3; ++a)
+    if (lo[a] > hi[a]) return fail(SB_ERR_INVALID, "lo > hi on axis %d", a);
+  int alo[3] = {0, 0, 0}, ahi[3] = {0, 0, 0};
+  for (int k = 0; k < nbuf; ++k) {
+    const sb_pitched &P = bufs[k];
+    if (!P.ptr) return fail(SB_ERR_INVALID, "buffer %s is NULL", names[mode][k]);
+    const int rc = to_alloc_box(P, es, acc_origin, lo, hi, alo, ahi);
+    if (rc != SB_OK) return fail(SB_ERR_INVALID, "buffer %s: %s", names[mode][k], g_err.c_str());
+    if (P.pitch != bufs[0].pitch || P.ysize != bufs[0].ysize) return fail(SB_ERR_INVALID, "the buffers have different pitches or row counts");
+    if ((uintptr_t(P.ptr) % uintptr_t(es)) || (P.pitch % es))
+      return fail(SB_ERR_INVALID, "buffer %s: pointer and pitch must be multiples of the %d-byte element", names[mode][k], es);
+  }
+  if ((long long)ahi[0] * es > bufs[0].pitch || ahi[1] > bufs[0].ysize) return fail(SB_ERR_INVALID, "box outside the allocation");
+  if (ahi[0] - alo[0] > (1 << 27)) return fail(SB_ERR_INVALID, "rows of more than 2^27 cells");
+  if ((long long)(ahi[1] - alo[1]) * (ahi[2] - alo[2]) >= (1ll << 31)) return fail(SB_ERR_INVALID, "more than 2^31 rows");
+  if (mode == SB_KRYLOV_XPBY && bufs[0].ptr == bufs[1].ptr) return fail(SB_ERR_INVALID, "SB_KRYLOV_XPBY: p must not be z");
+  if (mode == SB_KRYLOV_UPDATE)
+    for (int i = 0; i < 4; ++i)
+      for (int j = i + 1; j < 4; ++j)
+        if (bufs[i].ptr == bufs[j].ptr) return fail(SB_ERR_INVALID, "SB_KRYLOV_UPDATE: x, p, r and q must be four distinct buffers (%s is %s)", names[2][j], names[2][i]);
+  // a written buffer must not overlap another buffer of the pass: the bytes from the box's first cell to its last
+  if (mode != SB_KRYLOV_DOT && ahi[0] > alo[0] && ahi[1] > alo[1] && ahi[2] > alo[2]) {
+    const long long slice = bufs[0].pitch * bufs[0].ysize;
+    const long long first = (long long)alo[2] * slice + (long long)alo[1] * bufs[0].pitch + (long long)alo[0] * es;
+    const long long last = (long long)(ahi[2] - 1) * slice + (long long)(ahi[1] - 1) * bufs[0].pitch + (long long)ahi[0] * es;
+    for (int i = 0; i < nbuf; ++i)
+      for (int j = i + 1; j < nbuf; ++j) {
+        const uintptr_t a = uintptr_t(bufs[i].ptr), b = uintptr_t(bufs[j].ptr);
+        if (a + uintptr_t(first) < b + uintptr_t(last) && b + uintptr_t(first) < a + uintptr_t(last))
+          return fail(SB_ERR_INVALID, "%s: buffers %s and %s overlap over the box", mode == SB_KRYLOV_XPBY ? "SB_KRYLOV_XPBY" : "SB_KRYLOV_UPDATE",
+                      names[mode][i], names[mode][j]);
+      }
+  }
+  sb::KryParams kp{};
+  kp.pitch = bufs[0].pitch;
+  kp.slice = bufs[0].pitch * bufs[0].ysize;
+  for (int a = 0; a < 3; ++a) kp.ext[a] = ahi[a] - alo[a];
+  const long long off = (long long)alo[2] * kp.slice + (long long)alo[1] * kp.pitch + (long long)alo[0] * es;
+  bool wide = true;
+  for (int k = 0; k < 4; ++k) {
+    kp.buf[k] = static_cast<char *>(bufs[k < nbuf ? k : 0].ptr) + off;
+    wide = wide && ((uintptr_t(kp.buf[k]) - uintptr_t(kp.buf[0])) % 16 == 0);
+  }
+  // lanes per row and tile rows as for the reductions: a function of the box and the access width only
+  const long long nx = kp.ext[0], rows = (long long)kp.ext[1] * kp.ext[2];
+  kp.lg_group = int(std::min(5u, ceil_log2(unsigned(std::max(1ll, (nx * es + 15) / 16)))));
+  kp.count = nx * rows;
+  const long long N = wide ? 16 / es : 1, G = 1ll << kp.lg_group;
+  const long long per_row = N * (((nx / N) + G - 1) / G) + 2 * ((std::min(nx, N - 1) + G - 1) / G);
+  const long long rows_per_tile = std::max(1ll, sb::kRedChain / std::max(1ll, per_row)) * (sb::kRedThreads >> kp.lg_group);
+  kp.rows_per_tile = unsigned(rows_per_tile);
+  kp.ntiles = kp.count > 0 ? unsigned((rows + rows_per_tile - 1) / rows_per_tile) : 0u;
+  int kmode = sb::kKryUpdate;
+  if (mode == SB_KRYLOV_DOT) kmode = nbuf == 3 ? sb::kKryDot2 : sb::kKryDot1;
+  if (mode == SB_KRYLOV_XPBY) kmode = sb::kKryXpby;
+  // per cell: one element per distinct buffer read, one per buffer written
+  int nread = 0;
+  for (int k = 0; k < nbuf; ++k) {
+    bool dup = false;
+    for (int j = 0; j < k; ++j) dup = dup || bufs[j].ptr == bufs[k].ptr;
+    nread += !dup;
+  }
+  const int nwrite = mode == SB_KRYLOV_XPBY ? 1 : mode == SB_KRYLOV_UPDATE ? 2 : 0;
+  DeviceGuard guard(device);
+  if (!guard.ok) return fail(SB_ERR_NOGPU, "cannot select CUDA device %d", device);
+  sb_krylov_plan *p = new sb_krylov_plan();
+  p->device = device;
+  p->dtype = dtype;
+  p->mode = kmode;
+  p->wide = wide;
+  p->params = kp;
+  p->bytes = kp.count * es * (nread + nwrite);
+  const int ndots = sb::kry_dots(kmode);
+  if (ndots > 0) {
+    const cudaError_t e = cudaMalloc(&p->scratch, std::max<size_t>(1, kp.ntiles) * sizeof(sb::KryPartial));
+    if (e != cudaSuccess) {
+      sb_krylov_plan_destroy(p);
+      return fail(SB_ERR_CUDA, "krylov plan scratch: %s", cudaGetErrorString(e));
+    }
+  }
+  p->grid = sb::krylov_grid(device, dtype, kmode, wide, kp.ntiles);
+  p->copy_grid = mode == SB_KRYLOV_XPBY ? sb::krylov_grid(device, dtype, sb::kKryCopy, wide, kp.ntiles) : 0;
+  *out = p;
+  return SB_OK;
+}
+
+int sb_krylov_plan_launch(sb_krylov_plan *p, double s, sb_reduce_exact_part *parts_dev, void *stream) {
+  if (!p) return fail(SB_ERR_INVALID, "null plan");
+  if (!parts_dev && sb::kry_dots(p->mode) > 0) return fail(SB_ERR_INVALID, "null output buffer");
+  DeviceGuard guard(p->device);
+  if (!guard.ok) return fail(SB_ERR_NOGPU, "cannot select CUDA device %d", p->device);
+  int mode = p->mode, grid = p->grid;
+  // T(s) = +-0: p = z, never reading p (a NaN in p stays out)
+  if (mode == sb::kKryXpby && (p->dtype == SB_DTYPE_F32 ? float(s) == 0.0f : s == 0.0)) {
+    mode = sb::kKryCopy;
+    grid = p->copy_grid;
+  }
+  g_launches += uint64_t(sb::launch_krylov(p->params, p->dtype, mode, p->wide, grid, s, p->scratch, parts_dev, static_cast<cudaStream_t>(stream)));
+  SB_CUDA(cudaGetLastError());
+  return SB_OK;
+}
+
+int64_t sb_krylov_plan_bytes(const sb_krylov_plan *p) { return p ? p->bytes : 0; }
+
+int sb_krylov_plan_destroy(sb_krylov_plan *p) {
+  if (!p) return SB_OK;
+  DeviceGuard guard(p->device);
+  if (p->scratch) cudaFree(p->scratch);
+  delete p;
   return SB_OK;
 }
 

@@ -1,53 +1,9 @@
 // Exact reduction kernels (see reduce.cuh and the sb_reduce_exact_* entries of include/stencil_b200.h).
+#include "exact_acc.cuh"
 #include "reduce.cuh"
 
 namespace sb {
 namespace {
-
-// ---- exact sums (see reduce.cuh)
-struct ExShared {
-  unsigned long long digit[2][kExDigits]; // int64 counters of 32-bit digits, added to modulo 2^64
-  unsigned flags[2];
-};
-
-// Adds the double t exactly to accumulator w of the CTA: inf and NaN set flags; a finite t = m * 2^(p - 1074) (m < 2^53)
-// is m << (p mod 32), at most 85 bits, added as three unsigned 32-bit chunks (negated for t < 0) to digits p / 32 ...
-__device__ __forceinline__ void ex_add_shared(ExShared *sh, int w, double t) {
-  const unsigned long long b = (unsigned long long)__double_as_longlong(t);
-  const unsigned ex = unsigned(b >> 52) & 0x7ffu;
-  const unsigned long long frac = b & ((1ull << 52) - 1);
-  if (ex == 0x7ffu) {
-    atomicOr(&sh->flags[w], frac ? SB_EXACT_NAN : (b >> 63) ? SB_EXACT_NEG_INF : SB_EXACT_POS_INF);
-    return;
-  }
-  const unsigned long long m = ex ? frac | (1ull << 52) : frac;
-  if (!m) return;
-  const unsigned p = ex ? ex - 1 : 0, s = p & 31u, d = p >> 5;
-  const unsigned long long lo = m << s, hi = s ? m >> (64u - s) : 0ull;
-  const unsigned long long neg = (b >> 63) ? ~0ull : 0ull; // c -> (c ^ neg) - neg negates for t < 0
-  unsigned long long *dg = sh->digit[w] + d;
-  atomicAdd(dg, ((lo & 0xffffffffull) ^ neg) - neg);
-  atomicAdd(dg + 1, ((lo >> 32) ^ neg) - neg);
-  if (hi) atomicAdd(dg + 2, (hi ^ neg) - neg);
-}
-
-// t into the expansion f by TwoSum, level by level; the last error term, a term of magnitude >= 2^990 (the levels then
-// stay below 2^1018 for any chain a tile makes, so no TwoSum overflows), inf and NaN go to the CTA's accumulator.
-__device__ __forceinline__ void ex_add(double (&f)[kExFpe], double t, ExShared *sh, int w) {
-  if (!(fabs(t) < 0x1p990)) {
-    ex_add_shared(sh, w, t);
-    return;
-  }
-#pragma unroll
-  for (int i = 0; i < kExFpe; ++i) {
-    const double s = __dadd_rn(f[i], t);
-    const double bp = __dadd_rn(s, -f[i]);
-    const double e = __dadd_rn(__dadd_rn(f[i], -__dadd_rn(s, -bp)), __dadd_rn(t, -bp));
-    f[i] = s;
-    t = e;
-  }
-  if (t != 0.0) ex_add_shared(sh, w, t);
-}
 
 struct ExAcc {
   double mn, mx;
@@ -93,23 +49,7 @@ __global__ void __launch_bounds__(kRedThreads, 1) reduce_exact_tiles_kernel(cons
       a.mn = red_min(a.mn, __shfl_down_sync(0xffffffffu, a.mn, o));
       a.mx = red_max(a.mx, __shfl_down_sync(0xffffffffu, a.mx, o));
     }
-    // lane l + o into lane l for (l mod 2o) == 0: lane 0 ends with the warp's expansions (exact in any order)
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      double gv[kExFpe], gq[kExFpe];
-#pragma unroll
-      for (int i = 0; i < kExFpe; ++i) {
-        gv[i] = __shfl_down_sync(0xffffffffu, a.fv[i], o);
-        gq[i] = __shfl_down_sync(0xffffffffu, a.fq[i], o);
-      }
-      if (0 == (lane & unsigned(2 * o - 1))) {
-#pragma unroll
-        for (int i = 0; i < kExFpe; ++i) {
-          ex_add(a.fv, gv[i], &sh, 0);
-          ex_add(a.fq, gq[i], &sh, 1);
-        }
-      }
-    }
+    ex_warp_merge(a.fv, a.fq, &sh, lane); // lane 0 ends with the warp's expansions
     if (0 == lane) {
       warp_mn[threadIdx.x >> 5] = a.mn;
       warp_mx[threadIdx.x >> 5] = a.mx;
@@ -180,16 +120,7 @@ __global__ void __launch_bounds__(kExCombineThreads) reduce_exact_items_kernel(c
   if (threadIdx.x < 2) {
     const int w = int(threadIdx.x);
     sb_exact_sum &e = w ? o.sumsq : o.sum;
-    __int128 c = 0;
-    unsigned long long word = 0;
-    for (int k = 0; k < kExDigits; ++k) {
-      __int128 v = c;
-      for (int g = 0; g < kGroups; ++g) v += __int128(lo[g][w * kExDigits + k]) + (k ? __int128(hi[g][w * kExDigits + k - 1]) : 0);
-      const unsigned long long d = (unsigned long long)(v & 0xffffffff);
-      c = v >> 32;
-      word = (k & 1) ? word | (d << 32) : d;
-      if (k & 1) e.word[k >> 1] = word;
-    }
+    ex_carry(lo, hi, w, e);
     e.flags = flags[w];
   }
   if (0 == threadIdx.x) {

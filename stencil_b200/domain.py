@@ -565,6 +565,56 @@ class ExactReducePlan:
             pass
 
 
+class KrylovPlan:
+    """sb_krylov_plan: one Krylov vector pass (KRYLOV_DOT, KRYLOV_XPBY or KRYLOV_UPDATE) over one box, with its parts
+    (sb_reduce_exact_part, one per dot) written to a device buffer the plan owns.  One launch in flight at a time."""
+
+    def __init__(self, device: int, mode: int, dtype, bufs: Sequence[Pitched], acc_origin: Vec, lo: Vec, hi: Vec):
+        arr = (Pitched * max(1, len(bufs)))(*bufs)
+        h = C.c_void_p()
+        check(lib().sb_krylov_plan_create(C.byref(h), device, int(mode), bc_dtype(dtype), arr, len(bufs), i3(acc_origin), i3(lo), i3(hi)))
+        self._h = h
+        self.device = device
+        self.n = len(bufs) - 1 if mode == _lib.KRYLOV_DOT else 1 if mode == _lib.KRYLOV_UPDATE else 0
+        self.bytes = int(lib().sb_krylov_plan_bytes(h))
+        self.out_dev = None
+        if self.n:
+            out = C.c_void_p()
+            if lib().sb_malloc(C.byref(out), self.n * C.sizeof(_lib.ReduceExactPart), device) != 0:
+                self.destroy()
+                raise _lib.StencilError(f"krylov parts buffer: {lib().sb_last_error().decode()}")
+            self.out_dev = out.value
+        self.s = 0.0  # the scalar of the next launch
+
+    def launch(self, stream=None, s: Optional[float] = None) -> None:
+        """Queue the pass on `stream` with the scalar s (default: the attribute s, so a plan runs where a schedule
+        calls launch(stream) alone)."""
+        s = self.s if s is None else s
+        check(lib().sb_krylov_plan_launch(self._h, C.c_double(float(s)), C.c_void_p(self.out_dev or 0), stream_ptr(stream)))
+
+    def parts(self, stream=None) -> List[_lib.ReduceExactPart]:
+        """Copy the last launch's parts (ordered after it on `stream`) to the host."""
+        host = (_lib.ReduceExactPart * max(1, self.n))()
+        if self.n:
+            check(lib().sb_memcpy(C.addressof(host), C.c_void_p(self.out_dev), C.sizeof(host), self.device, stream_ptr(stream)))
+        check(lib().sb_stream_sync(self.device, stream_ptr(stream)))
+        return list(host)[: self.n]
+
+    def destroy(self) -> None:
+        if getattr(self, "out_dev", None):
+            lib().sb_free(C.c_void_p(self.out_dev), self.device)
+            self.out_dev = None
+        if getattr(self, "_h", None):
+            lib().sb_krylov_plan_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.destroy()
+        except Exception:
+            pass
+
+
 # ------------------------------------------------------------------------------------------ LocalDomain
 class LocalDomain:
     """One subdomain on one GPU: curr/next allocation per quantity (local_domain.cuh:34-276,
@@ -776,6 +826,7 @@ class DistributedDomain:
         self.topology_: Optional[Topology] = None
         self._bc_plans: List[List[Optional[BCPlan]]] = []  # [parity][local domain]
         self._reduce_plans: Dict[tuple, List[ReducePlan]] = {}  # (item keys, parity) -> one plan per local domain
+        self._krylov_plans: Dict[tuple, List[KrylovPlan]] = {}  # (mode, quantities, parity) -> one plan per local domain
         self._stencil_plans: Dict[tuple, list] = {}  # (op, buffers, exchange, parity) -> per local domain: plans
         self._apply_streams: list = []  # per local domain: (interior stream, exterior stream)
         self._transfer_plans: Dict[tuple, list] = {}  # (coarse domain, kind, buffers, both parities) -> per local domain
@@ -1259,16 +1310,13 @@ class DistributedDomain:
             check(lib().sb_device_sync(dev))
         for plan, s in zip(plans, self._streams):
             plan.launch(s)
-        dim = self.partition_.dim
         if exact:
-            mine = [(idx, [bytes(p) for p in plan.parts(s)]) for idx, plan, s in zip(self.domain_idx_, plans, self._streams)]
-        else:
-            mine = [(idx, [(r.min, r.max, r.sum, r.sumsq, r.count) for r in plan.results(s)])
-                    for idx, plan, s in zip(self.domain_idx_, plans, self._streams)]  # fmt: skip
+            return self._exact_gather([(idx, plan.parts(s)) for idx, plan, s in zip(self.domain_idx_, plans, self._streams)], n)
+        dim = self.partition_.dim
+        mine = [(idx, [(r.min, r.max, r.sum, r.sumsq, r.count) for r in plan.results(s)])
+                for idx, plan, s in zip(self.domain_idx_, plans, self._streams)]  # fmt: skip
         everyone = _dist.all_gather_object(mine) if self._world.size > 1 else [mine]
         parts = sorted((p for rank_parts in everyone for p in rank_parts), key=lambda p: p[0][0] + dim[0] * (p[0][1] + dim[1] * p[0][2]))
-        if exact:
-            return [reduce_exact_round(reduce_exact_combine([_lib.ReduceExactPart.from_buffer_copy(p[1][i]) for p in parts])) for i in range(n)]
         return [reduce_combine([Reduction(*p[1][i]) for p in parts]) for i in range(n)]
 
     def _reduce_key(self, it: tuple) -> tuple:
@@ -1300,6 +1348,60 @@ class DistributedDomain:
             srcs[1] = self._pitched_of(idx, qs[0], self._parity ^ 1)[0]
         lo, hi = d.get_compute_region()
         return _lib.ReduceItem(kind, bc_dtype(self.dtypes_[qs[0]]), (Pitched * 3)(*srcs), i3(d.accessor_origin()), i3(lo), i3(hi))
+
+    def _exact_gather(self, mine: Sequence[tuple], n: int) -> List[Reduction]:
+        """mine: (subdomain index, [n exact parts]) per local subdomain.  Every rank's parts gathered, combined by
+        sb_reduce_exact_combine and rounded once: the same bits on every rank and for every partition.  The one exact
+        combine of reduce_many(exact=True), dot() and the PCG solver."""
+        from . import dist as _dist
+
+        mine = [(idx, [bytes(p) for p in parts]) for idx, parts in mine]
+        everyone = _dist.all_gather_object(mine) if self._world.size > 1 else [mine]
+        dim = self.partition_.dim
+        parts = sorted((p for rank_parts in everyone for p in rank_parts), key=lambda p: p[0][0] + dim[0] * (p[0][1] + dim[1] * p[0][2]))
+        return [reduce_exact_round(reduce_exact_combine([_lib.ReduceExactPart.from_buffer_copy(p[1][i]) for p in parts])) for i in range(n)]
+
+    def krylov_plans(self, mode: int, handles: Sequence[DataHandle]) -> List[KrylovPlan]:
+        """The KrylovPlans of one pass over the compute region of every local subdomain, on the curr buffers of handles
+        (in sb_krylov_plan_create's order: DOT a, b[, c]; XPBY p, z; UPDATE x, p, r, q), for the current swap parity.
+        Built on first use and kept until close(), like reduce_plans()."""
+        if self.partition_ is None or not self._plans:
+            raise _lib.StencilError("krylov_plans: call realize() first")
+        qs = []
+        for h in handles:
+            if not isinstance(h, DataHandle) or not 0 <= h.id < len(self.dtypes_):
+                raise _lib.StencilError(f"krylov_plans: {h!r} is not a DataHandle of this domain")
+            qs.append(h.id)
+        dts = {self.dtypes_[q] for q in qs}
+        if len(dts) != 1 or bc_dtype(next(iter(dts))) == 0:
+            raise _lib.StencilError("krylov_plans: the quantities must all be float32 or all float64")
+        key = (int(mode), tuple(qs), self._parity)
+        plans = self._krylov_plans.get(key)
+        if plans is None:
+            plans = []
+            try:
+                for d in self.domains_:
+                    lo, hi = d.get_compute_region()
+                    plans.append(KrylovPlan(d.gpu(), mode, self.dtypes_[qs[0]], [d.pitched(q, "curr") for q in qs], d.accessor_origin(), lo, hi))
+            except Exception:
+                for p in plans:
+                    p.destroy()
+                raise
+            self._krylov_plans[key] = plans
+        return plans
+
+    def dot(self, a: DataHandle, b: DataHandle) -> float:
+        """The exact inner product <a, b> of the curr buffers of two float32 or float64 quantities over the whole compute
+        region (DESIGN.md section 2.13): the exact sum over the cells of fl64(double(a) * double(b)), rounded once to
+        double, so every partition, rank count and layout gives the same bits (a may be b: <a, a> = ||a||^2).  Waits for
+        all work queued on the local devices, computes on the exchange streams and gathers every rank's parts: collective
+        under torchrun.  The plans are cached as krylov_plans() describes."""
+        plans = self.krylov_plans(_lib.KRYLOV_DOT, (a, b))
+        for dev in sorted({d.gpu() for d in self.domains_}):
+            check(lib().sb_device_sync(dev))
+        for plan, s in zip(plans, self._streams):
+            plan.launch(s)
+        return self._exact_gather([(idx, plan.parts(s)) for idx, plan, s in zip(self.domain_idx_, plans, self._streams)], 1)[0].sum
 
     # -- linear stencil operators
     def apply(self, op, dst, src, aux=None, exchange: bool = True, coefs=None, colour=None) -> None:
@@ -1747,6 +1849,10 @@ class DistributedDomain:
             for p in plans:
                 p.destroy()
         self._reduce_plans = {}
+        for plans in self._krylov_plans.values():
+            for p in plans:
+                p.destroy()
+        self._krylov_plans = {}
         for plans in self._plans + getattr(self, "_unpack_plans", []) + self._bc_plans:
             for p in plans:
                 if p is not None:
