@@ -21,6 +21,11 @@
 // Coefficient ops are smoothed by the diagonal relaxation (DistributedDomain::relax, omega = 1) and their residual goes
 // through the fused coefficient restriction; update_coefficients() re-coarsens every level from the fine fields.
 //     stencil::Multigrid<double> mg(dd, u, f, r, [&](int l) { return A(l); }, {kx, ky, kz}, {"x", "y", "z"});
+//
+// cycle(u2, f2) runs the cycle on another fine-level pair through the same coarse levels and coarse coefficient fields
+// (DESIGN.md section 2.14): u2 and f2 are two different quantities of dd of type T, not coefficient fields, and u2
+// carries the constructor u's BC on every FIXED face (the coarse walls derive from it); the cycle is then the bits of one
+// on a Multigrid built on (u2, f2).
 #pragma once
 
 #include <cmath>
@@ -36,7 +41,8 @@
 namespace stencil {
 
 template <typename T> class Multigrid {
-  friend class PCG<T>; // queues this solver's cycle as its preconditioner
+  friend class PCG<T>;      // queues this solver's cycle as its preconditioner
+  friend class BiCGStab<T>; // the same, on two pairs
 
 public:
   Multigrid(DistributedDomain &dd, DataHandle<T> u, DataHandle<T> f, DataHandle<T> r, const std::function<LinearStencil(int)> &op_at, int nu1 = 2,
@@ -58,6 +64,14 @@ public:
   void cycle() {
     for (Level &L : levels_) L.dd->queued_ = true;
     vcycle(0);
+    finish();
+  }
+
+  // The same cycle on the fine-level pair (u, f) instead of the constructor's (see the header comment).
+  void cycle(DataHandle<T> u, DataHandle<T> f) {
+    Level &top = pair_level(u, f);
+    for (Level &L : levels_) L.dd->queued_ = true;
+    vcycle(0, &top);
     finish();
   }
 
@@ -110,6 +124,32 @@ private:
   DataHandle<T> r_;
   std::vector<Level> levels_;
   std::vector<int> axes_; // per coefficient field: the face axis, or -1 for a cell field
+  std::vector<std::pair<int, BC>> ubcs_; // the constructor u's BC on every FIXED face
+  std::vector<Level> pairs_;             // the fine levels of other pairs (cycle(u, f))
+
+  // the fine level of the pair (u, f): the constructor's, or one sharing A, the coefficient fields and the coarse levels
+  Level &pair_level(DataHandle<T> u, DataHandle<T> f) {
+    Level &L0 = levels_[0];
+    if (u.id() == L0.u.id() && f.id() == L0.f.id()) return L0;
+    for (Level &P : pairs_)
+      if (P.u.id() == u.id() && P.f.id() == f.id()) return P;
+    DistributedDomain &dd = *L0.dd;
+    if (u.id() == f.id()) LOG_FATAL("Multigrid::cycle: u and f must be two different quantities");
+    for (size_t q : {u.id(), f.id()})
+      if (q >= dd.dataDtype_.size() || dd.dataDtype_[q] != bc_dtype<T>()) LOG_FATAL("Multigrid::cycle: u and f must be quantities of dd of the constructor u's type");
+    for (const DataHandle<T> &k : L0.coefs)
+      if (k.id() == u.id() || k.id() == f.id()) LOG_FATAL("Multigrid::cycle: u and f must not be coefficient fields");
+    for (const auto &w : ubcs_) {
+      auto it = dd.bcs_.find(std::make_pair(u.id(), w.first));
+      const BC got = it == dd.bcs_.end() ? BC::NONE() : it->second;
+      if (got.kind != w.second.kind || got.value != w.second.value)
+        LOG_FATAL("Multigrid::cycle: u needs the constructor u's BC on every FIXED face (face " << w.first << ": kind " << int(w.second.kind) << ", value "
+                                                                                                << w.second.value << ", not kind " << int(got.kind) << ", value "
+                                                                                                << got.value << ")");
+    }
+    pairs_.push_back(Level{&dd, nullptr, u, f, L0.A, L0.gs, L0.res, L0.coefs});
+    return pairs_.back();
+  }
 
   void init(DistributedDomain &dd, DataHandle<T> u, DataHandle<T> f, const std::function<LinearStencil(int)> &op_at, int levels,
             const std::vector<DataHandle<T>> &coefs, const std::vector<std::string> &coef_kinds) {
@@ -142,6 +182,7 @@ private:
       if (kind == SB_BC_VALUE) LOG_FATAL("Multigrid: VALUE walls are not consistent across levels (DESIGN.md section 2.10); use ODD(c)");
       if (kind == SB_BC_NONE) LOG_FATAL("Multigrid: u needs a boundary condition (ODD or EVEN) on every FIXED face");
       walls.push_back(std::make_pair(fc, kind == SB_BC_ODD ? BC::ODD(0.0) : BC::EVEN()));
+      ubcs_.push_back(std::make_pair(fc, it->second));
     }
     // every coefficient field's BCs, kept on every level
     std::vector<std::vector<std::pair<int, BC>>> coef_walls(coefs.size());
@@ -267,8 +308,9 @@ private:
       }
   }
 
-  void vcycle(size_t l) {
-    Level &L = levels_[l];
+  // top: the fine level of another pair (pair_level), or nullptr for the constructor's
+  void vcycle(size_t l, Level *top = nullptr) {
+    Level &L = l == 0 && top ? *top : levels_[l];
     if (l + 1 == levels_.size()) {
       smooth(L, coarse_sweeps_);
       return;

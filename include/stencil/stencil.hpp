@@ -55,11 +55,13 @@ struct sb_transfer_plan;
 namespace stencil {
 template <typename T> class Multigrid;
 template <typename T> class PCG;
+template <typename T> class BiCGStab;
 }
 
 class DistributedDomain {
   template <typename T> friend class stencil::Multigrid;
   template <typename T> friend class stencil::PCG;
+  template <typename T> friend class stencil::BiCGStab;
 
 private:
   Dim3 size_; // compute extent of the whole grid
@@ -154,7 +156,9 @@ private:
   KrylovCache &krylov_plans(int mode, const std::vector<size_t> &qs);
   // one launch per local domain with the scalar s: queued (after the previous exterior, on the interior apply stream) or
   // on the exchange streams after all work queued on the local devices
-  void krylov_launch(KrylovCache &c, double s, bool queued);
+  void krylov_launch(KrylovCache &c, double s, bool queued) { krylov_launch(c, s, 0.0, queued); }
+  // the same with a second scalar t (SB_KRYLOV_BICG_P's omega; the other modes ignore it)
+  void krylov_launch(KrylovCache &c, double s, double t, bool queued);
   // the host wait: the parts of the last launch (on the streams krylov_launch used), gathered from every rank with
   // MPI_Allgatherv, combined and rounded once; one sum per part
   std::vector<double> krylov_sums(KrylovCache &c, bool queued);

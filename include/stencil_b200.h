@@ -325,28 +325,36 @@ int sb_reduce_exact_round(const sb_reduce_exact_part *part, sb_reduce_result *ou
  *   SB_KRYLOV_DOT     buffers a, b[, c]: part 0 = <a, b>, part 1 = <a, c> (with c).  Sources may alias.
  *   SB_KRYLOV_XPBY    buffers p, z:      p = z + T(s) * p; where T(s) is +0 or -0, p = z without reading p.  p and z
  *                                      must not overlap.
- *   SB_KRYLOV_UPDATE  buffers x, p, r, q: x = x + T(s) * p, r = r - T(s) * q, part 0 = <r, r> of the stored new r.
- *                     Four buffers, no two overlapping.
+ *   SB_KRYLOV_UPDATE  buffers x, p, r, q[, c]: x = x + T(s) * p, r = r - T(s) * q, part 0 = <r, r> of the stored new
+ *                     r and, with c, part 1 = <c, r> of the stored new r.  x, p, r and q are four buffers, no two
+ *                     overlapping; c must not overlap x or r, and may be p or q (DESIGN.md section 2.14).
+ *   SB_KRYLOV_BICG_P  buffers p, r, v:   p = r + T(s) * (p - T(t) * v), the BiCGStab direction with s = beta and
+ *                     t = omega (section 2.14).  p must not overlap r or v; r and v may alias.
  * Cells outside the box are neither read nor written.
  * ------------------------------------------------------------------------------------------- */
-typedef enum sb_krylov_mode { SB_KRYLOV_DOT = 0, SB_KRYLOV_XPBY = 1, SB_KRYLOV_UPDATE = 2 } sb_krylov_mode;
+typedef enum sb_krylov_mode { SB_KRYLOV_DOT = 0, SB_KRYLOV_XPBY = 1, SB_KRYLOV_UPDATE = 2, SB_KRYLOV_BICG_P = 4 } sb_krylov_mode;
 
-/* A persistent plan of one mode over one box.  bufs: nbuf buffers in the order above (DOT 2 or 3, XPBY 2, UPDATE 4),
- * acc_origin the global coordinate of their element (0,0,0).  dtype SB_DTYPE_F32 or SB_DTYPE_F64.  Errors
+/* A persistent plan of one mode over one box.  bufs: nbuf buffers in the order above (DOT 2 or 3, XPBY 2, UPDATE 4 or
+ * 5, BICG_P 3), acc_origin the global coordinate of their element (0,0,0).  dtype SB_DTYPE_F32 or SB_DTYPE_F64.  Errors
  * (SB_ERR_INVALID with a message, before anything is allocated): an unknown mode or dtype, a wrong buffer count, a NULL
  * buffer, buffers with different pitches or row counts, a pointer or pitch that is not a multiple of the element size,
  * lo > hi, a box outside the allocation, rows of more than 2^27 cells or more than 2^31 rows, and forbidden aliasing:
- * XPBY's p equal to z, UPDATE's buffers not distinct, and for XPBY and UPDATE any two buffers whose bytes from the box's
- * first cell to its last overlap (DOT sources may alias).  16-byte accesses are used when every buffer has the same address modulo 16.
+ * XPBY's p equal to z, UPDATE's x, p, r, q not distinct, UPDATE's c equal to x or r, BICG_P's p equal to r or v, and
+ * for XPBY, UPDATE and BICG_P any two buffers whose bytes from the box's first cell to its last overlap where one of
+ * them is written or both are among UPDATE's x, p, r, q (DOT sources may alias; so may BICG_P's r and v and UPDATE's c
+ * with p or q).  16-byte accesses are used when every buffer has the same address modulo 16.
  * sb_krylov_plan_launch runs the mode with the scalar s (ignored by DOT) and writes its parts (DOT: nbuf - 1, UPDATE: 1,
- * XPBY: none, parts_dev may be NULL) to parts_dev (device memory) in the order of `stream`; it allocates nothing, never
- * synchronises the host, may be captured in a CUDA graph, and at most one launch of a plan may be in flight at a time.
+ * or 2 with c, XPBY and BICG_P: none, parts_dev may be NULL) to parts_dev (device memory) in the order of `stream`; it
+ * allocates nothing, never synchronises the host, may be captured in a CUDA graph, and at most one launch of a plan may
+ * be in flight at a time.  It refuses a BICG_P plan, which takes two scalars: sb_krylov_plan_launch2 passes s and t to
+ * any mode (the modes other than BICG_P ignore t).
  * sb_krylov_plan_bytes: the algorithmic bytes of a launch, per cell one element per distinct buffer read (XPBY counts p)
  * and one per buffer written. */
 typedef struct sb_krylov_plan sb_krylov_plan;
 int sb_krylov_plan_create(sb_krylov_plan **out, int device, int mode, int dtype, const sb_pitched *bufs, int nbuf, const int64_t acc_origin[3],
                           const int64_t lo[3], const int64_t hi[3]);
 int sb_krylov_plan_launch(sb_krylov_plan *plan, double s, sb_reduce_exact_part *parts_dev, void *stream);
+int sb_krylov_plan_launch2(sb_krylov_plan *plan, double s, double t, sb_reduce_exact_part *parts_dev, void *stream);
 int64_t sb_krylov_plan_bytes(const sb_krylov_plan *plan);
 int sb_krylov_plan_destroy(sb_krylov_plan *plan);
 

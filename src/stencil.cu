@@ -1266,7 +1266,7 @@ DistributedDomain::KrylovCache &DistributedDomain::krylov_plans(int mode, const 
   auto found = krylovPlans_.find(key);
   if (found != krylovPlans_.end()) return found->second;
   KrylovCache c;
-  c.nparts = mode == SB_KRYLOV_DOT ? int(qs.size()) - 1 : mode == SB_KRYLOV_UPDATE ? 1 : 0;
+  c.nparts = mode == SB_KRYLOV_DOT ? int(qs.size()) - 1 : mode == SB_KRYLOV_UPDATE ? int(qs.size()) - 3 : 0; // UPDATE with c: 2
   for (LocalDomain &d : domains_) {
     const Rect3 cr = d.get_compute_region();
     const Dim3 ao = d.origin() - Dim3(radius_.x(-1), radius_.y(-1), radius_.z(-1));
@@ -1290,7 +1290,7 @@ DistributedDomain::KrylovCache &DistributedDomain::krylov_plans(int mode, const 
   return krylovPlans_.emplace(key, std::move(c)).first->second;
 }
 
-void DistributedDomain::krylov_launch(KrylovCache &c, double s, bool queued) {
+void DistributedDomain::krylov_launch(KrylovCache &c, double s, double t, bool queued) {
   if (queued) {
     create_apply_streams();
     queue_after_exterior();
@@ -1302,7 +1302,7 @@ void DistributedDomain::krylov_launch(KrylovCache &c, double s, bool queued) {
   }
   for (size_t di = 0; di < domains_.size(); ++di) {
     domains_[di].set_device();
-    if (SB_OK != sb_krylov_plan_launch(c.plans[di], s, c.out[di], queued ? applyStreams_[2 * di] : cudaStream_t(streams_[di])))
+    if (SB_OK != sb_krylov_plan_launch2(c.plans[di], s, t, c.out[di], queued ? applyStreams_[2 * di] : cudaStream_t(streams_[di])))
       LOG_FATAL("krylov: " << sb_last_error());
   }
 }

@@ -42,5 +42,6 @@ from .domain import (  # noqa: F401
 from .stencil_op import StencilOp, StencilPlan, StencilSystem, SystemPlan  # noqa: F401
 from .multigrid import Multigrid  # noqa: F401
 from .krylov import PCG  # noqa: F401
+from .bicgstab import BiCGStab  # noqa: F401
 
 __all__ = [n for n in dir() if not n.startswith("_")]

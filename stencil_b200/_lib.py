@@ -163,7 +163,7 @@ I6 = C.c_int32 * 6
 
 TRANSFER_RESTRICT, TRANSFER_PROLONG = 0, 1  # sb_transfer_kind
 
-KRYLOV_DOT, KRYLOV_XPBY, KRYLOV_UPDATE = 0, 1, 2  # sb_krylov_mode
+KRYLOV_DOT, KRYLOV_XPBY, KRYLOV_UPDATE, KRYLOV_BICG_P = 0, 1, 2, 4  # sb_krylov_mode (3 is not a mode)
 
 FUSED_MAX_GROUPS = 4096  # SB_FUSED_MAX_GROUPS
 
@@ -217,6 +217,7 @@ _SIGS = {
     "sb_reduce_exact_round": (C.c_int, [C.POINTER(ReduceExactPart), C.POINTER(ReduceResult)]),
     "sb_krylov_plan_create": (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, C.POINTER(Pitched), C.c_int, I3, I3, I3]),
     "sb_krylov_plan_launch": (C.c_int, [C.c_void_p, C.c_double, C.c_void_p, C.c_void_p]),
+    "sb_krylov_plan_launch2": (C.c_int, [C.c_void_p, C.c_double, C.c_double, C.c_void_p, C.c_void_p]),
     "sb_krylov_plan_bytes": (C.c_int64, [C.c_void_p]),
     "sb_krylov_plan_destroy": (C.c_int, [C.c_void_p]),
     "sb_stencil_check": (C.c_int, [C.POINTER(StencilTerm), C.c_int, I27]),

@@ -1,0 +1,225 @@
+"""Multigrid-preconditioned BiCGStab for A x = f on a DistributedDomain (DESIGN.md section 2.14): right-preconditioned
+BiCGStab for non-symmetric operators such as advection-diffusion, -div(kappa grad x) + b . grad x (+ sigma x), with one
+V-cycle of stencil_b200.Multigrid from zero as the preconditioner, the vector algebra in the fused sm_90a Krylov kernels
+and every inner product exact, so the iterates are the same bits on every partition and rank count.
+
+    A_at = lambda l: sb.StencilOp(diffusion(h * 2**l) + convection(b, h * 2**l), np.float64)
+    bi = sb.BiCGStab(dd, x, f, r, r0, p, v, phat, shat, t, A_at, coefs=[kx, ky, kz])   # nine quantities, then kappa
+    history = bi.solve(1e-8, 30)                                                      # sqrt(<r, r>) per step
+    bi.close()
+
+phat and shat must carry the homogeneous counterpart of x's wall BC on every FIXED face (homogeneous_bc), as PCG's p
+and z do; x keeps its own BC, which enters through the first residual.  A breakdown (<r0, v> zero or not finite, <t, t>
+zero, omega zero or not finite, or a new <r0, r> zero or not finite) stops the solve and is recorded in .breakdown.
+dd.swap() may be called between solves: every pass looks its buffers up for the current swap parity."""
+from __future__ import annotations
+
+import math
+from typing import Callable, List, Optional, Sequence
+
+import numpy as np
+
+from . import _lib
+from .domain import FACES, BC, BCKind, Boundary, DataHandle, DistributedDomain
+from .krylov import homogeneous_bc
+from .multigrid import Multigrid, _Clear, residual_op
+from .stencil_op import StencilOp
+
+
+class BiCGStab:
+    """Right-preconditioned BiCGStab for A x = f on the realized domain dd.  x, f, r, r0, p, v, phat, shat and t are nine
+    distinct float32 or float64 quantities of dd (curr buffers): x the solution (its initial value is the first guess),
+    f the right-hand side, r the residual (s from the half step on), r0 the shadow residual, p the direction, v = A phat,
+    phat = M p, shat = M s and t = A shat.  op_at(l) returns A on level l as Multigrid takes it; an internal
+    Multigrid(dd, phat, p, v, op_at, nu1, nu2, coarse_sweeps, levels, coefs, coef_kinds) is M, run on the pair (phat, p)
+    and, by Multigrid.cycle(u=shat, f=r), on (shat, r) (v is only the scratch of its residual_norm, which BiCGStab never
+    calls).  coefs / coef_kinds: as for Multigrid.  Building, solve(), residual_norm() and update_coefficients() are
+    collective under torchrun.  The solver never calls dd.swap(); a caller may swap between solves."""
+
+    NAMES = ("x", "f", "r", "r0", "p", "v", "phat", "shat", "t")
+
+    def __init__(self, dd: DistributedDomain, x: DataHandle, f: DataHandle, r: DataHandle, r0: DataHandle, p: DataHandle, v: DataHandle,
+                 phat: DataHandle, shat: DataHandle, t: DataHandle, op_at: Callable[[int], StencilOp], coefs: Optional[Sequence[DataHandle]] = None,
+                 coef_kinds: Optional[Sequence[str]] = None, nu1: int = 2, nu2: int = 2, coarse_sweeps: int = 30, levels: Optional[int] = None):
+        self.mg: Optional[Multigrid] = None
+        self.breakdown: Optional[int] = None
+        if not isinstance(dd, DistributedDomain) or dd.partition_ is None or not dd._plans:
+            raise _lib.StencilError("BiCGStab: dd must be a realized DistributedDomain")
+        named = list(zip(self.NAMES, (x, f, r, r0, p, v, phat, shat, t)))
+        for name, h in named:
+            if not isinstance(h, DataHandle) or not 0 <= h.id < len(dd.dtypes_):
+                raise _lib.StencilError(f"BiCGStab: {name} must be a DataHandle of dd, not {h!r}")
+        if len({h.id for _, h in named}) != len(named):
+            raise _lib.StencilError(f"BiCGStab: {', '.join(self.NAMES)} must be 9 different quantities")
+        dtype = dd.dtypes_[x.id]
+        if dtype not in (np.dtype(np.float32), np.dtype(np.float64)) or any(dd.dtypes_[h.id] != dtype for _, h in named):
+            raise _lib.StencilError(f"BiCGStab: {', '.join(self.NAMES)} must all be float32 or all float64")
+        coefs = list(coefs) if coefs is not None else []
+        for k, h in enumerate(coefs):
+            if not isinstance(h, DataHandle) or not 0 <= h.id < len(dd.dtypes_):
+                raise _lib.StencilError(f"BiCGStab: coefficient {k} must be a DataHandle of dd, not {h!r}")
+            if any(h.id == g.id for _, g in named) or dd.dtypes_[h.id] != dtype:
+                raise _lib.StencilError(f"BiCGStab: coefficient {k} must be a quantity of x's type other than the nine vectors")
+        # phat and shat are what A is applied to: the homogeneous counterpart of x's BC on every FIXED face
+        for fc in range(6):
+            if dd.boundary_[fc // 2] != Boundary.FIXED:
+                continue
+            bx = dd.bcs_.get((x.id, fc), BC.NONE())
+            if bx.kind == BCKind.NONE:
+                raise _lib.StencilError(f"BiCGStab: x needs a boundary condition (ODD, EVEN or VALUE) on every FIXED face (face {FACES[fc]})")
+            want = homogeneous_bc(bx)
+            for name, h in (("phat", phat), ("shat", shat)):
+                got = dd.bcs_.get((h.id, fc), BC.NONE())
+                if got != want:
+                    raise _lib.StencilError(f"BiCGStab: {name} needs {want!r} on face {FACES[fc]}, the homogeneous counterpart of x's {bx!r}, not {got!r}")
+        A = op_at(0)
+        if not isinstance(A, StencilOp) or A.dtype != dtype:
+            raise _lib.StencilError(f"BiCGStab: op_at(0) must be a StencilOp in {dtype}, not {A!r}")
+        if A.has_aux:
+            raise _lib.StencilError("BiCGStab: op_at(0) has an aux term; A reads x only")
+        if A.ncoef != len(coefs):
+            raise _lib.StencilError(f"BiCGStab: op_at(0) reads {A.ncoef} coefficient fields, but {len(coefs)} were given")
+        A.check(dd.radius_)
+        self.dd = dd
+        self.x, self.f, self.r, self.r0, self.p, self.v, self.phat, self.shat, self.t = x, f, r, r0, p, v, phat, shat, t
+        self.A, self.res = A, residual_op(A)
+        self.coefs = coefs or None
+        self.mg = Multigrid(dd, phat, p, v, op_at, nu1=nu1, nu2=nu2, coarse_sweeps=coarse_sweeps, levels=levels, coefs=coefs or None,
+                            coef_kinds=coef_kinds)
+        try:
+            self.mg._fine_level(shat, r)  # the second pair's checks, now rather than at the first solve
+        except Exception:
+            self.close()
+            raise
+        if not dd._apply_streams:
+            import torch
+
+            dd._apply_streams = [(torch.cuda.Stream(device=d.gpu()), torch.cuda.Stream(device=d.gpu())) for d in dd.domains_]
+        # <t, r> and <t, t> by one two-pair DOT in FP64; in FP32 by two one-pair DOTs, the faster form there (section
+        # 2.13).  The sums are exact either way, so the choice changes no bit.
+        self._split_tr_tt = dtype == np.dtype(np.float32)
+
+    # -- the queued schedule
+    def _plans(self, mode: int, *handles: DataHandle):
+        return self.dd.krylov_plans(mode, handles)
+
+    def _queue(self, plans, s: float = 0.0, t: float = 0.0) -> None:
+        for pl in plans:
+            pl.s, pl.t = float(s), float(t)
+        self.dd._run_plans([(pl,) for pl in plans], False, queued=True)
+
+    def _combine(self, *launched) -> List[float]:
+        """Host wait: the parts of the last launch of each plan list in launched, gathered across ranks in one exchange,
+        combined and rounded once (PCG._combine)."""
+        dd = self.dd
+        mine = []
+        for di, (idx, (si, _)) in enumerate(zip(dd.domain_idx_, dd._apply_streams)):
+            mine.append((idx, [part for plans in launched for part in plans[di].parts(si)]))
+        return [red.sum for red in dd._exact_gather(mine, sum(plans[0].n for plans in launched))]
+
+    def _apply_A(self, out: DataHandle, src: DataHandle) -> None:
+        self.dd._run_plans(*self.dd._apply_plans(self.A, (out, "curr"), src, None, True, self.coefs), queued=True)
+
+    def _precondition(self, u: DataHandle, f: DataHandle) -> None:
+        """u = M f: u set to +0, then one cycle on the pair (u, f), queued."""
+        dd = self.dd
+        dd._run_plans([(_Clear(d, u.id),) for d in dd.domains_], False, queued=True)
+        self.mg.cycle(wait=False, u=u, f=f)
+
+    def _start(self) -> float:
+        """r = f - A x with x's own BC through the exchange, r0 = r; returns rho = <r0, r> (= <r, r>)."""
+        import torch
+
+        dd = self.dd
+        for d, (si, se) in zip(dd.domains_, dd._apply_streams):
+            si.wait_stream(torch.cuda.current_stream(d.gpu()))
+            se.wait_stream(torch.cuda.current_stream(d.gpu()))
+        dd._run_plans(*dd._apply_plans(self.res, (self.r, "curr"), self.x, (self.f, "curr"), True, self.coefs), queued=True)
+        self._queue(self._plans(_lib.KRYLOV_XPBY, self.r0, self.r), 0.0)
+        rr = self._plans(_lib.KRYLOV_DOT, self.r0, self.r)
+        self._queue(rr)
+        return self._combine(rr)[0]
+
+    def _iterate(self, k: int, target: float, hist: List[float]) -> bool:
+        """Iteration k (from 0); appends sqrt(<r, r>) of each new x to hist.  Returns True to go on, False to stop (the
+        half-step or full-step residual reached target, or a breakdown, recorded in .breakdown)."""
+        K = _lib
+        if k == 0:
+            self._queue(self._plans(K.KRYLOV_XPBY, self.p, self.r), 0.0)
+        else:
+            beta = (self._rho / self._rho_prev) * (self._alpha / self._omega)
+            self._queue(self._plans(K.KRYLOV_BICG_P, self.p, self.r, self.v), beta, self._omega)
+        self._precondition(self.phat, self.p)
+        self._apply_A(self.v, self.phat)
+        rv = self._plans(K.KRYLOV_DOT, self.r0, self.v)
+        self._queue(rv)
+        sigma = self._combine(rv)[0]
+        if sigma == 0.0 or not math.isfinite(sigma):
+            self.breakdown = k
+            return False
+        alpha = self._rho / sigma
+        half = self._plans(K.KRYLOV_UPDATE, self.x, self.phat, self.r, self.v)
+        self._queue(half, alpha)
+        self._precondition(self.shat, self.r)
+        self._apply_A(self.t, self.shat)
+        if self._split_tr_tt:
+            tr, tt = self._plans(K.KRYLOV_DOT, self.t, self.r), self._plans(K.KRYLOV_DOT, self.t, self.t)
+            self._queue(tr)
+            self._queue(tt)
+            ss, t_r, t_t = self._combine(half, tr, tt)
+        else:
+            trt = self._plans(K.KRYLOV_DOT, self.t, self.r, self.t)
+            self._queue(trt)
+            ss, t_r, t_t = self._combine(half, trt)
+        hist.append(math.sqrt(ss))
+        if hist[-1] <= target:
+            return False
+        omega = t_r / t_t if t_t != 0.0 else 0.0
+        if t_t == 0.0 or omega == 0.0 or not math.isfinite(omega):
+            self.breakdown = k
+            return False
+        full = self._plans(K.KRYLOV_UPDATE, self.x, self.shat, self.r, self.t, self.r0)
+        self._queue(full, omega)
+        rr, rho = self._combine(full)
+        hist[-1] = math.sqrt(rr)
+        self._rho_prev, self._rho, self._alpha, self._omega = self._rho, rho, alpha, omega
+        if hist[-1] <= target:
+            return False
+        if rho == 0.0 or not math.isfinite(rho):
+            self.breakdown = k
+            return False
+        return True
+
+    def solve(self, rtol: float, max_iters: int) -> List[float]:
+        """Iterations from the current x until sqrt(<r, r>) <= rtol ||f||_2 (||f||_2 exact, as Multigrid.solve) or
+        max_iters iterations; returns sqrt(<r, r>) before the first iteration and after each, the last entry being that
+        of the x left behind: the half-step iterate when the half step reached the target or omega broke down.  r is
+        the recursive residual (residual_norm() gives the true one).  A breakdown stops the solve with the history so far
+        and sets .breakdown to its iteration (None otherwise).  Every rank calls it."""
+        target = float(rtol) * self.dd.reduce(self.f, "curr", exact=True).l2()
+        self.breakdown = None
+        self._rho = self._start()
+        hist = [math.sqrt(self._rho)]
+        k = 0
+        while hist[-1] > target and k < int(max_iters):
+            if not self._iterate(k, target, hist):
+                break
+            k += 1
+        return hist
+
+    def residual_norm(self) -> float:
+        """The true ||f - A x||_2 over dd's compute region (the residual into r, then an exact dot)."""
+        self.dd.apply(self.res, (self.r, "curr"), self.x, (self.f, "curr"), coefs=self.coefs)
+        return math.sqrt(self.dd.dot(self.r, self.r))
+
+    def update_coefficients(self) -> None:
+        """Re-coarsen the preconditioner's coefficient fields after they change (Multigrid.update_coefficients); A on
+        the fine level reads the fields directly."""
+        if self.mg is not None:
+            self.mg.update_coefficients()
+
+    def close(self) -> None:
+        """Release the preconditioner's coarse domains (the Krylov plans stay in dd's cache until dd.close())."""
+        if self.mg is not None:
+            self.mg.close()
+            self.mg = None

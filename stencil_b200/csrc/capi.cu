@@ -1290,13 +1290,18 @@ int sb_reduce_exact_round(const sb_reduce_exact_part *part, sb_reduce_result *ou
 int sb_krylov_plan_create(sb_krylov_plan **out, int device, int mode, int dtype, const sb_pitched *bufs, int nbuf, const int64_t acc_origin[3],
                           const int64_t lo[3], const int64_t hi[3]) {
   if (!out || !acc_origin || !lo || !hi) return fail(SB_ERR_INVALID, "sb_krylov_plan_create needs an output handle, acc_origin, lo and hi");
-  if (mode < SB_KRYLOV_DOT || mode > SB_KRYLOV_UPDATE) return fail(SB_ERR_INVALID, "unknown krylov mode %d", mode);
+  if (mode < SB_KRYLOV_DOT || mode > SB_KRYLOV_BICG_P || mode == 3) return fail(SB_ERR_INVALID, "unknown krylov mode %d", mode);
   if (dtype != SB_DTYPE_F32 && dtype != SB_DTYPE_F64) return fail(SB_ERR_INVALID, "dtype %d must be SB_DTYPE_F32 or SB_DTYPE_F64", dtype);
-  static const char *const names[3][4] = {{"a", "b", "c", ""}, {"p", "z", "", ""}, {"x", "p", "r", "q"}};
-  const bool count_ok = mode == SB_KRYLOV_DOT ? (nbuf == 2 || nbuf == 3) : mode == SB_KRYLOV_XPBY ? nbuf == 2 : nbuf == 4;
+  static const char *const names[5][5] = {{"a", "b", "c", "", ""}, {"p", "z", "", "", ""}, {"x", "p", "r", "q", "c"}, {}, {"p", "r", "v", "", ""}};
+  static const char *const mode_name[5] = {"SB_KRYLOV_DOT", "SB_KRYLOV_XPBY", "SB_KRYLOV_UPDATE", "", "SB_KRYLOV_BICG_P"};
+  const bool count_ok = mode == SB_KRYLOV_DOT      ? (nbuf == 2 || nbuf == 3)
+                        : mode == SB_KRYLOV_XPBY   ? nbuf == 2
+                        : mode == SB_KRYLOV_BICG_P ? nbuf == 3
+                                                   : (nbuf == 4 || nbuf == 5);
   if (!bufs || !count_ok)
-    return fail(SB_ERR_INVALID, "%s takes %s buffers, not %d", mode == SB_KRYLOV_DOT ? "SB_KRYLOV_DOT" : mode == SB_KRYLOV_XPBY ? "SB_KRYLOV_XPBY" : "SB_KRYLOV_UPDATE",
-                mode == SB_KRYLOV_DOT ? "2 or 3" : mode == SB_KRYLOV_XPBY ? "2" : "4", nbuf);
+    return fail(SB_ERR_INVALID, "%s takes %s buffers, not %d%s", mode_name[mode],
+                mode == SB_KRYLOV_DOT ? "2 or 3" : mode == SB_KRYLOV_XPBY ? "2" : mode == SB_KRYLOV_BICG_P ? "3" : "4", nbuf,
+                mode == SB_KRYLOV_UPDATE ? " (5 with c)" : "");
   const int es = dtype == SB_DTYPE_F32 ? 4 : 8;
   for (int a = 0; a < 3; ++a)
     if (lo[a] > hi[a]) return fail(SB_ERR_INVALID, "lo > hi on axis %d", a);
@@ -1318,17 +1323,24 @@ int sb_krylov_plan_create(sb_krylov_plan **out, int device, int mode, int dtype,
     for (int i = 0; i < 4; ++i)
       for (int j = i + 1; j < 4; ++j)
         if (bufs[i].ptr == bufs[j].ptr) return fail(SB_ERR_INVALID, "SB_KRYLOV_UPDATE: x, p, r and q must be four distinct buffers (%s is %s)", names[2][j], names[2][i]);
-  // a written buffer must not overlap another buffer of the pass: the bytes from the box's first cell to its last
+  if (mode == SB_KRYLOV_UPDATE && nbuf == 5 && (bufs[4].ptr == bufs[0].ptr || bufs[4].ptr == bufs[2].ptr))
+    return fail(SB_ERR_INVALID, "SB_KRYLOV_UPDATE: c must not be x or r (c is %s)", bufs[4].ptr == bufs[0].ptr ? "x" : "r");
+  if (mode == SB_KRYLOV_BICG_P && (bufs[0].ptr == bufs[1].ptr || bufs[0].ptr == bufs[2].ptr))
+    return fail(SB_ERR_INVALID, "SB_KRYLOV_BICG_P: p must not be r or v (%s is p)", bufs[0].ptr == bufs[1].ptr ? "r" : "v");
+  // a written buffer must not overlap another buffer of the pass: the bytes from the box's first cell to its last.  Of
+  // two read-only buffers, only UPDATE's p and q are checked (UPDATE's c and BICG_P's r and v may alias).
+  const unsigned written = mode == SB_KRYLOV_UPDATE ? 5u : 1u;
   if (mode != SB_KRYLOV_DOT && ahi[0] > alo[0] && ahi[1] > alo[1] && ahi[2] > alo[2]) {
     const long long slice = bufs[0].pitch * bufs[0].ysize;
     const long long first = (long long)alo[2] * slice + (long long)alo[1] * bufs[0].pitch + (long long)alo[0] * es;
     const long long last = (long long)(ahi[2] - 1) * slice + (long long)(ahi[1] - 1) * bufs[0].pitch + (long long)ahi[0] * es;
     for (int i = 0; i < nbuf; ++i)
       for (int j = i + 1; j < nbuf; ++j) {
+        const bool read_only = !((written >> i) & 1u) && !((written >> j) & 1u);
+        if (read_only && (mode == SB_KRYLOV_BICG_P || j == 4)) continue;
         const uintptr_t a = uintptr_t(bufs[i].ptr), b = uintptr_t(bufs[j].ptr);
         if (a + uintptr_t(first) < b + uintptr_t(last) && b + uintptr_t(first) < a + uintptr_t(last))
-          return fail(SB_ERR_INVALID, "%s: buffers %s and %s overlap over the box", mode == SB_KRYLOV_XPBY ? "SB_KRYLOV_XPBY" : "SB_KRYLOV_UPDATE",
-                      names[mode][i], names[mode][j]);
+          return fail(SB_ERR_INVALID, "%s: buffers %s and %s overlap over the box", mode_name[mode], names[mode][i], names[mode][j]);
       }
   }
   sb::KryParams kp{};
@@ -1337,7 +1349,7 @@ int sb_krylov_plan_create(sb_krylov_plan **out, int device, int mode, int dtype,
   for (int a = 0; a < 3; ++a) kp.ext[a] = ahi[a] - alo[a];
   const long long off = (long long)alo[2] * kp.slice + (long long)alo[1] * kp.pitch + (long long)alo[0] * es;
   bool wide = true;
-  for (int k = 0; k < 4; ++k) {
+  for (int k = 0; k < 5; ++k) {
     kp.buf[k] = static_cast<char *>(bufs[k < nbuf ? k : 0].ptr) + off;
     wide = wide && ((uintptr_t(kp.buf[k]) - uintptr_t(kp.buf[0])) % 16 == 0);
   }
@@ -1350,9 +1362,10 @@ int sb_krylov_plan_create(sb_krylov_plan **out, int device, int mode, int dtype,
   const long long rows_per_tile = std::max(1ll, sb::kRedChain / std::max(1ll, per_row)) * (sb::kRedThreads >> kp.lg_group);
   kp.rows_per_tile = unsigned(rows_per_tile);
   kp.ntiles = kp.count > 0 ? unsigned((rows + rows_per_tile - 1) / rows_per_tile) : 0u;
-  int kmode = sb::kKryUpdate;
+  int kmode = nbuf == 5 ? sb::kKryUpdateC : sb::kKryUpdate;
   if (mode == SB_KRYLOV_DOT) kmode = nbuf == 3 ? sb::kKryDot2 : sb::kKryDot1;
   if (mode == SB_KRYLOV_XPBY) kmode = sb::kKryXpby;
+  if (mode == SB_KRYLOV_BICG_P) kmode = sb::kKryBicgP;
   // per cell: one element per distinct buffer read, one per buffer written
   int nread = 0;
   for (int k = 0; k < nbuf; ++k) {
@@ -1360,7 +1373,7 @@ int sb_krylov_plan_create(sb_krylov_plan **out, int device, int mode, int dtype,
     for (int j = 0; j < k; ++j) dup = dup || bufs[j].ptr == bufs[k].ptr;
     nread += !dup;
   }
-  const int nwrite = mode == SB_KRYLOV_XPBY ? 1 : mode == SB_KRYLOV_UPDATE ? 2 : 0;
+  const int nwrite = mode == SB_KRYLOV_XPBY || mode == SB_KRYLOV_BICG_P ? 1 : mode == SB_KRYLOV_UPDATE ? 2 : 0;
   DeviceGuard guard(device);
   if (!guard.ok) return fail(SB_ERR_NOGPU, "cannot select CUDA device %d", device);
   sb_krylov_plan *p = new sb_krylov_plan();
@@ -1386,6 +1399,12 @@ int sb_krylov_plan_create(sb_krylov_plan **out, int device, int mode, int dtype,
 
 int sb_krylov_plan_launch(sb_krylov_plan *p, double s, sb_reduce_exact_part *parts_dev, void *stream) {
   if (!p) return fail(SB_ERR_INVALID, "null plan");
+  if (p->mode == sb::kKryBicgP) return fail(SB_ERR_INVALID, "sb_krylov_plan_launch: SB_KRYLOV_BICG_P takes two scalars; use sb_krylov_plan_launch2");
+  return sb_krylov_plan_launch2(p, s, 0.0, parts_dev, stream);
+}
+
+int sb_krylov_plan_launch2(sb_krylov_plan *p, double s, double t, sb_reduce_exact_part *parts_dev, void *stream) {
+  if (!p) return fail(SB_ERR_INVALID, "null plan");
   if (!parts_dev && sb::kry_dots(p->mode) > 0) return fail(SB_ERR_INVALID, "null output buffer");
   DeviceGuard guard(p->device);
   if (!guard.ok) return fail(SB_ERR_NOGPU, "cannot select CUDA device %d", p->device);
@@ -1395,7 +1414,7 @@ int sb_krylov_plan_launch(sb_krylov_plan *p, double s, sb_reduce_exact_part *par
     mode = sb::kKryCopy;
     grid = p->copy_grid;
   }
-  g_launches += uint64_t(sb::launch_krylov(p->params, p->dtype, mode, p->wide, grid, s, p->scratch, parts_dev, static_cast<cudaStream_t>(stream)));
+  g_launches += uint64_t(sb::launch_krylov(p->params, p->dtype, mode, p->wide, grid, s, t, p->scratch, parts_dev, static_cast<cudaStream_t>(stream)));
   SB_CUDA(cudaGetLastError());
   return SB_OK;
 }

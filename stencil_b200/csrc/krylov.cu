@@ -44,17 +44,19 @@ template <int D> __device__ __forceinline__ void kry_term(KryAcc &a, double v) {
 
 // the buffers a mode reads and writes (bit k: buffer k); a buffer read and not written goes through the read-only cache
 __host__ __device__ constexpr unsigned kry_reads(int m) {
-  return m == kKryDot1 ? 3u : m == kKryDot2 ? 7u : m == kKryCopy ? 2u : m == kKryXpby ? 3u : 15u;
+  return m == kKryDot1 ? 3u : m == kKryDot2 ? 7u : m == kKryCopy ? 2u : m == kKryXpby ? 3u : m == kKryBicgP ? 7u : m == kKryUpdateC ? 31u : 15u;
 }
-__host__ __device__ constexpr unsigned kry_writes(int m) { return m == kKryCopy || m == kKryXpby ? 1u : m == kKryUpdate ? 5u : 0u; }
+__host__ __device__ constexpr unsigned kry_writes(int m) {
+  return m == kKryCopy || m == kKryXpby || m == kKryBicgP ? 1u : m == kKryUpdate || m == kKryUpdateC ? 5u : 0u;
+}
 
 // N consecutive cells at byte offset `off` of every buffer: loaded, then the rule, then stored
 template <typename T, int MODE, int N> struct KryChunk {
   using V = typename KVec<T, N>::type;
-  T v[4][N];
+  T v[5][N];
   __device__ __forceinline__ void load(char *const *p, long long off) {
 #pragma unroll
-    for (int k = 0; k < 4; ++k) {
+    for (int k = 0; k < 5; ++k) {
       if (!((kry_reads(MODE) >> k) & 1u)) continue;
       const V *q = reinterpret_cast<const V *>(p[k] + off);
       V w;
@@ -66,10 +68,19 @@ template <typename T, int MODE, int N> struct KryChunk {
       for (int e = 0; e < N; ++e) v[k][e] = reinterpret_cast<const T *>(&w)[e];
     }
   }
-  __device__ __forceinline__ void apply(T s, KryAcc &a) {
+  __device__ __forceinline__ void apply(T s, T t, KryAcc &a) {
 #pragma unroll
     for (int e = 0; e < N; ++e) {
-      if (MODE == kKryDot1) {
+      if (MODE == kKryBicgP) {
+        // p = r + T(beta) * (p - T(omega) * v)
+        v[0][e] = t_add(v[1][e], t_mul(s, t_add(v[0][e], -t_mul(t, v[2][e]))));
+      } else if (MODE == kKryUpdateC) {
+        v[0][e] = t_add(v[0][e], t_mul(s, v[1][e]));
+        v[2][e] = t_add(v[2][e], -t_mul(s, v[3][e]));
+        const double r = double(v[2][e]);
+        kry_term<0>(a, __dmul_rn(r, r));
+        kry_term<1>(a, __dmul_rn(double(v[4][e]), r));
+      } else if (MODE == kKryDot1) {
         kry_term<0>(a, __dmul_rn(double(v[0][e]), double(v[1][e])));
       } else if (MODE == kKryDot2) {
         const double x = double(v[0][e]);
@@ -89,7 +100,7 @@ template <typename T, int MODE, int N> struct KryChunk {
   }
   __device__ __forceinline__ void store(char *const *p, long long off) const {
 #pragma unroll
-    for (int k = 0; k < 4; ++k) {
+    for (int k = 0; k < 5; ++k) {
       if (!((kry_writes(MODE) >> k) & 1u)) continue;
       V w;
 #pragma unroll
@@ -100,19 +111,22 @@ template <typename T, int MODE, int N> struct KryChunk {
 };
 
 // The tiles of the box, any CTA any tile.  Per tile: the rows by groups of G lanes (head and tail cells one by one, the
-// body in 16-byte vectors when WIDE, four per buffer in flight per lane); with dots, the expansions merged per warp into
+// body in 16-byte vectors when WIDE, IF per buffer in flight per lane); with dots, the expansions merged per warp into
 // the CTA's accumulator, which goes to the tile's partial with min / max and is cleared for the next tile.
 template <typename T, int MODE, bool WIDE>
-__global__ void __launch_bounds__(kRedThreads, 2) krylov_kernel(const KryParams P, const double s_, KryPartial *__restrict__ part) {
+__global__ void __launch_bounds__(kRedThreads, 2) krylov_kernel(const KryParams P, const double s_, const double t_, KryPartial *__restrict__ part) {
   constexpr int ND = kry_dots(MODE);
   constexpr int N = WIDE ? 16 / int(sizeof(T)) : 1;
+  // vectors per buffer in flight per lane: UPDATE with c holds five buffers and two accumulators, and with four it
+  // would spill under the two-CTA register cap
+  constexpr int IF = MODE == kKryUpdateC ? 2 : 4;
   __shared__ ExShared sh;
   __shared__ double warp_mn[2][kRedThreads / 32], warp_mx[2][kRedThreads / 32];
   if (ND) {
     for (int k = threadIdx.x; k < 2 * kExDigits; k += kRedThreads) sh.digit[k / kExDigits][k % kExDigits] = 0;
     if (threadIdx.x < 2) sh.flags[threadIdx.x] = 0;
   }
-  const T s = T(s_);
+  const T s = T(s_), t = T(t_);
   const unsigned lg = unsigned(P.lg_group), G = 1u << lg;
   const unsigned lane = threadIdx.x & (G - 1), per_pass = unsigned(kRedThreads) >> lg;
   const unsigned nx = unsigned(P.ext[0]), ey = unsigned(P.ext[1]), rows = ey * unsigned(P.ext[2]);
@@ -124,9 +138,9 @@ __global__ void __launch_bounds__(kRedThreads, 2) krylov_kernel(const KryParams 
 #pragma unroll 1
     for (unsigned row = r0 + (threadIdx.x >> lg); row < r1; row += per_pass) {
       const long long off = (long long)(row / ey) * P.slice + (long long)(row % ey) * P.pitch;
-      char *p[4];
+      char *p[5];
 #pragma unroll
-      for (int k = 0; k < 4; ++k) p[k] = P.buf[k] + off;
+      for (int k = 0; k < 5; ++k) p[k] = P.buf[k] + off;
       unsigned head = 0;
       if (WIDE) {
         head = unsigned((16 - (reinterpret_cast<uintptr_t>(p[0]) & 15)) & 15) / unsigned(sizeof(T));
@@ -138,28 +152,28 @@ __global__ void __launch_bounds__(kRedThreads, 2) krylov_kernel(const KryParams 
         for (unsigned j = lane; j < head; j += G) {
           KryChunk<T, MODE, 1> c;
           c.load(p, (long long)j * sizeof(T));
-          c.apply(s, a);
+          c.apply(s, t, a);
           c.store(p, (long long)j * sizeof(T));
         }
 #pragma unroll 1
         for (unsigned j = head + nvec * unsigned(N) + lane; j < nx; j += G) {
           KryChunk<T, MODE, 1> c;
           c.load(p, (long long)j * sizeof(T));
-          c.apply(s, a);
+          c.apply(s, t, a);
           c.store(p, (long long)j * sizeof(T));
         }
       }
       const long long body = (long long)head * sizeof(T);
 #pragma unroll 1
-      for (unsigned c0 = lane; c0 < nvec; c0 += 4 * G) {
-        KryChunk<T, MODE, N> c[4];
+      for (unsigned c0 = lane; c0 < nvec; c0 += unsigned(IF) * G) {
+        KryChunk<T, MODE, N> c[IF];
 #pragma unroll
-        for (int k = 0; k < 4; ++k)
+        for (int k = 0; k < IF; ++k)
           if (c0 + unsigned(k) * G < nvec) c[k].load(p, body + (long long)(c0 + unsigned(k) * G) * (N * sizeof(T)));
 #pragma unroll
-        for (int k = 0; k < 4; ++k) {
+        for (int k = 0; k < IF; ++k) {
           if (c0 + unsigned(k) * G < nvec) {
-            c[k].apply(s, a);
+            c[k].apply(s, t, a);
             c[k].store(p, body + (long long)(c0 + unsigned(k) * G) * (N * sizeof(T)));
           }
         }
@@ -264,13 +278,15 @@ __global__ void __launch_bounds__(kExCombineThreads) krylov_combine_kernel(const
   }
 }
 
-using KryKernel = void (*)(const KryParams, const double, KryPartial *);
+using KryKernel = void (*)(const KryParams, const double, const double, KryPartial *);
 template <typename T, bool WIDE> KryKernel kry_kernel_of(int mode) {
   switch (mode) {
   case kKryDot1: return krylov_kernel<T, kKryDot1, WIDE>;
   case kKryDot2: return krylov_kernel<T, kKryDot2, WIDE>;
   case kKryCopy: return krylov_kernel<T, kKryCopy, WIDE>;
   case kKryXpby: return krylov_kernel<T, kKryXpby, WIDE>;
+  case kKryBicgP: return krylov_kernel<T, kKryBicgP, WIDE>;
+  case kKryUpdateC: return krylov_kernel<T, kKryUpdateC, WIDE>;
   default: return krylov_kernel<T, kKryUpdate, WIDE>;
   }
 }
@@ -285,11 +301,11 @@ int krylov_grid(int device, int dtype, int mode, bool wide, unsigned ntiles) {
   return persistent_grid(device, reinterpret_cast<const void *>(kry_kernel(dtype, mode, wide)), ntiles);
 }
 
-int launch_krylov(const KryParams &p, int dtype, int mode, bool wide, int grid, double s, KryPartial *scratch, sb_reduce_exact_part *out,
+int launch_krylov(const KryParams &p, int dtype, int mode, bool wide, int grid, double s, double t, KryPartial *scratch, sb_reduce_exact_part *out,
                   cudaStream_t stream) {
   int launches = 0;
   if (p.ntiles > 0) {
-    kry_kernel(dtype, mode, wide)<<<grid, kRedThreads, 0, stream>>>(p, s, scratch);
+    kry_kernel(dtype, mode, wide)<<<grid, kRedThreads, 0, stream>>>(p, s, t, scratch);
     ++launches;
   }
   if (kry_dots(mode) > 0) {

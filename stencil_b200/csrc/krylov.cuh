@@ -18,11 +18,13 @@
 namespace sb {
 
 // kernel modes: the public SB_KRYLOV_DOT with one or two pairs, SB_KRYLOV_XPBY with T(s) = +-0 (a copy) or not, UPDATE
-enum KryMode { kKryDot1 = 0, kKryDot2 = 1, kKryCopy = 2, kKryXpby = 3, kKryUpdate = 4 };
-constexpr int kKryModes = 5;
+// without and with c, BICG_P (DESIGN.md section 2.14)
+enum KryMode { kKryDot1 = 0, kKryDot2 = 1, kKryCopy = 2, kKryXpby = 3, kKryUpdate = 4, kKryBicgP = 5, kKryUpdateC = 6 };
+constexpr int kKryModes = 7;
 
 struct KryParams {
-  char *buf[4];           // address of the box's cell lo in each buffer: DOT a, b[, c]; XPBY p, z; UPDATE x, p, r, q
+  char *buf[5];           // address of the box's cell lo in each buffer: DOT a, b[, c]; XPBY p, z; UPDATE x, p, r, q[, c];
+                          // BICG_P p, r, v
   long long pitch, slice; // bytes between rows / planes (the same for every buffer)
   int ext[3];             // box extent
   int lg_group;           // log2 of the lanes that share a row
@@ -38,13 +40,15 @@ struct KryPartial {
 };
 
 // dots written by a kernel mode
-__host__ __device__ constexpr int kry_dots(int mode) { return mode == kKryDot1 || mode == kKryUpdate ? 1 : mode == kKryDot2 ? 2 : 0; }
+__host__ __device__ constexpr int kry_dots(int mode) {
+  return mode == kKryDot1 || mode == kKryUpdate ? 1 : mode == kKryDot2 || mode == kKryUpdateC ? 2 : 0;
+}
 
 // the persistent grid of (dtype, mode, wide) for ntiles tiles
 int krylov_grid(int device, int dtype, int mode, bool wide, unsigned ntiles);
 // the tile launch (none for an empty box) and, for a mode with dots, the combine launch into out[0 .. dots); returns the
-// number of kernels launched
-int launch_krylov(const KryParams &p, int dtype, int mode, bool wide, int grid, double s, KryPartial *scratch, sb_reduce_exact_part *out,
+// number of kernels launched.  t is BICG_P's second scalar (omega); the other modes ignore it.
+int launch_krylov(const KryParams &p, int dtype, int mode, bool wide, int grid, double s, double t, KryPartial *scratch, sb_reduce_exact_part *out,
                   cudaStream_t stream);
 
 } // namespace sb

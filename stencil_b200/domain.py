@@ -566,8 +566,9 @@ class ExactReducePlan:
 
 
 class KrylovPlan:
-    """sb_krylov_plan: one Krylov vector pass (KRYLOV_DOT, KRYLOV_XPBY or KRYLOV_UPDATE) over one box, with its parts
-    (sb_reduce_exact_part, one per dot) written to a device buffer the plan owns.  One launch in flight at a time."""
+    """sb_krylov_plan: one Krylov vector pass (KRYLOV_DOT, KRYLOV_XPBY, KRYLOV_UPDATE or KRYLOV_BICG_P) over one box,
+    with its parts (sb_reduce_exact_part, one per dot) written to a device buffer the plan owns.  One launch in flight at
+    a time."""
 
     def __init__(self, device: int, mode: int, dtype, bufs: Sequence[Pitched], acc_origin: Vec, lo: Vec, hi: Vec):
         arr = (Pitched * max(1, len(bufs)))(*bufs)
@@ -575,7 +576,7 @@ class KrylovPlan:
         check(lib().sb_krylov_plan_create(C.byref(h), device, int(mode), bc_dtype(dtype), arr, len(bufs), i3(acc_origin), i3(lo), i3(hi)))
         self._h = h
         self.device = device
-        self.n = len(bufs) - 1 if mode == _lib.KRYLOV_DOT else 1 if mode == _lib.KRYLOV_UPDATE else 0
+        self.n = len(bufs) - 1 if mode == _lib.KRYLOV_DOT else len(bufs) - 3 if mode == _lib.KRYLOV_UPDATE else 0
         self.bytes = int(lib().sb_krylov_plan_bytes(h))
         self.out_dev = None
         if self.n:
@@ -585,12 +586,14 @@ class KrylovPlan:
                 raise _lib.StencilError(f"krylov parts buffer: {lib().sb_last_error().decode()}")
             self.out_dev = out.value
         self.s = 0.0  # the scalar of the next launch
+        self.t = 0.0  # the second scalar of the next launch (KRYLOV_BICG_P's omega; the other modes ignore it)
 
-    def launch(self, stream=None, s: Optional[float] = None) -> None:
-        """Queue the pass on `stream` with the scalar s (default: the attribute s, so a plan runs where a schedule
-        calls launch(stream) alone)."""
+    def launch(self, stream=None, s: Optional[float] = None, t: Optional[float] = None) -> None:
+        """Queue the pass on `stream` with the scalars s and t (default: the attributes s and t, so a plan runs where a
+        schedule calls launch(stream) alone)."""
         s = self.s if s is None else s
-        check(lib().sb_krylov_plan_launch(self._h, C.c_double(float(s)), C.c_void_p(self.out_dev or 0), stream_ptr(stream)))
+        t = self.t if t is None else t
+        check(lib().sb_krylov_plan_launch2(self._h, C.c_double(float(s)), C.c_double(float(t)), C.c_void_p(self.out_dev or 0), stream_ptr(stream)))
 
     def parts(self, stream=None) -> List[_lib.ReduceExactPart]:
         """Copy the last launch's parts (ordered after it on `stream`) to the host."""
@@ -1363,7 +1366,8 @@ class DistributedDomain:
 
     def krylov_plans(self, mode: int, handles: Sequence[DataHandle]) -> List[KrylovPlan]:
         """The KrylovPlans of one pass over the compute region of every local subdomain, on the curr buffers of handles
-        (in sb_krylov_plan_create's order: DOT a, b[, c]; XPBY p, z; UPDATE x, p, r, q), for the current swap parity.
+        (in sb_krylov_plan_create's order: DOT a, b[, c]; XPBY p, z; UPDATE x, p, r, q[, c]; BICG_P p, r, v), for the
+        current swap parity.
         Built on first use and kept until close(), like reduce_plans()."""
         if self.partition_ is None or not self._plans:
             raise _lib.StencilError("krylov_plans: call realize() first")

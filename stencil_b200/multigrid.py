@@ -186,6 +186,8 @@ class Multigrid:
             raise _lib.StencilError("Multigrid: A reads its own colour under both red-black and 8-colour orderings (or leaves the "
                                     "radius); no Gauss-Seidel smoother applies")
         self.levels: List[_Level] = [_Level(dd, u, f, ops[0], coefs)]
+        self._walls = {fc: dd.bcs_.get((u.id, fc), BC.NONE()) for fc in walls}  # u's own wall BCs, for cycle(u=, f=)
+        self._pairs = {}  # (u, f) ids -> the fine _Level of another pair (cycle(u=, f=))
         self.r = r
         self.coef_kinds = coef_kinds
         # every level queues on dd's apply streams, so stream order alone orders the work of consecutive levels
@@ -248,8 +250,8 @@ class Multigrid:
         if wait:
             self.wait()
 
-    def _vcycle(self, l: int) -> None:
-        L = self.levels[l]
+    def _vcycle(self, l: int, L: Optional[_Level] = None) -> None:
+        L = self.levels[l] if L is None else L
         if l == len(self.levels) - 1:
             self._smooth(L, self.coarse_sweeps)
             return
@@ -262,18 +264,56 @@ class Multigrid:
         L.dd._transfer(Cl.dd, _lib.TRANSFER_PROLONG, (L.u, "curr"), (Cl.u, "curr"), (L.u, "curr"), True, queued=True)
         self._smooth(L, self.nu2)
 
-    def cycle(self, wait: bool = True) -> None:
+    def _fine_level(self, u: DataHandle, f: DataHandle) -> _Level:
+        """The fine level of the pair (u, f): the constructor's, or one that shares A, the coefficient fields and every
+        coarse level (checked and built on first use)."""
+        L0 = self.levels[0]
+        if u is None and f is None:
+            return L0
+        key = (getattr(u, "id", None), getattr(f, "id", None))
+        if key == (L0.u.id, L0.f.id):
+            return L0
+        if key in self._pairs:
+            return self._pairs[key]
+        dd = L0.dd
+        for name, h in (("u", u), ("f", f)):
+            if not isinstance(h, DataHandle) or not 0 <= h.id < len(dd.dtypes_):
+                raise _lib.StencilError(f"Multigrid.cycle: {name} must be a DataHandle of dd, not {h!r}")
+        if u.id == f.id:
+            raise _lib.StencilError("Multigrid.cycle: u and f must be two different quantities")
+        dtype = dd.dtypes_[L0.u.id]
+        if dd.dtypes_[u.id] != dtype or dd.dtypes_[f.id] != dtype:
+            raise _lib.StencilError(f"Multigrid.cycle: u and f must be {dtype} quantities, like the constructor's u")
+        if any(h.id in {k.id for k in L0.coefs} for h in (u, f)):
+            raise _lib.StencilError("Multigrid.cycle: u and f must not be coefficient fields")
+        # the coarse walls were derived from the constructor u's BCs, so the new u must carry the same ones
+        for fc, want in self._walls.items():
+            got = dd.bcs_.get((u.id, fc), BC.NONE())
+            if got != want:
+                raise _lib.StencilError(f"Multigrid.cycle: u needs {want!r} on face {FACES[fc]}, the constructor u's BC, not {got!r}")
+        L = self._pairs[key] = _Level(dd, u, f, L0.A, L0.coefs)
+        return L
+
+    def cycle(self, wait: bool = True, u: Optional[DataHandle] = None, f: Optional[DataHandle] = None) -> None:
         """One V(nu1, nu2) cycle: per level nu1 sweeps, the fused residual-restriction into the coarse f, the coarse u set
         to +0, the recursion, the in-place prolongation u <- u + P e and nu2 sweeps; coarse_sweeps sweeps on the coarsest
         level.  Queued after the work on the caller's stream; returns when the cycle is complete (one host wait), or,
-        with wait=False, as soon as it is queued (call wait() before touching u)."""
+        with wait=False, as soon as it is queued (call wait() before touching u).
+
+        With u= and f=, the cycle runs on that fine-level pair instead of the constructor's, through the same coarse
+        levels and coarse coefficient fields: u and f are two different quantities of dd of the constructor u's type,
+        not coefficient fields, and u carries the constructor u's BC on every FIXED face (the coarse walls derive from
+        it).  The cycle is then the bits of one on a Multigrid built on (u, f).  Give both or neither."""
         import torch
 
+        if (u is None) != (f is None):
+            raise _lib.StencilError("Multigrid.cycle: give both u and f, or neither")
+        L = self._fine_level(u, f)
         dd = self.levels[0].dd
         for d, (si, se) in zip(dd.domains_, dd._apply_streams):
             si.wait_stream(torch.cuda.current_stream(d.gpu()))
             se.wait_stream(torch.cuda.current_stream(d.gpu()))
-        self._vcycle(0)
+        self._vcycle(0, L)
         if wait:
             self.wait()
 
@@ -318,3 +358,4 @@ class Multigrid:
         for cd in coarse:
             cd.close()
         self.levels = self.levels[:1]
+        self._pairs = {}
