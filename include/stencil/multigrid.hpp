@@ -41,8 +41,7 @@
 namespace stencil {
 
 template <typename T> class Multigrid {
-  friend class PCG<T>;      // queues this solver's cycle as its preconditioner
-  friend class BiCGStab<T>; // the same, on two pairs
+  friend class detail::KrylovSolver<T>; // queues this solver's cycles as the preconditioner of PCG and BiCGStab
 
 public:
   Multigrid(DistributedDomain &dd, DataHandle<T> u, DataHandle<T> f, DataHandle<T> r, const std::function<LinearStencil(int)> &op_at, int nu1 = 2,
@@ -62,7 +61,7 @@ public:
 
   // One V(nu1, nu2) cycle, queued after the work on the legacy default stream; returns when it is complete.
   void cycle() {
-    for (Level &L : levels_) L.dd->queued_ = true;
+    set_queued(true);
     vcycle(0);
     finish();
   }
@@ -70,7 +69,7 @@ public:
   // The same cycle on the fine-level pair (u, f) instead of the constructor's (see the header comment).
   void cycle(DataHandle<T> u, DataHandle<T> f) {
     Level &top = pair_level(u, f);
-    for (Level &L : levels_) L.dd->queued_ = true;
+    set_queued(true);
     vcycle(0, &top);
     finish();
   }
@@ -78,7 +77,7 @@ public:
   // Re-coarsen every level's coefficient fields from the current fine ones, level by level, queued like a cycle with one
   // host wait.  The constructor calls it once; call it again whenever the fine fields change.
   void update_coefficients() {
-    for (Level &L : levels_) L.dd->queued_ = true;
+    set_queued(true);
     for (size_t l = 0; l + 1 < levels_.size(); ++l)
       for (size_t k = 0; k < axes_.size(); ++k) {
         Level &F = levels_[l], &C = levels_[l + 1];
@@ -93,10 +92,7 @@ public:
   // ||f - A u||_2: the residual into r and an exact reduction, the same on every rank and partition
   double residual_norm() {
     Level &L = levels_[0];
-    if (L.coefs.empty())
-      L.dd->apply(L.res, curr(r_), L.u, curr(L.f));
-    else
-      L.dd->apply(L.res, curr(r_), L.u, curr(L.f), L.coefs);
+    L.dd->apply(L.res, curr(r_), L.u, curr(L.f), L.coefs);
     return std::sqrt(L.dd->reduce(r_, Which::curr, Sum::exact).sumsq);
   }
 
@@ -278,9 +274,14 @@ private:
 
   static LinearStencil smoother(const LinearStencil &A) { return A.ncoef() > 0 ? LinearStencil() : A.relax(1.0); }
 
+  // every level queues its work (or stops queueing it)
+  void set_queued(bool on) {
+    for (Level &L : levels_) L.dd->queued_ = on;
+  }
+
   // the end of a queued cycle: every apply stream and exchange of every level complete
   void finish() {
-    for (Level &L : levels_) L.dd->queued_ = false;
+    set_queued(false);
     DistributedDomain &dd = *levels_[0].dd;
     for (size_t i = 0; i < dd.applyStreams_.size(); ++i) {
       CUDA_RUNTIME(cudaSetDevice(dd.domains_[i / 2].gpu()));
@@ -317,18 +318,8 @@ private:
     }
     smooth(L, nu1_);
     Level &C = levels_[l + 1];
-    if (L.coefs.empty())
-      L.dd->restrict_to(*C.dd, curr(C.f), L.res, L.u, curr(L.f));
-    else
-      L.dd->restrict_to(*C.dd, curr(C.f), L.res, L.u, curr(L.f), L.coefs);
-    // coarse u <- +0: a memset of the curr allocation (an exchange refills the ghost cells before any read)
-    C.dd->queue_after_exterior();
-    for (size_t di = 0; di < C.dd->domains_.size(); ++di) {
-      LocalDomain &d = C.dd->domains_[di];
-      d.set_device();
-      const cudaPitchedPtr p = d.curr_data(C.u.id());
-      CUDA_RUNTIME(cudaMemsetAsync(p.ptr, 0, p.pitch * p.ysize * size_t(d.raw_size().z), C.dd->applyStreams_[2 * di]));
-    }
+    L.dd->restrict_to(*C.dd, curr(C.f), L.res, L.u, curr(L.f), L.coefs);
+    C.dd->clear_queued(C.u.id()); // coarse u <- +0
     vcycle(l + 1);
     L.dd->prolong_from(*C.dd, curr(L.u), curr(C.u), curr(L.u));
     smooth(L, nu2_);

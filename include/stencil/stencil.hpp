@@ -54,14 +54,14 @@ struct sb_transfer_plan;
 
 namespace stencil {
 template <typename T> class Multigrid;
-template <typename T> class PCG;
-template <typename T> class BiCGStab;
+namespace detail {
+template <typename T> class KrylovSolver;
+}
 }
 
 class DistributedDomain {
   template <typename T> friend class stencil::Multigrid;
-  template <typename T> friend class stencil::PCG;
-  template <typename T> friend class stencil::BiCGStab;
+  template <typename T> friend class stencil::detail::KrylovSolver;
 
 private:
   Dim3 size_; // compute extent of the whole grid
@@ -159,9 +159,9 @@ private:
   void krylov_launch(KrylovCache &c, double s, bool queued) { krylov_launch(c, s, 0.0, queued); }
   // the same with a second scalar t (SB_KRYLOV_BICG_P's omega; the other modes ignore it)
   void krylov_launch(KrylovCache &c, double s, double t, bool queued);
-  // the host wait: the parts of the last launch (on the streams krylov_launch used), gathered from every rank with
-  // MPI_Allgatherv, combined and rounded once; one sum per part
-  std::vector<double> krylov_sums(KrylovCache &c, bool queued);
+  // the host wait: the parts of the last launch of each cache (on the streams krylov_launch used), gathered from every
+  // rank in one MPI_Allgatherv, combined and rounded once; one sum per part, in the order of the caches
+  std::vector<double> krylov_sums(const std::vector<KrylovCache *> &cs, bool queued);
 
   // linear stencil operators: per (op, buffers, exchange, swap parity), per local domain the interior and exterior plans
   // (exchange = true) or the whole-region plan; two streams per local domain (interior, exterior)
@@ -191,6 +191,9 @@ private:
   bool sharedApplyStreams_ = false; // applyStreams_ belong to another domain (a solver's finer level)
   std::vector<cudaEvent_t> applyEvents_, exchangeEvents_; // one per apply / exchange stream, recorded again on each use
   void queue_after_exterior();
+  // quantity q's whole curr allocation set to +0 (ghost cells included; an exchange refills them before any read), on
+  // each interior apply stream after the previous exterior
+  void clear_queued(size_t q);
   void queue_exchange();
   void wait_exchange(DistributedDomain &other, bool interior);
   void ensure_queue_events();
@@ -358,7 +361,7 @@ public:
   template <typename T> double dot(const DataHandle<T> &a, const DataHandle<T> &b) {
     KrylovCache &c = krylov_plans(SB_KRYLOV_DOT, {a.id(), b.id()});
     krylov_launch(c, 0.0, false);
-    return krylov_sums(c, false)[0];
+    return krylov_sums({&c}, false)[0];
   }
 
   // dst = op(src, aux) over the whole compute region of every local subdomain (DESIGN.md section 2.7).  src is the curr

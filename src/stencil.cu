@@ -864,6 +864,16 @@ void DistributedDomain::queue_after_exterior() {
   }
 }
 
+void DistributedDomain::clear_queued(size_t q) {
+  queue_after_exterior();
+  for (size_t di = 0; di < domains_.size(); ++di) {
+    LocalDomain &d = domains_[di];
+    d.set_device();
+    const cudaPitchedPtr p = d.curr_data(q);
+    CUDA_RUNTIME(cudaMemsetAsync(p.ptr, 0, p.pitch * p.ysize * size_t(d.raw_size().z), applyStreams_[2 * di]));
+  }
+}
+
 void DistributedDomain::queue_exchange() {
   ensure_queue_events();
   for (size_t i = 0; i < applyStreams_.size(); ++i) {
@@ -1307,8 +1317,10 @@ void DistributedDomain::krylov_launch(KrylovCache &c, double s, double t, bool q
   }
 }
 
-std::vector<double> DistributedDomain::krylov_sums(KrylovCache &c, bool queued) {
-  const size_t n = size_t(c.nparts), rec = sizeof(int64_t) + n * sizeof(sb_reduce_exact_part);
+std::vector<double> DistributedDomain::krylov_sums(const std::vector<KrylovCache *> &cs, bool queued) {
+  size_t n = 0;
+  for (const KrylovCache *c : cs) n += size_t(c->nparts);
+  const size_t rec = sizeof(int64_t) + n * sizeof(sb_reduce_exact_part);
   const Dim3 dim = placement_->dim();
   std::vector<unsigned char> mine(domains_.size() * rec);
   for (size_t di = 0; di < domains_.size(); ++di) {
@@ -1317,7 +1329,12 @@ std::vector<double> DistributedDomain::krylov_sums(KrylovCache &c, bool queued) 
     const int64_t lin = idx.x + dim.x * (idx.y + dim.y * idx.z);
     std::memcpy(&mine[di * rec], &lin, sizeof(lin));
     const cudaStream_t st = queued ? applyStreams_[2 * di] : cudaStream_t(streams_[di]);
-    CUDA_RUNTIME(cudaMemcpyAsync(&mine[di * rec + sizeof(int64_t)], c.out[di], n * sizeof(sb_reduce_exact_part), cudaMemcpyDeviceToHost, st));
+    size_t at = di * rec + sizeof(int64_t);
+    for (const KrylovCache *c : cs) { // each cache's parts after the previous one's
+      const size_t bytes = size_t(c->nparts) * sizeof(sb_reduce_exact_part);
+      CUDA_RUNTIME(cudaMemcpyAsync(&mine[at], c->out[di], bytes, cudaMemcpyDeviceToHost, st));
+      at += bytes;
+    }
   }
   for (size_t di = 0; di < domains_.size(); ++di) {
     domains_[di].set_device();

@@ -20,13 +20,13 @@ from typing import Callable, List, Optional, Sequence
 import numpy as np
 
 from . import _lib
-from .domain import FACES, BC, BCKind, Boundary, DataHandle, DistributedDomain
-from .krylov import homogeneous_bc
-from .multigrid import Multigrid, _Clear, residual_op
+from .domain import DataHandle, DistributedDomain
+from .krylov import _KrylovSolver
+from .multigrid import Multigrid
 from .stencil_op import StencilOp
 
 
-class BiCGStab:
+class BiCGStab(_KrylovSolver):
     """Right-preconditioned BiCGStab for A x = f on the realized domain dd.  x, f, r, r0, p, v, phat, shat and t are nine
     distinct float32 or float64 quantities of dd (curr buffers): x the solution (its initial value is the first guess),
     f the right-hand side, r the residual (s from the half step on), r0 the shadow residual, p the direction, v = A phat,
@@ -41,100 +41,22 @@ class BiCGStab:
     def __init__(self, dd: DistributedDomain, x: DataHandle, f: DataHandle, r: DataHandle, r0: DataHandle, p: DataHandle, v: DataHandle,
                  phat: DataHandle, shat: DataHandle, t: DataHandle, op_at: Callable[[int], StencilOp], coefs: Optional[Sequence[DataHandle]] = None,
                  coef_kinds: Optional[Sequence[str]] = None, nu1: int = 2, nu2: int = 2, coarse_sweeps: int = 30, levels: Optional[int] = None):
-        self.mg: Optional[Multigrid] = None
-        self.breakdown: Optional[int] = None
-        if not isinstance(dd, DistributedDomain) or dd.partition_ is None or not dd._plans:
-            raise _lib.StencilError("BiCGStab: dd must be a realized DistributedDomain")
-        named = list(zip(self.NAMES, (x, f, r, r0, p, v, phat, shat, t)))
-        for name, h in named:
-            if not isinstance(h, DataHandle) or not 0 <= h.id < len(dd.dtypes_):
-                raise _lib.StencilError(f"BiCGStab: {name} must be a DataHandle of dd, not {h!r}")
-        if len({h.id for _, h in named}) != len(named):
-            raise _lib.StencilError(f"BiCGStab: {', '.join(self.NAMES)} must be 9 different quantities")
-        dtype = dd.dtypes_[x.id]
-        if dtype not in (np.dtype(np.float32), np.dtype(np.float64)) or any(dd.dtypes_[h.id] != dtype for _, h in named):
-            raise _lib.StencilError(f"BiCGStab: {', '.join(self.NAMES)} must all be float32 or all float64")
-        coefs = list(coefs) if coefs is not None else []
-        for k, h in enumerate(coefs):
-            if not isinstance(h, DataHandle) or not 0 <= h.id < len(dd.dtypes_):
-                raise _lib.StencilError(f"BiCGStab: coefficient {k} must be a DataHandle of dd, not {h!r}")
-            if any(h.id == g.id for _, g in named) or dd.dtypes_[h.id] != dtype:
-                raise _lib.StencilError(f"BiCGStab: coefficient {k} must be a quantity of x's type other than the nine vectors")
-        # phat and shat are what A is applied to: the homogeneous counterpart of x's BC on every FIXED face
-        for fc in range(6):
-            if dd.boundary_[fc // 2] != Boundary.FIXED:
-                continue
-            bx = dd.bcs_.get((x.id, fc), BC.NONE())
-            if bx.kind == BCKind.NONE:
-                raise _lib.StencilError(f"BiCGStab: x needs a boundary condition (ODD, EVEN or VALUE) on every FIXED face (face {FACES[fc]})")
-            want = homogeneous_bc(bx)
-            for name, h in (("phat", phat), ("shat", shat)):
-                got = dd.bcs_.get((h.id, fc), BC.NONE())
-                if got != want:
-                    raise _lib.StencilError(f"BiCGStab: {name} needs {want!r} on face {FACES[fc]}, the homogeneous counterpart of x's {bx!r}, not {got!r}")
-        A = op_at(0)
-        if not isinstance(A, StencilOp) or A.dtype != dtype:
-            raise _lib.StencilError(f"BiCGStab: op_at(0) must be a StencilOp in {dtype}, not {A!r}")
-        if A.has_aux:
-            raise _lib.StencilError("BiCGStab: op_at(0) has an aux term; A reads x only")
-        if A.ncoef != len(coefs):
-            raise _lib.StencilError(f"BiCGStab: op_at(0) reads {A.ncoef} coefficient fields, but {len(coefs)} were given")
-        A.check(dd.radius_)
-        self.dd = dd
-        self.x, self.f, self.r, self.r0, self.p, self.v, self.phat, self.shat, self.t = x, f, r, r0, p, v, phat, shat, t
-        self.A, self.res = A, residual_op(A)
-        self.coefs = coefs or None
-        self.mg = Multigrid(dd, phat, p, v, op_at, nu1=nu1, nu2=nu2, coarse_sweeps=coarse_sweeps, levels=levels, coefs=coefs or None,
+        super().__init__("BiCGStab", dd, dict(zip(self.NAMES, (x, f, r, r0, p, v, phat, shat, t))), ("phat", "shat"), op_at, coefs)
+        self.r0, self.p, self.v, self.phat, self.shat, self.t = r0, p, v, phat, shat, t
+        self.mg = Multigrid(dd, phat, p, v, op_at, nu1=nu1, nu2=nu2, coarse_sweeps=coarse_sweeps, levels=levels, coefs=self.coefs,
                             coef_kinds=coef_kinds)
         try:
             self.mg._fine_level(shat, r)  # the second pair's checks, now rather than at the first solve
         except Exception:
             self.close()
             raise
-        if not dd._apply_streams:
-            import torch
-
-            dd._apply_streams = [(torch.cuda.Stream(device=d.gpu()), torch.cuda.Stream(device=d.gpu())) for d in dd.domains_]
         # <t, r> and <t, t> by one two-pair DOT in FP64; in FP32 by two one-pair DOTs, the faster form there (section
         # 2.13).  The sums are exact either way, so the choice changes no bit.
-        self._split_tr_tt = dtype == np.dtype(np.float32)
-
-    # -- the queued schedule
-    def _plans(self, mode: int, *handles: DataHandle):
-        return self.dd.krylov_plans(mode, handles)
-
-    def _queue(self, plans, s: float = 0.0, t: float = 0.0) -> None:
-        for pl in plans:
-            pl.s, pl.t = float(s), float(t)
-        self.dd._run_plans([(pl,) for pl in plans], False, queued=True)
-
-    def _combine(self, *launched) -> List[float]:
-        """Host wait: the parts of the last launch of each plan list in launched, gathered across ranks in one exchange,
-        combined and rounded once (PCG._combine)."""
-        dd = self.dd
-        mine = []
-        for di, (idx, (si, _)) in enumerate(zip(dd.domain_idx_, dd._apply_streams)):
-            mine.append((idx, [part for plans in launched for part in plans[di].parts(si)]))
-        return [red.sum for red in dd._exact_gather(mine, sum(plans[0].n for plans in launched))]
-
-    def _apply_A(self, out: DataHandle, src: DataHandle) -> None:
-        self.dd._run_plans(*self.dd._apply_plans(self.A, (out, "curr"), src, None, True, self.coefs), queued=True)
-
-    def _precondition(self, u: DataHandle, f: DataHandle) -> None:
-        """u = M f: u set to +0, then one cycle on the pair (u, f), queued."""
-        dd = self.dd
-        dd._run_plans([(_Clear(d, u.id),) for d in dd.domains_], False, queued=True)
-        self.mg.cycle(wait=False, u=u, f=f)
+        self._split_tr_tt = dd.dtypes_[x.id] == np.dtype(np.float32)
 
     def _start(self) -> float:
         """r = f - A x with x's own BC through the exchange, r0 = r; returns rho = <r0, r> (= <r, r>)."""
-        import torch
-
-        dd = self.dd
-        for d, (si, se) in zip(dd.domains_, dd._apply_streams):
-            si.wait_stream(torch.cuda.current_stream(d.gpu()))
-            se.wait_stream(torch.cuda.current_stream(d.gpu()))
-        dd._run_plans(*dd._apply_plans(self.res, (self.r, "curr"), self.x, (self.f, "curr"), True, self.coefs), queued=True)
+        self._residual()
         self._queue(self._plans(_lib.KRYLOV_XPBY, self.r0, self.r), 0.0)
         rr = self._plans(_lib.KRYLOV_DOT, self.r0, self.r)
         self._queue(rr)
@@ -206,20 +128,3 @@ class BiCGStab:
                 break
             k += 1
         return hist
-
-    def residual_norm(self) -> float:
-        """The true ||f - A x||_2 over dd's compute region (the residual into r, then an exact dot)."""
-        self.dd.apply(self.res, (self.r, "curr"), self.x, (self.f, "curr"), coefs=self.coefs)
-        return math.sqrt(self.dd.dot(self.r, self.r))
-
-    def update_coefficients(self) -> None:
-        """Re-coarsen the preconditioner's coefficient fields after they change (Multigrid.update_coefficients); A on
-        the fine level reads the fields directly."""
-        if self.mg is not None:
-            self.mg.update_coefficients()
-
-    def close(self) -> None:
-        """Release the preconditioner's coarse domains (the Krylov plans stay in dd's cache until dd.close())."""
-        if self.mg is not None:
-            self.mg.close()
-            self.mg = None

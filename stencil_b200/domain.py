@@ -618,6 +618,18 @@ class KrylovPlan:
             pass
 
 
+class _Clear:
+    """A one-launch plan that sets a quantity's whole curr allocation to +0 (ghost cells included; an exchange refills
+    them before any read)."""
+
+    def __init__(self, d, q: int):
+        raw = d.raw_size()
+        self.gpu, self.ptr, self.nbytes = d.gpu(), d.curr_[q], raw[0] * raw[1] * raw[2] * d.elem_size(q)
+
+    def launch(self, stream=None) -> None:
+        check(lib().sb_memset(C.c_void_p(self.ptr), 0, self.nbytes, self.gpu, stream_ptr(stream)))
+
+
 # ------------------------------------------------------------------------------------------ LocalDomain
 class LocalDomain:
     """One subdomain on one GPU: curr/next allocation per quantity (local_domain.cuh:34-276,
@@ -1591,16 +1603,11 @@ class DistributedDomain:
         """The schedule of apply and apply_system: with exchange, every interior plan on its own stream while exchange()
         fills the ghost cells, then every exterior plan; without, the one plan per domain.  Returns when all are done.
         queued: the same launches, ordered by events only, and returns at once (_queue_plans)."""
-        import torch
-
-        if not self._apply_streams:
-            self._apply_streams = [(torch.cuda.Stream(device=d.gpu()), torch.cuda.Stream(device=d.gpu())) for d in self.domains_]
+        self._ensure_apply_streams()
         if queued:
             self._queue_plans(plans, exchange)
             return
-        for d, (si, se) in zip(self.domains_, self._apply_streams):  # after the work queued on the caller's stream
-            si.wait_stream(torch.cuda.current_stream(d.gpu()))
-            se.wait_stream(torch.cuda.current_stream(d.gpu()))
+        self._follow_caller()
         multi = len({d.gpu() for d in self.domains_}) > 1
         if exchange:
             for d, p, (si, _) in zip(self.domains_, plans, self._apply_streams):
@@ -1622,6 +1629,25 @@ class DistributedDomain:
             se.synchronize()
 
     # -- the queued schedule (the multigrid solver's): nothing waits on the host, CUDA events order the launches
+    def _ensure_apply_streams(self) -> None:
+        """Two apply streams per local domain (interior, exterior), made on first use."""
+        if not self._apply_streams:
+            import torch
+
+            self._apply_streams = [(torch.cuda.Stream(device=d.gpu()), torch.cuda.Stream(device=d.gpu())) for d in self.domains_]
+
+    def _follow_caller(self) -> None:
+        """Every apply stream waits for the work queued so far on the caller's current stream of its device."""
+        import torch
+
+        for d, (si, se) in zip(self.domains_, self._apply_streams):
+            si.wait_stream(torch.cuda.current_stream(d.gpu()))
+            se.wait_stream(torch.cuda.current_stream(d.gpu()))
+
+    def _queue_clear(self, h: DataHandle) -> None:
+        """h's whole curr allocation set to +0, queued on the interior apply streams after the previous exterior."""
+        self._run_plans([(_Clear(d, h.id),) for d in self.domains_], False, queued=True)
+
     def _queue_plans(self, plans, exchange: bool) -> None:
         """_run_plans without a host wait.  Each interior (or the one plan without exchange) waits for the previous
         exterior on its subdomain's apply streams; with exchange, the exchange waits for every apply stream as they were

@@ -19,13 +19,11 @@ diagonal relaxation (DistributedDomain.relax) instead of A.relax(1):
     mg.update_coefficients()               # every coarse level re-coarsened from kx, ky, kz"""
 from __future__ import annotations
 
-import ctypes as C
 from typing import Callable, List, Optional, Sequence
 
 import numpy as np
 
 from . import _lib
-from ._lib import check, lib, stream_ptr
 from .domain import FACES, BC, BCKind, Boundary, DataHandle, DistributedDomain, Partition, PlacementStrategy, Radius
 from .stencil_op import StencilOp
 
@@ -59,18 +57,6 @@ def level_count(sizes, levels: Optional[int] = None) -> int:
         cur = [tuple(v // 2 for v in s) for s in cur]
         n += 1
     return n
-
-
-class _Clear:
-    """A one-launch plan that sets a quantity's whole curr allocation to +0 (ghost cells included; an exchange refills
-    them before any read)."""
-
-    def __init__(self, d, q: int):
-        raw = d.raw_size()
-        self.gpu, self.ptr, self.nbytes = d.gpu(), d.curr_[q], raw[0] * raw[1] * raw[2] * d.elem_size(q)
-
-    def launch(self, stream=None) -> None:
-        check(lib().sb_memset(C.c_void_p(self.ptr), 0, self.nbytes, self.gpu, stream_ptr(stream)))
 
 
 class _Level:
@@ -191,10 +177,7 @@ class Multigrid:
         self.r = r
         self.coef_kinds = coef_kinds
         # every level queues on dd's apply streams, so stream order alone orders the work of consecutive levels
-        if not dd._apply_streams:
-            import torch
-
-            dd._apply_streams = [(torch.cuda.Stream(device=d.gpu()), torch.cuda.Stream(device=d.gpu())) for d in dd.domains_]
+        dd._ensure_apply_streams()
         size = dd.size()
         try:
             for l in range(1, nlev):
@@ -238,12 +221,7 @@ class Multigrid:
         face restriction, cell fields by the 8-cell restriction.  Queued like a cycle, after the work on the caller's
         stream, with one host wait (none with wait=False).  The constructor calls it once; call it again whenever the
         fine fields change.  The coarse ghost cells are filled by the exchanges of the next cycle."""
-        import torch
-
-        dd = self.levels[0].dd
-        for d, (si, se) in zip(dd.domains_, dd._apply_streams):
-            si.wait_stream(torch.cuda.current_stream(d.gpu()))
-            se.wait_stream(torch.cuda.current_stream(d.gpu()))
+        self.levels[0].dd._follow_caller()
         for F, Cl in zip(self.levels[:-1], self.levels[1:]):
             for kf, kc, kind in zip(F.coefs, Cl.coefs, self.coef_kinds):
                 F.dd._transfer(Cl.dd, _lib.TRANSFER_RESTRICT, (kc, "curr"), (kf, "curr"), None, False, queued=True, face=COEF_KINDS[kind])
@@ -259,7 +237,7 @@ class Multigrid:
         Cl = self.levels[l + 1]
         L.dd._transfer(Cl.dd, _lib.TRANSFER_RESTRICT, (Cl.f, "curr"), (L.u, "curr"), (L.f, "curr"), True, op=L.res, queued=True,
                        coefs=L.coefs if L.res.has_coef else None)
-        Cl.dd._run_plans([(_Clear(d, Cl.u.id),) for d in Cl.dd.domains_], False, queued=True)
+        Cl.dd._queue_clear(Cl.u)
         self._vcycle(l + 1)
         L.dd._transfer(Cl.dd, _lib.TRANSFER_PROLONG, (L.u, "curr"), (Cl.u, "curr"), (L.u, "curr"), True, queued=True)
         self._smooth(L, self.nu2)
@@ -304,15 +282,10 @@ class Multigrid:
         levels and coarse coefficient fields: u and f are two different quantities of dd of the constructor u's type,
         not coefficient fields, and u carries the constructor u's BC on every FIXED face (the coarse walls derive from
         it).  The cycle is then the bits of one on a Multigrid built on (u, f).  Give both or neither."""
-        import torch
-
         if (u is None) != (f is None):
             raise _lib.StencilError("Multigrid.cycle: give both u and f, or neither")
         L = self._fine_level(u, f)
-        dd = self.levels[0].dd
-        for d, (si, se) in zip(dd.domains_, dd._apply_streams):
-            si.wait_stream(torch.cuda.current_stream(d.gpu()))
-            se.wait_stream(torch.cuda.current_stream(d.gpu()))
+        self.levels[0].dd._follow_caller()
         self._vcycle(0, L)
         if wait:
             self.wait()
