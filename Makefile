@@ -36,7 +36,7 @@ LIBMPI    := lib/libmpi_shim.a
 all: $(SO) $(LIBA) $(LIBMPI) bin/sb_mpirun bin/jacobi3d_b200 bin/test_exchange_multigpu bin/test_boundary_multigpu \
           bin/test_reduce_multigpu bin/test_stencil_multigpu bin/test_vstencil_multigpu bin/test_system_multigpu \
           bin/test_reduce_exact_multigpu bin/test_colour_multigpu bin/test_mg_multigpu bin/test_multigrid_multigpu bin/test_vmultigrid_multigpu \
-          bin/test_krylov_multigpu bin/test_bicgstab_multigpu
+          bin/test_krylov_multigpu bin/test_bicgstab_multigpu bin/test_solver_parity
 
 build/mpi_shim.o: src/mpi_shim.cpp include/mpi_shim/mpi.h
 	@mkdir -p build
@@ -192,6 +192,12 @@ build/drv/test_bicgstab_multigpu.o: tests/cpp/test_bicgstab_multigpu.cu $(wildca
 	@mkdir -p $(dir $@)
 	$(NVCC) $(OWNDRVFLAGS) -c $< -o $@
 bin/test_bicgstab_multigpu: build/drv/test_bicgstab_multigpu.o $(LIBA) $(LIBMPI)
+	@mkdir -p bin
+	$(NVCC) $(DRVLINK) -o $@ $< $(LIBA) $(LIBMPI)
+build/drv/test_solver_parity.o: tests/cpp/test_solver_parity.cu $(wildcard include/stencil/*) include/stencil_b200.h
+	@mkdir -p $(dir $@)
+	$(NVCC) $(OWNDRVFLAGS) -c $< -o $@
+bin/test_solver_parity: build/drv/test_solver_parity.o $(LIBA) $(LIBMPI)
 	@mkdir -p bin
 	$(NVCC) $(DRVLINK) -o $@ $< $(LIBA) $(LIBMPI)
 build/drv/test_system_multigpu.o: tests/cpp/test_system_multigpu.cu $(wildcard include/stencil/*) include/stencil_b200.h
