@@ -3,14 +3,16 @@
 #include "stencil_b200.h"
 
 #include <algorithm>
-#include <array>
 #include <atomic>
 #include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
+#include <memory>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include <cuda_runtime.h>
@@ -64,6 +66,45 @@ struct DeviceGuard {
     if (prev >= 0) cudaSetDevice(prev);
   }
 };
+
+// A cudaMalloc block of a plan (a table uploaded at creation, or scratch), freed on its device with the plan.
+template <class T> struct DeviceTable {
+  int device = 0;
+  T *ptr = nullptr;
+  DeviceTable() = default;
+  DeviceTable(const DeviceTable &) = delete;
+  DeviceTable &operator=(const DeviceTable &) = delete;
+  ~DeviceTable() {
+    if (!ptr) return;
+    DeviceGuard guard(device);
+    cudaFree(ptr);
+  }
+  // n elements on dev, the current device, the first host.size() of them copied from host
+  cudaError_t upload(int dev, const std::vector<T> &host, size_t n) {
+    device = dev;
+    cudaError_t e = cudaMalloc(&ptr, n * sizeof(T));
+    if (e == cudaSuccess && !host.empty()) e = cudaMemcpy(ptr, host.data(), host.size() * sizeof(T), cudaMemcpyHostToDevice);
+    return e;
+  }
+};
+
+// The kernel launches of a stencil or transfer plan, in order: each holds its parameters by value and returns the
+// number of launches it issued (the launch_* functions of the kernel headers).
+struct LaunchList {
+  int device = 0;
+  int64_t bytes = 0;
+  std::vector<std::function<int(cudaStream_t)>> launches;
+};
+
+int run_launches(const LaunchList *p, void *stream) {
+  if (!p) return fail(SB_ERR_INVALID, "null plan");
+  if (p->launches.empty()) return SB_OK;
+  DeviceGuard guard(p->device);
+  if (!guard.ok) return fail(SB_ERR_NOGPU, "cannot select CUDA device %d", p->device);
+  for (const auto &launch : p->launches) g_launches += uint64_t(launch(static_cast<cudaStream_t>(stream)));
+  SB_CUDA(cudaGetLastError());
+  return SB_OK;
+}
 
 // The compute entry points take pointers and a stream but no device: the launch must happen on the device that owns the
 // memory (and the stream), whatever the calling thread's current device is -- a caller that drives several GPUs (or a test
@@ -307,91 +348,120 @@ int exchange_messages(const int64_t dim[3], const int64_t base[3], const int64_t
   return SB_OK;
 }
 
+// ------------------------------------------------------------------------------------------- boxes of a plan
+// The non-empty boxes of an operator, system or fused-restriction plan: lo in the destination's allocation coordinates,
+// and the extent.  Thick boxes go to the tile kernel, one launch each; thin ones to the cell kernel in groups.
+struct PlanBox {
+  int lo[3], ext[3];
+};
+struct PlanBoxes {
+  std::vector<PlanBox> thick, thin; // in box order
+  int64_t cells = 0;
+};
+
+// Checks and sorts the nbox boxes [lo, hi) (global coordinates, 3 per box) of a destination whose allocation starts at
+// acc_origin: a box is thick when its extent is at least `thick` on every axis.  reads(b, l, e) checks what box b reads
+// (allocation-relative lo l, extent e) and returns SB_OK or its error.
+template <class Reads>
+int plan_boxes(int nbox, const int64_t *lo, const int64_t *hi, const int64_t acc_origin[3], int thick, Reads reads, PlanBoxes &out) {
+  for (int b = 0; b < nbox; ++b) {
+    int64_t l[3], e[3];
+    bool empty = false;
+    for (int a = 0; a < 3; ++a) {
+      if (lo[3 * b + a] > hi[3 * b + a]) return fail(SB_ERR_INVALID, "box %d: lo > hi on axis %c", b, "xyz"[a]);
+      l[a] = lo[3 * b + a] - acc_origin[a];
+      e[a] = hi[3 * b + a] - lo[3 * b + a];
+      empty = empty || e[a] == 0;
+    }
+    if (empty) continue;
+    const int rc = reads(b, l, e);
+    if (rc != SB_OK) return rc;
+    if (e[0] * e[1] * e[2] >= (1ll << 32)) return fail(SB_ERR_INVALID, "box %d: more than 2^32 cells", b);
+    const PlanBox box = {{int(l[0]), int(l[1]), int(l[2])}, {int(e[0]), int(e[1]), int(e[2])}};
+    (e[0] >= thick && e[1] >= thick && e[2] >= thick ? out.thick : out.thin).push_back(box);
+    out.cells += e[0] * e[1] * e[2];
+  }
+  return SB_OK;
+}
+
+// The tile grid of a z-marching kernel (kernel: its name in the message) over a box of extent ext, in columns of tx x ty
+// cells: z chunks for at least two waves of per_sm resident CTAs per SM, no shorter than min_chunk planes (each chunk
+// reloads the planes around it).  Sets p.tiles_x, p.tiles_y and p.zchunk.
+template <class P> int tile_grid(P &p, const int ext[3], int tx, int ty, int sms, int per_sm, int min_chunk, const char *kernel, int &grid) {
+  p.tiles_x = (ext[0] + tx - 1) / tx;
+  p.tiles_y = (ext[1] + ty - 1) / ty;
+  const long long cols = (long long)p.tiles_x * p.tiles_y;
+  const long long want = (2ll * sms * per_sm + cols - 1) / cols;
+  p.zchunk = std::max(int((ext[2] + want - 1) / want), std::min(min_chunk, ext[2]));
+  const long long g = cols * ((ext[2] + p.zchunk - 1) / p.zchunk);
+  if (g >= (1ll << 31)) return fail(SB_ERR_INVALID, "box too large for the %s", kernel);
+  grid = int(g);
+  return SB_OK;
+}
+
+// The thin boxes in groups of as many as a cell kernel's parameters hold: each group is p with its boxes in lo / ext, its
+// box count in p.*count and the prefix sums of their cells in first.  add(group, grid) takes each group in order; the
+// grid has one thread per cell, at most 32 CTAs of 256 per SM.
+template <class P, class Q, class Add> void cell_groups(const std::vector<PlanBox> &thin, const P &p, int Q::*count, int sms, Add add) {
+  constexpr size_t kMax = std::extent<decltype(P::first)>::value - 1;
+  for (size_t b0 = 0; b0 < thin.size(); b0 += kMax) {
+    P g = p;
+    g.first[0] = 0;
+    for (size_t b = b0; b < thin.size() && b < b0 + kMax; ++b) {
+      const int m = (g.*count)++;
+      for (int a = 0; a < 3; ++a) {
+        g.lo[m][a] = thin[b].lo[a];
+        g.ext[m][a] = thin[b].ext[a];
+      }
+      g.first[m + 1] = g.first[m] + (long long)thin[b].ext[0] * thin[b].ext[1] * thin[b].ext[2];
+    }
+    add(g, int(std::min<long long>((g.first[g.*count] + 255) / 256, 32ll * sms)));
+  }
+}
+
 } // namespace
 
 struct sb_bc_plan {
   int device = 0;
-  sb::BcSeg *segs_dev = nullptr;
-  sb::BcTile *tiles_dev = nullptr;
+  DeviceTable<sb::BcSeg> segs;
+  DeviceTable<sb::BcTile> tiles;
   unsigned ntiles = 0;
   int grid = 0;
   int64_t bytes = 0;
 };
 
-struct sb_reduce_plan {
+// An ordered or exact reduction plan: Partial is the kernel's per-tile partial.
+template <class Partial> struct ReducePlan {
   int device = 0;
-  sb::RedItem *items_dev = nullptr;
-  sb::RedTile *tiles_dev = nullptr;
-  sb::RedPartial *scratch = nullptr; // one partial per tile, rewritten by every launch
-  unsigned nitems = 0, ntiles = 0;
+  DeviceTable<sb::RedItem> items;
+  DeviceTable<sb::RedTile> tiles;
+  DeviceTable<Partial> scratch; // one partial per tile, rewritten by every launch
+  unsigned nitems = 0;
   unsigned class_tiles[sb::kRedClasses][2] = {}; // tiles [begin, end) of each class
   int grids[sb::kRedClasses] = {};
   int64_t bytes = 0;
 };
-
-struct sb_reduce_exact_plan {
-  int device = 0;
-  sb::RedItem *items_dev = nullptr;
-  sb::RedTile *tiles_dev = nullptr;
-  sb::RedExactPartial *scratch = nullptr; // one partial per tile, rewritten by every launch
-  unsigned nitems = 0, ntiles = 0;
-  unsigned class_tiles[sb::kRedClasses][2] = {};
-  int grids[sb::kRedClasses] = {};
-  int64_t bytes = 0;
-};
+struct sb_reduce_plan : ReducePlan<sb::RedPartial> {};
+struct sb_reduce_exact_plan : ReducePlan<sb::RedExactPartial> {};
 
 struct sb_krylov_plan {
   int device = 0;
   int dtype = SB_DTYPE_F64, mode = 0; // mode: the kernel mode (krylov.cuh)
   bool wide = false;
   sb::KryParams params{};
-  sb::KryPartial *scratch = nullptr; // one partial per tile, rewritten by every launch (modes with dots)
+  DeviceTable<sb::KryPartial> scratch; // one partial per tile, rewritten by every launch (modes with dots)
   int grid = 0, copy_grid = 0;
   int64_t bytes = 0;
 };
 
-struct sb_stencil_plan {
-  int device = 0;
-  int es = 8, R = 1;
-  bool has_coef = false;                // some term reads a coefficient field: the HAS_COEF kernels
-  std::vector<sb::OpDTileParams> tiles; // one tile-kernel launch per thick box
-  std::vector<int> tile_grids;
-  std::vector<sb::OpDCellParams> cells; // one cell-kernel launch per group of thin boxes
-  std::vector<int> cell_grids;
-  std::vector<sb::SysTileParams> sys_tiles; // a system (sb_stencil_sys_plan_create): one tile launch per thick box
-  std::vector<int> sys_tile_grids;
-  size_t sys_smem = 0;
-  std::vector<sb::SysCellParams> sys_cells;
-  std::vector<int> sys_cell_grids;
-  int64_t bytes = 0;
-};
-
-struct sb_transfer_plan {
-  int device = 0;
-  int es = 8, kind = SB_TRANSFER_RESTRICT;
-  int launches = 0; // 0: an empty box
-  sb::RestrictParams r{};
-  sb::ProlongParams pr{};
-  int grid = 0; // prolongation CTAs
-  bool fused = false; // sb_transfer_oplan_create: the launches below instead
-  std::vector<sb::RopTileParams> rop_tiles; // one tile-kernel launch per thick box
-  std::vector<int> rop_tile_grids;
-  std::vector<sb::RopCellParams> rop_cells; // one cell-kernel launch per group of thin boxes
-  std::vector<int> rop_cell_grids;
-  std::vector<sb::RopVTileParams> rop_vtiles; // sb_transfer_voplan_create: the same launches with coefficient fields
-  std::vector<int> rop_vtile_grids;
-  std::vector<sb::RopVCellParams> rop_vcells;
-  std::vector<int> rop_vcell_grids;
-  int face = -1; // sb_transfer_fplan_create: the face axis of the restriction r
-  int64_t bytes = 0;
-};
+struct sb_stencil_plan : LaunchList {};  // an operator or a system: tile launches in box order, then the cell groups
+struct sb_transfer_plan : LaunchList {}; // no launch for an empty box
 
 struct sb_copy_plan {
   int device = 0;
-  sb::Seg *segs_dev = nullptr;
-  sb::Tile *tiles_dev = nullptr;
+  DeviceTable<sb::Seg> segs;
+  DeviceTable<sb::Tile> tiles;
   unsigned ntiles = 0;
-  unsigned nsegs = 0;
   int grid = 0;
   int64_t bytes = 0;
 };
@@ -535,22 +605,19 @@ int sb_copy_plan_create(sb_copy_plan **out, int device, const sb_box_copy *copie
   DeviceGuard guard(device);
   if (!guard.ok) return fail(SB_ERR_NOGPU, "cannot select CUDA device %d", device);
   sb::preload_box_copy_kernels();
-  sb_copy_plan *p = new sb_copy_plan();
+  std::unique_ptr<sb_copy_plan> p(new sb_copy_plan());
   p->device = device;
   p->bytes = bytes;
-  p->nsegs = unsigned(segs.size());
   p->ntiles = unsigned(tiles.size());
   if (p->ntiles) {
-    SB_CUDA(cudaMalloc(&p->segs_dev, (segs.size() + 1) * sizeof(sb::Seg)));
-    SB_CUDA(cudaMalloc(&p->tiles_dev, tiles.size() * sizeof(sb::Tile)));
-    SB_CUDA(cudaMemcpy(p->segs_dev, segs.data(), segs.size() * sizeof(sb::Seg), cudaMemcpyHostToDevice));
-    SB_CUDA(cudaMemcpy(p->tiles_dev, tiles.data(), tiles.size() * sizeof(sb::Tile), cudaMemcpyHostToDevice));
+    SB_CUDA(p->segs.upload(device, segs, segs.size() + 1));
+    SB_CUDA(p->tiles.upload(device, tiles, tiles.size()));
     int sms = 132;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
     const long long cap = (long long)sms * sb::kCopyCtasPerSm;
     p->grid = int(p->ntiles < cap ? p->ntiles : cap);
   }
-  *out = p;
+  *out = p.release();
   return SB_OK;
 }
 
@@ -559,7 +626,7 @@ int sb_copy_plan_launch(sb_copy_plan *p, void *stream) {
   if (0 == p->ntiles) return SB_OK;
   DeviceGuard guard(p->device);
   if (!guard.ok) return fail(SB_ERR_NOGPU, "cannot select CUDA device %d", p->device);
-  sb::launch_box_copy(p->segs_dev, p->tiles_dev, p->ntiles, p->grid, static_cast<cudaStream_t>(stream));
+  sb::launch_box_copy(p->segs.ptr, p->tiles.ptr, p->ntiles, p->grid, static_cast<cudaStream_t>(stream));
   ++g_launches;
   SB_CUDA(cudaGetLastError());
   return SB_OK;
@@ -569,10 +636,6 @@ int64_t sb_copy_plan_bytes(const sb_copy_plan *p) { return p ? p->bytes : 0; }
 int64_t sb_copy_plan_num_tiles(const sb_copy_plan *p) { return p ? p->ntiles : 0; }
 
 int sb_copy_plan_destroy(sb_copy_plan *p) {
-  if (!p) return SB_OK;
-  DeviceGuard guard(p->device);
-  if (p->segs_dev) cudaFree(p->segs_dev);
-  if (p->tiles_dev) cudaFree(p->tiles_dev);
   delete p;
   return SB_OK;
 }
@@ -700,25 +763,20 @@ int sb_bc_plan_create(sb_bc_plan **out, int device, const sb_bc_quantity *quanti
   }
   DeviceGuard guard(device);
   if (!guard.ok) return fail(SB_ERR_NOGPU, "cannot select CUDA device %d", device);
-  sb_bc_plan *p = new sb_bc_plan();
+  std::unique_ptr<sb_bc_plan> p(new sb_bc_plan());
   p->device = device;
   p->bytes = bytes;
   p->ntiles = unsigned(tiles.size());
   if (p->ntiles) {
-    cudaError_t e = cudaMalloc(&p->segs_dev, segs.size() * sizeof(sb::BcSeg));
-    if (e == cudaSuccess) e = cudaMalloc(&p->tiles_dev, tiles.size() * sizeof(sb::BcTile));
-    if (e == cudaSuccess) e = cudaMemcpy(p->segs_dev, segs.data(), segs.size() * sizeof(sb::BcSeg), cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMemcpy(p->tiles_dev, tiles.data(), tiles.size() * sizeof(sb::BcTile), cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) {
-      sb_bc_plan_destroy(p);
-      return fail(SB_ERR_CUDA, "BC plan upload: %s", cudaGetErrorString(e));
-    }
+    cudaError_t e = p->segs.upload(device, segs, segs.size());
+    if (e == cudaSuccess) e = p->tiles.upload(device, tiles, tiles.size());
+    if (e != cudaSuccess) return fail(SB_ERR_CUDA, "BC plan upload: %s", cudaGetErrorString(e));
     int sms = 132;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
     const long long cap = (long long)sms * 8;
     p->grid = int(p->ntiles < cap ? p->ntiles : cap);
   }
-  *out = p;
+  *out = p.release();
   return SB_OK;
 }
 
@@ -727,7 +785,7 @@ int sb_bc_plan_launch(sb_bc_plan *p, void *stream) {
   if (0 == p->ntiles) return SB_OK;
   DeviceGuard guard(p->device);
   if (!guard.ok) return fail(SB_ERR_NOGPU, "cannot select CUDA device %d", p->device);
-  sb::launch_bc_fill(p->segs_dev, p->tiles_dev, p->ntiles, p->grid, static_cast<cudaStream_t>(stream));
+  sb::launch_bc_fill(p->segs.ptr, p->tiles.ptr, p->ntiles, p->grid, static_cast<cudaStream_t>(stream));
   ++g_launches;
   SB_CUDA(cudaGetLastError());
   return SB_OK;
@@ -736,10 +794,6 @@ int sb_bc_plan_launch(sb_bc_plan *p, void *stream) {
 int64_t sb_bc_plan_bytes(const sb_bc_plan *p) { return p ? p->bytes : 0; }
 
 int sb_bc_plan_destroy(sb_bc_plan *p) {
-  if (!p) return SB_OK;
-  DeviceGuard guard(p->device);
-  if (p->segs_dev) cudaFree(p->segs_dev);
-  if (p->tiles_dev) cudaFree(p->tiles_dev);
   delete p;
   return SB_OK;
 }
@@ -1000,6 +1054,20 @@ int sb_sqdiff(sb_pitched a, sb_pitched b, int dtype_size, const int64_t acc_orig
 
 // ----------------------------------------------------------------------------------------- reductions
 namespace {
+// Lanes per row (log2) and rows per tile of a reduction or Krylov pass over rows of nx es-byte cells, read 16 bytes at
+// a time where wide: functions of the box and the access width only.
+struct RowTiles {
+  int lg_group;
+  long long rows_per_tile;
+};
+RowTiles row_tiles(long long nx, int es, bool wide) {
+  const int lg = int(std::min(5u, ceil_log2(unsigned(std::max(1ll, (nx * es + 15) / 16)))));
+  const long long N = wide ? 16 / es : 1, G = 1ll << lg;
+  // longest chain of one lane over one row: its body vectors, one head and one tail cell
+  const long long per_row = N * (((nx / N) + G - 1) / G) + 2 * ((std::min(nx, N - 1) + G - 1) / G);
+  return {lg, std::max(1ll, sb::kRedChain / std::max(1ll, per_row)) * (sb::kRedThreads >> lg)};
+}
+
 // The checks, items and tile table of a reduction plan, ordered or exact (`fn` names the entry point in the messages).
 struct RedTables {
   std::vector<sb::RedItem> its;
@@ -1048,9 +1116,8 @@ int reduce_tables(const char *fn, bool out_ok, const sb_reduce_item *items, int6
     r.kind = I.kind;
     r.dtype = I.dtype;
     r.vec = wide ? 16 : es;
-    // lanes per row and tile rows: functions of the box and the access width only
     const long long nx = r.ext[0], rows = (long long)r.ext[1] * r.ext[2];
-    r.lg_group = int(std::min(5u, ceil_log2(unsigned(std::max(1ll, (nx * es + 15) / 16)))));
+    r.lg_group = row_tiles(nx, es, wide).lg_group;
     r.count = nx * rows;
     if (rows >= (1ll << 31)) return fail(SB_ERR_INVALID, "item %lld: more than 2^31 rows", li);
     its.push_back(r);
@@ -1065,11 +1132,8 @@ int reduce_tables(const char *fn, bool out_ok, const sb_reduce_item *items, int6
       if (sb::reduce_class(r) != c) continue;
       r.tile0 = unsigned(tiles.size());
       if (r.count > 0) {
-        const long long nx = r.ext[0], rows = (long long)r.ext[1] * r.ext[2];
-        const long long N = r.vec / (r.dtype == SB_DTYPE_F32 ? 4 : 8), G = 1ll << r.lg_group;
-        // longest chain of one lane over one row: its body vectors, one head and one tail cell
-        const long long per_row = N * (((nx / N) + G - 1) / G) + 2 * ((std::min(nx, N - 1) + G - 1) / G);
-        const long long rows_per_tile = std::max(1ll, sb::kRedChain / std::max(1ll, per_row)) * (sb::kRedThreads >> r.lg_group);
+        const long long rows = (long long)r.ext[1] * r.ext[2];
+        const long long rows_per_tile = row_tiles(r.ext[0], r.dtype == SB_DTYPE_F32 ? 4 : 8, r.vec == 16).rows_per_tile;
         for (long long r0 = 0; r0 < rows; r0 += rows_per_tile)
           tiles.push_back(sb::RedTile{unsigned(i), unsigned(r0), unsigned(std::min(rows_per_tile, rows - r0))});
         if (tiles.size() >= (1ull << 31)) return fail(SB_ERR_INVALID, "too many tiles");
@@ -1080,39 +1144,36 @@ int reduce_tables(const char *fn, bool out_ok, const sb_reduce_item *items, int6
   }
   return SB_OK;
 }
+
+// An ordered or exact reduction plan over the tables T, its per-class grids from grid (reduce_grid or
+// reduce_exact_grid).  The tile table and the scratch hold at least one element.
+extern "C++" template <class Plan> int reduce_plan_upload(Plan **out, int device, const RedTables &T, int (*grid)(int, int, unsigned)) {
+  DeviceGuard guard(device);
+  if (!guard.ok) return fail(SB_ERR_NOGPU, "cannot select CUDA device %d", device);
+  std::unique_ptr<Plan> p(new Plan());
+  p->device = device;
+  p->bytes = T.bytes;
+  p->nitems = unsigned(T.its.size());
+  const size_t ntiles = std::max<size_t>(1, T.tiles.size());
+  cudaError_t e = p->items.upload(device, T.its, T.its.size());
+  if (e == cudaSuccess) e = p->tiles.upload(device, T.tiles, ntiles);
+  if (e == cudaSuccess) e = p->scratch.upload(device, {}, ntiles);
+  if (e != cudaSuccess) return fail(SB_ERR_CUDA, "reduction plan upload: %s", cudaGetErrorString(e));
+  for (int c = 0; c < sb::kRedClasses; ++c) {
+    p->class_tiles[c][0] = T.class_tiles[c][0];
+    p->class_tiles[c][1] = T.class_tiles[c][1];
+    p->grids[c] = grid(device, c, T.class_tiles[c][1] - T.class_tiles[c][0]);
+  }
+  *out = p.release();
+  return SB_OK;
+}
 } // namespace
 
 int sb_reduce_plan_create(sb_reduce_plan **out, int device, const sb_reduce_item *items, int64_t n) {
   RedTables T;
   const int rc = reduce_tables("sb_reduce_plan_create", out != nullptr, items, n, T);
   if (rc != SB_OK) return rc;
-  const std::vector<sb::RedItem> &its = T.its;
-  const std::vector<sb::RedTile> &tiles = T.tiles;
-  const unsigned(&class_tiles)[sb::kRedClasses][2] = T.class_tiles;
-  const int64_t bytes = T.bytes;
-  DeviceGuard guard(device);
-  if (!guard.ok) return fail(SB_ERR_NOGPU, "cannot select CUDA device %d", device);
-  sb_reduce_plan *p = new sb_reduce_plan();
-  p->device = device;
-  p->bytes = bytes;
-  p->nitems = unsigned(its.size());
-  p->ntiles = unsigned(tiles.size());
-  cudaError_t e = cudaMalloc(&p->items_dev, its.size() * sizeof(sb::RedItem));
-  if (e == cudaSuccess) e = cudaMalloc(&p->tiles_dev, std::max<size_t>(1, tiles.size()) * sizeof(sb::RedTile));
-  if (e == cudaSuccess) e = cudaMalloc(&p->scratch, std::max<size_t>(1, tiles.size()) * sizeof(sb::RedPartial));
-  if (e == cudaSuccess) e = cudaMemcpy(p->items_dev, its.data(), its.size() * sizeof(sb::RedItem), cudaMemcpyHostToDevice);
-  if (e == cudaSuccess && !tiles.empty()) e = cudaMemcpy(p->tiles_dev, tiles.data(), tiles.size() * sizeof(sb::RedTile), cudaMemcpyHostToDevice);
-  if (e != cudaSuccess) {
-    sb_reduce_plan_destroy(p);
-    return fail(SB_ERR_CUDA, "reduction plan upload: %s", cudaGetErrorString(e));
-  }
-  for (int c = 0; c < sb::kRedClasses; ++c) {
-    p->class_tiles[c][0] = class_tiles[c][0];
-    p->class_tiles[c][1] = class_tiles[c][1];
-    p->grids[c] = sb::reduce_grid(device, c, class_tiles[c][1] - class_tiles[c][0]);
-  }
-  *out = p;
-  return SB_OK;
+  return reduce_plan_upload(out, device, T, sb::reduce_grid);
 }
 
 int sb_reduce_plan_launch(sb_reduce_plan *p, sb_reduce_result *out_dev, void *stream) {
@@ -1120,7 +1181,7 @@ int sb_reduce_plan_launch(sb_reduce_plan *p, sb_reduce_result *out_dev, void *st
   if (!out_dev) return fail(SB_ERR_INVALID, "null output buffer");
   DeviceGuard guard(p->device);
   if (!guard.ok) return fail(SB_ERR_NOGPU, "cannot select CUDA device %d", p->device);
-  g_launches += uint64_t(sb::launch_reduce(p->items_dev, p->nitems, p->tiles_dev, p->class_tiles, p->grids, p->scratch, out_dev,
+  g_launches += uint64_t(sb::launch_reduce(p->items.ptr, p->nitems, p->tiles.ptr, p->class_tiles, p->grids, p->scratch.ptr, out_dev,
                                            static_cast<cudaStream_t>(stream)));
   SB_CUDA(cudaGetLastError());
   return SB_OK;
@@ -1129,11 +1190,6 @@ int sb_reduce_plan_launch(sb_reduce_plan *p, sb_reduce_result *out_dev, void *st
 int64_t sb_reduce_plan_bytes(const sb_reduce_plan *p) { return p ? p->bytes : 0; }
 
 int sb_reduce_plan_destroy(sb_reduce_plan *p) {
-  if (!p) return SB_OK;
-  DeviceGuard guard(p->device);
-  if (p->items_dev) cudaFree(p->items_dev);
-  if (p->tiles_dev) cudaFree(p->tiles_dev);
-  if (p->scratch) cudaFree(p->scratch);
   delete p;
   return SB_OK;
 }
@@ -1155,30 +1211,7 @@ int sb_reduce_exact_plan_create(sb_reduce_exact_plan **out, int device, const sb
   // a tile then holds at most 2^30 cells, and the kernel's per-tile digit counters cannot overflow (reduce.cuh)
   for (size_t i = 0; i < T.its.size(); ++i)
     if (T.its[i].ext[0] > (1 << 27)) return fail(SB_ERR_INVALID, "item %lld: rows of more than 2^27 cells", (long long)i);
-  DeviceGuard guard(device);
-  if (!guard.ok) return fail(SB_ERR_NOGPU, "cannot select CUDA device %d", device);
-  sb_reduce_exact_plan *p = new sb_reduce_exact_plan();
-  p->device = device;
-  p->bytes = T.bytes;
-  p->nitems = unsigned(T.its.size());
-  p->ntiles = unsigned(T.tiles.size());
-  cudaError_t e = cudaMalloc(&p->items_dev, T.its.size() * sizeof(sb::RedItem));
-  if (e == cudaSuccess) e = cudaMalloc(&p->tiles_dev, std::max<size_t>(1, T.tiles.size()) * sizeof(sb::RedTile));
-  if (e == cudaSuccess) e = cudaMalloc(&p->scratch, std::max<size_t>(1, T.tiles.size()) * sizeof(sb::RedExactPartial));
-  if (e == cudaSuccess) e = cudaMemcpy(p->items_dev, T.its.data(), T.its.size() * sizeof(sb::RedItem), cudaMemcpyHostToDevice);
-  if (e == cudaSuccess && !T.tiles.empty())
-    e = cudaMemcpy(p->tiles_dev, T.tiles.data(), T.tiles.size() * sizeof(sb::RedTile), cudaMemcpyHostToDevice);
-  if (e != cudaSuccess) {
-    sb_reduce_exact_plan_destroy(p);
-    return fail(SB_ERR_CUDA, "reduction plan upload: %s", cudaGetErrorString(e));
-  }
-  for (int c = 0; c < sb::kRedClasses; ++c) {
-    p->class_tiles[c][0] = T.class_tiles[c][0];
-    p->class_tiles[c][1] = T.class_tiles[c][1];
-    p->grids[c] = sb::reduce_exact_grid(device, c, T.class_tiles[c][1] - T.class_tiles[c][0]);
-  }
-  *out = p;
-  return SB_OK;
+  return reduce_plan_upload(out, device, T, sb::reduce_exact_grid);
 }
 
 int sb_reduce_exact_plan_launch(sb_reduce_exact_plan *p, sb_reduce_exact_part *out_dev, void *stream) {
@@ -1186,7 +1219,7 @@ int sb_reduce_exact_plan_launch(sb_reduce_exact_plan *p, sb_reduce_exact_part *o
   if (!out_dev) return fail(SB_ERR_INVALID, "null output buffer");
   DeviceGuard guard(p->device);
   if (!guard.ok) return fail(SB_ERR_NOGPU, "cannot select CUDA device %d", p->device);
-  g_launches += uint64_t(sb::launch_reduce_exact(p->items_dev, p->nitems, p->tiles_dev, p->class_tiles, p->grids, p->scratch, out_dev,
+  g_launches += uint64_t(sb::launch_reduce_exact(p->items.ptr, p->nitems, p->tiles.ptr, p->class_tiles, p->grids, p->scratch.ptr, out_dev,
                                                  static_cast<cudaStream_t>(stream)));
   SB_CUDA(cudaGetLastError());
   return SB_OK;
@@ -1195,11 +1228,6 @@ int sb_reduce_exact_plan_launch(sb_reduce_exact_plan *p, sb_reduce_exact_part *o
 int64_t sb_reduce_exact_plan_bytes(const sb_reduce_exact_plan *p) { return p ? p->bytes : 0; }
 
 int sb_reduce_exact_plan_destroy(sb_reduce_exact_plan *p) {
-  if (!p) return SB_OK;
-  DeviceGuard guard(p->device);
-  if (p->items_dev) cudaFree(p->items_dev);
-  if (p->tiles_dev) cudaFree(p->tiles_dev);
-  if (p->scratch) cudaFree(p->scratch);
   delete p;
   return SB_OK;
 }
@@ -1353,15 +1381,12 @@ int sb_krylov_plan_create(sb_krylov_plan **out, int device, int mode, int dtype,
     kp.buf[k] = static_cast<char *>(bufs[k < nbuf ? k : 0].ptr) + off;
     wide = wide && ((uintptr_t(kp.buf[k]) - uintptr_t(kp.buf[0])) % 16 == 0);
   }
-  // lanes per row and tile rows as for the reductions: a function of the box and the access width only
   const long long nx = kp.ext[0], rows = (long long)kp.ext[1] * kp.ext[2];
-  kp.lg_group = int(std::min(5u, ceil_log2(unsigned(std::max(1ll, (nx * es + 15) / 16)))));
+  const RowTiles rt = row_tiles(nx, es, wide);
+  kp.lg_group = rt.lg_group;
   kp.count = nx * rows;
-  const long long N = wide ? 16 / es : 1, G = 1ll << kp.lg_group;
-  const long long per_row = N * (((nx / N) + G - 1) / G) + 2 * ((std::min(nx, N - 1) + G - 1) / G);
-  const long long rows_per_tile = std::max(1ll, sb::kRedChain / std::max(1ll, per_row)) * (sb::kRedThreads >> kp.lg_group);
-  kp.rows_per_tile = unsigned(rows_per_tile);
-  kp.ntiles = kp.count > 0 ? unsigned((rows + rows_per_tile - 1) / rows_per_tile) : 0u;
+  kp.rows_per_tile = unsigned(rt.rows_per_tile);
+  kp.ntiles = kp.count > 0 ? unsigned((rows + rt.rows_per_tile - 1) / rt.rows_per_tile) : 0u;
   int kmode = nbuf == 5 ? sb::kKryUpdateC : sb::kKryUpdate;
   if (mode == SB_KRYLOV_DOT) kmode = nbuf == 3 ? sb::kKryDot2 : sb::kKryDot1;
   if (mode == SB_KRYLOV_XPBY) kmode = sb::kKryXpby;
@@ -1376,24 +1401,20 @@ int sb_krylov_plan_create(sb_krylov_plan **out, int device, int mode, int dtype,
   const int nwrite = mode == SB_KRYLOV_XPBY || mode == SB_KRYLOV_BICG_P ? 1 : mode == SB_KRYLOV_UPDATE ? 2 : 0;
   DeviceGuard guard(device);
   if (!guard.ok) return fail(SB_ERR_NOGPU, "cannot select CUDA device %d", device);
-  sb_krylov_plan *p = new sb_krylov_plan();
+  std::unique_ptr<sb_krylov_plan> p(new sb_krylov_plan());
   p->device = device;
   p->dtype = dtype;
   p->mode = kmode;
   p->wide = wide;
   p->params = kp;
   p->bytes = kp.count * es * (nread + nwrite);
-  const int ndots = sb::kry_dots(kmode);
-  if (ndots > 0) {
-    const cudaError_t e = cudaMalloc(&p->scratch, std::max<size_t>(1, kp.ntiles) * sizeof(sb::KryPartial));
-    if (e != cudaSuccess) {
-      sb_krylov_plan_destroy(p);
-      return fail(SB_ERR_CUDA, "krylov plan scratch: %s", cudaGetErrorString(e));
-    }
+  if (sb::kry_dots(kmode) > 0) {
+    const cudaError_t e = p->scratch.upload(device, {}, std::max<size_t>(1, kp.ntiles));
+    if (e != cudaSuccess) return fail(SB_ERR_CUDA, "krylov plan scratch: %s", cudaGetErrorString(e));
   }
   p->grid = sb::krylov_grid(device, dtype, kmode, wide, kp.ntiles);
   p->copy_grid = mode == SB_KRYLOV_XPBY ? sb::krylov_grid(device, dtype, sb::kKryCopy, wide, kp.ntiles) : 0;
-  *out = p;
+  *out = p.release();
   return SB_OK;
 }
 
@@ -1414,7 +1435,7 @@ int sb_krylov_plan_launch2(sb_krylov_plan *p, double s, double t, sb_reduce_exac
     mode = sb::kKryCopy;
     grid = p->copy_grid;
   }
-  g_launches += uint64_t(sb::launch_krylov(p->params, p->dtype, mode, p->wide, grid, s, t, p->scratch, parts_dev, static_cast<cudaStream_t>(stream)));
+  g_launches += uint64_t(sb::launch_krylov(p->params, p->dtype, mode, p->wide, grid, s, t, p->scratch.ptr, parts_dev, static_cast<cudaStream_t>(stream)));
   SB_CUDA(cudaGetLastError());
   return SB_OK;
 }
@@ -1422,9 +1443,6 @@ int sb_krylov_plan_launch2(sb_krylov_plan *p, double s, double t, sb_reduce_exac
 int64_t sb_krylov_plan_bytes(const sb_krylov_plan *p) { return p ? p->bytes : 0; }
 
 int sb_krylov_plan_destroy(sb_krylov_plan *p) {
-  if (!p) return SB_OK;
-  DeviceGuard guard(p->device);
-  if (p->scratch) cudaFree(p->scratch);
   delete p;
   return SB_OK;
 }
@@ -1773,28 +1791,16 @@ static int stencil_plan_build(sb_stencil_plan **out, int device, int dtype, cons
   if (!acc_origin || zsize < 1) return fail(SB_ERR_INVALID, "sb_stencil_plan_create needs acc_origin and zsize >= 1");
   if (nbox < 0 || (nbox > 0 && (!lo || !hi))) return fail(SB_ERR_INVALID, "nbox %d: needs nbox >= 0 and lo / hi arrays", nbox);
   const int64_t size[3] = {src.pitch / es, src.ysize, zsize};
-  std::vector<std::array<int, 6>> thick, thin; // allocation-relative lo, ext
-  int64_t cells = 0, written = 0;
-  for (int b = 0; b < nbox; ++b) {
-    int64_t l[3], e[3];
-    bool empty = false;
-    for (int a = 0; a < 3; ++a) {
-      if (lo[3 * b + a] > hi[3 * b + a]) return fail(SB_ERR_INVALID, "box %d: lo > hi on axis %d", b, a);
-      l[a] = lo[3 * b + a] - acc_origin[a];
-      e[a] = hi[3 * b + a] - lo[3 * b + a];
-      empty = empty || e[a] == 0;
-    }
-    if (empty) continue;
-    if ((rc = stencil_box_reads_ok(b, l, e, rm, rp, size, "the op reads")) != SB_OK) return rc;
-    for (int f = 0; f < nf; ++f)
-      if ((rc = stencil_box_reads_ok(b, l, e, crm[f], crp[f], size, "coefficient field " + std::to_string(fsrc[f]) + " is read at")) != SB_OK)
-        return rc;
-    if (e[0] * e[1] * e[2] >= (1ll << 32)) return fail(SB_ERR_INVALID, "box %d: more than 2^32 cells", b);
-    const std::array<int, 6> bx = {int(l[0]), int(l[1]), int(l[2]), int(e[0]), int(e[1]), int(e[2])};
-    (e[0] >= 8 && e[1] >= 8 && e[2] >= 8 ? thick : thin).push_back(bx);
-    cells += e[0] * e[1] * e[2];
+  PlanBoxes B;
+  int64_t written = 0;
+  rc = plan_boxes(nbox, lo, hi, acc_origin, 8, [&](int b, const int64_t l[3], const int64_t e[3]) {
+    int rc = stencil_box_reads_ok(b, l, e, rm, rp, size, "the op reads");
+    for (int f = 0; f < nf && rc == SB_OK; ++f)
+      rc = stencil_box_reads_ok(b, l, e, crm[f], crp[f], size, "coefficient field " + std::to_string(fsrc[f]) + " is read at");
     written += stencil_colour_cells(&lo[3 * b], e, ncolours, colour);
-  }
+    return rc;
+  }, B);
+  if (rc != SB_OK) return rc;
   sb::OpColour col{ncolours, colour, {}};
   for (int a = 0; a < 3; ++a) col.par[a] = int(((acc_origin[a] % 2) + 2) % 2);
   sb::OpDiag dg{diag ? 1 : 0, centre, diag ? *omega : 0.0, diag ? float(*omega) : 0.0f};
@@ -1817,21 +1823,15 @@ static int stencil_plan_build(sb_stencil_plan **out, int device, int dtype, cons
   if (!guard.ok) return fail(SB_ERR_NOGPU, "cannot select CUDA device %d", device);
   int sms = 0;
   SB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
-  sb_stencil_plan *p = new sb_stencil_plan();
+  std::unique_ptr<sb_stencil_plan> p(new sb_stencil_plan());
   p->device = device;
-  p->es = es;
-  p->R = R;
-  p->has_coef = nf > 0;
-  p->bytes = cells * es * ((has_aux ? 2 : 1) + nf) + written * es;
-  if (!thick.empty()) {
+  p->bytes = B.cells * es * ((has_aux ? 2 : 1) + nf) + written * es;
+  if (!B.thick.empty()) {
     const int per_sm = sb::op_tile_prepare(R, es, device, nf, ncolours > 1, diag);
-    if (per_sm <= 0) {
-      delete p;
-      return fail(SB_ERR_CUDA, "the R = %d tile kernel cannot be configured: %s", R, cudaGetErrorString(cudaGetLastError()));
-    }
+    if (per_sm <= 0) return fail(SB_ERR_CUDA, "the R = %d tile kernel cannot be configured: %s", R, cudaGetErrorString(cudaGetLastError()));
     const int SW = sb::op_tile_sw(R), P = sb::op_tile_plane(R), NS = 2 * R + 1;
     const int CSW = sb::op_tile_sw(1), CP = sb::op_tile_plane(1), CS = sb::kOpCoefSlots;
-    for (const auto &b : thick) {
+    for (const PlanBox &b : B.thick) {
       sb::OpDTileParams tp{};
       tp.c = com;
       tp.col = col;
@@ -1852,60 +1852,39 @@ static int stencil_plan_build(sb_stencil_plan **out, int device, int dtype, cons
       }
       tp.src_end = com.src + com.slice * zsize;
       for (int a = 0; a < 3; ++a) {
-        tp.lo[a] = b[a];
-        tp.ext[a] = b[3 + a];
+        tp.lo[a] = b.lo[a];
+        tp.ext[a] = b.ext[a];
         tp.rm[a] = rm[a];
         tp.rp[a] = rp[a];
       }
-      tp.tiles_x = (tp.ext[0] + sb::kOpTileX - 1) / sb::kOpTileX;
-      tp.tiles_y = (tp.ext[1] + sb::kOpTileY - 1) / sb::kOpTileY;
-      // z chunks: at least two waves of resident CTAs, chunks no shorter than 16 planes (each chunk reloads rm + rp planes)
-      const long long cols = (long long)tp.tiles_x * tp.tiles_y;
-      const long long want = (2ll * sms * per_sm + cols - 1) / cols;
-      int zc = int((tp.ext[2] + want - 1) / want);
-      zc = std::max(zc, std::min(16, tp.ext[2]));
-      tp.zchunk = zc;
-      const long long grid = cols * ((tp.ext[2] + zc - 1) / zc);
-      if (grid >= (1ll << 31)) {
-        delete p;
-        return fail(SB_ERR_INVALID, "box too large for the tile kernel");
-      }
+      // each chunk reloads rm + rp planes
+      int grid = 0;
+      if ((rc = tile_grid(tp, tp.ext, sb::kOpTileX, sb::kOpTileY, sms, per_sm, 16, "tile kernel", grid)) != SB_OK) return rc;
       for (int c = 0; c < NS; ++c)
         for (int t = 0; t < n; ++t) {
           const int32_t *o = terms[t].offset;
           tp.toff[c][t] = ((c + o[2] + NS) % NS) * P + o[1] * SW + o[0];
         }
-      p->tiles.push_back(tp);
-      p->tile_grids.push_back(int(grid));
+      p->launches.push_back([tp, R, es, grid](cudaStream_t s) { return sb::launch_op_tile(tp, R, es, grid, s); });
     }
   }
-  for (size_t b0 = 0; b0 < thin.size(); b0 += sb::kOpMaxBoxes) {
-    sb::OpDCellParams cp{};
-    cp.c = com;
-    cp.col = col;
-    cp.dg = dg;
-    for (int t = 0; t < n; ++t)
-      cp.goff[t] = (long long)terms[t].offset[2] * com.slice + (long long)terms[t].offset[1] * com.pitch + (long long)terms[t].offset[0] * es;
-    for (int f = 0; f < nf; ++f) cp.coef[f] = static_cast<const char *>(coef[fsrc[f]].ptr);
-    for (int t = 0; t < n; ++t) {
-      const int32_t *c = terms[t].coef_offset;
-      cp.cfield[t] = (signed char)(terms[t].coef < 0 ? -1 : fmap[terms[t].coef]);
-      cp.cgoff[t] = (long long)c[2] * com.slice + (long long)c[1] * com.pitch + (long long)c[0] * es;
-    }
-    cp.first[0] = 0;
-    for (size_t b = b0; b < thin.size() && b < b0 + sb::kOpMaxBoxes; ++b) {
-      const int m = cp.n++;
-      for (int a = 0; a < 3; ++a) {
-        cp.lo[m][a] = thin[b][a];
-        cp.ext[m][a] = thin[b][3 + a];
-      }
-      cp.first[m + 1] = cp.first[m] + (long long)thin[b][3] * thin[b][4] * thin[b][5];
-    }
-    const long long total = cp.first[cp.n];
-    p->cells.push_back(cp);
-    p->cell_grids.push_back(int(std::min<long long>((total + 255) / 256, 32ll * sms)));
+  sb::OpDCellParams cp{};
+  cp.c = com;
+  cp.col = col;
+  cp.dg = dg;
+  for (int t = 0; t < n; ++t)
+    cp.goff[t] = (long long)terms[t].offset[2] * com.slice + (long long)terms[t].offset[1] * com.pitch + (long long)terms[t].offset[0] * es;
+  for (int f = 0; f < nf; ++f) cp.coef[f] = static_cast<const char *>(coef[fsrc[f]].ptr);
+  for (int t = 0; t < n; ++t) {
+    const int32_t *c = terms[t].coef_offset;
+    cp.cfield[t] = (signed char)(terms[t].coef < 0 ? -1 : fmap[terms[t].coef]);
+    cp.cgoff[t] = (long long)c[2] * com.slice + (long long)c[1] * com.pitch + (long long)c[0] * es;
   }
-  *out = p;
+  const bool has_coef = nf > 0;
+  cell_groups(B.thin, cp, &sb::OpDCellParams::n, sms, [&](const sb::OpDCellParams &g, int grid) {
+    p->launches.push_back([g, es, has_coef, grid](cudaStream_t s) { return sb::launch_op_cells(g, es, has_coef, grid, s); });
+  });
+  *out = p.release();
   return SB_OK;
 }
 
@@ -2047,25 +2026,14 @@ int sb_stencil_sys_plan_create(sb_stencil_plan **out, int device, int dtype, con
   if (nbox < 0 || (nbox > 0 && (!lo || !hi))) return fail(SB_ERR_INVALID, "nbox %d: needs nbox >= 0 and lo / hi arrays", nbox);
   const int64_t pitch = outputs[0].pitch, slice = pitch * outputs[0].ysize;
   const int64_t size[3] = {pitch / es, outputs[0].ysize, zsize};
-  std::vector<std::array<int, 6>> thick, thin; // allocation-relative lo, ext
-  int64_t cells = 0;
-  for (int b = 0; b < nbox; ++b) {
-    int64_t l[3], e[3];
-    bool empty = false;
-    for (int a = 0; a < 3; ++a) {
-      if (lo[3 * b + a] > hi[3 * b + a]) return fail(SB_ERR_INVALID, "box %d: lo > hi on axis %d", b, a);
-      l[a] = lo[3 * b + a] - acc_origin[a];
-      e[a] = hi[3 * b + a] - lo[3 * b + a];
-      empty = empty || e[a] == 0;
-    }
-    if (empty) continue;
-    for (int i = 0; i < nin; ++i)
-      if (used[i] && (rc = stencil_box_reads_ok(b, l, e, rm[i], rp[i], size, "input " + std::to_string(i) + " is read at")) != SB_OK) return rc;
-    if (e[0] * e[1] * e[2] >= (1ll << 32)) return fail(SB_ERR_INVALID, "box %d: more than 2^32 cells", b);
-    const std::array<int, 6> bx = {int(l[0]), int(l[1]), int(l[2]), int(e[0]), int(e[1]), int(e[2])};
-    (e[0] >= 8 && e[1] >= 8 && e[2] >= 8 ? thick : thin).push_back(bx);
-    cells += e[0] * e[1] * e[2];
-  }
+  PlanBoxes B;
+  rc = plan_boxes(nbox, lo, hi, acc_origin, 8, [&](int b, const int64_t l[3], const int64_t e[3]) {
+    int rc = SB_OK;
+    for (int i = 0; i < nin && rc == SB_OK; ++i)
+      if (used[i]) rc = stencil_box_reads_ok(b, l, e, rm[i], rp[i], size, "input " + std::to_string(i) + " is read at");
+    return rc;
+  }, B);
+  if (rc != SB_OK) return rc;
 
   // the read inputs renumbered 0 .. nr - 1 (ring r of the tile kernel); each ring's plane size; the shared row width fits
   // the widest window shifted onto 16-byte phase
@@ -2093,7 +2061,7 @@ int sb_stencil_sys_plan_create(sb_stencil_plan **out, int device, int dtype, con
   int sms = 0, optin = 0;
   SB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
   SB_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device));
-  if (!thick.empty() && smem > size_t(optin))
+  if (!B.thick.empty() && smem > size_t(optin))
     return fail(SB_ERR_INVALID, "the system's tile kernel needs %zu bytes of shared memory per block, the device allows %d", smem, optin);
 
   // the terms sorted by output (stable): the rule sums each output's terms in list order
@@ -2118,18 +2086,13 @@ int sb_stencil_sys_plan_create(sb_stencil_plan **out, int device, int dtype, con
     com.wf[k] = float(T.weight); // round to nearest
   }
 
-  sb_stencil_plan *p = new sb_stencil_plan();
+  std::unique_ptr<sb_stencil_plan> p(new sb_stencil_plan());
   p->device = device;
-  p->es = es;
-  p->bytes = cells * es * (nr + nout);
-  p->sys_smem = smem;
-  if (!thick.empty()) {
+  p->bytes = B.cells * es * (nr + nout);
+  if (!B.thick.empty()) {
     const int per_sm = sb::sys_tile_prepare(es, device, smem);
-    if (per_sm <= 0) {
-      delete p;
-      return fail(SB_ERR_CUDA, "the system tile kernel cannot be configured: %s", cudaGetErrorString(cudaGetLastError()));
-    }
-    for (const auto &b : thick) {
+    if (per_sm <= 0) return fail(SB_ERR_CUDA, "the system tile kernel cannot be configured: %s", cudaGetErrorString(cudaGetLastError()));
+    for (const PlanBox &b : B.thick) {
       sb::SysTileParams tp{};
       tp.c = com;
       tp.nr = nr;
@@ -2139,7 +2102,7 @@ int sb_stencil_sys_plan_create(sb_stencil_plan **out, int device, int dtype, con
         const int i = src_of[r];
         tp.in[r] = static_cast<const char *>(inputs[i].ptr);
         tp.vec[r] = pitch % 16 == 0; // else rows alternate between 16-byte phases: elements one by one
-        shift[r] = tp.vec[r] ? int((uintptr_t(tp.in[r]) + uintptr_t(int64_t(b[0] - rm[i][0]) * es)) % 16) / es : 0;
+        shift[r] = tp.vec[r] ? int((uintptr_t(tp.in[r]) + uintptr_t(int64_t(b.lo[0] - rm[i][0]) * es)) % 16) / es : 0;
         tp.shift[r] = shift[r];
         tp.ns[r] = ns[r];
         tp.base[r] = base[r];
@@ -2160,66 +2123,33 @@ int sb_stencil_sys_plan_create(sb_stencil_plan **out, int device, int dtype, con
         }
       }
       for (int a = 0; a < 3; ++a) {
-        tp.lo[a] = b[a];
-        tp.ext[a] = b[3 + a];
+        tp.lo[a] = b.lo[a];
+        tp.ext[a] = b.ext[a];
       }
-      tp.tiles_x = (tp.ext[0] + sb::kOpTileX - 1) / sb::kOpTileX;
-      tp.tiles_y = (tp.ext[1] + sb::kOpTileY - 1) / sb::kOpTileY;
-      // z chunks as for an operator: at least two waves of resident CTAs, chunks no shorter than 16 planes
-      const long long cols = (long long)tp.tiles_x * tp.tiles_y;
-      const long long want = (2ll * sms * per_sm + cols - 1) / cols;
-      int zc = int((tp.ext[2] + want - 1) / want);
-      zc = std::max(zc, std::min(16, tp.ext[2]));
-      tp.zchunk = zc;
-      const long long grid = cols * ((tp.ext[2] + zc - 1) / zc);
-      if (grid >= (1ll << 31)) {
-        delete p;
-        return fail(SB_ERR_INVALID, "box too large for the tile kernel");
-      }
-      p->sys_tiles.push_back(tp);
-      p->sys_tile_grids.push_back(int(grid));
+      // z chunks as for an operator
+      int grid = 0;
+      if ((rc = tile_grid(tp, tp.ext, sb::kOpTileX, sb::kOpTileY, sms, per_sm, 16, "tile kernel", grid)) != SB_OK) return rc;
+      p->launches.push_back([tp, es, smem, grid](cudaStream_t s) { return sb::launch_sys_tile(tp, es, smem, grid, s); });
     }
   }
-  for (size_t b0 = 0; b0 < thin.size(); b0 += sb::kOpMaxBoxes) {
-    sb::SysCellParams cp{};
-    cp.c = com;
-    for (int r = 0; r < nr; ++r) cp.in[r] = static_cast<const char *>(inputs[src_of[r]].ptr);
-    for (int k = 0; k < n; ++k) {
-      const sb_stencil_sys_term &T = terms[order[size_t(k)]];
-      for (int a = 0; a < 3; ++a) {
-        cp.o[k][a] = (signed char)T.offset[a];
-        cp.co[k][a] = (signed char)T.coef_offset[a];
-      }
+  sb::SysCellParams cp{};
+  cp.c = com;
+  for (int r = 0; r < nr; ++r) cp.in[r] = static_cast<const char *>(inputs[src_of[r]].ptr);
+  for (int k = 0; k < n; ++k) {
+    const sb_stencil_sys_term &T = terms[order[size_t(k)]];
+    for (int a = 0; a < 3; ++a) {
+      cp.o[k][a] = (signed char)T.offset[a];
+      cp.co[k][a] = (signed char)T.coef_offset[a];
     }
-    cp.first[0] = 0;
-    for (size_t b = b0; b < thin.size() && b < b0 + sb::kOpMaxBoxes; ++b) {
-      const int m = cp.nb++;
-      for (int a = 0; a < 3; ++a) {
-        cp.lo[m][a] = thin[b][a];
-        cp.ext[m][a] = thin[b][3 + a];
-      }
-      cp.first[m + 1] = cp.first[m] + (long long)thin[b][3] * thin[b][4] * thin[b][5];
-    }
-    const long long total = cp.first[cp.nb];
-    p->sys_cells.push_back(cp);
-    p->sys_cell_grids.push_back(int(std::min<long long>((total + 255) / 256, 32ll * sms)));
   }
-  *out = p;
+  cell_groups(B.thin, cp, &sb::SysCellParams::nb, sms, [&](const sb::SysCellParams &g, int grid) {
+    p->launches.push_back([g, es, grid](cudaStream_t s) { return sb::launch_sys_cells(g, es, grid, s); });
+  });
+  *out = p.release();
   return SB_OK;
 }
 
-int sb_stencil_plan_launch(sb_stencil_plan *p, void *stream) {
-  if (!p) return fail(SB_ERR_INVALID, "null plan");
-  DeviceGuard guard(p->device);
-  if (!guard.ok) return fail(SB_ERR_NOGPU, "cannot select CUDA device %d", p->device);
-  const cudaStream_t s = static_cast<cudaStream_t>(stream);
-  for (size_t i = 0; i < p->tiles.size(); ++i) g_launches += uint64_t(sb::launch_op_tile(p->tiles[i], p->R, p->es, p->tile_grids[i], s));
-  for (size_t i = 0; i < p->cells.size(); ++i) g_launches += uint64_t(sb::launch_op_cells(p->cells[i], p->es, p->has_coef, p->cell_grids[i], s));
-  for (size_t i = 0; i < p->sys_tiles.size(); ++i) g_launches += uint64_t(sb::launch_sys_tile(p->sys_tiles[i], p->es, p->sys_smem, p->sys_tile_grids[i], s));
-  for (size_t i = 0; i < p->sys_cells.size(); ++i) g_launches += uint64_t(sb::launch_sys_cells(p->sys_cells[i], p->es, p->sys_cell_grids[i], s));
-  SB_CUDA(cudaGetLastError());
-  return SB_OK;
-}
+int sb_stencil_plan_launch(sb_stencil_plan *p, void *stream) { return run_launches(p, stream); }
 
 int64_t sb_stencil_plan_bytes(const sb_stencil_plan *p) { return p ? p->bytes : 0; }
 
@@ -2313,12 +2243,10 @@ static int transfer_plan_build(sb_transfer_plan **out, int device, int dtype, in
     e[a] = hi[a] - lo[a];
     empty = empty || e[a] == 0;
   }
-  sb_transfer_plan *p = nullptr;
+  std::unique_ptr<sb_transfer_plan> p(new sb_transfer_plan());
+  p->device = device;
   if (empty) {
-    p = new sb_transfer_plan();
-    p->device = device;
-    p->es = es;
-    *out = p;
+    *out = p.release();
     return SB_OK;
   }
   const int zero[3] = {0, 0, 0};
@@ -2342,14 +2270,9 @@ static int transfer_plan_build(sb_transfer_plan **out, int device, int dtype, in
   if (!guard.ok) return fail(SB_ERR_NOGPU, "cannot select CUDA device %d", device);
   int sms = 0;
   SB_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device));
-  p = new sb_transfer_plan();
-  p->device = device;
-  p->es = es;
-  p->kind = kind;
-  p->face = face;
   const int64_t cells = e[0] * e[1] * e[2];
   if (!prolong) {
-    sb::RestrictParams &r = p->r;
+    sb::RestrictParams r{};
     r.dst = static_cast<char *>(dst.ptr);
     r.src = static_cast<const char *>(src.ptr);
     r.dpitch = dst.pitch;
@@ -2362,9 +2285,12 @@ static int transfer_plan_build(sb_transfer_plan **out, int device, int dtype, in
       r.flo[a] = int(rl[a]);
     }
     p->bytes = (face >= 0 ? 4 + 1 : 8 + 1) * cells * es;
-    p->launches = 1;
+    if (face >= 0)
+      p->launches.push_back([r, es, face](cudaStream_t s) { return sb::launch_face_restrict(r, es, face, s); });
+    else
+      p->launches.push_back([r, es](cudaStream_t s) { return sb::launch_restrict(r, es, s); });
   } else {
-    sb::ProlongParams &q = p->pr;
+    sb::ProlongParams q{};
     q.dst = static_cast<char *>(dst.ptr);
     q.aux = has_aux ? static_cast<const char *>(aux.ptr) : nullptr;
     q.src = static_cast<const char *>(src.ptr);
@@ -2386,27 +2312,13 @@ static int transfer_plan_build(sb_transfer_plan **out, int device, int dtype, in
     }
     p->bytes = reads * es + cells * es * (has_aux ? 2 : 1);
     const int per_sm = sb::prolong_ctas_per_sm(es);
-    if (per_sm <= 0) {
-      delete p;
-      return fail(SB_ERR_CUDA, "the prolongation kernel cannot be configured: %s", cudaGetErrorString(cudaGetLastError()));
-    }
-    q.tiles_x = (q.pext[0] + sb::kProlongX - 1) / sb::kProlongX;
-    q.tiles_y = (q.pext[1] + sb::kProlongY - 1) / sb::kProlongY;
-    // z chunks: at least two waves of resident CTAs, no shorter than 8 parent planes (each chunk reloads 2 planes)
-    const long long cols = (long long)q.tiles_x * q.tiles_y;
-    const long long want = (2ll * sms * per_sm + cols - 1) / cols;
-    int zc = int((q.pext[2] + want - 1) / want);
-    zc = std::max(zc, std::min(8, q.pext[2]));
-    q.zchunk = zc;
-    const long long grid = cols * ((q.pext[2] + zc - 1) / zc);
-    if (grid >= (1ll << 31)) {
-      delete p;
-      return fail(SB_ERR_INVALID, "box too large for the prolongation kernel");
-    }
-    p->grid = int(grid);
-    p->launches = 1;
+    if (per_sm <= 0) return fail(SB_ERR_CUDA, "the prolongation kernel cannot be configured: %s", cudaGetErrorString(cudaGetLastError()));
+    // over the parents, chunks of at least 8 parent planes (each chunk reloads 2 planes)
+    int grid = 0;
+    if ((rc = tile_grid(q, q.pext, sb::kProlongX, sb::kProlongY, sms, per_sm, 8, "prolongation kernel", grid)) != SB_OK) return rc;
+    p->launches.push_back([q, es, grid](cudaStream_t s) { return sb::launch_prolong(q, es, grid, s); });
   }
-  *out = p;
+  *out = p.release();
   return SB_OK;
 }
 
@@ -2473,28 +2385,16 @@ static int transfer_oplan_build(const char *fn, sb_transfer_plan **out, int devi
   for (int k = 0; k < ncoef; ++k) nf += used[k] ? 1 : 0;
   const int64_t dsize[3] = {dst.pitch / es, dst.ysize, dst_zsize}, ssize[3] = {src.pitch / es, src.ysize, src_zsize};
   const int zero[3] = {0, 0, 0}, one[3] = {1, 1, 1};
-  // per box: coarse lo, extent (dst allocation coordinates), fine 2 * lo (src allocation coordinates)
-  std::vector<std::array<int, 9>> thick, thin;
-  int64_t cells = 0;
-  for (int b = 0; b < nbox; ++b) {
-    int64_t l[3], e[3], fl[3], fe[3];
-    bool empty = false;
-    for (int a = 0; a < 3; ++a) {
-      if (lo[3 * b + a] > hi[3 * b + a]) return fail(SB_ERR_INVALID, "box %d: lo > hi on axis %c", b, "xyz"[a]);
-      l[a] = lo[3 * b + a] - dst_acc_origin[a];
-      e[a] = hi[3 * b + a] - lo[3 * b + a];
-      fl[a] = 2 * lo[3 * b + a] - src_acc_origin[a];
-      fe[a] = 2 * e[a];
-      empty = empty || e[a] == 0;
-    }
-    if (empty) continue;
-    if ((rc = stencil_box_reads_ok(b, l, e, zero, zero, dsize, "dst is written at")) != SB_OK) return rc;
-    if ((rc = stencil_box_reads_ok(b, fl, fe, one, one, ssize, "the fused restriction reads fine")) != SB_OK) return rc;
-    if (e[0] * e[1] * e[2] >= (1ll << 32)) return fail(SB_ERR_INVALID, "box %d: more than 2^32 cells", b);
-    cells += e[0] * e[1] * e[2];
-    const std::array<int, 9> B = {int(l[0]), int(l[1]), int(l[2]), int(e[0]), int(e[1]), int(e[2]), int(fl[0]), int(fl[1]), int(fl[2])};
-    (e[0] >= 4 && e[1] >= 4 && e[2] >= 4 ? thick : thin).push_back(B);
-  }
+  // the fine cell 2 * (global lo) of a coarse box at l on axis a (dst allocation coordinates), in src allocation coordinates
+  auto fine_lo = [&](int64_t l, int a) { return 2 * (l + dst_acc_origin[a]) - src_acc_origin[a]; };
+  PlanBoxes B;
+  rc = plan_boxes(nbox, lo, hi, dst_acc_origin, 4, [&](int b, const int64_t l[3], const int64_t e[3]) {
+    const int64_t fl[3] = {fine_lo(l[0], 0), fine_lo(l[1], 1), fine_lo(l[2], 2)}, fe[3] = {2 * e[0], 2 * e[1], 2 * e[2]};
+    int rc = stencil_box_reads_ok(b, l, e, zero, zero, dsize, "dst is written at");
+    if (rc == SB_OK) rc = stencil_box_reads_ok(b, fl, fe, one, one, ssize, "the fused restriction reads fine");
+    return rc;
+  }, B);
+  if (rc != SB_OK) return rc;
 
   sb::RopCommon com{};
   com.dst = static_cast<char *>(dst.ptr);
@@ -2511,130 +2411,72 @@ static int transfer_oplan_build(const char *fn, sb_transfer_plan **out, int devi
     com.w[t] = terms[t].weight;
     com.wf[t] = float(terms[t].weight); // round to nearest
   }
-  sb_transfer_plan *p = new sb_transfer_plan();
+  std::unique_ptr<sb_transfer_plan> p(new sb_transfer_plan());
   p->device = device;
-  p->es = es;
-  p->kind = SB_TRANSFER_RESTRICT;
-  p->fused = true;
-  p->bytes = cells * es * (8 * ((aux_term ? 2 : 1) + nf) + 1);
-  if (cells == 0) {
-    *out = p;
+  p->bytes = B.cells * es * (8 * ((aux_term ? 2 : 1) + nf) + 1);
+  if (B.cells == 0) {
+    *out = p.release();
     return SB_OK;
   }
   DeviceGuard guard(device);
-  if (!guard.ok) {
-    delete p;
-    return fail(SB_ERR_NOGPU, "cannot select CUDA device %d", device);
-  }
+  if (!guard.ok) return fail(SB_ERR_NOGPU, "cannot select CUDA device %d", device);
   int sms = 0;
-  if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device) != cudaSuccess) {
-    delete p;
+  if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device) != cudaSuccess)
     return fail(SB_ERR_CUDA, "cudaDeviceGetAttribute: %s", cudaGetErrorString(cudaGetLastError()));
-  }
-  if (!thick.empty()) {
+  // the launches take the coefficient parameters only with coefficient terms (nf > 0): the plain kernels their base
+  if (!B.thick.empty()) {
     const int per_sm = sb::rop_tile_ctas_per_sm(es, nf > 0);
-    if (per_sm <= 0) {
-      delete p;
-      return fail(SB_ERR_CUDA, "the fused restriction's tile kernel cannot be configured: %s", cudaGetErrorString(cudaGetLastError()));
-    }
-    for (const auto &B : thick) {
-      sb::RopTileParams tp{};
+    if (per_sm <= 0) return fail(SB_ERR_CUDA, "the fused restriction's tile kernel cannot be configured: %s", cudaGetErrorString(cudaGetLastError()));
+    for (const PlanBox &b : B.thick) {
+      sb::RopVTileParams tp{};
       tp.c = com;
       for (int a = 0; a < 3; ++a) {
-        tp.lo[a] = B[a];
-        tp.ext[a] = B[3 + a];
-        tp.flo[a] = B[6 + a];
-        tp.rlo[a] = B[6 + a] - 1;
-        tp.rhi[a] = B[6 + a] + 2 * B[3 + a] + 1;
+        tp.lo[a] = b.lo[a];
+        tp.ext[a] = b.ext[a];
+        tp.flo[a] = int(fine_lo(b.lo[a], a));
+        tp.rlo[a] = tp.flo[a] - 1;
+        tp.rhi[a] = tp.flo[a] + 2 * b.ext[a] + 1;
       }
       for (int c = 0; c < 3; ++c)
         for (int t = 0; t < n; ++t) {
           const int32_t *o = terms[t].offset;
           tp.toff[c][t] = ((c + o[2] + 3) % 3) * sb::kRopPlane + o[1] * sb::kRopSW + o[0];
         }
-      tp.tiles_x = (tp.ext[0] + sb::kRestrictX - 1) / sb::kRestrictX;
-      tp.tiles_y = (tp.ext[1] + sb::kRestrictY - 1) / sb::kRestrictY;
-      // z chunks: at least two waves of resident CTAs, no shorter than 4 coarse planes (each chunk reloads 2 fine planes)
-      const long long cols = (long long)tp.tiles_x * tp.tiles_y;
-      const long long want = (2ll * sms * per_sm + cols - 1) / cols;
-      int zc = int((tp.ext[2] + want - 1) / want);
-      zc = std::max(zc, std::min(4, tp.ext[2]));
-      tp.zchunk = zc;
-      const long long grid = cols * ((tp.ext[2] + zc - 1) / zc);
-      if (grid >= (1ll << 31)) {
-        delete p;
-        return fail(SB_ERR_INVALID, "box too large for the fused restriction's tile kernel");
-      }
-      if (nf == 0) {
-        p->rop_tiles.push_back(tp);
-        p->rop_tile_grids.push_back(int(grid));
-        continue;
-      }
-      sb::RopVTileParams vp{};
-      static_cast<sb::RopTileParams &>(vp) = tp;
-      for (int k = 0; k < ncoef; ++k) vp.coef[k] = static_cast<const char *>(coef[k].ptr);
+      // each chunk reloads 2 fine planes
+      int grid = 0;
+      if ((rc = tile_grid(tp, tp.ext, sb::kRestrictX, sb::kRestrictY, sms, per_sm, 4, "fused restriction's tile kernel", grid)) != SB_OK) return rc;
+      for (int k = 0; k < ncoef; ++k) tp.coef[k] = static_cast<const char *>(coef[k].ptr);
       for (int t = 0; t < n; ++t) {
         const int32_t *c = terms[t].coef_offset;
-        vp.cfield[t] = (signed char)terms[t].coef;
-        vp.cgoff[t] = (long long)c[2] * com.sslice + (long long)c[1] * com.spitch + (long long)c[0] * es;
+        tp.cfield[t] = (signed char)terms[t].coef;
+        tp.cgoff[t] = (long long)c[2] * com.sslice + (long long)c[1] * com.spitch + (long long)c[0] * es;
       }
-      p->rop_vtiles.push_back(vp);
-      p->rop_vtile_grids.push_back(int(grid));
+      if (nf == 0)
+        p->launches.push_back([base = sb::RopTileParams(tp), es, grid](cudaStream_t s) { return sb::launch_rop_tile(base, es, grid, s); });
+      else
+        p->launches.push_back([tp, es, grid](cudaStream_t s) { return sb::launch_rop_vtile(tp, es, grid, s); });
     }
   }
-  for (size_t b0 = 0; b0 < thin.size(); b0 += sb::kRopMaxBoxes) {
-    sb::RopCellParams cp{};
-    cp.c = com;
-    cp.first[0] = 0;
-    for (size_t b = b0; b < thin.size() && b < b0 + sb::kRopMaxBoxes; ++b) {
-      const int m = cp.n++;
-      for (int a = 0; a < 3; ++a) {
-        cp.lo[m][a] = thin[b][a];
-        cp.ext[m][a] = thin[b][3 + a];
-        cp.flo[m][a] = thin[b][6 + a];
-      }
-      cp.first[m + 1] = cp.first[m] + (long long)thin[b][3] * thin[b][4] * thin[b][5];
-    }
-    const int grid = int(std::min<long long>((cp.first[cp.n] + 255) / 256, 32ll * sms));
-    if (nf == 0) {
-      p->rop_cells.push_back(cp);
-      p->rop_cell_grids.push_back(grid);
-      continue;
-    }
-    sb::RopVCellParams vp{};
-    static_cast<sb::RopCellParams &>(vp) = cp;
-    for (int k = 0; k < ncoef; ++k) vp.coef[k] = static_cast<const char *>(coef[k].ptr);
-    for (int t = 0; t < n; ++t) {
-      vp.cfield[t] = (signed char)terms[t].coef;
-      for (int a = 0; a < 3; ++a) vp.coff[t][a] = (signed char)terms[t].coef_offset[a];
-    }
-    p->rop_vcells.push_back(vp);
-    p->rop_vcell_grids.push_back(grid);
+  sb::RopVCellParams cp{};
+  cp.c = com;
+  for (int k = 0; k < ncoef; ++k) cp.coef[k] = static_cast<const char *>(coef[k].ptr);
+  for (int t = 0; t < n; ++t) {
+    cp.cfield[t] = (signed char)terms[t].coef;
+    for (int a = 0; a < 3; ++a) cp.coff[t][a] = (signed char)terms[t].coef_offset[a];
   }
-  p->launches = int(p->rop_tiles.size() + p->rop_cells.size() + p->rop_vtiles.size() + p->rop_vcells.size());
-  *out = p;
+  cell_groups(B.thin, cp, &sb::RopVCellParams::n, sms, [&](sb::RopVCellParams &g, int grid) {
+    for (int m = 0; m < g.n; ++m)
+      for (int a = 0; a < 3; ++a) g.flo[m][a] = int(fine_lo(g.lo[m][a], a));
+    if (nf == 0)
+      p->launches.push_back([base = sb::RopCellParams(g), es, grid](cudaStream_t s) { return sb::launch_rop_cells(base, es, grid, s); });
+    else
+      p->launches.push_back([g, es, grid](cudaStream_t s) { return sb::launch_rop_vcells(g, es, grid, s); });
+  });
+  *out = p.release();
   return SB_OK;
 }
 
-int sb_transfer_plan_launch(sb_transfer_plan *p, void *stream) {
-  if (!p) return fail(SB_ERR_INVALID, "null plan");
-  if (!p->launches) return SB_OK;
-  DeviceGuard guard(p->device);
-  if (!guard.ok) return fail(SB_ERR_NOGPU, "cannot select CUDA device %d", p->device);
-  const cudaStream_t s = static_cast<cudaStream_t>(stream);
-  if (p->fused) {
-    for (size_t i = 0; i < p->rop_tiles.size(); ++i) g_launches += uint64_t(sb::launch_rop_tile(p->rop_tiles[i], p->es, p->rop_tile_grids[i], s));
-    for (size_t i = 0; i < p->rop_cells.size(); ++i) g_launches += uint64_t(sb::launch_rop_cells(p->rop_cells[i], p->es, p->rop_cell_grids[i], s));
-    for (size_t i = 0; i < p->rop_vtiles.size(); ++i) g_launches += uint64_t(sb::launch_rop_vtile(p->rop_vtiles[i], p->es, p->rop_vtile_grids[i], s));
-    for (size_t i = 0; i < p->rop_vcells.size(); ++i) g_launches += uint64_t(sb::launch_rop_vcells(p->rop_vcells[i], p->es, p->rop_vcell_grids[i], s));
-  } else {
-    g_launches += uint64_t(p->kind == SB_TRANSFER_PROLONG ? sb::launch_prolong(p->pr, p->es, p->grid, s)
-                           : p->face >= 0             ? sb::launch_face_restrict(p->r, p->es, p->face, s)
-                                                      : sb::launch_restrict(p->r, p->es, s));
-  }
-  SB_CUDA(cudaGetLastError());
-  return SB_OK;
-}
+int sb_transfer_plan_launch(sb_transfer_plan *p, void *stream) { return run_launches(p, stream); }
 
 int64_t sb_transfer_plan_bytes(const sb_transfer_plan *p) { return p ? p->bytes : 0; }
 

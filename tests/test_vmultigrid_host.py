@@ -165,7 +165,7 @@ def dcreate(terms=KAPPA, dtype=2, dst=(0x10000, ROW, ROWS), src=(0x200000, ROW, 
     (dict(f=(0x400000, ROW, ROWS - 1)), "aux has another pitch or row count than src"),
     (dict(coefs=K4[:1] + ((0x900000, ROW + 8, ROWS),) + K4[2:]), "coefficient field 1 has another pitch or row count than src"),
     (dict(hi=((19, 8, 8),)), "box 0: the op reads cells 0 .. 20 on axis x, outside the allocation's 0 .. 19"),
-    (dict(lo=((0, 3, 0),), hi=((8, 2, 8),)), "box 0: lo > hi on axis 1"),
+    (dict(lo=((0, 3, 0),), hi=((8, 2, 8),)), "box 0: lo > hi on axis y"),
 ])
 def test_dplan_errors(kw, msg):
     rc, err = dcreate(**kw)
