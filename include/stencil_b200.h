@@ -395,7 +395,10 @@ int sb_stencil_laplacian(int order, const double spacing[3], sb_stencil_term *ou
  * every axis go to the z-marching tile kernel, one launch each; thinner boxes (exterior slabs) share one-thread-per-cell
  * launches of up to 16 boxes.  Errors (SB_ERR_INVALID with a message, checked before anything is allocated): an unknown
  * dtype, an invalid term list, an aux term without aux, dst == src, mismatched pitches or row counts, a pointer or pitch
- * that is not a multiple of the element size, lo > hi, and a box whose reads leave the allocation.
+ * that is not a multiple of the element size, lo > hi, and a box whose reads leave the allocation.  The kernels take
+ * allocation coordinates as 32-bit int, so a box whose read window (reach included) ends past 2^31 - 1 on some axis, or
+ * that has 2^32 cells or more, is SB_ERR_INVALID too, with a message naming the box and axis; this holds for every
+ * operator, coloured, diagonal and system plan.  Empty boxes keep their place in the numbering of the messages.
  * sb_stencil_plan_launch allocates nothing and never synchronises the host. */
 typedef struct sb_stencil_plan sb_stencil_plan;
 int sb_stencil_plan_create(sb_stencil_plan **out, int device, int dtype, const sb_stencil_term *terms, int n, sb_pitched dst,
@@ -592,7 +595,10 @@ int sb_transfer_check(const int64_t fine_dim[3], const int64_t coarse_dim[3], co
  * (SB_ERR_INVALID with a message, before anything is allocated): an unknown dtype or kind, a NULL dst or src, dst == src,
  * aux given to a restriction, aux with another pitch or row count than dst, a pointer or pitch that is not a multiple of
  * the element size, lo > hi, a box outside dst's allocation, and reads that leave src's allocation (restriction: fine
- * [2 lo, 2 hi); prolongation: coarse [floor(lo / 2) - 1, floor((hi - 1) / 2) + 2) on every axis).
+ * [2 lo, 2 hi); prolongation: coarse [floor(lo / 2) - 1, floor((hi - 1) / 2) + 2) on every axis).  The kernels take
+ * allocation coordinates as 32-bit int, so a box or read window that ends past 2^31 - 1 on some axis, a box of 2^32 cells
+ * or more, and a prolongation whose 2 * src_acc_origin - dst_acc_origin does not fit 32 bits are SB_ERR_INVALID too, with
+ * a message naming the axis; the fused restrictions below check their fine windows the same way.
  * sb_transfer_plan_launch allocates nothing and never synchronises the host.  sb_transfer_plan_bytes: the algorithmic
  * bytes of a launch, every element the rule reads counted once and one element written per cell of the box. */
 typedef struct sb_transfer_plan sb_transfer_plan;

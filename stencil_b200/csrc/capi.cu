@@ -359,9 +359,17 @@ struct PlanBoxes {
   int64_t cells = 0;
 };
 
+// Whether a non-empty box of extent e has 2^32 cells or more, without overflowing: the kernels count cells in 32 bits.
+bool over_2_32_cells(const int64_t e[3]) {
+  const int64_t cap = 1ll << 32;
+  if (e[0] >= cap || e[1] >= cap || e[2] >= cap) return true;
+  return uint64_t(e[0]) * uint64_t(e[1]) >= uint64_t((cap + e[2] - 1) / e[2]);
+}
+
 // Checks and sorts the nbox boxes [lo, hi) (global coordinates, 3 per box) of a destination whose allocation starts at
 // acc_origin: a box is thick when its extent is at least `thick` on every axis.  reads(b, l, e) checks what box b reads
-// (allocation-relative lo l, extent e) and returns SB_OK or its error.
+// (allocation-relative lo l, extent e) and returns SB_OK or its error; it checks a window that holds the box with
+// stencil_box_reads_ok, so l and l + e fit an int.
 template <class Reads>
 int plan_boxes(int nbox, const int64_t *lo, const int64_t *hi, const int64_t acc_origin[3], int thick, Reads reads, PlanBoxes &out) {
   for (int b = 0; b < nbox; ++b) {
@@ -376,7 +384,7 @@ int plan_boxes(int nbox, const int64_t *lo, const int64_t *hi, const int64_t acc
     if (empty) continue;
     const int rc = reads(b, l, e);
     if (rc != SB_OK) return rc;
-    if (e[0] * e[1] * e[2] >= (1ll << 32)) return fail(SB_ERR_INVALID, "box %d: more than 2^32 cells", b);
+    if (over_2_32_cells(e)) return fail(SB_ERR_INVALID, "box %d: more than 2^32 cells", b);
     const PlanBox box = {{int(l[0]), int(l[1]), int(l[2])}, {int(e[0]), int(e[1]), int(e[2])}};
     (e[0] >= thick && e[1] >= thick && e[2] >= thick ? out.thick : out.thin).push_back(box);
     out.cells += e[0] * e[1] * e[2];
@@ -1489,13 +1497,18 @@ static int stencil_terms_ok(const sb_stencil_vterm *terms, int n) {
 }
 
 // Whether box b (allocation-relative lo l, extent e), read rm cells below and rp above on each axis, stays inside an
-// allocation of size[3]; who: what reads ("the op reads", "input 2 is read at", ...).
+// allocation of size[3], with the window's end below 2^31: the kernels take these coordinates as int.  who: what reads
+// ("the op reads", "input 2 is read at", ...).
 static int stencil_box_reads_ok(int b, const int64_t l[3], const int64_t e[3], const int rm[3], const int rp[3], const int64_t size[3],
                                 const std::string &who) {
-  for (int a = 0; a < 3; ++a)
+  for (int a = 0; a < 3; ++a) {
     if (l[a] - rm[a] < 0 || l[a] + e[a] + rp[a] > size[a])
       return fail(SB_ERR_INVALID, "box %d: %s cells %lld .. %lld on axis %c, outside the allocation's 0 .. %lld", b, who.c_str(),
                   (long long)(l[a] - rm[a]), (long long)(l[a] + e[a] + rp[a] - 1), "xyz"[a], (long long)(size[a] - 1));
+    if (l[a] + e[a] + rp[a] >= (1ll << 31))
+      return fail(SB_ERR_INVALID, "box %d: %s cells %lld .. %lld on axis %c, beyond the kernels' 32-bit coordinates (at most 2^31 - 2)", b,
+                  who.c_str(), (long long)(l[a] - rm[a]), (long long)(l[a] + e[a] + rp[a] - 1), "xyz"[a]);
+  }
   return SB_OK;
 }
 
@@ -2264,7 +2277,13 @@ static int transfer_plan_build(sb_transfer_plan **out, int device, int dtype, in
   }
   if ((rc = stencil_box_reads_ok(0, rl, re, zero, zero, ssize, prolong ? "the prolongation reads coarse" : "the restriction reads fine")) != SB_OK)
     return rc;
-  if (e[0] * e[1] * e[2] >= (1ll << 32)) return fail(SB_ERR_INVALID, "a box of more than 2^32 cells");
+  if (over_2_32_cells(e)) return fail(SB_ERR_INVALID, "a box of more than 2^32 cells");
+  for (int a = 0; a < 3 && prolong; ++a) { // a child's dst coordinate is 2 * (its parent's src coordinate) + off, in int
+    const int64_t off = 2 * src_acc_origin[a] - dst_acc_origin[a];
+    if (off < -(1ll << 31) || off >= (1ll << 31))
+      return fail(SB_ERR_INVALID, "the prolongation's offset 2 * src_acc_origin - dst_acc_origin = %lld on axis %c does not fit 32 bits",
+                  (long long)off, "xyz"[a]);
+  }
 
   DeviceGuard guard(device);
   if (!guard.ok) return fail(SB_ERR_NOGPU, "cannot select CUDA device %d", device);
