@@ -33,7 +33,7 @@ LIBA      := lib/libstencil.a
 # inside libstencil.a would shadow or clash with the real one)
 LIBMPI    := lib/libmpi_shim.a
 
-all: $(SO) $(LIBA) $(LIBMPI) bin/sb_mpirun bin/jacobi3d_b200 bin/test_exchange_multigpu bin/test_boundary_multigpu \
+all: $(SO) $(LIBA) $(LIBMPI) bin/sb_mpirun bin/jacobi3d_b200 bin/test_exchange_multigpu bin/test_exchange_subset_multigpu bin/test_boundary_multigpu \
           bin/test_reduce_multigpu bin/test_stencil_multigpu bin/test_vstencil_multigpu bin/test_system_multigpu \
           bin/test_reduce_exact_multigpu bin/test_colour_multigpu bin/test_mg_multigpu bin/test_multigrid_multigpu bin/test_vmultigrid_multigpu \
           bin/test_krylov_multigpu bin/test_bicgstab_multigpu bin/test_solver_parity
@@ -126,6 +126,12 @@ build/drv/test_exchange_multigpu.o: tests/cpp/test_exchange_multigpu.cu $(wildca
 	@mkdir -p $(dir $@)
 	$(NVCC) $(OWNDRVFLAGS) -c $< -o $@
 bin/test_exchange_multigpu: build/drv/test_exchange_multigpu.o $(LIBA) $(LIBMPI)
+	@mkdir -p bin
+	$(NVCC) $(DRVLINK) -o $@ $< $(LIBA) $(LIBMPI)
+build/drv/test_exchange_subset_multigpu.o: tests/cpp/test_exchange_subset_multigpu.cu $(wildcard include/stencil/*) include/stencil_b200.h
+	@mkdir -p $(dir $@)
+	$(NVCC) $(OWNDRVFLAGS) -c $< -o $@
+bin/test_exchange_subset_multigpu: build/drv/test_exchange_subset_multigpu.o $(LIBA) $(LIBMPI)
 	@mkdir -p bin
 	$(NVCC) $(DRVLINK) -o $@ $< $(LIBA) $(LIBMPI)
 build/drv/test_boundary_multigpu.o: tests/cpp/test_boundary_multigpu.cu $(wildcard include/stencil/*) include/stencil_b200.h

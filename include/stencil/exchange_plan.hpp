@@ -55,12 +55,22 @@ struct Staged {
   int64_t q, offset;
 };
 
+// A subset of a domain's quantities: bit q set = quantity q takes part.  An exchange of a subset moves only the boxes
+// and fills only the BC regions of those quantities; kAllQuantities is the full exchange.  A subset names quantities
+// 0..63 only (a domain with more quantities exchanges them all, or a subset of the first 64).
+using QuantitySet = uint64_t;
+constexpr QuantitySet kAllQuantities = ~QuantitySet(0);
+inline bool in_set(QuantitySet set, size_t q) { return q >= 64 ? set == kAllQuantities : ((set >> q) & 1u) != 0; }
+
 // The layout of the (src -> dst) staging buffer: the messages of messagesFromSrc (= messages_from(src, ...)) bound for
 // dst in their order, the quantities of each in order; a (message, quantity) pair is staged when a row of it is
 // shorter than kStageMaxRowBytes.  Each entry starts at a 16-byte boundary; *total is the end of the last one (0 when
 // nothing is staged).  Whether staging applies at all (src and dst on different GPUs) is the caller's decision.
+// quantities: only the entries of those quantities are returned, at the offsets the full layout gives them, and *total
+// stays the full layout's, so an exchange of any subset uses the full exchange's staging buffers as they are.
 inline std::vector<Staged> staging_layout(const std::vector<Message> &messagesFromSrc, const Dim3 &dst,
-                                          const std::vector<int64_t> &elemSizes, int64_t *total) {
+                                          const std::vector<int64_t> &elemSizes, int64_t *total,
+                                          QuantitySet quantities = kAllQuantities) {
   std::vector<Staged> out;
   int64_t off = 0;
   for (size_t i = 0; i < messagesFromSrc.size(); ++i) {
@@ -70,7 +80,7 @@ inline std::vector<Staged> staging_layout(const std::vector<Message> &messagesFr
       const int64_t es = elemSizes[q];
       if (m.ext.x * es >= kStageMaxRowBytes) continue;
       off = (off + 15) & ~int64_t(15);
-      out.push_back(Staged{i, int64_t(q), off});
+      if (in_set(quantities, q)) out.push_back(Staged{i, int64_t(q), off});
       off += es * int64_t(m.ext.flatten());
     }
   }

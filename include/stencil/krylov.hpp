@@ -128,13 +128,15 @@ protected:
       dd_.queued_ = on;
   }
 
-  // the start of a queued solve: r = f - A x (x's own BC through the exchange)
+  // the start of a queued solve: the coefficient fields exchanged (once per solve: every later exchange moves only the
+  // vector A reads, DESIGN.md section 2.15), then r = f - A x (x's own BC through the exchange)
   void queue_residual() {
     queued(true);
-    dd_.apply(res_, curr(r_), x_, curr(f_), coefs_);
+    if (!coefs_.empty()) dd_.queue_exchange(Multigrid<T>::set_of(coefs_));
+    dd_.apply(res_, curr(r_), x_, curr(f_), coefs_, Multigrid<T>::only(x_));
   }
 
-  void apply_A(DataHandle<T> out, DataHandle<T> src) { dd_.apply(A_, curr(out), src, coefs_); }
+  void apply_A(DataHandle<T> out, DataHandle<T> src) { dd_.apply(A_, curr(out), src, coefs_, Multigrid<T>::only(src)); }
 
   // u = M f: u set to +0 (the cycle's exchanges refill the ghost cells), then one queued cycle on the pair (u, f)
   void precondition(DataHandle<T> u, DataHandle<T> f) {

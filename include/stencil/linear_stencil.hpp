@@ -32,6 +32,29 @@ struct Colour {
   int m = 1, c = 0;
 };
 
+// What an operator call (apply, relax, restrict_to with an op, prolong_from) exchanges before it reads ghost cells
+// (DESIGN.md section 2.15): true (the default) every quantity, false nothing (the caller guarantees the ghost cells),
+// Exchange::reads() only the quantities the call reads at a non-zero offset (src, the coefficient fields a term reads
+// at a non-zero coefficient offset, a system's inputs read at an offset; prolong_from: the coarse src), and
+// Exchange::only(set) the quantities of a bit set (bit q: quantity q), as the solvers use it.
+struct Exchange {
+  enum Mode { kNone, kAll, kReads, kOnly };
+  Mode mode;
+  uint64_t quantities = 0;
+  Exchange(bool all) : mode(all ? kAll : kNone) {} // NOLINT: a bool converts, as the parameter was a bool
+  static Exchange reads() {
+    Exchange e(true);
+    e.mode = kReads;
+    return e;
+  }
+  static Exchange only(uint64_t set) {
+    Exchange e(true);
+    e.mode = kOnly;
+    e.quantities = set;
+    return e;
+  }
+};
+
 // An operator: terms (source, offset, weight) applied in list order, each of which may also read a coefficient field k at
 // an offset of reach 1 (then it contributes (T(w) * C_k) * S).  Terms on aux have offset 0.
 class LinearStencil {

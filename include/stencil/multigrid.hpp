@@ -62,6 +62,7 @@ public:
   // One V(nu1, nu2) cycle, queued after the work on the legacy default stream; returns when it is complete.
   void cycle() {
     set_queued(true);
+    fine_coefs_current();
     vcycle(0);
     finish();
   }
@@ -70,12 +71,15 @@ public:
   void cycle(DataHandle<T> u, DataHandle<T> f) {
     Level &top = pair_level(u, f);
     set_queued(true);
+    fine_coefs_current();
     vcycle(0, &top);
     finish();
   }
 
   // Re-coarsen every level's coefficient fields from the current fine ones, level by level, queued like a cycle with one
-  // host wait.  The constructor calls it once; call it again whenever the fine fields change.
+  // host wait.  The constructor calls it once; call it again whenever the fine fields change.  It then exchanges the
+  // fields of every level: a cycle exchanges only the vector each call reads at an offset (DESIGN.md section 2.15), never
+  // a coefficient field, so after a cycle the ghost cells of the other quantities are not refreshed as a side effect.
   void update_coefficients() {
     set_queued(true);
     for (size_t l = 0; l + 1 < levels_.size(); ++l)
@@ -86,6 +90,9 @@ public:
         else
           F.dd->restrict_to(*C.dd, curr(C.coefs[k]), curr(F.coefs[k]));
       }
+    for (Level &L : levels_)
+      if (!L.coefs.empty()) L.dd->queue_exchange(set_of(L.coefs));
+    coefParity_ = levels_[0].dd->parity_;
     finish();
   }
 
@@ -117,6 +124,7 @@ private:
     std::vector<DataHandle<T>> coefs;
   };
   int nu1_, nu2_, coarse_sweeps_, colours_ = 0;
+  int coefParity_ = -1; // the fine swap parity the coefficient fields were last exchanged in
   DataHandle<T> r_;
   std::vector<Level> levels_;
   std::vector<int> axes_; // per coefficient field: the face axis, or -1 for a cell field
@@ -299,13 +307,31 @@ private:
     return res;
   }
 
+  // the bit set of some quantities (Exchange::only): each exchange of a cycle moves the one vector its call reads at an
+  // offset; the coefficient fields are exchanged by update_coefficients()
+  static uint64_t set_of(const std::vector<DataHandle<T>> &hs) {
+    uint64_t s = 0;
+    for (const DataHandle<T> &h : hs) s |= uint64_t(1) << h.id();
+    return s;
+  }
+  static Exchange only(DataHandle<T> h) { return Exchange::only(uint64_t(1) << h.id()); }
+
+  // after dd.swap() the fine coefficient fields' curr buffers are the other allocation: exchange them once
+  void fine_coefs_current() {
+    Level &L = levels_[0];
+    if (!L.coefs.empty() && coefParity_ != L.dd->parity_) {
+      L.dd->queue_exchange(set_of(L.coefs));
+      coefParity_ = L.dd->parity_;
+    }
+  }
+
   void smooth(Level &L, int sweeps) {
     for (int k = 0; k < sweeps; ++k)
       for (int c = 0; c < colours_; ++c) {
         if (L.coefs.empty())
-          L.dd->apply(L.gs, curr(L.u), L.u, curr(L.f), Colour{colours_, c});
+          L.dd->apply(L.gs, curr(L.u), L.u, curr(L.f), Colour{colours_, c}, only(L.u));
         else
-          L.dd->relax(L.A, curr(L.u), L.u, curr(L.f), L.coefs, Colour{colours_, c}, 1.0);
+          L.dd->relax(L.A, curr(L.u), L.u, curr(L.f), L.coefs, Colour{colours_, c}, 1.0, only(L.u));
       }
   }
 
@@ -318,10 +344,10 @@ private:
     }
     smooth(L, nu1_);
     Level &C = levels_[l + 1];
-    L.dd->restrict_to(*C.dd, curr(C.f), L.res, L.u, curr(L.f), L.coefs);
+    L.dd->restrict_to(*C.dd, curr(C.f), L.res, L.u, curr(L.f), L.coefs, only(L.u));
     C.dd->clear_queued(C.u.id()); // coarse u <- +0
     vcycle(l + 1);
-    L.dd->prolong_from(*C.dd, curr(L.u), curr(C.u), curr(L.u));
+    L.dd->prolong_from(*C.dd, curr(L.u), curr(C.u), curr(L.u), only(C.u));
     smooth(L, nu2_);
   }
 };

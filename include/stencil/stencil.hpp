@@ -107,6 +107,23 @@ private:
   std::vector<void *> stagingBufs_;                  // device allocations (on the receivers' GPUs)
   std::vector<int> stagingDevs_;
   std::vector<cudaEvent_t> phase1Done_;              // one per local domain
+  // exchanges of a quantity subset (DESIGN.md section 2.15): the full plans' box copies, BC quantities and phase-2 copies
+  // per [parity][local domain], each copy with its quantity, from which a subset's plans are cut on its first use and
+  // kept per (parity, set); agreedSets_: the sets every rank has been checked to pass alike
+  struct TaggedCopy {
+    size_t q;
+    sb_box_copy c;
+  };
+  std::vector<std::vector<TaggedCopy>> fullCopies_[2], fullScatter_[2];
+  std::vector<std::vector<sb_bc_quantity>> bcQuantities_[2];
+  struct SubsetPlans {
+    std::vector<sb_copy_plan *> copy, scatter;
+    std::vector<sb_bc_plan *> bc;
+  };
+  std::map<std::pair<int, uint64_t>, SubsetPlans> subsetPlans_;
+  std::set<uint64_t> agreedSets_;
+  const SubsetPlans &subset_plans(uint64_t set);
+  void exchange_async_set(uint64_t set);
   std::vector<RcStream> streams_; // one high-priority stream per local domain
   int parity_;
 
@@ -170,15 +187,18 @@ private:
   void destroy_stencil_plans();
   // omega non-NULL: relax()'s diagonal relaxation (sb_stencil_dplan_create), aq the right-hand side f
   void apply_op(const stencil::LinearStencil &op, int dtype, size_t dq, stencil::Which dw, size_t sq, int64_t aq, stencil::Which aw,
-                const std::vector<size_t> &cq, bool exchange, stencil::Colour colour = stencil::Colour{}, const double *omega = nullptr);
+                const std::vector<size_t> &cq, stencil::Exchange exchange, stencil::Colour colour = stencil::Colour{}, const double *omega = nullptr);
   void apply_sys(const stencil::LinearSystem &sys, int dtype, const std::vector<std::pair<size_t, stencil::Which>> &outs,
-                 const std::vector<std::pair<size_t, stencil::Which>> &ins, bool exchange);
+                 const std::vector<std::pair<size_t, stencil::Which>> &ins, stencil::Exchange exchange);
+  // the bit set an operator call exchanges (0: none): every quantity for true, `reads` for Exchange::reads() (the full
+  // set when it names every quantity), the given set for Exchange::only
+  uint64_t exchange_set(const char *name, const stencil::Exchange &exchange, uint64_t reads) const;
   // the schedule apply_op and apply_sys share: the cached per-domain plans of key (built by make(domain, boxes) on first
   // use), then the interior plans on their own streams while exchange() runs and the exterior plans after it, or the one
   // whole-region plan per domain; returns when every launch is complete.  writes_src: the launch writes src (a coloured
   // apply in place), so the interior also keeps clear of the slabs exchange() sends, which are as wide as the radius on
   // the opposite side.
-  void run_stencil_plans(const std::vector<int64_t> &key, bool exchange, bool writes_src,
+  void run_stencil_plans(const std::vector<int64_t> &key, uint64_t exchange, bool writes_src,
                          const std::function<sb_stencil_plan *(size_t, const std::vector<Rect3> &)> &make);
 
   // The queued schedule (the multigrid solver's, DESIGN.md section 2.11): while queued_ is set, run_stencil_plans and
@@ -194,12 +214,12 @@ private:
   // quantity q's whole curr allocation set to +0 (ghost cells included; an exchange refills them before any read), on
   // each interior apply stream after the previous exterior
   void clear_queued(size_t q);
-  void queue_exchange();
+  void queue_exchange(uint64_t quantities = ~uint64_t(0));
   void wait_exchange(DistributedDomain &other, bool interior);
   void ensure_queue_events();
   // the queued form of the interior / exchange / exterior schedule: launch(domain, part, stream), part 0 the interior (or
   // the whole region without exchange), 1 the exterior
-  void queued_schedule(const std::function<void(size_t, int, cudaStream_t)> &launch, bool exchange);
+  void queued_schedule(const std::function<void(size_t, int, cudaStream_t)> &launch, uint64_t exchange);
 
   // multigrid transfers: per (coarse domain, kind, buffers, the swap parity of both domains), one plan per local domain.
   // serial_ names a domain for the lifetime of the process (an address can be reused by a later domain)
@@ -210,7 +230,8 @@ private:
   // quantities cq; restriction only), with apply's schedule when exchange.  face >= 0: the face-coefficient restriction
   // of the faces normal to that axis (sb_transfer_fplan_create).
   void transfer(DistributedDomain &coarse, bool prolong, int dtype, size_t dq, stencil::Which dw, size_t sq, stencil::Which sw, int64_t aq,
-                stencil::Which aw, bool exchange, const stencil::LinearStencil *op = nullptr, const std::vector<size_t> &cq = {}, int face = -1);
+                stencil::Which aw, stencil::Exchange exchange, const stencil::LinearStencil *op = nullptr, const std::vector<size_t> &cq = {},
+                int face = -1);
   void check_pairing(DistributedDomain &coarse, bool ghosts);
   void destroy_transfer_plans();
   void create_apply_streams(); // two per local domain (interior, exterior), on first use
@@ -323,6 +344,16 @@ public:
   // neighbours; call exchange_wait() (or synchronize all of them) before reading ghost cells
   void exchange_async();
   void exchange_wait();
+  // Exchange of a subset of the quantities (DESIGN.md section 2.15): only their boxes are copied and only their walls'
+  // BCs filled, through the full exchange's kernels and staging buffers; every byte of the other quantities is left as
+  // it was.  A list naming every quantity is the full exchange.  An empty list, a quantity named twice or one that is
+  // not a quantity of this domain (or >= 64) is fatal.  The plans of a subset are built on its first use and kept per
+  // (swap parity, subset); collective like exchange(): every rank passes the same subset, which the first use of each
+  // subset checks with one MPI_Allreduce.
+  void exchange(const std::vector<size_t> &quantities);
+  void exchange_async(const std::vector<size_t> &quantities);
+  // the bit set of a quantity list (fatal on the errors above); every bit set when it names every quantity
+  uint64_t quantity_set(const std::vector<size_t> &quantities) const;
   cudaStream_t exchange_stream(size_t domain) const { return streams_[domain]; }
 
   // Reductions over the whole compute region (DESIGN.md section 2.6), the same bits on every rank.  Each call waits for
@@ -372,12 +403,12 @@ public:
   // ghost cells are current.  Returns when the update is complete.  The plans are kept, per (op, buffers, exchange, swap
   // parity), until the domain is destroyed.
   template <typename T>
-  void apply(const stencil::LinearStencil &op, const stencil::Buffer<T> &dst, const DataHandle<T> &src, bool exchange = true) {
+  void apply(const stencil::LinearStencil &op, const stencil::Buffer<T> &dst, const DataHandle<T> &src, stencil::Exchange exchange = true) {
     apply_op(op, stencil::bc_dtype<T>(), dst.h.id(), dst.which, src.id(), -1, stencil::Which::curr, {}, exchange);
   }
   template <typename T>
   void apply(const stencil::LinearStencil &op, const stencil::Buffer<T> &dst, const DataHandle<T> &src, const stencil::Buffer<T> &aux,
-             bool exchange = true) {
+             stencil::Exchange exchange = true) {
     apply_op(op, stencil::bc_dtype<T>(), dst.h.id(), dst.which, src.id(), int64_t(aux.h.id()), aux.which, {}, exchange);
   }
   // The same with coefficient fields: coefs[k] is field k of the op (op.ncoef() of them), read from its curr buffer, which
@@ -386,12 +417,12 @@ public:
   // curr and next.
   template <typename T>
   void apply(const stencil::LinearStencil &op, const stencil::Buffer<T> &dst, const DataHandle<T> &src, const std::vector<DataHandle<T>> &coefs,
-             bool exchange = true) {
+             stencil::Exchange exchange = true) {
     apply_op(op, stencil::bc_dtype<T>(), dst.h.id(), dst.which, src.id(), -1, stencil::Which::curr, ids_of(coefs), exchange);
   }
   template <typename T>
   void apply(const stencil::LinearStencil &op, const stencil::Buffer<T> &dst, const DataHandle<T> &src, const stencil::Buffer<T> &aux,
-             const std::vector<DataHandle<T>> &coefs, bool exchange = true) {
+             const std::vector<DataHandle<T>> &coefs, stencil::Exchange exchange = true) {
     apply_op(op, stencil::bc_dtype<T>(), dst.h.id(), dst.which, src.id(), int64_t(aux.h.id()), aux.which, ids_of(coefs), exchange);
   }
   // Coloured applies (DESIGN.md section 2.9): only the cells of colour colour.c of the colouring colour.m are written,
@@ -401,22 +432,22 @@ public:
   // Schedule, plan cache (with the colouring in its key) and failure rules are the uncoloured apply's.
   template <typename T>
   void apply(const stencil::LinearStencil &op, const stencil::Buffer<T> &dst, const DataHandle<T> &src, stencil::Colour colour,
-             bool exchange = true) {
+             stencil::Exchange exchange = true) {
     apply_op(op, stencil::bc_dtype<T>(), dst.h.id(), dst.which, src.id(), -1, stencil::Which::curr, {}, exchange, colour);
   }
   template <typename T>
   void apply(const stencil::LinearStencil &op, const stencil::Buffer<T> &dst, const DataHandle<T> &src, const stencil::Buffer<T> &aux,
-             stencil::Colour colour, bool exchange = true) {
+             stencil::Colour colour, stencil::Exchange exchange = true) {
     apply_op(op, stencil::bc_dtype<T>(), dst.h.id(), dst.which, src.id(), int64_t(aux.h.id()), aux.which, {}, exchange, colour);
   }
   template <typename T>
   void apply(const stencil::LinearStencil &op, const stencil::Buffer<T> &dst, const DataHandle<T> &src, const std::vector<DataHandle<T>> &coefs,
-             stencil::Colour colour, bool exchange = true) {
+             stencil::Colour colour, stencil::Exchange exchange = true) {
     apply_op(op, stencil::bc_dtype<T>(), dst.h.id(), dst.which, src.id(), -1, stencil::Which::curr, ids_of(coefs), exchange, colour);
   }
   template <typename T>
   void apply(const stencil::LinearStencil &op, const stencil::Buffer<T> &dst, const DataHandle<T> &src, const stencil::Buffer<T> &aux,
-             const std::vector<DataHandle<T>> &coefs, stencil::Colour colour, bool exchange = true) {
+             const std::vector<DataHandle<T>> &coefs, stencil::Colour colour, stencil::Exchange exchange = true) {
     apply_op(op, stencil::bc_dtype<T>(), dst.h.id(), dst.which, src.id(), int64_t(aux.h.id()), aux.which, ids_of(coefs), exchange, colour);
   }
   // One relaxation pass of A u = f that divides by A's own diagonal (DESIGN.md section 2.12, sb_stencil_dplan_create):
@@ -426,17 +457,17 @@ public:
   //     for (int c = 0; c < 2; ++c) dd.relax(A, stencil::curr(u), u, stencil::curr(f), {kx, ky, kz}, stencil::Colour{2, c});
   template <typename T>
   void relax(const stencil::LinearStencil &A, const stencil::Buffer<T> &dst, const DataHandle<T> &u, const stencil::Buffer<T> &f,
-             const std::vector<DataHandle<T>> &coefs, stencil::Colour colour, double omega = 1.0, bool exchange = true) {
+             const std::vector<DataHandle<T>> &coefs, stencil::Colour colour, double omega = 1.0, stencil::Exchange exchange = true) {
     apply_op(A, stencil::bc_dtype<T>(), dst.h.id(), dst.which, u.id(), int64_t(f.h.id()), f.which, ids_of(coefs), exchange, colour, &omega);
   }
   template <typename T>
   void relax(const stencil::LinearStencil &A, const stencil::Buffer<T> &dst, const DataHandle<T> &u, const stencil::Buffer<T> &f,
-             const std::vector<DataHandle<T>> &coefs, double omega = 1.0, bool exchange = true) {
+             const std::vector<DataHandle<T>> &coefs, double omega = 1.0, stencil::Exchange exchange = true) {
     apply_op(A, stencil::bc_dtype<T>(), dst.h.id(), dst.which, u.id(), int64_t(f.h.id()), f.which, ids_of(coefs), exchange, stencil::Colour{}, &omega);
   }
   template <typename T>
   void relax(const stencil::LinearStencil &A, const stencil::Buffer<T> &dst, const DataHandle<T> &u, const stencil::Buffer<T> &f,
-             stencil::Colour colour, double omega = 1.0, bool exchange = true) {
+             stencil::Colour colour, double omega = 1.0, stencil::Exchange exchange = true) {
     apply_op(A, stencil::bc_dtype<T>(), dst.h.id(), dst.which, u.id(), int64_t(f.h.id()), f.which, {}, exchange, colour, &omega);
   }
 
@@ -447,7 +478,7 @@ public:
   // are the operator apply's.
   template <typename T>
   void apply(const stencil::LinearSystem &sys, const std::vector<stencil::Buffer<T>> &outputs, const std::vector<stencil::Buffer<T>> &inputs,
-             bool exchange = true) {
+             stencil::Exchange exchange = true) {
     std::vector<std::pair<size_t, stencil::Which>> o, i;
     for (const stencil::Buffer<T> &b : outputs) o.emplace_back(b.h.id(), b.which);
     for (const stencil::Buffer<T> &b : inputs) i.emplace_back(b.h.id(), b.which);
@@ -482,12 +513,12 @@ public:
   //     fine.restrict_to(coarse, stencil::curr(f2), residual, u, stencil::curr(f));   // f2 = R (f - A u)
   template <typename T>
   void restrict_to(DistributedDomain &coarse, const stencil::Buffer<T> &dst, const stencil::LinearStencil &op, const DataHandle<T> &src,
-                   const stencil::Buffer<T> &aux, bool exchange = true) {
+                   const stencil::Buffer<T> &aux, stencil::Exchange exchange = true) {
     transfer(coarse, false, stencil::bc_dtype<T>(), dst.h.id(), dst.which, src.id(), stencil::Which::curr, int64_t(aux.h.id()), aux.which, exchange, &op);
   }
   template <typename T>
   void restrict_to(DistributedDomain &coarse, const stencil::Buffer<T> &dst, const stencil::LinearStencil &op, const DataHandle<T> &src,
-                   bool exchange = true) {
+                   stencil::Exchange exchange = true) {
     transfer(coarse, false, stencil::bc_dtype<T>(), dst.h.id(), dst.which, src.id(), stencil::Which::curr, -1, stencil::Which::curr, exchange, &op);
   }
   // restrict_to with a coefficient op (DESIGN.md section 2.12): coefs are op.ncoef() fine quantities (curr buffers,
@@ -495,7 +526,7 @@ public:
   //     fine.restrict_to(coarse, stencil::curr(f2), residual, u, stencil::curr(f), {kx, ky, kz});
   template <typename T>
   void restrict_to(DistributedDomain &coarse, const stencil::Buffer<T> &dst, const stencil::LinearStencil &op, const DataHandle<T> &src,
-                   const stencil::Buffer<T> &aux, const std::vector<DataHandle<T>> &coefs, bool exchange = true) {
+                   const stencil::Buffer<T> &aux, const std::vector<DataHandle<T>> &coefs, stencil::Exchange exchange = true) {
     transfer(coarse, false, stencil::bc_dtype<T>(), dst.h.id(), dst.which, src.id(), stencil::Which::curr, int64_t(aux.h.id()), aux.which, exchange, &op,
              ids_of(coefs));
   }
@@ -507,12 +538,12 @@ public:
     transfer(coarse, false, stencil::bc_dtype<T>(), dst.h.id(), dst.which, src.h.id(), src.which, -1, stencil::Which::curr, false, nullptr, {}, axis);
   }
   template <typename T>
-  void prolong_from(DistributedDomain &coarse, const stencil::Buffer<T> &dst, const stencil::Buffer<T> &src, bool exchange = true) {
+  void prolong_from(DistributedDomain &coarse, const stencil::Buffer<T> &dst, const stencil::Buffer<T> &src, stencil::Exchange exchange = true) {
     transfer(coarse, true, stencil::bc_dtype<T>(), dst.h.id(), dst.which, src.h.id(), src.which, -1, stencil::Which::curr, exchange);
   }
   template <typename T>
   void prolong_from(DistributedDomain &coarse, const stencil::Buffer<T> &dst, const stencil::Buffer<T> &src, const stencil::Buffer<T> &aux,
-                    bool exchange = true) {
+                    stencil::Exchange exchange = true) {
     transfer(coarse, true, stencil::bc_dtype<T>(), dst.h.id(), dst.which, src.h.id(), src.which, int64_t(aux.h.id()), aux.which, exchange);
   }
 

@@ -193,6 +193,13 @@ typedef struct sb_staged {
 int sb_staging_layout(const int64_t dim[3], const int64_t base[3], const int64_t rem[3], const int32_t boundary[3],
                       const int64_t radius27[27], const int64_t src_idx[3], const int64_t dst_idx[3],
                       const int64_t *elem_sizes, int nq, sb_staged *out, int cap, int64_t *total);
+/* sb_staging_layout of an exchange of a subset of the quantities: bit q of quantities set = quantity q is exchanged.
+ * Returns the full layout's entries of those quantities only, at the same offsets, and the same *total, so a subset
+ * exchange packs into the full exchange's staging buffers.  quantities ~0 is sb_staging_layout.  Errors besides
+ * sb_staging_layout's: an empty set, and a bit q >= nq ("quantity q is not one of the nq quantities"). */
+int sb_staging_layout_subset(const int64_t dim[3], const int64_t base[3], const int64_t rem[3], const int32_t boundary[3],
+                             const int64_t radius27[27], const int64_t src_idx[3], const int64_t dst_idx[3],
+                             const int64_t *elem_sizes, int nq, uint64_t quantities, sb_staged *out, int cap, int64_t *total);
 
 /* One quantity of a BC plan: its allocation (the CURRENT buffer the plan will read and write), element type, and
  * per-face kind and value.  dtype RAW takes elem_size 1, 2, 4, 8 or 16 and allows NONE and EVEN only; F32 needs

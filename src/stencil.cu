@@ -93,7 +93,19 @@ void DistributedDomain::destroy_plans() {
     for (sb_bc_plan *p : bcPlans_[parity])
       if (p) sb_bc_plan_destroy(p);
     bcPlans_[parity].clear();
+    fullCopies_[parity].clear();
+    fullScatter_[parity].clear();
+    bcQuantities_[parity].clear();
   }
+  for (auto &kv : subsetPlans_) {
+    for (auto *v : {&kv.second.copy, &kv.second.scatter})
+      for (sb_copy_plan *p : *v)
+        if (p) sb_copy_plan_destroy(p);
+    for (sb_bc_plan *p : kv.second.bc)
+      if (p) sb_bc_plan_destroy(p);
+  }
+  subsetPlans_.clear();
+  agreedSets_.clear();
   bcSenders_.clear();
   for (size_t i = 0; i < stagingBufs_.size(); ++i) {
     cudaSetDevice(stagingDevs_[i]);
@@ -456,6 +468,7 @@ void DistributedDomain::plan_exchange() {
         if (kv.first.first == domainIdx_[di])
           for (const stencil::Staged &st : kv.second.entries) stagedAt[st.msg * nq + size_t(st.q)] = st.offset;
       std::vector<sb_box_copy> copies;
+      std::vector<TaggedCopy> tagged;
       for (size_t i = 0; i < msgs.size(); ++i) {
         const stencil::Message &m = msgs[i];
         const bool sameGpu = gpu_key(m.srcIdx) == gpu_key(m.dstIdx);
@@ -485,6 +498,7 @@ void DistributedDomain::plan_exchange() {
             set3(c.dst_pos, m.dstPos);
           }
           copies.push_back(c);
+          tagged.push_back(TaggedCopy{q, c});
         }
         if (0 == parity) { // attribute the bytes the way the reference's planner picks a transport (src/stencil.cu:383-445)
           const char *how = "";
@@ -510,9 +524,11 @@ void DistributedDomain::plan_exchange() {
         LOG_FATAL("exchange plan: " << sb_last_error());
       }
       plans_[parity].push_back(plan);
+      fullCopies_[parity].push_back(std::move(tagged));
 
       // phase 2 of this subdomain as a receiver
       std::vector<sb_box_copy> scatter;
+      std::vector<TaggedCopy> taggedScatter;
       for (const auto &kv : layouts) {
         if (!(kv.first.second == domainIdx_[di])) continue;
         for (const stencil::Staged &st : kv.second.entries) {
@@ -524,6 +540,7 @@ void DistributedDomain::plan_exchange() {
           set3(c.dst_pos, m.dstPos);
           set3(c.extent, m.ext);
           scatter.push_back(c);
+          taggedScatter.push_back(TaggedCopy{size_t(st.q), c});
         }
       }
       sb_copy_plan *up = nullptr;
@@ -531,6 +548,7 @@ void DistributedDomain::plan_exchange() {
         LOG_FATAL("exchange scatter plan: " << sb_last_error());
       }
       unpackPlans_[parity].push_back(up);
+      fullScatter_[parity].push_back(std::move(taggedScatter));
     }
   }
   plan_boundaries(planFile);
@@ -603,6 +621,7 @@ void DistributedDomain::plan_boundaries(std::ofstream &planFile) {
         plan = nullptr;
       }
       bcPlans_[parity].push_back(plan);
+      bcQuantities_[parity].push_back(qs);
     }
   }
   for (size_t di = 0; di < domains_.size(); ++di) {
@@ -670,7 +689,8 @@ void DistributedDomain::destroy_stencil_plans() {
 }
 
 void DistributedDomain::apply_op(const stencil::LinearStencil &op, int dtype, size_t dq, stencil::Which dw, size_t sq, int64_t aq,
-                                 stencil::Which aw, const std::vector<size_t> &cq, bool exchange, stencil::Colour colour, const double *omega) {
+                                 stencil::Which aw, const std::vector<size_t> &cq, stencil::Exchange exchange, stencil::Colour colour,
+                                 const double *omega) {
   using stencil::Which;
   const char *name = omega ? "relax" : "apply";
   if (domains_.empty() || plans_[0].size() != domains_.size()) LOG_FATAL(name << ": call realize() first");
@@ -700,7 +720,11 @@ void DistributedDomain::apply_op(const stencil::LinearStencil &op, int dtype, si
   const std::vector<sb_stencil_vterm> &terms = op.vterms();
   if (SB_OK != sb_stencil_ccheck(terms.data(), int(terms.size()), r27, colour.m)) LOG_FATAL(name << ": " << sb_last_error());
   if (!op.has_aux() && !omega) aq = -1;
-  std::vector<int64_t> key = {dtype, int64_t(dq), int64_t(dw == Which::next), int64_t(sq), aq, int64_t(aw == Which::next), int64_t(exchange), parity_,
+  uint64_t reads = sq < 64 ? uint64_t(1) << sq : 0; // src and the coefficient fields read at a non-zero offset
+  for (const sb_stencil_vterm &t : terms)
+    if (t.coef >= 0 && (t.coef_offset[0] || t.coef_offset[1] || t.coef_offset[2]) && cq[size_t(t.coef)] < 64) reads |= uint64_t(1) << cq[size_t(t.coef)];
+  const uint64_t xq = exchange_set(name, exchange, reads);
+  std::vector<int64_t> key = {dtype, int64_t(dq), int64_t(dw == Which::next), int64_t(sq), aq, int64_t(aw == Which::next), int64_t(xq != 0), parity_,
                               colour.m, colour.c, int64_t(cq.size())};
   for (const size_t q : cq) key.push_back(int64_t(q));
   if (omega) { // the diagonal mode and omega's bits (the plain key ends with a term's 9 entries, so the two never collide)
@@ -713,7 +737,7 @@ void DistributedDomain::apply_op(const stencil::LinearStencil &op, int dtype, si
     std::memcpy(&wbits, &t.weight, 8);
     key.insert(key.end(), {t.source, t.offset[0], t.offset[1], t.offset[2], t.coef, t.coef_offset[0], t.coef_offset[1], t.coef_offset[2], wbits});
   }
-  run_stencil_plans(key, exchange, dq == sq && dw == Which::curr, [&](size_t di, const std::vector<Rect3> &boxes) {
+  run_stencil_plans(key, xq, dq == sq && dw == Which::curr, [&](size_t di, const std::vector<Rect3> &boxes) {
     LocalDomain &d = domains_[di];
     const sb_pitched dst = as_sb(dw == Which::curr ? d.curr_data(dq) : d.next_data(dq)), src = as_sb(d.curr_data(sq));
     const sb_pitched aux = aq < 0 ? sb_pitched{nullptr, 0, 0} : as_sb(aw == Which::curr ? d.curr_data(size_t(aq)) : d.next_data(size_t(aq)));
@@ -737,7 +761,7 @@ void DistributedDomain::apply_op(const stencil::LinearStencil &op, int dtype, si
 }
 
 void DistributedDomain::apply_sys(const stencil::LinearSystem &sys, int dtype, const std::vector<std::pair<size_t, stencil::Which>> &outs,
-                                  const std::vector<std::pair<size_t, stencil::Which>> &ins, bool exchange) {
+                                  const std::vector<std::pair<size_t, stencil::Which>> &ins, stencil::Exchange exchange) {
   using stencil::Which;
   if (domains_.empty() || plans_[0].size() != domains_.size()) LOG_FATAL("apply: call realize() first");
   if (dtype != SB_DTYPE_F32 && dtype != SB_DTYPE_F64) LOG_FATAL("apply: a stencil system computes in float or double");
@@ -768,7 +792,11 @@ void DistributedDomain::apply_sys(const stencil::LinearSystem &sys, int dtype, c
       for (int x = -1; x <= 1; ++x) r27[i++] = int64_t(radius_.dir(x, y, z));
   if (SB_OK != sb_stencil_sys_check(terms.data(), int(terms.size()), sys.nin(), sys.nout(), r27)) LOG_FATAL("apply: " << sb_last_error());
   // -1 first: a system's key never equals an operator's, whose first entry is a dtype code
-  std::vector<int64_t> key = {-1, dtype, int64_t(exchange), parity_, sys.nin(), sys.nout()};
+  uint64_t reads = 0; // the inputs read at a non-zero offset
+  for (size_t i = 0; i < ins.size(); ++i)
+    if (moved[i] && ins[i].first < 64) reads |= uint64_t(1) << ins[i].first;
+  const uint64_t xq = exchange_set("apply", exchange, reads);
+  std::vector<int64_t> key = {-1, dtype, int64_t(xq != 0), parity_, sys.nin(), sys.nout()};
   for (const auto *v : {&outs, &ins})
     for (const auto &b : *v) key.insert(key.end(), {int64_t(b.first), int64_t(b.second == Which::next)});
   for (const sb_stencil_sys_term &t : terms) {
@@ -776,7 +804,7 @@ void DistributedDomain::apply_sys(const stencil::LinearSystem &sys, int dtype, c
     std::memcpy(&wbits, &t.weight, 8);
     key.insert(key.end(), {t.output, t.input, t.offset[0], t.offset[1], t.offset[2], t.coef, t.coef_offset[0], t.coef_offset[1], t.coef_offset[2], wbits});
   }
-  run_stencil_plans(key, exchange, false, [&](size_t di, const std::vector<Rect3> &boxes) {
+  run_stencil_plans(key, xq, false, [&](size_t di, const std::vector<Rect3> &boxes) {
     LocalDomain &d = domains_[di];
     std::vector<sb_pitched> o, i;
     for (const auto &b : outs) o.push_back(as_sb(b.second == Which::curr ? d.curr_data(b.first) : d.next_data(b.first)));
@@ -796,7 +824,20 @@ void DistributedDomain::apply_sys(const stencil::LinearSystem &sys, int dtype, c
   });
 }
 
-void DistributedDomain::run_stencil_plans(const std::vector<int64_t> &key, bool exchange, bool writes_src,
+uint64_t DistributedDomain::exchange_set(const char *name, const stencil::Exchange &exchange, uint64_t reads) const {
+  const uint64_t all = dataElemSize_.size() >= 64 ? ~uint64_t(0) : (uint64_t(1) << dataElemSize_.size()) - 1;
+  switch (exchange.mode) {
+  case stencil::Exchange::kNone: return 0;
+  case stencil::Exchange::kAll: return stencil::kAllQuantities;
+  case stencil::Exchange::kReads: return reads == all ? stencil::kAllQuantities : reads;
+  case stencil::Exchange::kOnly:
+    if (exchange.quantities & ~all) LOG_FATAL(name << ": Exchange::only names a quantity the domain does not have");
+    return exchange.quantities == all ? stencil::kAllQuantities : exchange.quantities;
+  }
+  return stencil::kAllQuantities;
+}
+
+void DistributedDomain::run_stencil_plans(const std::vector<int64_t> &key, uint64_t exchange, bool writes_src,
                                           const std::function<sb_stencil_plan *(size_t, const std::vector<Rect3> &)> &make) {
   auto found = stencilPlans_.find(key);
   if (found == stencilPlans_.end()) {
@@ -828,7 +869,8 @@ void DistributedDomain::run_stencil_plans(const std::vector<int64_t> &key, bool 
   for (size_t di = 0; di < domains_.size(); ++di)
     if (SB_OK != sb_stencil_plan_launch(plans[di][0], applyStreams_[2 * di])) LOG_FATAL("apply: " << sb_last_error());
   if (exchange) {
-    this->exchange(); // returns when every ghost cell of this rank is filled
+    exchange_async_set(exchange); // and wait: every ghost cell this exchange fills is filled
+    exchange_wait();
     for (size_t di = 0; di < domains_.size(); ++di)
       if (SB_OK != sb_stencil_plan_launch(plans[di][1], applyStreams_[2 * di + 1])) LOG_FATAL("apply: " << sb_last_error());
   }
@@ -874,7 +916,7 @@ void DistributedDomain::clear_queued(size_t q) {
   }
 }
 
-void DistributedDomain::queue_exchange() {
+void DistributedDomain::queue_exchange(uint64_t quantities) {
   ensure_queue_events();
   for (size_t i = 0; i < applyStreams_.size(); ++i) {
     CUDA_RUNTIME(cudaSetDevice(domains_[i / 2].gpu()));
@@ -884,7 +926,7 @@ void DistributedDomain::queue_exchange() {
     CUDA_RUNTIME(cudaSetDevice(domains_[di].gpu()));
     for (cudaEvent_t e : applyEvents_) CUDA_RUNTIME(cudaStreamWaitEvent(streams_[di], e, 0));
   }
-  exchange_async();
+  exchange_async_set(quantities);
 }
 
 void DistributedDomain::wait_exchange(DistributedDomain &other, bool interior) {
@@ -903,9 +945,9 @@ void DistributedDomain::wait_exchange(DistributedDomain &other, bool interior) {
   }
 }
 
-void DistributedDomain::queued_schedule(const std::function<void(size_t, int, cudaStream_t)> &launch, bool exchange) {
+void DistributedDomain::queued_schedule(const std::function<void(size_t, int, cudaStream_t)> &launch, uint64_t exchange) {
   queue_after_exterior();
-  if (exchange) queue_exchange(); // waits for the apply streams as they are before this interior
+  if (exchange) queue_exchange(exchange); // waits for the apply streams as they are before this interior
   for (size_t di = 0; di < domains_.size(); ++di) {
     domains_[di].set_device();
     launch(di, 0, applyStreams_[2 * di]);
@@ -977,7 +1019,8 @@ void DistributedDomain::check_pairing(DistributedDomain &coarse, bool ghosts) {
 }
 
 void DistributedDomain::transfer(DistributedDomain &coarse, bool prolong, int dtype, size_t dq, stencil::Which dw, size_t sq, stencil::Which sw,
-                                 int64_t aq, stencil::Which aw, bool exchange, const stencil::LinearStencil *op, const std::vector<size_t> &cq, int face) {
+                                 int64_t aq, stencil::Which aw, stencil::Exchange exchange, const stencil::LinearStencil *op, const std::vector<size_t> &cq,
+                                 int face) {
   using stencil::Which;
   const char *name = prolong ? "prolong_from" : "restrict_to";
   if (&coarse == this) LOG_FATAL(name << ": coarse must be another DistributedDomain");
@@ -989,7 +1032,9 @@ void DistributedDomain::transfer(DistributedDomain &coarse, bool prolong, int dt
   if (sq >= S.dataDtype_.size() || S.dataDtype_[sq] != dtype) LOG_FATAL(name << ": src " << sq << " is not a quantity of that type");
   if (aq >= 0 && (size_t(aq) >= dataDtype_.size() || dataDtype_[size_t(aq)] != dtype)) LOG_FATAL(name << ": aux " << aq << " is not a quantity of that type");
   if (prolong && sw != Which::curr) LOG_FATAL(name << ": src must be a curr buffer (the one coarse.exchange() fills)");
-  const bool split = op && exchange; // the fused restriction with apply's schedule: interior and exterior plans
+  // what the call exchanges: before a prolongation the coarse src, in a fused restriction the fine src and the
+  // coefficient fields read at a non-zero offset (Exchange::reads()); nothing for a plain restriction
+  uint64_t xq = prolong ? coarse.exchange_set(name, exchange, sq < 64 ? uint64_t(1) << sq : 0) : 0;
   std::vector<int64_t> key = {int64_t(coarse.serial_), int64_t(prolong), int64_t(dq), int64_t(dw == Which::next), int64_t(sq),
                               int64_t(sw == Which::next), aq, int64_t(aw == Which::next), parity_, coarse.parity_};
   if (op) {
@@ -1009,7 +1054,11 @@ void DistributedDomain::transfer(DistributedDomain &coarse, bool prolong, int dt
       key[6] = -1;
       key[7] = 0;
     }
-    key.push_back(int64_t(exchange));
+    uint64_t reads = sq < 64 ? uint64_t(1) << sq : 0;
+    for (const sb_stencil_vterm &t : op->vterms())
+      if (t.coef >= 0 && (t.coef_offset[0] || t.coef_offset[1] || t.coef_offset[2]) && cq[size_t(t.coef)] < 64) reads |= uint64_t(1) << cq[size_t(t.coef)];
+    xq = exchange_set(name, exchange, reads);
+    key.push_back(int64_t(xq != 0));
     if (cq.empty()) {
       for (const sb_stencil_term &t : op->terms()) {
         int64_t wbits;
@@ -1030,6 +1079,7 @@ void DistributedDomain::transfer(DistributedDomain &coarse, bool prolong, int dt
     if (op || prolong) LOG_FATAL(name << ": a face restriction takes no op");
     key.insert(key.end(), {-3, int64_t(face)});
   }
+  const bool split = op && xq; // the fused restriction with apply's schedule: interior and exterior plans
   check_pairing(coarse, prolong);
   auto found = transferPlans_.find(key);
   if (found == transferPlans_.end()) {
@@ -1093,17 +1143,21 @@ void DistributedDomain::transfer(DistributedDomain &coarse, bool prolong, int dt
     if (SB_OK != sb_transfer_plan_launch(plans[per * di + size_t(part)], s)) LOG_FATAL(name << ": " << sb_last_error());
   };
   if (queued_) {
-    if (prolong && exchange) {
-      coarse.queue_exchange();
+    if (prolong && xq) {
+      coarse.queue_exchange(xq);
       wait_exchange(coarse, true);
     }
-    queued_schedule(launch, split);
+    queued_schedule(launch, split ? xq : 0);
     return;
   }
-  if (prolong && exchange) coarse.exchange();
+  if (prolong && xq) {
+    coarse.exchange_async_set(xq);
+    coarse.exchange_wait();
+  }
   for (size_t di = 0; di < domains_.size(); ++di) launch(di, 0, applyStreams_[2 * di]);
   if (split) {
-    this->exchange(); // returns when every ghost cell of this rank is filled
+    exchange_async_set(xq); // and wait: every ghost cell this exchange fills is filled
+    exchange_wait();
     for (size_t di = 0; di < domains_.size(); ++di) launch(di, 1, applyStreams_[2 * di + 1]);
   }
   for (size_t di = 0; di < domains_.size(); ++di) {
@@ -1370,10 +1424,87 @@ std::vector<std::vector<Rect3>> DistributedDomain::get_exterior() const {
 
 const Rect3 DistributedDomain::get_compute_region() const noexcept { return Rect3(Dim3(0, 0, 0), size_); }
 
-void DistributedDomain::exchange_async() {
+uint64_t DistributedDomain::quantity_set(const std::vector<size_t> &quantities) const {
+  if (quantities.empty()) LOG_FATAL("exchange: the quantity list is empty (exchange() exchanges every quantity)");
+  uint64_t set = 0;
+  std::set<size_t> seen;
+  for (const size_t q : quantities) {
+    if (q >= dataElemSize_.size()) LOG_FATAL("exchange: quantity " << q << " is not one of the domain's " << dataElemSize_.size() << " quantities");
+    if (!seen.insert(q).second) LOG_FATAL("exchange: quantity " << q << " is named twice");
+  }
+  if (seen.size() == dataElemSize_.size()) return stencil::kAllQuantities;
+  for (const size_t q : seen) {
+    if (q >= 64) LOG_FATAL("exchange: quantity " << q << ": a subset names quantities 0..63 only");
+    set |= uint64_t(1) << q;
+  }
+  return set;
+}
+
+void DistributedDomain::exchange(const std::vector<size_t> &quantities) {
+  exchange_async(quantities);
+  exchange_wait();
+}
+
+void DistributedDomain::exchange_async(const std::vector<size_t> &quantities) {
+  if (domains_.empty() || plans_[0].size() != domains_.size()) LOG_FATAL("exchange: call realize() first");
+  exchange_async_set(quantity_set(quantities));
+}
+
+const DistributedDomain::SubsetPlans &DistributedDomain::subset_plans(uint64_t set) {
+  const auto key = std::make_pair(parity_, set);
+  auto found = subsetPlans_.find(key);
+  if (found != subsetPlans_.end()) return found->second;
+  if (!agreedSets_.count(set)) { // exchange() is collective: every rank must move the same quantities
+    uint64_t lo = set, hi = set;
+    MPI_Allreduce(MPI_IN_PLACE, &lo, 1, MPI_UINT64_T, MPI_MIN, MPI_COMM_WORLD);
+    MPI_Allreduce(MPI_IN_PLACE, &hi, 1, MPI_UINT64_T, MPI_MAX, MPI_COMM_WORLD);
+    if (lo != set || hi != set)
+      LOG_FATAL("exchange: rank " << rank_ << " exchanges the quantity set 0x" << std::hex << set << ", another rank 0x" << (lo != set ? lo : hi)
+                                  << std::dec << ": every rank must pass the same subset");
+    agreedSets_.insert(set);
+  }
+  SubsetPlans sp;
+  for (size_t di = 0; di < domains_.size(); ++di) {
+    const int dev = domains_[di].gpu();
+    std::vector<sb_box_copy> copies, scatter;
+    for (const TaggedCopy &t : fullCopies_[parity_][di])
+      if (stencil::in_set(set, t.q)) copies.push_back(t.c);
+    for (const TaggedCopy &t : fullScatter_[parity_][di])
+      if (stencil::in_set(set, t.q)) scatter.push_back(t.c);
+    sb_copy_plan *p = nullptr, *u = nullptr;
+    if (SB_OK != sb_copy_plan_create(&p, dev, copies.data(), int64_t(copies.size()))) LOG_FATAL("exchange plan: " << sb_last_error());
+    if (!scatter.empty() && SB_OK != sb_copy_plan_create(&u, dev, scatter.data(), int64_t(scatter.size())))
+      LOG_FATAL("exchange scatter plan: " << sb_last_error());
+    sp.copy.push_back(p);
+    sp.scatter.push_back(u);
+    if (!bcPlans_[parity_].empty()) {
+      std::vector<sb_bc_quantity> qs;
+      for (size_t q = 0; q < bcQuantities_[parity_][di].size(); ++q)
+        if (stencil::in_set(set, q)) qs.push_back(bcQuantities_[parity_][di][q]);
+      int64_t sz[3], r27[27];
+      set3(sz, domains_[di].size());
+      for (int z = -1, i = 0; z <= 1; ++z)
+        for (int y = -1; y <= 1; ++y)
+          for (int x = -1; x <= 1; ++x) r27[i++] = int64_t(radius_.dir(x, y, z));
+      sb_bc_plan *b = nullptr;
+      if (SB_OK != sb_bc_plan_create(&b, dev, qs.data(), int64_t(qs.size()), sz, r27)) LOG_FATAL("boundary conditions: " << sb_last_error());
+      if (0 == sb_bc_plan_bytes(b)) {
+        sb_bc_plan_destroy(b);
+        b = nullptr;
+      }
+      sp.bc.push_back(b);
+    }
+  }
+  return subsetPlans_.emplace(key, std::move(sp)).first->second;
+}
+
+void DistributedDomain::exchange_async() { exchange_async_set(stencil::kAllQuantities); }
+
+void DistributedDomain::exchange_async_set(uint64_t set) {
   nvtxRangePush("DD::exchange_async");
-  const std::vector<sb_copy_plan *> &plans = plans_[parity_];
-  const std::vector<sb_copy_plan *> &scatter = unpackPlans_[parity_];
+  const SubsetPlans *sub = set == stencil::kAllQuantities ? nullptr : &subset_plans(set);
+  const std::vector<sb_copy_plan *> &plans = sub ? sub->copy : plans_[parity_];
+  const std::vector<sb_copy_plan *> &scatter = sub ? sub->scatter : unpackPlans_[parity_];
   const bool ranks = !nbrRanks_.empty();
   if (ranks) {
     ++epoch_;
@@ -1387,7 +1518,7 @@ void DistributedDomain::exchange_async() {
     anyStaged = anyStaged || (scatter[di] != nullptr);
   }
   if (ranks) flags_finish(); // every remote sender's phase 1 has landed (and stream order covers the local ones below)
-  const std::vector<sb_bc_plan *> &bc = bcPlans_[parity_];
+  const std::vector<sb_bc_plan *> &bc = sub ? sub->bc : bcPlans_[parity_];
   if (!ranks && (anyStaged || !bc.empty())) {
     for (size_t di = 0; di < plans.size(); ++di) {
       CUDA_RUNTIME(cudaSetDevice(domains_[di].gpu()));

@@ -200,6 +200,8 @@ _SIGS = {
     "sb_bc_regions": (C.c_int, [I3, I27, I6, C.POINTER(BcRegion), C.c_int]),
     "sb_exchange_messages": (C.c_int, [I3, I3, I3, C.c_int32 * 3, I27, I3, C.POINTER(Message), C.c_int]),
     "sb_staging_layout": (C.c_int, [I3, I3, I3, C.c_int32 * 3, I27, I3, I3, C.POINTER(C.c_int64), C.c_int, C.POINTER(Staged), C.c_int, C.POINTER(C.c_int64)]),
+    "sb_staging_layout_subset": (C.c_int, [I3, I3, I3, C.c_int32 * 3, I27, I3, I3, C.POINTER(C.c_int64), C.c_int, C.c_uint64, C.POINTER(Staged), C.c_int,
+                                           C.POINTER(C.c_int64)]),
     "sb_bc_plan_create": (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.POINTER(BcQuantity), C.c_int64, I3, I27]),
     "sb_bc_plan_launch": (C.c_int, [C.c_void_p, C.c_void_p]),
     "sb_bc_plan_bytes": (C.c_int64, [C.c_void_p]),

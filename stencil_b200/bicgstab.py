@@ -34,7 +34,10 @@ class BiCGStab(_KrylovSolver):
     Multigrid(dd, phat, p, v, op_at, nu1, nu2, coarse_sweeps, levels, coefs, coef_kinds) is M, run on the pair (phat, p)
     and, by Multigrid.cycle(u=shat, f=r), on (shat, r) (v is only the scratch of its residual_norm, which BiCGStab never
     calls).  coefs / coef_kinds: as for Multigrid.  Building, solve(), residual_norm() and update_coefficients() are
-    collective under torchrun.  The solver never calls dd.swap(); a caller may swap between solves."""
+    collective under torchrun.  The solver never calls dd.swap(); a caller may swap between solves.
+    Each exchange of a solve moves only what the pass reads at an offset (x for the residual, the vector A is applied to,
+    u on each V-cycle level; the coefficient fields once per solve), so after a solve the ghost cells of the solver's
+    scratch quantities are no longer refreshed as a side effect (DESIGN.md section 2.15)."""
 
     NAMES = ("x", "f", "r", "r0", "p", "v", "phat", "shat", "t")
 

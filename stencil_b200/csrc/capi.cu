@@ -679,8 +679,18 @@ int sb_exchange_messages(const int64_t dim[3], const int64_t base[3], const int6
 int sb_staging_layout(const int64_t dim[3], const int64_t base[3], const int64_t rem[3], const int32_t boundary[3],
                       const int64_t radius27[27], const int64_t src_idx[3], const int64_t dst_idx[3],
                       const int64_t *elem_sizes, int nq, sb_staged *out, int cap, int64_t *total) {
+  return sb_staging_layout_subset(dim, base, rem, boundary, radius27, src_idx, dst_idx, elem_sizes, nq, stencil::kAllQuantities, out, cap, total);
+}
+
+int sb_staging_layout_subset(const int64_t dim[3], const int64_t base[3], const int64_t rem[3], const int32_t boundary[3],
+                             const int64_t radius27[27], const int64_t src_idx[3], const int64_t dst_idx[3],
+                             const int64_t *elem_sizes, int nq, uint64_t quantities, sb_staged *out, int cap, int64_t *total) {
   static_assert(SB_STAGE_MAX_ROW_BYTES == stencil::kStageMaxRowBytes, "one staging threshold");
   if (!dst_idx || !total || nq < 0 || (nq > 0 && !elem_sizes)) return fail(SB_ERR_INVALID, "bad arguments to sb_staging_layout");
+  if (0 == quantities) return fail(SB_ERR_INVALID, "the quantity subset is empty");
+  if (quantities != stencil::kAllQuantities)
+    for (int q = 0; q < 64; ++q)
+      if (((quantities >> q) & 1u) && q >= nq) return fail(SB_ERR_INVALID, "quantity %d is not one of the %d quantities", q, nq);
   std::vector<stencil::Message> msgs;
   const int rc = exchange_messages(dim, base, rem, boundary, radius27, src_idx, msgs);
   if (rc != SB_OK) return rc;
@@ -688,7 +698,7 @@ int sb_staging_layout(const int64_t dim[3], const int64_t base[3], const int64_t
   for (int q = 0; q < nq; ++q)
     if (elem_sizes[q] <= 0) return fail(SB_ERR_INVALID, "quantity %d: elem_size %lld must be > 0", q, (long long)elem_sizes[q]);
   const std::vector<stencil::Staged> staged =
-      stencil::staging_layout(msgs, d3(dst_idx), std::vector<int64_t>(elem_sizes, elem_sizes + nq), total);
+      stencil::staging_layout(msgs, d3(dst_idx), std::vector<int64_t>(elem_sizes, elem_sizes + nq), total, quantities);
   if (cap < int(staged.size()) || (!staged.empty() && !out))
     return fail(SB_ERR_INVALID, "output capacity %d too small for %zu staged entries", cap, staged.size());
   for (size_t i = 0; i < staged.size(); ++i) out[i] = sb_staged{int64_t(staged[i].msg), staged[i].q, staged[i].offset};

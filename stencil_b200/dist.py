@@ -227,21 +227,23 @@ def messages_from(dd, src_rank: int) -> List[dict]:
     return dd.plan_messages(src_rank)
 
 
-def staging_layout(dd, src_idx, dst_idx):
+def staging_layout(dd, src_idx, dst_idx, qs=None):
     """Messages from subdomain src_idx to subdomain dst_idx (on a DIFFERENT GPU) whose rows are shorter than
     SB_STAGE_MAX_ROW_BYTES (x-faces, x-edges, corners): storing such rows straight into the peer's ghost cells costs one
     tiny NVLink transaction per row (1.6 M 8-byte remote stores per exchange on two GPUs, and a much slower
     interior kernel), so the sender packs them into ONE dense receive buffer in the peer's memory (contiguous 128-byte
     NVLink packets) and the receiver scatters them locally.  Pure geometry (sb_staging_layout): both sides compute the
-    same layout.  Returns (total_bytes, [dict(dir, q, offset, ext, src_pos, dst_pos, es)])."""
-    from .domain import exchange_messages, grid_args
+    same layout.  qs: a sorted tuple of quantities (sb_staging_layout_subset: the full layout's entries of those
+    quantities, at the same offsets), None for all.  Returns (total_bytes, [dict(dir, q, offset, ext, src_pos, dst_pos,
+    es)]); total_bytes is the full layout's."""
+    from .domain import exchange_messages, grid_args, quantity_mask
 
     es = dd._elem_sizes()
     msgs = exchange_messages(dd.partition_, dd.topology_, dd.radius_, src_idx)
     cap = len(msgs) * len(es)
     out, total = (Staged * max(cap, 1))(), C.c_int64(0)
-    n = check(lib().sb_staging_layout(*grid_args(dd.partition_, dd.topology_, dd.radius_), i3(src_idx), i3(dst_idx),
-                                      (C.c_int64 * len(es))(*es), len(es), out, cap, C.byref(total)))
+    n = check(lib().sb_staging_layout_subset(*grid_args(dd.partition_, dd.topology_, dd.radius_), i3(src_idx), i3(dst_idx),
+                                             (C.c_int64 * len(es))(*es), len(es), quantity_mask(qs), out, cap, C.byref(total)))
     entries = []
     for st in out[:n]:
         m = msgs[st.msg]
@@ -267,32 +269,47 @@ class NcclExchange:
     def __init__(self, dd, w: World):
         import torch
 
-        from .domain import CopyPlan, box_copy
-
         self.dd, self.w = dd, w
         self.dev = dd.domains_[0].gpu()
-        es = [d for d in dd.domains_[0].elem_sizes_]
-
-        def layout(msgs):
-            off, entries = 0, []
-            for m in wire_order(msgs):
-                n = m["ext"][0] * m["ext"][1] * m["ext"][2]
-                for q, e in enumerate(es):
-                    off = (off + e - 1) & ~(e - 1)
-                    entries.append((m, q, off))
-                    off += n * e
-            return off, entries
-
-        mine = dd.plan_messages(w.rank)
-        self.peers = sorted({m["dst_rank"] for m in mine} - {w.rank})
-        self.send_buf, self.recv_buf, self.pack, self.unpack = {}, {}, {}, {}
+        self._es = list(dd.domains_[0].elem_sizes_)
+        self._mine = dd.plan_messages(w.rank)
+        self.peers = sorted({m["dst_rank"] for m in self._mine} - {w.rank})
+        self._theirs = {b: [m for m in dd.plan_messages(b) if m["dst_rank"] == w.rank] for b in self.peers}
+        # the buffers of the full exchange; a subset packs into a prefix of them
+        self.send_buf, self.recv_buf = {}, {}
         for b in self.peers:
-            out_total, out_entries = layout([m for m in mine if m["dst_rank"] == b])
-            in_total, in_entries = layout([m for m in dd.plan_messages(b) if m["dst_rank"] == w.rank])
+            out_total, _ = self._layout([m for m in self._mine if m["dst_rank"] == b], None)
+            in_total, _ = self._layout(self._theirs[b], None)
             self.send_buf[b] = torch.empty(max(out_total, 1), dtype=torch.uint8, device=f"cuda:{self.dev}")
             self.recv_buf[b] = torch.empty(max(in_total, 1), dtype=torch.uint8, device=f"cuda:{self.dev}")
-            self.pack[b], self.unpack[b] = [], []
-            for parity in (0, 1):
+        self._plans: Dict[tuple, dict] = {}  # (parity, quantities or None) -> peer -> (pack, unpack, send bytes, recv bytes)
+        for parity in (0, 1):
+            self._plans_for(parity, None)
+        self.bytes_per_exchange = sum(t.numel() for t in self.send_buf.values())
+
+    def _layout(self, msgs: List[dict], qs):
+        """The wire layout of one (src rank -> dst rank) buffer: the messages in wire order, the quantities qs (None: all)
+        of each in order, each at an offset aligned to its element size."""
+        off, entries = 0, []
+        for m in wire_order(msgs):
+            n = m["ext"][0] * m["ext"][1] * m["ext"][2]
+            for q, e in enumerate(self._es):
+                if qs is not None and q not in qs:
+                    continue
+                off = (off + e - 1) & ~(e - 1)
+                entries.append((m, q, off))
+                off += n * e
+        return off, entries
+
+    def _plans_for(self, parity: int, qs) -> dict:
+        from .domain import CopyPlan, box_copy
+
+        key = (parity, qs)
+        if key not in self._plans:
+            dd, es, plans = self.dd, self._es, {}
+            for b in self.peers:
+                out_total, out_entries = self._layout([m for m in self._mine if m["dst_rank"] == b], qs)
+                in_total, in_entries = self._layout(self._theirs[b], qs)
                 pk, up = [], []
                 for m, q, off in out_entries:
                     d = dd.domains_[m["src_slot"]]
@@ -304,29 +321,33 @@ class NcclExchange:
                     dst = Pitched((d._curr0 if parity == 0 else d._next0)[q], d.raw_size()[0] * es[q], d.raw_size()[1])
                     dense = Pitched(self.recv_buf[b].data_ptr() + off, m["ext"][0] * es[q], m["ext"][1])
                     up.append(box_copy(dst, m["dst_pos"], dense, (0, 0, 0), m["ext"], es[q]))
-                self.pack[b].append(CopyPlan(self.dev, pk))
-                self.unpack[b].append(CopyPlan(self.dev, up))
-        self.bytes_per_exchange = sum(t.numel() for t in self.send_buf.values())
+                plans[b] = (CopyPlan(self.dev, pk), CopyPlan(self.dev, up), max(out_total, 1), max(in_total, 1))
+            self._plans[key] = plans
+        return self._plans[key]
 
-    def exchange(self, parity: int, stream) -> None:
+    def exchange(self, parity: int, stream, qs=None) -> None:
+        """Pack, send / receive and unpack the quantities qs (a sorted tuple; None: all) of every message to and from
+        another rank.  Every rank passes the same qs (DistributedDomain.exchange checks it when the plans are built)."""
         import torch
         import torch.distributed as td
 
+        plans = self._plans_for(parity, qs)
         with torch.cuda.stream(stream):
             for b in self.peers:
-                self.pack[b][parity].launch(stream)
+                plans[b][0].launch(stream)
             ops = []
             for b in self.peers:
-                ops.append(td.P2POp(td.isend, self.send_buf[b], b))
-                ops.append(td.P2POp(td.irecv, self.recv_buf[b], b))
+                ops.append(td.P2POp(td.isend, self.send_buf[b][: plans[b][2]], b))
+                ops.append(td.P2POp(td.irecv, self.recv_buf[b][: plans[b][3]], b))
             if ops:
                 for r in td.batch_isend_irecv(ops):
                     r.wait()
             for b in self.peers:
-                self.unpack[b][parity].launch(stream)
+                plans[b][1].launch(stream)
 
     def close(self) -> None:
-        for plans in list(self.pack.values()) + list(self.unpack.values()):
-            for p in plans:
-                p.destroy()
-        self.pack, self.unpack = {}, {}
+        for plans in self._plans.values():
+            for pk, up, _, _ in plans.values():
+                pk.destroy()
+                up.destroy()
+        self._plans = {}

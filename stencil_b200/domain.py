@@ -27,6 +27,7 @@ import ctypes as C
 import dataclasses
 import enum
 import math
+import itertools
 import os
 from typing import Dict, List, Optional, Sequence, Tuple
 
@@ -240,6 +241,18 @@ def exchange_messages(part: Partition, topology: Topology, radius: Radius, src_i
         dict(src_idx=tuple(src_idx), dst_idx=t3(m.dst_idx), dir=t3(m.dir), src_pos=t3(m.src_pos), dst_pos=t3(m.dst_pos), ext=t3(m.extent))
         for m in out[:n]
     ]
+
+
+def quantity_mask(qs) -> int:
+    """The quantity set of sb_staging_layout_subset: bit q for each quantity q of qs (a sorted tuple), every bit for None
+    (all quantities)."""
+    return (1 << 64) - 1 if qs is None else sum(1 << q for q in qs)
+
+
+def op_moved_coefs(op, coef_qs: Sequence[int]) -> List[int]:
+    """The coefficient quantities (coef_qs[k] is field k) that a term of op reads at a non-zero coefficient offset: with
+    the src, what exchange="reads" moves."""
+    return [coef_qs[k] for k in sorted({t[3] for t in op.terms if len(t) == 5 and any(t[4])})]
 
 
 class BCKind(enum.IntEnum):
@@ -813,11 +826,15 @@ def box_copy(dst: Pitched, dst_pos: Vec, src: Pitched, src_pos: Vec, ext: Vec, e
 
 
 # ------------------------------------------------------------------------------------------ DistributedDomain
+_SERIALS = itertools.count()
+
+
 class DistributedDomain:
     """include/stencil/stencil.hpp:33-225 / src/stencil.cu for one NVSwitch node."""
 
     def __init__(self, x: int, y: int, z: int):
         self.size_ = (int(x), int(y), int(z))
+        self._serial = next(_SERIALS)  # names this domain in its handles (picklable, unlike a reference)
         self.radius_ = Radius.constant(0)
         self.dtypes_: List[np.dtype] = []
         self.names_: List[str] = []
@@ -840,6 +857,8 @@ class DistributedDomain:
         self.bcs_: Dict[Tuple[int, int], BC] = {}  # (quantity, face 0..5) -> BC
         self.topology_: Optional[Topology] = None
         self._bc_plans: List[List[Optional[BCPlan]]] = []  # [parity][local domain]
+        self._subset_plans: Dict[tuple, tuple] = {}  # (parity, quantities) -> exchange(only=) plans (_exchange_plans)
+        self._agreed: set = set()  # the subsets every rank has been checked to pass alike
         self._reduce_plans: Dict[tuple, List[ReducePlan]] = {}  # (item keys, parity) -> one plan per local domain
         self._krylov_plans: Dict[tuple, List[KrylovPlan]] = {}  # (mode, quantities, parity) -> one plan per local domain
         self._stencil_plans: Dict[tuple, list] = {}  # (op, buffers, exchange, parity) -> per local domain: plans
@@ -900,7 +919,9 @@ class DistributedDomain:
     def add_data(self, dtype, name: str = "") -> DataHandle:
         self.dtypes_.append(np.dtype(dtype))
         self.names_.append(name)
-        return DataHandle(len(self.dtypes_) - 1, dtype, name)
+        h = DataHandle(len(self.dtypes_) - 1, dtype, name)
+        h._domain = self._serial  # exchange(only=) refuses the handles of another domain
+        return h
 
     def set_methods(self, flags: Method) -> None:
         if (flags & Method.ColoQuantityKernel) and (flags & Method.ColoPackMemcpyUnpack):
@@ -1052,11 +1073,11 @@ class DistributedDomain:
         for key in [k for k in self._recv_local if self._owner[k[0]][0] != self._world.rank]:
             lib().sb_free(C.c_void_p(self._recv_local.pop(key)), self.domains_[0].gpu())
 
-    def _layout(self, src_idx: Vec, dst_idx: Vec) -> Tuple[int, List[dict]]:
-        """dist.staging_layout of the (src -> dst) pair, computed once per realize()."""
+    def _layout(self, src_idx: Vec, dst_idx: Vec, qs=None) -> Tuple[int, List[dict]]:
+        """dist.staging_layout of the (src -> dst) pair for the quantities qs (None: all), computed once per realize()."""
         from . import dist as _dist
 
-        key = (tuple(src_idx), tuple(dst_idx))
+        key = (tuple(src_idx), tuple(dst_idx), qs)
         if key not in self._layouts:
             self._layouts[key] = _dist.staging_layout(self, *key)
         return self._layouts[key]
@@ -1109,62 +1130,19 @@ class DistributedDomain:
         self._owner = {idx: (k // per_rank, k % per_rank) for k, idx in enumerate(self.partition_.indices())}
 
     def _build_plans(self) -> None:
-        """Phase 1 (one launch per local subdomain): every outgoing halo region is stored either straight into the
-        neighbour's ghost cells (same GPU, or wide rows over NVLink) or, for thin rows bound for another GPU, into
-        the neighbour's dense staging buffer.  Phase 2 (one launch per local subdomain that has staged senders):
-        scatter the staging buffers into the ghost cells."""
+        """The exchange plans of every quantity, for both swap parities (_copy_plans), their byte counts and the stream
+        dependencies of phase 2 and of the BC launches."""
         for d in self.domains_:
             d._curr0, d._next0 = list(d.curr_), list(d.next_)
         self._plans, self._unpack_plans = [], []
-        self._bytes_kernel = self._bytes_peer = 0
-        self._staged_bytes = 0
+        self._subset_plans, self._agreed = {}, set()
         msgs = self.plan_messages()
         for parity in (0, 1):
-            plans, unplans = [], []
-            for di, d in enumerate(self.domains_):
-                copies: List[BoxCopy] = []
-                for m in msgs:
-                    if m["src_slot"] != di:
-                        continue
-                    remote = m["dst_rank"] != self._world.rank
-                    if self._use_nccl and remote:
-                        if parity == 0:
-                            self._bytes_peer += sum(d.elem_size(q) for q in range(d.num_data())) * m["ext"][0] * m["ext"][1] * m["ext"][2]
-                        continue  # carried by the NCCL fallback, not by the fused kernel
-                    stage_base = None if self._gpu_key(m["src_idx"]) == self._gpu_key(m["dst_idx"]) else self._staging_target(m["src_idx"], m["dst_idx"])
-                    staged = {}
-                    if stage_base is not None:
-                        staged = {e["q"]: e for e in self._layout(m["src_idx"], m["dst_idx"])[1] if e["dir"] == m["dir"]}
-                    for q in range(d.num_data()):
-                        es = d.elem_size(q)
-                        src_p, _ = self._pitched_of(m["src_idx"], q, parity)
-                        nbytes = es * m["ext"][0] * m["ext"][1] * m["ext"][2]
-                        if q in staged:
-                            dense = Pitched(stage_base + staged[q]["offset"], m["ext"][0] * es, m["ext"][1])
-                            copies.append(box_copy(dense, (0, 0, 0), src_p, m["src_pos"], m["ext"], es))
-                            if parity == 0:
-                                self._staged_bytes += nbytes
-                        else:
-                            dst_p, _ = self._pitched_of(m["dst_idx"], q, parity)
-                            copies.append(box_copy(dst_p, m["dst_pos"], src_p, m["src_pos"], m["ext"], es))
-                        if parity == 0:
-                            if self._gpu_key(m["src_idx"]) == self._gpu_key(m["dst_idx"]):
-                                self._bytes_kernel += nbytes
-                            else:
-                                self._bytes_peer += nbytes
-                plans.append(CopyPlan(d.gpu(), copies))
-                # phase 2 of this subdomain as a receiver
-                ucopies: List[BoxCopy] = []
-                for (src_idx, dst_idx), base in self._recv_local.items():
-                    if dst_idx != tuple(self.domain_idx_[di]):
-                        continue
-                    for e in self._layout(src_idx, dst_idx)[1]:
-                        dst_p, _ = self._pitched_of(dst_idx, e["q"], parity)
-                        dense = Pitched(base + e["offset"], e["ext"][0] * e["es"], e["ext"][1])
-                        ucopies.append(box_copy(dst_p, e["dst_pos"], dense, (0, 0, 0), e["ext"], e["es"]))
-                unplans.append(CopyPlan(d.gpu(), ucopies) if ucopies else None)
+            plans, unplans, count = self._copy_plans(msgs, parity, None)
             self._plans.append(plans)
             self._unpack_plans.append(unplans)
+            if parity == 0:
+                self._bytes_kernel, self._bytes_peer, self._staged_bytes = count
         # in-process senders of each local receiver (for the phase-1 -> phase-2 stream dependency)
         self._stage_senders: List[List[int]] = []
         for di, dst_idx in enumerate(self.domain_idx_):
@@ -1173,37 +1151,157 @@ class DistributedDomain:
                 if d_idx == tuple(dst_idx) and self._owner[src_idx][0] == self._world.rank:
                     snd.add(self._owner[src_idx][1])
             self._stage_senders.append(sorted(snd))
-        self._build_bc_plans()
+        self._bc_senders = []
+        if self.has_boundary_conditions():
+            self._bc_plans = [self._bc_plans_of(parity, None) for parity in (0, 1)]
+            for idx in self.domain_idx_:
+                srcs = {self.topology_.get_neighbor(idx, dv) for dv in ALL_DIRS} - {None}
+                self._bc_senders.append(sorted({self._owner[s][1] for s in srcs if self._owner[s][0] == self._world.rank}))
+        else:
+            self._bc_plans = []
 
-    def _build_bc_plans(self) -> None:
-        """One boundary-condition plan per local subdomain and swap parity (None where the subdomain has no wall face
-        with a BC), and the local subdomains whose phase 1 writes into each one (the BC launch waits for them)."""
-        self._bc_plans, self._bc_senders = [], []
-        if not self.has_boundary_conditions():
-            return
-        for parity in (0, 1):
-            plans = []
-            for di, d in enumerate(self.domains_):
-                idx = self.domain_idx_[di]
-                qs = []
-                for q in range(d.num_data()):
-                    kinds, values = self.wall_kinds(idx, q)
-                    p, _ = self._pitched_of(idx, q, parity)
-                    qs.append(_lib.BcQuantity(p, d.elem_size(q), (C.c_double * 6)(*values), bc_dtype(self.dtypes_[q]), _lib.I6(*kinds)))
-                plan = BCPlan(d.gpu(), qs, d.size(), self.radius_)
-                plans.append(plan if plan.bytes else None)
-            self._bc_plans.append(plans)
-        for idx in self.domain_idx_:
-            srcs = {self.topology_.get_neighbor(idx, dv) for dv in ALL_DIRS} - {None}
-            self._bc_senders.append(sorted({self._owner[s][1] for s in srcs if self._owner[s][0] == self._world.rank}))
+    def _copy_plans(self, msgs: List[dict], parity: int, qs):
+        """The two copy phases of an exchange of the quantities qs (a sorted tuple; None: every quantity) for one swap
+        parity.  Phase 1 (one launch per local subdomain): every outgoing halo region is stored either straight into
+        the neighbour's ghost cells (same GPU, or wide rows over NVLink) or, for thin rows bound for another GPU, into
+        the neighbour's dense staging buffer.  Phase 2 (one launch per local subdomain that has staged senders):
+        scatter the staging buffers into the ghost cells.  A subset stages at the full layout's offsets
+        (dist.staging_layout), so it uses the buffers realize() allocated.  Returns (phase 1 plans, phase 2 plans or
+        None, (same-GPU bytes, cross-GPU bytes, staged bytes))."""
+        plans, unplans = [], []
+        kernel = peer = staged_bytes = 0
+        for di, d in enumerate(self.domains_):
+            mine = range(d.num_data()) if qs is None else qs
+            copies: List[BoxCopy] = []
+            for m in msgs:
+                if m["src_slot"] != di:
+                    continue
+                remote = m["dst_rank"] != self._world.rank
+                if self._use_nccl and remote:
+                    peer += sum(d.elem_size(q) for q in mine) * m["ext"][0] * m["ext"][1] * m["ext"][2]
+                    continue  # carried by the NCCL fallback, not by the fused kernel
+                stage_base = None if self._gpu_key(m["src_idx"]) == self._gpu_key(m["dst_idx"]) else self._staging_target(m["src_idx"], m["dst_idx"])
+                staged = {}
+                if stage_base is not None:
+                    staged = {e["q"]: e for e in self._layout(m["src_idx"], m["dst_idx"], qs)[1] if e["dir"] == m["dir"]}
+                for q in mine:
+                    es = d.elem_size(q)
+                    src_p, _ = self._pitched_of(m["src_idx"], q, parity)
+                    nbytes = es * m["ext"][0] * m["ext"][1] * m["ext"][2]
+                    if q in staged:
+                        dense = Pitched(stage_base + staged[q]["offset"], m["ext"][0] * es, m["ext"][1])
+                        copies.append(box_copy(dense, (0, 0, 0), src_p, m["src_pos"], m["ext"], es))
+                        staged_bytes += nbytes
+                    else:
+                        dst_p, _ = self._pitched_of(m["dst_idx"], q, parity)
+                        copies.append(box_copy(dst_p, m["dst_pos"], src_p, m["src_pos"], m["ext"], es))
+                    if self._gpu_key(m["src_idx"]) == self._gpu_key(m["dst_idx"]):
+                        kernel += nbytes
+                    else:
+                        peer += nbytes
+            plans.append(CopyPlan(d.gpu(), copies))
+            # phase 2 of this subdomain as a receiver
+            ucopies: List[BoxCopy] = []
+            for (src_idx, dst_idx), base in self._recv_local.items():
+                if dst_idx != tuple(self.domain_idx_[di]):
+                    continue
+                for e in self._layout(src_idx, dst_idx, qs)[1]:
+                    dst_p, _ = self._pitched_of(dst_idx, e["q"], parity)
+                    dense = Pitched(base + e["offset"], e["ext"][0] * e["es"], e["ext"][1])
+                    ucopies.append(box_copy(dst_p, e["dst_pos"], dense, (0, 0, 0), e["ext"], e["es"]))
+            unplans.append(CopyPlan(d.gpu(), ucopies) if ucopies else None)
+        return plans, unplans, (kernel, peer, staged_bytes)
+
+    def _bc_plans_of(self, parity: int, qs) -> List[Optional[BCPlan]]:
+        """One boundary-condition plan per local subdomain over the quantities qs (None: all), for one swap parity (None
+        where the subdomain has no wall face with a BC of those quantities)."""
+        plans = []
+        for di, d in enumerate(self.domains_):
+            idx = self.domain_idx_[di]
+            bq = []
+            for q in range(d.num_data()) if qs is None else qs:
+                kinds, values = self.wall_kinds(idx, q)
+                p, _ = self._pitched_of(idx, q, parity)
+                bq.append(_lib.BcQuantity(p, d.elem_size(q), (C.c_double * 6)(*values), bc_dtype(self.dtypes_[q]), _lib.I6(*kinds)))
+            plan = BCPlan(d.gpu(), bq, d.size(), self.radius_)
+            plans.append(plan if plan.bytes else None)
+        return plans
 
     # -- the hot path
-    def exchange_async(self) -> None:
-        """Enqueue the halo exchange on the library's high-priority streams (one per local subdomain)."""
+    def exchange_key(self, only) -> Optional[Tuple[int, ...]]:
+        """The quantities exchange(only=only) moves, as a sorted tuple of quantity indices; None for every quantity (only
+        is None, or names every quantity of the domain).  Refuses (StencilError) an empty subset, a quantity named twice
+        and anything that is not a DataHandle of this domain.  Host only."""
+        if only is None:
+            return None
+        if isinstance(only, DataHandle):
+            raise _lib.StencilError("exchange: only must be a sequence of DataHandles (or None), not one DataHandle")
+        qs = []
+        for h in only:
+            owner = getattr(h, "_domain", None)
+            if not isinstance(h, DataHandle) or not 0 <= h.id < len(self.dtypes_) or (owner is not None and owner != self._serial):
+                raise _lib.StencilError(f"exchange: {h!r} is not a DataHandle of this domain")
+            if h.id in qs:
+                raise _lib.StencilError(f"exchange: quantity {h.id} ({self.names_[h.id] or 'unnamed'}) is named twice")
+            qs.append(h.id)
+        if not qs:
+            raise _lib.StencilError("exchange: only names no quantity (None exchanges every quantity)")
+        if len(qs) == len(self.dtypes_):
+            return None
+        if max(qs) >= 64:
+            raise _lib.StencilError(f"exchange: quantity {max(qs)}: a subset names quantities 0..63 only")
+        return tuple(sorted(qs))
+
+    def _agree_on_subset(self, qs: Tuple[int, ...]) -> None:
+        """exchange() is collective, so every rank must exchange the same quantities: checked once per subset, when its
+        plans are first built (one all_gather_object), never on later calls."""
+        if qs in self._agreed:
+            return
+        if self._world.size > 1:
+            from . import dist as _dist
+
+            everyone = _dist.all_gather_object(qs)
+            for r, theirs in enumerate(everyone):
+                if tuple(theirs) != qs:
+                    raise _lib.StencilError(f"exchange: rank {r} exchanges quantities {list(theirs)}, rank {self._world.rank} "
+                                            f"{list(qs)}: every rank must pass the same subset")
+        self._agreed.add(qs)
+
+    def _exchange_plans(self, qs):
+        """(phase 1, phase 2, BC plans or None) of an exchange of qs (None: every quantity) for the current swap parity;
+        a subset's are built on first use and kept per (swap parity, subset) until close()."""
+        parity = self._parity
+        if qs is None:
+            return self._plans[parity], self._unpack_plans[parity], self._bc_plans[parity] if self._bc_plans else None
+        key = (parity, qs)
+        if key not in self._subset_plans:
+            self._agree_on_subset(qs)
+            plans, unplans, _ = self._copy_plans(self.plan_messages(), parity, qs)
+            bcs = self._bc_plans_of(parity, qs) if self._bc_plans else None
+            if bcs is not None and all(b is None for b in bcs):
+                bcs = None
+            self._subset_plans[key] = (plans, unplans, bcs)
+        return self._subset_plans[key]
+
+    def exchange_bytes(self, only=None) -> int:
+        """Bytes the first copy phase of one exchange(only=only) moves on this rank (the box copies of every local
+        subdomain, staged rows included); the messages the NCCL fallback carries and the ghost bytes of the BC fill are
+        not counted.  For a subset not used yet it builds the subset's plans, which is collective under torchrun like
+        exchange() itself: every rank calls it with the same subset."""
+        plans, _, _ = self._exchange_plans(self.exchange_key(only))
+        return sum(p.bytes for p in plans)
+
+    def exchange_async(self, only=None) -> None:
+        """Enqueue the halo exchange on the library's high-priority streams (one per local subdomain).  only: the
+        quantities to exchange, a sequence of DataHandles of this domain (see exchange()); None: every quantity."""
+        if self.partition_ is None or not self._plans:
+            raise _lib.StencilError("exchange: call realize() first")
+        self._exchange_async(self.exchange_key(only))
+
+    def _exchange_async(self, qs) -> None:
         import torch
 
-        plans, unplans = self._plans[self._parity], self._unpack_plans[self._parity]
-        bcs = self._bc_plans[self._parity] if self._bc_plans else None
+        plans, unplans, bcs = self._exchange_plans(qs)
         if self._remote is not None:
             self._epoch += 1
             self._remote.begin(self._epoch, self._streams)
@@ -1222,7 +1320,7 @@ class DistributedDomain:
                 for o in self._streams[1:]:
                     o.wait_event(ev0)
         if self._nccl is not None:
-            self._nccl.exchange(self._parity, self._streams[0])
+            self._nccl.exchange(self._parity, self._streams[0], qs)
         # phase 2: scatter what other GPUs staged for my subdomains
         if any(u is not None for u in unplans):
             events = {}
@@ -1257,12 +1355,44 @@ class DistributedDomain:
                     s.wait_event(nccl_done)
                 b.launch(s)
 
-    def exchange(self) -> None:
+    def exchange(self, only=None) -> None:
         """DistributedDomain::exchange (src/stencil.cu:1002-1186): returns when every ghost cell of
-        every local subdomain holds its neighbour's current value."""
-        self.exchange_async()
+        every local subdomain holds its neighbour's current value.
+
+        only: a sequence of DataHandles of this domain (DESIGN.md section 2.15).  Only those quantities' boxes are
+        copied and only their walls' boundary conditions filled, with the same kernels, staging buffers and ordering as
+        the full exchange; every byte of the other quantities, ghost cells included, is left as it was.  None, or every
+        quantity, is the full exchange.  An empty subset, a quantity named twice or a handle of another domain is a
+        StencilError.  The plans of a subset are built on its first use and kept per (swap parity, subset) until close().
+        Under torchrun the exchange is collective and every rank passes the same subset: the first use of each subset
+        checks that with one all_gather_object (later calls do not).
+            dd.exchange(only=[u])          # before a sweep that reads u at an offset and f at offset 0"""
+        self.exchange_async(only)
         for d, s in zip(self.domains_, self._streams):
             check(lib().sb_stream_sync(d.gpu(), stream_ptr(s)))
+
+    def _exchange_sync(self, exchange) -> None:
+        """exchange() of what _exchange_sel returned (True: every quantity, or a tuple of quantities)."""
+        self._exchange_async(None if exchange is True else exchange)
+        for d, s in zip(self.domains_, self._streams):
+            check(lib().sb_stream_sync(d.gpu(), stream_ptr(s)))
+
+    def _exchange_sel(self, name: str, exchange, reads) -> object:
+        """What an operator call exchanges: False (nothing), True (every quantity) or a sorted tuple of quantities.
+        exchange: a bool, "reads" (the quantities of `reads`, those the call reads at a non-zero offset; none of them
+        means no exchange, all of them the full exchange), or a tuple of DataHandles of this domain (the solvers: the
+        vector the call reads at an offset, its coefficient fields exchanged when they change)."""
+        if isinstance(exchange, str) and exchange == "reads":
+            qs = set(reads)
+        elif isinstance(exchange, tuple):
+            qs = {h.id for h in exchange}
+        elif isinstance(exchange, str):
+            raise _lib.StencilError(f"{name}: exchange must be True, False or 'reads', not {exchange!r}")
+        else:
+            return bool(exchange)  # any other value by its truth, as before "reads" existed
+        if not qs:
+            return False
+        return True if len(qs) == len(self.dtypes_) else tuple(sorted(qs))
 
     def exchange_streams(self):
         return self._streams
@@ -1420,7 +1550,7 @@ class DistributedDomain:
         return self._exact_gather([(idx, plan.parts(s)) for idx, plan, s in zip(self.domain_idx_, plans, self._streams)], 1)[0].sum
 
     # -- linear stencil operators
-    def apply(self, op, dst, src, aux=None, exchange: bool = True, coefs=None, colour=None) -> None:
+    def apply(self, op, dst, src, aux=None, exchange=True, coefs=None, colour=None) -> None:
         """dst = op(src, aux, coefs) over the whole compute region of every local subdomain (DESIGN.md section 2.7).
 
         Buffers are (DataHandle, "curr" | "next"); a bare handle means "next" for dst and "curr" for src and aux.  src is
@@ -1431,9 +1561,11 @@ class DistributedDomain:
         compute cells in curr and next.
         exchange=True: the interior runs on its own stream while exchange() fills the ghost cells, then the exterior slabs
         of each subdomain run as one launch; exchange=False: one launch over the whole region, and the caller guarantees
-        the ghost cells are current.  Returns when the update is complete.  The plans are built on first use and kept,
-        per (op, buffers, exchange, swap parity, colour), until close().  Under torchrun every rank calls it (exchange() is
-        collective).
+        the ghost cells are current; exchange="reads": the schedule of True, with an exchange of only the quantities the
+        call reads at a non-zero offset (exchange(only=...), DESIGN.md section 2.15): src, and each coefficient field
+        that a term reads at a non-zero coefficient offset.  Returns when the update is complete.  The plans are built
+        on first use and kept, per (op, buffers, exchange, swap parity, colour), until close().  Under torchrun every
+        rank calls it (exchange() is collective).
         colour=(m, c), m in 1, 2, 8 (DESIGN.md section 2.9): only the cells of colour c of the colouring m (taken from global
         coordinates) are written, each from the buffers as they were before the call, and with m > 1 dst may be src, so
         a Gauss-Seidel / SOR sweep is one call per colour:
@@ -1445,14 +1577,15 @@ class DistributedDomain:
         no cell exchange() sends (a slab as wide as the opposite side's radius); the exterior runs after exchange()."""
         self._run_plans(*self._apply_plans(op, dst, src, aux, exchange, coefs, colour))
 
-    def relax(self, A, dst, u, f, coefs=None, colour=None, omega: float = 1.0, exchange: bool = True) -> None:
+    def relax(self, A, dst, u, f, coefs=None, colour=None, omega: float = 1.0, exchange=True) -> None:
         """One relaxation pass of A u = f that divides by A's own diagonal (DESIGN.md section 2.12): dst[p] = u(p) +
         omega ((f(p) - (A u)(p)) / d(p)), d(p) the sum of the factors (weight, times the coefficient for a coefficient
         term) of A's terms at offset 0, for the cells of colour c of colour=(m, c) (None: every cell, weighted Jacobi,
         dst must not be u).  A has src terms only (plain or coefficient terms) and at least one term at offset 0; for
         div(kappa grad u) the diagonal differs from cell to cell, which A.relax(omega) cannot express.  Buffers, coefs,
-        the colour condition, the schedule, the in-place interior cut and the plan cache are apply()'s, with u as src and
-        f as aux; omega joins the plan key.  A red-black Gauss-Seidel sweep of -div(kappa grad u) = f:
+        the colour condition, the schedule (exchange="reads" included: u and the coefficients read at an offset, f is
+        read at offset 0), the in-place interior cut and the plan cache are apply()'s, with u as src and f as aux; omega
+        joins the plan key.  A red-black Gauss-Seidel sweep of -div(kappa grad u) = f:
             A = StencilOp.div_grad((h, h, h), np.float64).scaled(-1.0)
             for c in range(2):
                 dd.relax(A, (u, "curr"), u, f, coefs=[kx, ky, kz], colour=(2, c))
@@ -1461,7 +1594,7 @@ class DistributedDomain:
             raise _lib.StencilError(f"relax: omega = {omega} must be finite")
         self._run_plans(*self._apply_plans(A, dst, u, f, exchange, coefs, colour, omega=float(omega)))
 
-    def _apply_plans(self, op, dst, src, aux=None, exchange: bool = True, coefs=None, colour=None, omega=None):
+    def _apply_plans(self, op, dst, src, aux=None, exchange=True, coefs=None, colour=None, omega=None):
         """apply()'s checks and cached plans, returned with its schedule as the arguments of _run_plans.  omega: relax()'s
         plans (aux is f)."""
         from .stencil_op import StencilOp, StencilPlan
@@ -1512,6 +1645,7 @@ class DistributedDomain:
             c_q.append(q)
         op.check(self.radius_, colours=ncol)
         reads_aux = op.has_aux or omega is not None
+        exchange = self._exchange_sel(name, exchange, [s_q] + op_moved_coefs(op, c_q))
         key = (op.key(), (d_q, d_w), s_q, a if reads_aux else None, tuple(c_q), bool(exchange), self._parity, (ncol, col))
         if omega is not None:
             key += ("diag", omega)
@@ -1523,7 +1657,7 @@ class DistributedDomain:
 
         return self._plans_for(key, exchange, make, writes_src=(d_q, d_w) == (s_q, s_w)), exchange
 
-    def apply_system(self, system, outputs, inputs, exchange: bool = True) -> None:
+    def apply_system(self, system, outputs, inputs, exchange=True) -> None:
         """outputs = system(inputs) over the whole compute region of every local subdomain (DESIGN.md section 2.8).
 
         outputs: system.nout buffers, inputs: system.nin buffers, each (DataHandle, "curr" | "next"); a bare handle means
@@ -1531,7 +1665,8 @@ class DistributedDomain:
         type.  An input read at a non-zero offset (as a source or a coefficient) must be a curr buffer, the one
         exchange() fills.  Outputs are pairwise distinct; an output may be an input only if every read of that input is
         at offset 0 (an in-place update such as E = E + dt curl H).
-        The schedule, the plan cache (per system, buffers, exchange and swap parity) and the torchrun rule are apply()'s."""
+        The schedule, the plan cache (per system, buffers, exchange and swap parity) and the torchrun rule are apply()'s;
+        exchange="reads" exchanges the inputs of system.moved_inputs() only."""
         from .stencil_op import StencilSystem, SystemPlan
 
         if not isinstance(system, StencilSystem):
@@ -1571,6 +1706,7 @@ class DistributedDomain:
                 if ins[i] == o:
                     raise _lib.StencilError(f"apply_system: output {j} is input {i}, which is read at a non-zero offset")
         system.check(self.radius_)
+        exchange = self._exchange_sel("apply_system", exchange, [ins[i][0] for i in moved])
         key = ("system", system.key(), tuple(outs), tuple(ins), bool(exchange), self._parity)
 
         def make(di, d, boxes):
@@ -1614,7 +1750,7 @@ class DistributedDomain:
                 if multi:
                     _set_current_device(d.gpu())
                 p[0].launch(si)
-            self.exchange()  # returns when every ghost cell of every local subdomain is filled
+            self._exchange_sync(exchange)  # returns when every ghost cell it fills is filled
             for d, p, (_, se) in zip(self.domains_, plans, self._apply_streams):
                 if multi:
                     _set_current_device(d.gpu())
@@ -1660,7 +1796,7 @@ class DistributedDomain:
             pair[1].record(se)
             si.wait_event(pair[1])
         if exchange:
-            self._queue_exchange()
+            self._queue_exchange(exchange)
         for d, p, (si, _) in zip(self.domains_, plans, self._apply_streams):
             if multi:
                 _set_current_device(d.gpu())
@@ -1683,10 +1819,11 @@ class DistributedDomain:
             self._queue_ev = ev
         return ev
 
-    def _queue_exchange(self) -> None:
+    def _queue_exchange(self, exchange=True) -> None:
         """exchange() without a host wait.  Every exchange stream first waits for every local apply stream, on every GPU
         of the process: the exchange then neither sends a value still being written nor overwrites a ghost cell an
-        earlier launch still reads, and across ranks the exchange signals its neighbours only after those waits."""
+        earlier launch still reads, and across ranks the exchange signals its neighbours only after those waits.
+        exchange: what _exchange_sel returned (True: every quantity, or a tuple of quantities)."""
         apply_ev, _ = self._queue_events()
         for pair, evs in zip(self._apply_streams, apply_ev):
             for st, ev in zip(pair, evs):
@@ -1695,7 +1832,7 @@ class DistributedDomain:
             for evs in apply_ev:
                 for ev in evs:
                     x.wait_event(ev)
-        self.exchange_async()
+        self._exchange_async(None if exchange is True else exchange)
 
     def _wait_exchange(self, other: "DistributedDomain", interior: bool = True) -> None:
         """Every exterior apply stream of this domain (and every interior one with interior=True) waits for the
@@ -1710,7 +1847,7 @@ class DistributedDomain:
                     si.wait_event(ev)
 
     # -- multigrid transfers
-    def restrict_to(self, coarse: "DistributedDomain", dst, src, op=None, aux=None, exchange: bool = True, coefs=None, face=None) -> None:
+    def restrict_to(self, coarse: "DistributedDomain", dst, src, op=None, aux=None, exchange=True, coefs=None, face=None) -> None:
         """dst (a quantity of coarse) = the 8-cell average of src (a quantity of this domain) over every coarse compute
         cell (DESIGN.md section 2.10).  Buffers follow apply(): a bare handle means "next" for dst and "curr" for src;
         src may be curr or next, as restriction reads no ghost cells.  coarse must pair with this domain: the same
@@ -1723,7 +1860,8 @@ class DistributedDomain:
         src must then be a curr buffer, as op reads its ghost cells; aux (a bare handle means "curr") is needed when a
         term reads it.  exchange=True follows apply(): the coarse interior (the coarse compute region cut by 1, which
         reads no fine ghost cell) runs while exchange() fills the ghost cells, then the exterior slabs; exchange=False:
-        one launch over the whole region, the caller guarantees the ghost cells.  The op is part of the plan key.
+        one launch over the whole region, the caller guarantees the ghost cells; exchange="reads": only src and the
+        coefficient fields the op reads at a non-zero offset are exchanged.  The op is part of the plan key.
             fine.restrict_to(coarse, (f2, "curr"), u, op=residual, aux=(f, "curr"))   # f2 = R (f - A u)
         An op with coefficient terms takes coefs, as apply() does (op.ncoef DataHandles of this domain, curr buffers,
         exchanged like src); the result is the bits of apply() into a scratch quantity followed by restrict_to()
@@ -1745,18 +1883,19 @@ class DistributedDomain:
         else:
             self._transfer(coarse, _lib.TRANSFER_RESTRICT, dst, src, aux, exchange, op, coefs=coefs)
 
-    def prolong_from(self, coarse: "DistributedDomain", dst, src, aux=None, exchange: bool = True) -> None:
+    def prolong_from(self, coarse: "DistributedDomain", dst, src, aux=None, exchange=True) -> None:
         """dst = aux + P src (or P src without aux) over every fine compute cell, P the trilinear interpolation from the
         coarse grid (DESIGN.md section 2.10).  dst and aux are quantities of this domain (bare handles: "next" and
         "curr"); aux may be dst, which gives the in-place correction u <- u + P e.  src is a quantity of coarse and must
         be a curr buffer: its ghost cells are read.  exchange=True runs coarse.exchange() first (collective: every rank
-        calls it), with exchange=False the caller guarantees the coarse ghost cells.  The coarse radius must be >= 1 in
+        calls it), with exchange=False the caller guarantees the coarse ghost cells, exchange="reads" exchanges the coarse
+        src only (coarse.exchange(only=[src])).  The coarse radius must be >= 1 in
         all 26 directions.  Plans are built on first use and kept, per (coarse domain, kind, buffers, the swap parity
         of both domains), until close().
             fine.prolong_from(coarse, (u, "curr"), (e, "curr"), aux=(u, "curr"))"""
         self._transfer(coarse, _lib.TRANSFER_PROLONG, dst, src, aux, exchange)
 
-    def _transfer(self, coarse, kind: int, dst, src, aux, exchange: bool, op=None, queued: bool = False, coefs=None, face=None) -> None:
+    def _transfer(self, coarse, kind: int, dst, src, aux, exchange, op=None, queued: bool = False, coefs=None, face=None) -> None:
         """restrict_to / prolong_from; queued: the schedule of _run_plans(queued=True), for a solver that owns the cycle;
         coefs: the fine coefficient quantities of a coefficient op; face: the axis of a face restriction."""
         from .stencil_op import StencilOp
@@ -1805,6 +1944,10 @@ class DistributedDomain:
             op.check(self.radius_)
             a = a if op.has_aux else None
         self._check_pairing(coarse, not restrict)
+        if restrict:
+            exchange = self._exchange_sel(name, exchange, [s[0]] + op_moved_coefs(op, c_q)) if op is not None else False
+        else:
+            exchange = coarse._exchange_sel(name, exchange, [s[0]])
         fused_exchange = op is not None and bool(exchange)
         key = (coarse, kind, d, s, a, self._parity, coarse._parity) + ((op.key(), fused_exchange, tuple(c_q)) if op is not None else ())
         if face is not None:
@@ -1836,11 +1979,11 @@ class DistributedDomain:
             self._transfer_plans[key] = plans
         if not restrict and exchange:
             if queued:
-                coarse._queue_exchange()
+                coarse._queue_exchange(exchange)
                 self._wait_exchange(coarse)
             else:
-                coarse.exchange()
-        self._run_plans(plans, fused_exchange, queued)
+                coarse._exchange_sync(exchange)
+        self._run_plans(plans, exchange if fused_exchange else False, queued)
 
     def _check_pairing(self, coarse, ghosts: bool) -> None:
         """The pairing of sb_transfer_check over every subdomain index (global information, so every rank reaches the same
@@ -1883,11 +2026,12 @@ class DistributedDomain:
             for p in plans:
                 p.destroy()
         self._krylov_plans = {}
-        for plans in self._plans + getattr(self, "_unpack_plans", []) + self._bc_plans:
+        subset = [plans for per_key in self._subset_plans.values() for plans in per_key if plans is not None]
+        for plans in self._plans + getattr(self, "_unpack_plans", []) + self._bc_plans + subset:
             for p in plans:
                 if p is not None:
                     p.destroy()
-        self._plans, self._unpack_plans, self._bc_plans = [], [], []
+        self._plans, self._unpack_plans, self._bc_plans, self._subset_plans = [], [], [], {}
 
         if self._remote is not None:
             self._remote.close()

@@ -111,13 +111,17 @@ class _KrylovSolver:
         return [red.sum for red in dd._exact_gather(mine, sum(plans[0].n for plans in launched))]
 
     def _apply_A(self, out: DataHandle, src: DataHandle) -> None:
-        self.dd._run_plans(*self.dd._apply_plans(self.A, (out, "curr"), src, None, True, self.coefs), queued=True)
+        self.dd._run_plans(*self.dd._apply_plans(self.A, (out, "curr"), src, None, (src,), self.coefs), queued=True)
 
     def _residual(self) -> None:
-        """r = f - A x with x's own BC through the exchange, queued after the work on the caller's stream."""
+        """r = f - A x with x's own BC through the exchange, queued after the work on the caller's stream.  The first pass
+        of a solve: the coefficient fields are exchanged here, once per solve, as every later exchange moves only the
+        vector A reads (DESIGN.md section 2.15)."""
         dd = self.dd
         dd._follow_caller()
-        dd._run_plans(*dd._apply_plans(self.res, (self.r, "curr"), self.x, (self.f, "curr"), True, self.coefs), queued=True)
+        if self.coefs:
+            dd._queue_exchange(dd._exchange_sel(type(self).__name__, tuple(self.coefs), ()))
+        dd._run_plans(*dd._apply_plans(self.res, (self.r, "curr"), self.x, (self.f, "curr"), (self.x,), self.coefs), queued=True)
 
     def _precondition(self, u: DataHandle, f: DataHandle) -> None:
         """u = M f: u set to +0, then one cycle on the pair (u, f), queued."""
@@ -150,7 +154,10 @@ class PCG(_KrylovSolver):
     coefs, coef_kinds) is the preconditioner (its u is z, its f is r; q is only the scratch of its residual_norm, which
     PCG never calls).  With precond=None, z must be None, z is r, and only op_at(0) is used.  coefs / coef_kinds: as for
     Multigrid.  Building, solve(), residual_norm() and update_coefficients() are collective under torchrun.  The solver
-    never calls dd.swap(); a caller may swap between solves (the passes follow the current curr buffers)."""
+    never calls dd.swap(); a caller may swap between solves (the passes follow the current curr buffers).
+    Each exchange of a solve moves only what the pass reads at an offset (x for the residual, the vector A is applied to,
+    u on each V-cycle level; the coefficient fields once per solve), so after a solve the ghost cells of the solver's
+    scratch quantities are no longer refreshed as a side effect (DESIGN.md section 2.15)."""
 
     def __init__(self, dd: DistributedDomain, x: DataHandle, f: DataHandle, r: DataHandle, z: Optional[DataHandle], p: DataHandle, q: DataHandle,
                  op_at: Callable[[int], StencilOp], precond: Optional[str] = "multigrid", coefs: Optional[Sequence[DataHandle]] = None,

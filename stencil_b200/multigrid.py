@@ -176,6 +176,7 @@ class Multigrid:
         self._pairs = {}  # (u, f) ids -> the fine _Level of another pair (cycle(u=, f=))
         self.r = r
         self.coef_kinds = coef_kinds
+        self._coef_parity = None
         # every level queues on dd's apply streams, so stream order alone orders the work of consecutive levels
         dd._ensure_apply_streams()
         size = dd.size()
@@ -211,22 +212,35 @@ class Multigrid:
         for _ in range(sweeps):
             for c in range(self.colours):
                 if L.gs is None:
-                    plans = L.dd._apply_plans(L.A, (L.u, "curr"), L.u, (L.f, "curr"), coefs=L.coefs, colour=(self.colours, c), omega=1.0)
+                    plans = L.dd._apply_plans(L.A, (L.u, "curr"), L.u, (L.f, "curr"), (L.u,), L.coefs, (self.colours, c), omega=1.0)
                 else:
-                    plans = L.dd._apply_plans(L.gs, (L.u, "curr"), L.u, (L.f, "curr"), colour=(self.colours, c))
+                    plans = L.dd._apply_plans(L.gs, (L.u, "curr"), L.u, (L.f, "curr"), (L.u,), colour=(self.colours, c))
                 L.dd._run_plans(*plans, queued=True)
 
     def update_coefficients(self, wait: bool = True) -> None:
         """Re-coarsen every level's coefficient fields from the current fine ones, level by level: face fields by the
         face restriction, cell fields by the 8-cell restriction.  Queued like a cycle, after the work on the caller's
         stream, with one host wait (none with wait=False).  The constructor calls it once; call it again whenever the
-        fine fields change.  The coarse ghost cells are filled by the exchanges of the next cycle."""
+        fine fields change.  It then exchanges the fields of every level, fine and coarse: the cycles exchange only the
+        vector each call reads at an offset (DESIGN.md section 2.15), never a coefficient field.  A cycle after dd.swap()
+        exchanges the fine fields once more, as their curr buffers are then the other allocation."""
         self.levels[0].dd._follow_caller()
         for F, Cl in zip(self.levels[:-1], self.levels[1:]):
             for kf, kc, kind in zip(F.coefs, Cl.coefs, self.coef_kinds):
                 F.dd._transfer(Cl.dd, _lib.TRANSFER_RESTRICT, (kc, "curr"), (kf, "curr"), None, False, queued=True, face=COEF_KINDS[kind])
+        for L in self.levels:
+            if L.coefs:
+                L.dd._queue_exchange(L.dd._exchange_sel("Multigrid", tuple(L.coefs), ()))
+        self._coef_parity = self.levels[0].dd._parity
         if wait:
             self.wait()
+
+    def _fine_coefs_current(self) -> None:
+        """After dd.swap() the fine coefficient fields' curr buffers are the other allocation: exchange them once."""
+        L0 = self.levels[0]
+        if L0.coefs and self._coef_parity != L0.dd._parity:
+            L0.dd._queue_exchange(L0.dd._exchange_sel("Multigrid", tuple(L0.coefs), ()))
+            self._coef_parity = L0.dd._parity
 
     def _vcycle(self, l: int, L: Optional[_Level] = None) -> None:
         L = self.levels[l] if L is None else L
@@ -235,11 +249,11 @@ class Multigrid:
             return
         self._smooth(L, self.nu1)
         Cl = self.levels[l + 1]
-        L.dd._transfer(Cl.dd, _lib.TRANSFER_RESTRICT, (Cl.f, "curr"), (L.u, "curr"), (L.f, "curr"), True, op=L.res, queued=True,
+        L.dd._transfer(Cl.dd, _lib.TRANSFER_RESTRICT, (Cl.f, "curr"), (L.u, "curr"), (L.f, "curr"), (L.u,), op=L.res, queued=True,
                        coefs=L.coefs if L.res.has_coef else None)
         Cl.dd._queue_clear(Cl.u)
         self._vcycle(l + 1)
-        L.dd._transfer(Cl.dd, _lib.TRANSFER_PROLONG, (L.u, "curr"), (Cl.u, "curr"), (L.u, "curr"), True, queued=True)
+        L.dd._transfer(Cl.dd, _lib.TRANSFER_PROLONG, (L.u, "curr"), (Cl.u, "curr"), (L.u, "curr"), (Cl.u,), queued=True)
         self._smooth(L, self.nu2)
 
     def _fine_level(self, u: DataHandle, f: DataHandle) -> _Level:
@@ -281,11 +295,14 @@ class Multigrid:
         With u= and f=, the cycle runs on that fine-level pair instead of the constructor's, through the same coarse
         levels and coarse coefficient fields: u and f are two different quantities of dd of the constructor u's type,
         not coefficient fields, and u carries the constructor u's BC on every FIXED face (the coarse walls derive from
-        it).  The cycle is then the bits of one on a Multigrid built on (u, f).  Give both or neither."""
+        it).  The cycle is then the bits of one on a Multigrid built on (u, f).  Give both or neither.
+        Each exchange inside a cycle moves only the vector the call reads at an offset (u on each level), so after a cycle
+        the ghost cells of the other quantities, the solver's scratch included, are no longer refreshed as a side effect."""
         if (u is None) != (f is None):
             raise _lib.StencilError("Multigrid.cycle: give both u and f, or neither")
         L = self._fine_level(u, f)
         self.levels[0].dd._follow_caller()
+        self._fine_coefs_current()
         self._vcycle(0, L)
         if wait:
             self.wait()
