@@ -152,11 +152,7 @@ protected:
       return;
     }
     queued(false);
-    for (size_t i = 0; i < dd_.applyStreams_.size(); ++i) {
-      CUDA_RUNTIME(cudaSetDevice(dd_.domains_[i / 2].gpu()));
-      CUDA_RUNTIME(cudaStreamSynchronize(dd_.applyStreams_[i]));
-    }
-    dd_.exchange_wait();
+    DistributedDomain::wait_queued({&dd_});
   }
 };
 

@@ -290,12 +290,9 @@ private:
   // the end of a queued cycle: every apply stream and exchange of every level complete
   void finish() {
     set_queued(false);
-    DistributedDomain &dd = *levels_[0].dd;
-    for (size_t i = 0; i < dd.applyStreams_.size(); ++i) {
-      CUDA_RUNTIME(cudaSetDevice(dd.domains_[i / 2].gpu()));
-      CUDA_RUNTIME(cudaStreamSynchronize(dd.applyStreams_[i]));
-    }
-    for (Level &L : levels_) L.dd->exchange_wait();
+    std::vector<DistributedDomain *> doms;
+    for (Level &L : levels_) doms.push_back(L.dd);
+    DistributedDomain::wait_queued(doms);
   }
 
   // r = f - A u: (aux, 0, 1), then each term of A with its weight negated (a coefficient term keeps its field)

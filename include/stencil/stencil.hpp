@@ -193,20 +193,21 @@ private:
   // the bit set an operator call exchanges (0: none): every quantity for true, `reads` for Exchange::reads() (the full
   // set when it names every quantity), the given set for Exchange::only
   uint64_t exchange_set(const char *name, const stencil::Exchange &exchange, uint64_t reads) const;
-  // the schedule apply_op and apply_sys share: the cached per-domain plans of key (built by make(domain, boxes) on first
-  // use), then the interior plans on their own streams while exchange() runs and the exterior plans after it, or the one
-  // whole-region plan per domain; returns when every launch is complete.  writes_src: the launch writes src (a coloured
-  // apply in place), so the interior also keeps clear of the slabs exchange() sends, which are as wide as the radius on
-  // the opposite side.
+  // the plans apply_op and apply_sys share: the cached per-domain plans of key (built by make(domain, boxes) on first
+  // use), run by queued_schedule: the interior plans while exchange() runs and the exterior plans after it, or the one
+  // whole-region plan per domain.  writes_src: the launch writes src (a coloured apply in place), so the interior also
+  // keeps clear of the slabs exchange() sends, which are as wide as the radius on the opposite side.
   void run_stencil_plans(const std::vector<int64_t> &key, uint64_t exchange, bool writes_src,
                          const std::function<sb_stencil_plan *(size_t, const std::vector<Rect3> &)> &make);
 
-  // The queued schedule (the multigrid solver's, DESIGN.md section 2.11): while queued_ is set, run_stencil_plans and
-  // transfer issue the same launches but return at once, ordered by CUDA events only.  Each interior (or whole-region
-  // launch) waits for the previous exterior of its subdomain; queue_exchange() makes every exchange stream wait for every
-  // local apply stream before exchange_async(), so an exchange neither sends a value still being written nor overwrites
-  // a ghost cell an earlier launch still reads (and, across ranks, signals its neighbours only after those waits);
-  // wait_exchange(other, interior) makes this domain's exterior (and interior) apply streams wait for other's exchange.
+  // The schedule of every operator call (DESIGN.md section 2.11), ordered by CUDA events only.  Each interior (or
+  // whole-region launch) waits for the previous exterior of its subdomain; queue_exchange() makes every exchange stream
+  // wait for every local apply stream before exchange_async(), so an exchange neither sends a value still being written
+  // nor overwrites a ghost cell an earlier launch still reads (and, across ranks, signals its neighbours only after those
+  // waits); wait_exchange(other, interior) makes this domain's exterior (and interior) apply streams wait for other's
+  // exchange.  The apply streams are blocking streams, so a call follows the work on the legacy default stream.  A
+  // public call ends with one host wait (wait_queued); while queued_ is set (a solver that owns the schedule) it returns
+  // at once.
   bool queued_ = false;
   bool sharedApplyStreams_ = false; // applyStreams_ belong to another domain (a solver's finer level)
   std::vector<cudaEvent_t> applyEvents_, exchangeEvents_; // one per apply / exchange stream, recorded again on each use
@@ -217,9 +218,13 @@ private:
   void queue_exchange(uint64_t quantities = ~uint64_t(0));
   void wait_exchange(DistributedDomain &other, bool interior);
   void ensure_queue_events();
-  // the queued form of the interior / exchange / exterior schedule: launch(domain, part, stream), part 0 the interior (or
-  // the whole region without exchange), 1 the exterior
+  // the interior / exchange / exterior schedule: launch(domain, part, stream), part 0 the interior (or the whole region
+  // without exchange), 1 the exterior; then, unless queued_, wait_queued({this})
   void queued_schedule(const std::function<void(size_t, int, cudaStream_t)> &launch, uint64_t exchange);
+  // returns when the work queued on the apply and exchange streams of every domain in doms is complete: the end of a
+  // public operator call, of a Multigrid cycle and of a Krylov solve (apply streams several domains share are waited for
+  // once)
+  static void wait_queued(const std::vector<DistributedDomain *> &doms);
 
   // multigrid transfers: per (coarse domain, kind, buffers, the swap parity of both domains), one plan per local domain.
   // serial_ names a domain for the lifetime of the process (an address can be reused by a later domain)
@@ -400,8 +405,9 @@ public:
   // or next and may be dst.  Fails loudly unless realize() has run and sb_stencil_check accepts the op for this domain's
   // radius.  exchange = true: the interior runs on its own stream while exchange() fills the ghost cells, then one launch
   // per subdomain covers its exterior slabs; exchange = false: one launch over the whole region, the caller guarantees the
-  // ghost cells are current.  Returns when the update is complete.  The plans are kept, per (op, buffers, exchange, swap
-  // parity), until the domain is destroyed.
+  // ghost cells are current.  The launches and the exchange follow the work on the legacy default stream, and the call
+  // returns when the update is complete.  The plans are kept, per (op, buffers, exchange, swap parity), until the domain
+  // is destroyed.
   template <typename T>
   void apply(const stencil::LinearStencil &op, const stencil::Buffer<T> &dst, const DataHandle<T> &src, stencil::Exchange exchange = true) {
     apply_op(op, stencil::bc_dtype<T>(), dst.h.id(), dst.which, src.id(), -1, stencil::Which::curr, {}, exchange);
@@ -499,8 +505,9 @@ public:
   // this domain and aux may be dst (the in-place correction u <- u + P e); src is a curr buffer of coarse, whose radius
   // must be >= 1 in all 26 directions.  exchange = true runs coarse.exchange() first (collective), exchange = false
   // leaves the coarse ghost cells to the caller.
-  // One launch per local subdomain on the apply streams; returns when complete.  Plans are kept, per (coarse domain,
-  // kind, buffers, swap parity of both domains), until this domain is destroyed.
+  // One launch per local subdomain on the apply streams; the launches and any exchange follow the work on the legacy
+  // default stream, and the call returns when they are complete.  Plans are kept, per (coarse domain, kind, buffers,
+  // swap parity of both domains), until this domain is destroyed.
   //     fine.restrict_to(coarse, stencil::curr(f2), stencil::curr(r));
   //     fine.prolong_from(coarse, stencil::curr(u), stencil::curr(e), stencil::curr(u));
   template <typename T> void restrict_to(DistributedDomain &coarse, const stencil::Buffer<T> &dst, const stencil::Buffer<T> &src) {

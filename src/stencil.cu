@@ -858,27 +858,10 @@ void DistributedDomain::run_stencil_plans(const std::vector<int64_t> &key, uint6
     }
     found = stencilPlans_.emplace(key, std::move(per_dom)).first;
   }
-  create_apply_streams();
   const std::vector<std::vector<sb_stencil_plan *>> &plans = found->second;
-  if (queued_) {
-    queued_schedule([&](size_t di, int part, cudaStream_t s) {
-      if (SB_OK != sb_stencil_plan_launch(plans[di][size_t(part)], s)) LOG_FATAL("apply: " << sb_last_error());
-    }, exchange);
-    return;
-  }
-  for (size_t di = 0; di < domains_.size(); ++di)
-    if (SB_OK != sb_stencil_plan_launch(plans[di][0], applyStreams_[2 * di])) LOG_FATAL("apply: " << sb_last_error());
-  if (exchange) {
-    exchange_async_set(exchange); // and wait: every ghost cell this exchange fills is filled
-    exchange_wait();
-    for (size_t di = 0; di < domains_.size(); ++di)
-      if (SB_OK != sb_stencil_plan_launch(plans[di][1], applyStreams_[2 * di + 1])) LOG_FATAL("apply: " << sb_last_error());
-  }
-  for (size_t di = 0; di < domains_.size(); ++di) {
-    domains_[di].set_device();
-    CUDA_RUNTIME(cudaStreamSynchronize(applyStreams_[2 * di]));
-    CUDA_RUNTIME(cudaStreamSynchronize(applyStreams_[2 * di + 1]));
-  }
+  queued_schedule([&](size_t di, int part, cudaStream_t s) {
+    if (SB_OK != sb_stencil_plan_launch(plans[di][size_t(part)], s)) LOG_FATAL("apply: " << sb_last_error());
+  }, exchange);
 }
 
 void DistributedDomain::ensure_queue_events() {
@@ -958,6 +941,19 @@ void DistributedDomain::queued_schedule(const std::function<void(size_t, int, cu
       domains_[di].set_device();
       launch(di, 1, applyStreams_[2 * di + 1]);
     }
+  }
+  if (!queued_) wait_queued({this});
+}
+
+void DistributedDomain::wait_queued(const std::vector<DistributedDomain *> &doms) {
+  std::set<cudaStream_t> waited; // a solver's levels share the finest level's apply streams
+  for (DistributedDomain *dd : doms) {
+    for (size_t i = 0; i < dd->applyStreams_.size(); ++i)
+      if (waited.insert(dd->applyStreams_[i]).second) {
+        CUDA_RUNTIME(cudaSetDevice(dd->domains_[i / 2].gpu()));
+        CUDA_RUNTIME(cudaStreamSynchronize(dd->applyStreams_[i]));
+      }
+    dd->exchange_wait();
   }
 }
 
@@ -1136,35 +1132,15 @@ void DistributedDomain::transfer(DistributedDomain &coarse, bool prolong, int dt
     }
     found = transferPlans_.emplace(key, std::move(per_dom)).first;
   }
-  create_apply_streams();
   const std::vector<sb_transfer_plan *> &plans = found->second;
   const size_t per = split ? 2 : 1;
-  auto launch = [&](size_t di, int part, cudaStream_t s) {
+  if (prolong && xq) { // the coarse apply streams it waits for follow the legacy default stream (blocking streams)
+    coarse.queue_exchange(xq);
+    wait_exchange(coarse, true);
+  }
+  queued_schedule([&](size_t di, int part, cudaStream_t s) {
     if (SB_OK != sb_transfer_plan_launch(plans[per * di + size_t(part)], s)) LOG_FATAL(name << ": " << sb_last_error());
-  };
-  if (queued_) {
-    if (prolong && xq) {
-      coarse.queue_exchange(xq);
-      wait_exchange(coarse, true);
-    }
-    queued_schedule(launch, split ? xq : 0);
-    return;
-  }
-  if (prolong && xq) {
-    coarse.exchange_async_set(xq);
-    coarse.exchange_wait();
-  }
-  for (size_t di = 0; di < domains_.size(); ++di) launch(di, 0, applyStreams_[2 * di]);
-  if (split) {
-    exchange_async_set(xq); // and wait: every ghost cell this exchange fills is filled
-    exchange_wait();
-    for (size_t di = 0; di < domains_.size(); ++di) launch(di, 1, applyStreams_[2 * di + 1]);
-  }
-  for (size_t di = 0; di < domains_.size(); ++di) {
-    domains_[di].set_device();
-    CUDA_RUNTIME(cudaStreamSynchronize(applyStreams_[2 * di]));
-    CUDA_RUNTIME(cudaStreamSynchronize(applyStreams_[2 * di + 1]));
-  }
+  }, split ? xq : 0);
 }
 
 std::vector<unsigned char> DistributedDomain::allgather_records(const std::vector<unsigned char> &mine) const {

@@ -1371,12 +1371,6 @@ class DistributedDomain:
         for d, s in zip(self.domains_, self._streams):
             check(lib().sb_stream_sync(d.gpu(), stream_ptr(s)))
 
-    def _exchange_sync(self, exchange) -> None:
-        """exchange() of what _exchange_sel returned (True: every quantity, or a tuple of quantities)."""
-        self._exchange_async(None if exchange is True else exchange)
-        for d, s in zip(self.domains_, self._streams):
-            check(lib().sb_stream_sync(d.gpu(), stream_ptr(s)))
-
     def _exchange_sel(self, name: str, exchange, reads) -> object:
         """What an operator call exchanges: False (nothing), True (every quantity) or a sorted tuple of quantities.
         exchange: a bool, "reads" (the quantities of `reads`, those the call reads at a non-zero offset; none of them
@@ -1563,7 +1557,8 @@ class DistributedDomain:
         of each subdomain run as one launch; exchange=False: one launch over the whole region, and the caller guarantees
         the ghost cells are current; exchange="reads": the schedule of True, with an exchange of only the quantities the
         call reads at a non-zero offset (exchange(only=...), DESIGN.md section 2.15): src, and each coefficient field
-        that a term reads at a non-zero coefficient offset.  Returns when the update is complete.  The plans are built
+        that a term reads at a non-zero coefficient offset.  The launches and the exchange are ordered after the work
+        queued on the caller's current stream, and the call returns when the update is complete.  The plans are built
         on first use and kept, per (op, buffers, exchange, swap parity, colour), until close().  Under torchrun every
         rank calls it (exchange() is collective).
         colour=(m, c), m in 1, 2, 8 (DESIGN.md section 2.9): only the cells of colour c of the colouring m (taken from global
@@ -1736,60 +1731,14 @@ class DistributedDomain:
         return plans
 
     def _run_plans(self, plans, exchange: bool, queued: bool = False) -> None:
-        """The schedule of apply and apply_system: with exchange, every interior plan on its own stream while exchange()
-        fills the ghost cells, then every exterior plan; without, the one plan per domain.  Returns when all are done.
-        queued: the same launches, ordered by events only, and returns at once (_queue_plans)."""
+        """The schedule of every operator call, ordered by CUDA events only.  Each interior (or the one plan without
+        exchange) waits for the previous exterior on its subdomain's apply streams; with exchange, the exchange waits for
+        every apply stream as they were before this interior (_queue_exchange), and each exterior waits for the exchange.
+        A public call first orders the apply streams after the caller's stream and returns when its work is complete
+        (wait_queued); queued=True (a solver that owns the schedule) returns at once."""
         self._ensure_apply_streams()
-        if queued:
-            self._queue_plans(plans, exchange)
-            return
-        self._follow_caller()
-        multi = len({d.gpu() for d in self.domains_}) > 1
-        if exchange:
-            for d, p, (si, _) in zip(self.domains_, plans, self._apply_streams):
-                if multi:
-                    _set_current_device(d.gpu())
-                p[0].launch(si)
-            self._exchange_sync(exchange)  # returns when every ghost cell it fills is filled
-            for d, p, (_, se) in zip(self.domains_, plans, self._apply_streams):
-                if multi:
-                    _set_current_device(d.gpu())
-                p[1].launch(se)
-        else:
-            for d, p, (si, _) in zip(self.domains_, plans, self._apply_streams):
-                if multi:
-                    _set_current_device(d.gpu())
-                p[0].launch(si)
-        for si, se in self._apply_streams:
-            si.synchronize()
-            se.synchronize()
-
-    # -- the queued schedule (the multigrid solver's): nothing waits on the host, CUDA events order the launches
-    def _ensure_apply_streams(self) -> None:
-        """Two apply streams per local domain (interior, exterior), made on first use."""
-        if not self._apply_streams:
-            import torch
-
-            self._apply_streams = [(torch.cuda.Stream(device=d.gpu()), torch.cuda.Stream(device=d.gpu())) for d in self.domains_]
-
-    def _follow_caller(self) -> None:
-        """Every apply stream waits for the work queued so far on the caller's current stream of its device."""
-        import torch
-
-        for d, (si, se) in zip(self.domains_, self._apply_streams):
-            si.wait_stream(torch.cuda.current_stream(d.gpu()))
-            se.wait_stream(torch.cuda.current_stream(d.gpu()))
-
-    def _queue_clear(self, h: DataHandle) -> None:
-        """h's whole curr allocation set to +0, queued on the interior apply streams after the previous exterior."""
-        self._run_plans([(_Clear(d, h.id),) for d in self.domains_], False, queued=True)
-
-    def _queue_plans(self, plans, exchange: bool) -> None:
-        """_run_plans without a host wait.  Each interior (or the one plan without exchange) waits for the previous
-        exterior on its subdomain's apply streams; with exchange, the exchange waits for every apply stream as they were
-        before this interior (_queue_exchange), and each exterior waits for the exchange."""
-        import torch
-
+        if not queued:
+            self._follow_caller()
         multi = len({d.gpu() for d in self.domains_}) > 1
         apply_ev, _ = self._queue_events()
         for (si, se), pair in zip(self._apply_streams, apply_ev):
@@ -1807,6 +1756,30 @@ class DistributedDomain:
                 if multi:
                     _set_current_device(d.gpu())
                 p[1].launch(se)
+        if not queued:
+            wait_queued([self])
+
+    # -- the queued schedule: nothing waits on the host, CUDA events order the launches
+    def _ensure_apply_streams(self) -> None:
+        """Two apply streams per local domain (interior, exterior), made on first use."""
+        if not self._apply_streams:
+            import torch
+
+            self._apply_streams = [(torch.cuda.Stream(device=d.gpu()), torch.cuda.Stream(device=d.gpu())) for d in self.domains_]
+
+    def _follow_caller(self) -> None:
+        """Every apply stream waits for the work queued so far on the caller's current stream of its device."""
+        import torch
+
+        self._ensure_apply_streams()
+        for d, (si, se) in zip(self.domains_, self._apply_streams):
+            ev = torch.cuda.current_stream(d.gpu()).record_event()
+            si.wait_event(ev)
+            se.wait_event(ev)
+
+    def _queue_clear(self, h: DataHandle) -> None:
+        """h's whole curr allocation set to +0, queued on the interior apply streams after the previous exterior."""
+        self._run_plans([(_Clear(d, h.id),) for d in self.domains_], False, queued=True)
 
     def _queue_events(self):
         """The events of the queued schedule, created once and recorded again on each use (a wait takes the record made
@@ -1837,6 +1810,7 @@ class DistributedDomain:
     def _wait_exchange(self, other: "DistributedDomain", interior: bool = True) -> None:
         """Every exterior apply stream of this domain (and every interior one with interior=True) waits for the
         exchange queued last on other's exchange streams."""
+        self._ensure_apply_streams()
         _, evs = other._queue_events()
         for x, ev in zip(other._streams, evs):
             ev.record(x)
@@ -1853,7 +1827,8 @@ class DistributedDomain:
         src may be curr or next, as restriction reads no ghost cells.  coarse must pair with this domain: the same
         partition dim, every subdomain exactly twice as coarse, on the same rank and GPU (sb_transfer_check; checked
         once per coarse domain).  One launch per local subdomain on the apply streams, after the work queued on the
-        caller's stream; returns when it is complete.  Plans are cached as prolong_from() describes.
+        caller's current stream (with an op and exchange, the exchange too); returns when it is complete.  Plans are
+        cached as prolong_from() describes.
             fine.restrict_to(coarse, (f2, "curr"), (r, "curr"))
         op: a StencilOp (plain terms, reach <= 1): dst = the 8-cell average of op(src, aux), the fine values never
         stored (DESIGN.md section 2.11), the same bits as apply() into a scratch quantity followed by restrict_to().
@@ -1889,15 +1864,16 @@ class DistributedDomain:
         "curr"); aux may be dst, which gives the in-place correction u <- u + P e.  src is a quantity of coarse and must
         be a curr buffer: its ghost cells are read.  exchange=True runs coarse.exchange() first (collective: every rank
         calls it), with exchange=False the caller guarantees the coarse ghost cells, exchange="reads" exchanges the coarse
-        src only (coarse.exchange(only=[src])).  The coarse radius must be >= 1 in
+        src only (coarse.exchange(only=[src])).  The exchange and the launches are ordered after the work queued on the
+        caller's current stream, and the call returns when they are complete.  The coarse radius must be >= 1 in
         all 26 directions.  Plans are built on first use and kept, per (coarse domain, kind, buffers, the swap parity
         of both domains), until close().
             fine.prolong_from(coarse, (u, "curr"), (e, "curr"), aux=(u, "curr"))"""
         self._transfer(coarse, _lib.TRANSFER_PROLONG, dst, src, aux, exchange)
 
     def _transfer(self, coarse, kind: int, dst, src, aux, exchange, op=None, queued: bool = False, coefs=None, face=None) -> None:
-        """restrict_to / prolong_from; queued: the schedule of _run_plans(queued=True), for a solver that owns the cycle;
-        coefs: the fine coefficient quantities of a coefficient op; face: the axis of a face restriction."""
+        """restrict_to / prolong_from, through _run_plans; queued: no host wait, for a solver that owns the cycle; coefs:
+        the fine coefficient quantities of a coefficient op; face: the axis of a face restriction."""
         from .stencil_op import StencilOp
 
         name = "restrict_to" if kind == _lib.TRANSFER_RESTRICT else "prolong_from"
@@ -1978,11 +1954,10 @@ class DistributedDomain:
                                            sd.accessor_origin(), sd.raw_size()[2], fd.pitched(*a) if a is not None else None, lo, hi),))
             self._transfer_plans[key] = plans
         if not restrict and exchange:
-            if queued:
-                coarse._queue_exchange(exchange)
-                self._wait_exchange(coarse)
-            else:
-                coarse._exchange_sync(exchange)
+            if not queued:  # the coarse exchange waits for coarse's apply streams, which are this domain's only in a solver
+                coarse._follow_caller()
+            coarse._queue_exchange(exchange)
+            self._wait_exchange(coarse)
         self._run_plans(plans, exchange if fused_exchange else False, queued)
 
     def _check_pairing(self, coarse, ghosts: bool) -> None:
@@ -2046,6 +2021,17 @@ class DistributedDomain:
         for d in self.domains_:
             d.free()
         self.domains_ = []
+
+
+def wait_queued(doms: Sequence[DistributedDomain]) -> None:
+    """Return when the work queued on the apply and exchange streams of every domain in doms is complete: the one host
+    wait that ends a public operator call and a Multigrid cycle.  Apply streams that several domains share (a solver's
+    levels) are waited for once."""
+    for s in dict.fromkeys(s for dd in doms for pair in dd._apply_streams for s in pair):
+        s.synchronize()
+    for dd in doms:
+        for x in dd._streams:
+            x.synchronize()
 
 
 # ------------------------------------------------------------------------------------------ jacobi helpers

@@ -24,7 +24,7 @@ from typing import Callable, List, Optional, Sequence
 import numpy as np
 
 from . import _lib
-from .domain import FACES, BC, BCKind, Boundary, DataHandle, DistributedDomain, Partition, PlacementStrategy, Radius
+from .domain import FACES, BC, BCKind, Boundary, DataHandle, DistributedDomain, Partition, PlacementStrategy, Radius, wait_queued
 from .stencil_op import StencilOp
 
 
@@ -309,13 +309,7 @@ class Multigrid:
 
     def wait(self) -> None:
         """Return when every queued cycle is complete."""
-        dd = self.levels[0].dd
-        for si, se in dd._apply_streams:
-            si.synchronize()
-            se.synchronize()
-        for L in self.levels:
-            for x in L.dd._streams:
-                x.synchronize()
+        wait_queued([L.dd for L in self.levels])
 
     def residual_norm(self) -> float:
         """||f - A u||_2 over dd's compute region: the residual into r (apply) and an exact reduction, so every rank and
